@@ -81,12 +81,14 @@ int b2_launch_leaf_values(const B2LeafDev*, const int32_t*, const long long*, co
 int b2_launch_tree_init(B2TreeDev, B2LevelCtl*, B2NodeSeg*, B2EvalNode*, int32_t*, int, B2HistWork*, cudaStream_t);
 int b2_launch_root_record(B2TreeDev, const B2EvalNode*, cudaStream_t);
 int b2_launch_iota(int32_t*, int64_t, cudaStream_t);
-int b2_launch_gradient(int, int, const float*, const float*, const float*, int64_t, float, float2*, uint32_t*, int, cudaStream_t);
+int b2_launch_gradient(int, int, const float*, const float*, const float*, int64_t, float, float, float2*, uint32_t*, uint32_t*, int,
+                       cudaStream_t);
+int b2_launch_label_check(int, const float*, int64_t, uint32_t*, int, cudaStream_t);
 int b2_launch_pack_custom(const float*, const float*, int, int64_t, float2*, int, cudaStream_t);
 int b2_launch_absmax(const float2*, int64_t, uint32_t*, int, cudaStream_t);
 int b2_launch_quant_exponent(const uint32_t*, int32_t*, cudaStream_t);
 int b2_launch_quantize(const float2*, int64_t, const int32_t*, int, int2*, int, cudaStream_t);
-int b2_launch_metric(int, int, int, const float*, const float*, const float*, int64_t, double*, int, cudaStream_t);
+int b2_launch_metric(int, int, int, float, const float*, const float*, const float*, int64_t, double*, int, cudaStream_t);
 int b2_launch_predict(const float*, int64_t, int, float, const B2TreeNodeDev*, const int32_t*, const uint32_t*, int, int, int, int,
                       float*, int, cudaStream_t);
 int b2_launch_fill(float*, int64_t, float, int, cudaStream_t);
@@ -693,7 +695,13 @@ void bin_matrix(Matrix* m) {
 }
 
 // ---------------------------------------------------------------- booster
-enum { kObjSquaredError = 0, kObjLogistic = 1, kObjSoftprob = 2 };
+// objective ids, shared with objective_kernel.cu (the kernels take them as plain ints)
+enum { kObjSquaredError = 0, kObjLogistic = 1, kObjSoftprob = 2, kObjRegLogistic = 3, kObjLogitRaw = 4, kObjSquaredLog = 5,
+       kObjPseudoHuber = 6, kObjPoisson = 7, kObjGamma = 8, kObjTweedie = 9 };
+bool obj_log_link(int o) { return o == kObjPoisson || o == kObjGamma || o == kObjTweedie; }
+bool obj_sigmoid(int o) { return o == kObjLogistic || o == kObjRegLogistic; }
+// objectives whose gradient kernel reports non-finite gradient pairs (gradient_param_kernel)
+bool obj_checks_finite(int o) { return o >= kObjSquaredLog; }
 struct Params {
   int objective = kObjSquaredError;
   std::string objective_name = "reg:squarederror";
@@ -708,6 +716,9 @@ struct Params {
   int device = 0;
   int max_cat_to_onehot = 4, max_cat_threshold = 64;   // xgboost defaults (src/tree/param.h)
   float scale_pos_weight = 1.0f, max_delta_step = 0.0f;
+  bool max_delta_step_set = false;             // false: count:poisson uses 0.7 (xgboost's Learner::ConfigureObjective)
+  float huber_slope = 1.0f;                    // reg:pseudohubererror delta (also the mphe metric's)
+  float tweedie_variance_power = 1.5f;         // reg:tweedie rho in [1, 2)
   float subsample = 1.0f, colsample_bytree = 1.0f, colsample_bylevel = 1.0f, colsample_bynode = 1.0f;
   int seed = 0;
   bool base_score_set = false;   // false: estimated from the labels before the first tree (xgboost >= 2.0, A.3)
@@ -803,6 +814,9 @@ struct Booster : HandleBase {
   std::map<int, int> direct_trees;         // trees grown with direct launches per class slot (the first one allocates)
   bool graph_failed = false;
   bool absmax_fused = false;               // this round's gradient kernel already produced d_absmax[k]
+  bool labels_checked = false;             // the train labels are inside the objective's domain (check_labels)
+  DevBuf<uint32_t> d_grad_err;             // set by the gradient kernel when a gradient pair is not finite
+  uint32_t* h_grad_err = nullptr;          // pinned copy, written at the end of the round's stream work
   DevBuf<uint16_t> pos;                    // [n] leaf index of every row (final_assign / leaf_sums -> margin_update)
   size_t slice_elems = 0;
   size_t node_elems = 0;
@@ -844,6 +858,7 @@ struct Booster : HandleBase {
     if (round_stop) cudaEventDestroy(round_stop);
     for (auto& kv : eval_cache) delete kv.second;
     for (void* h : staging) cudaFreeHost(h);
+    if (h_grad_err) cudaFreeHost(h_grad_err);
   }
 };
 
@@ -890,7 +905,16 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
       if (v == "reg:squarederror" || v == "reg:linear") p->objective = kObjSquaredError;
       else if (v == "binary:logistic") p->objective = kObjLogistic;
       else if (v == "multi:softprob" || v == "multi:softmax") p->objective = kObjSoftprob;
-      else fail("unsupported objective '%s' (supported: reg:squarederror, binary:logistic, multi:softprob, multi:softmax)", v.c_str());
+      else if (v == "reg:logistic") p->objective = kObjRegLogistic;
+      else if (v == "binary:logitraw") p->objective = kObjLogitRaw;
+      else if (v == "reg:squaredlogerror") p->objective = kObjSquaredLog;
+      else if (v == "reg:pseudohubererror") p->objective = kObjPseudoHuber;
+      else if (v == "count:poisson") p->objective = kObjPoisson;
+      else if (v == "reg:gamma") p->objective = kObjGamma;
+      else if (v == "reg:tweedie") p->objective = kObjTweedie;
+      else fail("unsupported objective '%s' (supported: reg:squarederror, reg:logistic, binary:logistic, binary:logitraw, "
+                "reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie, multi:softprob, "
+                "multi:softmax)", v.c_str());
     } else if (k == "num_class") p->num_class = i();
     else if (k == "num_parallel_tree") p->num_parallel_tree = i();
     else if (k == "max_depth") p->max_depth = i();
@@ -911,7 +935,9 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     else if (k == "colsample_bynode") p->colsample_bynode = f();
     else if (k == "seed" || k == "random_state") p->seed = i();
     else if (k == "scale_pos_weight") p->scale_pos_weight = f();
-    else if (k == "max_delta_step") p->max_delta_step = f();
+    else if (k == "max_delta_step") { p->max_delta_step = f(); p->max_delta_step_set = true; }
+    else if (k == "huber_slope") p->huber_slope = f();
+    else if (k == "tweedie_variance_power") p->tweedie_variance_power = f();
     else if (k == "max_cat_to_onehot") p->max_cat_to_onehot = i();
     else if (k == "max_cat_threshold") p->max_cat_threshold = i();
     else if (k == "max_bin") { if (max_bin_out) *max_bin_out = i(); }
@@ -926,10 +952,34 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     if (!(v > 0.0f && v <= 1.0f)) fail("subsample / colsample_* must be in (0, 1], got %g", (double)v);
   if (p->max_cat_to_onehot < 1) fail("max_cat_to_onehot must be >= 1, got %d", p->max_cat_to_onehot);
   if (p->max_cat_threshold < 1) fail("max_cat_threshold must be >= 1, got %d", p->max_cat_threshold);
+  if (p->objective == kObjPoisson) {
+    if (!p->max_delta_step_set) p->max_delta_step = 0.7f;   // both the hessian's shift and the leaf-step clamp
+    if (!(p->max_delta_step >= 0.0f)) fail("max_delta_step must be >= 0 for count:poisson, got %g", (double)p->max_delta_step);
+  }
+  if (p->objective == kObjPseudoHuber && !(p->huber_slope > 0.0f))
+    fail("huber_slope must be > 0 for reg:pseudohubererror, got %g", (double)p->huber_slope);
+  if (p->objective == kObjTweedie && !(p->tweedie_variance_power >= 1.0f && p->tweedie_variance_power < 2.0f))
+    fail("tweedie_variance_power must be in [1, 2), got %g", (double)p->tweedie_variance_power);
+  if (p->base_score_set) {
+    if (p->objective == kObjRegLogistic && !(p->base_score > 0.0f && p->base_score < 1.0f))
+      fail("base_score must be in (0, 1) for reg:logistic, got %g", (double)p->base_score);
+    if (obj_log_link(p->objective) && !(p->base_score > 0.0f))
+      fail("base_score must be > 0 for %s, got %g", p->objective_name.c_str(), (double)p->base_score);
+  }
 }
 
+// the parameter that the gradient kernel of an objective takes (gradient_param_kernel)
+float objective_param(const Params& p) {
+  if (p.objective == kObjPseudoHuber) return p.huber_slope;
+  if (p.objective == kObjPoisson) return p.max_delta_step;
+  if (p.objective == kObjTweedie) return p.tweedie_variance_power;
+  return 0.0f;
+}
+
+// margin of base_score (the inverse of the prediction transform), evaluated on the host with libm's logf
 float base_margin_value(const Params& p) {
-  if (p.objective == kObjLogistic) return -logf(1.0f / p.base_score - 1.0f);
+  if (obj_sigmoid(p.objective)) return -logf(1.0f / p.base_score - 1.0f);
+  if (obj_log_link(p.objective)) return logf(p.base_score);
   return p.base_score;
 }
 
@@ -1625,7 +1675,7 @@ void estimate_base_score(Booster* b) {
   zeros.ensure((size_t)std::max<int64_t>(n, 1)); gh.ensure((size_t)std::max<int64_t>(n, 1)); sums.ensure(2);
   CUDA_CHECK(cudaMemsetAsync(zeros.p, 0, (size_t)std::max<int64_t>(n, 1) * sizeof(float), s));
   LAUNCH_CHECK(b2_launch_gradient(p.objective, 1, zeros.p, m->label.p, m->n_weight ? m->weight.p : nullptr, n, p.scale_pos_weight,
-                                  gh.p, nullptr, b->ctx->num_sms, s));
+                                  objective_param(p), gh.p, nullptr, nullptr, b->ctx->num_sms, s));
   b->d_absmax.ensure(2); b->d_qexp.ensure(2);
   CUDA_CHECK(cudaMemsetAsync(b->d_absmax.p, 0, 2 * sizeof(uint32_t), s));
   LAUNCH_CHECK(b2_launch_absmax(gh.p, n, b->d_absmax.p, b->ctx->num_sms, s));
@@ -1640,11 +1690,11 @@ void estimate_base_score(Booster* b) {
   CUDA_CHECK(cudaStreamSynchronize(s));
   const double G = (double)h_s[0] / ldexp(1.0, 40 - h_e[0]), H = (double)h_s[1] / ldexp(1.0, 40 - h_e[1]);
   const float stump = H <= 1e-6 ? 0.0f : (float)(-G / H);
-  if (p.objective == kObjLogistic) {
-    // margin -> probability with the engine's own sigmoid (same IEEE sequence as the kernels): evaluated on the device
+  if (obj_sigmoid(p.objective) || obj_log_link(p.objective)) {
+    // margin -> output space with the engine's own sigmoid / exp (same IEEE sequence as the kernels): evaluated on the device
     DevBuf<float> one; one.ensure(1);
     CUDA_CHECK(cudaMemcpyAsync(one.p, &stump, sizeof(float), cudaMemcpyHostToDevice, s));
-    LAUNCH_CHECK(b2_launch_transform(kObjLogistic, 1, one.p, 1, b->ctx->num_sms, s));
+    LAUNCH_CHECK(b2_launch_transform(p.objective, 1, one.p, 1, b->ctx->num_sms, s));
     float prob = 0.5f;
     CUDA_CHECK(cudaMemcpyAsync(&prob, one.p, sizeof(float), cudaMemcpyDeviceToHost, s));
     CUDA_CHECK(cudaStreamSynchronize(s));
@@ -1655,9 +1705,31 @@ void estimate_base_score(Booster* b) {
   p.base_score_set = true;
 }
 
+// labels outside the objective's domain fail training (xgboost's CheckLabel); once per train matrix, before the first tree
+void check_labels(Booster* b) {
+  Matrix* m = b->train; const int o = b->p.objective; cudaStream_t s = b->ctx->stream;
+  if (o == kObjSquaredError || o == kObjLogistic || o == kObjSoftprob || o == kObjPseudoHuber || b->labels_checked) return;
+  if (m->n_label != m->n) fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)m->n);
+  DevBuf<uint32_t> bad; bad.ensure(1);
+  CUDA_CHECK(cudaMemsetAsync(bad.p, 0, sizeof(uint32_t), s));
+  LAUNCH_CHECK(b2_launch_label_check(o, m->label.p, m->n, bad.p, b->ctx->num_sms, s));
+  allreduce(b->comm, bad.p, 1, kNcclUint32, kNcclMax, s);
+  uint32_t h = 0;
+  CUDA_CHECK(cudaMemcpyAsync(&h, bad.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  if (h) {
+    const char* cond = (o == kObjRegLogistic || o == kObjLogitRaw) ? "label must be in [0, 1]"
+                       : o == kObjSquaredLog ? "label must be greater than -1"
+                       : o == kObjGamma ? "label must be positive" : "label must be nonnegative";
+    fail("%s for %s", cond, b->p.objective_name.c_str());
+  }
+  b->labels_checked = true;
+}
+
 void ensure_train_margin(Booster* b) {
   if (b->margin_ready) return;
   Matrix* m = b->train;
+  check_labels(b);
   estimate_base_score(b);
   b->margin.ensure((size_t)std::max<int64_t>(m->n * b->p.num_class, 1));
   init_margin(b, b->margin.p, m);
@@ -1681,6 +1753,7 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
   b->gh.ensure((size_t)std::max<int64_t>(n * K, 1));
   b->d_absmax.ensure(2 * (size_t)K); b->d_qexp.ensure(2);
   b->absmax_fused = false;
+  bool check_finite = false;
   if (custom_g) {
     if (len != n * K) fail("custom gradient has %lld values, expected %lld", (long long)len, (long long)(n * K));
     b->d_custom_g.ensure((size_t)std::max<int64_t>(len, 1)); b->d_custom_h.ensure((size_t)std::max<int64_t>(len, 1));
@@ -1692,8 +1765,15 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
     // the |g|,|h| maxima of every class tree come out of the same pass unless rows are dropped afterwards (subsample)
     b->absmax_fused = b->p.subsample >= 1.0f && K <= b2_gradient_fused_max_classes();
     if (b->absmax_fused) CUDA_CHECK(cudaMemsetAsync(b->d_absmax.p, 0, 2 * (size_t)K * sizeof(uint32_t), s));
+    check_finite = obj_checks_finite(b->p.objective);
+    if (check_finite) {
+      if (!b->h_grad_err) { CUDA_CHECK(cudaMallocHost(&b->h_grad_err, sizeof(uint32_t))); b->d_grad_err.ensure(1); }
+      CUDA_CHECK(cudaMemsetAsync(b->d_grad_err.p, 0, sizeof(uint32_t), s));
+    }
     LAUNCH_CHECK(b2_launch_gradient(b->p.objective, K, b->margin.p, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
-                                    b->p.scale_pos_weight, b->gh.p, b->absmax_fused ? b->d_absmax.p : nullptr, b->ctx->num_sms, s));
+                                    b->p.scale_pos_weight, objective_param(b->p), b->gh.p,
+                                    b->absmax_fused ? b->d_absmax.p : nullptr, check_finite ? b->d_grad_err.p : nullptr,
+                                    b->ctx->num_sms, s));
   }
   b->t.kernel_launches++;
   const int npt = b->p.num_parallel_tree;
@@ -1710,6 +1790,12 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
         CUDA_CHECK(cudaMemcpyAsync(b->gh.p + (size_t)k * n, b->gh_round.p + (size_t)k * n, (size_t)n * sizeof(float2), cudaMemcpyDeviceToDevice, s));
       run_tree(b, k, k * npt + j);
     }
+  if (check_finite) {
+    // every rank fails the round together; the flag is read back with the round's own synchronisation below (pinned
+    // memory: the copy is ordered on the stream)
+    allreduce(b->comm, b->d_grad_err.p, 1, kNcclUint32, kNcclMax, s);
+    CUDA_CHECK(cudaMemcpyAsync(b->h_grad_err, b->d_grad_err.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  }
   if (b->p.profile) {
     CUDA_CHECK(cudaEventRecord(b->round_stop, s));
     CUDA_CHECK(cudaEventSynchronize(b->round_stop));
@@ -1725,12 +1811,39 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
     if (perr) fail("peer-memory exchange: %s while waiting for another rank (flag slot %u)",
                    b->comm && b->comm->aborted.load() ? "communicator aborted" : "timed out", perr - 1);
   }
+  if (check_finite && *b->h_grad_err) {
+    // the trees of this round were grown with those rows zeroed and are dropped; the train margin already holds their
+    // leaves, so it is rebuilt from the kept trees before the next round
+    b->margin_ready = false;
+    fail("%s: a gradient or hessian is not finite (the margin left the range where the objective's exp is finite)",
+         b->p.objective_name.c_str());
+  }
   for (int slot = 0; slot < K * npt; ++slot) materialize_tree(b, slot);
   b->t.rounds++;
 }
 
-int metric_id(const char* name) {
+// metric id of an eval_metric name; *param receives the metric's parameter (rho of tweedie-nloglik@rho, huber_slope for mphe)
+int metric_id(const char* name, const Params& p, float* param) {
   std::string s(name ? name : "");
+  *param = 0.0f;
+  if (s == "rmsle") return 7;
+  if (s == "mape") return 8;
+  if (s == "mphe") { *param = p.huber_slope; return 9; }
+  if (s == "poisson-nloglik") return 10;
+  if (s == "gamma-nloglik") return 11;
+  if (s == "gamma-deviance") return 12;
+  if (s.rfind("tweedie-nloglik", 0) == 0) {
+    *param = 1.5f;   // xgboost's default when the name carries no @rho
+    if (s.size() > 15) {
+      char* end = nullptr;
+      const std::string r = s.substr(16);
+      const double v = s[15] == '@' ? strtod(r.c_str(), &end) : NAN;
+      if (s[15] != '@' || r.empty() || *end != '\0' || !(v >= 1.0 && v < 2.0))
+        fail("eval metric '%s': the Tweedie power must be given as tweedie-nloglik@rho with rho in [1, 2)", s.c_str());
+      *param = (float)v;
+    }
+    return 13;
+  }
   if (s == "rmse") return 0;
   if (s == "logloss") return 1;
   if (s == "error") return 2;
@@ -1738,7 +1851,8 @@ int metric_id(const char* name) {
   if (s == "merror") return 4;
   if (s == "mae") return 5;
   if (s == "auc") return 6;
-  fail("unsupported eval metric '%s' (supported: rmse, mae, logloss, error, auc, mlogloss, merror)", s.c_str());
+  fail("unsupported eval metric '%s' (supported: rmse, mae, logloss, error, auc, mlogloss, merror, rmsle, mape, mphe, "
+       "poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho)", s.c_str());
 }
 
 // margin of matrix m under the current model (cached per matrix, only new trees are applied)
@@ -2217,7 +2331,8 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
   Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
   cudaStream_t s = b->ctx->stream;
-  const int mid = metric_id(metric);
+  float mparam = 0.0f;
+  const int mid = metric_id(metric, b->p, &mparam);
   if (m->n_label != m->n) fail("evaluation matrix has no labels");
   float* margin = eval_margin(b, m);
   b->d_metric.ensure(2);
@@ -2242,14 +2357,14 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
     *out = h[1] > 0 ? h[0] / h[1] : 0.5;   // only one class present: xgboost reports 0.5
     return 0;
   }
-  LAUNCH_CHECK(b2_launch_metric(b->p.objective, mid, b->p.num_class, margin, m->label.p, m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p,
+  LAUNCH_CHECK(b2_launch_metric(b->p.objective, mid, b->p.num_class, mparam, margin, m->label.p, m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p,
                                 b->ctx->num_sms, s));
   allreduce(b->comm, b->d_metric.p, 2, kNcclFloat64, kNcclSum, s);
   double h[2];
   CUDA_CHECK(cudaMemcpyAsync(h, b->d_metric.p, sizeof(h), cudaMemcpyDeviceToHost, s));
   CUDA_CHECK(cudaStreamSynchronize(s));
   double v = h[1] > 0 ? h[0] / h[1] : 0.0;
-  *out = mid == 0 ? sqrt(v) : v;
+  *out = (mid == 0 || mid == 7) ? sqrt(v) : v;
   API_END
 }
 int B2_BoosterPredict(B2Handle bh, B2Handle mh, int32_t output_margin, int32_t tree_begin, int32_t tree_end, float* out,

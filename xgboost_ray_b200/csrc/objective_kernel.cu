@@ -2,8 +2,11 @@
 //
 // Replaces the objective / metric / predictor stages that the reference reaches through
 // xgb.train() and Booster.predict() (xgboost_ray/main.py:745-752, 804; SURVEY.md 8a rows a9, a14;
-// Appendix A.4, A.9, A.10).  Compiled with --fmad=false: b2_expf below is a fixed sequence of
-// IEEE-754 binary32 mul/add, replayed identically by the CPU oracle, so gradients are bit-equal.
+// Appendix A.4, A.9, A.10).  Compiled with --fmad=false: b2_expf and b2_log1pf below are fixed sequences
+// of IEEE-754 binary32 operations, replayed identically on the host by the test references (the CPU oracle,
+// tests/objective_reference.py), so gradients are bit-equal.
+#include <cfloat>
+#include <cmath>
 #include "common.cuh"
 #include "sampling.cuh"
 
@@ -42,6 +45,89 @@ __device__ __forceinline__ float b2_sigmoid(float x) {
   return __fdiv_rn(1.0f, denom);
 }
 
+// log1p as a fixed binary32 sequence (tests/objective_reference.py replays it): the classic fdlibm reduction.  1+x = 2^k (1+f)
+// with sqrt(2)/2 <= 1+f < sqrt(2), c corrects the rounding of 1+x, and log(1+f) = f - f^2/2 + s (f^2/2 + R(s^2)) with
+// s = f / (2+f), with fdlibm's polynomial coefficients Lg1..Lg4 (about 1 ulp on (-1, inf)).
+__device__ __forceinline__ float b2_log1pf(float x) {
+  const uint32_t ix = __float_as_uint(x);
+  if (!(x > -1.0f)) return x == -1.0f ? -INFINITY : NAN;
+  if (x == INFINITY) return x;
+  if ((ix & 0x7fffffffu) < 0x33800000u) return x;   // |x| < 2^-24: log1p(x) = x within half an ulp
+  const float ln2_hi = __uint_as_float(0x3f317180u), ln2_lo = __uint_as_float(0x3717f7d1u);
+  const float Lg1 = __uint_as_float(0x3f2aaaaau), Lg2 = __uint_as_float(0x3ecccce1u);
+  const float Lg3 = __uint_as_float(0x3e91e9eeu), Lg4 = __uint_as_float(0x3e789e26u);
+  int k = 1;
+  float f = x, c = 0.0f;
+  if (ix < 0x3ed413d0u || (ix >> 31)) {               // 1+x < sqrt(2)
+    if (ix <= 0xbe95f619u) k = 0;                      // sqrt(2)/2 <= 1+x: no reduction
+  }
+  if (k) {
+    const float u = __fadd_rn(1.0f, x);
+    uint32_t iu = __float_as_uint(u) + (0x3f800000u - 0x3f3504f3u);
+    k = (int)(iu >> 23) - 0x7f;
+    if (k < 25) {
+      c = k >= 2 ? __fadd_rn(1.0f, -__fadd_rn(u, -x)) : __fadd_rn(x, -__fadd_rn(u, -1.0f));
+      c = __fdiv_rn(c, u);
+    }
+    iu = (iu & 0x007fffffu) + 0x3f3504f3u;
+    f = __fadd_rn(__uint_as_float(iu), -1.0f);
+  }
+  const float s = __fdiv_rn(f, __fadd_rn(2.0f, f));
+  const float z = __fmul_rn(s, s), w = __fmul_rn(z, z);
+  const float t1 = __fmul_rn(w, __fadd_rn(Lg2, __fmul_rn(w, Lg4)));
+  const float t2 = __fmul_rn(z, __fadd_rn(Lg1, __fmul_rn(w, Lg3)));
+  const float R = __fadd_rn(t2, t1);
+  const float hfsq = __fmul_rn(__fmul_rn(0.5f, f), f);
+  const float dk = (float)k;
+  float r = __fadd_rn(__fadd_rn(__fmul_rn(dk, ln2_lo), -hfsq), f);
+  r = __fadd_rn(r, c);
+  r = __fadd_rn(__fmul_rn(s, __fadd_rn(hfsq, R)), r);
+  return __fadd_rn(r, __fmul_rn(dk, ln2_hi));
+}
+
+// objective ids (engine.cu kObj*): 0 reg:squarederror, 1 binary:logistic, 2 multi:softprob, 3 reg:logistic,
+// 4 binary:logitraw, 5 reg:squaredlogerror, 6 reg:pseudohubererror, 7 count:poisson, 8 reg:gamma, 9 reg:tweedie
+constexpr int kObjRegLogistic = 3, kObjLogitRaw = 4, kObjSquaredLog = 5, kObjPseudoHuber = 6, kObjPoisson = 7,
+              kObjGamma = 8, kObjTweedie = 9;
+// the parameter of an objective that has one: huber_slope, max_delta_step (Poisson hessian), tweedie_variance_power
+struct ObjParam { float a; };
+
+// margin -> prediction of one scalar output (ObjFunction::PredTransform): sigmoid, exp or identity
+__device__ __forceinline__ float b2_pred_transform(int objective, float m) {
+  if (objective == 1 || objective == kObjRegLogistic) return b2_sigmoid(m);
+  if (objective == kObjPoisson || objective == kObjGamma || objective == kObjTweedie) return b2_expf(m);
+  return m;
+}
+
+// (g, h) of one row before the weight, for the objectives added after the first three (the same IEEE sequence as
+// tests/objective_reference.py::gradients); `a` is the objective's parameter
+template <int kObjective>
+__device__ __forceinline__ float2 scalar_grad(float p, float y, float a) {
+  if (kObjective == kObjSquaredLog) {
+    const float kMin = -1.0f + 1e-6f;
+    const float q = p < kMin ? kMin : p;
+    const float lq = b2_log1pf(q), ly = b2_log1pf(y), q1 = __fadd_rn(q, 1.0f);
+    const float g = __fdiv_rn(__fadd_rn(lq, -ly), q1);
+    float h = __fdiv_rn(__fadd_rn(__fadd_rn(-lq, ly), 1.0f), __fmul_rn(q1, q1));
+    if (h < 1e-6f) h = 1e-6f;
+    return make_float2(g, h);
+  } else if (kObjective == kObjPseudoHuber) {
+    const float z = __fadd_rn(p, -y), zd = __fdiv_rn(z, a);
+    const float s = __fadd_rn(1.0f, __fmul_rn(zd, zd)), sq = __fsqrt_rn(s);
+    return make_float2(__fdiv_rn(z, sq), __fdiv_rn(1.0f, __fmul_rn(s, sq)));
+  } else if (kObjective == kObjPoisson) {
+    return make_float2(__fadd_rn(b2_expf(p), -y), b2_expf(__fadd_rn(p, a)));
+  } else if (kObjective == kObjGamma) {
+    const float r = __fdiv_rn(y, b2_expf(p));
+    return make_float2(__fadd_rn(1.0f, -r), r);
+  } else {   // kObjTweedie, a = rho
+    const float e1 = b2_expf(__fmul_rn(__fadd_rn(1.0f, -a), p)), e2 = b2_expf(__fmul_rn(__fadd_rn(2.0f, -a), p));
+    const float g = __fadd_rn(-__fmul_rn(y, e1), e2);
+    const float h = __fadd_rn(__fmul_rn(__fmul_rn(-y, __fadd_rn(1.0f, -a)), e1), __fmul_rn(__fadd_rn(2.0f, -a), e2));
+    return make_float2(g, h);
+  }
+}
+
 // gh layout: class-major [K][n] float2 so that each class tree reads a contiguous slice.
 // absmax (nullable, [K][2] uint32 float bit patterns, zeroed by the caller): max |g|, max |h| per class, gathered in
 // the same pass (the fixed-point scale of each class tree needs it; a separate pass re-read 8 bytes per row).
@@ -71,9 +157,9 @@ __device__ __forceinline__ void absmax_publish(float mg, float mh, uint32_t* __r
   }
 }
 
-// scalar objectives (reg:squarederror, binary:logistic): their own kernel so that the register budget of the softprob
-// path (2 x 16 running maxima) does not cut the occupancy of this streaming loop (72 registers -> 3 blocks per SM made
-// the 10M-row launch take 63 us instead of ~25)
+// scalar objectives (reg:squarederror, binary:logistic and its variants): their own kernel so that the register budget
+// of the softprob path (2 x 16 running maxima) does not cut the occupancy of this streaming loop (72 registers -> 3 blocks
+// per SM made the 10M-row launch take 63 us instead of ~25)
 template <int kObjective>
 __global__ void __launch_bounds__(256)
 gradient_scalar_kernel(const float* __restrict__ margin, const float* __restrict__ label, const float* __restrict__ weight,
@@ -95,6 +181,30 @@ gradient_scalar_kernel(const float* __restrict__ margin, const float* __restrict
     gh[i] = v;
     mg = fmaxf(mg, fabsf(v.x)); mh = fmaxf(mh, fabsf(v.y));
   }
+  if (absmax) absmax_publish(mg, mh, absmax);
+}
+
+// the objectives whose gradient can leave the finite range (exp, division by exp): a row with a non-finite g or h is
+// written as (0, 0), so that the quantisation scale and the tree of this round stay finite, and raises *err (zeroed by
+// the caller, read at the end of the round), which fails the round before its trees join the model
+template <int kObjective>
+__global__ void __launch_bounds__(256)
+gradient_param_kernel(const float* __restrict__ margin, const float* __restrict__ label, const float* __restrict__ weight,
+                      int64_t n, float scale_pos_weight, ObjParam op, float2* __restrict__ gh, uint32_t* __restrict__ absmax,
+                      uint32_t* __restrict__ err) {
+  float mg = 0.0f, mh = 0.0f;
+  bool bad = false;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float w = weight ? weight[i] : 1.0f;
+    const float y = label[i], m = margin[i];
+    if (kObjective == kObjSquaredLog && y == 1.0f) w = __fmul_rn(w, scale_pos_weight);   // RegLossObj: positive rows
+    const float2 r = scalar_grad<kObjective>(m, y, op.a);
+    float2 v = make_float2(__fmul_rn(r.x, w), __fmul_rn(r.y, w));
+    if (!(fabsf(v.x) <= FLT_MAX && fabsf(v.y) <= FLT_MAX)) { bad = true; v = make_float2(0.0f, 0.0f); }
+    gh[i] = v;
+    mg = fmaxf(mg, fabsf(v.x)); mh = fmaxf(mh, fabsf(v.y));
+  }
+  if (bad && err) atomicOr(err, 1u);
   if (absmax) absmax_publish(mg, mh, absmax);
 }
 
@@ -213,17 +323,31 @@ __global__ void quantize_kernel(const float2* __restrict__ gh, int64_t n, const 
   }
 }
 
-// metric sums (sum loss*w, sum w) -> out[2] doubles; metric: 0 rmse 1 logloss 2 error 3 mlogloss 4 merror
-// Metrics see the TRANSFORMED prediction (ObjFunction::EvalTransform, src/learner.cc): the probability for
-// binary:logistic, the raw value for reg:squarederror.  metric: 0 rmse, 1 logloss, 2 error, 3 mlogloss, 4 merror, 5 mae.
-__global__ void metric_kernel(int objective, int metric, int K, const float* __restrict__ margin, const float* __restrict__ label,
-                              const float* __restrict__ weight, int64_t n, double* __restrict__ out) {
+// metric sums (sum loss*w, sum w) -> out[2] doubles.  Metrics see the TRANSFORMED prediction (ObjFunction::EvalTransform,
+// src/learner.cc): the probability for binary:logistic / reg:logistic, exp(margin) for the log-link objectives, the raw
+// value otherwise.  metric: 0 rmse, 1 logloss, 2 error, 3 mlogloss, 4 merror, 5 mae, 7 rmsle, 8 mape, 9 mphe (a = huber
+// slope), 10 poisson-nloglik, 11 gamma-nloglik, 12 gamma-deviance, 13 tweedie-nloglik (a = rho); 6 (auc) is auc_kernel.cu.
+// the elementwise metrics of the objectives added after the first three, on the transformed prediction q
+__device__ __forceinline__ double scalar_metric(int metric, float a, double q, double y) {
+  if (metric == 7) { const double d = log1p(y) - log1p(fmax(q, -1.0 + 1e-6)); return d * d; }
+  if (metric == 8) return fabs((y - q) / y);
+  if (metric == 9) { const double z = (y - q) / (double)a; return (double)a * (double)a * (sqrt(1.0 + z * z) - 1.0); }
+  if (metric == 10) { const double qq = fmax(q, 1e-16); return lgamma(y + 1.0) + qq - y * log(qq); }
+  if (metric == 11) return y / q + log(q);
+  if (metric == 12) { const double qq = q + 1e-6, yy = y + 1e-6; return 2.0 * (log(qq / yy) + yy / qq - 1.0); }
+  const double r = (double)a;
+  return -y * pow(q, 1.0 - r) / (1.0 - r) + pow(q, 2.0 - r) / (2.0 - r);
+}
+
+__global__ void metric_kernel(int objective, int metric, int K, float a, const float* __restrict__ margin,
+                              const float* __restrict__ label, const float* __restrict__ weight, int64_t n,
+                              double* __restrict__ out) {
   double s = 0.0, ws = 0.0;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const double w = weight ? (double)weight[i] : 1.0;
     double v = 0.0;
     if (metric <= 2 || metric == 5) {
-      const float p = objective == 1 ? b2_sigmoid(margin[i]) : margin[i];
+      const float p = b2_pred_transform(objective, margin[i]);
       if (metric == 0) { const double d = (double)p - (double)label[i]; v = d * d; }
       else if (metric == 5) v = fabs((double)p - (double)label[i]);
       else if (metric == 1) {
@@ -232,6 +356,7 @@ __global__ void metric_kernel(int objective, int metric, int K, const float* __r
         v = -((double)y * log((double)a) + (1.0 - (double)y) * log((double)b));
       } else v = ((p > 0.5f) != (label[i] > 0.5f)) ? 1.0 : 0.0;
     }
+    else if (metric >= 7) v = scalar_metric(metric, a, (double)b2_pred_transform(objective, margin[i]), (double)label[i]);
     else {
       const float* r = margin + i * K; const int y = (int)label[i]; float mx = r[0]; int am = 0;
       for (int k = 1; k < K; ++k) if (r[k] > mx) { mx = r[k]; am = k; }
@@ -249,6 +374,21 @@ __global__ void metric_kernel(int objective, int metric, int K, const float* __r
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ws += __shfl_xor_sync(0xffffffffu, ws, o); }
   if ((threadIdx.x & 31) == 0) { atomicAdd(&out[0], s); atomicAdd(&out[1], ws); }
+}
+
+// label domain of an objective (checked once per train matrix): *bad |= 1 when some label is outside it (NaN included)
+__global__ void label_check_kernel(int objective, const float* __restrict__ label, int64_t n, uint32_t* __restrict__ bad) {
+  bool any = false;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float y = label[i];
+    bool ok = true;
+    if (objective == kObjRegLogistic || objective == kObjLogitRaw) ok = y >= 0.0f && y <= 1.0f;
+    else if (objective == kObjSquaredLog) ok = y > -1.0f;
+    else if (objective == kObjPoisson || objective == kObjTweedie) ok = y >= 0.0f;
+    else if (objective == kObjGamma) ok = y > 0.0f;
+    any |= !ok;
+  }
+  if (__any_sync(0xffffffffu, any) && (threadIdx.x & 31) == 0) atomicOr(bad, 1u);
 }
 
 // A.9 traversal on raw floats (the node step is b2_tree_step, common.cuh).  nodes of all trees are
@@ -272,16 +412,17 @@ __global__ void fill_kernel(float* out, int64_t n, float v) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = v;
 }
 
-// margin -> prediction transform in place (sigmoid / softmax)
+// margin -> prediction transform in place (sigmoid / exp / softmax)
 __global__ void transform_kernel(int objective, int K, float* __restrict__ m, int64_t n) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    if (objective == 1) m[i] = b2_sigmoid(m[i]);
-    else if (objective == 2) {
+    if (objective == 2) {
       float* r = m + i * K; float mx = r[0];
       for (int k = 1; k < K; ++k) if (r[k] > mx) mx = r[k];
       float s = 0.0f;
       for (int k = 0; k < K; ++k) { r[k] = b2_expf(__fadd_rn(r[k], -mx)); s = __fadd_rn(s, r[k]); }
       for (int k = 0; k < K; ++k) r[k] = __fdiv_rn(r[k], s);
+    } else {
+      m[i] = b2_pred_transform(objective, m[i]);
     }
   }
 }
@@ -299,11 +440,28 @@ static inline int grid_for(int64_t n, int num_sms) {
 extern "C" {
 int b2_gradient_fused_max_classes() { return b2::kFusedMaxK; }
 int b2_launch_gradient(int objective, int K, const float* margin, const float* label, const float* weight, int64_t n,
-                       float scale_pos_weight, float2* gh, uint32_t* absmax, int num_sms, cudaStream_t s) {
+                       float scale_pos_weight, float obj_param, float2* gh, uint32_t* absmax, uint32_t* err, int num_sms,
+                       cudaStream_t s) {
   if (n <= 0) return 0;
-  if (objective == 0) b2::gradient_scalar_kernel<0><<<grid_for(n, num_sms), 256, 0, s>>>(margin, label, weight, n, scale_pos_weight, gh, absmax);
-  else if (objective == 1) b2::gradient_scalar_kernel<1><<<grid_for(n, num_sms), 256, 0, s>>>(margin, label, weight, n, scale_pos_weight, gh, absmax);
-  else b2::gradient_softprob_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(K, margin, label, weight, n, gh, absmax);
+  const int g = grid_for(n, num_sms);
+  const b2::ObjParam op{obj_param};
+  switch (objective) {
+    case 0: b2::gradient_scalar_kernel<0><<<g, 256, 0, s>>>(margin, label, weight, n, scale_pos_weight, gh, absmax); break;
+    case 1: case b2::kObjRegLogistic: case b2::kObjLogitRaw:   // the logistic variants differ only in the transform
+      b2::gradient_scalar_kernel<1><<<g, 256, 0, s>>>(margin, label, weight, n, scale_pos_weight, gh, absmax); break;
+    case 2: b2::gradient_softprob_kernel<<<g, 256, 0, s>>>(K, margin, label, weight, n, gh, absmax); break;
+#define B2_PARAM_OBJ(id) \
+    case id: b2::gradient_param_kernel<id><<<g, 256, 0, s>>>(margin, label, weight, n, scale_pos_weight, op, gh, absmax, err); break;
+    B2_PARAM_OBJ(b2::kObjSquaredLog) B2_PARAM_OBJ(b2::kObjPseudoHuber) B2_PARAM_OBJ(b2::kObjPoisson)
+    B2_PARAM_OBJ(b2::kObjGamma) B2_PARAM_OBJ(b2::kObjTweedie)
+#undef B2_PARAM_OBJ
+    default: return (int)cudaErrorInvalidValue;
+  }
+  return (int)cudaGetLastError();
+}
+int b2_launch_label_check(int objective, const float* label, int64_t n, uint32_t* bad, int num_sms, cudaStream_t s) {
+  if (n <= 0) return 0;
+  b2::label_check_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(objective, label, n, bad);
   return (int)cudaGetLastError();
 }
 int b2_launch_subsample(float2* gh, int64_t n, uint32_t seed, uint32_t tree, uint32_t rank, double subsample, int num_sms,
@@ -336,10 +494,10 @@ int b2_launch_quantize(const float2* gh, int64_t n, const int32_t* qexp, int qbi
   b2::quantize_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(gh, n, qexp, qbits, q);
   return (int)cudaGetLastError();
 }
-int b2_launch_metric(int objective, int metric, int K, const float* margin, const float* label, const float* weight, int64_t n,
-                     double* out, int num_sms, cudaStream_t s) {
+int b2_launch_metric(int objective, int metric, int K, float metric_param, const float* margin, const float* label,
+                     const float* weight, int64_t n, double* out, int num_sms, cudaStream_t s) {
   if (n <= 0) return 0;
-  b2::metric_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(objective, metric, K, margin, label, weight, n, out);
+  b2::metric_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(objective, metric, K, metric_param, margin, label, weight, n, out);
   return (int)cudaGetLastError();
 }
 int b2_launch_predict(const float* X, int64_t n, int F, float missing, const B2TreeNodeDev* nodes,

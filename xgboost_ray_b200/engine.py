@@ -481,15 +481,51 @@ class callback:  # namespace shim: xgb.callback.TrainingCallback
 
 
 # ----------------------------------------------------------------------------- Booster
-_DEFAULT_METRIC = {"reg:squarederror": "rmse", "reg:linear": "rmse", "binary:logistic": "logloss",
-                   "multi:softprob": "mlogloss", "multi:softmax": "mlogloss"}
+# Everything the Python side knows about an objective, in one place: its default eval metric, the margin -> prediction
+# transform, and the parameter block of xgboost 2.x's JSON model ({json key: default}; "num_class" is the model's class
+# count).  The engine (csrc/engine.cu) owns the gradients.
+class _Objective:
+    def __init__(self, metric, transform, block=None, block_params=None):
+        self.metric, self.transform, self.block, self.block_params = metric, transform, block, block_params or {}
+
+    def default_metric(self, params):
+        if self.metric == "tweedie-nloglik":   # the metric carries the objective's variance power in its name
+            return "tweedie-nloglik@%g" % float(params.get("tweedie_variance_power", 1.5))
+        return self.metric
+
+
+_REG_LOSS = ("reg_loss_param", {"scale_pos_weight": 1})
+_SOFTMAX = ("softmax_multiclass_param", {"num_class": None})
+_OBJECTIVES = {
+    "reg:squarederror": _Objective("rmse", None, *_REG_LOSS),
+    "reg:linear": _Objective("rmse", None, *_REG_LOSS),
+    "reg:logistic": _Objective("rmse", "sigmoid", *_REG_LOSS),
+    "binary:logistic": _Objective("logloss", "sigmoid", *_REG_LOSS),
+    "binary:logitraw": _Objective("logloss", None, *_REG_LOSS),
+    "reg:squaredlogerror": _Objective("rmsle", None, *_REG_LOSS),
+    "reg:pseudohubererror": _Objective("mphe", None, "pseudo_huber_param", {"huber_slope": 1}),
+    "count:poisson": _Objective("poisson-nloglik", "exp", "poisson_regression_param", {"max_delta_step": 0.7}),
+    "reg:gamma": _Objective("gamma-nloglik", "exp"),
+    "reg:tweedie": _Objective("tweedie-nloglik", "exp", "tweedie_regression_param", {"tweedie_variance_power": 1.5}),
+    "multi:softprob": _Objective("mlogloss", "softmax", *_SOFTMAX),
+    "multi:softmax": _Objective("mlogloss", "softmax", *_SOFTMAX),
+}
+
+
+def _objective(name):
+    o = _OBJECTIVES.get(name)
+    if o is None:
+        raise XGBoostError("unsupported objective '%s' (supported: %s)" % (name, ", ".join(sorted(_OBJECTIVES))))
+    return o
+
+
 _TREE_FIELDS = ("left", "right", "parent", "split_feature", "split_bin", "split_cond", "default_left", "value",
                 "base_weight", "loss_chg", "sum_hess")
 _ENGINE_KEYS = ("objective", "num_class", "max_depth", "eta", "learning_rate", "gamma", "min_split_loss",
                 "min_child_weight", "lambda", "reg_lambda", "alpha", "reg_alpha", "base_score", "hist_qbits",
                 "hist_chunk_rows", "profile", "max_cat_to_onehot", "max_cat_threshold", "scale_pos_weight",
                 "max_delta_step", "subsample", "colsample_bytree", "colsample_bylevel", "colsample_bynode", "seed",
-                "random_state", "num_parallel_tree")
+                "random_state", "num_parallel_tree", "huber_slope", "tweedie_variance_power")
 
 # xgboost parameters that change the trained model and that this engine does not implement: a value different
 # from the neutral one is an error, never silently ignored (a drop-in must not train a different model quietly)
@@ -703,7 +739,7 @@ class Booster:
     def _metric_names(self):
         m = self.params.get("eval_metric")
         if m is None:
-            return [_DEFAULT_METRIC[self.params.get("objective", "reg:squarederror")]]
+            return [_objective(self.params.get("objective", "reg:squarederror")).default_metric(self.params)]
         return list(m) if isinstance(m, (list, tuple)) else [m]
 
     def eval_set(self, evals, iteration=0, feval=None, output_margin=True):
@@ -868,10 +904,11 @@ class Booster:
             cache.append((self._tree_json(i, src[i], self.n_features), [int(x) for x in src[i]["split_bin"]]))
         trees = [c[0] for c in cache]
         obj = self.params.get("objective", "reg:squarederror")
-        if obj.startswith("multi:"):
-            obj_block = {"name": obj, "softmax_multiclass_param": {"num_class": str(K)}}
-        else:
-            obj_block = {"name": obj, "reg_loss_param": {"scale_pos_weight": _num_str(self.params.get("scale_pos_weight", 1))}}
+        spec = _OBJECTIVES.get(obj, _OBJECTIVES["reg:squarederror"])
+        obj_block = {"name": obj}
+        if spec.block:
+            obj_block[spec.block] = {k: str(K) if k == "num_class" else _num_str(self.params.get(k, d))
+                                     for k, d in spec.block_params.items()}
         attrs = {k: str(v) for k, v in self._attrs.items() if not k.startswith("b2.")}
         attrs["b2.params"] = json.dumps({k: self.params[k] for k in sorted(self.params) if _json_ok(self.params[k]) and
                                          k not in ("objective", "num_class", "base_score", "scale_pos_weight", "num_parallel_tree")})   # those have their own fields
@@ -922,6 +959,11 @@ class Booster:
         spw = L["objective"].get("reg_loss_param", {}).get("scale_pos_weight")
         if spw is not None and float(spw) != 1.0:
             params["scale_pos_weight"] = float(spw)
+        spec = _OBJECTIVES.get(params["objective"])
+        if spec is not None and spec.block not in (None, "reg_loss_param", "softmax_multiclass_param"):
+            for k, v in L["objective"].get(spec.block, {}).items():
+                if k in spec.block_params:
+                    params[k] = float(v)
         params["base_score"] = float(L["learner_model_param"]["base_score"])
         npt = int(L["gradient_booster"]["model"].get("gbtree_model_param", {}).get("num_parallel_tree", "1"))
         if npt > 1:
@@ -1125,9 +1167,12 @@ def _dump_text(t, nid, depth, names, with_stats, lines):
 
 
 def _transform(objective, m):
-    if objective == "binary:logistic":
+    t = _OBJECTIVES[objective].transform if objective in _OBJECTIVES else None
+    if t == "sigmoid":
         return (1.0 / (1.0 + np.exp(-m.astype(np.float64)))).astype(np.float32)
-    if objective.startswith("multi:"):
+    if t == "exp":
+        return np.exp(m.astype(np.float64)).astype(np.float32)
+    if t == "softmax":
         e = np.exp(m - m.max(axis=1, keepdims=True))
         return (e / e.sum(axis=1, keepdims=True)).astype(np.float32)
     return m
