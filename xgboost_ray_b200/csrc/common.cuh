@@ -167,6 +167,27 @@ struct B2ColSample {
   uint32_t seed, tree;
 };
 
+// what the last CTA of a level's partition does once every row is placed (level_finalize.cuh)
+struct B2FinalizeArgs {
+  B2LevelCtl* ctl_nxt;
+  B2NodeSeg* seg_nxt;
+  B2EvalNode* ev_nxt;
+  const int32_t* pair_parent_hist;
+  B2HistWork* hist_work;
+  int32_t* triples;
+  long long* stat_rows;
+  uint32_t* done;               // CTAs of the partition that finished; the last one resets it to 0
+  int32_t max_pairs, need_hist, n_streams, window_rows, chunk_rows_override;
+};
+
+// sibling = parent - built inside the split scan (split_kernel.cu eval_splits_kernel), instead of a separate pass
+struct B2SiblingSub {
+  const long long* parent_level;   // nullptr: every node's slot already holds its histogram
+  const int32_t* triples;          // [pair][3]: parent slot (previous level), built slot, sibling slot
+  long long* sib_out;              // nullable: store the siblings here (the level buffer) for the next level's parents
+  int32_t sib_base;                // first sibling slot of the level
+};
+
 // ---- peer-memory exchange over NVLink / NVSwitch (p2p.cuh, p2p_exchange.cu, control_kernel.cu)
 // Every rank maps four regions of every peer (cudaIpc): the histogram build buffer (peers READ their owned slices out
 // of it), and three tables the peers WRITE into -- split candidates, per-tree |g|,|h| maxima + leaf sums, and epoch

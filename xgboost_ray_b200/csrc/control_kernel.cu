@@ -160,75 +160,6 @@ decide_kernel(B2LevelCtl* __restrict__ ctl_cur, B2LevelCtl* __restrict__ ctl_nxt
   }
 }
 
-// ---- finalize a level after its partition: child segments, build-child choice, next hist work list
-__global__ void __launch_bounds__(kCtlThreads)
-finalize_level_kernel(const B2LevelCtl* __restrict__ ctl_cur, B2LevelCtl* __restrict__ ctl_nxt, B2NodeSeg* __restrict__ seg_nxt,
-                      B2EvalNode* __restrict__ ev_nxt, const B2SplitWork* __restrict__ split_work,
-                      const int32_t* __restrict__ counters, const int32_t* __restrict__ pair_parent_hist,
-                      B2HistWork* __restrict__ hist_work, int32_t* __restrict__ triples, int max_pairs, int need_hist,
-                      int n_streams, int window_rows, int chunk_rows_override, long long* __restrict__ stat_rows) {
-  __shared__ typename TileScan::Scan::TempStorage tmp;
-  __shared__ long long s_rows;
-  __shared__ int s_chunk_rows;
-  const int ns = ctl_cur->n_split;
-  if (threadIdx.x == 0) s_rows = 0;
-  __syncthreads();
-  // pass 1: segments + total rows to build
-  long long my_rows = 0;
-  for (int j = threadIdx.x; j < ns; j += kCtlThreads) {
-    const B2SplitWork sw = split_work[j];
-    const int cl = counters[2 * j];
-    B2NodeSeg sl = seg_nxt[2 * j], sr = seg_nxt[2 * j + 1];
-    sl.begin = sw.seg_begin; sl.count = cl;
-    sr.begin = sw.seg_begin + cl; sr.count = sw.seg_count - cl;
-    seg_nxt[2 * j] = sl; seg_nxt[2 * j + 1] = sr;
-    if (need_hist) {
-      const bool build_left = ev_nxt[2 * j].sum_h < ev_nxt[2 * j + 1].sum_h;   // smaller hessian (A.5)
-      my_rows += build_left ? sl.count : sr.count;
-    }
-  }
-  if (need_hist) {
-    atomicAdd((unsigned long long*)&s_rows, (unsigned long long)my_rows);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      int c = chunk_rows_override;
-      if (c <= 0) {
-        // large levels: ~4 chunks per CTA stream for balance; small levels: ~1, because every extra
-        // (CTA, node) pair costs a full 16K-cell flush
-        const long long per_stream = s_rows / n_streams;
-        const long long target = per_stream >= 16384 ? per_stream / 4 : per_stream;
-        c = 512;
-        while (c < target && c < 8192) c <<= 1;
-      }
-      if (c > window_rows) c = window_rows;   // one chunk = one int32 window
-      s_chunk_rows = c;
-      if (stat_rows) *stat_rows = s_rows;
-    }
-    __syncthreads();
-    const int chunk_rows = s_chunk_rows;
-    TileScan scan(&tmp);
-    for (int base = 0; base < ns; base += kCtlThreads) {
-      const int j = base + threadIdx.x;
-      int chunks = 0, begin = 0, count = 0;
-      if (j < ns) {
-        const bool build_left = ev_nxt[2 * j].sum_h < ev_nxt[2 * j + 1].sum_h;
-        const int b = build_left ? 2 * j : 2 * j + 1, s = b ^ 1;
-        begin = seg_nxt[b].begin; count = seg_nxt[b].count;
-        chunks = (count + chunk_rows - 1) / chunk_rows;
-        ev_nxt[b].hist_index = j; ev_nxt[s].hist_index = max_pairs + j;
-        triples[3 * j] = pair_parent_hist[j]; triples[3 * j + 1] = j; triples[3 * j + 2] = max_pairs + j;
-      }
-      const int cb = scan.step(chunks);
-      if (j < ns) { B2HistWork w; w.seg_begin = begin; w.seg_count = count; w.hist_index = j; w.chunk_begin = cb; hist_work[j] = w; }
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      ctl_nxt->hist_n_work = ns; ctl_nxt->hist_total_chunks = scan.carry; ctl_nxt->hist_chunk_rows = chunk_rows;
-      ctl_nxt->n_pairs = ns;
-    }
-  }
-}
-
 // ---- leaves: chunked work list over the leaf segments
 __global__ void __launch_bounds__(kCtlThreads)
 leaf_plan_kernel(const B2LeafDev* __restrict__ leaves, const int32_t* __restrict__ n_leaves, B2SegWork* __restrict__ work,
@@ -251,11 +182,13 @@ leaf_plan_kernel(const B2LeafDev* __restrict__ leaves, const int32_t* __restrict
   if (threadIdx.x == 0) { leaf_ctl->hist_n_work = n; leaf_ctl->hist_total_chunks = scan.carry; }
 }
 
-// leaf weight from the 40-bit fixed-point sums (A.7 leaf refinement), value = weight * eta (fp32)
+// leaf weight from the 40-bit fixed-point sums (A.7 leaf refinement), value = weight * eta (fp32); also keeps the
+// tree's quantisation exponents in its read-back block (qexp_out)
 __global__ void leaf_values_kernel(const B2LeafDev* __restrict__ leaves, const int32_t* __restrict__ n_leaves,
                                    const long long* __restrict__ sums, const int32_t* __restrict__ qexp, int leaf_bits,
-                                   B2CtlParams p, float* __restrict__ leaf_value, B2TreeDev tree) {
+                                   B2CtlParams p, float* __restrict__ leaf_value, B2TreeDev tree, int32_t* __restrict__ qexp_out) {
   const int n = *n_leaves;
+  if (blockIdx.x == 0 && threadIdx.x < 2) qexp_out[threadIdx.x] = qexp[threadIdx.x];
   const double kg = ldexp(1.0, leaf_bits - qexp[0]), kh = ldexp(1.0, leaf_bits - qexp[1]);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const double G = __ddiv_rn(__ll2double_rn(sums[2 * i]), kg), H = __ddiv_rn(__ll2double_rn(sums[2 * i + 1]), kh);
@@ -281,10 +214,6 @@ __global__ void tree_init_kernel(B2TreeDev tree, B2LevelCtl* ctl0, B2NodeSeg* se
     B2EvalNode e; e.sum_g = 0; e.sum_h = 0; e.hist_index = 0; e.root_gain = 0.f; ev0[0] = e;
   }
 }
-// after root_totals: copy the root sums into the tree table
-__global__ void root_record_kernel(B2TreeDev tree, const B2EvalNode* ev0) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) { tree.sum_g[0] = ev0[0].sum_g; tree.sum_h[0] = ev0[0].sum_h; }
-}
 
 }  // namespace b2
 
@@ -301,31 +230,18 @@ int b2_launch_decide(B2LevelCtl* ctl_cur, B2LevelCtl* ctl_nxt, const B2NodeSeg* 
                                                  part_counters, local_cands, p2p ? 1 : 0, pp);
   return (int)cudaGetLastError();
 }
-int b2_launch_finalize_level(const B2LevelCtl* ctl_cur, B2LevelCtl* ctl_nxt, B2NodeSeg* seg_nxt, B2EvalNode* ev_nxt,
-                             const B2SplitWork* split_work, const int32_t* counters, const int32_t* pair_parent_hist,
-                             B2HistWork* hist_work, int32_t* triples, int max_pairs, int need_hist, int n_streams,
-                             int window_rows, int chunk_rows_override, long long* stat_rows, cudaStream_t s) {
-  b2::finalize_level_kernel<<<1, b2::kCtlThreads, 0, s>>>(ctl_cur, ctl_nxt, seg_nxt, ev_nxt, split_work, counters,
-                                                         pair_parent_hist, hist_work, triples, max_pairs, need_hist, n_streams,
-                                                         window_rows, chunk_rows_override, stat_rows);
-  return (int)cudaGetLastError();
-}
 int b2_launch_leaf_plan(const B2LeafDev* leaves, const int32_t* n_leaves, B2SegWork* work, B2LevelCtl* leaf_ctl, cudaStream_t s) {
   b2::leaf_plan_kernel<<<1, b2::kCtlThreads, 0, s>>>(leaves, n_leaves, work, leaf_ctl);
   return (int)cudaGetLastError();
 }
 int b2_launch_leaf_values(const B2LeafDev* leaves, const int32_t* n_leaves, const long long* sums, const int32_t* qexp,
-                          int leaf_bits, B2CtlParams p, float* leaf_value, B2TreeDev tree, cudaStream_t s) {
-  b2::leaf_values_kernel<<<8, 256, 0, s>>>(leaves, n_leaves, sums, qexp, leaf_bits, p, leaf_value, tree);
+                          int leaf_bits, B2CtlParams p, float* leaf_value, B2TreeDev tree, int32_t* qexp_out, cudaStream_t s) {
+  b2::leaf_values_kernel<<<8, 256, 0, s>>>(leaves, n_leaves, sums, qexp, leaf_bits, p, leaf_value, tree, qexp_out);
   return (int)cudaGetLastError();
 }
 int b2_launch_tree_init(B2TreeDev tree, B2LevelCtl* ctl0, B2NodeSeg* seg0, B2EvalNode* ev0, int32_t* n_leaves, int n_rows,
                         B2HistWork* hist_work0, cudaStream_t s) {
   b2::tree_init_kernel<<<1, 32, 0, s>>>(tree, ctl0, seg0, ev0, n_leaves, n_rows, hist_work0);
-  return (int)cudaGetLastError();
-}
-int b2_launch_root_record(B2TreeDev tree, const B2EvalNode* ev0, cudaStream_t s) {
-  b2::root_record_kernel<<<1, 32, 0, s>>>(tree, ev0);
   return (int)cudaGetLastError();
 }
 }

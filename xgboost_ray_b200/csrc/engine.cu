@@ -41,7 +41,7 @@ int b2_launch_hist_tma(const uint8_t*, int, const void*, const int2*, const int3
 int b2_launch_hist_subtract(const long long*, long long*, const int32_t*, int, int64_t, const B2LevelCtl*, cudaStream_t);
 int b2_launch_eval_splits(const long long*, int, const B2EvalNode*, int, const int32_t*, const int32_t*, const int32_t*,
                           const uint8_t*, const uint8_t*, const int32_t*, int, B2TrainParamDev, B2SplitCand*, int, const B2LevelCtl*,
-                          int, int, B2ColSample, const B2NodeSeg*, cudaStream_t);
+                          int, int, B2ColSample, const B2NodeSeg*, B2SiblingSub, cudaStream_t);
 int b2_launch_subsample(float2*, int64_t, uint32_t, uint32_t, uint32_t, double, int, cudaStream_t);
 int b2_p2p_flag_words(int);
 int b2_launch_p2p_reduce_subtract(const void*, const long long*, long long*, const int32_t*, const B2LevelCtl*, int, int, int64_t, int,
@@ -54,6 +54,8 @@ int b2_launch_gather_interleaved_rows(const void*, float*, int, cudaStream_t);
 int b2_launch_final_assign(const uint8_t*, int64_t, const int32_t*, const B2SplitWork*, const B2LevelCtl*, int, const float2*,
                            const int32_t*, int, long long*, uint16_t*, int, int, cudaStream_t);
 int b2_launch_margin_update(float*, int, int, const uint16_t*, const float*, int64_t, int, cudaStream_t);
+int b2_leaf_acc_max_depth();
+int b2_launch_leaf_accumulate(const float2*, const uint16_t*, int64_t, int, const int32_t*, int, long long*, int, cudaStream_t);
 int b2_gradient_fused_max_classes();
 int b2_launch_sum_fixed(const float2*, int64_t, const int32_t*, int, long long*, int, cudaStream_t);
 int b2_cat_ctas();
@@ -61,11 +63,12 @@ int b2_launch_eval_cat_splits(const long long*, int, const B2EvalNode*, int, con
                               const int32_t*, int, B2TrainParamDev, B2SplitCand*, int, int, const B2LevelCtl*, int, int,
                               B2ColSample, const B2NodeSeg*, cudaStream_t);
 int b2_launch_cat_stats(const float*, int64_t, int, float, const int32_t*, int, int32_t*, int, cudaStream_t);
-int b2_launch_root_totals(const long long*, int, B2EvalNode*, const int32_t*, int, B2TrainParamDev, int, cudaStream_t);
+int b2_launch_root_totals(const long long*, int, B2EvalNode*, const int32_t*, int, B2TrainParamDev, int, long long*, long long*,
+                          cudaStream_t);
 int b2_part_chunk_rows();
 int b2_split_chunk_rows();
 int b2_launch_partition(const uint8_t*, int64_t, const int32_t*, int32_t*, const B2SplitWork*, const B2LevelCtl*, int, int32_t*,
-                        int, int, cudaStream_t);
+                        int, B2FinalizeArgs, int, cudaStream_t);
 int b2_launch_leaf_sums(const float2*, const int32_t*, const int32_t*, const void*, const B2LevelCtl*, int, const int32_t*, int,
                         long long*, uint16_t*, int, cudaStream_t);
 int b2_launch_pred_update(float*, int, int, const int32_t*, const int32_t*, const void*, const B2LevelCtl*, int, const float*, int,
@@ -73,13 +76,10 @@ int b2_launch_pred_update(float*, int, int, const int32_t*, const int32_t*, cons
 int b2_launch_decide(B2LevelCtl*, B2LevelCtl*, const B2NodeSeg*, B2NodeSeg*, const B2EvalNode*, B2EvalNode*, const B2SplitCand*,
                      int, int, int, int, B2TreeDev, B2SplitWork*, int32_t*, B2LeafDev*, int32_t*, const uint8_t*, const int32_t*, int,
                      B2CtlParams, int32_t*, const B2SplitCand*, const void*, cudaStream_t);
-int b2_launch_finalize_level(const B2LevelCtl*, B2LevelCtl*, B2NodeSeg*, B2EvalNode*, const B2SplitWork*, const int32_t*,
-                             const int32_t*, B2HistWork*, int32_t*, int, int, int, int, int, long long*, cudaStream_t);
 int b2_launch_leaf_plan(const B2LeafDev*, const int32_t*, B2SegWork*, B2LevelCtl*, cudaStream_t);
 int b2_launch_leaf_values(const B2LeafDev*, const int32_t*, const long long*, const int32_t*, int, B2CtlParams, float*, B2TreeDev,
-                          cudaStream_t);
+                          int32_t*, cudaStream_t);
 int b2_launch_tree_init(B2TreeDev, B2LevelCtl*, B2NodeSeg*, B2EvalNode*, int32_t*, int, B2HistWork*, cudaStream_t);
-int b2_launch_root_record(B2TreeDev, const B2EvalNode*, cudaStream_t);
 int b2_launch_iota(int32_t*, int64_t, cudaStream_t);
 int b2_launch_gradient(int, int, const float*, const float*, const float*, int64_t, float, float, float2*, uint32_t*, uint32_t*, int,
                        cudaStream_t);
@@ -790,7 +790,7 @@ struct Booster : HandleBase {
   View<B2SplitCand> d_cands_all;    // candidates of all ranks [shards][nodes][cpn]
   int shards = 1, log2_shards = 0, sp = 32, cpn = 1;   // cpn = candidates per node (numeric CTAs + categorical CTAs)
   int cpn_num = 1;
-  DevBuf<uint32_t> t_cat;                  // [max_nodes][8] category sets of the tree being grown
+  View<uint32_t> t_cat;                    // [max_nodes][8] category sets of the tree being grown (in t_block)
   DevBuf<uint8_t> d_col_masks;             // [max_depth][F] level feature sets of the tree being grown (column sampling)
   // NVLink peer-memory exchange (p2p.cuh, p2p_exchange.cu): on when every rank mapped its peers; B2_EXCHANGE=nccl keeps NCCL
   struct P2PState {
@@ -823,13 +823,17 @@ struct Booster : HandleBase {
   DevBuf<uint32_t> d_absmax; DevBuf<int32_t> d_qexp;
   // device-resident control tables of the sync-free level loop (control_kernel.cu)
   int ctl_depth = 0;                       // max_depth the tables are sized for
-  DevBuf<int32_t> t_i32;                   // 6 int32 arrays [max_nodes] + n_nodes + n_leaves
-  DevBuf<float> t_f32;                     // loss_chg, leaf_weight, leaf_value [max_nodes]
-  DevBuf<long long> t_i64;                 // sum_g, sum_h [max_nodes] + level_rows [max_depth+1]
+  // the tree being grown, laid out as its pinned read-back block (TreeLayout) so that one copy brings it back
+  DevBuf<uint8_t> t_block;
+  View<int32_t> t_i32;                     // 7 int32 arrays [max_nodes] + n_nodes + n_leaves
+  View<float> t_f32;                       // loss_chg, leaf_weight, leaf_value [max_nodes]
+  View<long long> t_i64;                   // sum_g, sum_h [max_nodes] + level_rows [max_depth+1]
+  View<int32_t> t_qexp;                    // the tree's quantisation exponents (written by leaf_values_kernel)
   DevBuf<B2LevelCtl> d_ctl;                // [0],[1] level ping-pong, [2] leaf pass
   DevBuf<B2NodeSeg> d_seg[2]; DevBuf<B2EvalNode> d_ev[2];
   DevBuf<B2HistWork> d_hist_work; DevBuf<B2SplitWork> d_split_work; DevBuf<B2SegWork> d_seg_work;
   DevBuf<B2SplitCand> d_cands; DevBuf<int32_t> d_counters, d_triples, d_pair_parent;
+  DevBuf<uint32_t> d_part_done;            // CTAs of a partition that finished (zero between launches: the last resets it)
   DevBuf<B2LeafDev> d_leaves;
   DevBuf<long long> d_leaf_sums; DevBuf<float> d_leaf_values; DevBuf<double> d_metric;
   std::vector<void*> staging;              // pinned host copies of finished trees, one per class tree of a round
@@ -1115,12 +1119,15 @@ void ensure_ctl_tables(Booster* b) {
   b->ctl_depth = D;
   const TreeLayout L = tree_layout(D);
   const size_t lcap = (size_t)1 << D, half = (size_t)1 << (D > 0 ? D - 1 : 0);
-  b->t_i32.ensure(L.i32_count); b->t_f32.ensure(L.f32_count); b->t_i64.ensure(L.i64_count);
-  b->t_cat.ensure(b->train->any_cat() ? L.max_nodes * 8 : 8);
+  b->t_block.ensure(L.bytes);
+  b->t_i32.p = (int32_t*)b->t_block.p; b->t_f32.p = (float*)(b->t_block.p + L.off_f32);
+  b->t_i64.p = (long long*)(b->t_block.p + L.off_i64); b->t_qexp.p = (int32_t*)(b->t_block.p + L.off_qexp);
+  b->t_cat.p = (uint32_t*)(b->t_block.p + L.off_cat);
   b->d_ctl.ensure(3);
   for (int k = 0; k < 2; ++k) { b->d_seg[k].ensure(lcap); b->d_ev[k].ensure(lcap); }
   b->d_hist_work.ensure(half); b->d_split_work.ensure(half);
   b->d_counters.ensure(2 * half); b->d_triples.ensure(3 * half); b->d_pair_parent.ensure(half);
+  if (!b->d_part_done.p) { b->d_part_done.ensure(1); CUDA_CHECK(cudaMemsetAsync(b->d_part_done.p, 0, sizeof(uint32_t), b->ctx->stream)); }
   b->d_leaves.ensure(L.max_nodes); b->d_seg_work.ensure(L.max_nodes);
   b->d_leaf_sums.ensure(2 * lcap); b->d_leaf_values.ensure(lcap);
   b->node_elems = (size_t)G * B2_GROUP_ELEMS;
@@ -1235,6 +1242,11 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   const bool multi = b->comm && b->comm->world > 1;
   const bool p2p = multi && b->p2p.enabled;
   static const bool leaf_fused = env_flag("B2_LEAF_FUSED", true);
+  // leaf sums from a streaming pass over (pos, gh) in row order; needs one shared-memory accumulator per leaf
+  const bool leaf_stream = leaf_fused && D >= 1 && D <= b2_leaf_acc_max_depth();
+  // sibling subtraction inside eval_splits_kernel (no hist_subtract pass).  The peer-memory exchange subtracts while it
+  // reduces, and the categorical scan reads the sibling slots itself, so both keep the stored siblings.
+  const bool sub_in_scan = !p2p && !m->any_cat();
   mark_phase(b, -1);
   // ---- fixed-point quantisation (global scale via max over the ranks)
   const uint32_t tree_index = (uint32_t)b->trees.size() + (uint32_t)slot;   // position of this tree in the model (sampling seed)
@@ -1321,9 +1333,8 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   }
   mark_phase(b, 1);
   exchange_and_subtract(b, st, nullptr, b->hist[0].p, nullptr, nullptr, 1, 1);
-  LAUNCH_CHECK(b2_launch_root_totals(b->hist[0].p, G, b->d_ev[0].p, b->d_qexp.p, p.qbits, dp, sh, s));
-  LAUNCH_CHECK(b2_launch_root_record(tree, b->d_ev[0].p, s));
-  st.kernel_launches += 3;
+  LAUNCH_CHECK(b2_launch_root_totals(b->hist[0].p, G, b->d_ev[0].p, b->d_qexp.p, p.qbits, dp, sh, tree.sum_g, tree.sum_h, s));
+  st.kernel_launches += 2;
   int hb = 0;  // hist buffer holding the current level
   for (int d = 0; d <= D; ++d) {
     const int cur = d & 1, nxt = cur ^ 1;
@@ -1338,9 +1349,16 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
       cs.fwq = m->fwq.empty() ? nullptr : m->d_fwq.p;
       cs.bynode = (double)p.colsample_bynode; cs.n_level = n_level_feats[d]; cs.n_features = m->F;
       cs.seed = (uint32_t)p.seed; cs.tree = p.use_cols() ? tree_index : 0u;
+      // siblings of this level: parent (previous level buffer) - built, formed in the scan; stored only when the next
+      // level takes them as parents
+      B2SiblingSub sub{nullptr, nullptr, nullptr, 0};
+      if (sub_in_scan && d > 0) {
+        sub.parent_level = b->hist[hb ^ 1].p; sub.triples = b->d_triples.p;
+        sub.sib_out = d + 1 < D ? b->hist[hb].p : nullptr; sub.sib_base = max_nodes_level / 2;
+      }
       LAUNCH_CHECK(b2_launch_eval_splits(b->hist[hb].p, G, b->d_ev[cur].p, max_nodes_level, m->d_group_first.p, m->d_group_size.p,
                                          m->d_nbins.p, m->d_has_missing.p, m->any_cat() ? m->d_is_cat.p : nullptr, b->d_qexp.p,
-                                         p.qbits, dp, b->d_cands.p, b->cpn, ctl + cur, sh, shard_rank, cs, b->d_seg[cur].p, s));
+                                         p.qbits, dp, b->d_cands.p, b->cpn, ctl + cur, sh, shard_rank, cs, b->d_seg[cur].p, sub, s));
       st.kernel_launches++;
       if (m->any_cat()) {
         LAUNCH_CHECK(b2_launch_eval_cat_splits(b->hist[hb].p, G, b->d_ev[cur].p, max_nodes_level, m->d_cat_feats.p,
@@ -1367,27 +1385,32 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
     if (!can_split) break;
     const int32_t* ridx_in = d == 0 ? nullptr : b->ridx[cur].p;   // the root's rows are the identity list
     if (last_split_level && leaf_fused) {
-      // ---- the children of this level are leaves: no ordered index lists any more.  Leaves that stopped earlier are
-      // summed from their segments, rows of the nodes that split here are assigned in one pass (partition_kernel.cu)
+      // ---- the children of this level are leaves: no ordered index lists any more.  Leaves that stopped earlier get
+      // their rows' leaf index from their segments, rows of the nodes that split here are assigned in one pass
+      // (partition_kernel.cu).  With leaf_stream the sums are left to leaf_accumulate_kernel after the last decide.
+      long long* sums = leaf_stream ? nullptr : b->d_leaf_sums.p;
       LAUNCH_CHECK(b2_launch_leaf_plan(b->d_leaves.p, &ctl[cur].leaf_base_next, b->d_seg_work.p, ctl + 2, s));
       LAUNCH_CHECK(b2_launch_leaf_sums(gh, b->ridx[0].p, b->ridx[1].p, b->d_seg_work.p, ctl + 2, max_leaf_chunks, b->d_qexp.p, 40,
-                                       b->d_leaf_sums.p, b->pos.p, ctx->num_sms, s));
+                                       sums, b->pos.p, ctx->num_sms, s));
       LAUNCH_CHECK(b2_launch_final_assign(m->bins_col.p, m->col_stride, ridx_in, b->d_split_work.p, ctl + cur,
-                                          max_part_chunks_total + max_nodes_level, gh, b->d_qexp.p, 40, b->d_leaf_sums.p, b->pos.p,
+                                          max_part_chunks_total + max_nodes_level, gh, b->d_qexp.p, 40, sums, b->pos.p,
                                           m->any_cat() ? 1 : 0, ctx->num_sms, s));
       st.kernel_launches += 3;
       mark_phase(b, 5);
       continue;
     }
-    // ---- partition rows of the expanding nodes into the other index list (decide zeroed the counters)
-    LAUNCH_CHECK(b2_launch_partition(m->bins_col.p, m->col_stride, ridx_in, b->ridx[nxt].p, b->d_split_work.p, ctl + cur,
-                                     max_part_chunks_total + max_nodes_level, b->d_counters.p, m->any_cat() ? 1 : 0,
-                                     ctx->num_sms, s));
+    // ---- partition rows of the expanding nodes into the other index list (decide zeroed the counters); the last CTA
+    // of the partition finalises the level: child segments, build-child choice, next histogram work list
     const bool need_hist = d + 1 < D;
-    LAUNCH_CHECK(b2_launch_finalize_level(ctl + cur, ctl + nxt, b->d_seg[nxt].p, b->d_ev[nxt].p, b->d_split_work.p, b->d_counters.p,
-                                          b->d_pair_parent.p, b->d_hist_work.p, b->d_triples.p, max_nodes_level, need_hist ? 1 : 0,
-                                          n_streams, window, p.hist_chunk_rows, d_level_rows + d + 1, s));
-    st.kernel_launches += 2;
+    B2FinalizeArgs fin;
+    fin.ctl_nxt = ctl + nxt; fin.seg_nxt = b->d_seg[nxt].p; fin.ev_nxt = b->d_ev[nxt].p; fin.pair_parent_hist = b->d_pair_parent.p;
+    fin.hist_work = b->d_hist_work.p; fin.triples = b->d_triples.p; fin.stat_rows = d_level_rows + d + 1; fin.done = b->d_part_done.p;
+    fin.max_pairs = max_nodes_level; fin.need_hist = need_hist ? 1 : 0; fin.n_streams = n_streams; fin.window_rows = window;
+    fin.chunk_rows_override = p.hist_chunk_rows;
+    LAUNCH_CHECK(b2_launch_partition(m->bins_col.p, m->col_stride, ridx_in, b->ridx[nxt].p, b->d_split_work.p, ctl + cur,
+                                     max_part_chunks_total + max_nodes_level, b->d_counters.p, m->any_cat() ? 1 : 0, fin,
+                                     ctx->num_sms, s));
+    st.kernel_launches++;
     mark_phase(b, 5);
     if (need_hist) {
       // ---- histograms of level d+1: built children in slots [0, 2^d), siblings in [2^d, 2^(d+1))
@@ -1407,7 +1430,8 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
       record_hist_launch(b, st, e0, e1, false);
       st.hist_launches++; st.kernel_launches++;
       mark_phase(b, 1);
-      exchange_and_subtract(b, st, b->hist[hb].p, b->hist[nh].p, b->d_triples.p, ctl + nxt, max_nodes_level, max_nodes_level);
+      exchange_and_subtract(b, st, b->hist[hb].p, b->hist[nh].p, sub_in_scan ? nullptr : b->d_triples.p, ctl + nxt,
+                            max_nodes_level, max_nodes_level);
       hb = nh;
     }
   }
@@ -1417,10 +1441,13 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
     LAUNCH_CHECK(b2_launch_leaf_sums(gh, b->ridx[0].p, b->ridx[1].p, b->d_seg_work.p, ctl + 2, max_leaf_chunks, b->d_qexp.p, 40,
                                      b->d_leaf_sums.p, nullptr, ctx->num_sms, s));
     st.kernel_launches += 2;
+  } else if (leaf_stream) {   // every row's leaf index is in pos: sum the leaves in row order
+    LAUNCH_CHECK(b2_launch_leaf_accumulate(gh, b->pos.p, n, D, b->d_qexp.p, 40, b->d_leaf_sums.p, ctx->num_sms, s));
+    st.kernel_launches++;
   }
   if (p2p) { LAUNCH_CHECK(b2_launch_p2p_leaf_sums(&b->p2p.pp, d_n_leaves, b->d_leaf_sums.p, s)); st.kernel_launches++; }
   else allreduce(b->comm, b->d_leaf_sums.p, 2 * lcap, kNcclInt64, kNcclSum, s);
-  LAUNCH_CHECK(b2_launch_leaf_values(b->d_leaves.p, d_n_leaves, b->d_leaf_sums.p, b->d_qexp.p, 40, cp, b->d_leaf_values.p, tree, s));
+  LAUNCH_CHECK(b2_launch_leaf_values(b->d_leaves.p, d_n_leaves, b->d_leaf_sums.p, b->d_qexp.p, 40, cp, b->d_leaf_values.p, tree, b->t_qexp.p, s));
   if (leaf_fused)
     LAUNCH_CHECK(b2_launch_margin_update(b->margin.p, K, k, b->pos.p, b->d_leaf_values.p, n, ctx->num_sms, s));
   else
@@ -1430,11 +1457,8 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   mark_phase(b, 6);
   // ---- read the finished tree back (pinned, asynchronous; resolved at the end of the round)
   char* stg = (char*)b->staging[slot];
-  CUDA_CHECK(cudaMemcpyAsync(stg, b->t_i32.p, L.i32_count * 4, cudaMemcpyDeviceToHost, s));
-  CUDA_CHECK(cudaMemcpyAsync(stg + L.off_f32, b->t_f32.p, L.f32_count * 4, cudaMemcpyDeviceToHost, s));
-  CUDA_CHECK(cudaMemcpyAsync(stg + L.off_i64, b->t_i64.p, L.i64_count * 8, cudaMemcpyDeviceToHost, s));
-  CUDA_CHECK(cudaMemcpyAsync(stg + L.off_qexp, b->d_qexp.p, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  if (m->any_cat()) CUDA_CHECK(cudaMemcpyAsync(stg + L.off_cat, b->t_cat.p, L.max_nodes * 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  // one copy: the category sets (the block's tail) only when the matrix has categorical features
+  CUDA_CHECK(cudaMemcpyAsync(stg, b->t_block.p, m->any_cat() ? L.bytes : L.off_cat, cudaMemcpyDeviceToHost, s));
 }
 
 void apply_tree_stats(Booster* b, long long hist_launches, long long kernel_launches, double allreduce_bytes,

@@ -8,6 +8,7 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "level_finalize.cuh"
 
 namespace b2 {
 
@@ -33,7 +34,7 @@ template <int kMode, bool kRoot>
 __global__ void __launch_bounds__(kPartThreads)
 partition_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, const int32_t* __restrict__ ridx_in,
                  int32_t* __restrict__ ridx_out, const B2SplitWork* __restrict__ work, const B2LevelCtl* __restrict__ ctl,
-                 int32_t* __restrict__ counters /* [2*n_work]: low word lefts, high word rows claimed */) {
+                 int32_t* counters /* [2*n_work]: low word lefts, high word rows claimed */, B2FinalizeArgs fin) {
   const int n_work = ctl->n_split, total_chunks = ctl->part_chunks;
   constexpr int kIters = kPartChunk / kPartThreads;                  // 8 rows per thread and pass
   constexpr int kWarps = kPartThreads / 32;
@@ -144,13 +145,28 @@ partition_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, const
     }
     __syncthreads();
   }
+  // The last CTA to finish finalises the level (no separate single-CTA launch).  Its counter resets itself, so the
+  // next level and every replay of the captured tree start from zero.
+  __shared__ FinalizeScratch<kPartThreads> s_fin;
+  __shared__ bool s_last;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();   // this CTA's counter atomics and row-id stores before its arrival
+    const unsigned prev = atomicAdd(fin.done, 1u);
+    s_last = prev == gridDim.x - 1;
+    if (s_last) { __threadfence(); *fin.done = 0u; }
+  }
+  __syncthreads();
+  if (!s_last) return;
+  finalize_level_block<kPartThreads>(s_fin, ctl, work, counters, fin);
 }
 
 // ---- leaf refinement: 40-bit fixed-point sums of the fp32 gradients per leaf (exact int64)
+// sums == nullptr: only record the leaf index of every row (pos); leaf_accumulate_kernel sums the leaves afterwards.
 __global__ void __launch_bounds__(256)
 leaf_sums_kernel(const float2* __restrict__ gh, const int32_t* __restrict__ ridx0, const int32_t* __restrict__ ridx1,
                  const SegWork* __restrict__ work, const B2LevelCtl* __restrict__ ctl, const int32_t* __restrict__ qexp,
-                 int leaf_bits, long long* __restrict__ sums /* [n_leaves][2] */,
+                 int leaf_bits, long long* __restrict__ sums /* nullable: [n_leaves][2] */,
                  uint16_t* __restrict__ pos /* nullable: row -> leaf index, read by margin_update_kernel */) {
   const int n_work = ctl->hist_n_work, total_chunks = ctl->hist_total_chunks;
   __shared__ long long sg[8], sh[8];
@@ -165,6 +181,11 @@ leaf_sums_kernel(const float2* __restrict__ gh, const int32_t* __restrict__ ridx
     const int32_t* ridx = w.pad0 ? nullptr : (w.buf ? ridx1 : ridx0);   // pad0: the leaf is the root (rows = identity)
     const int row0 = (chunk - w.chunk_begin) * kPartChunk;
     const int nrows = min(kPartChunk, w.seg_count - row0);
+    if (!sums) {   // uniform
+      for (int r = threadIdx.x; r < nrows; r += blockDim.x)
+        pos[ridx ? __ldg(ridx + w.seg_begin + row0 + r) : (w.seg_begin + row0 + r)] = (uint16_t)w.id;
+      continue;
+    }
     long long ag = 0, ah = 0;
     for (int r = threadIdx.x; r < nrows; r += blockDim.x) {
       const int row = ridx ? __ldg(ridx + w.seg_begin + row0 + r) : (w.seg_begin + row0 + r);
@@ -217,7 +238,10 @@ pred_update_kernel(float* __restrict__ margin, int K, int k, const int32_t* __re
 // the leaf index of the row; the margin is then updated by a streaming kernel (margin_update_kernel).
 // Leaf index of child `side` of split j: leaf_base + 2 j + side -- exactly the index decide_kernel gives the node at
 // the next level (leaves are numbered in node order; leaf_base = leaves that existed before this level's children).
-template <bool kCat, bool kRoot>
+// kSums = false (the default whenever the per-leaf accumulators fit in shared memory): only pos is written, and
+// leaf_accumulate_kernel sums the gradient pairs afterwards in row order.  Gathering gh[rid] here costs a 32-byte
+// sector per 8-byte pair at the last level, where a node's rows are spread over the whole matrix.
+template <bool kCat, bool kRoot, bool kSums>
 __global__ void __launch_bounds__(kPartThreads)
 final_assign_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, const int32_t* __restrict__ ridx_in,
                     const B2SplitWork* __restrict__ work, const B2LevelCtl* __restrict__ ctl, const float2* __restrict__ gh,
@@ -225,7 +249,7 @@ final_assign_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, co
                     uint16_t* __restrict__ pos) {
   const int n_work = ctl->n_split, total_chunks = ctl->part_chunks, leaf_base = ctl->leaf_base_next;
   __shared__ long long s_acc[kPartThreads / 32][4];
-  const double kg = ldexp(1.0, leaf_bits - qexp[0]), kh = ldexp(1.0, leaf_bits - qexp[1]);
+  const double kg = kSums ? ldexp(1.0, leaf_bits - qexp[0]) : 0.0, kh = kSums ? ldexp(1.0, leaf_bits - qexp[1]) : 0.0;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int chunk = blockIdx.x; chunk < total_chunks; chunk += gridDim.x) {
     int lo = 0, hi = n_work - 1;
@@ -240,7 +264,8 @@ final_assign_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, co
     const int leaf_l = leaf_base + 2 * lo;
     long long lg = 0, lh = 0, rg = 0, rh = 0;
     // batches of 4 rows per thread: 4 row-id loads, then 4 bin bytes + 4 gradient pairs, all in flight together
-    constexpr int kBatch = 4;
+    // (8 rows when no gradient pair is loaded)
+    constexpr int kBatch = kSums ? 4 : 8;
     const uint8_t* col = bins_col + (int64_t)w.feature * col_stride;
     for (int r0 = threadIdx.x; r0 < nrows; r0 += kBatch * kPartThreads) {
       int rid[kBatch]; int bin[kBatch]; float2 v[kBatch];
@@ -250,7 +275,10 @@ final_assign_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, co
         rid[k] = r < nrows ? (kRoot ? w.seg_begin + row0 + r : __ldg(ridx_in + w.seg_begin + row0 + r)) : -1;
       }
 #pragma unroll
-      for (int k = 0; k < kBatch; ++k) { bin[k] = (int)__ldg(col + (rid[k] < 0 ? 0 : rid[k])); v[k] = __ldg(gh + (rid[k] < 0 ? 0 : rid[k])); }
+      for (int k = 0; k < kBatch; ++k) {
+        bin[k] = (int)__ldg(col + (rid[k] < 0 ? 0 : rid[k]));
+        if (kSums) v[k] = __ldg(gh + (rid[k] < 0 ? 0 : rid[k]));
+      }
 #pragma unroll
       for (int k = 0; k < kBatch; ++k) {
         if (rid[k] < 0) continue;
@@ -258,11 +286,14 @@ final_assign_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, co
         bool go_left = b <= w.split_bin;
         if (kCat && is_cat) go_left = ((__ldg(&work[lo].cat_bits[b >> 5]) >> (b & 31)) & 1u) == 0u;   // category in the set -> right
         const bool l = (w.has_missing && b == B2_MISSING_BIN) ? (w.default_left != 0) : go_left;
-        const long long qg = __double2ll_rn(__dmul_rn((double)v[k].x, kg)), qh = __double2ll_rn(__dmul_rn((double)v[k].y, kh));
-        if (l) { lg += qg; lh += qh; } else { rg += qg; rh += qh; }
+        if (kSums) {
+          const long long qg = __double2ll_rn(__dmul_rn((double)v[k].x, kg)), qh = __double2ll_rn(__dmul_rn((double)v[k].y, kh));
+          if (l) { lg += qg; lh += qh; } else { rg += qg; rh += qh; }
+        }
         pos[rid[k]] = (uint16_t)(leaf_l + (l ? 0 : 1));
       }
     }
+    if (!kSums) continue;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
       lg += __shfl_xor_sync(0xffffffffu, lg, o); lh += __shfl_xor_sync(0xffffffffu, lh, o);
@@ -287,6 +318,67 @@ margin_update_kernel(float* __restrict__ margin, int K, int k, const uint16_t* _
     margin[i * K + k] += __ldg(leaf_value + pos[i]);
 }
 
+// ---- leaf sums in natural row order: sums[pos[i]] += fixed(gh[i]).  pos and gh stream (10 bytes per row) instead of
+// being gathered per leaf.  The values are the same 40-bit fixed-point integers leaf_sums_kernel / final_assign_kernel
+// add, so the sums are bit-identical in any order.
+// Every CTA keeps its sums in shared memory as two 32-bit words per int64 and adds with native 32-bit shared atomics:
+// the carry out of the low word is known from the value the atomic returns, so low += lo; high += hi + carry is exact
+// modulo 2^64, like an int64 add.  (A 64-bit shared atomic is a compare-and-swap loop on sm_90, and lanes of a warp
+// that hit the same popular leaf retry one after another.)  Lanes spread over `copies` copies of the table
+// (lane % copies), so that a popular leaf is not one shared-memory word for the whole warp.  At the end the copies are
+// added up and every non-empty leaf costs one global atomic per CTA.
+constexpr int kLeafAccThreads = 512;
+constexpr int kLeafAccMaxDepth = 11;            // 2^11 leaves x 16 bytes = 32 KB of shared memory per CTA
+constexpr int kLeafAccSmem = 32 * 1024;         // copies of the table: as many as fit here, at most 8
+__device__ __forceinline__ void acc_add64(uint32_t* lo, uint32_t* hi, long long q) {
+  const uint32_t l = (uint32_t)(unsigned long long)q, h = (uint32_t)((unsigned long long)q >> 32);
+  const uint32_t old = atomicAdd(lo, l);
+  const uint32_t hadd = h + ((uint32_t)(old + l) < old ? 1u : 0u);
+  if (hadd != 0u) atomicAdd(hi, hadd);
+}
+__global__ void __launch_bounds__(kLeafAccThreads)
+leaf_accumulate_kernel(const float2* __restrict__ gh, const uint16_t* __restrict__ pos, int64_t n, int n_acc, int log2_copies,
+                       const int32_t* __restrict__ qexp, int leaf_bits, long long* __restrict__ sums /* [n_leaves][2] */) {
+  extern __shared__ uint32_t s_acc[];   // 4 planes (g lo, g hi, h lo, h hi) of [n_acc][copies]
+  const int copies = 1 << log2_copies, plane = n_acc << log2_copies;
+  for (int i = threadIdx.x; i < 4 * plane; i += blockDim.x) s_acc[i] = 0u;
+  __syncthreads();
+  uint32_t *glo = s_acc, *ghi = s_acc + plane, *hlo = s_acc + 2 * plane, *hhi = s_acc + 3 * plane;
+  const int copy = threadIdx.x & (copies - 1);
+  const double kg = ldexp(1.0, leaf_bits - qexp[0]), kh = ldexp(1.0, leaf_bits - qexp[1]);
+  constexpr int kBatch = 4;   // 4 leaf indices + 4 gradient pairs in flight per thread
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  for (; i + (kBatch - 1) * stride < n; i += kBatch * stride) {
+    int leaf[kBatch]; float2 v[kBatch];
+#pragma unroll
+    for (int b = 0; b < kBatch; ++b) { leaf[b] = pos[i + b * stride]; v[b] = __ldg(gh + i + b * stride); }
+#pragma unroll
+    for (int b = 0; b < kBatch; ++b) {
+      const int a = (leaf[b] << log2_copies) + copy;
+      acc_add64(glo + a, ghi + a, __double2ll_rn(__dmul_rn((double)v[b].x, kg)));
+      acc_add64(hlo + a, hhi + a, __double2ll_rn(__dmul_rn((double)v[b].y, kh)));
+    }
+  }
+  for (; i < n; i += stride) {
+    const int a = ((int)pos[i] << log2_copies) + copy;
+    const float2 v = __ldg(gh + i);
+    acc_add64(glo + a, ghi + a, __double2ll_rn(__dmul_rn((double)v.x, kg)));
+    acc_add64(hlo + a, hhi + a, __double2ll_rn(__dmul_rn((double)v.y, kh)));
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < 2 * n_acc; j += blockDim.x) {   // j = 2 * leaf + (0: g, 1: h)
+    const uint32_t* lo = (j & 1) ? hlo : glo;
+    const uint32_t* hi = (j & 1) ? hhi : ghi;
+    unsigned long long t = 0ull;
+    for (int c = 0; c < copies; ++c) {
+      const int a = ((j >> 1) << log2_copies) + c;
+      t += ((unsigned long long)hi[a] << 32) | (unsigned long long)lo[a];
+    }
+    if (t != 0ull) atomicAdd((unsigned long long*)&sums[j], t);
+  }
+}
+
 __global__ void iota_kernel(int32_t* out, int64_t n) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = (int32_t)i;
 }
@@ -297,15 +389,16 @@ extern "C" {
 int b2_part_chunk_rows() { return b2::kPartChunk; }     // leaf-segment work items (leaf_sums / pred_update)
 int b2_split_chunk_rows() { return b2::kSplitChunk; }   // split-node work items (partition / final_assign)
 
+// partition + finalize of a level: `fin` is what the last CTA writes (level_finalize.cuh)
 int b2_launch_partition(const uint8_t* bins_col, int64_t col_stride, const int32_t* ridx_in, int32_t* ridx_out,
                         const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, int32_t* counters, int any_categorical,
-                        int num_sms, cudaStream_t stream) {
-  if (max_chunks <= 0) return 0;
+                        B2FinalizeArgs fin, int num_sms, cudaStream_t stream) {
+  if (max_chunks <= 0) max_chunks = 1;   // the last CTA finalises the level, so even an empty level launches one
   int grid = max_chunks < num_sms * 6 ? max_chunks : num_sms * 6;   // 6 CTAs per SM are resident (33 KB of shared memory, 48 registers)
 #define B2_PART_LAUNCH(MODE)                                                                                                  \
   do {                                                                                                                        \
-    if (ridx_in) b2::partition_kernel<MODE, false><<<grid, b2::kPartThreads, 0, stream>>>(bins_col, col_stride, ridx_in, ridx_out, work, ctl, counters); \
-    else b2::partition_kernel<MODE, true><<<grid, b2::kPartThreads, 0, stream>>>(bins_col, col_stride, ridx_in, ridx_out, work, ctl, counters);         \
+    if (ridx_in) b2::partition_kernel<MODE, false><<<grid, b2::kPartThreads, 0, stream>>>(bins_col, col_stride, ridx_in, ridx_out, work, ctl, counters, fin); \
+    else b2::partition_kernel<MODE, true><<<grid, b2::kPartThreads, 0, stream>>>(bins_col, col_stride, ridx_in, ridx_out, work, ctl, counters, fin);    \
   } while (0)
   if (any_categorical) B2_PART_LAUNCH(1);
   else B2_PART_LAUNCH(0);
@@ -325,10 +418,29 @@ int b2_launch_final_assign(const uint8_t* bins_col, int64_t col_stride, const in
                            long long* sums, uint16_t* pos, int any_categorical, int num_sms, cudaStream_t stream) {
   if (max_chunks <= 0) return 0;
   int grid = max_chunks < num_sms * 8 ? max_chunks : num_sms * 8;
-#define B2_FA_LAUNCH(CAT, ROOT) b2::final_assign_kernel<CAT, ROOT><<<grid, b2::kPartThreads, 0, stream>>>(bins_col, col_stride, ridx_in, work, ctl, gh, qexp, leaf_bits, sums, pos)
+  // sums == nullptr: pos only (the leaves are summed by leaf_accumulate_kernel)
+#define B2_FA_LAUNCH(CAT, ROOT)                                                                                               \
+  do {                                                                                                                        \
+    if (sums) b2::final_assign_kernel<CAT, ROOT, true><<<grid, b2::kPartThreads, 0, stream>>>(bins_col, col_stride, ridx_in, work, ctl, gh, qexp, leaf_bits, sums, pos); \
+    else b2::final_assign_kernel<CAT, ROOT, false><<<grid, b2::kPartThreads, 0, stream>>>(bins_col, col_stride, ridx_in, work, ctl, gh, qexp, leaf_bits, sums, pos);    \
+  } while (0)
   if (any_categorical) { if (ridx_in) B2_FA_LAUNCH(true, false); else B2_FA_LAUNCH(true, true); }
   else { if (ridx_in) B2_FA_LAUNCH(false, false); else B2_FA_LAUNCH(false, true); }
 #undef B2_FA_LAUNCH
+  return (int)cudaGetLastError();
+}
+int b2_leaf_acc_max_depth() { return b2::kLeafAccMaxDepth; }
+int b2_launch_leaf_accumulate(const float2* gh, const uint16_t* pos, int64_t n, int max_depth, const int32_t* qexp, int leaf_bits,
+                              long long* sums, int num_sms, cudaStream_t stream) {
+  if (n <= 0) return 0;
+  if (max_depth > b2::kLeafAccMaxDepth) return (int)cudaErrorInvalidValue;
+  const int n_acc = 1 << max_depth;
+  int log2_copies = 0;
+  while (log2_copies < 3 && ((size_t)n_acc * 16 << (log2_copies + 1)) <= (size_t)b2::kLeafAccSmem) ++log2_copies;
+  const size_t smem = (size_t)n_acc * 16 << log2_copies;
+  const int64_t want = (n + b2::kLeafAccThreads - 1) / b2::kLeafAccThreads;
+  const int grid = (int)(want < (int64_t)num_sms * 2 ? want : (int64_t)num_sms * 2);
+  b2::leaf_accumulate_kernel<<<grid, b2::kLeafAccThreads, smem, stream>>>(gh, pos, n, n_acc, log2_copies, qexp, leaf_bits, sums);
   return (int)cudaGetLastError();
 }
 int b2_launch_margin_update(float* margin, int K, int k, const uint16_t* pos, const float* leaf_value, int64_t n, int num_sms,

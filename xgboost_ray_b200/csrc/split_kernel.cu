@@ -33,6 +33,13 @@ __device__ __forceinline__ void consider(Best& b, float chg, uint32_t order, int
 constexpr int kEvalChunks = 32;                 // bin chunks per feature
 constexpr int kEvalBinsPerChunk = 256 / kEvalChunks;
 
+// Sibling subtraction in the scan (B2SiblingSub, parent_level != nullptr): a node whose histogram slot is a sibling
+// slot (>= sib_base) was never built or subtracted.  Its bins are formed in registers as parent - built, exact int64,
+// with (parent slot, built slot) = triples[3 j], triples[3 j + 1] for j = slot - sib_base.  With sib_out the CTA also
+// stores the whole sibling slice (every bin of every slot it covers, sampled or not), because the next level reads it
+// as a parent; the bin scan then re-reads the stored values.  Without sib_out (the last histogram level) nothing is
+// stored and the scan subtracts again.  level_hist is only read at built slots in this mode, sib_out only at sibling
+// slots, so the two never alias.
 __global__ void __launch_bounds__(32 * kEvalChunks)
 eval_splits_kernel(const long long* __restrict__ level_hist, int n_groups, const B2EvalNode* __restrict__ nodes,
                    const int32_t* __restrict__ group_first, const int32_t* __restrict__ group_size,
@@ -40,7 +47,7 @@ eval_splits_kernel(const long long* __restrict__ level_hist, int n_groups, const
                    const uint8_t* __restrict__ is_cat /* nullable: categorical features are scanned by eval_cat_splits_kernel */,
                    const int32_t* __restrict__ qexp, int qbits, B2TrainParamDev p, B2SplitCand* __restrict__ cands,
                    int cand_stride, const B2LevelCtl* __restrict__ ctl, int log2_shards, int shard_rank, B2ColSample cs,
-                   const B2NodeSeg* __restrict__ seg) {
+                   const B2NodeSeg* __restrict__ seg, B2SiblingSub sub) {
   // This rank owns sp = 32 >> log2_shards slots of every group (slot s is owned by s % shards): the
   // G*sp owned "virtual slots" of a node are covered by cpn = ceil(G*sp/32) CTAs.
   const int sp = B2_GROUP_SLOTS >> log2_shards;
@@ -59,8 +66,15 @@ eval_splits_kernel(const long long* __restrict__ level_hist, int n_groups, const
   const int group = v_ok ? v / sp : 0, sl = v_ok ? v % sp : 0;
   const int slot = (sl << log2_shards) + shard_rank;       // real slot inside the group
   const size_t slice_elems = (size_t)n_groups * 2 * B2_BINS * sp;
-  const long long* hg = level_hist + (size_t)nd.hist_index * slice_elems + (size_t)(group * 2) * B2_BINS * sp + sl;
+  const size_t in_slice = (size_t)(group * 2) * B2_BINS * sp + sl;
+  const bool fused = sub.parent_level != nullptr && nd.hist_index >= sub.sib_base;   // uniform over the CTA
+  const int pair = fused ? nd.hist_index - sub.sib_base : 0;
+  const long long* hg = level_hist + (size_t)(fused ? sub.triples[3 * pair + 1] : nd.hist_index) * slice_elems + in_slice;
   const long long* hh = hg + (size_t)B2_BINS * sp;
+  const long long* pgp = fused ? sub.parent_level + (size_t)sub.triples[3 * pair] * slice_elems + in_slice : nullptr;
+  const long long* php = fused ? pgp + (size_t)B2_BINS * sp : nullptr;
+  long long* sgp = (fused && sub.sib_out) ? sub.sib_out + (size_t)nd.hist_index * slice_elems + in_slice : nullptr;
+  long long* shp = sgp ? sgp + (size_t)B2_BINS * sp : nullptr;
   const int f = group_first[group] + slot;
   bool active = v_ok && slot < group_size[group] && !(is_cat && is_cat[f]);
   if (active && cs.level_mask) active = cs.level_mask[f] != 0;          // colsample_bytree / bylevel
@@ -76,7 +90,17 @@ eval_splits_kernel(const long long* __restrict__ level_hist, int n_groups, const
   const bool fmiss = active ? (has_missing[f] != 0) : false;
 
   long long sg = 0, sh = 0;
-  if (active) {
+  if (fused) {
+    if (v_ok && (sgp || active)) {
+#pragma unroll
+      for (int i = 0; i < kEvalBinsPerChunk; ++i) {
+        const int b = q * kEvalBinsPerChunk + i;
+        const long long g = pgp[b * sp] - hg[b * sp], h = php[b * sp] - hh[b * sp];
+        if (sgp) { sgp[b * sp] = g; shp[b * sp] = h; }
+        if (active && b < nf) { sg += g; sh += h; }
+      }
+    }
+  } else if (active) {
 #pragma unroll
     for (int i = 0; i < kEvalBinsPerChunk; ++i) {
       int b = q * kEvalBinsPerChunk + i;
@@ -103,7 +127,9 @@ eval_splits_kernel(const long long* __restrict__ level_hist, int n_groups, const
       const int b = q * kEvalBinsPerChunk + i;
       if (b >= nf) break;
       const long long eg_excl = pg, eh_excl = ph;
-      pg += hg[b * sp]; ph += hh[b * sp];
+      if (!fused) { pg += hg[b * sp]; ph += hh[b * sp]; }
+      else if (sgp) { pg += sgp[b * sp]; ph += shp[b * sp]; }   // stored by this thread in the first pass
+      else { pg += pgp[b * sp] - hg[b * sp]; ph += php[b * sp] - hh[b * sp]; }
       {  // forward: left = prefix inclusive, missing -> right
         const double lh_d = __dmul_rn(__ll2double_rn(ph), p.inv_scale_h);
         if (lh_d >= p.min_child_weight) {
@@ -331,9 +357,10 @@ eval_cat_splits_kernel(const long long* __restrict__ level_hist, int n_groups, c
 }
 
 // root totals: sum of all 256 bins of slot 0 / group 0 (every row lands in exactly one bin, the
-// missing sentinel included) -> nodes[0].sum_g/h and root_gain
+// missing sentinel included) -> nodes[0].sum_g/h and root_gain, and the root's sums in the tree table
 __global__ void root_totals_kernel(const long long* __restrict__ level_hist, int n_groups, B2EvalNode* nodes,
-                                   const int32_t* __restrict__ qexp, int qbits, B2TrainParamDev p, int log2_shards) {
+                                   const int32_t* __restrict__ qexp, int qbits, B2TrainParamDev p, int log2_shards,
+                                   long long* __restrict__ tree_sum_g, long long* __restrict__ tree_sum_h) {
   __shared__ long long sg[256], sh[256];
   const int sp = B2_GROUP_SLOTS >> log2_shards;
   const size_t slice_elems = (size_t)n_groups * 2 * B2_BINS * sp;
@@ -350,6 +377,7 @@ __global__ void root_totals_kernel(const long long* __restrict__ level_hist, int
     p.inv_scale_g = ldexp(1.0, qexp[0] - qbits);
     p.inv_scale_h = ldexp(1.0, qexp[1] - qbits);
     nodes[0].sum_g = sg[0]; nodes[0].sum_h = sh[0];
+    tree_sum_g[0] = sg[0]; tree_sum_h[0] = sh[0];
     double G = __dmul_rn(__ll2double_rn(sg[0]), p.inv_scale_g), H = __dmul_rn(__ll2double_rn(sh[0]), p.inv_scale_h);
     nodes[0].root_gain = __double2float_rn(calc_gain(G, H, p));
   }
@@ -362,12 +390,12 @@ int b2_launch_eval_splits(const long long* level_hist, int n_groups, const B2Eva
                           const int32_t* group_first, const int32_t* group_size, const int32_t* nbins,
                           const uint8_t* has_missing, const uint8_t* is_cat, const int32_t* qexp, int qbits, B2TrainParamDev p,
                           B2SplitCand* cands, int cand_stride, const B2LevelCtl* ctl, int log2_shards, int shard_rank,
-                          B2ColSample cs, const B2NodeSeg* seg, cudaStream_t stream) {
+                          B2ColSample cs, const B2NodeSeg* seg, B2SiblingSub sub, cudaStream_t stream) {
   if (n_nodes <= 0) return 0;   // with ctl: n_nodes is the upper bound of the level
   const int sp = B2_GROUP_SLOTS >> log2_shards, cpn = (n_groups * sp + 31) >> 5;
   b2::eval_splits_kernel<<<n_nodes * cpn, 32 * b2::kEvalChunks, 0, stream>>>(level_hist, n_groups, nodes, group_first, group_size,
                                                                          nbins, has_missing, is_cat, qexp, qbits, p, cands,
-                                                                         cand_stride, ctl, log2_shards, shard_rank, cs, seg);
+                                                                         cand_stride, ctl, log2_shards, shard_rank, cs, seg, sub);
   return (int)cudaGetLastError();
 }
 int b2_cat_ctas() { return b2::kCatCtas; }
@@ -384,8 +412,9 @@ int b2_launch_eval_cat_splits(const long long* level_hist, int n_groups, const B
   return (int)cudaGetLastError();
 }
 int b2_launch_root_totals(const long long* level_hist, int n_groups, B2EvalNode* nodes, const int32_t* qexp, int qbits,
-                          B2TrainParamDev p, int log2_shards, cudaStream_t stream) {
-  b2::root_totals_kernel<<<1, 256, 0, stream>>>(level_hist, n_groups, nodes, qexp, qbits, p, log2_shards);
+                          B2TrainParamDev p, int log2_shards, long long* tree_sum_g, long long* tree_sum_h,
+                          cudaStream_t stream) {
+  b2::root_totals_kernel<<<1, 256, 0, stream>>>(level_hist, n_groups, nodes, qexp, qbits, p, log2_shards, tree_sum_g, tree_sum_h);
   return (int)cudaGetLastError();
 }
 }
