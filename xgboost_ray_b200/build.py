@@ -41,7 +41,7 @@ def _stale(target, deps):
 
 def build(force=False, verbose=False):
     os.makedirs(OBJ_DIR, exist_ok=True)
-    headers = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "hist_common.cuh"), os.path.join(CSRC, "sampling.cuh"), os.path.join(CSRC, "p2p.cuh"), os.path.join(CSRC, "level_finalize.cuh"), os.path.join(HERE, "..", "include", "b2hist.h"), __file__]
+    headers = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "hist_common.cuh"), os.path.join(CSRC, "sampling.cuh"), os.path.join(CSRC, "p2p.cuh"), os.path.join(CSRC, "level_finalize.cuh"), os.path.join(CSRC, "decide.cuh"), os.path.join(HERE, "..", "include", "b2hist.h"), __file__]
     jobs = []
     objs = []
     for src, extra in SOURCES.items():

@@ -188,6 +188,30 @@ struct B2SiblingSub {
   int32_t sib_base;                // first sibling slot of the level
 };
 
+// what decide does at the end of a level's split scan (decide.cuh): run by decide_kernel, or by the last CTA of
+// eval_splits_kernel on one GPU
+struct B2DecideArgs {
+  B2LevelCtl* ctl_cur;
+  B2LevelCtl* ctl_nxt;
+  const B2NodeSeg* seg_cur;
+  B2NodeSeg* seg_nxt;
+  const B2EvalNode* ev_cur;
+  B2EvalNode* ev_nxt;
+  const B2SplitCand* cands;        // [cand_ranks][cand_rank_stride]: cands_per_node candidates per node
+  B2SplitCand* cand_best;          // [nodes] the winner of every node (scratch)
+  const B2SplitCand* local_cands;  // peer-memory exchange: this rank's own candidates
+  B2TreeDev tree;
+  B2SplitWork* split_work;
+  int32_t* pair_parent_hist;
+  B2LeafDev* leaves;
+  int32_t* n_leaves;
+  const uint8_t* has_missing;
+  const int32_t* qexp;
+  int32_t* part_counters;          // nullable: zeroed for the level's partition
+  B2CtlParams p;
+  int32_t cands_per_node, cand_ranks, cand_rank_stride, can_split, qbits;
+};
+
 // ---- peer-memory exchange over NVLink / NVSwitch (p2p.cuh, p2p_exchange.cu, control_kernel.cu)
 // Every rank maps four regions of every peer (cudaIpc): the histogram build buffer (peers READ their owned slices out
 // of it), and three tables the peers WRITE into -- split candidates, per-tree |g|,|h| maxima + leaf sums, and epoch

@@ -41,7 +41,9 @@ int b2_launch_hist_tma(const uint8_t*, int, const void*, const int2*, const int3
 int b2_launch_hist_subtract(const long long*, long long*, const int32_t*, int, int64_t, const B2LevelCtl*, cudaStream_t);
 int b2_launch_eval_splits(const long long*, int, const B2EvalNode*, int, const int32_t*, const int32_t*, const int32_t*,
                           const uint8_t*, const uint8_t*, const int32_t*, int, B2TrainParamDev, B2SplitCand*, int, const B2LevelCtl*,
-                          int, int, B2ColSample, const B2NodeSeg*, B2SiblingSub, cudaStream_t);
+                          int, int, B2ColSample, const B2NodeSeg*, B2SiblingSub, const B2DecideArgs*, uint32_t*, cudaStream_t);
+int b2_eval_ctas_per_node(int, int, int);
+int b2_eval_narrow_max_nodes();
 int b2_launch_subsample(float2*, int64_t, uint32_t, uint32_t, uint32_t, double, int, cudaStream_t);
 int b2_p2p_flag_words(int);
 int b2_launch_p2p_reduce_subtract(const void*, const long long*, long long*, const int32_t*, const B2LevelCtl*, int, int, int64_t, int,
@@ -73,9 +75,7 @@ int b2_launch_leaf_sums(const float2*, const int32_t*, const int32_t*, const voi
                         long long*, uint16_t*, int, cudaStream_t);
 int b2_launch_pred_update(float*, int, int, const int32_t*, const int32_t*, const void*, const B2LevelCtl*, int, const float*, int,
                           cudaStream_t);
-int b2_launch_decide(B2LevelCtl*, B2LevelCtl*, const B2NodeSeg*, B2NodeSeg*, const B2EvalNode*, B2EvalNode*, const B2SplitCand*,
-                     int, int, int, int, B2TreeDev, B2SplitWork*, int32_t*, B2LeafDev*, int32_t*, const uint8_t*, const int32_t*, int,
-                     B2CtlParams, int32_t*, const B2SplitCand*, const void*, cudaStream_t);
+int b2_launch_decide(const B2DecideArgs*, const void*, cudaStream_t);
 int b2_launch_leaf_plan(const B2LeafDev*, const int32_t*, B2SegWork*, B2LevelCtl*, cudaStream_t);
 int b2_launch_leaf_values(const B2LeafDev*, const int32_t*, const long long*, const int32_t*, int, B2CtlParams, float*, B2TreeDev,
                           int32_t*, cudaStream_t);
@@ -788,7 +788,7 @@ struct Booster : HandleBase {
   size_t xoff_cands = 0, xoff_misc = 0, xoff_flags = 0, x_misc_stride = 0;
   View<long long> hist_build;       // reduce-scatter send buffer [shards][node_cap][slice] (only when shards > 1)
   View<B2SplitCand> d_cands_all;    // candidates of all ranks [shards][nodes][cpn]
-  int shards = 1, log2_shards = 0, sp = 32, cpn = 1;   // cpn = candidates per node (numeric CTAs + categorical CTAs)
+  int shards = 1, log2_shards = 0, sp = 32, cpn = 1;   // cpn = most candidates per node of a level (numeric CTAs + categorical CTAs)
   int cpn_num = 1;
   View<uint32_t> t_cat;                    // [max_nodes][8] category sets of the tree being grown (in t_block)
   DevBuf<uint8_t> d_col_masks;             // [max_depth][F] level feature sets of the tree being grown (column sampling)
@@ -834,6 +834,8 @@ struct Booster : HandleBase {
   DevBuf<B2HistWork> d_hist_work; DevBuf<B2SplitWork> d_split_work; DevBuf<B2SegWork> d_seg_work;
   DevBuf<B2SplitCand> d_cands; DevBuf<int32_t> d_counters, d_triples, d_pair_parent;
   DevBuf<uint32_t> d_part_done;            // CTAs of a partition that finished (zero between launches: the last resets it)
+  DevBuf<uint32_t> d_eval_done;            // CTAs of a split scan that finished when it decides the level (same rule)
+  DevBuf<B2SplitCand> d_cand_best;         // [nodes of a level] decide's winner of every node
   DevBuf<B2LeafDev> d_leaves;
   DevBuf<long long> d_leaf_sums; DevBuf<float> d_leaf_values; DevBuf<double> d_metric;
   std::vector<void*> staging;              // pinned host copies of finished trees, one per class tree of a round
@@ -1128,6 +1130,8 @@ void ensure_ctl_tables(Booster* b) {
   b->d_hist_work.ensure(half); b->d_split_work.ensure(half);
   b->d_counters.ensure(2 * half); b->d_triples.ensure(3 * half); b->d_pair_parent.ensure(half);
   if (!b->d_part_done.p) { b->d_part_done.ensure(1); CUDA_CHECK(cudaMemsetAsync(b->d_part_done.p, 0, sizeof(uint32_t), b->ctx->stream)); }
+  if (!b->d_eval_done.p) { b->d_eval_done.ensure(1); CUDA_CHECK(cudaMemsetAsync(b->d_eval_done.p, 0, sizeof(uint32_t), b->ctx->stream)); }
+  b->d_cand_best.ensure(half);
   b->d_leaves.ensure(L.max_nodes); b->d_seg_work.ensure(L.max_nodes);
   b->d_leaf_sums.ensure(2 * lcap); b->d_leaf_values.ensure(lcap);
   b->node_elems = (size_t)G * B2_GROUP_ELEMS;
@@ -1137,7 +1141,7 @@ void ensure_ctl_tables(Booster* b) {
   b->log2_shards = 0; while ((1 << b->log2_shards) < b->shards) b->log2_shards++;
   b->sp = B2_GROUP_SLOTS / b->shards;
   b->slice_elems = (size_t)G * 2 * B2_BINS * b->sp;
-  b->cpn_num = (G * b->sp + 31) / 32;
+  b->cpn_num = b2_eval_ctas_per_node(G, b->log2_shards, 1);   // the most numeric candidates per node of any level
   b->cpn = b->cpn_num + (b->train->any_cat() ? b2_cat_ctas() : 0);
   b->hist[0].ensure(half * b->slice_elems); b->hist[1].ensure(half * b->slice_elems);
   if (b->shards > 1) {
@@ -1341,8 +1345,21 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
     const int max_nodes_level = 1 << d;
     const bool can_split = d < D;
     const bool last_split_level = d == D - 1;
-    const B2SplitCand* cands_for_decide = b->d_cands.p;
-    int cand_rank_stride = max_nodes_level * b->cpn;
+    // candidates per node of this level: the scan's CTAs per node (its layout depends on the node count) + categorical
+    const int cpn_num = b2_eval_ctas_per_node(G, sh, max_nodes_level);
+    const int cpn = cpn_num + (m->any_cat() ? b2_cat_ctas() : 0);
+    B2DecideArgs da;
+    da.ctl_cur = ctl + cur; da.ctl_nxt = ctl + nxt; da.seg_cur = b->d_seg[cur].p; da.seg_nxt = b->d_seg[nxt].p;
+    da.ev_cur = b->d_ev[cur].p; da.ev_nxt = b->d_ev[nxt].p;
+    da.cands = b->d_cands.p; da.cand_best = b->d_cand_best.p; da.local_cands = b->d_cands.p;
+    da.tree = tree; da.split_work = b->d_split_work.p; da.pair_parent_hist = b->d_pair_parent.p; da.leaves = b->d_leaves.p;
+    da.n_leaves = d_n_leaves; da.has_missing = m->d_has_missing.p; da.qexp = b->d_qexp.p;
+    da.part_counters = can_split ? b->d_counters.p : nullptr; da.p = cp;
+    da.cands_per_node = cpn; da.cand_ranks = b->shards; da.cand_rank_stride = max_nodes_level * cpn;
+    da.can_split = can_split ? 1 : 0; da.qbits = p.qbits;
+    // one GPU, numeric features only, levels scanned by the narrow layout: the last CTA of the scan decides the level
+    // (no decide launch)
+    const bool fold_decide = can_split && !multi && !m->any_cat() && max_nodes_level <= b2_eval_narrow_max_nodes();
     if (can_split) {
       B2ColSample cs;
       cs.level_mask = p.use_cols() ? b->d_col_masks.p + (size_t)d * m->F : nullptr;
@@ -1358,29 +1375,28 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
       }
       LAUNCH_CHECK(b2_launch_eval_splits(b->hist[hb].p, G, b->d_ev[cur].p, max_nodes_level, m->d_group_first.p, m->d_group_size.p,
                                          m->d_nbins.p, m->d_has_missing.p, m->any_cat() ? m->d_is_cat.p : nullptr, b->d_qexp.p,
-                                         p.qbits, dp, b->d_cands.p, b->cpn, ctl + cur, sh, shard_rank, cs, b->d_seg[cur].p, sub, s));
+                                         p.qbits, dp, b->d_cands.p, cpn, ctl + cur, sh, shard_rank, cs, b->d_seg[cur].p, sub,
+                                         fold_decide ? &da : nullptr, b->d_eval_done.p, s));
       st.kernel_launches++;
       if (m->any_cat()) {
         LAUNCH_CHECK(b2_launch_eval_cat_splits(b->hist[hb].p, G, b->d_ev[cur].p, max_nodes_level, m->d_cat_feats.p,
                                                (int)m->cat_feats.size(), m->d_feat_byte.p, m->d_nbins.p, b->d_qexp.p, p.qbits, dp,
-                                               b->d_cands.p, b->cpn, b->cpn_num, ctl + cur, sh, shard_rank, cs, b->d_seg[cur].p, s));
+                                               b->d_cands.p, cpn, cpn_num, ctl + cur, sh, shard_rank, cs, b->d_seg[cur].p, s));
         st.kernel_launches++;
       }
       if (p2p) {   // decide_kernel stores the candidates straight into the peers' tables and waits for theirs
-        cands_for_decide = b->d_cands_all.p;
-        cand_rank_stride = b->p2p.cand_cap;
+        da.cands = b->d_cands_all.p;
+        da.cand_rank_stride = b->p2p.cand_cap;
       } else if (b->shards > 1) {   // every rank scanned only its own slots: gather the per-node candidates
-        const size_t bytes = (size_t)max_nodes_level * b->cpn * sizeof(B2SplitCand);
+        const size_t bytes = (size_t)max_nodes_level * cpn * sizeof(B2SplitCand);
         NCCL_CHECK(nccl()->AllGather(b->d_cands.p, b->d_cands_all.p, bytes, kNcclUint8, b->comm->comm, s));
-        cands_for_decide = b->d_cands_all.p;
+        da.cands = b->d_cands_all.p;
       }
     }
-    LAUNCH_CHECK(b2_launch_decide(ctl + cur, ctl + nxt, b->d_seg[cur].p, b->d_seg[nxt].p, b->d_ev[cur].p, b->d_ev[nxt].p,
-                                  cands_for_decide, b->cpn, b->shards, cand_rank_stride, can_split ? 1 : 0, tree,
-                                  b->d_split_work.p, b->d_pair_parent.p, b->d_leaves.p,
-                                  d_n_leaves, m->d_has_missing.p, b->d_qexp.p, p.qbits, cp, can_split ? b->d_counters.p : nullptr, b->d_cands.p,
-                                  (p2p && can_split) ? &b->p2p.pp : nullptr, s));
-    st.kernel_launches++;
+    if (!fold_decide) {
+      LAUNCH_CHECK(b2_launch_decide(&da, (p2p && can_split) ? &b->p2p.pp : nullptr, s));
+      st.kernel_launches++;
+    }
     mark_phase(b, 4);
     if (!can_split) break;
     const int32_t* ridx_in = d == 0 ? nullptr : b->ridx[cur].p;   // the root's rows are the identity list

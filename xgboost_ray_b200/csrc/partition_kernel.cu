@@ -264,7 +264,8 @@ final_assign_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, co
     const int leaf_l = leaf_base + 2 * lo;
     long long lg = 0, lh = 0, rg = 0, rh = 0;
     // batches of 4 rows per thread: 4 row-id loads, then 4 bin bytes + 4 gradient pairs, all in flight together
-    // (8 rows when no gradient pair is loaded)
+    // (8 rows when no gradient pair is loaded).  Row ids and bin bytes are streamed with the evict-first hint (__ldcs), so that L2
+    // keeps the partly written 32-byte sectors of pos until their other rows have been stored
     constexpr int kBatch = kSums ? 4 : 8;
     const uint8_t* col = bins_col + (int64_t)w.feature * col_stride;
     for (int r0 = threadIdx.x; r0 < nrows; r0 += kBatch * kPartThreads) {
@@ -272,11 +273,11 @@ final_assign_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, co
 #pragma unroll
       for (int k = 0; k < kBatch; ++k) {
         const int r = r0 + k * kPartThreads;
-        rid[k] = r < nrows ? (kRoot ? w.seg_begin + row0 + r : __ldg(ridx_in + w.seg_begin + row0 + r)) : -1;
+        rid[k] = r < nrows ? (kRoot ? w.seg_begin + row0 + r : __ldcs(ridx_in + w.seg_begin + row0 + r)) : -1;
       }
 #pragma unroll
       for (int k = 0; k < kBatch; ++k) {
-        bin[k] = (int)__ldg(col + (rid[k] < 0 ? 0 : rid[k]));
+        bin[k] = (int)__ldcs(col + (rid[k] < 0 ? 0 : rid[k]));
         if (kSums) v[k] = __ldg(gh + (rid[k] < 0 ? 0 : rid[k]));
       }
 #pragma unroll
