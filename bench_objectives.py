@@ -8,7 +8,9 @@ per objective with the matrix quantised and resident in HBM (the `value` arm of 
 timed rounds).  Labels are a fixed map of the C3 label y, with no new randomness:
   float32(log1p(exp(y/10)) + 1e-3)  for count:poisson, reg:gamma, reg:tweedie, reg:squaredlogerror, reg:pseudohubererror;
   float32(sigmoid(y/10))            for reg:logistic, binary:logistic, binary:logitraw;
-  y itself                          for reg:squarederror.
+  y itself                          for reg:squarederror;
+  survival:aft reads bounds built from the positive map t by row index: row mod 4 = 0 -> [t, t], 1 -> [t, +inf),
+  2 -> [0, t], 3 -> [t, 2t].
 For every objective a 200k-row, 3-round sub-problem is also compared tree for tree with the CPU oracle grown from the
 gradients of tests/objective_reference.py (split feature / bin / default direction exact, leaf values within 1e-5).
 Prints one JSON line with one entry per objective.  Writes nothing to the tree.
@@ -25,7 +27,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-POSITIVE = ("count:poisson", "reg:gamma", "reg:tweedie", "reg:squaredlogerror", "reg:pseudohubererror")
+POSITIVE = ("count:poisson", "reg:gamma", "reg:tweedie", "reg:squaredlogerror", "reg:pseudohubererror", "survival:aft")
 UNIT = ("reg:logistic", "binary:logistic", "binary:logitraw")
 
 
@@ -39,12 +41,30 @@ def objective_labels(objective, y):
     return y
 
 
+def aft_bounds(t):
+    """survival:aft bounds of the positive label map t (see the module docstring)."""
+    k = np.arange(len(t)) % 4
+    lo = np.where(k == 2, np.float32(0.0), t).astype(np.float32)
+    hi = np.where(k == 1, np.float32(np.inf), np.where(k == 3, t * np.float32(2.0), t)).astype(np.float32)
+    return lo, hi
+
+
+def make_matrix(E, objective, X, y):
+    if objective == "survival:aft":
+        lo, hi = aft_bounds(y)
+        return E.DMatrix(X, label=y, label_lower_bound=lo, label_upper_bound=hi)
+    return E.DMatrix(X, label=y)
+
+
 def oracle_match(E, params, X, y):
     from oracle import oracle as O
     from tests import objective_reference as R
-    d = E.DMatrix(X, label=y)
+    d = make_matrix(E, params["objective"], X, y)
     b = E.train(params, d, num_boost_round=3, verbose_eval=False)
-    if params["objective"] in R.OBJECTIVES:
+    if params["objective"] == "survival:aft":
+        from tests import survival_reference as S
+        ob = S.train(O, params, X, *aft_bounds(y), 3)
+    elif params["objective"] in R.OBJECTIVES:
         ob = R.train(O, params, X, y, 3)
     else:
         ob, _ = O.train(params, X, y, 3)
@@ -76,7 +96,7 @@ def main():
     out = {}
     for obj in args.objectives.split(","):
         params = dict(bench.PARAMS, max_depth=depth, objective=obj)
-        dm = E.DMatrix(X, label=objective_labels(obj, y0))
+        dm = make_matrix(E, obj, X, objective_labels(obj, y0))
         dm._ensure_quantized(256)
         bst = E.Booster(params, cache=[dm])
         for r in range(args.warmup):

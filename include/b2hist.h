@@ -73,7 +73,9 @@ int B2_MatrixCreateFromProcess(int64_t pid, uint64_t remote_addr, int64_t remote
  * peer memory).  Result: the same device matrix B2_MatrixCreateFromProcess builds from the strided shard. */
 int B2_MatrixCreateFromProcessInterleaved(int64_t pid, uint64_t remote_addr, int64_t n_total_rows, int32_t n_cols,
                                           int32_t shard_rank, B2Handle comm, float missing, int device, B2Handle* out);
-/* field: "label" | "weight" | "base_margin" (len n_rows, or n_rows*num_class for base_margin) */
+/* field: "label" | "weight" | "base_margin" (len n_rows, or n_rows*num_class for base_margin) |
+ * "label_lower_bound" | "label_upper_bound" (len n_rows, 0 clears): the survival bounds of each row, read by
+ * survival:aft only (lower == upper: exact time; upper = +inf: right-censored; lower = 0: left-censored) */
 int B2_MatrixSetFloatInfo(B2Handle m, const char* field, const float* values, int64_t len);
 /* feature types: is_cat[f] != 0 marks feature f categorical (xgb.DMatrix(feature_types=[...'c'...],
  * enable_categorical=True), forwarded by _get_dmatrix, xgboost_ray/main.py:365-376 / matrix.py:159,193).  Must be
@@ -109,8 +111,12 @@ int B2_BoosterCreate(const char* params, B2Handle train, B2Handle comm, B2Handle
 int B2_BoosterUpdateOneIter(B2Handle b, int32_t iter);
 /* custom objective (xgb.train(obj=...), tests/test_xgboost_api.py:77-102): grad/hess [n_rows*num_class] */
 int B2_BoosterBoostOneIter(B2Handle b, const float* grad, const float* hess, int64_t len);
+/* diagnostic: the fp32 gradient pairs of the last round on the train matrix, class-major ([num_class][n_rows]),
+ * as the trees of that round saw them (after the weight, before quantisation).  len = n_rows * num_class. */
+int B2_BoosterGetGradients(B2Handle b, float* grad, float* hess, int64_t len);
 /* metric value of `m` (the train matrix or a matrix with raw data) under the current model, reduced
- * over comm like xgboost's (sum, wsum) allreduce.  metric: rmse|logloss|error|mlogloss|merror */
+ * over comm like xgboost's (sum, wsum) allreduce.  metric: rmse|logloss|error|mlogloss|merror|...|aft-nloglik|
+ * interval-regression-accuracy (the last two need survival:aft and the label bounds of `m`) */
 int B2_BoosterEvalSet(B2Handle b, B2Handle m, const char* metric, double* out);
 /* out [n_rows*num_class].  tree_end == 0 means all trees.  training == margin cache of train set. */
 int B2_BoosterPredict(B2Handle b, B2Handle m, int32_t output_margin, int32_t tree_begin, int32_t tree_end,

@@ -84,6 +84,11 @@ int b2_launch_iota(int32_t*, int64_t, cudaStream_t);
 int b2_launch_gradient(int, int, const float*, const float*, const float*, int64_t, float, float, float2*, uint32_t*, uint32_t*, int,
                        cudaStream_t);
 int b2_launch_label_check(int, const float*, int64_t, uint32_t*, int, cudaStream_t);
+int b2_launch_gradient_aft(int, double, const float*, const float*, const float*, const float*, int64_t, float2*, uint32_t*,
+                           uint32_t*, int, cudaStream_t);
+int b2_launch_aft_bounds_check(const float*, const float*, int64_t, uint32_t*, int, cudaStream_t);
+int b2_launch_aft_metric(int, int, double, const float*, const float*, const float*, const float*, int64_t, double*, int,
+                         cudaStream_t);
 int b2_launch_pack_custom(const float*, const float*, int, int64_t, float2*, int, cudaStream_t);
 int b2_launch_absmax(const float2*, int64_t, uint32_t*, int, cudaStream_t);
 int b2_launch_quant_exponent(const uint32_t*, int32_t*, cudaStream_t);
@@ -487,6 +492,9 @@ struct Matrix : HandleBase {
   bool any_cat() const { return !cat_feats.empty(); }
   DevBuf<float> label, weight, base_margin;
   int64_t n_label = 0, n_weight = 0, n_base_margin = 0;
+  DevBuf<float> lower, upper;          // survival label bounds (label_lower_bound / label_upper_bound), read by survival:aft
+  int64_t n_lower = 0, n_upper = 0;
+  bool has_bounds() const { return n_lower == n && n_upper == n; }
   std::vector<uint32_t> fwq;          // feature_weights in Q16 (empty = all 1.0)
   DevBuf<uint32_t> d_fwq;
 };
@@ -697,8 +705,8 @@ void bin_matrix(Matrix* m) {
 // ---------------------------------------------------------------- booster
 // objective ids, shared with objective_kernel.cu (the kernels take them as plain ints)
 enum { kObjSquaredError = 0, kObjLogistic = 1, kObjSoftprob = 2, kObjRegLogistic = 3, kObjLogitRaw = 4, kObjSquaredLog = 5,
-       kObjPseudoHuber = 6, kObjPoisson = 7, kObjGamma = 8, kObjTweedie = 9 };
-bool obj_log_link(int o) { return o == kObjPoisson || o == kObjGamma || o == kObjTweedie; }
+       kObjPseudoHuber = 6, kObjPoisson = 7, kObjGamma = 8, kObjTweedie = 9, kObjAft = 10 };
+bool obj_log_link(int o) { return o == kObjPoisson || o == kObjGamma || o == kObjTweedie || o == kObjAft; }
 bool obj_sigmoid(int o) { return o == kObjLogistic || o == kObjRegLogistic; }
 // objectives whose gradient kernel reports non-finite gradient pairs (gradient_param_kernel)
 bool obj_checks_finite(int o) { return o >= kObjSquaredLog; }
@@ -719,6 +727,8 @@ struct Params {
   bool max_delta_step_set = false;             // false: count:poisson uses 0.7 (xgboost's Learner::ConfigureObjective)
   float huber_slope = 1.0f;                    // reg:pseudohubererror delta (also the mphe metric's)
   float tweedie_variance_power = 1.5f;         // reg:tweedie rho in [1, 2)
+  int aft_dist = 0;                            // survival:aft distribution: 0 normal, 1 logistic, 2 extreme
+  float aft_sigma = 1.0f;                      // survival:aft scale sigma > 0
   float subsample = 1.0f, colsample_bytree = 1.0f, colsample_bylevel = 1.0f, colsample_bynode = 1.0f;
   int seed = 0;
   bool base_score_set = false;   // false: estimated from the labels before the first tree (xgboost >= 2.0, A.3)
@@ -815,6 +825,7 @@ struct Booster : HandleBase {
   bool graph_failed = false;
   bool absmax_fused = false;               // this round's gradient kernel already produced d_absmax[k]
   bool labels_checked = false;             // the train labels are inside the objective's domain (check_labels)
+  bool gh_ready = false;                   // gh holds the gradient pairs of a round (B2_BoosterGetGradients)
   DevBuf<uint32_t> d_grad_err;             // set by the gradient kernel when a gradient pair is not finite
   uint32_t* h_grad_err = nullptr;          // pinned copy, written at the end of the round's stream work
   DevBuf<uint16_t> pos;                    // [n] leaf index of every row (final_assign / leaf_sums -> margin_update)
@@ -918,9 +929,10 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
       else if (v == "count:poisson") p->objective = kObjPoisson;
       else if (v == "reg:gamma") p->objective = kObjGamma;
       else if (v == "reg:tweedie") p->objective = kObjTweedie;
+      else if (v == "survival:aft") p->objective = kObjAft;
       else fail("unsupported objective '%s' (supported: reg:squarederror, reg:logistic, binary:logistic, binary:logitraw, "
-                "reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie, multi:softprob, "
-                "multi:softmax)", v.c_str());
+                "reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie, survival:aft, "
+                "multi:softprob, multi:softmax)", v.c_str());
     } else if (k == "num_class") p->num_class = i();
     else if (k == "num_parallel_tree") p->num_parallel_tree = i();
     else if (k == "max_depth") p->max_depth = i();
@@ -944,6 +956,13 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     else if (k == "max_delta_step") { p->max_delta_step = f(); p->max_delta_step_set = true; }
     else if (k == "huber_slope") p->huber_slope = f();
     else if (k == "tweedie_variance_power") p->tweedie_variance_power = f();
+    else if (k == "aft_loss_distribution") {
+      if (v == "normal") p->aft_dist = 0;
+      else if (v == "logistic") p->aft_dist = 1;
+      else if (v == "extreme") p->aft_dist = 2;
+      else fail("aft_loss_distribution must be normal, logistic or extreme, got '%s'", v.c_str());
+    }
+    else if (k == "aft_loss_distribution_scale") p->aft_sigma = f();
     else if (k == "max_cat_to_onehot") p->max_cat_to_onehot = i();
     else if (k == "max_cat_threshold") p->max_cat_threshold = i();
     else if (k == "max_bin") { if (max_bin_out) *max_bin_out = i(); }
@@ -966,6 +985,10 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     fail("huber_slope must be > 0 for reg:pseudohubererror, got %g", (double)p->huber_slope);
   if (p->objective == kObjTweedie && !(p->tweedie_variance_power >= 1.0f && p->tweedie_variance_power < 2.0f))
     fail("tweedie_variance_power must be in [1, 2), got %g", (double)p->tweedie_variance_power);
+  if (!(p->aft_sigma > 0.0f) || std::isinf(p->aft_sigma))
+    fail("aft_loss_distribution_scale must be finite and > 0, got %g", (double)p->aft_sigma);
+  // survival:aft fits no intercept: base_score defaults to 0.5 (margin log 0.5) and is never estimated
+  if (p->objective == kObjAft && !p->base_score_set) { p->base_score = 0.5f; p->base_score_set = true; }
   if (p->base_score_set) {
     if (p->objective == kObjRegLogistic && !(p->base_score > 0.0f && p->base_score < 1.0f))
       fail("base_score must be in (0, 1) for reg:logistic, got %g", (double)p->base_score);
@@ -1745,9 +1768,30 @@ void estimate_base_score(Booster* b) {
   p.base_score_set = true;
 }
 
+// survival:aft reads the label bounds instead of the label: both present, no NaN, 0 <= lower (finite) <= upper, and an
+// uncensored row (lower == upper) needs y > 0.  Once per train matrix, like check_labels.
+void check_bounds(Booster* b) {
+  Matrix* m = b->train; cudaStream_t s = b->ctx->stream;
+  if (b->labels_checked) return;
+  if (!m->has_bounds()) fail("survival:aft needs label_lower_bound and label_upper_bound");
+  DevBuf<uint32_t> bad; bad.ensure(4);
+  CUDA_CHECK(cudaMemsetAsync(bad.p, 0, 4 * sizeof(uint32_t), s));
+  LAUNCH_CHECK(b2_launch_aft_bounds_check(m->lower.p, m->upper.p, m->n, bad.p, b->ctx->num_sms, s));
+  allreduce(b->comm, bad.p, 4, kNcclUint32, kNcclMax, s);
+  uint32_t h[4] = {0, 0, 0, 0};
+  CUDA_CHECK(cudaMemcpyAsync(h, bad.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  if (h[0]) fail("survival:aft: label bounds must not be NaN");
+  if (h[1]) fail("survival:aft: label_lower_bound must be finite and >= 0");
+  if (h[2]) fail("survival:aft: label_upper_bound must be >= label_lower_bound");
+  if (h[3]) fail("survival:aft: an uncensored row (lower == upper) needs a label > 0");
+  b->labels_checked = true;
+}
+
 // labels outside the objective's domain fail training (xgboost's CheckLabel); once per train matrix, before the first tree
 void check_labels(Booster* b) {
   Matrix* m = b->train; const int o = b->p.objective; cudaStream_t s = b->ctx->stream;
+  if (o == kObjAft) { check_bounds(b); return; }
   if (o == kObjSquaredError || o == kObjLogistic || o == kObjSoftprob || o == kObjPseudoHuber || b->labels_checked) return;
   if (m->n_label != m->n) fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)m->n);
   DevBuf<uint32_t> bad; bad.ensure(1);
@@ -1801,7 +1845,8 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
     CUDA_CHECK(cudaMemcpyAsync(b->d_custom_h.p, custom_h, len * sizeof(float), cudaMemcpyHostToDevice, s));
     LAUNCH_CHECK(b2_launch_pack_custom(b->d_custom_g.p, b->d_custom_h.p, K, n, b->gh.p, b->ctx->num_sms, s));
   } else {
-    if (m->n_label != n) fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)n);
+    if (b->p.objective != kObjAft && m->n_label != n)
+      fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)n);
     // the |g|,|h| maxima of every class tree come out of the same pass unless rows are dropped afterwards (subsample)
     b->absmax_fused = b->p.subsample >= 1.0f && K <= b2_gradient_fused_max_classes();
     if (b->absmax_fused) CUDA_CHECK(cudaMemsetAsync(b->d_absmax.p, 0, 2 * (size_t)K * sizeof(uint32_t), s));
@@ -1810,11 +1855,17 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
       if (!b->h_grad_err) { CUDA_CHECK(cudaMallocHost(&b->h_grad_err, sizeof(uint32_t))); b->d_grad_err.ensure(1); }
       CUDA_CHECK(cudaMemsetAsync(b->d_grad_err.p, 0, sizeof(uint32_t), s));
     }
-    LAUNCH_CHECK(b2_launch_gradient(b->p.objective, K, b->margin.p, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
-                                    b->p.scale_pos_weight, objective_param(b->p), b->gh.p,
-                                    b->absmax_fused ? b->d_absmax.p : nullptr, check_finite ? b->d_grad_err.p : nullptr,
-                                    b->ctx->num_sms, s));
+    if (b->p.objective == kObjAft)
+      LAUNCH_CHECK(b2_launch_gradient_aft(b->p.aft_dist, (double)b->p.aft_sigma, b->margin.p, m->lower.p, m->upper.p,
+                                          m->n_weight ? m->weight.p : nullptr, n, b->gh.p,
+                                          b->absmax_fused ? b->d_absmax.p : nullptr, b->d_grad_err.p, b->ctx->num_sms, s));
+    else
+      LAUNCH_CHECK(b2_launch_gradient(b->p.objective, K, b->margin.p, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
+                                      b->p.scale_pos_weight, objective_param(b->p), b->gh.p,
+                                      b->absmax_fused ? b->d_absmax.p : nullptr, check_finite ? b->d_grad_err.p : nullptr,
+                                      b->ctx->num_sms, s));
   }
+  b->gh_ready = true;
   b->t.kernel_launches++;
   const int npt = b->p.num_parallel_tree;
   // row sampling zeroes the dropped rows' gradient pairs in place: the parallel trees of a round each sample from the
@@ -1891,8 +1942,11 @@ int metric_id(const char* name, const Params& p, float* param) {
   if (s == "merror") return 4;
   if (s == "mae") return 5;
   if (s == "auc") return 6;
+  if (s == "aft-nloglik") return 14;
+  if (s == "interval-regression-accuracy") return 15;
   fail("unsupported eval metric '%s' (supported: rmse, mae, logloss, error, auc, mlogloss, merror, rmsle, mape, mphe, "
-       "poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho)", s.c_str());
+       "poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy)",
+       s.c_str());
 }
 
 // margin of matrix m under the current model (cached per matrix, only new trees are applied)
@@ -2206,6 +2260,11 @@ int B2_MatrixSetFloatInfo(B2Handle mh, const char* field, const float* values, i
   DevBuf<float>* dst = nullptr; int64_t* cnt = nullptr;
   if (f == "label") { dst = &m->label; cnt = &m->n_label; if (len != m->n) fail("label length %lld != rows %lld", (long long)len, (long long)m->n); }
   else if (f == "weight") { dst = &m->weight; cnt = &m->n_weight; if (len != m->n && len != 0) fail("weight length %lld != rows %lld", (long long)len, (long long)m->n); }
+  else if (f == "label_lower_bound" || f == "label_upper_bound") {
+    const bool lo = f == "label_lower_bound";
+    dst = lo ? &m->lower : &m->upper; cnt = lo ? &m->n_lower : &m->n_upper;
+    if (len != m->n && len != 0) fail("%s length %lld != rows %lld", f.c_str(), (long long)len, (long long)m->n);
+  }
   else if (f == "base_margin") { dst = &m->base_margin; cnt = &m->n_base_margin; m->margin_version++; if (len != 0 && (m->n == 0 || len % m->n != 0)) fail("base_margin length %lld is not a multiple of rows %lld", (long long)len, (long long)m->n); }
   else if (f == "feature_weights") {
     // DMatrix.set_info(feature_weights=...) (main.py:439-442): weights of the column sampler, Q16 fixed point
@@ -2365,6 +2424,20 @@ int B2_BoosterBoostOneIter(B2Handle bh, const float* grad, const float* hess, in
   boost_round(b, grad, hess, len);
   API_END
 }
+int B2_BoosterGetGradients(B2Handle bh, float* grad, float* hess, int64_t len) {
+  API_BEGIN
+  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  if (!b->train) fail("this booster has no train matrix (prediction-only)");
+  const int64_t nk = b->train->n * b->p.num_class;
+  if (len != nk) fail("gradient buffers have %lld values, expected %lld", (long long)len, (long long)nk);
+  if (!b->gh_ready) fail("no gradients yet: run a boosting round first");
+  CUDA_CHECK(cudaSetDevice(b->ctx->device));
+  std::vector<float2> h((size_t)std::max<int64_t>(nk, 1));
+  if (nk > 0) CUDA_CHECK(cudaMemcpyAsync(h.data(), b->gh.p, (size_t)nk * sizeof(float2), cudaMemcpyDeviceToHost, b->ctx->stream));
+  CUDA_CHECK(cudaStreamSynchronize(b->ctx->stream));
+  for (int64_t i = 0; i < nk; ++i) { grad[i] = h[i].x; hess[i] = h[i].y; }
+  API_END
+}
 int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
@@ -2373,12 +2446,26 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
   cudaStream_t s = b->ctx->stream;
   float mparam = 0.0f;
   const int mid = metric_id(metric, b->p, &mparam);
-  if (m->n_label != m->n) fail("evaluation matrix has no labels");
+  const bool aft_metric = mid == 14 || mid == 15;
+  if (aft_metric && b->p.objective != kObjAft)
+    fail("metric '%s' does not fit objective '%s'", metric, b->p.objective_name.c_str());
+  if (aft_metric && !m->has_bounds()) fail("metric '%s' needs label_lower_bound and label_upper_bound on the evaluation matrix", metric);
+  if (!aft_metric && m->n_label != m->n) fail("evaluation matrix has no labels");
   float* margin = eval_margin(b, m);
   b->d_metric.ensure(2);
   CUDA_CHECK(cudaMemsetAsync(b->d_metric.p, 0, 2 * sizeof(double), s));
   if ((mid == 3 || mid == 4) != (b->p.objective == kObjSoftprob))
     fail("metric '%s' does not fit objective '%s'", metric, b->p.objective_name.c_str());
+  if (aft_metric) {
+    LAUNCH_CHECK(b2_launch_aft_metric(b->p.aft_dist, mid, (double)b->p.aft_sigma, margin, m->lower.p, m->upper.p,
+                                      m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p, b->ctx->num_sms, s));
+    allreduce(b->comm, b->d_metric.p, 2, kNcclFloat64, kNcclSum, s);
+    double h[2];
+    CUDA_CHECK(cudaMemcpyAsync(h, b->d_metric.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    *out = h[1] > 0 ? h[0] / h[1] : 0.0;
+    return 0;
+  }
   if (mid == 6) {
     // binary ROC AUC on the transformed prediction (auc_kernel.cu): local (area, fp*tp) pairs summed over the workers
     if (b->p.objective == kObjSoftprob) fail("metric 'auc' is implemented for binary labels (binary:logistic / regression scores) only");

@@ -85,17 +85,156 @@ __device__ __forceinline__ float b2_log1pf(float x) {
   return __fadd_rn(r, __fmul_rn(dk, ln2_hi));
 }
 
+// binary64 exp, log and erf for survival:aft: fdlibm's published algorithms (e_exp.c, e_log.c, s_erf.c) written out
+// in __dadd_rn / __dmul_rn / __ddiv_rn, so that tests/survival_reference.py replays them bit for bit (CUDA's own
+// exp / log / erf are not fixed sequences a host can repeat).  Both are within 1 ulp of the correctly rounded value.
+#define B2_DA __dadd_rn
+#define B2_DS(a, b) __dadd_rn(a, -(b))
+#define B2_DM __dmul_rn
+#define B2_DD __ddiv_rn
+__device__ __forceinline__ double b2_add_exponent(double y, int k) {
+  return __longlong_as_double(__double_as_longlong(y) + ((long long)k << 52));
+}
+__device__ __forceinline__ double b2_exp(double x) {
+  const double ln2_hi = 6.93147180369123816490e-01, ln2_lo = 1.90821492927058770002e-10;
+  const double P1 = 1.66666666666666019037e-01, P2 = -2.77777777770155933842e-03, P3 = 6.61375632143793436117e-05,
+               P4 = -1.65339022054652515390e-06, P5 = 4.13813679705723846039e-08;
+  const int hx0 = __double2hiint(x), xsb = (hx0 >> 31) & 1, hx = hx0 & 0x7fffffff;
+  if (hx >= 0x40862E42) {                                 // |x| >= 709.78
+    if (hx >= 0x7ff00000) return x != x ? B2_DA(x, x) : (xsb ? 0.0 : x);
+    if (x > 7.09782712893383973096e+02) return INFINITY;
+    if (x < -7.45133219101941108420e+02) return 0.0;
+  }
+  double hi = x, lo = 0.0;
+  int k = 0;
+  if (hx > 0x3fd62e42) {                                  // |x| > 0.5 ln2
+    if (hx < 0x3FF0A2B2) {                                // and |x| < 1.5 ln2
+      hi = xsb ? B2_DA(x, ln2_hi) : B2_DS(x, ln2_hi); lo = xsb ? -ln2_lo : ln2_lo; k = 1 - xsb - xsb;
+    } else {
+      k = (int)B2_DA(B2_DM(1.44269504088896338700e+00, x), xsb ? -0.5 : 0.5);
+      const double t = (double)k;
+      hi = B2_DS(x, B2_DM(t, ln2_hi)); lo = B2_DM(t, ln2_lo);
+    }
+    x = B2_DS(hi, lo);
+  } else if (hx < 0x3e300000) {                           // |x| < 2^-28
+    return B2_DA(1.0, x);
+  }
+  const double t = B2_DM(x, x);
+  const double c = B2_DS(x, B2_DM(t, B2_DA(P1, B2_DM(t, B2_DA(P2, B2_DM(t, B2_DA(P3, B2_DM(t, B2_DA(P4, B2_DM(t, P5))))))))));
+  if (k == 0) return B2_DS(1.0, B2_DS(B2_DD(B2_DM(x, c), B2_DS(c, 2.0)), x));
+  const double y = B2_DS(1.0, B2_DS(B2_DS(lo, B2_DD(B2_DM(x, c), B2_DS(2.0, c))), hi));
+  if (k >= -1021) return b2_add_exponent(y, k);
+  return B2_DM(b2_add_exponent(y, k + 1000), 9.33263618503218878990e-302);
+}
+__device__ __forceinline__ double b2_log(double x) {
+  const double ln2_hi = 6.93147180369123816490e-01, ln2_lo = 1.90821492927058770002e-10;
+  const double Lg1 = 6.666666666666735130e-01, Lg2 = 3.999999999940941908e-01, Lg3 = 2.857142874366239149e-01,
+               Lg4 = 2.222219843214978396e-01, Lg5 = 1.818357216161805012e-01, Lg6 = 1.531383769920937332e-01,
+               Lg7 = 1.479819860511658591e-01;
+  int hx = __double2hiint(x);
+  const int lx = __double2loint(x);
+  int k = 0;
+  if (hx < 0x00100000) {                                  // x < 2^-1022
+    if (((hx & 0x7fffffff) | lx) == 0) return -INFINITY;
+    if (hx < 0) return NAN;
+    k -= 54; x = B2_DM(x, 1.80143985094819840000e+16);   // subnormal: scale up
+    hx = __double2hiint(x);
+  }
+  if (hx >= 0x7ff00000) return B2_DA(x, x);
+  k += (hx >> 20) - 1023;
+  hx &= 0x000fffff;
+  int i = (hx + 0x95f64) & 0x100000;
+  x = __hiloint2double(hx | (i ^ 0x3ff00000), __double2loint(x));   // normalise x or x/2
+  k += i >> 20;
+  const double f = B2_DS(x, 1.0), dk = (double)k;
+  if ((0x000fffff & (2 + hx)) < 3) {                      // |f| < 2^-20
+    if (f == 0.0) return k == 0 ? 0.0 : B2_DA(B2_DM(dk, ln2_hi), B2_DM(dk, ln2_lo));
+    const double R = B2_DM(B2_DM(f, f), B2_DS(0.5, B2_DM(0.33333333333333333, f)));
+    return k == 0 ? B2_DS(f, R) : B2_DS(B2_DM(dk, ln2_hi), B2_DS(B2_DS(R, B2_DM(dk, ln2_lo)), f));
+  }
+  const double s = B2_DD(f, B2_DA(2.0, f)), z = B2_DM(s, s), w = B2_DM(z, z);
+  i = hx - 0x6147a;
+  const int j = 0x6b851 - hx;
+  const double t1 = B2_DM(w, B2_DA(Lg2, B2_DM(w, B2_DA(Lg4, B2_DM(w, Lg6)))));
+  const double t2 = B2_DM(z, B2_DA(Lg1, B2_DM(w, B2_DA(Lg3, B2_DM(w, B2_DA(Lg5, B2_DM(w, Lg7)))))));
+  i |= j;
+  const double R = B2_DA(t2, t1);
+  if (i > 0) {
+    const double hfsq = B2_DM(B2_DM(0.5, f), f);
+    if (k == 0) return B2_DS(f, B2_DS(hfsq, B2_DM(s, B2_DA(hfsq, R))));
+    return B2_DS(B2_DM(dk, ln2_hi), B2_DS(B2_DS(hfsq, B2_DA(B2_DM(s, B2_DA(hfsq, R)), B2_DM(dk, ln2_lo))), f));
+  }
+  if (k == 0) return B2_DS(f, B2_DM(s, B2_DS(f, R)));
+  return B2_DS(B2_DM(dk, ln2_hi), B2_DS(B2_DS(B2_DM(s, B2_DS(f, R)), B2_DM(dk, ln2_lo)), f));
+}
+__device__ double b2_erf(double x) {
+  const int hx = __double2hiint(x), ix = hx & 0x7fffffff;
+  if (ix >= 0x7ff00000) return x != x ? B2_DA(x, x) : (hx < 0 ? -1.0 : 1.0);
+  if (ix < 0x3feb0000) {                                  // |x| < 0.84375
+    if (ix < 0x3e300000) {                                // |x| < 2^-28
+      if (ix < 0x00800000) return B2_DM(0.125, B2_DA(B2_DM(8.0, x), B2_DM(1.02703333676410069053e+00, x)));
+      return B2_DA(x, B2_DM(1.28379167095512586316e-01, x));
+    }
+    const double z = B2_DM(x, x);
+    const double r = B2_DA(1.28379167095512558561e-01, B2_DM(z, B2_DA(-3.25042107247001499370e-01, B2_DM(z,
+                     B2_DA(-2.84817495755985104766e-02, B2_DM(z, B2_DA(-5.77027029648944159157e-03,
+                     B2_DM(z, -2.37630166566501626084e-05))))))));
+    const double s = B2_DA(1.0, B2_DM(z, B2_DA(3.97917223959155352819e-01, B2_DM(z, B2_DA(6.50222499887672944485e-02,
+                     B2_DM(z, B2_DA(5.08130628187576562776e-03, B2_DM(z, B2_DA(1.32494738004321644526e-04,
+                     B2_DM(z, -3.96022827877536812320e-06))))))))));
+    return B2_DA(x, B2_DM(x, B2_DD(r, s)));
+  }
+  if (ix < 0x3ff40000) {                                  // 0.84375 <= |x| < 1.25
+    const double s = B2_DS(fabs(x), 1.0);
+    const double P = B2_DA(-2.36211856075265944077e-03, B2_DM(s, B2_DA(4.14856118683748331666e-01, B2_DM(s,
+                     B2_DA(-3.72207876035701323847e-01, B2_DM(s, B2_DA(3.18346619901161753674e-01, B2_DM(s,
+                     B2_DA(-1.10894694282396677476e-01, B2_DM(s, B2_DA(3.54783043256182359371e-02,
+                     B2_DM(s, -2.16637559486879084300e-03))))))))))));
+    const double Q = B2_DA(1.0, B2_DM(s, B2_DA(1.06420880400844228286e-01, B2_DM(s, B2_DA(5.40397917702171048937e-01,
+                     B2_DM(s, B2_DA(7.18286544141962662868e-02, B2_DM(s, B2_DA(1.26171219808761642112e-01,
+                     B2_DM(s, B2_DA(1.36370839120290507362e-02, B2_DM(s, 1.19844998467991074170e-02))))))))))));
+    const double erx = 8.45062911510467529297e-01;
+    return hx >= 0 ? B2_DA(erx, B2_DD(P, Q)) : B2_DS(-erx, B2_DD(P, Q));
+  }
+  if (ix >= 0x40180000) return hx >= 0 ? B2_DS(1.0, 1e-300) : B2_DS(1e-300, 1.0);   // |x| >= 6
+  const double ax = fabs(x), s = B2_DD(1.0, B2_DM(ax, ax));
+  double R, S;
+  if (ix < 0x4006DB6E) {                                  // |x| < 1/0.35
+    R = B2_DA(-9.86494403484714822705e-03, B2_DM(s, B2_DA(-6.93858572707181764372e-01, B2_DM(s,
+        B2_DA(-1.05586262253232909814e+01, B2_DM(s, B2_DA(-6.23753324503260060396e+01, B2_DM(s,
+        B2_DA(-1.62396669462573470355e+02, B2_DM(s, B2_DA(-1.84605092906711035994e+02, B2_DM(s,
+        B2_DA(-8.12874355063065934246e+01, B2_DM(s, -9.81432934416914548592e+00))))))))))))));
+    S = B2_DA(1.0, B2_DM(s, B2_DA(1.96512716674392571292e+01, B2_DM(s, B2_DA(1.37657754143519042600e+02, B2_DM(s,
+        B2_DA(4.34565877475229228821e+02, B2_DM(s, B2_DA(6.45387271733267880336e+02, B2_DM(s,
+        B2_DA(4.29008140027567833386e+02, B2_DM(s, B2_DA(1.08635005541779435134e+02, B2_DM(s,
+        B2_DA(6.57024977031928170135e+00, B2_DM(s, -6.04244152148580987438e-02))))))))))))))));
+  } else {
+    R = B2_DA(-9.86494292470009928597e-03, B2_DM(s, B2_DA(-7.99283237680523006574e-01, B2_DM(s,
+        B2_DA(-1.77579549177547519889e+01, B2_DM(s, B2_DA(-1.60636384855821916062e+02, B2_DM(s,
+        B2_DA(-6.37566443368389627722e+02, B2_DM(s, B2_DA(-1.02509513161107724954e+03,
+        B2_DM(s, -4.83519191608651397019e+02))))))))))));
+    S = B2_DA(1.0, B2_DM(s, B2_DA(3.03380607434824582924e+01, B2_DM(s, B2_DA(3.25792512996573918826e+02, B2_DM(s,
+        B2_DA(1.53672958608443695994e+03, B2_DM(s, B2_DA(3.19985821950859553908e+03, B2_DM(s,
+        B2_DA(2.55305040643316442583e+03, B2_DM(s, B2_DA(4.74528541206955367215e+02,
+        B2_DM(s, -2.24409524465858183362e+01))))))))))))));
+  }
+  const double z = __hiloint2double(__double2hiint(ax), 0);
+  const double r = B2_DM(b2_exp(B2_DS(B2_DM(-z, z), 0.5625)), b2_exp(B2_DA(B2_DM(B2_DS(z, ax), B2_DA(z, ax)), B2_DD(R, S))));
+  return hx >= 0 ? B2_DS(1.0, B2_DD(r, ax)) : B2_DS(B2_DD(r, ax), 1.0);
+}
+
 // objective ids (engine.cu kObj*): 0 reg:squarederror, 1 binary:logistic, 2 multi:softprob, 3 reg:logistic,
-// 4 binary:logitraw, 5 reg:squaredlogerror, 6 reg:pseudohubererror, 7 count:poisson, 8 reg:gamma, 9 reg:tweedie
+// 4 binary:logitraw, 5 reg:squaredlogerror, 6 reg:pseudohubererror, 7 count:poisson, 8 reg:gamma, 9 reg:tweedie,
+// 10 survival:aft
 constexpr int kObjRegLogistic = 3, kObjLogitRaw = 4, kObjSquaredLog = 5, kObjPseudoHuber = 6, kObjPoisson = 7,
-              kObjGamma = 8, kObjTweedie = 9;
+              kObjGamma = 8, kObjTweedie = 9, kObjAft = 10;
 // the parameter of an objective that has one: huber_slope, max_delta_step (Poisson hessian), tweedie_variance_power
 struct ObjParam { float a; };
 
 // margin -> prediction of one scalar output (ObjFunction::PredTransform): sigmoid, exp or identity
 __device__ __forceinline__ float b2_pred_transform(int objective, float m) {
   if (objective == 1 || objective == kObjRegLogistic) return b2_sigmoid(m);
-  if (objective == kObjPoisson || objective == kObjGamma || objective == kObjTweedie) return b2_expf(m);
+  if (objective == kObjPoisson || objective == kObjGamma || objective == kObjTweedie || objective == kObjAft) return b2_expf(m);
   return m;
 }
 
@@ -206,6 +345,177 @@ gradient_param_kernel(const float* __restrict__ margin, const float* __restrict_
   }
   if (bad && err) atomicOr(err, 1u);
   if (absmax) absmax_publish(mg, mh, absmax);
+}
+
+// ---- survival:aft (accelerated failure time).  log y = margin + sigma Z with Z standard normal, logistic or extreme
+// (Gumbel-min); a row gives a bound pair [lower, upper]: lower == upper is an exact time, upper = +inf right-censored,
+// lower = 0 left-censored, otherwise interval-censored.  With z = (log y - margin) / sigma, f the pdf and F the CDF of Z:
+//   uncensored  loss -log(max(f(z) / (sigma y), kEps)),   g = f'/(sigma f),   h = -(f'' f - f'^2) / (sigma^2 f^2)
+//   censored    loss -log(max(F(z_u) - F(z_l), kEps)),   g = (f_u - f_l) / (sigma dF),
+//               h = ((f_u - f_l)^2 - (f'_u - f'_l) dF) / (sigma^2 dF^2)
+// in binary64 (tests/survival_reference.py replays the sequence).  A quotient that is not finite while its denominator
+// is below kEps takes its limit as the margin goes to -inf (z > 0; z_u > 0 or z_l > 0 for censored rows) or +inf; then
+// g is clipped to [-15, 15] and h to [1e-16, 15].
+constexpr int kAftNormal = 0, kAftLogistic = 1, kAftExtreme = 2;
+constexpr double kAftEps = 1e-12;
+struct AftDensity { double pdf, cdf, dpdf, d2pdf; };
+
+template <int kDist>
+__device__ __forceinline__ AftDensity aft_density(double z) {
+  AftDensity d;
+  if (kDist == kAftNormal) {
+    d.pdf = B2_DM(b2_exp(B2_DM(B2_DM(-z, z), 0.5)), 0.3989422804014327);     // 1 / sqrt(2 pi)
+    d.cdf = B2_DM(0.5, B2_DA(1.0, b2_erf(B2_DM(z, 0.7071067811865476))));   // erf(z / sqrt(2))
+    d.dpdf = B2_DM(-z, d.pdf);
+    d.d2pdf = B2_DM(B2_DS(B2_DM(z, z), 1.0), d.pdf);
+  } else {
+    const double w = b2_exp(z), w2 = B2_DM(w, w);
+    const bool inf_w = isinf(w), inf_w2 = inf_w || isinf(w2);
+    if (kDist == kAftLogistic) {
+      const double opw = B2_DA(1.0, w);
+      d.pdf = inf_w2 ? 0.0 : B2_DD(w, B2_DM(opw, opw));
+      d.cdf = inf_w ? 1.0 : B2_DD(w, opw);
+      d.dpdf = inf_w ? 0.0 : B2_DD(B2_DM(d.pdf, B2_DS(1.0, w)), opw);
+      d.d2pdf = inf_w2 ? 0.0 : B2_DD(B2_DM(d.pdf, B2_DA(B2_DS(w2, B2_DM(4.0, w)), 1.0)), B2_DM(opw, opw));
+    } else {
+      const double ew = b2_exp(-w);
+      d.pdf = inf_w ? 0.0 : B2_DM(w, ew);
+      d.cdf = B2_DS(1.0, ew);
+      d.dpdf = inf_w ? 0.0 : B2_DM(B2_DS(1.0, w), d.pdf);
+      d.d2pdf = inf_w2 ? 0.0 : B2_DM(B2_DA(B2_DS(w2, B2_DM(3.0, w)), 1.0), d.pdf);
+    }
+  }
+  return d;
+}
+
+template <int kDist>
+__device__ __forceinline__ double aft_limit_grad(bool z_sign, double sigma) {
+  if (kDist == kAftNormal) return z_sign ? -15.0 : 15.0;
+  if (kDist == kAftLogistic) return z_sign ? B2_DD(-1.0, sigma) : B2_DD(1.0, sigma);
+  return z_sign ? -15.0 : B2_DD(1.0, sigma);
+}
+template <int kDist>
+__device__ __forceinline__ double aft_limit_hess(bool z_sign, double sigma) {
+  if (kDist == kAftNormal) return B2_DD(1.0, B2_DM(sigma, sigma));
+  if (kDist == kAftLogistic) return 1e-16;
+  return z_sign ? 15.0 : 1e-16;
+}
+
+// the pieces of one row that the loss and the gradient share
+struct AftRow {
+  bool unc, z_sign;
+  double f, fp, fpp;       // uncensored: density, f', f'' at z
+  double dF, df, dg;       // censored: F_u - F_l, f_u - f_l, f'_u - f'_l
+};
+template <int kDist>
+__device__ __forceinline__ AftRow aft_row(double m, float lower, float upper, double sigma) {
+  AftRow r;
+  r.unc = lower == upper;
+  if (r.unc) {
+    const double z = B2_DD(B2_DS(b2_log((double)lower), m), sigma);
+    const AftDensity d = aft_density<kDist>(z);
+    r.z_sign = z > 0.0; r.f = d.pdf; r.fp = d.dpdf; r.fpp = d.d2pdf;
+    r.dF = r.df = r.dg = 0.0;
+  } else {
+    double z_u = 0.0, z_l = 0.0, f_u = 0.0, F_u = 1.0, g_u = 0.0, f_l = 0.0, F_l = 0.0, g_l = 0.0;
+    if (!isinf(upper)) {
+      z_u = B2_DD(B2_DS(b2_log((double)upper), m), sigma);
+      const AftDensity d = aft_density<kDist>(z_u);
+      f_u = d.pdf; F_u = d.cdf; g_u = d.dpdf;
+    }
+    if (lower > 0.0f) {
+      z_l = B2_DD(B2_DS(b2_log((double)lower), m), sigma);
+      const AftDensity d = aft_density<kDist>(z_l);
+      f_l = d.pdf; F_l = d.cdf; g_l = d.dpdf;
+    }
+    r.z_sign = z_u > 0.0 || z_l > 0.0;
+    r.dF = B2_DS(F_u, F_l); r.df = B2_DS(f_u, f_l); r.dg = B2_DS(g_u, g_l);
+    r.f = r.fp = r.fpp = 0.0;
+  }
+  return r;
+}
+
+template <int kDist>
+__device__ __forceinline__ double aft_loss(double m, float lower, float upper, double sigma) {
+  const AftRow r = aft_row<kDist>(m, lower, upper, sigma);
+  if (r.unc) return -b2_log(fmax(B2_DD(r.f, B2_DM(sigma, (double)lower)), kAftEps));
+  return -b2_log(fmax(r.dF, kAftEps));
+}
+
+// gradient pairs of survival:aft, one instantiation per distribution; weight applied in binary64, rounded once.  A row
+// whose pair is not finite (a NaN margin) is written as (0, 0) and raises *err, like gradient_param_kernel.
+template <int kDist>
+__global__ void __launch_bounds__(256)
+gradient_aft_kernel(const float* __restrict__ margin, const float* __restrict__ lower, const float* __restrict__ upper,
+                    const float* __restrict__ weight, int64_t n, double sigma, float2* __restrict__ gh,
+                    uint32_t* __restrict__ absmax, uint32_t* __restrict__ err) {
+  float mg = 0.0f, mh = 0.0f;
+  bool bad = false;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const AftRow r = aft_row<kDist>((double)margin[i], lower[i], upper[i], sigma);
+    double g_num, g_den, h_num, h_den;
+    if (r.unc) {
+      g_num = r.fp; g_den = B2_DM(sigma, r.f);
+      h_num = -B2_DS(B2_DM(r.f, r.fpp), B2_DM(r.fp, r.fp)); h_den = B2_DM(B2_DM(sigma, sigma), B2_DM(r.f, r.f));
+    } else {
+      const double sd = B2_DM(sigma, r.dF);
+      g_num = r.df; g_den = sd;
+      h_num = -B2_DS(B2_DM(r.dF, r.dg), B2_DM(r.df, r.df)); h_den = B2_DM(sd, sd);
+    }
+    double g = B2_DD(g_num, g_den), h = B2_DD(h_num, h_den);
+    if (g_den < kAftEps && !isfinite(g)) g = aft_limit_grad<kDist>(r.z_sign, sigma);
+    if (h_den < kAftEps && !isfinite(h)) h = aft_limit_hess<kDist>(r.z_sign, sigma);
+    g = g < -15.0 ? -15.0 : (g > 15.0 ? 15.0 : g);
+    h = h < 1e-16 ? 1e-16 : (h > 15.0 ? 15.0 : h);
+    const double w = weight ? (double)weight[i] : 1.0;
+    float2 v = make_float2(__double2float_rn(B2_DM(g, w)), __double2float_rn(B2_DM(h, w)));
+    if (!(fabsf(v.x) <= FLT_MAX && fabsf(v.y) <= FLT_MAX)) { bad = true; v = make_float2(0.0f, 0.0f); }
+    gh[i] = v;
+    mg = fmaxf(mg, fabsf(v.x)); mh = fmaxf(mh, fabsf(v.y));
+  }
+  if (bad && err) atomicOr(err, 1u);
+  if (absmax) absmax_publish(mg, mh, absmax);
+}
+
+// label bounds of survival:aft (once per train matrix): bad[0] a NaN bound, bad[1] lower < 0 or not finite,
+// bad[2] upper < lower, bad[3] an uncensored row with y <= 0 (max-reduced over the workers, so one word per rule)
+__global__ void aft_bounds_check_kernel(const float* __restrict__ lower, const float* __restrict__ upper, int64_t n,
+                                        uint32_t* __restrict__ bad) {
+  bool b0 = false, b1 = false, b2 = false, b3 = false;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float lo = lower[i], up = upper[i];
+    b0 |= lo != lo || up != up;
+    b1 |= !(lo >= 0.0f) || isinf(lo);
+    b2 |= up < lo;
+    b3 |= lo == up && lo <= 0.0f;
+  }
+  if (__any_sync(0xffffffffu, b0) && (threadIdx.x & 31) == 0) atomicOr(&bad[0], 1u);
+  if (__any_sync(0xffffffffu, b1) && (threadIdx.x & 31) == 0) atomicOr(&bad[1], 1u);
+  if (__any_sync(0xffffffffu, b2) && (threadIdx.x & 31) == 0) atomicOr(&bad[2], 1u);
+  if (__any_sync(0xffffffffu, b3) && (threadIdx.x & 31) == 0) atomicOr(&bad[3], 1u);
+}
+
+// aft-nloglik (metric 14) and interval-regression-accuracy (metric 15): (sum w v, sum w) in double
+template <int kDist>
+__device__ __forceinline__ double aft_metric_value(int metric, float m, float lower, float upper, double sigma) {
+  if (metric == 14) return aft_loss<kDist>((double)m, lower, upper, sigma);
+  const double p = b2_exp((double)m);
+  return ((double)lower <= p && p <= (double)upper) ? 1.0 : 0.0;
+}
+__global__ void aft_metric_kernel(int dist, int metric, double sigma, const float* __restrict__ margin,
+                                  const float* __restrict__ lower, const float* __restrict__ upper,
+                                  const float* __restrict__ weight, int64_t n, double* __restrict__ out) {
+  double s = 0.0, ws = 0.0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const double w = weight ? (double)weight[i] : 1.0;
+    const double v = dist == kAftNormal ? aft_metric_value<kAftNormal>(metric, margin[i], lower[i], upper[i], sigma)
+                   : dist == kAftLogistic ? aft_metric_value<kAftLogistic>(metric, margin[i], lower[i], upper[i], sigma)
+                   : aft_metric_value<kAftExtreme>(metric, margin[i], lower[i], upper[i], sigma);
+    s += v * w; ws += w;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ws += __shfl_xor_sync(0xffffffffu, ws, o); }
+  if ((threadIdx.x & 31) == 0) { atomicAdd(&out[0], s); atomicAdd(&out[1], ws); }
 }
 
 __global__ void gradient_softprob_kernel(int K, const float* __restrict__ margin, const float* __restrict__ label,
@@ -457,6 +767,31 @@ int b2_launch_gradient(int objective, int K, const float* margin, const float* l
 #undef B2_PARAM_OBJ
     default: return (int)cudaErrorInvalidValue;
   }
+  return (int)cudaGetLastError();
+}
+int b2_launch_gradient_aft(int dist, double sigma, const float* margin, const float* lower, const float* upper,
+                           const float* weight, int64_t n, float2* gh, uint32_t* absmax, uint32_t* err, int num_sms,
+                           cudaStream_t s) {
+  if (n <= 0) return 0;
+  const int g = grid_for(n, num_sms);
+  switch (dist) {
+#define B2_AFT(d) \
+    case d: b2::gradient_aft_kernel<d><<<g, 256, 0, s>>>(margin, lower, upper, weight, n, sigma, gh, absmax, err); break;
+    B2_AFT(b2::kAftNormal) B2_AFT(b2::kAftLogistic) B2_AFT(b2::kAftExtreme)
+#undef B2_AFT
+    default: return (int)cudaErrorInvalidValue;
+  }
+  return (int)cudaGetLastError();
+}
+int b2_launch_aft_bounds_check(const float* lower, const float* upper, int64_t n, uint32_t* bad, int num_sms, cudaStream_t s) {
+  if (n <= 0) return 0;
+  b2::aft_bounds_check_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(lower, upper, n, bad);
+  return (int)cudaGetLastError();
+}
+int b2_launch_aft_metric(int dist, int metric, double sigma, const float* margin, const float* lower, const float* upper,
+                         const float* weight, int64_t n, double* out, int num_sms, cudaStream_t s) {
+  if (n <= 0) return 0;
+  b2::aft_metric_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(dist, metric, sigma, margin, lower, upper, weight, n, out);
   return (int)cudaGetLastError();
 }
 int b2_launch_label_check(int objective, const float* label, int64_t n, uint32_t* bad, int num_sms, cudaStream_t s) {

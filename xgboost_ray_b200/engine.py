@@ -69,6 +69,7 @@ ABI = {
     "B2_BoosterCreate": (C.c_int, [C.c_char_p, _H, _H, C.POINTER(_H)]),
     "B2_BoosterUpdateOneIter": (C.c_int, [_H, C.c_int32]),
     "B2_BoosterBoostOneIter": (C.c_int, [_H, _FP, _FP, C.c_int64]),
+    "B2_BoosterGetGradients": (C.c_int, [_H, _FP, _FP, C.c_int64]),
     "B2_BoosterEvalSet": (C.c_int, [_H, _H, C.c_char_p, _DP]),
     "B2_BoosterPredict": (C.c_int, [_H, _H, C.c_int32, C.c_int32, C.c_int32, _FP, C.c_int64]),
     "B2_BoosterPredictContribs": (C.c_int, [_H, _H, C.c_int32, C.c_int32, C.c_int32, _FP, C.c_int64]),
@@ -224,7 +225,7 @@ class DMatrix:
 
     def __init__(self, data, label=None, weight=None, base_margin=None, missing=None, feature_names=None,
                  feature_types=None, nthread=None, enable_categorical=False, max_bin=None, ref=None,
-                 device=None, **kwargs):
+                 device=None, label_lower_bound=None, label_upper_bound=None, **kwargs):
         if hasattr(data, "values") and not isinstance(data, np.ndarray):  # pandas
             if feature_names is None and hasattr(data, "columns"):
                 feature_names = [str(c) for c in data.columns]
@@ -317,13 +318,16 @@ class DMatrix:
                 if not enable_categorical:
                     raise XGBoostError("feature_types marks categorical features: pass enable_categorical=True")
                 _check(lib().B2_MatrixSetFeatureTypes(self.handle, _bp(is_cat), f))
-        self.set_info(label=label, weight=weight, base_margin=base_margin)
+        self.set_info(label=label, weight=weight, base_margin=base_margin, label_lower_bound=label_lower_bound,
+                      label_upper_bound=label_upper_bound)
 
     # -- info
     def set_info(self, label=None, weight=None, base_margin=None, feature_weights=None,
                  label_lower_bound=None, label_upper_bound=None, **kw):
+        # the survival bounds are stored for every objective and read by survival:aft only, as in xgboost
         for field, v in (("label", label), ("weight", weight), ("base_margin", base_margin),
-                         ("feature_weights", feature_weights)):
+                         ("feature_weights", feature_weights), ("label_lower_bound", label_lower_bound),
+                         ("label_upper_bound", label_upper_bound)):
             if v is None:
                 continue
             if hasattr(v, "values") and not isinstance(v, np.ndarray):
@@ -507,6 +511,8 @@ _OBJECTIVES = {
     "count:poisson": _Objective("poisson-nloglik", "exp", "poisson_regression_param", {"max_delta_step": 0.7}),
     "reg:gamma": _Objective("gamma-nloglik", "exp"),
     "reg:tweedie": _Objective("tweedie-nloglik", "exp", "tweedie_regression_param", {"tweedie_variance_power": 1.5}),
+    "survival:aft": _Objective("aft-nloglik", "exp", "aft_loss_param",
+                               {"aft_loss_distribution": "normal", "aft_loss_distribution_scale": 1}),
     "multi:softprob": _Objective("mlogloss", "softmax", *_SOFTMAX),
     "multi:softmax": _Objective("mlogloss", "softmax", *_SOFTMAX),
 }
@@ -525,7 +531,8 @@ _ENGINE_KEYS = ("objective", "num_class", "max_depth", "eta", "learning_rate", "
                 "min_child_weight", "lambda", "reg_lambda", "alpha", "reg_alpha", "base_score", "hist_qbits",
                 "hist_chunk_rows", "profile", "max_cat_to_onehot", "max_cat_threshold", "scale_pos_weight",
                 "max_delta_step", "subsample", "colsample_bytree", "colsample_bylevel", "colsample_bynode", "seed",
-                "random_state", "num_parallel_tree", "huber_slope", "tweedie_variance_power")
+                "random_state", "num_parallel_tree", "huber_slope", "tweedie_variance_power", "aft_loss_distribution",
+                "aft_loss_distribution_scale")
 
 # xgboost parameters that change the trained model and that this engine does not implement: a value different
 # from the neutral one is an error, never silently ignored (a drop-in must not train a different model quietly)
@@ -907,7 +914,8 @@ class Booster:
         spec = _OBJECTIVES.get(obj, _OBJECTIVES["reg:squarederror"])
         obj_block = {"name": obj}
         if spec.block:
-            obj_block[spec.block] = {k: str(K) if k == "num_class" else _num_str(self.params.get(k, d))
+            obj_block[spec.block] = {k: str(K) if k == "num_class" else
+                                     str(self.params.get(k, d)) if isinstance(d, str) else _num_str(self.params.get(k, d))
                                      for k, d in spec.block_params.items()}
         attrs = {k: str(v) for k, v in self._attrs.items() if not k.startswith("b2.")}
         attrs["b2.params"] = json.dumps({k: self.params[k] for k in sorted(self.params) if _json_ok(self.params[k]) and
@@ -963,7 +971,7 @@ class Booster:
         if spec is not None and spec.block not in (None, "reg_loss_param", "softmax_multiclass_param"):
             for k, v in L["objective"].get(spec.block, {}).items():
                 if k in spec.block_params:
-                    params[k] = float(v)
+                    params[k] = str(v) if isinstance(spec.block_params[k], str) else float(v)
         params["base_score"] = float(L["learner_model_param"]["base_score"])
         npt = int(L["gradient_booster"]["model"].get("gbtree_model_param", {}).get("num_parallel_tree", "1"))
         if npt > 1:
@@ -1239,7 +1247,7 @@ def train(params, dtrain, num_boost_round=10, evals=(), obj=None, feval=None, ma
                     print(msg, flush=True)
                 if early_stopping_rounds:
                     data, metric, v = _parse_eval_str(msg)[-1]
-                    mx = maximize if maximize is not None else metric in ("auc", "map", "ndcg")
+                    mx = maximize if maximize is not None else metric in ("auc", "map", "ndcg", "interval-regression-accuracy")
                     better = best_score is None or (v > best_score if mx else v < best_score)
                     if better:
                         best_score, best_iter, best_msg = v, epoch, msg
