@@ -10,7 +10,9 @@ timed rounds).  Labels are a fixed map of the C3 label y, with no new randomness
   float32(sigmoid(y/10))            for reg:logistic, binary:logistic, binary:logitraw;
   y itself                          for reg:squarederror;
   survival:aft reads bounds built from the positive map t by row index: row mod 4 = 0 -> [t, t], 1 -> [t, +inf),
-  2 -> [0, t], 3 -> [t, 2t].
+  2 -> [0, t], 3 -> [t, 2t];
+  rank:pairwise and rank:ndcg read the relevance digitize(y, quantiles of y at 20/40/60/80 %) in 0..4 and the query
+  groups qid = row // 100 (the C3 matrix has 100k groups of 100 rows; the oracle sub-problem 2,000).
 For every objective a 200k-row, 3-round sub-problem is also compared tree for tree with the CPU oracle grown from the
 gradients of tests/objective_reference.py (split feature / bin / default direction exact, leaf values within 1e-5).
 Prints one JSON line with one entry per objective.  Writes nothing to the tree.
@@ -27,6 +29,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
+RANK = ("rank:pairwise", "rank:ndcg")
 POSITIVE = ("count:poisson", "reg:gamma", "reg:tweedie", "reg:squaredlogerror", "reg:pseudohubererror", "survival:aft")
 UNIT = ("reg:logistic", "binary:logistic", "binary:logitraw")
 
@@ -38,6 +41,8 @@ def objective_labels(objective, y):
         return (np.logaddexp(0.0, t) + 1e-3).astype(np.float32)     # log1p(exp(t)) without overflow
     if objective in UNIT:
         return (1.0 / (1.0 + np.exp(-t))).astype(np.float32)
+    if objective in RANK:
+        return np.digitize(y, np.quantile(y, [0.2, 0.4, 0.6, 0.8])).astype(np.float32)
     return y
 
 
@@ -53,6 +58,8 @@ def make_matrix(E, objective, X, y):
     if objective == "survival:aft":
         lo, hi = aft_bounds(y)
         return E.DMatrix(X, label=y, label_lower_bound=lo, label_upper_bound=hi)
+    if objective in RANK:
+        return E.DMatrix(X, label=y, qid=np.arange(len(y)) // 100)
     return E.DMatrix(X, label=y)
 
 
@@ -64,6 +71,9 @@ def oracle_match(E, params, X, y):
     if params["objective"] == "survival:aft":
         from tests import survival_reference as S
         ob = S.train(O, params, X, *aft_bounds(y), 3)
+    elif params["objective"] in RANK:
+        from tests import ranking_reference as RR
+        ob = RR.train(O, params, X, y, np.arange(len(y)) // 100, 3)
     elif params["objective"] in R.OBJECTIVES:
         ob = R.train(O, params, X, y, 3)
     else:

@@ -77,6 +77,11 @@ int B2_MatrixCreateFromProcessInterleaved(int64_t pid, uint64_t remote_addr, int
  * "label_lower_bound" | "label_upper_bound" (len n_rows, 0 clears): the survival bounds of each row, read by
  * survival:aft only (lower == upper: exact time; upper = +inf: right-censored; lower = 0: left-censored) */
 int B2_MatrixSetFloatInfo(B2Handle m, const char* field, const float* values, int64_t len);
+/* query groups of a ranking matrix (xgb.DMatrix(qid=...) / set_group; the reference sorts rows by qid and ships qid per
+ * shard, xgboost_ray/matrix.py:70-100, 300-304, 483, 689 and main.py:371, 399, 431): group g is the next group_sizes[g]
+ * rows.  Every size is >= 1 and the sizes sum to the row count; the engine builds the int64 row offsets itself.
+ * n_groups = 0 clears the groups.  Read by rank:pairwise / rank:ndcg and the ndcg / map / pre metrics. */
+int B2_MatrixSetGroups(B2Handle m, const int32_t* group_sizes, int64_t n_groups);
 /* feature types: is_cat[f] != 0 marks feature f categorical (xgb.DMatrix(feature_types=[...'c'...],
  * enable_categorical=True), forwarded by _get_dmatrix, xgboost_ray/main.py:365-376 / matrix.py:159,193).  Must be
  * called before B2_MatrixQuantize.  A categorical value is its category code: an integer in [0, 255]
@@ -116,7 +121,8 @@ int B2_BoosterBoostOneIter(B2Handle b, const float* grad, const float* hess, int
 int B2_BoosterGetGradients(B2Handle b, float* grad, float* hess, int64_t len);
 /* metric value of `m` (the train matrix or a matrix with raw data) under the current model, reduced
  * over comm like xgboost's (sum, wsum) allreduce.  metric: rmse|logloss|error|mlogloss|merror|...|aft-nloglik|
- * interval-regression-accuracy (the last two need survival:aft and the label bounds of `m`) */
+ * interval-regression-accuracy (the last two need survival:aft and the label bounds of `m`) | ndcg[@k][-] |
+ * map[@k][-] | pre[@k][-] (need the query groups of `m`: per-group values, (sum, group count) reduced over comm) */
 int B2_BoosterEvalSet(B2Handle b, B2Handle m, const char* metric, double* out);
 /* out [n_rows*num_class].  tree_end == 0 means all trees.  training == margin cache of train set. */
 int B2_BoosterPredict(B2Handle b, B2Handle m, int32_t output_margin, int32_t tree_begin, int32_t tree_end,

@@ -26,6 +26,7 @@ SOURCES = {
     "objective_kernel.cu": ["--fmad=false"],   # bit-exact gradients vs the oracle
     "sketch.cu": ["--fmad=false"],
     "auc_kernel.cu": ["--fmad=false"],
+    "rank_kernel.cu": ["--fmad=false"],        # LambdaMART gradients and ranking metrics, bit-exact vs the reference
     "p2p_exchange.cu": [],                     # NVLink peer-memory histogram exchange
     "shap_kernel.cu": [],                      # TreeSHAP contributions / interactions, leaf indices
     "engine.cu": [],
@@ -41,7 +42,7 @@ def _stale(target, deps):
 
 def build(force=False, verbose=False):
     os.makedirs(OBJ_DIR, exist_ok=True)
-    headers = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "hist_common.cuh"), os.path.join(CSRC, "sampling.cuh"), os.path.join(CSRC, "p2p.cuh"), os.path.join(CSRC, "level_finalize.cuh"), os.path.join(CSRC, "decide.cuh"), os.path.join(HERE, "..", "include", "b2hist.h"), __file__]
+    headers = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "hist_common.cuh"), os.path.join(CSRC, "sampling.cuh"), os.path.join(CSRC, "p2p.cuh"), os.path.join(CSRC, "level_finalize.cuh"), os.path.join(CSRC, "decide.cuh"), os.path.join(CSRC, "objective_common.cuh"), os.path.join(HERE, "..", "include", "b2hist.h"), __file__]
     jobs = []
     objs = []
     for src, extra in SOURCES.items():

@@ -104,6 +104,19 @@ int b2_launch_shap_interactions(const float*, int64_t, int64_t, int, float, cons
                                 const uint32_t*, int, const double*, const float*, float, double*, float*, int, cudaStream_t);
 int b2_launch_leaf_index(const float*, int64_t, int64_t, int, float, const B2TreeNodeDev*, const int32_t*, const uint32_t*, int, int,
                          float*, int, cudaStream_t);
+int b2_rank_stage_rows();
+size_t b2_rank_order_temp_bytes(int64_t, int64_t);
+int b2_launch_rank_iota(int32_t*, int64_t, int, cudaStream_t);
+int b2_rank_order(const float*, int64_t, const int64_t*, int64_t, const int32_t*, uint32_t*, uint32_t*, int32_t*, void*, size_t,
+                  int, cudaStream_t);
+int b2_launch_rank_disc(double*, int64_t, int, cudaStream_t);
+int b2_launch_rank_inv_idcg(const int64_t*, int64_t, const uint32_t*, const double*, int, int, double*, int, cudaStream_t);
+int b2_launch_rank_label_check(const float*, int64_t, int, uint32_t*, int, cudaStream_t);
+int b2_launch_lambdarank_gradient(int, const int64_t*, int64_t, int64_t, const uint32_t*, const int32_t*, const float*,
+                                  const double*, const double*, int, int, float*, float*, double*, float2*, uint32_t*, uint32_t*,
+                                  int, cudaStream_t);
+int b2_launch_rank_metric(int, int, int, int, const int64_t*, int64_t, const int32_t*, const float*, const uint32_t*,
+                          const double*, double*, double*, int, cudaStream_t);
 size_t b2_auc_temp_bytes(int64_t);
 int b2_auc_binary(const float*, const float*, const float*, int64_t, void*, size_t, double*, int, cudaStream_t);
 int b2_launch_transform(int, int, float*, int64_t, int, cudaStream_t);
@@ -495,7 +508,14 @@ struct Matrix : HandleBase {
   DevBuf<float> lower, upper;          // survival label bounds (label_lower_bound / label_upper_bound), read by survival:aft
   int64_t n_lower = 0, n_upper = 0;
   bool has_bounds() const { return n_lower == n && n_upper == n; }
-  std::vector<uint32_t> fwq;          // feature_weights in Q16 (empty = all 1.0)
+  // query groups (B2_MatrixSetGroups): group g is rows [qgroup_ptr[g], qgroup_ptr[g+1]); read by the rank objectives and
+  // the ndcg / map / pre metrics.  rank_version changes with the groups and the labels (the 1/IDCG cache key)
+  std::vector<int64_t> h_qgroup_ptr;
+  DevBuf<int64_t> qgroup_ptr;
+  int64_t n_qgroups = 0, max_qgroup = 0;
+  uint64_t rank_version = 0;
+  bool has_qgroups() const { return n_qgroups > 0; }
+  std::vector<uint32_t> fwq;         // feature_weights in Q16 (empty = all 1.0)
   DevBuf<uint32_t> d_fwq;
 };
 
@@ -705,9 +725,11 @@ void bin_matrix(Matrix* m) {
 // ---------------------------------------------------------------- booster
 // objective ids, shared with objective_kernel.cu (the kernels take them as plain ints)
 enum { kObjSquaredError = 0, kObjLogistic = 1, kObjSoftprob = 2, kObjRegLogistic = 3, kObjLogitRaw = 4, kObjSquaredLog = 5,
-       kObjPseudoHuber = 6, kObjPoisson = 7, kObjGamma = 8, kObjTweedie = 9, kObjAft = 10 };
+       kObjPseudoHuber = 6, kObjPoisson = 7, kObjGamma = 8, kObjTweedie = 9, kObjAft = 10, kObjRankPairwise = 11,
+       kObjRankNdcg = 12 };
 bool obj_log_link(int o) { return o == kObjPoisson || o == kObjGamma || o == kObjTweedie || o == kObjAft; }
 bool obj_sigmoid(int o) { return o == kObjLogistic || o == kObjRegLogistic; }
+bool obj_rank(int o) { return o == kObjRankPairwise || o == kObjRankNdcg; }
 // objectives whose gradient kernel reports non-finite gradient pairs (gradient_param_kernel)
 bool obj_checks_finite(int o) { return o >= kObjSquaredLog; }
 struct Params {
@@ -729,6 +751,8 @@ struct Params {
   float tweedie_variance_power = 1.5f;         // reg:tweedie rho in [1, 2)
   int aft_dist = 0;                            // survival:aft distribution: 0 normal, 1 logistic, 2 extreme
   float aft_sigma = 1.0f;                      // survival:aft scale sigma > 0
+  int rank_k = 32;                             // lambdarank_num_pair_per_sample (topk pairs: the first k model positions)
+  bool ndcg_exp_gain = true;                   // ndcg gain 2^y - 1 (true) or y (rank:ndcg and the ndcg metrics)
   float subsample = 1.0f, colsample_bytree = 1.0f, colsample_bylevel = 1.0f, colsample_bynode = 1.0f;
   int seed = 0;
   bool base_score_set = false;   // false: estimated from the labels before the first tree (xgboost >= 2.0, A.3)
@@ -765,6 +789,26 @@ struct Timers {
 };
 
 struct EvalCache { DevBuf<float> margin; int n_trees_applied = 0; int64_t n = 0; uint64_t margin_version = 0; };
+
+// per-group descending order of a row vector (rank_kernel.cu b2_rank_order): keys_sorted / rows hold, for every model
+// position, the sort key (the value) and the row.  The buffers are pooled and kept, so a booster sorts its train margins
+// every round without allocating.
+struct RankOrder {
+  DevBuf<int32_t> iota, rows; DevBuf<uint32_t> keys, keys_sorted; DevBuf<uint8_t> temp;
+  int64_t n = -1, groups = -1; size_t temp_bytes = 0;
+  void run(Matrix* m, const float* v, int num_sms, cudaStream_t s) {
+    if (n != m->n || groups != m->n_qgroups) {
+      const size_t rows_cap = (size_t)std::max<int64_t>(m->n, 1);
+      iota.ensure(rows_cap); rows.ensure(rows_cap); keys.ensure(rows_cap); keys_sorted.ensure(rows_cap);
+      temp_bytes = b2_rank_order_temp_bytes(m->n, m->n_qgroups);
+      temp.ensure(std::max<size_t>(temp_bytes, 1));
+      LAUNCH_CHECK(b2_launch_rank_iota(iota.p, m->n, num_sms, s));
+      n = m->n; groups = m->n_qgroups;
+    }
+    LAUNCH_CHECK(b2_rank_order(v, m->n, m->qgroup_ptr.p, m->n_qgroups, iota.p, keys.p, keys_sorted.p, rows.p, temp.p,
+                               temp_bytes, num_sms, s));
+  }
+};
 
 struct Booster : HandleBase {
   Ctx* ctx = nullptr;
@@ -853,6 +897,13 @@ struct Booster : HandleBase {
   size_t staging_bytes = 0;
   DevBuf<float> d_custom_g, d_custom_h;
   std::map<uint64_t, EvalCache*> eval_cache;   // keyed by Matrix::uid
+  // learning to rank: the train margins' order (every round), the discount table ln2 / log(r + 2) (grown to the largest
+  // group seen), 1/IDCG of the train groups (keyed by matrix, its rank_version, k and the gain) and the stage of the
+  // groups larger than the gradient kernel's shared-memory stage
+  RankOrder rank_order;
+  DevBuf<double> rank_disc; int64_t rank_disc_len = 0;
+  DevBuf<double> rank_inv_idcg; uint64_t idcg_uid = 0, idcg_version = 0; int idcg_k = -1, idcg_gain = -1;
+  DevBuf<float> rank_scratch_m, rank_scratch_y; DevBuf<double> rank_scratch_p;
   // profiling
   Timers t;
   std::vector<cudaEvent_t> ev_pool; size_t ev_used = 0;
@@ -930,9 +981,11 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
       else if (v == "reg:gamma") p->objective = kObjGamma;
       else if (v == "reg:tweedie") p->objective = kObjTweedie;
       else if (v == "survival:aft") p->objective = kObjAft;
+      else if (v == "rank:pairwise") p->objective = kObjRankPairwise;
+      else if (v == "rank:ndcg") p->objective = kObjRankNdcg;
       else fail("unsupported objective '%s' (supported: reg:squarederror, reg:logistic, binary:logistic, binary:logitraw, "
                 "reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie, survival:aft, "
-                "multi:softprob, multi:softmax)", v.c_str());
+                "rank:pairwise, rank:ndcg, multi:softprob, multi:softmax)", v.c_str());
     } else if (k == "num_class") p->num_class = i();
     else if (k == "num_parallel_tree") p->num_parallel_tree = i();
     else if (k == "max_depth") p->max_depth = i();
@@ -963,11 +1016,32 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
       else fail("aft_loss_distribution must be normal, logistic or extreme, got '%s'", v.c_str());
     }
     else if (k == "aft_loss_distribution_scale") p->aft_sigma = f();
+    else if (k == "lambdarank_pair_method") {
+      if (v != "topk") fail("lambdarank_pair_method='%s' is not supported (supported: topk; random pair sampling "
+                            "(mean) is not implemented)", v.c_str());
+    }
+    else if (k == "lambdarank_num_pair_per_sample") {
+      char* end = nullptr;
+      const long long kv = strtoll(v.c_str(), &end, 10);
+      if (v.empty() || *end != '\0' || kv < 1 || kv > INT32_MAX)
+        fail("lambdarank_num_pair_per_sample must be an integer >= 1, got '%s'", v.c_str());
+      p->rank_k = (int)kv;
+    }
+    else if (k == "lambdarank_unbiased" || k == "ndcg_exp_gain") {
+      bool on;
+      if (v == "1" || v == "true" || v == "True") on = true;
+      else if (v == "0" || v == "false" || v == "False") on = false;
+      else fail("%s must be a boolean, got '%s'", k.c_str(), v.c_str());
+      if (k == "ndcg_exp_gain") p->ndcg_exp_gain = on;
+      else if (on) fail("lambdarank_unbiased=true is not supported (position-bias estimation is not implemented)");
+    }
     else if (k == "max_cat_to_onehot") p->max_cat_to_onehot = i();
     else if (k == "max_cat_threshold") p->max_cat_threshold = i();
     else if (k == "max_bin") { if (max_bin_out) *max_bin_out = i(); }
     // unknown keys (nthread, tree_method, verbosity, ...) are accepted and ignored, like xgboost
   }
+  if (obj_rank(p->objective) && p->num_class > 1)
+    fail("%s has one output per row: num_class must be 1, got %d", p->objective_name.c_str(), p->num_class);
   if (p->objective != kObjSoftprob) p->num_class = 1;
   if (p->objective == kObjSoftprob && p->num_class < 2) fail("multi:softprob needs num_class >= 2");
   if (p->max_depth < 1 || p->max_depth > 14) fail("max_depth must be in [1, 14], got %d", p->max_depth);
@@ -989,6 +1063,8 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     fail("aft_loss_distribution_scale must be finite and > 0, got %g", (double)p->aft_sigma);
   // survival:aft fits no intercept: base_score defaults to 0.5 (margin log 0.5) and is never estimated
   if (p->objective == kObjAft && !p->base_score_set) { p->base_score = 0.5f; p->base_score_set = true; }
+  // the rank objectives neither: their margin is the score itself (identity transform)
+  if (obj_rank(p->objective) && !p->base_score_set) { p->base_score = 0.5f; p->base_score_set = true; }
   if (p->base_score_set) {
     if (p->objective == kObjRegLogistic && !(p->base_score > 0.0f && p->base_score < 1.0f))
       fail("base_score must be in (0, 1) for reg:logistic, got %g", (double)p->base_score);
@@ -1788,10 +1864,68 @@ void check_bounds(Booster* b) {
   b->labels_checked = true;
 }
 
+// the rank objectives need query groups and labels that are finite, >= 0 and, with the exponential gain, <= 31
+void check_rank_labels(Booster* b) {
+  Matrix* m = b->train; cudaStream_t s = b->ctx->stream;
+  if (!m->has_qgroups())
+    fail("%s needs query groups on the train matrix: pass qid (or group) to the DMatrix", b->p.objective_name.c_str());
+  if (b->labels_checked) return;
+  if (m->n_label != m->n) fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)m->n);
+  DevBuf<uint32_t> bad; bad.ensure(2);
+  CUDA_CHECK(cudaMemsetAsync(bad.p, 0, 2 * sizeof(uint32_t), s));
+  LAUNCH_CHECK(b2_launch_rank_label_check(m->label.p, m->n, b->p.ndcg_exp_gain ? 1 : 0, bad.p, b->ctx->num_sms, s));
+  allreduce(b->comm, bad.p, 2, kNcclUint32, kNcclMax, s);
+  uint32_t h[2] = {0, 0};
+  CUDA_CHECK(cudaMemcpyAsync(h, bad.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  if (h[0]) fail("%s: labels must be finite and >= 0", b->p.objective_name.c_str());
+  if (h[1]) fail("%s: with ndcg_exp_gain the labels must be <= 31 (the gain is 2^label - 1); set ndcg_exp_gain=false "
+                 "for larger relevance degrees", b->p.objective_name.c_str());
+  b->labels_checked = true;
+}
+
+// discount table ln2 / log(r + 2) for model positions r < len
+void ensure_rank_disc(Booster* b, int64_t len) {
+  len = std::max<int64_t>(len, 1);
+  if (b->rank_disc_len >= len) return;
+  b->rank_disc.ensure((size_t)len);
+  LAUNCH_CHECK(b2_launch_rank_disc(b->rank_disc.p, len, b->ctx->num_sms, b->ctx->stream));
+  b->rank_disc_len = len;
+}
+
+// LambdaMART gradients of the train matrix (rank_kernel.cu): order the margins per group, then one pass over the groups
+void rank_gradient(Booster* b, uint32_t* absmax, uint32_t* err) {
+  Matrix* m = b->train; cudaStream_t s = b->ctx->stream; const Params& p = b->p; const int sms = b->ctx->num_sms;
+  ensure_rank_disc(b, m->max_qgroup);
+  const bool ndcg = p.objective == kObjRankNdcg;
+  if (ndcg && (b->idcg_uid != m->uid || b->idcg_version != m->rank_version || b->idcg_k != p.rank_k ||
+               b->idcg_gain != (int)p.ndcg_exp_gain)) {
+    // 1/IDCG depends on the labels, k and the gain only: computed once per (matrix, k, gain)
+    RankOrder lo;
+    lo.run(m, m->label.p, sms, s);
+    b->rank_inv_idcg.ensure((size_t)std::max<int64_t>(m->n_qgroups, 1));
+    LAUNCH_CHECK(b2_launch_rank_inv_idcg(m->qgroup_ptr.p, m->n_qgroups, lo.keys_sorted.p, b->rank_disc.p, p.rank_k,
+                                         p.ndcg_exp_gain ? 1 : 0, b->rank_inv_idcg.p, sms, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));   // lo's buffers go back to the pool
+    b->idcg_uid = m->uid; b->idcg_version = m->rank_version; b->idcg_k = p.rank_k; b->idcg_gain = (int)p.ndcg_exp_gain;
+  }
+  b->rank_order.run(m, b->margin.p, sms, s);
+  if (m->max_qgroup > b2_rank_stage_rows()) {
+    const size_t rows = (size_t)std::max<int64_t>(m->n, 1);
+    b->rank_scratch_m.ensure(rows); b->rank_scratch_y.ensure(rows); b->rank_scratch_p.ensure(rows);
+  }
+  LAUNCH_CHECK(b2_launch_lambdarank_gradient(ndcg ? 1 : 0, m->qgroup_ptr.p, m->n_qgroups, m->max_qgroup,
+                                             b->rank_order.keys_sorted.p, b->rank_order.rows.p, m->label.p,
+                                             ndcg ? b->rank_inv_idcg.p : nullptr, b->rank_disc.p, p.rank_k,
+                                             p.ndcg_exp_gain ? 1 : 0, b->rank_scratch_m.p, b->rank_scratch_y.p,
+                                             b->rank_scratch_p.p, b->gh.p, absmax, err, sms, s));
+}
+
 // labels outside the objective's domain fail training (xgboost's CheckLabel); once per train matrix, before the first tree
 void check_labels(Booster* b) {
   Matrix* m = b->train; const int o = b->p.objective; cudaStream_t s = b->ctx->stream;
   if (o == kObjAft) { check_bounds(b); return; }
+  if (obj_rank(o)) { check_rank_labels(b); return; }
   if (o == kObjSquaredError || o == kObjLogistic || o == kObjSoftprob || o == kObjPseudoHuber || b->labels_checked) return;
   if (m->n_label != m->n) fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)m->n);
   DevBuf<uint32_t> bad; bad.ensure(1);
@@ -1859,6 +1993,8 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
       LAUNCH_CHECK(b2_launch_gradient_aft(b->p.aft_dist, (double)b->p.aft_sigma, b->margin.p, m->lower.p, m->upper.p,
                                           m->n_weight ? m->weight.p : nullptr, n, b->gh.p,
                                           b->absmax_fused ? b->d_absmax.p : nullptr, b->d_grad_err.p, b->ctx->num_sms, s));
+    else if (obj_rank(b->p.objective))
+      rank_gradient(b, b->absmax_fused ? b->d_absmax.p : nullptr, b->d_grad_err.p);
     else
       LAUNCH_CHECK(b2_launch_gradient(b->p.objective, K, b->margin.p, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
                                       b->p.scale_pos_weight, objective_param(b->p), b->gh.p,
@@ -1914,9 +2050,9 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
 }
 
 // metric id of an eval_metric name; *param receives the metric's parameter (rho of tweedie-nloglik@rho, huber_slope for mphe)
-int metric_id(const char* name, const Params& p, float* param) {
+int metric_id(const char* name, const Params& p, float* param, int* minus) {
   std::string s(name ? name : "");
-  *param = 0.0f;
+  *param = 0.0f; *minus = 0;
   if (s == "rmsle") return 7;
   if (s == "mape") return 8;
   if (s == "mphe") { *param = p.huber_slope; return 9; }
@@ -1944,9 +2080,24 @@ int metric_id(const char* name, const Params& p, float* param) {
   if (s == "auc") return 6;
   if (s == "aft-nloglik") return 14;
   if (s == "interval-regression-accuracy") return 15;
+  // ranking metrics: ndcg[@k][-] (16), map[@k][-] (17), pre[@k][-] (18).  *param = k (0: the whole group), *minus = the
+  // trailing '-' (a group without relevant rows scores 0 instead of 1)
+  for (int id = 16; id <= 18; ++id) {
+    const std::string base = id == 16 ? "ndcg" : id == 17 ? "map" : "pre";
+    if (s.compare(0, base.size(), base) != 0) continue;
+    std::string rest = s.substr(base.size());
+    if (!rest.empty() && rest.back() == '-') { *minus = 1; rest.pop_back(); }
+    if (rest.empty()) return id;
+    char* end = nullptr;
+    const long long k = rest[0] == '@' && rest.size() > 1 ? strtoll(rest.c_str() + 1, &end, 10) : -1;
+    if (rest[0] != '@' || rest.size() < 2 || *end != '\0' || k < 1 || k > (1 << 24))
+      fail("eval metric '%s': the cut-off must be given as %s@k with an integer k >= 1", s.c_str(), base.c_str());
+    *param = (float)k;
+    return id;
+  }
   fail("unsupported eval metric '%s' (supported: rmse, mae, logloss, error, auc, mlogloss, merror, rmsle, mape, mphe, "
-       "poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy)",
-       s.c_str());
+       "poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy, "
+       "ndcg[@k][-], map[@k][-], pre[@k][-])", s.c_str());
 }
 
 // margin of matrix m under the current model (cached per matrix, only new trees are applied)
@@ -2258,7 +2409,7 @@ int B2_MatrixSetFloatInfo(B2Handle mh, const char* field, const float* values, i
   CUDA_CHECK(cudaSetDevice(m->ctx->device));
   std::string f(field ? field : "");
   DevBuf<float>* dst = nullptr; int64_t* cnt = nullptr;
-  if (f == "label") { dst = &m->label; cnt = &m->n_label; if (len != m->n) fail("label length %lld != rows %lld", (long long)len, (long long)m->n); }
+  if (f == "label") { dst = &m->label; cnt = &m->n_label; m->rank_version++; if (len != m->n) fail("label length %lld != rows %lld", (long long)len, (long long)m->n); }
   else if (f == "weight") { dst = &m->weight; cnt = &m->n_weight; if (len != m->n && len != 0) fail("weight length %lld != rows %lld", (long long)len, (long long)m->n); }
   else if (f == "label_lower_bound" || f == "label_upper_bound") {
     const bool lo = f == "label_lower_bound";
@@ -2285,6 +2436,28 @@ int B2_MatrixSetFloatInfo(B2Handle mh, const char* field, const float* values, i
   if (len > 0) CUDA_CHECK(cudaMemcpyAsync(dst->p, values, len * sizeof(float), cudaMemcpyHostToDevice, m->ctx->stream));
   CUDA_CHECK(cudaStreamSynchronize(m->ctx->stream));
   *cnt = len;
+  API_END
+}
+int B2_MatrixSetGroups(B2Handle mh, const int32_t* group_sizes, int64_t n_groups) {
+  API_BEGIN
+  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
+  CUDA_CHECK(cudaSetDevice(m->ctx->device));
+  if (n_groups < 0) fail("query groups: negative group count %lld", (long long)n_groups);
+  std::vector<int64_t> ptr((size_t)n_groups + 1, 0);
+  int64_t mx = 0;
+  for (int64_t g = 0; g < n_groups; ++g) {
+    if (group_sizes[g] < 1) fail("query group %lld has %d rows: every group needs at least one", (long long)g, group_sizes[g]);
+    ptr[g + 1] = ptr[g] + group_sizes[g];
+    mx = std::max<int64_t>(mx, group_sizes[g]);
+  }
+  if (n_groups > 0 && ptr[n_groups] != m->n)
+    fail("query groups cover %lld rows, the matrix has %lld", (long long)ptr[n_groups], (long long)m->n);
+  m->qgroup_ptr.ensure(ptr.size());
+  CUDA_CHECK(cudaMemcpyAsync(m->qgroup_ptr.p, ptr.data(), ptr.size() * sizeof(int64_t), cudaMemcpyHostToDevice, m->ctx->stream));
+  CUDA_CHECK(cudaStreamSynchronize(m->ctx->stream));
+  m->h_qgroup_ptr = std::move(ptr);
+  m->n_qgroups = n_groups; m->max_qgroup = mx;
+  m->rank_version++;
   API_END
 }
 int B2_MatrixSetFeatureTypes(B2Handle mh, const uint8_t* is_cat, int32_t len) {
@@ -2445,8 +2618,37 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
   cudaStream_t s = b->ctx->stream;
   float mparam = 0.0f;
-  const int mid = metric_id(metric, b->p, &mparam);
+  int minus = 0;
+  const int mid = metric_id(metric, b->p, &mparam, &minus);
   const bool aft_metric = mid == 14 || mid == 15;
+  if (mid >= 16 && mid <= 18) {
+    // ndcg / map / pre: per query group on the prediction order (rank_kernel.cu), averaged over the groups of all workers
+    if (b->p.num_class > 1) fail("metric '%s' needs a single-output objective", metric);
+    if (!m->has_qgroups()) fail("metric '%s' needs query groups (qid) on the evaluation matrix", metric);
+    if (m->n_label != m->n) fail("evaluation matrix has no labels");
+    float* margin = eval_margin(b, m);
+    DevBuf<float> pred; DevBuf<double> vals; RankOrder po, lo;
+    pred.ensure((size_t)std::max<int64_t>(m->n, 1));
+    if (m->n > 0) CUDA_CHECK(cudaMemcpyAsync(pred.p, margin, (size_t)m->n * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    LAUNCH_CHECK(b2_launch_transform(b->p.objective, 1, pred.p, m->n, b->ctx->num_sms, s));
+    po.run(m, pred.p, b->ctx->num_sms, s);
+    if (mid == 16) lo.run(m, m->label.p, b->ctx->num_sms, s);
+    ensure_rank_disc(b, m->max_qgroup);
+    vals.ensure((size_t)std::max<int64_t>(m->n_qgroups, 1));
+    b->d_metric.ensure(2);
+    LAUNCH_CHECK(b2_launch_rank_metric(mid, (int)mparam, minus, b->p.ndcg_exp_gain ? 1 : 0, m->qgroup_ptr.p, m->n_qgroups,
+                                       po.rows.p, m->label.p, mid == 16 ? lo.keys_sorted.p : nullptr, b->rank_disc.p, vals.p,
+                                       b->d_metric.p, b->ctx->num_sms, s));
+    allreduce(b->comm, b->d_metric.p, 2, kNcclFloat64, kNcclSum, s);
+    double h[2];
+    CUDA_CHECK(cudaMemcpyAsync(h, b->d_metric.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    *out = h[1] > 0 ? h[0] / h[1] : 0.0;
+    return 0;
+  }
+  // xgboost computes a per-group ranking AUC on a matrix with groups; this engine's auc is the binary one only
+  if (mid == 6 && m->has_qgroups())
+    fail("metric 'auc' on a matrix with query groups (per-group ranking AUC) is not supported; use ndcg or map");
   if (aft_metric && b->p.objective != kObjAft)
     fail("metric '%s' does not fit objective '%s'", metric, b->p.objective_name.c_str());
   if (aft_metric && !m->has_bounds()) fail("metric '%s' needs label_lower_bound and label_upper_bound on the evaluation matrix", metric);

@@ -55,6 +55,7 @@ ABI = {
                                              C.POINTER(_H)]),
     "B2_MatrixSetRows": (C.c_int, [_H, C.c_int64, _FP, C.c_int64]),
     "B2_MatrixSetFloatInfo": (C.c_int, [_H, C.c_char_p, _FP, C.c_int64]),
+    "B2_MatrixSetGroups": (C.c_int, [_H, _IP, C.c_int64]),
     "B2_MatrixSetFeatureTypes": (C.c_int, [_H, _BP, C.c_int32]),
     "B2_MatrixGetFeatureTypes": (C.c_int, [_H, _BP]),
     "B2_MatrixNumRow": (C.c_int, [_H, C.POINTER(C.c_int64)]),
@@ -225,7 +226,7 @@ class DMatrix:
 
     def __init__(self, data, label=None, weight=None, base_margin=None, missing=None, feature_names=None,
                  feature_types=None, nthread=None, enable_categorical=False, max_bin=None, ref=None,
-                 device=None, label_lower_bound=None, label_upper_bound=None, **kwargs):
+                 device=None, label_lower_bound=None, label_upper_bound=None, qid=None, group=None, **kwargs):
         if hasattr(data, "values") and not isinstance(data, np.ndarray):  # pandas
             if feature_names is None and hasattr(data, "columns"):
                 feature_names = [str(c) for c in data.columns]
@@ -282,6 +283,7 @@ class DMatrix:
         self._label = None
         self._weight = None
         self._base_margin = None
+        self._group_sizes = None
         h = _H(0)
         n, f = self._host.shape
         self.ingest = "host"
@@ -319,11 +321,15 @@ class DMatrix:
                     raise XGBoostError("feature_types marks categorical features: pass enable_categorical=True")
                 _check(lib().B2_MatrixSetFeatureTypes(self.handle, _bp(is_cat), f))
         self.set_info(label=label, weight=weight, base_margin=base_margin, label_lower_bound=label_lower_bound,
-                      label_upper_bound=label_upper_bound)
+                      label_upper_bound=label_upper_bound, qid=qid, group=group)
 
     # -- info
     def set_info(self, label=None, weight=None, base_margin=None, feature_weights=None,
-                 label_lower_bound=None, label_upper_bound=None, **kw):
+                 label_lower_bound=None, label_upper_bound=None, qid=None, group=None, **kw):
+        if qid is not None or group is not None:
+            self._set_groups(qid, group, weighted=weight is not None or self._weight is not None)
+        elif weight is not None and self._group_sizes is not None:
+            raise XGBoostError("sample weights on a matrix with query groups (per-group weights) are not supported")
         # the survival bounds are stored for every objective and read by survival:aft only, as in xgboost
         for field, v in (("label", label), ("weight", weight), ("base_margin", base_margin),
                          ("feature_weights", feature_weights), ("label_lower_bound", label_lower_bound),
@@ -335,6 +341,38 @@ class DMatrix:
             a = _f32c(np.asarray(v).reshape(-1))
             _check(lib().B2_MatrixSetFloatInfo(self.handle, field.encode(), _fp(a), a.size))
             setattr(self, "_" + field, a)
+
+    def _set_groups(self, qid, group, weighted):
+        """Query groups from `qid` (one id per row, non-decreasing: a group is a run of equal ids) or from `group`
+        (the sizes of consecutive groups), as xgboost's DMatrix takes them."""
+        if qid is not None and group is not None:
+            raise XGBoostError("pass either qid or group, not both")
+        if weighted:
+            raise XGBoostError("sample weights on a matrix with query groups (per-group weights) are not supported")
+        n = self.num_row()
+        if qid is not None:
+            q = np.asarray(qid.values if hasattr(qid, "values") and not isinstance(qid, np.ndarray) else qid).reshape(-1)
+            if q.size != n:
+                raise XGBoostError("qid has %d values for %d rows" % (q.size, n))
+            if q.size and np.any(q[1:] < q[:-1]):
+                raise XGBoostError("qid must be sorted in non-decreasing order (sort the rows by qid first)")
+            starts = np.flatnonzero(np.r_[True, q[1:] != q[:-1]]) if q.size else np.zeros(0, np.int64)
+            sizes = np.diff(np.r_[starts, q.size])
+        else:
+            sizes = np.asarray(group, np.int64).reshape(-1)
+            if np.any(sizes < 1) or int(sizes.sum()) != n:
+                raise XGBoostError("group sizes must be >= 1 and sum to the row count %d" % n)
+        if sizes.size and sizes.max() > np.iinfo(np.int32).max:
+            raise XGBoostError("a query group has more than 2^31 - 1 rows")
+        sizes = np.ascontiguousarray(sizes, np.int32)
+        _check(lib().B2_MatrixSetGroups(self.handle, _ip(sizes), sizes.size))
+        self._group_sizes = sizes
+
+    def get_group(self):
+        return self._group_sizes.copy() if self._group_sizes is not None else np.zeros(0, np.int32)
+
+    def set_group(self, group):
+        self.set_info(group=group)
 
     def set_label(self, label):
         self.set_info(label=label)
@@ -495,11 +533,16 @@ class _Objective:
     def default_metric(self, params):
         if self.metric == "tweedie-nloglik":   # the metric carries the objective's variance power in its name
             return "tweedie-nloglik@%g" % float(params.get("tweedie_variance_power", 1.5))
+        if self.metric == "ndcg":              # ranking: ndcg at the objective's pair cut-off
+            return "ndcg@%d" % int(params.get("lambdarank_num_pair_per_sample", 32))
         return self.metric
 
 
 _REG_LOSS = ("reg_loss_param", {"scale_pos_weight": 1})
 _SOFTMAX = ("softmax_multiclass_param", {"num_class": None})
+# xgboost 2.x writes every lambdarank parameter as a string; lambdarank_bias_norm only matters with lambdarank_unbiased
+_LAMBDARANK = ("lambdarank_param", {"lambdarank_pair_method": "topk", "lambdarank_num_pair_per_sample": "32",
+                                    "lambdarank_unbiased": "0", "lambdarank_bias_norm": "2", "ndcg_exp_gain": "1"})
 _OBJECTIVES = {
     "reg:squarederror": _Objective("rmse", None, *_REG_LOSS),
     "reg:linear": _Objective("rmse", None, *_REG_LOSS),
@@ -513,6 +556,8 @@ _OBJECTIVES = {
     "reg:tweedie": _Objective("tweedie-nloglik", "exp", "tweedie_regression_param", {"tweedie_variance_power": 1.5}),
     "survival:aft": _Objective("aft-nloglik", "exp", "aft_loss_param",
                                {"aft_loss_distribution": "normal", "aft_loss_distribution_scale": 1}),
+    "rank:pairwise": _Objective("ndcg", None, *_LAMBDARANK),
+    "rank:ndcg": _Objective("ndcg", None, *_LAMBDARANK),
     "multi:softprob": _Objective("mlogloss", "softmax", *_SOFTMAX),
     "multi:softmax": _Objective("mlogloss", "softmax", *_SOFTMAX),
 }
@@ -532,7 +577,8 @@ _ENGINE_KEYS = ("objective", "num_class", "max_depth", "eta", "learning_rate", "
                 "hist_chunk_rows", "profile", "max_cat_to_onehot", "max_cat_threshold", "scale_pos_weight",
                 "max_delta_step", "subsample", "colsample_bytree", "colsample_bylevel", "colsample_bynode", "seed",
                 "random_state", "num_parallel_tree", "huber_slope", "tweedie_variance_power", "aft_loss_distribution",
-                "aft_loss_distribution_scale")
+                "aft_loss_distribution_scale", "lambdarank_pair_method", "lambdarank_num_pair_per_sample",
+                "lambdarank_unbiased", "ndcg_exp_gain")
 
 # xgboost parameters that change the trained model and that this engine does not implement: a value different
 # from the neutral one is an error, never silently ignored (a drop-in must not train a different model quietly)
@@ -915,7 +961,7 @@ class Booster:
         obj_block = {"name": obj}
         if spec.block:
             obj_block[spec.block] = {k: str(K) if k == "num_class" else
-                                     str(self.params.get(k, d)) if isinstance(d, str) else _num_str(self.params.get(k, d))
+                                     _str_param(self.params.get(k, d)) if isinstance(d, str) else _num_str(self.params.get(k, d))
                                      for k, d in spec.block_params.items()}
         attrs = {k: str(v) for k, v in self._attrs.items() if not k.startswith("b2.")}
         attrs["b2.params"] = json.dumps({k: self.params[k] for k in sorted(self.params) if _json_ok(self.params[k]) and
@@ -1101,6 +1147,21 @@ def _num_str(v):
     return str(int(f)) if f == int(f) and abs(f) < 1e15 else "%.9g" % f
 
 
+def _str_param(v):
+    """A string-valued parameter as xgboost writes it: booleans as "1" / "0"."""
+    if isinstance(v, (bool, np.bool_)):
+        return "1" if v else "0"
+    return str(v)
+
+
+def _maximized(metric):
+    """Metrics where larger is better (early stopping): auc, interval-regression-accuracy and every ndcg / map / pre
+    form (ndcg@5, map-, pre@10, ...)."""
+    if metric in ("auc", "interval-regression-accuracy"):
+        return True
+    return metric.split("@")[0].rstrip("-") in ("ndcg", "map", "pre")
+
+
 def _xgb_feature_type(t):
     """'q' / 'c' of the DMatrix interface -> the names xgboost stores in a model file."""
     return {"q": "float", "c": "c", "i": "int"}.get(str(t), str(t))
@@ -1247,7 +1308,7 @@ def train(params, dtrain, num_boost_round=10, evals=(), obj=None, feval=None, ma
                     print(msg, flush=True)
                 if early_stopping_rounds:
                     data, metric, v = _parse_eval_str(msg)[-1]
-                    mx = maximize if maximize is not None else metric in ("auc", "map", "ndcg", "interval-regression-accuracy")
+                    mx = maximize if maximize is not None else _maximized(metric)
                     better = best_score is None or (v > best_score if mx else v < best_score)
                     if better:
                         best_score, best_iter, best_msg = v, epoch, msg

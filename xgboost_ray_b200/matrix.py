@@ -45,6 +45,51 @@ def _get_sharding_indices(sharding: RayShardingMode, rank: int, num_actors: int,
         f"\nFIX THIS by passing any item of the `RayShardingMode` enum, for instance `RayShardingMode.BATCH`.")
 
 
+def group_offsets(qid: np.ndarray) -> np.ndarray:
+    """Row offsets of the query groups of a non-decreasing qid: a group is a maximal run of equal ids."""
+    q = np.asarray(qid).reshape(-1)
+    if q.size == 0:
+        return np.zeros(1, np.int64)
+    starts = np.flatnonzero(np.r_[True, q[1:] != q[:-1]])
+    return np.r_[starts, q.size].astype(np.int64)
+
+
+def group_sharding_rows(sharding: RayShardingMode, rank: int, num_actors: int, offsets: np.ndarray) -> np.ndarray:
+    """Rows of `rank` when every query group goes whole to one actor: group g to rank g mod W (INTERLEAVED), or the
+    group list split like numpy.array_split (BATCH).  A LambdaMART gradient depends on the rows of its group only, so
+    whole groups make the gradients independent of the number of actors."""
+    n_groups = len(offsets) - 1
+    if n_groups < num_actors:
+        raise ValueError(f"Trying to shard {n_groups} query groups (qid) over {num_actors} actors: every group goes "
+                         f"whole to one actor, so there must be at least as many groups as actors."
+                         f"\nFIX THIS by using at most {n_groups} actors.")
+    if sharding == RayShardingMode.INTERLEAVED:
+        groups = np.arange(rank, n_groups, num_actors)
+    elif sharding == RayShardingMode.BATCH:
+        groups = np.array_split(np.arange(n_groups), num_actors)[rank]
+    else:
+        raise ValueError(f"Invalid value for `sharding` parameter: {sharding}"
+                         f"\nFIX THIS by passing any item of the `RayShardingMode` enum, for instance `RayShardingMode.BATCH`.")
+    if len(groups) == 0:
+        return np.zeros(0, np.int64)
+    sizes = offsets[groups + 1] - offsets[groups]
+    starts = np.repeat(offsets[groups] - np.r_[0, np.cumsum(sizes)[:-1]], sizes)
+    return (starts + np.arange(int(sizes.sum()))).astype(np.int64)
+
+
+def combine_by_index(row_index: Sequence[np.ndarray], data: Iterable) -> np.ndarray:
+    """Reassemble per-actor prediction arrays whose rows are `row_index[rank]` (group-aligned shards)."""
+    data = [np.asarray(d) for d in data]
+    n = sum(len(ix) for ix in row_index)
+    shaped = [d for d in data if len(d)]
+    if not shaped:
+        return np.zeros(0, np.float32)
+    out = np.empty((n,) + shaped[0].shape[1:], dtype=shaped[0].dtype)
+    for ix, d in zip(row_index, data):
+        out[ix] = d
+    return out
+
+
 def combine_data(sharding: RayShardingMode, data: Iterable) -> np.ndarray:
     """Reassemble per-actor prediction arrays in original row order (matrix.py:1113-1157)."""
     if sharding not in (RayShardingMode.BATCH, RayShardingMode.INTERLEAVED):
@@ -232,8 +277,6 @@ class RayDMatrix:
             raise ValueError("`group` parameter is not supported. If you are using XGBoost-Ray, use `qid` parameter instead.")
         if qid is not None and weight is not None:
             raise NotImplementedError("per-group weight is not implemented.")
-        if qid is not None:
-            raise NotImplementedError("ranking (qid) is not supported by the H100 engine")
         self._uid = uuid.uuid4().int
         self.data, self.label, self.weight, self.base_margin = data, label, weight, base_margin
         self.feature_weights = feature_weights
@@ -254,6 +297,11 @@ class RayDMatrix:
             raise ValueError(f"Distributed data loading is not supported for input data of type {type(data)}. "
                              f"\nFIX THIS by passing file names or setting `distributed=False`.")
         self.distributed = bool(distributed)
+        if self.distributed and qid is not None:
+            raise ValueError("ranking (qid) with distributed loading (a list of files read by the actors) is not "
+                             "supported: a query group may span files.\nFIX THIS by loading the data centrally "
+                             "(`distributed=False`).")
+        self._row_index: Optional[List[np.ndarray]] = None   # qid: rows of every rank in the qid-sorted order
         if self.distributed:
             self.sharding = RayShardingMode.FIXED if sharding == RayShardingMode.FIXED else sharding
         self.refs: Dict[int, Dict[str, Optional[np.ndarray]]] = {}
@@ -287,6 +335,15 @@ class RayDMatrix:
         ll = _column_or_array(frame, self.label_lower_bound, exclude)
         lu = _column_or_array(frame, self.label_upper_bound, exclude)
         fw = None if self.feature_weights is None else np.asarray(self.feature_weights, np.float32)
+        q = None
+        if self.qid is not None:                # the ids keep their dtype (float32 would merge large ids)
+            if isinstance(self.qid, str):
+                exclude.add(self.qid)
+                q = np.asarray(frame.column(self.qid)).reshape(-1)
+            else:
+                q = np.asarray(self.qid.values if hasattr(self.qid, "values") and not isinstance(self.qid, np.ndarray)
+                               else self.qid).reshape(-1)
+        self._qid_rows = q
         x = frame.drop(exclude) if exclude else frame
         if x.feature_types is not None:
             if not self.enable_categorical:
@@ -352,6 +409,11 @@ class RayDMatrix:
                 if v is not None and len(v) != n:
                     raise ValueError(f"`{name}` has {len(v)} rows but the data has {n}")
             self._columns = x.columns
+            if self._qid_rows is not None:
+                self._load_groups(x.values, {"label": y, "weight": w, "base_margin": b, "label_lower_bound": ll,
+                                             "label_upper_bound": lu}, fw, self._qid_rows, W)
+                self.loaded = True
+                return
             remote = getattr(self, "_transport", "shm") == "remote" and x.values.flags.c_contiguous and n > 0
             if remote:
                 allow_actors_to_read_this_process()
@@ -374,6 +436,32 @@ class RayDMatrix:
                 self.refs[r], self._shared[r] = ref, shared
             self.n = n
         self.loaded = True
+
+    def _load_groups(self, xv: np.ndarray, side: Dict[str, Optional[np.ndarray]], fw, q: np.ndarray, W: int):
+        """Shards of a ranking matrix: rows sorted stably by qid (merge sort; the reference's pandas sort is not
+        stable), then whole query groups per actor.  Every shard is a gathered copy, so it always travels as a /dev/shm
+        file; its qid is the shard-local group number (exact in float32)."""
+        n = len(xv)
+        if len(q) != n:
+            raise ValueError(f"`qid` has {len(q)} rows but the data has {n}")
+        order = None if n < 2 or not np.any(q[1:] < q[:-1]) else np.argsort(q, kind="mergesort")
+        qs = q if order is None else q[order]
+        offsets = group_offsets(qs)
+        self._row_index = []
+        for r in range(W):
+            rows = group_sharding_rows(self.sharding, r, W, offsets)     # positions in the qid-sorted order
+            src = rows if order is None else order[rows]                 # rows of the caller's arrays
+            ref, shared = {"feature_weights": fw}, {"feature_weights": fw}
+            tag = "%x_%d_" % (self._uid & 0xffffffff, r)
+            ref["data"], shared["data"] = _shared_copy(xv[src], tag + "data")
+            for name, a in side.items():
+                ref[name], shared[name] = _shared_copy(None if a is None else a[src], tag + name)
+            local = group_offsets(qs[rows])
+            gid = np.repeat(np.arange(len(local) - 1), np.diff(local)).astype(np.float32)
+            ref["qid"], shared["qid"] = _shared_copy(gid, tag + "qid")
+            self.refs[r], self._shared[r] = ref, shared
+            self._row_index.append(rows)
+        self.n = n
 
     def get_data(self, rank: int, num_actors: Optional[int] = None) -> Dict[str, Optional[np.ndarray]]:
         self.load_data(num_actors=num_actors, rank=rank if (self.distributed and rank not in self.refs) else None)
