@@ -48,10 +48,20 @@ def case_data(name):
             + (np.nan_to_num(x[:, 10]) % 7 < 2) * 1
         return x, score.astype(np.float32), None, \
             {"objective": "multi:softprob", "num_class": 5, "max_depth": 5, "eta": 0.3}, 3
+    if name == "synthetic_softprob_k20_weighted_missing":
+        # more classes than the engine's fused gradient path takes (16): unfused gradients, one absmax pass per class tree
+        rng = np.random.RandomState(2020)
+        x = rng.uniform(0, 10, size=(3000, 10)).astype(np.float32)
+        x[rng.uniform(size=x.shape) < 0.1] = np.nan
+        v = np.nan_to_num(x[:, 0]) * 2 + np.nan_to_num(x[:, 1]) * 0.7 + rng.normal(scale=0.5, size=3000)
+        y = (np.floor(v) % 20).astype(np.float32)
+        w = rng.uniform(0.5, 2.0, size=3000).astype(np.float32)
+        return x, y, w, {"objective": "multi:softprob", "num_class": 20, "max_depth": 4, "eta": 0.3}, 2
     raise KeyError(name)
 
 
-CASES = ["toy_softmax", "breast_cancer_logistic", "synthetic_missing_regression", "synthetic_categorical_softprob"]
+CASES = ["toy_softmax", "breast_cancer_logistic", "synthetic_missing_regression", "synthetic_categorical_softprob",
+         "synthetic_softprob_k20_weighted_missing"]
 # feature kinds of the cases that have categorical columns ('c'); everything else is numeric
 FEATURE_TYPES = {"synthetic_categorical_softprob": ["q"] * 6 + ["c"] * 5}
 

@@ -39,7 +39,8 @@ def make_data(n, f, seed, kind="uniform", nan_frac=0.0):
 # pow2ceil(r) steps, 32 / w shared-memory replicas): widths 1, 2, 4, 8, 16 alone and behind full groups are all covered
 @pytest.mark.parametrize("narrow", [0, 1])
 @pytest.mark.parametrize("n,f", [(1, 1), (17, 3), (1000, 28), (5000, 100), (3000, 50), (2000, 200), (4097, 33),
-                                 (3001, 2), (2500, 34), (3000, 12), (777, 16), (2000, 48), (1500, 7), (6000, 104)])
+                                 (3001, 2), (2500, 34), (3000, 12), (777, 16), (2000, 48), (1500, 7), (6000, 104),
+                                 (1500, 800)])   # more groups than the pair plan holds: one group per CTA
 def test_hist_kernel_bit_exact(eng, oracle, n, f, narrow):
     rng = np.random.RandomState(n + f)
     bins = rng.randint(0, 256, size=(n, f)).astype(np.uint8)

@@ -83,7 +83,7 @@ int b2_launch_tree_init(B2TreeDev, B2LevelCtl*, B2NodeSeg*, B2EvalNode*, int32_t
 int b2_launch_iota(int32_t*, int64_t, cudaStream_t);
 int b2_launch_gradient(int, int, const float*, const float*, const float*, int64_t, float, float, float2*, uint32_t*, uint32_t*, int,
                        cudaStream_t);
-int b2_launch_label_check(int, const float*, int64_t, uint32_t*, int, cudaStream_t);
+int b2_launch_label_check(int, int, const float*, int64_t, uint32_t*, int, cudaStream_t);
 int b2_launch_gradient_aft(int, double, const float*, const float*, const float*, const float*, int64_t, float2*, uint32_t*,
                            uint32_t*, int, cudaStream_t);
 int b2_launch_aft_bounds_check(const float*, const float*, int64_t, uint32_t*, int, cudaStream_t);
@@ -1926,16 +1926,19 @@ void check_labels(Booster* b) {
   Matrix* m = b->train; const int o = b->p.objective; cudaStream_t s = b->ctx->stream;
   if (o == kObjAft) { check_bounds(b); return; }
   if (obj_rank(o)) { check_rank_labels(b); return; }
-  if (o == kObjSquaredError || o == kObjLogistic || o == kObjSoftprob || o == kObjPseudoHuber || b->labels_checked) return;
+  if (o == kObjSquaredError || o == kObjLogistic || o == kObjPseudoHuber || b->labels_checked) return;
   if (m->n_label != m->n) fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)m->n);
   DevBuf<uint32_t> bad; bad.ensure(1);
   CUDA_CHECK(cudaMemsetAsync(bad.p, 0, sizeof(uint32_t), s));
-  LAUNCH_CHECK(b2_launch_label_check(o, m->label.p, m->n, bad.p, b->ctx->num_sms, s));
+  LAUNCH_CHECK(b2_launch_label_check(o, b->p.num_class, m->label.p, m->n, bad.p, b->ctx->num_sms, s));
   allreduce(b->comm, bad.p, 1, kNcclUint32, kNcclMax, s);
   uint32_t h = 0;
   CUDA_CHECK(cudaMemcpyAsync(&h, bad.p, sizeof(h), cudaMemcpyDeviceToHost, s));
   CUDA_CHECK(cudaStreamSynchronize(s));
   if (h) {
+    // a class index; non-integer labels truncate like xgboost's, NaN is rejected (xgboost lets it through)
+    if (o == kObjSoftprob)
+      fail("label must be in [0, num_class) for %s, num_class = %d", b->p.objective_name.c_str(), b->p.num_class);
     const char* cond = (o == kObjRegLogistic || o == kObjLogitRaw) ? "label must be in [0, 1]"
                        : o == kObjSquaredLog ? "label must be greater than -1"
                        : o == kObjGamma ? "label must be positive" : "label must be nonnegative";
@@ -2654,8 +2657,8 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
   if (aft_metric && !m->has_bounds()) fail("metric '%s' needs label_lower_bound and label_upper_bound on the evaluation matrix", metric);
   if (!aft_metric && m->n_label != m->n) fail("evaluation matrix has no labels");
   float* margin = eval_margin(b, m);
-  b->d_metric.ensure(2);
-  CUDA_CHECK(cudaMemsetAsync(b->d_metric.p, 0, 2 * sizeof(double), s));
+  b->d_metric.ensure(3);
+  CUDA_CHECK(cudaMemsetAsync(b->d_metric.p, 0, 3 * sizeof(double), s));
   if ((mid == 3 || mid == 4) != (b->p.objective == kObjSoftprob))
     fail("metric '%s' does not fit objective '%s'", metric, b->p.objective_name.c_str());
   if (aft_metric) {
@@ -2688,10 +2691,13 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
   }
   LAUNCH_CHECK(b2_launch_metric(b->p.objective, mid, b->p.num_class, mparam, margin, m->label.p, m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p,
                                 b->ctx->num_sms, s));
-  allreduce(b->comm, b->d_metric.p, 2, kNcclFloat64, kNcclSum, s);
-  double h[2];
+  // (sum, wsum, rows with a label outside [0, num_class)): the count travels with the sums, so every rank fails together
+  allreduce(b->comm, b->d_metric.p, 3, kNcclFloat64, kNcclSum, s);
+  double h[3];
   CUDA_CHECK(cudaMemcpyAsync(h, b->d_metric.p, sizeof(h), cudaMemcpyDeviceToHost, s));
   CUDA_CHECK(cudaStreamSynchronize(s));
+  if (h[2] > 0)
+    fail("metric '%s': label must be in [0, num_class), num_class = %d (%.0f rows outside)", metric, b->p.num_class, h[2]);
   double v = h[1] > 0 ? h[0] / h[1] : 0.0;
   *out = (mid == 0 || mid == 7) ? sqrt(v) : v;
   API_END

@@ -610,6 +610,8 @@ int b2_launch_hist(const uint8_t* bins, int row_stride, const int2* gpair, const
     return (int)cudaGetLastError();
   }
   if (variant == 4) variant = 3;   // other feature counts: group pairs
+  // more groups than the pair plan holds (F > 32 * 2 * B2_HIST_MAX_TYPES = 512): one group per CTA, 512 threads
+  if (variant == 3 && (n_groups + 1) / 2 > B2_HIST_MAX_TYPES) variant = 1;
   if (variant == 3) {
     // ---- group pairs with a narrow last group: CTAs per type in proportion to the atomic wavefronts per row
     static bool attr3 = false;

@@ -495,7 +495,7 @@ __global__ void quantize_kernel(const float2* __restrict__ gh, int64_t n, const 
   }
 }
 
-// metric sums (sum loss*w, sum w) -> out[2] doubles.  Metrics see the TRANSFORMED prediction (ObjFunction::EvalTransform,
+// metric sums (sum loss*w, sum w, rows with an invalid class label) -> out[3] doubles.  Metrics see the TRANSFORMED prediction (ObjFunction::EvalTransform,
 // src/learner.cc): the probability for binary:logistic / reg:logistic, exp(margin) for the log-link objectives, the raw
 // value otherwise.  metric: 0 rmse, 1 logloss, 2 error, 3 mlogloss, 4 merror, 5 mae, 7 rmsle, 8 mape, 9 mphe (a = huber
 // slope), 10 poisson-nloglik, 11 gamma-nloglik, 12 gamma-deviance, 13 tweedie-nloglik (a = rho); 6 (auc) is auc_kernel.cu.
@@ -511,10 +511,16 @@ __device__ __forceinline__ double scalar_metric(int metric, float a, double q, d
   return -y * pow(q, 1.0 - r) / (1.0 - r) + pow(q, 2.0 - r) / (2.0 - r);
 }
 
+// a multi-class label is a class index in [0, K): non-integer labels truncate (2.7 -> class 2); NaN is outside
+__device__ __forceinline__ bool b2_class_label_ok(float y, int K) { return y >= 0.0f && y < (float)K; }
+
+// out[2] counts the rows of mlogloss / merror whose label is not a class index: they add nothing to the sums (r[y] is
+// never read for them) and the caller fails the evaluation
 __global__ void metric_kernel(int objective, int metric, int K, float a, const float* __restrict__ margin,
                               const float* __restrict__ label, const float* __restrict__ weight, int64_t n,
                               double* __restrict__ out) {
   double s = 0.0, ws = 0.0;
+  unsigned bad = 0;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const double w = weight ? (double)weight[i] : 1.0;
     double v = 0.0;
@@ -530,7 +536,9 @@ __global__ void metric_kernel(int objective, int metric, int K, float a, const f
     }
     else if (metric >= 7) v = scalar_metric(metric, a, (double)b2_pred_transform(objective, margin[i]), (double)label[i]);
     else {
-      const float* r = margin + i * K; const int y = (int)label[i]; float mx = r[0]; int am = 0;
+      const float yf = label[i];
+      if (!b2_class_label_ok(yf, K)) { ++bad; continue; }
+      const float* r = margin + i * K; const int y = (int)yf; float mx = r[0]; int am = 0;
       for (int k = 1; k < K; ++k) if (r[k] > mx) { mx = r[k]; am = k; }
       if (metric == 4) v = (am != y) ? 1.0 : 0.0;
       else {
@@ -545,16 +553,22 @@ __global__ void metric_kernel(int objective, int metric, int K, float a, const f
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ws += __shfl_xor_sync(0xffffffffu, ws, o); }
-  if ((threadIdx.x & 31) == 0) { atomicAdd(&out[0], s); atomicAdd(&out[1], ws); }
+  bad = __reduce_add_sync(0xffffffffu, bad);
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(&out[0], s); atomicAdd(&out[1], ws);
+    if (bad) atomicAdd(&out[2], (double)bad);
+  }
 }
 
-// label domain of an objective (checked once per train matrix): *bad |= 1 when some label is outside it (NaN included)
-__global__ void label_check_kernel(int objective, const float* __restrict__ label, int64_t n, uint32_t* __restrict__ bad) {
+// label domain of an objective (checked once per train matrix): *bad |= 1 when some label is outside it (NaN included);
+// K is the class count of multi:softprob
+__global__ void label_check_kernel(int objective, int K, const float* __restrict__ label, int64_t n, uint32_t* __restrict__ bad) {
   bool any = false;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const float y = label[i];
     bool ok = true;
-    if (objective == kObjRegLogistic || objective == kObjLogitRaw) ok = y >= 0.0f && y <= 1.0f;
+    if (objective == 2) ok = b2_class_label_ok(y, K);
+    else if (objective == kObjRegLogistic || objective == kObjLogitRaw) ok = y >= 0.0f && y <= 1.0f;
     else if (objective == kObjSquaredLog) ok = y > -1.0f;
     else if (objective == kObjPoisson || objective == kObjTweedie) ok = y >= 0.0f;
     else if (objective == kObjGamma) ok = y > 0.0f;
@@ -656,9 +670,9 @@ int b2_launch_aft_metric(int dist, int metric, double sigma, const float* margin
   b2::aft_metric_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(dist, metric, sigma, margin, lower, upper, weight, n, out);
   return (int)cudaGetLastError();
 }
-int b2_launch_label_check(int objective, const float* label, int64_t n, uint32_t* bad, int num_sms, cudaStream_t s) {
+int b2_launch_label_check(int objective, int K, const float* label, int64_t n, uint32_t* bad, int num_sms, cudaStream_t s) {
   if (n <= 0) return 0;
-  b2::label_check_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(objective, label, n, bad);
+  b2::label_check_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(objective, K, label, n, bad);
   return (int)cudaGetLastError();
 }
 int b2_launch_subsample(float2* gh, int64_t n, uint32_t seed, uint32_t tree, uint32_t rank, double subsample, int num_sms,
