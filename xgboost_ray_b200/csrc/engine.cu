@@ -1232,7 +1232,7 @@ void ensure_ctl_tables(Booster* b) {
   if (!b->d_eval_done.p) { b->d_eval_done.ensure(1); CUDA_CHECK(cudaMemsetAsync(b->d_eval_done.p, 0, sizeof(uint32_t), b->ctx->stream)); }
   b->d_cand_best.ensure(half);
   b->d_leaves.ensure(L.max_nodes); b->d_seg_work.ensure(L.max_nodes);
-  b->d_leaf_sums.ensure(2 * lcap); b->d_leaf_values.ensure(lcap);
+  b->d_leaf_sums.ensure(4 * lcap); b->d_leaf_values.ensure(lcap);   // [leaf][g, h][hi, lo] limbs (common.cuh)
   b->node_elems = (size_t)G * B2_GROUP_ELEMS;
   // feature-slot sharding of the histogram exchange: rank r owns slots s with s % shards == r (DESIGN.md 5)
   const int world = b->comm ? b->comm->world : 1;
@@ -1247,7 +1247,7 @@ void ensure_ctl_tables(Booster* b) {
     auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
     const size_t build_bytes = up(half * b->node_elems * sizeof(long long));
     const size_t cands_bytes = up(half * b->cpn * b->shards * sizeof(B2SplitCand));
-    b->x_misc_stride = 2 + 2 * lcap;                                   // even: 16-byte aligned regions
+    b->x_misc_stride = 2 + 4 * lcap;                                   // even: 16-byte aligned regions
     const size_t misc_bytes = up((size_t)b->shards * b->x_misc_stride * sizeof(long long));
     const size_t flag_bytes = up((size_t)b2_p2p_flag_words(b->shards) * sizeof(uint32_t));
     b->xoff_cands = build_bytes; b->xoff_misc = b->xoff_cands + cands_bytes; b->xoff_flags = b->xoff_misc + misc_bytes;
@@ -1412,7 +1412,7 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   const int max_leaf_chunks = (int)((n + lchunk - 1) / lchunk) + (int)lcap;
 
   LAUNCH_CHECK(b2_launch_tree_init(tree, ctl, b->d_seg[0].p, b->d_ev[0].p, d_n_leaves, (int)n, b->d_hist_work.p, s));
-  CUDA_CHECK(cudaMemsetAsync(b->d_leaf_sums.p, 0, 2 * lcap * sizeof(long long), s));
+  CUDA_CHECK(cudaMemsetAsync(b->d_leaf_sums.p, 0, 4 * lcap * sizeof(long long), s));
   mark_phase(b, 0);
   // ---- root histogram (no gather; row count known on the host)
   const int sh = b->log2_shards;
@@ -1561,7 +1561,7 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
     st.kernel_launches++;
   }
   if (p2p) { LAUNCH_CHECK(b2_launch_p2p_leaf_sums(&b->p2p.pp, d_n_leaves, b->d_leaf_sums.p, s)); st.kernel_launches++; }
-  else allreduce(b->comm, b->d_leaf_sums.p, 2 * lcap, kNcclInt64, kNcclSum, s);
+  else allreduce(b->comm, b->d_leaf_sums.p, 4 * lcap, kNcclInt64, kNcclSum, s);   // limb by limb: exact
   LAUNCH_CHECK(b2_launch_leaf_values(b->d_leaves.p, d_n_leaves, b->d_leaf_sums.p, b->d_qexp.p, 40, cp, b->d_leaf_values.p, tree, b->t_qexp.p, s));
   if (leaf_fused)
     LAUNCH_CHECK(b2_launch_margin_update(b->margin.p, K, k, b->pos.p, b->d_leaf_values.p, n, ctx->num_sms, s));
@@ -1802,7 +1802,7 @@ void init_margin(Booster* b, float* margin, Matrix* m) {
 
 // base_score when the user gave none (xgboost >= 2.0: ObjFunction::InitEstimation -> FitIntercept, tree::FitStump;
 // SURVEY.md A.3): one Newton step of a stump at margin 0, -sum(g)/sum(h) over ALL workers, then the inverse link.
-// Sums are 40-bit fixed-point integers, so every rank (and the oracle) computes the same value.
+// Sums are 40-bit fixed-point integers (exact below 2^31 rows), so every rank (and the oracle) computes the same value.
 void estimate_base_score(Booster* b) {
   Matrix* m = b->train; cudaStream_t s = b->ctx->stream; Params& p = b->p;
   if (p.base_score_set || p.objective == kObjSoftprob) { p.base_score_set = true; return; }
@@ -1811,7 +1811,7 @@ void estimate_base_score(Booster* b) {
   if (m->n_label != m->n) fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)m->n);
   const int64_t n = m->n;
   DevBuf<float> zeros; DevBuf<float2> gh; DevBuf<long long> sums;
-  zeros.ensure((size_t)std::max<int64_t>(n, 1)); gh.ensure((size_t)std::max<int64_t>(n, 1)); sums.ensure(2);
+  zeros.ensure((size_t)std::max<int64_t>(n, 1)); gh.ensure((size_t)std::max<int64_t>(n, 1)); sums.ensure(4);
   CUDA_CHECK(cudaMemsetAsync(zeros.p, 0, (size_t)std::max<int64_t>(n, 1) * sizeof(float), s));
   LAUNCH_CHECK(b2_launch_gradient(p.objective, 1, zeros.p, m->label.p, m->n_weight ? m->weight.p : nullptr, n, p.scale_pos_weight,
                                   objective_param(p), gh.p, nullptr, nullptr, b->ctx->num_sms, s));
@@ -1820,14 +1820,19 @@ void estimate_base_score(Booster* b) {
   LAUNCH_CHECK(b2_launch_absmax(gh.p, n, b->d_absmax.p, b->ctx->num_sms, s));
   allreduce(b->comm, b->d_absmax.p, 2, kNcclUint32, kNcclMax, s);
   LAUNCH_CHECK(b2_launch_quant_exponent(b->d_absmax.p, b->d_qexp.p, s));
-  CUDA_CHECK(cudaMemsetAsync(sums.p, 0, 2 * sizeof(long long), s));
+  CUDA_CHECK(cudaMemsetAsync(sums.p, 0, 4 * sizeof(long long), s));
   LAUNCH_CHECK(b2_launch_sum_fixed(gh.p, n, b->d_qexp.p, 40, sums.p, b->ctx->num_sms, s));
-  allreduce(b->comm, sums.p, 2, kNcclInt64, kNcclSum, s);
-  long long h_s[2]; int32_t h_e[2];
+  allreduce(b->comm, sums.p, 4, kNcclInt64, kNcclSum, s);   // [g, h][hi, lo] limbs (common.cuh): exact over all ranks
+  long long h_s[4]; int32_t h_e[2];
   CUDA_CHECK(cudaMemcpyAsync(h_s, sums.p, sizeof(h_s), cudaMemcpyDeviceToHost, s));
   CUDA_CHECK(cudaMemcpyAsync(h_e, b->d_qexp.p, sizeof(h_e), cudaMemcpyDeviceToHost, s));
   CUDA_CHECK(cudaStreamSynchronize(s));
-  const double G = (double)h_s[0] / ldexp(1.0, 40 - h_e[0]), H = (double)h_s[1] / ldexp(1.0, 40 - h_e[1]);
+  auto limbs_to_double = [](long long hi, long long lo) {   // b2_limbs_to_double on the host: one rounding
+    hi += lo >> B2_LIMB_SHIFT; lo &= (1ll << B2_LIMB_SHIFT) - 1;
+    return (double)hi * (double)(1ll << B2_LIMB_SHIFT) + (double)lo;
+  };
+  const double G = limbs_to_double(h_s[0], h_s[1]) / ldexp(1.0, 40 - h_e[0]);
+  const double H = limbs_to_double(h_s[2], h_s[3]) / ldexp(1.0, 40 - h_e[1]);
   const float stump = H <= 1e-6 ? 0.0f : (float)(-G / H);
   if (obj_sigmoid(p.objective) || obj_log_link(p.objective)) {
     // margin -> output space with the engine's own sigmoid / exp (same IEEE sequence as the kernels): evaluated on the device

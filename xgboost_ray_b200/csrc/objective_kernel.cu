@@ -432,10 +432,12 @@ __global__ void subsample_kernel(float2* __restrict__ gh, int64_t n, uint32_t se
     if (!(b2_hash4(seed, tree, rank, (uint32_t)i) < thr)) gh[i] = make_float2(0.0f, 0.0f);
 }
 
-// exact sums of one gradient-pair array in fixed point (bits relative to the quantisation exponents): int64 atomics
-// of block partials, so the result does not depend on the order of rows, blocks or GPUs (base_score estimation)
+// exact sums of one gradient-pair array in fixed point (bits relative to the quantisation exponents), kept as two
+// int64 limbs per sum (common.cuh), so the result does not depend on the order of rows, blocks or GPUs (base_score
+// estimation).  A thread sums at most ceil(n / 4096) rows (grid_for launches at least 16 CTAs once n > 4096), below
+// 2^20 for n < 2^31, so its int64 partial is exact; the warp then adds the partials limb by limb.
 __global__ void sum_fixed_kernel(const float2* __restrict__ gh, int64_t n, const int32_t* __restrict__ qexp, int bits,
-                                 long long* __restrict__ out /*[2]*/) {
+                                 long long* __restrict__ out /*[g, h][hi, lo]*/) {
   const double kg = ldexp(1.0, bits - qexp[0]), kh = ldexp(1.0, bits - qexp[1]);
   long long ag = 0, ah = 0;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -443,12 +445,15 @@ __global__ void sum_fixed_kernel(const float2* __restrict__ gh, int64_t n, const
     ag += __double2ll_rn(__dmul_rn((double)v.x, kg));
     ah += __double2ll_rn(__dmul_rn((double)v.y, kh));
   }
+  constexpr long long kLoMask = (1ll << B2_LIMB_SHIFT) - 1;
+  long long limb[4] = {ag >> B2_LIMB_SHIFT, ag & kLoMask, ah >> B2_LIMB_SHIFT, ah & kLoMask};
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) { ag += __shfl_xor_sync(0xffffffffu, ag, o); ah += __shfl_xor_sync(0xffffffffu, ah, o); }
-  if ((threadIdx.x & 31) == 0) {
-    atomicAdd((unsigned long long*)&out[0], (unsigned long long)ag);
-    atomicAdd((unsigned long long*)&out[1], (unsigned long long)ah);
-  }
+  for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) limb[j] += __shfl_xor_sync(0xffffffffu, limb[j], o);
+  if ((threadIdx.x & 31) == 0)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) atomicAdd((unsigned long long*)&out[j], (unsigned long long)limb[j]);
 }
 
 // interleave user-supplied gradients (custom objective): g,h row-major [n][K] -> gh [K][n]

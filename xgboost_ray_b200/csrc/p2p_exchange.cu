@@ -71,12 +71,13 @@ __global__ void p2p_quant_exponent_kernel(B2P2P pp, const uint32_t* __restrict__
   p2p_finish_single(pp, kSlotAbsmax, epoch);
 }
 
-// leaf sums: every rank stores its [n_leaves][2] int64 sums into every rank's misc table (offset 2), then replaces its
-// local sums with the total over the ranks (replaces ncclAllReduce(sum) in front of leaf_values_kernel)
+// leaf sums: every rank stores its [n_leaves][g, h][hi, lo] int64 limbs (common.cuh) into every rank's misc table
+// (offset 2), then replaces its local limbs with the total over the ranks (replaces ncclAllReduce(sum) in front of
+// leaf_values_kernel).  Limbs add limb by limb without wrapping, so the total is exact below 2^31 rows over all ranks.
 __global__ void __launch_bounds__(1024)
 p2p_leaf_sums_kernel(B2P2P pp, const int32_t* __restrict__ n_leaves, long long* __restrict__ sums) {
   const uint32_t epoch = p2p_next_epoch(pp, kSlotLeaf);
-  const int n = 2 * *n_leaves;
+  const int n = 4 * *n_leaves;
   for (int w = 0; w < pp.world; ++w)
     for (int i = threadIdx.x; i < n; i += blockDim.x) st_volatile_u64(pp.misc[w] + (size_t)pp.rank * pp.misc_stride + 2 + i, sums[i]);
   __syncthreads();

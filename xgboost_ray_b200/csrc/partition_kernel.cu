@@ -161,12 +161,13 @@ partition_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, const
   finalize_level_block<kPartThreads>(s_fin, ctl, work, counters, fin);
 }
 
-// ---- leaf refinement: 40-bit fixed-point sums of the fp32 gradients per leaf (exact int64)
+// ---- leaf refinement: 40-bit fixed-point sums of the fp32 gradients per leaf (exact: int64 partials of at most 2048
+// rows, added to the leaf's limbs, common.cuh)
 // sums == nullptr: only record the leaf index of every row (pos); leaf_accumulate_kernel sums the leaves afterwards.
 __global__ void __launch_bounds__(256)
 leaf_sums_kernel(const float2* __restrict__ gh, const int32_t* __restrict__ ridx0, const int32_t* __restrict__ ridx1,
                  const SegWork* __restrict__ work, const B2LevelCtl* __restrict__ ctl, const int32_t* __restrict__ qexp,
-                 int leaf_bits, long long* __restrict__ sums /* nullable: [n_leaves][2] */,
+                 int leaf_bits, long long* __restrict__ sums /* nullable: [n_leaves][g, h][hi, lo] */,
                  uint16_t* __restrict__ pos /* nullable: row -> leaf index, read by margin_update_kernel */) {
   const int n_work = ctl->hist_n_work, total_chunks = ctl->hist_total_chunks;
   __shared__ long long sg[8], sh[8];
@@ -201,8 +202,8 @@ leaf_sums_kernel(const float2* __restrict__ gh, const int32_t* __restrict__ ridx
     if (threadIdx.x == 0) {
       long long tg = 0, th = 0;
       for (int i = 0; i < 8; ++i) { tg += sg[i]; th += sh[i]; }
-      atomicAdd((unsigned long long*)&sums[2 * w.id], (unsigned long long)tg);
-      atomicAdd((unsigned long long*)&sums[2 * w.id + 1], (unsigned long long)th);
+      b2_atomic_add_limbs(&sums[4 * w.id], tg);
+      b2_atomic_add_limbs(&sums[4 * w.id + 2], th);
     }
     __syncthreads();
   }
@@ -304,8 +305,8 @@ final_assign_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, co
     __syncthreads();
     if (threadIdx.x < 4) {
       long long t = 0;
-      for (int i = 0; i < kPartThreads / 32; ++i) t += s_acc[i][threadIdx.x];
-      atomicAdd((unsigned long long*)&sums[2 * leaf_l + threadIdx.x], (unsigned long long)t);   // [leaf_l][g,h], [leaf_l+1][g,h]
+      for (int i = 0; i < kPartThreads / 32; ++i) t += s_acc[i][threadIdx.x];   // at most 8192 rows: exact
+      b2_atomic_add_limbs(&sums[2 * (2 * leaf_l + threadIdx.x)], t);   // [leaf_l][g,h], [leaf_l+1][g,h]
     }
     __syncthreads();
   }
@@ -327,10 +328,13 @@ margin_update_kernel(float* __restrict__ margin, int K, int k, const uint16_t* _
 // modulo 2^64, like an int64 add.  (A 64-bit shared atomic is a compare-and-swap loop on sm_90, and lanes of a warp
 // that hit the same popular leaf retry one after another.)  Lanes spread over `copies` copies of the table
 // (lane % copies), so that a popular leaf is not one shared-memory word for the whole warp.  At the end the copies are
-// added up and every non-empty leaf costs one global atomic per CTA.
+// added up and every non-empty leaf adds its CTA total to the leaf's two limbs (common.cuh).  A CTA sums at most
+// kLeafAccCtaRows + 512 rows (the launch sizes the grid for it), so its total is below 2^63 in magnitude and the
+// int64 arithmetic modulo 2^64 gives it exactly.
 constexpr int kLeafAccThreads = 512;
 constexpr int kLeafAccMaxDepth = 11;            // 2^11 leaves x 16 bytes = 32 KB of shared memory per CTA
 constexpr int kLeafAccSmem = 32 * 1024;         // copies of the table: as many as fit here, at most 8
+constexpr int64_t kLeafAccCtaRows = 1 << 22;    // rows per CTA at most (rounded up to a grid stride): 2^22 x 2^40 < 2^63
 __device__ __forceinline__ void acc_add64(uint32_t* lo, uint32_t* hi, long long q) {
   const uint32_t l = (uint32_t)(unsigned long long)q, h = (uint32_t)((unsigned long long)q >> 32);
   const uint32_t old = atomicAdd(lo, l);
@@ -339,7 +343,8 @@ __device__ __forceinline__ void acc_add64(uint32_t* lo, uint32_t* hi, long long 
 }
 __global__ void __launch_bounds__(kLeafAccThreads)
 leaf_accumulate_kernel(const float2* __restrict__ gh, const uint16_t* __restrict__ pos, int64_t n, int n_acc, int log2_copies,
-                       const int32_t* __restrict__ qexp, int leaf_bits, long long* __restrict__ sums /* [n_leaves][2] */) {
+                       const int32_t* __restrict__ qexp, int leaf_bits,
+                       long long* __restrict__ sums /* [n_leaves][g, h][hi, lo] */) {
   extern __shared__ uint32_t s_acc[];   // 4 planes (g lo, g hi, h lo, h hi) of [n_acc][copies]
   const int copies = 1 << log2_copies, plane = n_acc << log2_copies;
   for (int i = threadIdx.x; i < 4 * plane; i += blockDim.x) s_acc[i] = 0u;
@@ -376,7 +381,7 @@ leaf_accumulate_kernel(const float2* __restrict__ gh, const uint16_t* __restrict
       const int a = ((j >> 1) << log2_copies) + c;
       t += ((unsigned long long)hi[a] << 32) | (unsigned long long)lo[a];
     }
-    if (t != 0ull) atomicAdd((unsigned long long*)&sums[j], t);
+    if (t != 0ull) b2_atomic_add_limbs(&sums[2 * j], (long long)t);
   }
 }
 
@@ -440,7 +445,10 @@ int b2_launch_leaf_accumulate(const float2* gh, const uint16_t* pos, int64_t n, 
   while (log2_copies < 3 && ((size_t)n_acc * 16 << (log2_copies + 1)) <= (size_t)b2::kLeafAccSmem) ++log2_copies;
   const size_t smem = (size_t)n_acc * 16 << log2_copies;
   const int64_t want = (n + b2::kLeafAccThreads - 1) / b2::kLeafAccThreads;
-  const int grid = (int)(want < (int64_t)num_sms * 2 ? want : (int64_t)num_sms * 2);
+  int64_t cap = (int64_t)num_sms * 2;
+  const int64_t exact_min = (n + b2::kLeafAccCtaRows - 1) / b2::kLeafAccCtaRows;   // keeps every CTA total exact
+  if (cap < exact_min) cap = exact_min;
+  const int grid = (int)(want < cap ? want : cap);
   b2::leaf_accumulate_kernel<<<grid, b2::kLeafAccThreads, smem, stream>>>(gh, pos, n, n_acc, log2_copies, qexp, leaf_bits, sums);
   return (int)cudaGetLastError();
 }
