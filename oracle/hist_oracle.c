@@ -702,6 +702,11 @@ static int select_features(uint32_t seed, uint32_t tree, uint32_t scope, const u
   free(key);
   return cnt;
 }
+/* select_features as the tree loop calls it, for the column-sampling tests */
+int or_select_features(uint32_t seed, uint32_t tree, uint32_t scope, const uint8_t *parent, const uint32_t *fwq, int32_t F,
+                       double frac, uint8_t *out) {
+  return select_features(seed, tree, scope, parent, fwq, F, frac, out);
+}
 
 /* ------------------------------------------------------------------ A.6 split */
 static double thr_l1(double g, double a) {

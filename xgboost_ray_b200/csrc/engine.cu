@@ -1369,18 +1369,13 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
     const int F = m->F;
     const uint32_t* fwq = m->fwq.empty() ? nullptr : m->fwq.data();
     std::vector<uint8_t> mask_tree(F), masks((size_t)std::max(D, 1) * F);
-    for (int f = 0; f < F; ++f)
-      mask_tree[f] = b2_col_selected((uint32_t)p.seed, tree_index, B2_SCOPE_TREE, f, nullptr, fwq, F, b2_sample_count((double)p.colsample_bytree, F));
-    int n_tree = 0; for (int f = 0; f < F; ++f) n_tree += mask_tree[f];
-    for (int d = 0; d < D; ++d) {
-      int cnt = 0;
-      for (int f = 0; f < F; ++f) {
-        masks[(size_t)d * F + f] = b2_col_selected((uint32_t)p.seed, tree_index, B2_SCOPE_LEVEL(d), f, mask_tree.data(), fwq, F,
-                                                   b2_sample_count((double)p.colsample_bylevel, n_tree));
-        cnt += masks[(size_t)d * F + f];
-      }
-      n_level_feats[d] = cnt;
-    }
+    std::vector<B2ColRank> col_scratch(F);
+    const int n_tree = b2_col_select((uint32_t)p.seed, tree_index, B2_SCOPE_TREE, nullptr, fwq, F,
+                                     b2_sample_count((double)p.colsample_bytree, F), col_scratch.data(), mask_tree.data());
+    for (int d = 0; d < D; ++d)
+      n_level_feats[d] = b2_col_select((uint32_t)p.seed, tree_index, B2_SCOPE_LEVEL(d), mask_tree.data(), fwq, F,
+                                       b2_sample_count((double)p.colsample_bylevel, n_tree), col_scratch.data(),
+                                       masks.data() + (size_t)d * F);
     b->d_col_masks.ensure(masks.size());
     CUDA_CHECK(cudaMemcpyAsync(b->d_col_masks.p, masks.data(), masks.size(), cudaMemcpyHostToDevice, s));   // pageable source: staged before return
   }

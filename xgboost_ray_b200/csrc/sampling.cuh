@@ -12,6 +12,7 @@
 //   w_f = feature_weights[f] (1 when absent), features of weight 0 come last.
 #pragma once
 #include <stdint.h>
+#include <stdlib.h>
 #ifndef __cplusplus
 #include <stdbool.h>
 #endif
@@ -62,7 +63,8 @@ B2_HD int b2_sample_count(double frac, int n_parent) {
   int n = (int)(frac * (double)n_parent);
   return n < 1 ? 1 : n;
 }
-// is feature f among the n_sel smallest keys of the features with parent[f'] != 0 ?
+// is feature f among the n_sel smallest keys of the features with parent[f'] != 0 ?  One answer costs F key
+// evaluations: the per-node path of the split scan asks it for the few slots of one CTA.
 B2_HD bool b2_col_selected(uint32_t seed, uint32_t tree, uint32_t scope, int f, const uint8_t* parent, const uint32_t* wq, int F,
                            int n_sel) {
   if (parent && !parent[f]) return false;
@@ -74,6 +76,37 @@ B2_HD bool b2_col_selected(uint32_t seed, uint32_t tree, uint32_t scope, int f, 
     rank += (kg < kf || (kg == kf && g < f)) ? 1 : 0;
   }
   return rank < n_sel;
+}
+// Host-only whole-mask form of b2_col_selected: out[f] = 1 for the n_sel features of the parent set with the smallest
+// (key, f), 0 elsewhere.  Each key is computed once and the parent set sorted, O(F log F) instead of F^2 key
+// evaluations; (key, f) is a total order, so the set is exactly the one b2_col_selected picks.  scratch holds F
+// entries.  Returns the number of features selected.
+typedef struct { uint64_t key; int32_t f; } B2ColRank;
+static inline int b2_col_rank_cmp(const void* a, const void* b) {
+  const B2ColRank* x = (const B2ColRank*)a;
+  const B2ColRank* y = (const B2ColRank*)b;
+  if (x->key != y->key) return x->key < y->key ? -1 : 1;
+  return (x->f > y->f) - (x->f < y->f);
+}
+static inline int b2_col_select(uint32_t seed, uint32_t tree, uint32_t scope, const uint8_t* parent, const uint32_t* wq, int F,
+                                int n_sel, B2ColRank* scratch, uint8_t* out) {
+  int m = 0;
+  for (int f = 0; f < F; ++f) m += (!parent || parent[f]) ? 1 : 0;
+  if (n_sel >= m) {                      // the whole parent set (a fraction of 1.0): no key is needed
+    for (int f = 0; f < F; ++f) out[f] = (!parent || parent[f]) ? 1 : 0;
+    return m;
+  }
+  m = 0;
+  for (int f = 0; f < F; ++f) {
+    out[f] = 0;
+    if (parent && !parent[f]) continue;
+    scratch[m].key = b2_col_key(seed, tree, scope, (uint32_t)f, wq ? wq[f] : 65536u);
+    scratch[m].f = f;
+    ++m;
+  }
+  qsort(scratch, (size_t)m, sizeof(B2ColRank), b2_col_rank_cmp);
+  for (int i = 0; i < n_sel; ++i) out[scratch[i].f] = 1;
+  return n_sel;
 }
 B2_HD uint32_t b2_subsample_threshold(double subsample) {
   const double t = subsample * 4294967296.0;
