@@ -864,7 +864,22 @@ struct Booster : HandleBase {
     long long hist_launches = 0, kernel_launches = 0;
     double allreduce_bytes = 0;
   };
-  std::map<int, TreeGraph> graphs;
+  // Everything a round writes on the host side while it runs: the pinned read-back blocks of its trees, its timing
+  // events and the tree graphs whose copy and event-record nodes point at them.  Two sets alternate by round parity, so
+  // that round r+1 is enqueued while round r's blocks and events are still unread (boost_round, drain_round).
+  struct RoundBuffers {
+    std::vector<void*> staging;            // pinned host copies of finished trees, one per class tree of a round
+    std::map<int, TreeGraph> graphs;       // per class slot
+    std::vector<cudaEvent_t> ev_pool; size_t ev_used = 0;
+    std::vector<std::pair<cudaEvent_t, cudaEvent_t>> hist_events;
+    std::vector<std::pair<int, cudaEvent_t>> phase_marks;   // (phase that ENDS at this event)
+    cudaEvent_t start = nullptr, stop = nullptr;
+    uint32_t* h_p2p_err = nullptr;         // pinned copy of the peer-memory error word, written at the end of the round
+  };
+  RoundBuffers rb[2];
+  int rb_cur = 0;                          // parity of the next round to enqueue
+  int pending_trees = 0;                   // trees of the enqueued round not drained yet (in rb[rb_cur ^ 1]); 0 = none
+  bool pending_check_finite = false;       // that round's gradient kernel reports non-finite pairs into h_grad_err
   std::map<int, int> direct_trees;         // trees grown with direct launches per class slot (the first one allocates)
   bool graph_failed = false;
   bool absmax_fused = false;               // this round's gradient kernel already produced d_absmax[k]
@@ -893,8 +908,7 @@ struct Booster : HandleBase {
   DevBuf<B2SplitCand> d_cand_best;         // [nodes of a level] decide's winner of every node
   DevBuf<B2LeafDev> d_leaves;
   DevBuf<long long> d_leaf_sums; DevBuf<float> d_leaf_values; DevBuf<double> d_metric;
-  std::vector<void*> staging;              // pinned host copies of finished trees, one per class tree of a round
-  size_t staging_bytes = 0;
+  size_t staging_bytes = 0;                // bytes of every block in rb[].staging
   DevBuf<float> d_custom_g, d_custom_h;
   std::map<uint64_t, EvalCache*> eval_cache;   // keyed by Matrix::uid
   // learning to rank: the train margins' order (every round), the discount table ln2 / log(r + 2) (grown to the largest
@@ -906,53 +920,56 @@ struct Booster : HandleBase {
   DevBuf<float> rank_scratch_m, rank_scratch_y; DevBuf<double> rank_scratch_p;
   // profiling
   Timers t;
-  std::vector<cudaEvent_t> ev_pool; size_t ev_used = 0;
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> hist_events;
-  std::vector<std::pair<int, cudaEvent_t>> phase_marks;   // (phase that ENDS at this event)
-  cudaEvent_t round_start = nullptr, round_stop = nullptr;
   ~Booster() {
-    for (auto& kv : graphs) {
-      if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-      for (auto& pr : kv.second.hist_ev) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
-    }
+    // (a pending round is not drained: the stream synchronisation below waits for it and its trees are dropped)
+    for (auto& r : rb)
+      for (auto& kv : r.graphs) {
+        if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+        for (auto& pr : kv.second.hist_ev) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
+      }
     // No barrier with the peers here: a peer touches this rank's arena only inside the exchange kernels of a round, and
     // every one of those accesses happens-before a flag that this rank waited for before ITS round completed -- once the
     // last round is synchronised the arena is quiescent.  (A barrier in the destructor made a rank whose peer keeps its
     // Booster alive -- the rank that returns the model -- spin until the peer-wait timeout: 23 s per train() call.)
     if (ctx) cudaStreamSynchronize(ctx->stream);
     for (void* q : p2p.opened) cudaIpcCloseMemHandle(q);
-    for (auto e : ev_pool) cudaEventDestroy(e);
-    if (round_start) cudaEventDestroy(round_start);
-    if (round_stop) cudaEventDestroy(round_stop);
+    for (auto& r : rb) {
+      for (auto e : r.ev_pool) cudaEventDestroy(e);
+      if (r.start) cudaEventDestroy(r.start);
+      if (r.stop) cudaEventDestroy(r.stop);
+      for (void* h : r.staging) cudaFreeHost(h);
+      if (r.h_p2p_err) cudaFreeHost(r.h_p2p_err);
+    }
     for (auto& kv : eval_cache) delete kv.second;
-    for (void* h : staging) cudaFreeHost(h);
     if (h_grad_err) cudaFreeHost(h_grad_err);
   }
 };
 
+// timing events of the round being enqueued
 cudaEvent_t get_event(Booster* b) {
-  if (b->ev_used == b->ev_pool.size()) { cudaEvent_t e; CUDA_CHECK(cudaEventCreate(&e)); b->ev_pool.push_back(e); }
-  return b->ev_pool[b->ev_used++];
+  Booster::RoundBuffers& R = b->rb[b->rb_cur];
+  if (R.ev_used == R.ev_pool.size()) { cudaEvent_t e; CUDA_CHECK(cudaEventCreate(&e)); R.ev_pool.push_back(e); }
+  return R.ev_pool[R.ev_used++];
 }
 void mark_phase(Booster* b, int phase) {
   if (b->p.profile < 2) return;
   cudaEvent_t e = get_event(b);
   CUDA_CHECK(cudaEventRecord(e, b->ctx->stream));
-  b->phase_marks.push_back({phase, e});
+  b->rb[b->rb_cur].phase_marks.push_back({phase, e});
 }
-void resolve_events(Booster* b) {
-  for (size_t i = 1; i < b->phase_marks.size(); ++i) {
+void resolve_events(Booster* b, Booster::RoundBuffers& R) {
+  for (size_t i = 1; i < R.phase_marks.size(); ++i) {
     float ms = 0.f;
-    if (b->phase_marks[i].first >= 0 && cudaEventElapsedTime(&ms, b->phase_marks[i - 1].second, b->phase_marks[i].second) == cudaSuccess)
-      b->t.phase_ms[b->phase_marks[i].first] += ms;
+    if (R.phase_marks[i].first >= 0 && cudaEventElapsedTime(&ms, R.phase_marks[i - 1].second, R.phase_marks[i].second) == cudaSuccess)
+      b->t.phase_ms[R.phase_marks[i].first] += ms;
   }
-  b->phase_marks.clear();
-  for (auto& pr : b->hist_events) {
+  R.phase_marks.clear();
+  for (auto& pr : R.hist_events) {
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, pr.first, pr.second) == cudaSuccess) b->t.hist_ms += ms;
   }
-  b->hist_events.clear();
-  b->ev_used = 0;
+  R.hist_events.clear();
+  R.ev_used = 0;
 }
 
 void parse_params(const char* text, Params* p, int* max_bin_out) {
@@ -1215,11 +1232,14 @@ void ensure_ctl_tables(Booster* b) {
   const int D = b->p.max_depth; const int G = b->train->n_groups;
   if (b->ctl_depth == D) return;
   if (b->ctl_depth != 0 && b->p2p.enabled) fail("max_depth cannot change while the peer-memory exchange is mapped");
-  for (auto& kv : b->graphs) {   // captured launch sequences hold the old table addresses
-    if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-    for (auto& pr : kv.second.hist_ev) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
+  for (auto& r : b->rb) {   // captured launch sequences hold the old table addresses
+    for (auto& kv : r.graphs) {
+      if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+      for (auto& pr : kv.second.hist_ev) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
+    }
+    r.graphs.clear();
   }
-  b->graphs.clear(); b->direct_trees.clear();
+  b->direct_trees.clear();
   b->ctl_depth = D;
   const TreeLayout L = tree_layout(D);
   const size_t lcap = (size_t)1 << D, half = (size_t)1 << (D > 0 ? D - 1 : 0);
@@ -1355,7 +1375,8 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   const bool sub_in_scan = !p2p && !m->any_cat();
   mark_phase(b, -1);
   // ---- fixed-point quantisation (global scale via max over the ranks)
-  const uint32_t tree_index = (uint32_t)b->trees.size() + (uint32_t)slot;   // position of this tree in the model (sampling seed)
+  // position of this tree in the model (sampling seed): the trees of a round still pending come before it
+  const uint32_t tree_index = (uint32_t)b->trees.size() + (uint32_t)b->pending_trees + (uint32_t)slot;
   uint32_t* d_absmax = b->d_absmax.p + 2 * k;
   if (p.subsample < 1.0f) {
     LAUNCH_CHECK(b2_launch_subsample(b->gh.p + (size_t)k * n, n, (uint32_t)p.seed, tree_index, b->comm ? (uint32_t)b->comm->rank : 0u,
@@ -1568,8 +1589,8 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
                                        b->d_leaf_values.p, ctx->num_sms, s));
   st.kernel_launches += 2;
   mark_phase(b, 6);
-  // ---- read the finished tree back (pinned, asynchronous; resolved at the end of the round)
-  char* stg = (char*)b->staging[slot];
+  // ---- read the finished tree back (pinned, asynchronous; resolved when the round is drained)
+  char* stg = (char*)b->rb[b->rb_cur].staging[slot];
   // one copy: the category sets (the block's tail) only when the matrix has categorical features
   CUDA_CHECK(cudaMemcpyAsync(stg, b->t_block.p, m->any_cat() ? L.bytes : L.off_cat, cudaMemcpyDeviceToHost, s));
 }
@@ -1577,7 +1598,7 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
 void apply_tree_stats(Booster* b, long long hist_launches, long long kernel_launches, double allreduce_bytes,
                       const std::vector<std::pair<cudaEvent_t, cudaEvent_t>>& ev) {
   b->t.hist_launches += hist_launches; b->t.kernel_launches += kernel_launches; b->t.allreduce_bytes += allreduce_bytes;
-  for (auto& pr : ev) b->hist_events.push_back(pr);
+  for (auto& pr : ev) b->rb[b->rb_cur].hist_events.push_back(pr);
 }
 
 // buffers a tree needs, allocated outside of any capture
@@ -1589,15 +1610,20 @@ void prepare_tree_buffers(Booster* b, int slot) {
   b->d_absmax.ensure(2 * (size_t)b->p.num_class); b->d_qexp.ensure(2);
   b->q.ensure(rows); b->ridx[0].ensure(rows); b->ridx[1].ensure(rows); b->pos.ensure(rows);
   if (b->staging_bytes != L.bytes) {
-    for (void* h : b->staging) cudaFreeHost(h);
-    b->staging.clear(); b->staging_bytes = L.bytes;
+    for (auto& r : b->rb) {
+      for (void* h : r.staging) cudaFreeHost(h);
+      r.staging.clear();
+    }
+    b->staging_bytes = L.bytes;
   }
-  while ((int)b->staging.size() <= slot) { void* h = nullptr; CUDA_CHECK(cudaMallocHost(&h, L.bytes)); b->staging.push_back(h); }
+  std::vector<void*>& staging = b->rb[b->rb_cur].staging;
+  while ((int)staging.size() <= slot) { void* h = nullptr; CUDA_CHECK(cudaMallocHost(&h, L.bytes)); staging.push_back(h); }
 }
 
 // One class tree: replay its CUDA graph when the launch sequence is the same for every tree (no row / column sampling,
 // fused |g|,|h| maxima, no per-phase profiling), otherwise enqueue the kernels one by one.  The first tree of a class
-// slot always runs with direct launches (it allocates), the second is captured, the following ones replay.
+// slot always runs with direct launches (it allocates); the next two are captured, one graph per round parity (each
+// copies into its own read-back block and records its own events), and the following ones replay them alternately.
 void run_tree(Booster* b, int k, int slot) {
   cudaStream_t s = b->ctx->stream; const Params& p = b->p;
   prepare_tree_buffers(b, slot);
@@ -1611,8 +1637,9 @@ void run_tree(Booster* b, int k, int slot) {
     b->direct_trees[k]++;
   };
   if (!eligible) { direct(); return; }
-  auto it = b->graphs.find(k);
-  if (it == b->graphs.end()) {
+  std::map<int, Booster::TreeGraph>& graphs = b->rb[b->rb_cur].graphs;
+  auto it = graphs.find(k);
+  if (it == graphs.end()) {
     if (b->direct_trees[k] == 0) { direct(); return; }
     TreeStats st; st.capturing = true;
     cudaGraph_t graph = nullptr; cudaGraphExec_t exec = nullptr;
@@ -1635,17 +1662,17 @@ void run_tree(Booster* b, int k, int slot) {
     Booster::TreeGraph g;
     g.exec = exec; g.hist_ev = st.hist_ev; g.hist_launches = st.hist_launches; g.kernel_launches = st.kernel_launches;
     g.allreduce_bytes = st.allreduce_bytes;
-    it = b->graphs.emplace(k, std::move(g)).first;
+    it = graphs.emplace(k, std::move(g)).first;
   }
   CUDA_CHECK(cudaGraphLaunch(it->second.exec, s));
   apply_tree_stats(b, it->second.hist_launches, it->second.kernel_launches, it->second.allreduce_bytes, it->second.hist_ev);
 }
 
-// after the stream is synchronised: turn read-back block `slot` into a host tree (A.7 bookkeeping)
-void materialize_tree(Booster* b, int slot) {
+// after the round's stop event: turn read-back block `block` into a host tree (A.7 bookkeeping)
+void materialize_tree(Booster* b, const void* block) {
   Matrix* m = b->train; const Params& p = b->p;
   const TreeLayout L = tree_layout(p.max_depth);
-  const char* st = (const char*)b->staging[slot];
+  const char* st = (const char*)block;
   const int32_t* i32 = (const int32_t*)st; const size_t mx = L.max_nodes;
   const float* f32 = (const float*)(st + L.off_f32);
   const long long* i64 = (const long long*)(st + L.off_i64);
@@ -1950,8 +1977,42 @@ void check_labels(Booster* b) {
   b->labels_checked = true;
 }
 
+// Finish an enqueued round: wait for its stop event, resolve its timers, raise a peer-memory or non-finite-gradient
+// error, and turn its read-back blocks into host trees.
+void finish_round(Booster* b, Booster::RoundBuffers& R, int n_trees, bool check_finite) {
+  CUDA_CHECK(cudaEventSynchronize(R.stop));
+  if (b->p.profile) {
+    float ms = 0.f; CUDA_CHECK(cudaEventElapsedTime(&ms, R.start, R.stop));
+    b->t.round_ms += ms;
+    resolve_events(b, R);
+  }
+  if (b->p2p.enabled && *R.h_p2p_err) {
+    const uint32_t perr = *R.h_p2p_err;
+    fail("peer-memory exchange: %s while waiting for another rank (flag slot %u)",
+         b->comm && b->comm->aborted.load() ? "communicator aborted" : "timed out", perr - 1);
+  }
+  if (check_finite && *b->h_grad_err) {
+    // the trees of this round were grown with those rows zeroed and are dropped; the train margin already holds their
+    // leaves, so it is rebuilt from the kept trees before the next round
+    b->margin_ready = false;
+    fail("%s: a gradient or hessian is not finite (the margin left the range where the objective's exp is finite)",
+         b->p.objective_name.c_str());
+  }
+  for (int slot = 0; slot < n_trees; ++slot) materialize_tree(b, R.staging[slot]);
+  b->t.rounds++;
+}
+// Finish the round boost_round left pending.  Every entry point that reads the trees, the timers, the margin or the
+// gradients calls this first.  The round stops being pending before anything can throw, so an error is raised once.
+void drain_round(Booster* b) {
+  const int n_trees = b->pending_trees;
+  if (n_trees == 0) return;
+  b->pending_trees = 0;
+  finish_round(b, b->rb[b->rb_cur ^ 1], n_trees, b->pending_check_finite);
+}
+
 void ensure_train_margin(Booster* b) {
   if (b->margin_ready) return;
+  drain_round(b);   // the margin is rebuilt from every tree of the model
   Matrix* m = b->train;
   check_labels(b);
   estimate_base_score(b);
@@ -1966,13 +2027,19 @@ void ensure_train_margin(Booster* b) {
   b->margin_ready = true;
 }
 
+// One boosting round, pipelined with the previous one: round r+1 (gradients, then its class trees) is enqueued first,
+// round r is drained while the device works on r+1, and r+1 is left pending.  Nothing of r+1 needs the host: the margin
+// it reads was updated on the device by r's margin_update_kernel, in stream order.  A round whose gradient kernel checks
+// finiteness is drained before returning, so that its error is raised by its own call and its trees never exist.
 void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64_t len) {
   if (!b->train) fail("this booster has no train matrix (prediction-only)");
   Matrix* m = b->train; cudaStream_t s = b->ctx->stream; const int K = b->p.num_class; const int64_t n = m->n;
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
-  if (b->cancel.load()) fail("training cancelled");
-  if (!b->round_start) { CUDA_CHECK(cudaEventCreate(&b->round_start)); CUDA_CHECK(cudaEventCreate(&b->round_stop)); }
-  if (b->p.profile) CUDA_CHECK(cudaEventRecord(b->round_start, s));
+  if (b->cancel.load()) { drain_round(b); fail("training cancelled"); }
+  Booster::RoundBuffers& R = b->rb[b->rb_cur];   // not pending: the pending round (if any) is in the other set
+  R.hist_events.clear(); R.phase_marks.clear(); R.ev_used = 0;   // left over from a round that failed while enqueuing
+  if (!R.start) { CUDA_CHECK(cudaEventCreate(&R.start)); CUDA_CHECK(cudaEventCreate(&R.stop)); }
+  if (b->p.profile) CUDA_CHECK(cudaEventRecord(R.start, s));
   ensure_train_margin(b);
   b->gh.ensure((size_t)std::max<int64_t>(n * K, 1));
   b->d_absmax.ensure(2 * (size_t)K); b->d_qexp.ensure(2);
@@ -2024,35 +2091,23 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
       run_tree(b, k, k * npt + j);
     }
   if (check_finite) {
-    // every rank fails the round together; the flag is read back with the round's own synchronisation below (pinned
-    // memory: the copy is ordered on the stream)
+    // every rank fails the round together; the flag is read back when the round is drained (pinned memory: the copy
+    // is ordered on the stream)
     allreduce(b->comm, b->d_grad_err.p, 1, kNcclUint32, kNcclMax, s);
     CUDA_CHECK(cudaMemcpyAsync(b->h_grad_err, b->d_grad_err.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   }
-  if (b->p.profile) {
-    CUDA_CHECK(cudaEventRecord(b->round_stop, s));
-    CUDA_CHECK(cudaEventSynchronize(b->round_stop));
-    float ms = 0.f; CUDA_CHECK(cudaEventElapsedTime(&ms, b->round_start, b->round_stop));
-    b->t.round_ms += ms;
-    resolve_events(b);
-  } else {
-    CUDA_CHECK(cudaStreamSynchronize(s));
-  }
   if (b->p2p.enabled) {
-    uint32_t perr = 0;
-    CUDA_CHECK(cudaMemcpy(&perr, b->p2p.pp.err, sizeof(perr), cudaMemcpyDeviceToHost));
-    if (perr) fail("peer-memory exchange: %s while waiting for another rank (flag slot %u)",
-                   b->comm && b->comm->aborted.load() ? "communicator aborted" : "timed out", perr - 1);
+    if (!R.h_p2p_err) CUDA_CHECK(cudaMallocHost(&R.h_p2p_err, sizeof(uint32_t)));
+    CUDA_CHECK(cudaMemcpyAsync(R.h_p2p_err, b->p2p.pp.err, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   }
-  if (check_finite && *b->h_grad_err) {
-    // the trees of this round were grown with those rows zeroed and are dropped; the train margin already holds their
-    // leaves, so it is rebuilt from the kept trees before the next round
-    b->margin_ready = false;
-    fail("%s: a gradient or hessian is not finite (the margin left the range where the objective's exp is finite)",
-         b->p.objective_name.c_str());
-  }
-  for (int slot = 0; slot < K * npt; ++slot) materialize_tree(b, slot);
-  b->t.rounds++;
+  CUDA_CHECK(cudaEventRecord(R.stop, s));
+  // this round is queued behind the previous one: make it the pending round, then finish the previous one while the
+  // device works (its buffers are the set the next round enqueues into)
+  const int prev_trees = b->pending_trees; const bool prev_check = b->pending_check_finite;
+  b->pending_trees = K * npt; b->pending_check_finite = check_finite;
+  b->rb_cur ^= 1;
+  if (prev_trees) finish_round(b, b->rb[b->rb_cur], prev_trees, prev_check);
+  if (check_finite) drain_round(b);
 }
 
 // metric id of an eval_metric name; *param receives the metric's parameter (rho of tweedie-nloglik@rho, huber_slope for mphe)
@@ -2599,6 +2654,7 @@ int B2_BoosterUpdateOneIter(B2Handle bh, int32_t iter) {
 int B2_BoosterBoostOneIter(B2Handle bh, const float* grad, const float* hess, int64_t len) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   if (!grad || !hess) fail("grad/hess must not be NULL");
   boost_round(b, grad, hess, len);
   API_END
@@ -2606,6 +2662,7 @@ int B2_BoosterBoostOneIter(B2Handle bh, const float* grad, const float* hess, in
 int B2_BoosterGetGradients(B2Handle bh, float* grad, float* hess, int64_t len) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   if (!b->train) fail("this booster has no train matrix (prediction-only)");
   const int64_t nk = b->train->n * b->p.num_class;
   if (len != nk) fail("gradient buffers have %lld values, expected %lld", (long long)len, (long long)nk);
@@ -2620,6 +2677,7 @@ int B2_BoosterGetGradients(B2Handle bh, float* grad, float* hess, int64_t len) {
 int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
   cudaStream_t s = b->ctx->stream;
@@ -2709,6 +2767,7 @@ int B2_BoosterPredict(B2Handle bh, B2Handle mh, int32_t output_margin, int32_t t
                       int64_t out_len) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
   cudaStream_t s = b->ctx->stream; const int K = b->p.num_class;
@@ -2750,6 +2809,7 @@ int B2_BoosterPredictContribs(B2Handle bh, B2Handle mh, int32_t tree_begin, int3
                               int64_t out_len) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
   cudaStream_t s = b->ctx->stream; const int K = b->p.num_class; const int F = m->F;
@@ -2805,6 +2865,7 @@ int B2_BoosterPredictContribs(B2Handle bh, B2Handle mh, int32_t tree_begin, int3
 int B2_BoosterPredictLeaf(B2Handle bh, B2Handle mh, int32_t tree_begin, int32_t tree_end, float* out, int64_t out_len) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
   cudaStream_t s = b->ctx->stream;
@@ -2828,6 +2889,7 @@ int B2_BoosterPredictLeaf(B2Handle bh, B2Handle mh, int32_t tree_begin, int32_t 
 int B2_BoosterGetTrainMargin(B2Handle bh, float* out, int64_t out_len) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
   if (!b->train) fail("this booster has no train matrix (prediction-only)");
   const int64_t want = b->train->n * b->p.num_class;
@@ -2840,6 +2902,7 @@ int B2_BoosterGetTrainMargin(B2Handle bh, float* out, int64_t out_len) {
 int B2_BoosterResetTrainMargin(B2Handle bh) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
   if (!b->train) fail("this booster has no train matrix (prediction-only)");
   b->margin_ready = false;
@@ -2847,16 +2910,25 @@ int B2_BoosterResetTrainMargin(B2Handle bh) {
   CUDA_CHECK(cudaStreamSynchronize(b->ctx->stream));
   API_END
 }
+// No drain: the intercept is settled on the host before the first round is enqueued (estimate_base_score), and the
+// Python booster reads it after every update() until it is final -- a drain here would stall the round pipeline.
 int B2_BoosterGetBaseScore(B2Handle bh, float* out, int32_t* is_final) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
   *out = b->p.base_score; *is_final = b->p.base_score_set ? 1 : 0;
   API_END
 }
-int B2_BoosterNumTrees(B2Handle bh, int32_t* out) { API_BEGIN *out = (int32_t)from_handle<Booster>(bh, kBooster, "booster")->trees.size(); API_END }
+int B2_BoosterNumTrees(B2Handle bh, int32_t* out) {
+  API_BEGIN
+  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
+  *out = (int32_t)b->trees.size();
+  API_END
+}
 int B2_BoosterTreeNumNodes(B2Handle bh, int32_t tree, int32_t* out) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   if (tree < 0 || tree >= (int)b->trees.size()) fail("tree index %d out of range", tree);
   *out = b->trees[tree].size();
   API_END
@@ -2866,6 +2938,7 @@ int B2_BoosterGetTree(B2Handle bh, int32_t tree, int32_t* left, int32_t* right, 
                       float* loss_chg, double* sum_hess) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   if (tree < 0 || tree >= (int)b->trees.size()) fail("tree index %d out of range", tree);
   const TreeHost& t = b->trees[tree]; const size_t n = t.size();
   memcpy(left, t.left.data(), n * 4); memcpy(right, t.right.data(), n * 4); memcpy(parent, t.parent.data(), n * 4);
@@ -2881,6 +2954,7 @@ int B2_BoosterAddTree(B2Handle bh, int32_t n_nodes, const int32_t* left, const i
                       const double* sum_hess) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   if (n_nodes < 1) fail("a tree needs at least one node");
   TreeHost t;
   for (int i = 0; i < n_nodes; ++i) {
@@ -2899,6 +2973,7 @@ int B2_BoosterAddTree(B2Handle bh, int32_t n_nodes, const int32_t* left, const i
 int B2_BoosterGetTreeCategories(B2Handle bh, int32_t tree, uint8_t* split_type, uint32_t* cat_bits) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   if (tree < 0 || tree >= (int)b->trees.size()) fail("tree index %d out of range", tree);
   const TreeHost& t = b->trees[tree]; const size_t n = t.size();
   memcpy(split_type, t.split_type.data(), n); memcpy(cat_bits, t.cat_bits.data(), n * 8 * sizeof(uint32_t));
@@ -2907,6 +2982,7 @@ int B2_BoosterGetTreeCategories(B2Handle bh, int32_t tree, uint8_t* split_type, 
 int B2_BoosterSetTreeCategories(B2Handle bh, int32_t tree, const uint8_t* split_type, const uint32_t* cat_bits) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   if (tree < 0 || tree >= (int)b->trees.size()) fail("tree index %d out of range", tree);
   TreeHost& t = b->trees[tree]; const size_t n = t.size();
   for (size_t i = 0; i < n; ++i) {
@@ -2921,6 +2997,7 @@ int B2_BoosterSetTreeCategories(B2Handle bh, int32_t tree, const uint8_t* split_
 int B2_BoosterGetTimers(B2Handle bh, int32_t reset, char* out, int64_t out_cap) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
   const Timers& t = b->t;
   snprintf(out, (size_t)out_cap,
            "{\"hist_ms\": %.6f, \"hist_launches\": %lld, \"hist_rows\": %lld, \"hist_bytes\": %.1f, \"kernel_launches\": %lld, "
@@ -2933,12 +3010,16 @@ int B2_BoosterGetTimers(B2Handle bh, int32_t reset, char* out, int64_t out_cap) 
   if (reset) b->t.reset();
   API_END
 }
+// No drain: this only raises a flag and may be called from another thread while update() runs; the next update()
+// drains the pending round and then fails.
 int B2_BoosterCancel(B2Handle bh) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
   b->cancel.store(true);
   API_END
 }
+// A pending round is not drained (its trees are dropped with the booster); the destructor waits for it on the stream
+// before it frees the read-back blocks.
 int B2_BoosterFree(B2Handle bh) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
