@@ -190,8 +190,27 @@ struct B2TreeDev {            // arrays of capacity max_nodes
 };
 struct B2CtlParams { double mcw, lambda, alpha, max_delta_step; float gamma, eta; };
 
+// interaction constraints (DESIGN.md 2, 4.2): bit k of sets_of[f] is set when feature f is in set S_k, bit k of
+// compat[nid] when S_k holds every feature split on along the path to node nid.  decide writes compat for the
+// children it creates; the root has no entry (every feature is allowed there).  sets_of == nullptr: no constraints.
+struct B2Interaction {
+  const unsigned long long* sets_of;   // [F][words]
+  unsigned long long* compat;          // [max_nodes][words]
+  int32_t words;                       // ceil(sets / 64)
+};
+
+#ifdef __CUDACC__
+__device__ __forceinline__ bool b2_interaction_allowed(const B2Interaction& ic, int nid, int f) {
+  if (nid == 0) return true;
+  for (int w = 0; w < ic.words; ++w)
+    if (ic.compat[(size_t)nid * ic.words + w] & ic.sets_of[(size_t)f * ic.words + w]) return true;
+  return false;
+}
+#endif
+
 // column sampling of one level (sampling.cuh): level_mask = features of the level's set (nullptr = all);
-// bynode < 1 makes every node draw its own subset of that set on the device
+// bynode < 1 makes every node draw its own subset of that set on the device.  ic: the interaction constraints, which
+// filter the sampled features per node.
 struct B2ColSample {
   const uint8_t* level_mask;
   const uint32_t* fwq;      // feature weights in Q16 (nullptr = all 1.0)
@@ -199,6 +218,7 @@ struct B2ColSample {
   int32_t n_level;          // features in the level's set
   int32_t n_features;
   uint32_t seed, tree;
+  B2Interaction ic;
 };
 
 // what the last CTA of a level's partition does once every row is placed (level_finalize.cuh)
@@ -242,6 +262,7 @@ struct B2DecideArgs {
   const uint8_t* has_missing;
   const int32_t* qexp;
   int32_t* part_counters;          // nullable: zeroed for the level's partition
+  B2Interaction ic;                // sets_of != nullptr: write the children's compat entries
   B2CtlParams p;
   int32_t cands_per_node, cand_ranks, cand_rank_stride, can_split, qbits;
 };

@@ -173,6 +173,17 @@ __device__ __forceinline__ void decide_block(DecideScratch<kThreads>& sm, const 
     }
   }
   __syncthreads();
+  if (a.ic.sets_of) {   // interaction constraints: the children's paths still fit the parent's sets that hold its feature
+    const int W = a.ic.words;
+    for (int j = threadIdx.x; j < scan_split.carry; j += kThreads) {
+      const int l = node_base + 2 * j, nid = tree.parent[l];
+      const unsigned long long* sets = a.ic.sets_of + (size_t)tree.feature[nid] * W;
+      for (int w = 0; w < W; ++w) {
+        const unsigned long long c = (nid == 0 ? ~0ull : a.ic.compat[(size_t)nid * W + w]) & sets[w];
+        a.ic.compat[(size_t)l * W + w] = c; a.ic.compat[(size_t)(l + 1) * W + w] = c;
+      }
+    }
+  }
   if (threadIdx.x == 0) {
     const int n_split = scan_split.carry;
     a.ctl_cur->n_split = n_split; a.ctl_cur->part_chunks = scan_chunks.carry;

@@ -756,6 +756,9 @@ struct Params {
   float subsample = 1.0f, colsample_bytree = 1.0f, colsample_bylevel = 1.0f, colsample_bynode = 1.0f;
   int seed = 0;
   bool base_score_set = false;   // false: estimated from the labels before the first tree (xgboost >= 2.0, A.3)
+  // interaction_constraints: feature sets S_1 .. S_C (a tree path with two or more features stays inside one set);
+  // empty = no constraints.  Text form "0,1;2,3,4": sets separated by ';', features by ','.
+  std::vector<std::vector<int64_t>> interaction_sets;
   bool use_cols() const { return colsample_bytree < 1.0f || colsample_bylevel < 1.0f || colsample_bynode < 1.0f; }
 };
 
@@ -846,6 +849,10 @@ struct Booster : HandleBase {
   int cpn_num = 1;
   View<uint32_t> t_cat;                    // [max_nodes][8] category sets of the tree being grown (in t_block)
   DevBuf<uint8_t> d_col_masks;             // [max_depth][F] level feature sets of the tree being grown (column sampling)
+  // interaction constraints (B2Interaction): set membership of every feature, fixed for the booster, and the sets
+  // compatible with each node's path in the tree being grown (written by decide)
+  DevBuf<unsigned long long> d_ic_sets_of, d_ic_compat;
+  int ic_words = 0;                        // 0 = no constraints
   // NVLink peer-memory exchange (p2p.cuh, p2p_exchange.cu): on when every rank mapped its peers; B2_EXCHANGE=nccl keeps NCCL
   struct P2PState {
     bool enabled = false, tried = false;
@@ -972,6 +979,32 @@ void resolve_events(Booster* b, Booster::RoundBuffers& R) {
   R.ev_used = 0;
 }
 
+// "0,1;2,3,4" -> {{0, 1}, {2, 3, 4}}; empty sets are dropped, the indices are checked against F in B2_BoosterCreate
+std::vector<std::vector<int64_t>> parse_interaction_sets(const std::string& v) {
+  std::vector<std::vector<int64_t>> sets;
+  size_t pos = 0;
+  while (pos <= v.size()) {
+    size_t semi = v.find(';', pos);
+    if (semi == std::string::npos) semi = v.size();
+    std::vector<int64_t> set;
+    size_t q = pos;
+    while (q < semi) {
+      size_t comma = v.find(',', q);
+      if (comma == std::string::npos || comma > semi) comma = semi;
+      const std::string tok = v.substr(q, comma - q);
+      char* end = nullptr;
+      const long long f = strtoll(tok.c_str(), &end, 10);
+      if (tok.empty() || *end != '\0' || f < 0)
+        fail("interaction_constraints: '%s' is not a feature index (expected sets like 0,1;2,3,4)", tok.c_str());
+      set.push_back(f);
+      q = comma + 1;
+    }
+    if (!set.empty()) sets.push_back(set);
+    pos = semi + 1;
+  }
+  return sets;
+}
+
 void parse_params(const char* text, Params* p, int* max_bin_out) {
   std::string s(text ? text : "");
   size_t pos = 0;
@@ -1055,6 +1088,7 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     else if (k == "max_cat_to_onehot") p->max_cat_to_onehot = i();
     else if (k == "max_cat_threshold") p->max_cat_threshold = i();
     else if (k == "max_bin") { if (max_bin_out) *max_bin_out = i(); }
+    else if (k == "interaction_constraints") p->interaction_sets = parse_interaction_sets(v);
     // unknown keys (nthread, tree_method, verbosity, ...) are accepted and ignored, like xgboost
   }
   if (obj_rank(p->objective) && p->num_class > 1)
@@ -1256,6 +1290,7 @@ void ensure_ctl_tables(Booster* b) {
   b->d_cand_best.ensure(half);
   b->d_leaves.ensure(L.max_nodes); b->d_seg_work.ensure(L.max_nodes);
   b->d_leaf_sums.ensure(4 * lcap); b->d_leaf_values.ensure(lcap);   // [leaf][g, h][hi, lo] limbs (common.cuh)
+  if (b->ic_words > 0) b->d_ic_compat.ensure(L.max_nodes * (size_t)b->ic_words);
   b->node_elems = (size_t)G * B2_GROUP_ELEMS;
   // feature-slot sharding of the histogram exchange: rank r owns slots s with s % shards == r (DESIGN.md 5)
   const int world = b->comm ? b->comm->world : 1;
@@ -1473,6 +1508,9 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
     da.tree = tree; da.split_work = b->d_split_work.p; da.pair_parent_hist = b->d_pair_parent.p; da.leaves = b->d_leaves.p;
     da.n_leaves = d_n_leaves; da.has_missing = m->d_has_missing.p; da.qexp = b->d_qexp.p;
     da.part_counters = can_split ? b->d_counters.p : nullptr; da.p = cp;
+    B2Interaction ic{nullptr, nullptr, 0};
+    if (b->ic_words > 0) { ic.sets_of = b->d_ic_sets_of.p; ic.compat = b->d_ic_compat.p; ic.words = b->ic_words; }
+    da.ic = ic;
     da.cands_per_node = cpn; da.cand_ranks = b->shards; da.cand_rank_stride = max_nodes_level * cpn;
     da.can_split = can_split ? 1 : 0; da.qbits = p.qbits;
     // one GPU, numeric features only, levels scanned by the narrow layout: the last CTA of the scan decides the level
@@ -1484,6 +1522,7 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
       cs.fwq = m->fwq.empty() ? nullptr : m->d_fwq.p;
       cs.bynode = (double)p.colsample_bynode; cs.n_level = n_level_feats[d]; cs.n_features = m->F;
       cs.seed = (uint32_t)p.seed; cs.tree = p.use_cols() ? tree_index : 0u;
+      cs.ic = ic;
       // siblings of this level: parent (previous level buffer) - built, formed in the scan; stored only when the next
       // level takes them as parents
       B2SiblingSub sub{nullptr, nullptr, nullptr, 0};
@@ -2635,7 +2674,20 @@ int B2_BoosterCreate(const char* params, B2Handle trainh, B2Handle commh, B2Hand
   b->comm = commh ? &from_handle<CommH>(commh, kComm, "communicator")->c : nullptr;
   try {
     parse_params(params, &b->p, nullptr);
-    if (m) { b->ctx = m->ctx; b->n_features = m->F; CUDA_CHECK(cudaSetDevice(m->ctx->device)); }
+    if (m) {
+      b->ctx = m->ctx; b->n_features = m->F; CUDA_CHECK(cudaSetDevice(m->ctx->device));
+      if (!b->p.interaction_sets.empty()) {   // sets_of[f] bit k: feature f is in set k
+        const int W = (int)((b->p.interaction_sets.size() + 63) / 64);
+        std::vector<unsigned long long> sets_of((size_t)m->F * W, 0ull);
+        for (size_t k = 0; k < b->p.interaction_sets.size(); ++k)
+          for (int64_t f : b->p.interaction_sets[k]) {
+            if (f >= m->F) fail("interaction_constraints: feature index %lld is out of range for %d features", (long long)f, m->F);
+            sets_of[(size_t)f * W + k / 64] |= 1ull << (k % 64);
+          }
+        upload(b->d_ic_sets_of, sets_of, m->ctx->stream);   // pageable source: staged before return
+        b->ic_words = W;
+      }
+    }
     else {  // prediction-only booster (model loaded with B2_BoosterAddTree)
       if (b->p.num_feature <= 0) fail("a booster without a train matrix needs num_feature=<n> in params");
       b->ctx = get_ctx(b->p.device); b->n_features = b->p.num_feature;

@@ -123,10 +123,16 @@ __device__ __forceinline__ void eval_node_cta(const long long* __restrict__ leve
   const int f = group_first[group] + slot;
   bool active = v_ok && slot < group_size[group] && !(is_cat && is_cat[f]);
   if (active && cs.level_mask) active = cs.level_mask[f] != 0;          // colsample_bytree / bylevel
-  if (cs.bynode < 1.0) {                                                // colsample_bynode: this node's own subset
-    if (threadIdx.x < kEvalSlots)
-      s_allowed[s] = active && b2_col_selected(cs.seed, cs.tree, B2_SCOPE_NODE(seg[node].nid), f, cs.level_mask, cs.fwq,
-                                               cs.n_features, b2_sample_count(cs.bynode, cs.n_level));
+  if (cs.bynode < 1.0 || cs.ic.sets_of) {   // colsample_bynode / interaction constraints: this node's own subset
+    if (threadIdx.x < kEvalSlots) {
+      const int nid = seg[node].nid;
+      bool ok = active;
+      if (ok && cs.bynode < 1.0)
+        ok = b2_col_selected(cs.seed, cs.tree, B2_SCOPE_NODE(nid), f, cs.level_mask, cs.fwq, cs.n_features,
+                             b2_sample_count(cs.bynode, cs.n_level));
+      if (ok && cs.ic.sets_of) ok = b2_interaction_allowed(cs.ic, nid, f);
+      s_allowed[s] = ok;
+    }
     __syncthreads();
     active = active && s_allowed[s];
   }
@@ -307,11 +313,17 @@ eval_splits_wide_kernel(const long long* __restrict__ level_hist, int n_groups, 
   const int f = group_first[group] + slot;
   bool active = v_ok && slot < group_size[group] && !(is_cat && is_cat[f]);
   if (active && cs.level_mask) active = cs.level_mask[f] != 0;          // colsample_bytree / bylevel
-  if (cs.bynode < 1.0) {                                                // colsample_bynode: this node's own subset
+  if (cs.bynode < 1.0 || cs.ic.sets_of) {   // colsample_bynode / interaction constraints: this node's own subset
     __shared__ uint8_t s_allowed[32];
-    if (q == 0)
-      s_allowed[s] = active && b2_col_selected(cs.seed, cs.tree, B2_SCOPE_NODE(seg[node].nid), f, cs.level_mask, cs.fwq,
-                                               cs.n_features, b2_sample_count(cs.bynode, cs.n_level));
+    if (q == 0) {
+      const int nid = seg[node].nid;
+      bool ok = active;
+      if (ok && cs.bynode < 1.0)
+        ok = b2_col_selected(cs.seed, cs.tree, B2_SCOPE_NODE(nid), f, cs.level_mask, cs.fwq, cs.n_features,
+                             b2_sample_count(cs.bynode, cs.n_level));
+      if (ok && cs.ic.sets_of) ok = b2_interaction_allowed(cs.ic, nid, f);
+      s_allowed[s] = ok;
+    }
     __syncthreads();
     active = active && s_allowed[s];
   }
@@ -457,12 +469,13 @@ eval_cat_splits_kernel(const long long* __restrict__ level_hist, int n_groups, c
     const int f = cat_feats[ci];
     const int fb = feat_byte[f], group = fb >> 5, slot = fb & 31;
     if ((slot & (shards - 1)) != shard_rank) continue;          // another rank owns this slot (uniform)
-    if (cs.level_mask || cs.bynode < 1.0) {                     // column sampling (uniform decision per feature)
+    if (cs.level_mask || cs.bynode < 1.0 || cs.ic.sets_of) {    // column sampling, interaction constraints (uniform per feature)
       if (b == 0) {
         bool ok = !cs.level_mask || cs.level_mask[f] != 0;
         if (ok && cs.bynode < 1.0)
           ok = b2_col_selected(cs.seed, cs.tree, B2_SCOPE_NODE(seg[node].nid), f, cs.level_mask, cs.fwq, cs.n_features,
                                b2_sample_count(cs.bynode, cs.n_level));
+        if (ok && cs.ic.sets_of) ok = b2_interaction_allowed(cs.ic, seg[node].nid, f);
         s_skip = ok ? 0 : 1;
       }
       __syncthreads();

@@ -9,6 +9,7 @@ This module is the import seam the reference keeps in ``xgboost_ray/xgb.py:1-11`
 There is NO CPU fallback: if the CUDA extension is not built or no H100 is visible, the first
 compute call raises ``XGBoostError``.
 """
+import ast
 import ctypes as C
 import json
 import os
@@ -585,7 +586,7 @@ _ENGINE_KEYS = ("objective", "num_class", "max_depth", "eta", "learning_rate", "
 # from the neutral one is an error, never silently ignored (a drop-in must not train a different model quietly)
 _UNSUPPORTED_NEUTRAL = {
     "sampling_method": ("uniform",), "max_leaves": (0,), "grow_policy": ("depthwise",),
-    "monotone_constraints": (None, "", "()", (), []), "interaction_constraints": (None, "", "[]", (), []),
+    "monotone_constraints": (None, "", "()", (), []),
     "multi_strategy": ("one_output_per_tree",), "refresh_leaf": (1, True), "process_type": ("default",),
     "updater": (None, "grow_quantile_histmaker", "grow_gpu_hist"),
 }
@@ -606,6 +607,45 @@ def _check_supported(params):
             if v not in neutral:
                 raise XGBoostError("parameter %s=%r is not supported by the H100 hist engine (supported: %s)"
                                    % (k, v, ", ".join(repr(x) for x in neutral[:4])))
+
+
+def interaction_sets(value, n_features, feature_names=None):
+    """xgboost's interaction_constraints in any accepted form -> list of sorted feature-index sets.
+
+    value: a string such as "[[0, 1], [2, 3, 4]]", or a list / tuple of iterables of integer indices (numpy integers
+    included) or of feature names (resolved against feature_names).  Duplicates inside a set are dropped, empty sets are
+    ignored; None, "", "[]" and [] give [] (no constraints).  A bad entry raises XGBoostError naming it."""
+    if value is None:
+        return []
+    if isinstance(value, str):
+        if not value.strip():
+            return []
+        try:
+            value = ast.literal_eval(value.strip())
+        except (ValueError, SyntaxError) as e:
+            raise XGBoostError("interaction_constraints=%r does not parse as a list of feature sets (%s)" % (value, e))
+    if isinstance(value, (str, bytes)) or not isinstance(value, (list, tuple)):
+        raise XGBoostError("interaction_constraints must be a list of feature sets, got %r" % (value,))
+    names = {str(n): i for i, n in enumerate(feature_names)} if feature_names is not None else {}
+    sets = []
+    for s in value:
+        if isinstance(s, (str, bytes)) or not hasattr(s, "__iter__"):
+            raise XGBoostError("interaction_constraints: %r is not a set of features" % (s,))
+        idx = set()
+        for f in s:
+            if isinstance(f, str):
+                if f not in names:
+                    raise XGBoostError("interaction_constraints: unknown feature name %r" % (f,))
+                f = names[f]
+            elif isinstance(f, (bool, np.bool_)) or not isinstance(f, (int, np.integer)):
+                raise XGBoostError("interaction_constraints: %r is not an integer feature index" % (f,))
+            f = int(f)
+            if not 0 <= f < n_features:
+                raise XGBoostError("interaction_constraints: feature index %d is outside [0, %d)" % (f, n_features))
+            idx.add(f)
+        if idx:
+            sets.append(sorted(idx))
+    return sets
 
 
 def _params_dict(params):
@@ -649,14 +689,23 @@ class Booster:
             p.update(extra)
         return "\n".join("%s=%s" % (k, v) for k, v in p.items()).encode()
 
+    def _interaction_sets(self, n_features=None, feature_names=None):
+        return interaction_sets(self.params.get("interaction_constraints"),
+                                self.n_features if n_features is None else n_features,
+                                self.feature_names if feature_names is None else feature_names)
+
     def _attach(self, dtrain):
         """Create the device booster bound to `dtrain` (quantising it if needed)."""
         old_trees = self.get_trees() if (self.handle or self._trees) else []
         self._free()
         dtrain._ensure_quantized(int(self.params.get("max_bin", 256)), cuts=self._cuts if old_trees else None)
         self._cuts = dtrain.get_cuts()
+        sets = self._interaction_sets(dtrain.num_col(),
+                                      self.feature_names if self.feature_names is not None else dtrain.feature_names)
+        # one param line: sets separated by ';', features by ','
+        extra = {"interaction_constraints": ";".join(",".join(map(str, s)) for s in sets)} if sets else None
         h = _H(0)
-        _check(lib().B2_BoosterCreate(self._param_text(), dtrain.handle, _coll.handle, C.byref(h)))
+        _check(lib().B2_BoosterCreate(self._param_text(extra), dtrain.handle, _coll.handle, C.byref(h)))
         self.handle = h.value
         self._train = dtrain
         self.n_features = dtrain.num_col()
@@ -965,8 +1014,12 @@ class Booster:
                                      _str_param(self.params.get(k, d)) if isinstance(d, str) else _num_str(self.params.get(k, d))
                                      for k, d in spec.block_params.items()}
         attrs = {k: str(v) for k, v in self._attrs.items() if not k.startswith("b2.")}
-        attrs["b2.params"] = json.dumps({k: self.params[k] for k in sorted(self.params) if _json_ok(self.params[k]) and
-                                         k not in ("objective", "num_class", "base_score", "scale_pos_weight", "num_parallel_tree")})   # those have their own fields
+        b2p = {k: self.params[k] for k in self.params if _json_ok(self.params[k]) and
+               k not in ("objective", "num_class", "base_score", "scale_pos_weight", "num_parallel_tree")}   # those have their own fields
+        sets = self._interaction_sets() if self.n_features is not None else []
+        if sets:   # in its resolved string form, which also keeps list / feature-name / numpy inputs
+            b2p["interaction_constraints"] = str(sets)
+        attrs["b2.params"] = json.dumps({k: b2p[k] for k in sorted(b2p)})
         attrs["b2.split_bins"] = json.dumps([c[1] for c in cache], separators=(",", ":"))
         return {
             "learner": {
@@ -1089,7 +1142,11 @@ class Booster:
         return b
 
     def save_config(self):
-        return json.dumps({"learner": {"gradient_booster": {"name": "gbtree"},
+        gbtree = {"name": "gbtree"}
+        sets = self._interaction_sets() if self.n_features is not None else []
+        if sets:
+            gbtree["tree_train_param"] = {"interaction_constraints": str(sets)}
+        return json.dumps({"learner": {"gradient_booster": gbtree,
                                        "objective": {"name": self.params.get("objective", "reg:squarederror")},
                                        "b2_params": {k: v for k, v in self.params.items() if _json_ok(v)}},
                            "version": [2, 0, 3]})

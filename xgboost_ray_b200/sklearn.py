@@ -17,7 +17,7 @@ from xgboost_ray_b200.matrix import RayDMatrix
 _PARAM_NAMES = ("max_depth", "learning_rate", "gamma", "min_child_weight", "reg_lambda", "reg_alpha", "max_bin",
                 "base_score", "tree_method", "subsample", "colsample_bytree", "colsample_bylevel", "colsample_bynode",
                 "scale_pos_weight", "max_delta_step", "max_cat_to_onehot", "max_cat_threshold", "eval_metric",
-                "tweedie_variance_power", "huber_slope")
+                "tweedie_variance_power", "huber_slope", "interaction_constraints")
 
 
 def _check_if_params_are_ray_dmatrix(X, sample_weight, base_margin, eval_set):
@@ -45,7 +45,8 @@ class RayXGBMixin(BaseEstimator):
                  max_delta_step: Optional[float] = None, max_cat_to_onehot: Optional[int] = None,
                  max_cat_threshold: Optional[int] = None, enable_categorical: bool = False, missing: float = np.nan,
                  eval_metric=None, early_stopping_rounds: Optional[int] = None, callbacks=None,
-                 tweedie_variance_power: Optional[float] = None, huber_slope: Optional[float] = None):
+                 tweedie_variance_power: Optional[float] = None, huber_slope: Optional[float] = None,
+                 interaction_constraints=None):
         self.n_estimators = n_estimators
         self.max_depth = max_depth
         self.learning_rate = learning_rate
@@ -74,6 +75,7 @@ class RayXGBMixin(BaseEstimator):
         self.callbacks = callbacks
         self.tweedie_variance_power = tweedie_variance_power   # reg:tweedie rho in [1, 2); None = 1.5
         self.huber_slope = huber_slope                         # reg:pseudohubererror delta > 0; None = 1
+        self.interaction_constraints = interaction_constraints   # feature sets, e.g. "[[0, 1], [2, 3, 4]]"; None = off
 
     def get_xgb_params(self):
         p = {k: getattr(self, k) for k in _PARAM_NAMES if getattr(self, k) is not None}
