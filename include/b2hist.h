@@ -26,9 +26,6 @@ typedef uint64_t B2Handle;
 
 const char* B2_GetLastError(void);
 int B2_GetVersion(void);
-/* process-wide engine options (the environment variables of the same name in upper case with a B2_ prefix are their
- * defaults): "hist_narrow" = "0" | "1" -- feature-group layout of matrices quantised from now on (DESIGN.md 4.1). */
-int B2_SetOption(const char* key, const char* value);
 int B2_DeviceCount(int* out);
 
 /* ---- communicator: replaces the Rabit bridge.

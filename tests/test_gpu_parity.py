@@ -35,76 +35,67 @@ def make_data(n, f, seed, kind="uniform", nan_frac=0.0):
 
 
 # ------------------------------------------------------------------ histogram kernel (a10)
-# with B2_HIST_NARROW=1 F = 32 a + r, 0 < r <= 16 puts the r leftover features into a NARROW last group (one lane per row,
-# pow2ceil(r) steps, 32 / w shared-memory replicas): widths 1, 2, 4, 8, 16 alone and behind full groups are all covered
-@pytest.mark.parametrize("narrow", [0, 1])
+@pytest.mark.parametrize("gather", [False, True])   # root rows / every row through a permutation of the row ids
 @pytest.mark.parametrize("n,f", [(1, 1), (17, 3), (1000, 28), (5000, 100), (3000, 50), (2000, 200), (4097, 33),
                                  (3001, 2), (2500, 34), (3000, 12), (777, 16), (2000, 48), (1500, 7), (6000, 104),
                                  (1500, 800)])   # more groups than the pair plan holds: one group per CTA
-def test_hist_kernel_bit_exact(eng, oracle, n, f, narrow):
+def test_hist_kernel_bit_exact(eng, oracle, n, f, gather):
     rng = np.random.RandomState(n + f)
     bins = rng.randint(0, 256, size=(n, f)).astype(np.uint8)
     qg = rng.randint(-(1 << 18), 1 << 18, size=n).astype(np.int32)
     qh = rng.randint(0, 1 << 18, size=n).astype(np.int32)
-    ref = oracle.hist_int(bins, qg, qh)
-    got, _ = eng.hist_build_raw(bins, qg, qh, window_rows=4096, chunk_rows=512, narrow=narrow)
+    ridx = rng.permutation(n).astype(np.int32) if gather else None
+    ref = oracle.hist_int(bins, qg, qh, ridx)
+    got, _ = eng.hist_build_raw(bins, qg, qh, ridx=ridx, window_rows=4096, chunk_rows=512)
     assert np.array_equal(ref, got)
 
 
 def test_hist_kernel_adversarial_and_windows(eng, oracle):
-    n, f = 20000, 37
-    rng = np.random.RandomState(7)
-    bins = rng.randint(0, 256, size=(n, f)).astype(np.uint8)
-    bins[:, 0] = 9          # constant feature: every row hits the same cell
-    bins[:, 1] = bins[:, 1] & 1   # binary feature
-    bins[:, 2] = 255
-    qg = np.full(n, (1 << 18), np.int32)     # extreme values: the guard interval for 18 bits is 2^12 rows
-    qg[::2] = -(1 << 18)
-    qg[: n // 2] = (1 << 18)                 # long same-sign runs on the constant feature: its cell saturates
-    qh = np.full(n, (1 << 18), np.int32)
-    ref = oracle.hist_int(bins, qg, qh)
-    for window, chunk in ((4096, 512), (1024, 256), (4096, 4096), (4096, 8192)):
-        got, _ = eng.hist_build_raw(bins, qg, qh, window_rows=window, chunk_rows=chunk)
-        assert np.array_equal(ref, got), (window, chunk)
+    n = 20000
+    for f in (37, 530):   # 2 groups (one group-pair CTA type); 17 groups (one group per CTA)
+        rng = np.random.RandomState(7)
+        bins = rng.randint(0, 256, size=(n, f)).astype(np.uint8)
+        bins[:, 0] = 9          # constant feature: every row hits the same cell
+        bins[:, 1] = bins[:, 1] & 1   # binary feature
+        bins[:, 2] = 255
+        qg = np.full(n, (1 << 18), np.int32)     # extreme values: the guard interval for 18 bits is 2^12 rows
+        qg[::2] = -(1 << 18)
+        qg[: n // 2] = (1 << 18)                 # long same-sign runs on the constant feature: its cell saturates
+        qh = np.full(n, (1 << 18), np.int32)
+        ref = oracle.hist_int(bins, qg, qh)
+        for window, chunk in ((4096, 512), (1024, 256), (4096, 4096), (4096, 8192)):
+            got, _ = eng.hist_build_raw(bins, qg, qh, window_rows=window, chunk_rows=chunk)
+            assert np.array_equal(ref, got), (f, window, chunk)
 
 
 def test_hist_kernel_gather(eng, oracle):
-    n, f = 30000, 100
-    rng = np.random.RandomState(11)
-    bins = rng.randint(0, 256, size=(n, f)).astype(np.uint8)
-    qg = rng.randint(-1000, 1000, size=n).astype(np.int32)
-    qh = rng.randint(0, 1000, size=n).astype(np.int32)
-    for nsel in (0, 1, 15, 16, 17, 4999, 30000):
-        ridx = rng.permutation(n)[:nsel].astype(np.int32)
-        ref = oracle.hist_int(bins, qg, qh, ridx) if nsel else np.zeros((f, 256, 2), np.int64)
-        got, _ = eng.hist_build_raw(bins, qg, qh, ridx=ridx, window_rows=4096, chunk_rows=1024)
-        assert np.array_equal(ref, got), nsel
+    n = 30000
+    for f in (100, 530):   # 4 groups (two group-pair CTA types); 17 groups (one group per CTA)
+        rng = np.random.RandomState(11)
+        bins = rng.randint(0, 256, size=(n, f)).astype(np.uint8)
+        qg = rng.randint(-1000, 1000, size=n).astype(np.int32)
+        qh = rng.randint(0, 1000, size=n).astype(np.int32)
+        for nsel in (0, 1, 15, 16, 17, 4999, 30000):
+            ridx = rng.permutation(n)[:nsel].astype(np.int32)
+            ref = oracle.hist_int(bins, qg, qh, ridx) if nsel else np.zeros((f, 256, 2), np.int64)
+            got, _ = eng.hist_build_raw(bins, qg, qh, ridx=ridx, window_rows=4096, chunk_rows=1024)
+            assert np.array_equal(ref, got), (f, nsel)
 
 
-def test_hist_kernel_variants_bit_exact(oracle):
-    """Every kernel variant (TMA-staged rows; 3x8 / 2x16 warps with one group per CTA; 32 warps with two groups
-    per CTA) produces the same integers."""
-    import os
-    import subprocess
-    import sys
-    code = (
-        "import numpy as np, sys; sys.path.insert(0, %r)\n"
-        "from xgboost_ray_b200 import engine as E\n"
-        "from oracle import oracle as O\n"
-        "rng = np.random.RandomState(3); n = 70001\n"
-        "qg = rng.randint(-(1 << 18), 1 << 18, size=n).astype(np.int32); qh = rng.randint(0, 1 << 18, size=n).astype(np.int32)\n"
-        "sel = np.sort(rng.choice(n, 33333, replace=False)).astype(np.int32)\n"
-        "for f in (100, 70, 17, 96, 105, 112):\n"   # 4, 3 (odd: a half-empty CTA in the two-group variant) and 1 feature groups; 96..112: the all-groups-per-CTA kernel
-        "    bins = rng.randint(0, 256, size=(n, f)).astype(np.uint8)\n"
-        "    for ridx in (None, sel):\n"
-        "        ref = O.hist_int(bins, qg, qh, ridx); got, _ = E.hist_build_raw(bins, qg, qh, ridx=ridx, window_rows=4096, chunk_rows=2048)\n"
-        "        assert np.array_equal(ref, got), (f, ridx is None)\n"
-        "print('variant ok')\n") % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    for env in ({"B2_HIST_TMA": "1"}, {"B2_HIST_VARIANT": "0"}, {"B2_HIST_VARIANT": "1"}, {"B2_HIST_VARIANT": "2"},
-                {"B2_HIST_VARIANT": "3"}, {"B2_HIST_VARIANT": "4"}, {"B2_HIST_ALIGNED": "1"}, {"B2_HIST_NARROW": "1"},
-                {"B2_HIST_NARROW": "1", "B2_HIST_ALIGNED": "1"}, {"B2_HIST_VARIANT": "2", "B2_HIST_NARROW": "1"}):
-        r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, **env), capture_output=True, text=True, timeout=300)
-        assert r.returncode == 0 and "variant ok" in r.stdout, (env, r.stdout[-500:], r.stderr[-1500:])
+def test_hist_kernel_variants_bit_exact(eng, oracle):
+    """Feature-group counts 4, 3 (odd: a half-empty group pair), 1, 3, 4 and 4 on 70,001 rows in 2,048-row chunks with
+    a 4,096-row window, at the root and through a sorted half of the rows."""
+    rng = np.random.RandomState(3)
+    n = 70001
+    qg = rng.randint(-(1 << 18), 1 << 18, size=n).astype(np.int32)
+    qh = rng.randint(0, 1 << 18, size=n).astype(np.int32)
+    sel = np.sort(rng.choice(n, 33333, replace=False)).astype(np.int32)
+    for f in (100, 70, 17, 96, 105, 112):
+        bins = rng.randint(0, 256, size=(n, f)).astype(np.uint8)
+        for ridx in (None, sel):
+            ref = oracle.hist_int(bins, qg, qh, ridx)
+            got, _ = eng.hist_build_raw(bins, qg, qh, ridx=ridx, window_rows=4096, chunk_rows=2048)
+            assert np.array_equal(ref, got), (f, ridx is None)
 
 
 # ------------------------------------------------------------------ cuts and bins (a7, a8)

@@ -9,10 +9,6 @@ the split scan, the level decision and the gathering leaf path at 4,096-8,192 no
 Tolerance: trees are compared exactly (topology, splits, default directions, loss_chg); leaf values, margins and
 predictions within 1e-5, except where a test says bit for bit.  Device memory: depth 14 keeps 2 GiB of level
 histograms per feature group, so every deep case uses at most 16 features (one group)."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
@@ -23,7 +19,6 @@ from tests.test_oracle_quantisation import (binade_bounds, grow_tiny_hessian, qu
 pytestmark = pytest.mark.gpu
 
 F = np.float32
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
@@ -35,16 +30,16 @@ def eng():
 
 
 # ------------------------------------------------------------------ histogram kernel at the window edges (a10)
-def window_edge_cases():
-    """(label, bins, qg, qh, ridx, window, chunk) at qbits 22-24: |q| = 2^qbits exactly, and on the constant feature 0
-    a run of window rows of +2^qbits (cell exactly 2^30 at the window boundary), a run of 2^qbits - 1 that leaves the
-    cell just below 2^30 at the check followed by a full window of +2^qbits (the cell reaches 2^31 - window), and the
-    same runs negated"""
+def window_edge_cases(f):
+    """(label, bins, qg, qh, ridx, window, chunk) of f features at qbits 22-24: |q| = 2^qbits exactly, and on the
+    constant feature 0 a run of window rows of +2^qbits (cell exactly 2^30 at the window boundary), a run of
+    2^qbits - 1 that leaves the cell just below 2^30 at the check followed by a full window of +2^qbits (the cell
+    reaches 2^31 - window), and the same runs negated"""
     for qbits in (22, 23, 24):
         window = 1 << (30 - qbits)
         top = 1 << qbits
         rng = np.random.RandomState(qbits)
-        n, f = 9 * window + 3000, 37
+        n = 9 * window + 3000
         bins = rng.randint(0, 256, size=(n, f)).astype(np.uint8)
         bins[:, 0] = 7
         bins[:, 1] &= 1
@@ -60,33 +55,13 @@ def window_edge_cases():
                 yield (qbits, chunk, None if ridx is None else ridx.size), bins, qg, qh, ridx, window, chunk
 
 
-def check_window_edges(E, O, narrow=None):
-    for label, bins, qg, qh, ridx, window, chunk in window_edge_cases():
-        ref = O.hist_int(bins, qg, qh, ridx)
+@pytest.mark.parametrize("f", [37, 530])   # 2 groups (one group-pair CTA type); 17 groups (one group per CTA)
+def test_hist_window_edges_bit_exact(eng, oracle, f):
+    for label, bins, qg, qh, ridx, window, chunk in window_edge_cases(f):
+        ref = oracle.hist_int(bins, qg, qh, ridx)
         assert ref[0, 7, 0] == int(qg.astype(np.int64)[ridx if ridx is not None else slice(None)].sum())
-        got, _ = E.hist_build_raw(bins, qg, qh, ridx=ridx, window_rows=window, chunk_rows=chunk, narrow=narrow)
+        got, _ = eng.hist_build_raw(bins, qg, qh, ridx=ridx, window_rows=window, chunk_rows=chunk)
         assert np.array_equal(ref, got), label
-
-
-@pytest.mark.parametrize("narrow", [0, 1])
-def test_hist_window_edges_bit_exact(eng, oracle, narrow):
-    check_window_edges(eng, oracle, narrow)
-
-
-def test_hist_window_edges_every_variant(oracle):
-    """The same cases through every environment-selected kernel (the choice is read once per process)."""
-    code = ("import sys; sys.path.insert(0, %r)\n"
-            "from xgboost_ray_b200 import engine as E\n"
-            "from oracle import oracle as O\n"
-            "from tests.test_gpu_qbits_depth import check_window_edges\n"
-            "check_window_edges(E, O)\n"
-            "print('variant ok')\n") % ROOT
-    for env in ({"B2_HIST_TMA": "1"}, {"B2_HIST_VARIANT": "0"}, {"B2_HIST_VARIANT": "1"}, {"B2_HIST_VARIANT": "2"},
-                {"B2_HIST_VARIANT": "3"}, {"B2_HIST_VARIANT": "4"}, {"B2_HIST_ALIGNED": "1"}, {"B2_HIST_NARROW": "1"},
-                {"B2_HIST_NARROW": "1", "B2_HIST_ALIGNED": "1"}, {"B2_HIST_VARIANT": "2", "B2_HIST_NARROW": "1"}):
-        r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, **env), capture_output=True, text=True,
-                           timeout=300)
-        assert r.returncode == 0 and "variant ok" in r.stdout, (env, r.stdout[-500:], r.stderr[-1500:])
 
 
 def test_hist_qbits8_window_of_four_million_rows(eng, oracle):

@@ -12,9 +12,6 @@ Device memory: the level histograms take 2 * 2^(D-1) * G * 128 KiB at depth D, s
 (2 GiB of histograms there) and depth 6 at F = 4300 (1.06 GiB).  With the bin matrix, the raw rows and the CUDA
 context the largest case peaked at 2,650 MiB of device memory on an H100 (DESIGN.md §7)."""
 import ctypes as C
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -23,8 +20,6 @@ from tests import shap_reference as R
 from tests.test_gpu_parity import LEAF_TOL, assert_same_model, run_both
 
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
@@ -291,52 +286,16 @@ def test_interactions_wide(eng):
     assert (split_features(bst) >= 513).any()
 
 
-# ------------------------------------------------------------------ histogram kernel variants through training
-VARIANT_CODE = r"""
-import sys, numpy as np
-sys.path.insert(0, %(root)r)
-from xgboost_ray_b200 import engine as E
-d = np.load(%(data)r)
-for F in %(widths)r:
-    X, y = d["X%%d" %% F], d["y%%d" %% F]
-    bst = E.train(%(params)r, E.DMatrix(X, label=y), num_boost_round=3, verbose_eval=False)
-    np.savez(%(out)r %% F, **{"%%d_%%s" %% (i, k): v for i, t in enumerate(bst.get_trees()) for k, v in t.items()})
-print("variant ok")
-"""
-
-
-class _Saved:
-    def __init__(self, path):
-        z = np.load(path)
-        n = 1 + max(int(k.split("_", 1)[0]) for k in z.files)
-        self.trees = [{k.split("_", 1)[1]: z[k] for k in z.files if int(k.split("_", 1)[0]) == i} for i in range(n)]
-
-    def get_trees(self):
-        return self.trees
-
-
-def test_hist_variants_through_training(oracle, tmp_path):
-    """The one-group-per-CTA kernels (256 / 512 threads), the two-groups-per-CTA kernel at an even (F = 1000) and an
-    odd (F = 990) group count and the TMA-staged root level all train the oracle's trees at these widths."""
+# ------------------------------------------------------------------ one-group-per-CTA histogram kernel through training
+def test_hist_variants_through_training(eng, oracle):
+    """The one-group-per-CTA histogram kernel at an even (F = 1000, 32 groups) and an odd (F = 990, 31 groups) group
+    count trains the oracle's trees."""
     params = {"objective": "reg:squarederror", "max_depth": 6, "eta": 0.3, "base_score": 0.5}
-    widths = (1000, 990)
-    arrays, ref = {}, {}
-    for F in widths:
+    for F in (1000, 990):
         X, rng = wide_X(12000, F, 400 + F, nan_frac=0.02)
         y, _ = wide_label(X, "reg:squarederror", rng)
-        arrays["X%d" % F], arrays["y%d" % F] = X, y
-        ref[F], _ = oracle.train(params, X, y, 3)
-    data = str(tmp_path / "data.npz")
-    np.savez(data, **arrays)
-    for env in ({"B2_HIST_VARIANT": "0"}, {"B2_HIST_VARIANT": "1"}, {"B2_HIST_VARIANT": "2"}, {"B2_HIST_TMA": "1"}):
-        tag = "_".join("%s%s" % kv for kv in env.items())
-        out = str(tmp_path / (tag + "_%d.npz"))
-        code = VARIANT_CODE % {"root": ROOT, "data": data, "widths": widths, "params": params, "out": out}
-        r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, **env), capture_output=True, text=True,
-                           timeout=600)
-        assert r.returncode == 0 and "variant ok" in r.stdout, (env, r.stdout[-500:], r.stderr[-1500:])
-        for F in widths:
-            assert_same_model(_Saved(out % F), ref[F])
+        ebst, obst, _ = run_both(eng, oracle, params, X, y, 3)
+        assert_same_model(ebst, obst)
 
 
 # ------------------------------------------------------------------ two GPUs: feature-slot sharding at width

@@ -1,10 +1,8 @@
 """CPU restatement of the shared-memory addressing of the histogram kernels (csrc/hist_common.cuh::accumulate_row,
-hist_kernel.cu::full_pass / narrow_pass / narrow_pass16 / row_pass_v4): at every step the 32 lanes of a warp must address
+hist_kernel.cu::full_pass with one or two feature groups per CTA): at every step the 32 lanes of a warp must address
 32 different banks for ANY bin values (one wavefront per red.shared.add), and every (row, feature) pair must be added
 exactly once to the cell of its (bin, plane, feature slot).  The GPU suite proves the sums; this pins the bank layout the
 design (DESIGN.md 4.1) rests on: one wavefront per shared atomic instruction."""
-import itertools
-
 import numpy as np
 import pytest
 
@@ -44,59 +42,3 @@ def test_full_groups_are_bank_conflict_free_and_complete(groups_per_cta):
         assert len(set(banks)) == 32, (j, sorted(banks))
         assert len({bank(a + 128) for a in banks}) <= 32                    # the h plane is 128 B further: same banks, next instruction
     assert len(seen) == rows_per_warp * groups_per_cta * 32                # every (row, group, feature) exactly once
-
-
-@pytest.mark.parametrize("w", [1, 2, 4, 8, 16])
-def test_narrow_group_replicas_are_bank_conflict_free(w):
-    """narrow_pass: lane = row, 32 / w replicas of the w slots side by side in the 32-slot layout"""
-    rng = np.random.RandomState(w)
-    bins = rng.randint(0, 256, size=(32, w))
-    seen = set()
-    for j in range(w):
-        banks = []
-        for lane in range(32):
-            rot, rep = lane & (w - 1), lane // w
-            slot = (j + rot) & (w - 1)
-            addr = int(bins[lane, slot]) * 256 + (rep * w + slot) * 4
-            banks.append(bank(addr))
-            seen.add((lane, slot))
-        assert len(set(banks)) == 32
-    assert len(seen) == 32 * w
-
-
-@pytest.mark.parametrize("w", [1, 2, 4, 8, 16])
-def test_narrow16_block_two_lanes_per_bank(w):
-    """narrow_pass16 (kernel v4, leftovers wider than 4): [256][2][16] block, lanes l and l + 16 share a bank"""
-    for j in range(w):
-        banks = {}
-        for lane in range(32):
-            rot, rep = lane & (w - 1), (lane // w) & (16 // w - 1)
-            slot = (j + rot) & (w - 1)
-            for b in (0, 255):
-                addr = b * 128 + (rep * w + slot) * 4
-                assert (addr >> 2) % 32 // 16 == 0 and addr + 64 < 256 * 128       # g plane in banks 0..15, h plane 64 B further
-            banks.setdefault(rep * w + slot, []).append(lane)
-        assert sorted(len(v) for v in banks.values()) == [2] * 16
-
-
-@pytest.mark.parametrize("w", [0, 1, 2, 4])
-def test_v4_row_pass_banks(w):
-    """row_pass_v4: lane pair = row, three full groups then the even lane's w narrow features (16 lanes -> 16 banks)"""
-    for g, j in itertools.product(range(3), range(16)):
-        banks = set()
-        for lane in range(32):
-            sub, half = lane >> 1, lane & 1
-            banks.add(bank(g * GROUP_BYTES + half * 64 + 37 * 256 + ((j + sub) & 15) * 4))
-        assert len(banks) == 32
-    if w:
-        covered = set()
-        for j in range(w):
-            banks = []
-            for lane in range(0, 32, 2):                        # even lanes only
-                sub = lane >> 1
-                nrot, rep = sub & (w - 1), (sub // w) & (16 // w - 1)
-                idx = (j + nrot) & (w - 1)
-                banks.append(bank(3 * GROUP_BYTES + 201 * 128 + (rep * w + idx) * 4))
-                covered.add((sub, idx))
-            assert len(set(banks)) == 16
-        assert len(covered) == 16 * w

@@ -19,7 +19,6 @@ COMMON = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=
           "-Xcompiler", "-fPIC,-ffp-contract=off", "-ccbin", "/usr/bin/g++"]
 SOURCES = {
     "hist_kernel.cu": [],
-    "hist_tma_kernel.cu": [],
     "split_kernel.cu": ["--fmad=false"],
     "partition_kernel.cu": ["--fmad=false"],
     "control_kernel.cu": ["--fmad=false"],

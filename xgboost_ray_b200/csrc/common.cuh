@@ -61,16 +61,6 @@ struct B2HistWork {
   int32_t chunk_begin;  // exclusive prefix sum of ceil(seg_count / chunk_rows)
 };
 
-// CTA plan of the histogram kernel: a CTA type owns one PAIR of feature groups (2 x 64 KiB of shared memory); its
-// share of the persistent grid is proportional to the shared-atomic wavefronts the pair costs per row, because the last
-// group may be NARROW (w <= 16 features, processed one lane per row in w steps instead of two lanes in 16).
-#define B2_HIST_MAX_TYPES 8
-struct B2HistPlan {
-  int32_t n_types;
-  int32_t cta_begin[B2_HIST_MAX_TYPES + 1];   // type t owns CTAs [cta_begin[t], cta_begin[t+1])
-  int32_t narrow_w;                           // width of the last group if it is narrow (power of two <= 16), else 0
-};
-
 // per-split-node descriptor for the row partition kernel
 struct B2SplitWork {
   int32_t seg_begin, seg_count;

@@ -34,10 +34,7 @@
 // ---------------------------------------------------------------- kernel launchers (other TUs)
 extern "C" {
 int b2_launch_hist(const uint8_t*, int, const int2*, const int32_t*, const B2HistWork*, int, int, int, int, int, long long*,
-                   const B2LevelCtl*, int, int, int, int, cudaStream_t);
-int b2_make_bins_tensor_map(void*, const uint8_t*, int64_t, int, int);
-int b2_launch_hist_tma(const uint8_t*, int, const void*, const int2*, const int32_t*, const B2HistWork*, int, int, int, int, int, long long*,
-                       const B2LevelCtl*, int, int, int64_t, int, cudaStream_t);
+                   const B2LevelCtl*, int, int, int, cudaStream_t);
 int b2_launch_hist_subtract(const long long*, long long*, const int32_t*, int, int64_t, const B2LevelCtl*, cudaStream_t);
 int b2_launch_eval_splits(const long long*, int, const B2EvalNode*, int, const int32_t*, const int32_t*, const int32_t*,
                           const uint8_t*, const uint8_t*, const int32_t*, int, B2TrainParamDev, B2SplitCand*, int, const B2LevelCtl*,
@@ -50,7 +47,6 @@ int b2_launch_p2p_reduce_subtract(const void*, const long long*, long long*, con
                                   cudaStream_t);
 int b2_launch_p2p_quant_exponent(const void*, const uint32_t*, int32_t*, cudaStream_t);
 int b2_launch_p2p_leaf_sums(const void*, const int32_t*, long long*, cudaStream_t);
-int b2_hist_variant();
 int b2_launch_p2p_close(const void*, cudaStream_t);
 int b2_launch_gather_interleaved_rows(const void*, float*, int, cudaStream_t);
 int b2_launch_final_assign(const uint8_t*, int64_t, const int32_t*, const B2SplitWork*, const B2LevelCtl*, int, const float2*,
@@ -485,13 +481,10 @@ struct Matrix : HandleBase {
   DevBuf<float> raw;     // [n][F], optional
   bool has_raw = false;
   DevBuf<uint8_t> bins;  // [n][row_stride]
-  alignas(64) unsigned char tmap_tile[128];   // TMA tensor map over bins, box {32 B, 64 rows}, for the contiguous root stage
-  bool has_tmap = false;
   DevBuf<uint8_t> bins_col;  // [F][col_stride] feature-major copy for the row partition
   int64_t col_stride = 0;
   bool quantized = false;
   int n_groups = 0, row_stride = 0, max_bin = 0;
-  int narrow_w = 0;                   // > 0: the last group is narrow (<= 16 features, width rounded up to a power of two)
   std::vector<int32_t> group_first, group_size, feat_byte;
   std::vector<int32_t> cut_ptrs;
   std::vector<float> cut_vals, min_vals;
@@ -519,34 +512,23 @@ struct Matrix : HandleBase {
   DevBuf<uint32_t> d_fwq;
 };
 
-// Feature -> (group, slot) layout of the bin matrix.  Default: the features are spread EVENLY over ceil(F / 32) groups, so
-// that every CTA type of the histogram kernel (one pair of groups) costs the same and the types walk the chunk list in
-// lock step -- the CTAs that read the two 64-byte halves of a row do it at the same time and the row is fetched from
-// DRAM once.  B2_HIST_NARROW=1 selects the layout "a full groups + one NARROW group of the r = F mod 32 <= 16 leftover
-// features" (one lane per row, pow2ceil(r) steps; hist_kernel.cu v3).  It removes the padding-slot atomics (F = 100:
-// 6.25 instead of 8 wavefronts per row) but the CTA types then cost 4 : 2.25 and drift apart, so the two halves of a
-// row are no longer read together and DRAM traffic grows.  Kept as an opt-in, parity-tested variant.
-int g_hist_narrow = -1;   // -1: read B2_HIST_NARROW on first use; B2_SetOption("hist_narrow", ...) overrides it
+// Feature -> (group, slot) layout of the bin matrix: the features are spread EVENLY over ceil(F / 32) groups, so that
+// every CTA type of the histogram kernel (one pair of groups) costs the same and the types walk the chunk list in lock
+// step -- the CTAs that read the two 64-byte halves of a row do it at the same time and the row is fetched from DRAM
+// once.  (Packing the F mod 32 leftover features into a narrow last group saves padding-slot atomics, but the types then
+// differ in cost, drift apart and read the halves of a row at different times; DESIGN.md 4.1.)
 void setup_groups(Matrix* m) {
   const int F = m->F;
-  if (g_hist_narrow < 0) { const char* e = getenv("B2_HIST_NARROW"); g_hist_narrow = (e && atoi(e) != 0) ? 1 : 0; }
-  const int narrow_on = g_hist_narrow;
   m->n_groups = (F + B2_GROUP_SLOTS - 1) / B2_GROUP_SLOTS;
   if (m->n_groups < 1) m->n_groups = 1;
   m->row_stride = m->n_groups * B2_GROUP_SLOTS;
   m->group_first.assign(m->n_groups, 0);
   m->group_size.assign(m->n_groups, 0);
   m->feat_byte.assign(F, 0);
-  m->narrow_w = 0;
-  const int r = F % B2_GROUP_SLOTS;
-  // kernel v4 (all groups of a row in one CTA) wants three full groups + a narrow leftover group
-  const bool v4_layout = b2_hist_variant() == 4 && F > 96 && F <= 112;
-  const bool narrow = (narrow_on || v4_layout) && r > 0 && r <= 16;
-  if (narrow) { m->narrow_w = 1; while (m->narrow_w < r) m->narrow_w <<= 1; }
   const int base = F / m->n_groups, rem = F % m->n_groups;
   int f = 0;
   for (int g = 0; g < m->n_groups; ++g) {
-    const int sz = narrow ? (g + 1 < m->n_groups ? B2_GROUP_SLOTS : r) : base + (g < rem ? 1 : 0);
+    const int sz = base + (g < rem ? 1 : 0);
     m->group_first[g] = f; m->group_size[g] = sz;
     for (int s = 0; s < sz; ++s) m->feat_byte[f + s] = g * B2_GROUP_SLOTS + s;
     f += sz;
@@ -718,7 +700,6 @@ void bin_matrix(Matrix* m) {
                              m->any_cat() ? m->d_is_cat.p : nullptr, m->row_stride, m->bins.p, m->bins_col.p, m->col_stride,
                              ctx->num_sms, s));
   CUDA_CHECK(cudaStreamSynchronize(s));
-  m->has_tmap = b2_make_bins_tensor_map(m->tmap_tile, m->bins.p, m->n, m->row_stride, 64) == 0;
   m->quantized = true;
 }
 
@@ -1343,11 +1324,6 @@ void record_hist_launch(Booster* b, TreeStats& st, cudaEvent_t& e0, cudaEvent_t&
   }
 }
 
-bool use_tma_hist() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("B2_HIST_TMA"); v = (e && atoi(e) != 0) ? 1 : 0; }
-  return v == 1;
-}
 bool env_flag(const char* name, bool dflt) {
   const char* e = getenv(name);
   return e ? atoi(e) != 0 : dflt;
@@ -1478,12 +1454,8 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
     if (n > 0) {
       cudaEvent_t e0 = nullptr, e1 = nullptr;
       record_hist_launch(b, st, e0, e1, true);
-      if (use_tma_hist() && m->has_tmap)
-        LAUNCH_CHECK(b2_launch_hist_tma(m->bins.p, m->row_stride, m->tmap_tile, b->q.p, nullptr, b->d_hist_work.p, 1, chunks, chunk_rows, window, G,
-                                        build_target(b, b->hist[0].p), nullptr, sh, 1, n, ctx->num_sms, s));
-      else
-        LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, b->q.p, nullptr, b->d_hist_work.p, 1, chunks, chunk_rows, window, G,
-                                    build_target(b, b->hist[0].p), nullptr, sh, 1, m->narrow_w, ctx->num_sms, s));
+      LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, b->q.p, nullptr, b->d_hist_work.p, 1, chunks, chunk_rows, window, G,
+                                  build_target(b, b->hist[0].p), nullptr, sh, 1, ctx->num_sms, s));
       record_hist_launch(b, st, e0, e1, false);
       st.hist_launches++; st.kernel_launches++;
     }
@@ -1594,12 +1566,8 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
       CUDA_CHECK(cudaMemsetAsync(tgt, 0, (size_t)max_nodes_level * b->node_elems * sizeof(long long), s));
       cudaEvent_t e0 = nullptr, e1 = nullptr;
       record_hist_launch(b, st, e0, e1, true);
-      if (use_tma_hist() && m->has_tmap)
-        LAUNCH_CHECK(b2_launch_hist_tma(m->bins.p, m->row_stride, m->tmap_tile, b->q.p, b->ridx[nxt].p, b->d_hist_work.p, 0, 0, 0, window, G, tgt, ctl + nxt, sh,
-                                        max_nodes_level, n, ctx->num_sms, s));
-      else
-        LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, b->q.p, b->ridx[nxt].p, b->d_hist_work.p, 0, 0, 0, window, G, tgt,
-                                    ctl + nxt, sh, max_nodes_level, m->narrow_w, ctx->num_sms, s));
+      LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, b->q.p, b->ridx[nxt].p, b->d_hist_work.p, 0, 0, 0, window, G, tgt,
+                                  ctl + nxt, sh, max_nodes_level, ctx->num_sms, s));
       record_hist_launch(b, st, e0, e1, false);
       st.hist_launches++; st.kernel_launches++;
       mark_phase(b, 1);
@@ -1668,7 +1636,7 @@ void run_tree(Booster* b, int k, int slot) {
   prepare_tree_buffers(b, slot);
   static const bool want_graph = env_flag("B2_GRAPH", true);
   const bool eligible = want_graph && !b->graph_failed && b->absmax_fused && p.subsample >= 1.0f && !p.use_cols() &&
-                        p.profile < 2 && !use_tma_hist() && p.num_parallel_tree == 1;
+                        p.profile < 2 && p.num_parallel_tree == 1;
   auto direct = [&]() {
     TreeStats st;
     grow_tree(b, k, slot, st);
@@ -2236,13 +2204,6 @@ float* eval_margin(Booster* b, Matrix* m) {
 extern "C" {
 
 const char* B2_GetLastError(void) { return g_last_error.c_str(); }
-int B2_SetOption(const char* key, const char* value) {
-  API_BEGIN
-  std::string k(key ? key : ""), v(value ? value : "");
-  if (k == "hist_narrow") g_hist_narrow = atoi(v.c_str()) != 0 ? 1 : 0;   // layout of matrices quantised from now on
-  else fail("unknown option '%s'", k.c_str());
-  API_END
-}
 int B2_GetVersion(void) { return 100; }
 int B2_DeviceCount(int* out) {
   API_BEGIN
@@ -3113,15 +3074,8 @@ int B2_HistBuildRaw(const uint8_t* bins, int64_t n_rows, int32_t n_cols, const i
   cudaEvent_t e0, e1; CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
   CUDA_CHECK(cudaEventRecord(e0, s));
   if (n_sel > 0)
-  {
-    alignas(64) unsigned char tt[128];
-    if (use_tma_hist() && b2_make_bins_tensor_map(tt, d_bins.p, n_rows, m.row_stride, 64) == 0)
-      LAUNCH_CHECK(b2_launch_hist_tma(d_bins.p, m.row_stride, tt, d_gp.p, ridx ? d_ridx.p : nullptr, d_work.p, 1, chunks, chunk_rows, window_rows, m.n_groups,
-                                      d_hist.p, nullptr, 0, 1, n_rows, ctx->num_sms, s));
-    else
-      LAUNCH_CHECK(b2_launch_hist(d_bins.p, m.row_stride, d_gp.p, ridx ? d_ridx.p : nullptr, d_work.p, 1, chunks, chunk_rows,
-                                  window_rows, m.n_groups, d_hist.p, nullptr, 0, 1, m.narrow_w, ctx->num_sms, s));
-  }
+    LAUNCH_CHECK(b2_launch_hist(d_bins.p, m.row_stride, d_gp.p, ridx ? d_ridx.p : nullptr, d_work.p, 1, chunks, chunk_rows,
+                                window_rows, m.n_groups, d_hist.p, nullptr, 0, 1, ctx->num_sms, s));
   CUDA_CHECK(cudaEventRecord(e1, s));
   std::vector<long long> h(node_elems);
   CUDA_CHECK(cudaMemcpyAsync(h.data(), d_hist.p, node_elems * sizeof(long long), cudaMemcpyDeviceToHost, s));

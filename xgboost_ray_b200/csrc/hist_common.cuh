@@ -1,11 +1,9 @@
-// hist_common.cuh -- device helpers shared by the LDG-staged and the TMA-staged histogram kernels.
+// hist_common.cuh -- device helpers of the histogram kernels (hist_kernel.cu): row loads, the conflict-free shared
+// atomics and the flushes to the global int64 histogram.
 #pragma once
 #include "common.cuh"
 
 namespace b2 {
-
-constexpr int kHistThreads = 256;
-constexpr int kRowsPerWarpIter = 16;
 
 __device__ __forceinline__ uint4 ldg_nc_v4(const void* p) {
   uint4 r;
@@ -54,24 +52,11 @@ __device__ __forceinline__ RowData load_row_id(const uint8_t* __restrict__ bins,
   }
   return d;
 }
-// diagnostic (debug_mode 2): synthesise the row instead of loading it
-__device__ __forceinline__ RowData fake_row(int64_t rid) {
-  RowData d;
-  uint32_t x = (uint32_t)rid * 2654435761u + 12345u;
-  d.bins = make_uint4(x, x * 1664525u + 1013904223u, x ^ (x >> 13), x * 22695477u + 1u);
-  d.gp = make_int2(rid >= 0 ? 3 : 0, rid >= 0 ? 1 : 0);
-  return d;
-}
 
 // 16 steps: one byte (= one feature slot) per step, two conflict-free shared atomics per step.
 // Shared layout: int32 [256 bins][2 planes (g,h)][32 slots] = 256 B per bin, so bin*256 is the byte
 // placed at byte position 1 by ONE prmt; the cell address is that plus a per-lane, per-step offset.
-__device__ __forceinline__ void accumulate_row(const RowData& d, uint32_t smem_g, int rot, int half, int debug_mode = 0,
-                                               unsigned* sink = nullptr) {
-  if (debug_mode == 1) {  // diagnostic: consume the loads without touching shared memory
-    *sink += d.bins.x ^ d.bins.y ^ d.bins.z ^ d.bins.w ^ (unsigned)d.gp.x ^ (unsigned)d.gp.y;
-    return;
-  }
+__device__ __forceinline__ void accumulate_row(const RowData& d, uint32_t smem_g, int rot, int half) {
   uint4 b = rotate_bytes(d.bins, rot);
   const uint32_t w[4] = {b.x, b.y, b.z, b.w};
   const uint32_t base = smem_g + half * 64;
@@ -95,54 +80,35 @@ struct HistTarget {
   int node_cap;               // node slots per shard in this launch's buffer
   int n_groups;
 };
-// slot_mask = 31 for a full group; w - 1 for a narrow group of width w (its shared-memory histogram holds 32 / w
-// replicas of the w slots side by side, all of which fold onto the same global cell here)
-__device__ __forceinline__ size_t target_index(const HistTarget& t, int node_slot, int group, int e, int slot_mask = 31) {
-  const int bin = e >> 6, plane = (e >> 5) & 1, slot = e & 31 & slot_mask;
+__device__ __forceinline__ size_t target_index(const HistTarget& t, int node_slot, int group, int e) {
+  const int bin = e >> 6, plane = (e >> 5) & 1, slot = e & 31;
   const int shards = 1 << t.log2_shards, sp = B2_GROUP_SLOTS >> t.log2_shards;
   const int r = slot & (shards - 1), sl = slot >> t.log2_shards;
   const size_t slice_elems = (size_t)t.n_groups * 2 * B2_BINS * sp;
   return ((size_t)r * t.node_cap + node_slot) * slice_elems + ((size_t)(group * 2 + plane) * B2_BINS + bin) * sp + sl;
 }
 
-// Same 16 steps when the group's shared-memory histogram starts on a 64 KiB boundary: the cell address
-//   group_base | bin << 8 | (half * 64 + slot * 4)
-// has the bin in byte 1 and everything else in bytes 0, 2, 3, so ONE prmt merges the bin byte of the row with the
-// per-step base (a loop-invariant register) -- 3 instructions per update pair instead of 4 (no add).
-__device__ __forceinline__ void accumulate_row_aligned(const RowData& d, uint32_t smem_g /* multiple of 65536 */, int rot, int half) {
-  uint4 b = rotate_bytes(d.bins, rot);
-  const uint32_t w[4] = {b.x, b.y, b.z, b.w};
-  const uint32_t base = smem_g + half * 64;
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    const uint32_t bj = base + (((uint32_t)(j + rot) & 15u) << 2);            // loop invariant: byte 1 is zero
-    const uint32_t a = __byte_perm(w[j >> 2], bj, 0x7604u | ((uint32_t)(j & 3) << 4));
-    red_shared_add(a, d.gp.x);
-    red_shared_add(a + B2_GROUP_SLOTS * 4, d.gp.y);
-  }
-}
-
 // lazy window flush: only cells whose magnitude reached 2^30 are moved to the global histogram.  Called
 // (between barriers) at least every `window_rows` = 2^(30 - qbits) rows, during which a cell can grow by
 // less than 2^30, so no int32 cell can overflow; for well spread bins nothing is flushed at all.
-__device__ __forceinline__ void flush_large_cells(int32_t* s_hist, const HistTarget& t, int node_slot, int group, int slot_mask = 31) {
+__device__ __forceinline__ void flush_large_cells(int32_t* s_hist, const HistTarget& t, int node_slot, int group) {
   for (int e = threadIdx.x * 4; e < B2_GROUP_ELEMS; e += blockDim.x * 4) {
     const int4 v = *reinterpret_cast<const int4*>(s_hist + e);
     const int vv[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       if (vv[k] >= (1 << 30) || vv[k] <= -(1 << 30)) {
-        atomicAdd(t.base + target_index(t, node_slot, group, e + k, slot_mask), (unsigned long long)(long long)vv[k]);
+        atomicAdd(t.base + target_index(t, node_slot, group, e + k), (unsigned long long)(long long)vv[k]);
         s_hist[e + k] = 0;
       }
     }
   }
 }
 // node flush: shared int32 partial sums -> global int64 histogram (RED.64), cells are left zeroed
-__device__ __forceinline__ void flush_planes(int32_t* s_hist, const HistTarget& t, int node_slot, int group, int slot_mask = 31) {
+__device__ __forceinline__ void flush_planes(int32_t* s_hist, const HistTarget& t, int node_slot, int group) {
   for (int e = threadIdx.x; e < B2_GROUP_ELEMS; e += blockDim.x) {
     const long long v = s_hist[e];
-    if (v != 0) { atomicAdd(t.base + target_index(t, node_slot, group, e, slot_mask), (unsigned long long)v); s_hist[e] = 0; }
+    if (v != 0) { atomicAdd(t.base + target_index(t, node_slot, group, e), (unsigned long long)v); s_hist[e] = 0; }
   }
 }
 

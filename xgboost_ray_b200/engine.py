@@ -40,7 +40,6 @@ _H = C.c_uint64
 ABI = {
     "B2_GetLastError": (C.c_char_p, []),
     "B2_GetVersion": (C.c_int, []),
-    "B2_SetOption": (C.c_int, [C.c_char_p, C.c_char_p]),
     "B2_DeviceCount": (C.c_int, [C.POINTER(C.c_int)]),
     "B2_GetUniqueId": (C.c_int, [_BP]),
     "B2_CommCreate": (C.c_int, [_BP, C.c_int, C.c_int, C.c_int, C.POINTER(_H)]),
@@ -1392,20 +1391,8 @@ def train(params, dtrain, num_boost_round=10, evals=(), obj=None, feval=None, ma
     return bst
 
 
-def set_option(key, value):
-    """Process-wide engine option (B2_SetOption)."""
-    _check(lib().B2_SetOption(str(key).encode(), str(value).encode()))
-
-
-def hist_build_raw(bins, qg, qh, ridx=None, window_rows=8192, chunk_rows=2048, device=None, narrow=None):
-    """Kernel-level entry (tests / roofline probe): returns (hist [F,256,2] int64, kernel_ms).  narrow = 0 / 1 selects
-    the feature-group layout for this call (None: the process default)."""
-    if narrow is not None:
-        try:
-            set_option("hist_narrow", int(narrow))
-            return hist_build_raw(bins, qg, qh, ridx, window_rows, chunk_rows, device)
-        finally:
-            set_option("hist_narrow", 1 if os.environ.get("B2_HIST_NARROW", "0") not in ("", "0") else 0)
+def hist_build_raw(bins, qg, qh, ridx=None, window_rows=8192, chunk_rows=2048, device=None):
+    """Kernel-level entry (tests / roofline probe): returns (hist [F,256,2] int64, kernel_ms)."""
     bins = np.ascontiguousarray(bins, np.uint8)
     n, f = bins.shape
     qg = np.ascontiguousarray(qg, np.int32)
