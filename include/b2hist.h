@@ -135,8 +135,10 @@ int B2_BoosterPredictContribs(B2Handle b, B2Handle m, int32_t tree_begin, int32_
 /* model.predict(local_data, pred_leaf=True) at main.py:804: out [n_rows][tree_end - tree_begin] = node id (as in the
  * model JSON / get_dump) of the leaf each row reaches in each tree of the range (tree_end == 0: all trees). */
 int B2_BoosterPredictLeaf(B2Handle b, B2Handle m, int32_t tree_begin, int32_t tree_end, float* out, int64_t out_len);
-/* copy of the training-set margin cache (what the next round's gradient is taken at) */
-int B2_BoosterGetTrainMargin(B2Handle b, float* out, int64_t out_len);
+/* copy of the training-set margin cache.  full = 0: what the next round's gradient is taken at (booster=dart: that
+ * round's drop margin, whose drops B2_BoosterBoostOneIter then keeps); full = 1: the margin of the whole model (the
+ * same for gbtree), what predict and the metrics see, without a traversal of the model. */
+int B2_BoosterGetTrainMargin(B2Handle b, int32_t full, float* out, int64_t out_len);
 /* (re)initialise the training margin cache from base_margin/base_score plus all current trees
  * (continuation from xgb_model=, main.py:1211-1220); needs the raw data of the train matrix */
 int B2_BoosterResetTrainMargin(B2Handle b);
@@ -158,6 +160,12 @@ int B2_BoosterAddTree(B2Handle b, int32_t n_nodes, const int32_t* left, const in
  * after B2_BoosterAddTree when a model with categorical splits is loaded. */
 int B2_BoosterGetTreeCategories(B2Handle b, int32_t tree, uint8_t* split_type /*[n]*/, uint32_t* cat_bits /*[n*8]*/);
 int B2_BoosterSetTreeCategories(B2Handle b, int32_t tree, const uint8_t* split_type, const uint32_t* cat_bits);
+/* booster=dart: the weight of every tree in model order (model JSON gradient_booster.weight_drop); tree t adds
+ * fl(w[t] * leaf) to the margin.  Get on a gbtree booster returns 1 for every tree.  Set (after the trees were added
+ * with B2_BoosterAddTree; a tree added to a dart booster starts at weight 1) needs finite weights >= 0 and one per
+ * tree, and makes the train margin rebuild from the new weights. */
+int B2_BoosterGetTreeWeights(B2Handle b, float* out, int64_t len);
+int B2_BoosterSetTreeWeights(B2Handle b, const float* w, int64_t len);
 /* JSON object with accumulated device timings / counters of the hot path (since last reset):
  * hist_ms, hist_launches, hist_rows, hist_bytes, kernel_launches, round_ms, allreduce_bytes ... */
 int B2_BoosterGetTimers(B2Handle b, int32_t reset, char* out, int64_t out_cap);

@@ -28,6 +28,7 @@ SOURCES = {
     "rank_kernel.cu": ["--fmad=false"],        # LambdaMART gradients and ranking metrics, bit-exact vs the reference
     "p2p_exchange.cu": [],                     # NVLink peer-memory histogram exchange
     "shap_kernel.cu": [],                      # TreeSHAP contributions / interactions, leaf indices
+    "dart_kernel.cu": ["--fmad=false"],        # DART margin rebuild, bit-exact vs the weighted predict and the reference
     "engine.cu": [],
 }
 

@@ -51,7 +51,7 @@ int b2_launch_p2p_close(const void*, cudaStream_t);
 int b2_launch_gather_interleaved_rows(const void*, float*, int, cudaStream_t);
 int b2_launch_final_assign(const uint8_t*, int64_t, const int32_t*, const B2SplitWork*, const B2LevelCtl*, int, const float2*,
                            const int32_t*, int, long long*, uint16_t*, int, int, cudaStream_t);
-int b2_launch_margin_update(float*, int, int, const uint16_t*, const float*, int64_t, int, cudaStream_t);
+int b2_launch_margin_update(float*, int, int, const uint16_t*, const float*, const float*, int64_t, int, cudaStream_t);
 int b2_leaf_acc_max_depth();
 int b2_launch_leaf_accumulate(const float2*, const uint16_t*, int64_t, int, const int32_t*, int, long long*, int, cudaStream_t);
 int b2_gradient_fused_max_classes();
@@ -91,7 +91,10 @@ int b2_launch_quant_exponent(const uint32_t*, int32_t*, cudaStream_t);
 int b2_launch_quantize(const float2*, int64_t, const int32_t*, int, int2*, int, cudaStream_t);
 int b2_launch_metric(int, int, int, float, const float*, const float*, const float*, int64_t, double*, int, cudaStream_t);
 int b2_launch_predict(const float*, int64_t, int, float, const B2TreeNodeDev*, const int32_t*, const uint32_t*, int, int, int, int,
-                      float*, int, cudaStream_t);
+                      const float*, float*, int, cudaStream_t);
+int b2_launch_dart_margins(const uint8_t*, int64_t, int, const int32_t*, const uint8_t*, const B2TreeNodeDev*, const int32_t*,
+                           const uint32_t*, int, int, int, const float*, const uint8_t*, const float*, float*, float*, int,
+                           cudaStream_t);
 int b2_launch_fill(float*, int64_t, float, int, cudaStream_t);
 size_t b2_shap_contribs_smem(int, int, int);
 int b2_launch_shap_contribs(const float*, int64_t, int64_t, int, float, const B2PathElem*, const B2PathInfo*, int, int,
@@ -740,6 +743,12 @@ struct Params {
   // interaction_constraints: feature sets S_1 .. S_C (a tree path with two or more features stays inside one set);
   // empty = no constraints.  Text form "0,1;2,3,4": sets separated by ';', features by ','.
   std::vector<std::vector<int64_t>> interaction_sets;
+  // booster=dart (Dart in xgboost's gbtree.cc): trees dropped at random each round, per-tree weights
+  bool dart = false;
+  double rate_drop = 0.0, skip_drop = 0.0;
+  bool dart_weighted = false;       // sample_type: uniform (false) / weighted
+  bool dart_forest = false;         // normalize_type: tree (false) / forest
+  bool one_drop = false;
   bool use_cols() const { return colsample_bytree < 1.0f || colsample_bylevel < 1.0f || colsample_bynode < 1.0f; }
 };
 
@@ -772,7 +781,7 @@ struct Timers {
   void reset() { *this = Timers(); }
 };
 
-struct EvalCache { DevBuf<float> margin; int n_trees_applied = 0; int64_t n = 0; uint64_t margin_version = 0; };
+struct EvalCache { DevBuf<float> margin; int n_trees_applied = 0; int64_t n = 0; uint64_t margin_version = 0; uint64_t weights_version = 0; };
 
 // per-group descending order of a row vector (rank_kernel.cu b2_rank_order): keys_sorted / rows hold, for every model
 // position, the sort key (the value) and the row.  The buffers are pooled and kept, so a booster sorts its train margins
@@ -863,6 +872,8 @@ struct Booster : HandleBase {
     std::vector<std::pair<int, cudaEvent_t>> phase_marks;   // (phase that ENDS at this event)
     cudaEvent_t start = nullptr, stop = nullptr;
     uint32_t* h_p2p_err = nullptr;         // pinned copy of the peer-memory error word, written at the end of the round
+    std::vector<float> dart_w;             // DART: the weights once this round is committed (trees before it + its own)
+    bool dart_dropped = false;             // the round changed weights of earlier trees
   };
   RoundBuffers rb[2];
   int rb_cur = 0;                          // parity of the next round to enqueue
@@ -906,6 +917,23 @@ struct Booster : HandleBase {
   DevBuf<double> rank_disc; int64_t rank_disc_len = 0;
   DevBuf<double> rank_inv_idcg; uint64_t idcg_uid = 0, idcg_version = 0; int idcg_k = -1, idcg_gain = -1;
   DevBuf<float> rank_scratch_m, rank_scratch_y; DevBuf<double> rank_scratch_p;
+  // DART: the weight of every committed tree (empty for gbtree).  weights_version changes whenever weights of existing
+  // trees change (a round that dropped trees, B2_BoosterSetTreeWeights): margins cached from the old weights are stale.
+  std::vector<float> tree_w;
+  uint64_t weights_version = 0;
+  DevBuf<float> d_tree_w; uint64_t d_tree_w_version = ~0ull; size_t d_tree_w_count = 0;   // device copy for prediction
+  int paths_weights_version = -1;
+  // The next round's drop decision, taken before its gradients (dart_prepare): r = its round number, dropped[t] for the
+  // T trees before it, w_after = the weights once it is committed (T old + its new trees).  With drops, dart_drop holds
+  // its drop margin (the gradients' margin) and dart_prefix the full-margin prefix under the new weights.
+  struct DartNext {
+    int64_t r = -1;
+    std::vector<uint8_t> dropped;
+    std::vector<float> w_after;
+    int n_dropped = 0;
+  } dart_next;
+  DevBuf<float> dart_drop, dart_prefix, d_dart_w_old, d_dart_w_full, d_dart_w_new;
+  DevBuf<uint8_t> d_dart_dropped;
   // profiling
   Timers t;
   ~Booster() {
@@ -988,6 +1016,7 @@ std::vector<std::vector<int64_t>> parse_interaction_sets(const std::string& v) {
 
 void parse_params(const char* text, Params* p, int* max_bin_out) {
   std::string s(text ? text : "");
+  std::map<std::string, std::string> dart_text;
   size_t pos = 0;
   while (pos < s.size()) {
     size_t nl = s.find('\n', pos);
@@ -1070,7 +1099,35 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     else if (k == "max_cat_threshold") p->max_cat_threshold = i();
     else if (k == "max_bin") { if (max_bin_out) *max_bin_out = i(); }
     else if (k == "interaction_constraints") p->interaction_sets = parse_interaction_sets(v);
+    else if (k == "booster") {
+      if (v == "gbtree") p->dart = false;
+      else if (v == "dart") p->dart = true;
+      else fail("booster='%s' is not supported (supported: gbtree, dart)", v.c_str());
+    }
+    else if (k == "rate_drop" || k == "skip_drop" || k == "sample_type" || k == "normalize_type" || k == "one_drop")
+      dart_text[k] = v;   // checked below, and only for booster=dart (gbtree ignores them, like xgboost)
     // unknown keys (nthread, tree_method, verbosity, ...) are accepted and ignored, like xgboost
+  }
+  if (p->dart) {
+    for (const auto& kv : dart_text) {
+      const std::string& k = kv.first; const std::string& v = kv.second;
+      if (k == "sample_type") {
+        if (v != "uniform" && v != "weighted") fail("sample_type must be uniform or weighted, got '%s'", v.c_str());
+        p->dart_weighted = v == "weighted";
+      } else if (k == "normalize_type") {
+        if (v != "tree" && v != "forest") fail("normalize_type must be tree or forest, got '%s'", v.c_str());
+        p->dart_forest = v == "forest";
+      } else if (k == "one_drop") {
+        if (v == "1" || v == "true" || v == "True") p->one_drop = true;
+        else if (v == "0" || v == "false" || v == "False") p->one_drop = false;
+        else fail("one_drop must be 0 or 1, got '%s'", v.c_str());
+      } else {
+        char* end = nullptr;
+        const double x = strtod(v.c_str(), &end);
+        if (v.empty() || *end != '\0' || !(x >= 0.0 && x <= 1.0)) fail("%s must be a number in [0, 1], got '%s'", k.c_str(), v.c_str());
+        (k == "rate_drop" ? p->rate_drop : p->skip_drop) = x;
+      }
+    }
   }
   if (obj_rank(p->objective) && p->num_class > 1)
     fail("%s has one output per row: num_class must be 1, got %d", p->objective_name.c_str(), p->num_class);
@@ -1379,6 +1436,7 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   const bool multi = b->comm && b->comm->world > 1;
   const bool p2p = multi && b->p2p.enabled;
   static const bool leaf_fused = env_flag("B2_LEAF_FUSED", true);
+  if (p.dart && !leaf_fused) fail("booster=dart needs the fused leaf pass (unset B2_LEAF_FUSED)");
   // leaf sums from a streaming pass over (pos, gh) in row order; needs one shared-memory accumulator per leaf
   const bool leaf_stream = leaf_fused && D >= 1 && D <= b2_leaf_acc_max_depth();
   // sibling subtraction inside eval_splits_kernel (no hist_subtract pass).  The peer-memory exchange subtracts while it
@@ -1590,7 +1648,8 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   else allreduce(b->comm, b->d_leaf_sums.p, 4 * lcap, kNcclInt64, kNcclSum, s);   // limb by limb: exact
   LAUNCH_CHECK(b2_launch_leaf_values(b->d_leaves.p, d_n_leaves, b->d_leaf_sums.p, b->d_qexp.p, 40, cp, b->d_leaf_values.p, tree, b->t_qexp.p, s));
   if (leaf_fused)
-    LAUNCH_CHECK(b2_launch_margin_update(b->margin.p, K, k, b->pos.p, b->d_leaf_values.p, n, ctx->num_sms, s));
+    LAUNCH_CHECK(b2_launch_margin_update(b->margin.p, K, k, b->pos.p, b->d_leaf_values.p, p.dart ? b->d_dart_w_new.p : nullptr, n,
+                                         ctx->num_sms, s));
   else
     LAUNCH_CHECK(b2_launch_pred_update(b->margin.p, K, k, b->ridx[0].p, b->ridx[1].p, b->d_seg_work.p, ctl + 2, max_leaf_chunks,
                                        b->d_leaf_values.p, ctx->num_sms, s));
@@ -1734,8 +1793,9 @@ void sync_device_trees(Booster* b) {
         cat_slot = (int32_t)(b->h_cat_table.size() / 8);
         b->h_cat_table.insert(b->h_cat_table.end(), t.cat_bits.begin() + (size_t)i * 8, t.cat_bits.begin() + (size_t)i * 8 + 8);
       }
+      // pad: the split bin, read by the DART margin rebuild on the bin matrix (dart_kernel.cu)
       b->h_nodes.push_back(B2TreeNodeDev{t.left[i], t.right[i], t.feature[i], t.cond[i], t.value[i], (int32_t)t.default_left[i],
-                                         cat_slot, 0});
+                                         cat_slot, t.split_bin[i]});
     }
   }
   cudaStream_t s = b->ctx->stream;
@@ -1805,14 +1865,20 @@ void walk_paths(const TreeHost& t, int nid, std::vector<PathBuildElem>& path, in
 }
 
 void build_paths(Booster* b) {
-  if (b->paths_synced == (int)b->trees.size()) return;
+  if (b->paths_synced == (int)b->trees.size() && b->paths_weights_version == (int)b->weights_version) return;
   std::vector<B2PathElem> elems; std::vector<B2PathInfo> infos; std::vector<uint32_t> cats;
   b->tree_path_offset.assign(1, 0); b->tree_expected.clear();
   const int K = b->p.num_class, npt = std::max(1, b->p.num_parallel_tree);
   for (int t = 0; t < (int)b->trees.size(); ++t) {
     std::vector<PathBuildElem> path;
     double expected = 0.0;
+    const int32_t first = (int32_t)infos.size();
     walk_paths(b->trees[t], 0, path, t, (t / npt) % K, b, elems, infos, cats, &expected);
+    if (b->p.dart) {   // DART: the tree's leaves count with its weight
+      const double w = (double)b->tree_w[t];
+      for (size_t i = first; i < infos.size(); ++i) infos[i].value *= w;
+      expected *= w;
+    }
     b->tree_path_offset.push_back((int32_t)infos.size());
     b->tree_expected.push_back(expected);
   }
@@ -1820,6 +1886,17 @@ void build_paths(Booster* b) {
   upload(b->d_path_elems, elems, s); upload(b->d_paths, infos, s); upload(b->d_path_cats, cats, s);
   CUDA_CHECK(cudaStreamSynchronize(s));
   b->paths_synced = (int)b->trees.size();
+  b->paths_weights_version = (int)b->weights_version;
+}
+
+// DART: the tree weights on the device (nullptr for gbtree: the kernels then add the plain leaf values)
+const float* device_weights(Booster* b) {
+  if (!b->p.dart) return nullptr;
+  if (b->d_tree_w_version != b->weights_version || b->d_tree_w_count != b->tree_w.size()) {
+    upload(b->d_tree_w, b->tree_w, b->ctx->stream);   // pageable source: staged before return
+    b->d_tree_w_version = b->weights_version; b->d_tree_w_count = b->tree_w.size();
+  }
+  return b->d_tree_w.p;
 }
 
 void init_margin(Booster* b, float* margin, Matrix* m) {
@@ -1931,7 +2008,7 @@ void ensure_rank_disc(Booster* b, int64_t len) {
 }
 
 // LambdaMART gradients of the train matrix (rank_kernel.cu): order the margins per group, then one pass over the groups
-void rank_gradient(Booster* b, uint32_t* absmax, uint32_t* err) {
+void rank_gradient(Booster* b, const float* margin, uint32_t* absmax, uint32_t* err) {
   Matrix* m = b->train; cudaStream_t s = b->ctx->stream; const Params& p = b->p; const int sms = b->ctx->num_sms;
   ensure_rank_disc(b, m->max_qgroup);
   const bool ndcg = p.objective == kObjRankNdcg;
@@ -1946,7 +2023,7 @@ void rank_gradient(Booster* b, uint32_t* absmax, uint32_t* err) {
     CUDA_CHECK(cudaStreamSynchronize(s));   // lo's buffers go back to the pool
     b->idcg_uid = m->uid; b->idcg_version = m->rank_version; b->idcg_k = p.rank_k; b->idcg_gain = (int)p.ndcg_exp_gain;
   }
-  b->rank_order.run(m, b->margin.p, sms, s);
+  b->rank_order.run(m, margin, sms, s);
   if (m->max_qgroup > b2_rank_stage_rows()) {
     const size_t rows = (size_t)std::max<int64_t>(m->n, 1);
     b->rank_scratch_m.ensure(rows); b->rank_scratch_y.ensure(rows); b->rank_scratch_p.ensure(rows);
@@ -2006,6 +2083,10 @@ void finish_round(Booster* b, Booster::RoundBuffers& R, int n_trees, bool check_
          b->p.objective_name.c_str());
   }
   for (int slot = 0; slot < n_trees; ++slot) materialize_tree(b, R.staging[slot]);
+  if (b->p.dart) {   // the weights are committed with the trees
+    b->tree_w = R.dart_w;
+    if (R.dart_dropped) b->weights_version++;
+  }
   b->t.rounds++;
 }
 // Finish the round boost_round left pending.  Every entry point that reads the trees, the timers, the margin or the
@@ -2017,6 +2098,40 @@ void drain_round(Booster* b) {
   finish_round(b, b->rb[b->rb_cur ^ 1], n_trees, b->pending_check_finite);
 }
 
+// DART walks the train matrix's bins: every numeric split of a tree must name the bin whose cut is its condition (trees
+// grown by this engine on these cuts do; a model from elsewhere, or one continued on a matrix with other cuts, does not)
+void check_dart_split_bins(Booster* b) {
+  const Matrix* m = b->train;
+  for (size_t ti = 0; ti < b->trees.size(); ++ti) {
+    const TreeHost& t = b->trees[ti];
+    for (int i = 0; i < t.size(); ++i) {
+      const int f = t.feature[i];
+      if (f < 0 || t.split_type[i]) continue;
+      const int sb = t.split_bin[i];
+      const bool ok = sb < 0 ? (sb == -1 && t.cond[i] == m->min_vals[f])
+                             : (sb < m->nbins[f] && t.cond[i] == m->cut_vals[m->cut_ptrs[f] + sb]);
+      if (!ok)
+        fail("continuing a DART model needs the split bins of the train matrix's cuts: tree %zu node %d (feature %d, "
+             "condition %g) has none; continue on the matrix the model was trained on, with the model this engine wrote",
+             ti, i, f, (double)t.cond[i]);
+    }
+  }
+}
+
+// Rebuild margins of the train rows from the trees on the device (dart_kernel.cu): drop (nullable) without the trees
+// flagged in dropped, with weights w_old; full with weights w_full.  Both hold the starting margin on entry.
+void dart_margins(Booster* b, const std::vector<float>& w_old, const std::vector<uint8_t>& dropped,
+                  const std::vector<float>& w_full, float* drop, float* full) {
+  Matrix* m = b->train; cudaStream_t s = b->ctx->stream; const int T = (int)b->trees.size();
+  sync_device_trees(b);
+  upload(b->d_dart_w_full, w_full, s);
+  if (drop) { upload(b->d_dart_w_old, w_old, s); upload(b->d_dart_dropped, dropped, s); }
+  LAUNCH_CHECK(b2_launch_dart_margins(m->bins.p, m->n, m->row_stride, m->d_feat_byte.p, m->d_has_missing.p, b->d_nodes.p,
+                                      b->d_tree_offset.p, b->d_cat_table.p, T, b->p.num_class, b->p.num_parallel_tree,
+                                      drop ? b->d_dart_w_old.p : nullptr, drop ? b->d_dart_dropped.p : nullptr,
+                                      b->d_dart_w_full.p, drop, full, b->ctx->num_sms, s));
+}
+
 void ensure_train_margin(Booster* b) {
   if (b->margin_ready) return;
   drain_round(b);   // the margin is rebuilt from every tree of the model
@@ -2025,13 +2140,89 @@ void ensure_train_margin(Booster* b) {
   estimate_base_score(b);
   b->margin.ensure((size_t)std::max<int64_t>(m->n * b->p.num_class, 1));
   init_margin(b, b->margin.p, m);
-  if (!b->trees.empty()) {
+  b->dart_next.r = -1;
+  if (!b->trees.empty() && b->p.dart) {
+    check_dart_split_bins(b);
+    dart_margins(b, {}, {}, b->tree_w, nullptr, b->margin.p);
+  } else if (!b->trees.empty()) {
     if (!m->has_raw) fail("continuing training from existing trees needs the raw data of the train matrix (B2_MatrixEnsureRaw)");
     sync_device_trees(b);
     LAUNCH_CHECK(b2_launch_predict(m->raw.p, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, 0, (int)b->trees.size(),
-                                   b->p.num_class, b->p.num_parallel_tree, b->margin.p, b->ctx->num_sms, b->ctx->stream));
+                                   b->p.num_class, b->p.num_parallel_tree, nullptr, b->margin.p, b->ctx->num_sms, b->ctx->stream));
   }
   b->margin_ready = true;
+}
+
+// The DART drop set of round r over trees with weights w (DESIGN.md 2): u_j = hash(seed, r, j, B2_SCOPE_DART) / 2^32.
+// Keyed by the round, never by the rank, so every worker drops the same trees and a restart replays the same drops.
+std::vector<uint8_t> dart_drop_set(const Params& p, uint32_t r, const std::vector<float>& w) {
+  const size_t T = w.size();
+  std::vector<uint8_t> dropped(T, 0);
+  if (T == 0) return dropped;
+  auto u = [&](uint32_t j) { return (double)b2_hash4((uint32_t)p.seed, r, j, B2_SCOPE_DART) * 0x1p-32; };
+  if (p.skip_drop > 0.0 && u(0xFFFFFFFFu) < p.skip_drop) return dropped;
+  // S > 0: the newest trees of a trained model have positive weights, and B2_BoosterSetTreeWeights refuses a total
+  // that is not finite and positive
+  float S = 0.0f;
+  for (float x : w) S += x;   // binary32, in tree order
+  size_t k = 0;
+  for (size_t t = 0; t < T; ++t) {
+    const double thr = p.dart_weighted ? p.rate_drop * (double)T * (double)w[t] / (double)S : p.rate_drop;
+    if (u((uint32_t)t) < thr) { dropped[t] = 1; ++k; }
+  }
+  if (p.one_drop && k == 0) {
+    const double v = u(0xFFFFFFFEu);
+    size_t pick = T - 1;
+    if (!p.dart_weighted) {
+      pick = std::min(T - 1, (size_t)floor(v * (double)T));
+    } else {
+      double cum = 0.0;
+      for (size_t t = 0; t < T; ++t) { cum += (double)w[t]; if (cum > v * (double)S) { pick = t; break; } }
+    }
+    dropped[pick] = 1;
+  }
+  return dropped;
+}
+
+// Decide the next round's drops (once per round: B2_BoosterGetTrainMargin and the round itself share the decision) and,
+// when it drops trees, rebuild its drop margin and full-margin prefix in one pass over the bin matrix.  The weights
+// before the round include a pending round's; a dropping round needs that round's trees on the device, so it is drained.
+void dart_prepare(Booster* b) {
+  ensure_train_margin(b);
+  const Params& p = b->p; const int K = p.num_class, npt = p.num_parallel_tree;
+  const int64_t T = (int64_t)b->trees.size() + b->pending_trees;
+  const int64_t r = T / (K * npt);
+  Booster::DartNext& dn = b->dart_next;
+  if (dn.r == r && (int64_t)dn.dropped.size() == T) return;
+  const std::vector<float> w = b->pending_trees ? b->rb[b->rb_cur ^ 1].dart_w : b->tree_w;
+  if ((int64_t)w.size() != T) fail("DART: %zu tree weights for %lld trees", w.size(), (long long)T);
+  dn.dropped = dart_drop_set(p, (uint32_t)r, w);
+  dn.n_dropped = 0;
+  for (uint8_t d : dn.dropped) dn.n_dropped += d;
+  // normalisation (Dart::NormalizeTrees) for the round's n_new trees
+  const int n_new = K * npt;
+  const float lr = (float)((double)p.eta / (double)n_new);
+  const int k = dn.n_dropped;
+  float w_new = 1.0f;
+  dn.w_after = w;
+  if (k > 0) {
+    const float f = p.dart_forest ? (float)(1.0 / (1.0 + (double)lr)) : (float)((double)k / ((double)k + (double)lr));
+    for (int64_t t = 0; t < T; ++t) if (dn.dropped[t]) dn.w_after[t] *= f;
+    w_new = p.dart_forest ? f : (float)(1.0 / ((double)k + (double)lr));
+  }
+  dn.w_after.insert(dn.w_after.end(), n_new, w_new);
+  if (k > 0) {
+    drain_round(b);   // the weights of the drained round are w
+    Matrix* m = b->train;
+    const size_t nk = (size_t)std::max<int64_t>(m->n * K, 1);
+    b->dart_drop.ensure(nk); b->dart_prefix.ensure(nk);
+    init_margin(b, b->dart_drop.p, m);
+    init_margin(b, b->dart_prefix.p, m);
+    dart_margins(b, w, dn.dropped, std::vector<float>(dn.w_after.begin(), dn.w_after.begin() + T), b->dart_drop.p,
+                 b->dart_prefix.p);
+    b->t.kernel_launches++;
+  }
+  dn.r = r;
 }
 
 // One boosting round, pipelined with the previous one: round r+1 (gradients, then its class trees) is enqueued first,
@@ -2048,6 +2239,20 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
   if (!R.start) { CUDA_CHECK(cudaEventCreate(&R.start)); CUDA_CHECK(cudaEventCreate(&R.stop)); }
   if (b->p.profile) CUDA_CHECK(cudaEventRecord(R.start, s));
   ensure_train_margin(b);
+  // DART: the gradients are taken at the drop margin; the round's trees are added to the full-margin prefix
+  const float* gm = b->margin.p;
+  if (b->p.dart) {
+    dart_prepare(b);
+    const float w_new = b->dart_next.w_after.back();
+    b->d_dart_w_new.ensure(1);
+    CUDA_CHECK(cudaMemcpyAsync(b->d_dart_w_new.p, &w_new, sizeof(float), cudaMemcpyHostToDevice, s));   // staged before return
+    if (b->dart_next.n_dropped > 0) {
+      gm = b->dart_drop.p;
+      CUDA_CHECK(cudaMemcpyAsync(b->margin.p, b->dart_prefix.p, (size_t)n * K * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    }
+    R.dart_w = b->dart_next.w_after; R.dart_dropped = b->dart_next.n_dropped > 0;
+    b->dart_next.r = -1;
+  }
   b->gh.ensure((size_t)std::max<int64_t>(n * K, 1));
   b->d_absmax.ensure(2 * (size_t)K); b->d_qexp.ensure(2);
   b->absmax_fused = false;
@@ -2070,13 +2275,13 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
       CUDA_CHECK(cudaMemsetAsync(b->d_grad_err.p, 0, sizeof(uint32_t), s));
     }
     if (b->p.objective == kObjAft)
-      LAUNCH_CHECK(b2_launch_gradient_aft(b->p.aft_dist, (double)b->p.aft_sigma, b->margin.p, m->lower.p, m->upper.p,
+      LAUNCH_CHECK(b2_launch_gradient_aft(b->p.aft_dist, (double)b->p.aft_sigma, gm, m->lower.p, m->upper.p,
                                           m->n_weight ? m->weight.p : nullptr, n, b->gh.p,
                                           b->absmax_fused ? b->d_absmax.p : nullptr, b->d_grad_err.p, b->ctx->num_sms, s));
     else if (obj_rank(b->p.objective))
-      rank_gradient(b, b->absmax_fused ? b->d_absmax.p : nullptr, b->d_grad_err.p);
+      rank_gradient(b, gm, b->absmax_fused ? b->d_absmax.p : nullptr, b->d_grad_err.p);
     else
-      LAUNCH_CHECK(b2_launch_gradient(b->p.objective, K, b->margin.p, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
+      LAUNCH_CHECK(b2_launch_gradient(b->p.objective, K, gm, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
                                       b->p.scale_pos_weight, objective_param(b->p), b->gh.p,
                                       b->absmax_fused ? b->d_absmax.p : nullptr, check_finite ? b->d_grad_err.p : nullptr,
                                       b->ctx->num_sms, s));
@@ -2182,8 +2387,8 @@ float* eval_margin(Booster* b, Matrix* m) {
   if (!m->uid) fail("evaluation matrix is not a registered matrix handle");
   EvalCache*& c = b->eval_cache[m->uid];
   const int K = b->p.num_class;
-  if (!c || c->n != m->n || c->margin_version != m->margin_version) {
-    delete c; c = new EvalCache(); c->n = m->n; c->margin_version = m->margin_version;
+  if (!c || c->n != m->n || c->margin_version != m->margin_version || c->weights_version != b->weights_version) {
+    delete c; c = new EvalCache(); c->n = m->n; c->margin_version = m->margin_version; c->weights_version = b->weights_version;
     c->margin.ensure((size_t)std::max<int64_t>(m->n * K, 1));
     init_margin(b, c->margin.p, m);
     c->n_trees_applied = 0;
@@ -2192,7 +2397,7 @@ float* eval_margin(Booster* b, Matrix* m) {
   if (c->n_trees_applied < nt) {
     sync_device_trees(b);
     LAUNCH_CHECK(b2_launch_predict(m->raw.p, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, c->n_trees_applied, nt, K, b->p.num_parallel_tree,
-                                   c->margin.p, b->ctx->num_sms, b->ctx->stream));
+                                   device_weights(b), c->margin.p, b->ctx->num_sms, b->ctx->stream));
     c->n_trees_applied = nt;
   }
   return c->margin.p;
@@ -2793,8 +2998,8 @@ int B2_BoosterPredict(B2Handle bh, B2Handle mh, int32_t output_margin, int32_t t
   DevBuf<float> tmp; tmp.ensure((size_t)std::max<int64_t>(out_len, 1));
   init_margin(b, tmp.p, m);
   sync_device_trees(b);
-  LAUNCH_CHECK(b2_launch_predict(m->raw.p, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, tree_begin, tree_end, K, b->p.num_parallel_tree, tmp.p,
-                                 b->ctx->num_sms, s));
+  LAUNCH_CHECK(b2_launch_predict(m->raw.p, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, tree_begin, tree_end, K, b->p.num_parallel_tree,
+                                 device_weights(b), tmp.p, b->ctx->num_sms, s));
   if (!output_margin) LAUNCH_CHECK(b2_launch_transform(b->p.objective, K, tmp.p, m->n, b->ctx->num_sms, s));
   if (out_len > 0) CUDA_CHECK(cudaMemcpyAsync(out, tmp.p, out_len * sizeof(float), cudaMemcpyDeviceToHost, s));
   CUDA_CHECK(cudaStreamSynchronize(s));
@@ -2899,7 +3104,7 @@ int B2_BoosterPredictLeaf(B2Handle bh, B2Handle mh, int32_t tree_begin, int32_t 
   API_END
 }
 
-int B2_BoosterGetTrainMargin(B2Handle bh, float* out, int64_t out_len) {
+int B2_BoosterGetTrainMargin(B2Handle bh, int32_t full, float* out, int64_t out_len) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
   drain_round(b);
@@ -2908,7 +3113,11 @@ int B2_BoosterGetTrainMargin(B2Handle bh, float* out, int64_t out_len) {
   const int64_t want = b->train->n * b->p.num_class;
   if (out_len != want) fail("output buffer has %lld values, expected %lld", (long long)out_len, (long long)want);
   ensure_train_margin(b);
-  if (want > 0) CUDA_CHECK(cudaMemcpyAsync(out, b->margin.p, want * sizeof(float), cudaMemcpyDeviceToHost, b->ctx->stream));
+  // DART: the margin the next round's gradients are taken at (its drop margin); B2_BoosterBoostOneIter keeps its drops.
+  // full != 0 returns the margin of the whole model instead (what predict and the metrics see)
+  const float* src = b->margin.p;
+  if (b->p.dart && !full) { dart_prepare(b); if (b->dart_next.n_dropped > 0) src = b->dart_drop.p; }
+  if (want > 0) CUDA_CHECK(cudaMemcpyAsync(out, src, want * sizeof(float), cudaMemcpyDeviceToHost, b->ctx->stream));
   CUDA_CHECK(cudaStreamSynchronize(b->ctx->stream));
   API_END
 }
@@ -2980,6 +3189,33 @@ int B2_BoosterAddTree(B2Handle bh, int32_t n_nodes, const int32_t* left, const i
     t.sum_hess[i] = sum_hess ? sum_hess[i] : 0.0;
   }
   b->trees.push_back(std::move(t));
+  if (b->p.dart) b->tree_w.push_back(1.0f);   // B2_BoosterSetTreeWeights sets the model's weights
+  b->margin_ready = false;
+  API_END
+}
+int B2_BoosterGetTreeWeights(B2Handle bh, float* out, int64_t len) {
+  API_BEGIN
+  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
+  if (len != (int64_t)b->trees.size()) fail("weight buffer has %lld values for %zu trees", (long long)len, b->trees.size());
+  for (int64_t t = 0; t < len; ++t) out[t] = b->p.dart ? b->tree_w[t] : 1.0f;
+  API_END
+}
+int B2_BoosterSetTreeWeights(B2Handle bh, const float* w, int64_t len) {
+  API_BEGIN
+  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
+  if (!b->p.dart) fail("tree weights belong to booster=dart; this booster is gbtree");
+  if (len != (int64_t)b->trees.size()) fail("%lld tree weights for %zu trees", (long long)len, b->trees.size());
+  float S = 0.0f;   // the binary32 sum sample_type=weighted divides by (dart_drop_set)
+  for (int64_t t = 0; t < len; ++t) {
+    if (!std::isfinite(w[t]) || w[t] < 0.0f) fail("tree weight %lld is %g: weights must be finite and >= 0", (long long)t, (double)w[t]);
+    S += w[t];
+  }
+  if (len > 0 && !(S > 0.0f && std::isfinite(S)))
+    fail("tree weights sum to %g: a DART model needs a finite, positive total weight", (double)S);
+  b->tree_w.assign(w, w + len);
+  b->weights_version++;
   b->margin_ready = false;
   API_END
 }

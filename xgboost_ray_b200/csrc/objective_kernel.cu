@@ -582,16 +582,18 @@ __global__ void label_check_kernel(int objective, int K, const float* __restrict
 
 // A.9 traversal on raw floats (the node step is b2_tree_step, common.cuh).  nodes of all trees are
 // concatenated; tree_offset[t] is the first node of tree t; tree t adds to class (t / npt) % K (xgboost lays the
-// num_parallel_tree trees of a class out next to each other, GBTree::BoostNewTrees).
+// num_parallel_tree trees of a class out next to each other, GBTree::BoostNewTrees).  weights (DART, nullable): tree t
+// adds fl(weights[t] * leaf), a separate multiply and add like dart_margins_kernel.
 __global__ void predict_kernel(const float* __restrict__ X, int64_t n, int F, float missing, int missing_is_nan,
                                const B2TreeNodeDev* __restrict__ nodes, const int32_t* __restrict__ tree_offset,
                                const uint32_t* __restrict__ cat_table, int tree_begin, int tree_end, int K, int npt,
-                               float* __restrict__ out) {
+                               const float* __restrict__ weights, float* __restrict__ out) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const float* x = X + i * F;
     for (int t = tree_begin; t < tree_end; ++t) {
       float v;
       b2_tree_leaf(nodes + tree_offset[t], x, missing, missing_is_nan, cat_table, &v);
+      if (weights) v = __fmul_rn(__ldg(weights + t), v);
       out[i * K + ((t / npt) % K)] += v;
     }
   }
@@ -716,10 +718,10 @@ int b2_launch_metric(int objective, int metric, int K, float metric_param, const
 }
 int b2_launch_predict(const float* X, int64_t n, int F, float missing, const B2TreeNodeDev* nodes,
                       const int32_t* tree_offset, const uint32_t* cat_table, int tree_begin, int tree_end, int K, int npt,
-                      float* out, int num_sms, cudaStream_t s) {
+                      const float* weights, float* out, int num_sms, cudaStream_t s) {
   if (n <= 0 || tree_end <= tree_begin) return 0;
   b2::predict_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(X, n, F, missing, missing != missing ? 1 : 0, nodes, tree_offset,
-                                                         cat_table, tree_begin, tree_end, K, npt < 1 ? 1 : npt, out);
+                                                         cat_table, tree_begin, tree_end, K, npt < 1 ? 1 : npt, weights, out);
   return (int)cudaGetLastError();
 }
 int b2_launch_fill(float* out, int64_t n, float v, int num_sms, cudaStream_t s) {

@@ -312,10 +312,18 @@ final_assign_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, co
   }
 }
 
-// margin[row*K + k] += leaf_value[pos[row]] -- streaming, rows in natural order
+// margin[row*K + k] += leaf_value[pos[row]] -- streaming, rows in natural order.  DART passes the new tree's weight in
+// device memory (the launch may be replayed from a CUDA graph with a different weight every round): the row adds
+// fl(*weight * leaf), a separate multiply and add.
 __global__ void __launch_bounds__(256)
 margin_update_kernel(float* __restrict__ margin, int K, int k, const uint16_t* __restrict__ pos,
-                     const float* __restrict__ leaf_value, int64_t n) {
+                     const float* __restrict__ leaf_value, const float* __restrict__ weight, int64_t n) {
+  if (weight) {
+    const float w = *weight;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+      margin[i * K + k] += __fmul_rn(w, __ldg(leaf_value + pos[i]));
+    return;
+  }
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     margin[i * K + k] += __ldg(leaf_value + pos[i]);
 }
@@ -452,12 +460,12 @@ int b2_launch_leaf_accumulate(const float2* gh, const uint16_t* pos, int64_t n, 
   b2::leaf_accumulate_kernel<<<grid, b2::kLeafAccThreads, smem, stream>>>(gh, pos, n, n_acc, log2_copies, qexp, leaf_bits, sums);
   return (int)cudaGetLastError();
 }
-int b2_launch_margin_update(float* margin, int K, int k, const uint16_t* pos, const float* leaf_value, int64_t n, int num_sms,
-                            cudaStream_t stream) {
+int b2_launch_margin_update(float* margin, int K, int k, const uint16_t* pos, const float* leaf_value, const float* weight,
+                            int64_t n, int num_sms, cudaStream_t stream) {
   if (n <= 0) return 0;
   int64_t want = (n + 255) / 256;
   int grid = (int)(want < (int64_t)num_sms * 16 ? want : (int64_t)num_sms * 16);
-  b2::margin_update_kernel<<<grid, 256, 0, stream>>>(margin, K, k, pos, leaf_value, n);
+  b2::margin_update_kernel<<<grid, 256, 0, stream>>>(margin, K, k, pos, leaf_value, weight, n);
   return (int)cudaGetLastError();
 }
 int b2_launch_pred_update(float* margin, int K, int k, const int32_t* ridx0, const int32_t* ridx1, const void* work,

@@ -54,6 +54,9 @@ B2_HD uint32_t b2_neg_log2_q16(uint32_t u) {
 #define B2_SCOPE_TREE 1u
 #define B2_SCOPE_LEVEL(d) (16u + (uint32_t)(d))
 #define B2_SCOPE_NODE(nid) (4096u + (uint32_t)(nid))
+// DART drop draws: u = hash(seed, round, j, B2_SCOPE_DART) / 2^32 for tree j, j = 0xFFFFFFFF for skip_drop and
+// j = 0xFFFFFFFE for the one_drop pick (engine.cu dart_drop_set)
+#define B2_SCOPE_DART 2u
 // wq: feature weight in Q16 (65536 = 1.0); 0 sorts last
 B2_HD uint64_t b2_col_key(uint32_t seed, uint32_t tree, uint32_t scope, uint32_t f, uint32_t wq) {
   if (wq == 0) return 0xffffffffffffffffull;

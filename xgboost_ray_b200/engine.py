@@ -75,7 +75,7 @@ ABI = {
     "B2_BoosterPredict": (C.c_int, [_H, _H, C.c_int32, C.c_int32, C.c_int32, _FP, C.c_int64]),
     "B2_BoosterPredictContribs": (C.c_int, [_H, _H, C.c_int32, C.c_int32, C.c_int32, _FP, C.c_int64]),
     "B2_BoosterPredictLeaf": (C.c_int, [_H, _H, C.c_int32, C.c_int32, _FP, C.c_int64]),
-    "B2_BoosterGetTrainMargin": (C.c_int, [_H, _FP, C.c_int64]),
+    "B2_BoosterGetTrainMargin": (C.c_int, [_H, C.c_int32, _FP, C.c_int64]),
     "B2_BoosterResetTrainMargin": (C.c_int, [_H]),
     "B2_BoosterGetBaseScore": (C.c_int, [_H, _FP, _IP]),
     "B2_BoosterNumTrees": (C.c_int, [_H, _IP]),
@@ -84,6 +84,8 @@ ABI = {
     "B2_BoosterAddTree": (C.c_int, [_H, C.c_int32, _IP, _IP, _IP, _IP, _IP, _FP, _BP, _FP, _FP, _FP, _DP]),
     "B2_BoosterGetTreeCategories": (C.c_int, [_H, C.c_int32, _BP, C.POINTER(C.c_uint32)]),
     "B2_BoosterSetTreeCategories": (C.c_int, [_H, C.c_int32, _BP, C.POINTER(C.c_uint32)]),
+    "B2_BoosterGetTreeWeights": (C.c_int, [_H, _FP, C.c_int64]),
+    "B2_BoosterSetTreeWeights": (C.c_int, [_H, _FP, C.c_int64]),
     "B2_BoosterGetTimers": (C.c_int, [_H, C.c_int32, C.c_char_p, C.c_int64]),
     "B2_BoosterCancel": (C.c_int, [_H]),
     "B2_BoosterFree": (C.c_int, [_H]),
@@ -579,7 +581,10 @@ _ENGINE_KEYS = ("objective", "num_class", "max_depth", "eta", "learning_rate", "
                 "max_delta_step", "subsample", "colsample_bytree", "colsample_bylevel", "colsample_bynode", "seed",
                 "random_state", "num_parallel_tree", "huber_slope", "tweedie_variance_power", "aft_loss_distribution",
                 "aft_loss_distribution_scale", "lambdarank_pair_method", "lambdarank_num_pair_per_sample",
-                "lambdarank_unbiased", "ndcg_exp_gain")
+                "lambdarank_unbiased", "ndcg_exp_gain", "booster", "rate_drop", "skip_drop", "sample_type",
+                "normalize_type", "one_drop")
+# booster=dart's parameters with xgboost's defaults (save_config's dart_train_param)
+_DART_DEFAULTS = {"rate_drop": 0.0, "skip_drop": 0.0, "sample_type": "uniform", "normalize_type": "tree", "one_drop": 0}
 
 # xgboost parameters that change the trained model and that this engine does not implement: a value different
 # from the neutral one is an error, never silently ignored (a drop-in must not train a different model quietly)
@@ -661,6 +666,7 @@ class Booster:
         self.handle = 0
         self._train = None
         self._trees = []          # list of dict of numpy arrays (host copy for pickling / dumps)
+        self._weights = None      # booster=dart: float32 weight of every tree in self._trees (None = all 1)
         self._cuts = None         # (ptrs, vals, mins, has_missing) of the matrix this model was trained on; travels with
         #                           pickles (checkpoints) so that a restarted training quantises with the SAME cuts
         self._attrs = {}
@@ -672,8 +678,8 @@ class Booster:
         tm = self.params.get("tree_method", "hist")
         if tm not in ("hist", "gpu_hist", "auto", "approx"):
             raise XGBoostError("tree_method=%r is not supported (hist / gpu_hist only)" % (tm,))
-        if self.params.get("booster", "gbtree") != "gbtree":
-            raise XGBoostError("only booster=gbtree is supported")
+        if (self.params.get("booster") or "gbtree") not in ("gbtree", "dart"):
+            raise XGBoostError("booster=%r is not supported (supported: gbtree, dart)" % (self.params.get("booster"),))
         for d in cache:
             if isinstance(d, DMatrix) and self._train is None:
                 self._attach(d)
@@ -696,6 +702,7 @@ class Booster:
     def _attach(self, dtrain):
         """Create the device booster bound to `dtrain` (quantising it if needed)."""
         old_trees = self.get_trees() if (self.handle or self._trees) else []
+        old_weights = self.get_tree_weights() if old_trees else None
         self._free()
         dtrain._ensure_quantized(int(self.params.get("max_bin", 256)), cuts=self._cuts if old_trees else None)
         self._cuts = dtrain.get_cuts()
@@ -714,7 +721,7 @@ class Booster:
             self.feature_types = dtrain.feature_types
         if old_trees:
             dtrain._ensure_raw()
-            self._push_trees(old_trees)
+            self._push_trees(old_trees, old_weights)
             _check(lib().B2_BoosterResetTrainMargin(self.handle))
 
     def _ensure_predictor(self, device=None):
@@ -726,9 +733,9 @@ class Booster:
         extra = {"num_feature": self.n_features, "device": _default_device() if device is None else device}
         _check(lib().B2_BoosterCreate(self._param_text(extra), 0, 0, C.byref(h)))
         self.handle = h.value
-        self._push_trees(self._trees)
+        self._push_trees(self._trees, self._weights)
 
-    def _push_trees(self, trees):
+    def _push_trees(self, trees, weights=None):
         for t in trees:
             n = len(t["left"])
             _check(lib().B2_BoosterAddTree(
@@ -746,6 +753,11 @@ class Booster:
                 _check(lib().B2_BoosterSetTreeCategories(
                     self.handle, nt.value - 1, _bp(np.ascontiguousarray(st, np.uint8)),
                     np.ascontiguousarray(t["cat_bits"], np.uint32).ctypes.data_as(C.POINTER(C.c_uint32))))
+        if self.is_dart and trees and weights is not None:
+            w = _f32c(weights)
+            if w.size != len(trees):
+                raise XGBoostError("DART model has %d tree weights for %d trees" % (w.size, len(trees)))
+            _check(lib().B2_BoosterSetTreeWeights(self.handle, _fp(w), w.size))
 
     def _free(self):
         if self.handle:
@@ -771,6 +783,21 @@ class Booster:
     def num_class(self):
         obj = self.params.get("objective", "reg:squarederror")
         return int(self.params.get("num_class", 1)) if obj.startswith("multi:") else 1
+
+    @property
+    def is_dart(self):
+        return (self.params.get("booster") or "gbtree") == "dart"
+
+    def get_tree_weights(self):
+        """Per-tree weights (float32, model order): DART's weight_drop; 1 for every gbtree tree."""
+        if self.handle:
+            w = np.zeros(self.num_trees(), np.float32)
+            _check(lib().B2_BoosterGetTreeWeights(self.handle, _fp(w), w.size))
+            self._weights = w if self.is_dart else None
+            return w.copy()
+        if self._weights is not None:
+            return np.array(self._weights, np.float32)
+        return np.ones(len(self._trees), np.float32)
 
     @property
     def num_parallel_tree(self):
@@ -855,7 +882,8 @@ class Booster:
                 _check(lib().B2_BoosterEvalSet(self.handle, dm.handle, metric.encode(), C.byref(v)))
                 parts.append("%s-%s:%.6f" % (name, metric, v.value))
             if feval is not None:
-                pred = self.predict(dm, output_margin=output_margin, training=(dm is self._train))
+                # the train matrix: the engine's full-model margin (for DART, not the next round's drop margin)
+                pred = self.predict(dm, output_margin=output_margin, training=(dm is self._train), _full_margin=True)
                 res = feval(pred, dm)
                 res = res if isinstance(res, list) else [res]
                 if _coll.world > 1:   # xgboost averages custom metric values over the workers (_allreduce_metric)
@@ -879,7 +907,7 @@ class Booster:
 
     def predict(self, data, output_margin=False, ntree_limit=0, validate_features=True, training=False,
                 iteration_range=(0, 0), strict_shape=False, pred_leaf=False, pred_contribs=False, approx_contribs=False,
-                pred_interactions=False, **kwargs):
+                pred_interactions=False, _full_margin=False, **kwargs):
         """xgboost's Booster.predict.  Precedence as in xgboost: pred_leaf, then pred_interactions, then pred_contribs
         (exact TreeSHAP in margin space; output_margin does not apply)."""
         if not isinstance(data, DMatrix):
@@ -898,7 +926,7 @@ class Booster:
         n = data.num_row()
         out = np.zeros(n * K, np.float32)
         if training and data is self._train:
-            _check(lib().B2_BoosterGetTrainMargin(self.handle, _fp(out), out.size))
+            _check(lib().B2_BoosterGetTrainMargin(self.handle, 1 if _full_margin else 0, _fp(out), out.size))
             if not output_margin:
                 out = _transform(self.params.get("objective", "reg:squarederror"), out.reshape(n, K)).reshape(-1)
         else:
@@ -1020,16 +1048,20 @@ class Booster:
             b2p["interaction_constraints"] = str(sets)
         attrs["b2.params"] = json.dumps({k: b2p[k] for k in sorted(b2p)})
         attrs["b2.split_bins"] = json.dumps([c[1] for c in cache], separators=(",", ":"))
+        gbtree = {"model": {
+            "gbtree_model_param": {"num_parallel_tree": str(self.num_parallel_tree), "num_trees": str(len(trees))},
+            "iteration_indptr": list(range(0, len(trees) + 1, K * self.num_parallel_tree)),
+            "tree_info": [(i // self.num_parallel_tree) % K for i in range(len(trees))],
+            "trees": trees}, "name": "gbtree"}
+        if self.is_dart:   # xgboost's Dart::SaveModel: the gbtree block plus one weight per tree
+            gbtree = {"name": "dart", "gbtree": gbtree,
+                      "weight_drop": [float(x) for x in self.get_tree_weights()[:len(trees)]]}
         return {
             "learner": {
                 "attributes": attrs,
                 "feature_names": [str(x) for x in (self.feature_names or [])],
                 "feature_types": [_xgb_feature_type(x) for x in (self.feature_types or [])],
-                "gradient_booster": {"model": {
-                    "gbtree_model_param": {"num_parallel_tree": str(self.num_parallel_tree), "num_trees": str(len(trees))},
-                    "iteration_indptr": list(range(0, len(trees) + 1, K * self.num_parallel_tree)),
-                    "tree_info": [(i // self.num_parallel_tree) % K for i in range(len(trees))],
-                    "trees": trees}, "name": "gbtree"},
+                "gradient_booster": gbtree,
                 "learner_model_param": {"base_score": _num_str(self.params.get("base_score", 0.5) if self.params.get("base_score") is not None else 0.5),
                                         "boost_from_average": "1", "num_class": str(K if K > 1 else 0),
                                         "num_feature": str(self.n_features), "num_target": "1"},
@@ -1072,7 +1104,18 @@ class Booster:
                 if k in spec.block_params:
                     params[k] = str(v) if isinstance(spec.block_params[k], str) else float(v)
         params["base_score"] = float(L["learner_model_param"]["base_score"])
-        npt = int(L["gradient_booster"]["model"].get("gbtree_model_param", {}).get("num_parallel_tree", "1"))
+        gb = L["gradient_booster"]
+        weights = None
+        if gb.get("name") == "dart":
+            params["booster"] = "dart"
+            weights = np.asarray(gb.get("weight_drop", []), np.float32)
+            gb = gb["gbtree"]
+            if weights.size != len(gb["model"]["trees"]):
+                raise XGBoostError("DART model has %d weight_drop entries for %d trees"
+                                   % (weights.size, len(gb["model"]["trees"])))
+        elif params.get("booster") == "dart":
+            params["booster"] = "gbtree"
+        npt = int(gb["model"].get("gbtree_model_param", {}).get("num_parallel_tree", "1"))
         if npt > 1:
             params["num_parallel_tree"] = npt
         params.update({k: v for k, v in self.params.items() if k not in params})
@@ -1082,7 +1125,8 @@ class Booster:
         self.feature_types = [_b2_feature_type(x) for x in L.get("feature_types") or []] or None
         self._attrs = attrs
         self._trees = []
-        for ti, t in enumerate(L["gradient_booster"]["model"]["trees"]):
+        self._weights = weights
+        for ti, t in enumerate(gb["model"]["trees"]):
             left = np.asarray(t["left_children"], np.int32)
             leaf = left < 0
             sc = np.asarray(t["split_conditions"], np.float32)
@@ -1125,6 +1169,7 @@ class Booster:
         self.handle = 0
         self._train = None
         self._trees = []
+        self._weights = None
         self._attrs = {}
         self.feature_names = None
         self.feature_types = None
@@ -1145,6 +1190,10 @@ class Booster:
         sets = self._interaction_sets() if self.n_features is not None else []
         if sets:
             gbtree["tree_train_param"] = {"interaction_constraints": str(sets)}
+        if self.is_dart:
+            gbtree = {"name": "dart", "gbtree": gbtree,
+                      "dart_train_param": {k: _str_param(self.params.get(k, d)) if isinstance(d, str) else
+                                           _num_str(self.params.get(k, d)) for k, d in _DART_DEFAULTS.items()}}
         return json.dumps({"learner": {"gradient_booster": gbtree,
                                        "objective": {"name": self.params.get("objective", "reg:squarederror")},
                                        "b2_params": {k: v for k, v in self.params.items() if _json_ok(v)}},
@@ -1331,6 +1380,12 @@ def train(params, dtrain, num_boost_round=10, evals=(), obj=None, feval=None, ma
             src = Booster(params)
             src.load_model(xgb_model)
         bst._trees = list(src._trees)
+        if src.is_dart and "booster" not in params:   # a DART model continues as DART
+            bst.params["booster"] = "dart"
+        elif src.is_dart and not bst.is_dart:
+            raise XGBoostError("cannot continue a DART model with booster=%r: its trees carry weights that a gbtree "
+                               "model would drop (continue with booster='dart')" % (bst.params.get("booster"),))
+        bst._weights = src.get_tree_weights() if bst.is_dart and src.is_dart else None
         bst.n_features, bst.feature_names, bst.feature_types = src.n_features, src.feature_names, src.feature_types
         bst._attrs = dict(src._attrs)
         # a restart after an actor failure (main.py sets _freeze_cuts on the unpickled checkpoint) continues with the

@@ -17,7 +17,8 @@ from xgboost_ray_b200.matrix import RayDMatrix
 _PARAM_NAMES = ("max_depth", "learning_rate", "gamma", "min_child_weight", "reg_lambda", "reg_alpha", "max_bin",
                 "base_score", "tree_method", "subsample", "colsample_bytree", "colsample_bylevel", "colsample_bynode",
                 "scale_pos_weight", "max_delta_step", "max_cat_to_onehot", "max_cat_threshold", "eval_metric",
-                "tweedie_variance_power", "huber_slope", "interaction_constraints")
+                "tweedie_variance_power", "huber_slope", "interaction_constraints", "booster", "rate_drop", "skip_drop",
+                "sample_type", "normalize_type", "one_drop")
 
 
 def _check_if_params_are_ray_dmatrix(X, sample_weight, base_margin, eval_set):
@@ -46,7 +47,9 @@ class RayXGBMixin(BaseEstimator):
                  max_cat_threshold: Optional[int] = None, enable_categorical: bool = False, missing: float = np.nan,
                  eval_metric=None, early_stopping_rounds: Optional[int] = None, callbacks=None,
                  tweedie_variance_power: Optional[float] = None, huber_slope: Optional[float] = None,
-                 interaction_constraints=None):
+                 interaction_constraints=None, booster: Optional[str] = None, rate_drop: Optional[float] = None,
+                 skip_drop: Optional[float] = None, sample_type: Optional[str] = None,
+                 normalize_type: Optional[str] = None, one_drop: Optional[int] = None):
         self.n_estimators = n_estimators
         self.max_depth = max_depth
         self.learning_rate = learning_rate
@@ -76,6 +79,12 @@ class RayXGBMixin(BaseEstimator):
         self.tweedie_variance_power = tweedie_variance_power   # reg:tweedie rho in [1, 2); None = 1.5
         self.huber_slope = huber_slope                         # reg:pseudohubererror delta > 0; None = 1
         self.interaction_constraints = interaction_constraints   # feature sets, e.g. "[[0, 1], [2, 3, 4]]"; None = off
+        self.booster = booster                 # "gbtree" (None) or "dart"; the next five are DART's, ignored by gbtree
+        self.rate_drop = rate_drop
+        self.skip_drop = skip_drop
+        self.sample_type = sample_type
+        self.normalize_type = normalize_type
+        self.one_drop = one_drop
 
     def get_xgb_params(self):
         p = {k: getattr(self, k) for k in _PARAM_NAMES if getattr(self, k) is not None}
