@@ -29,6 +29,7 @@ SOURCES = {
     "p2p_exchange.cu": [],                     # NVLink peer-memory histogram exchange
     "shap_kernel.cu": [],                      # TreeSHAP contributions / interactions, leaf indices
     "dart_kernel.cu": ["--fmad=false"],        # DART margin rebuild, bit-exact vs the weighted predict and the reference
+    "quantile_kernel.cu": ["--fmad=false"],    # quantile gradients, metric and leaf refresh, bit-exact vs the reference
     "engine.cu": [],
 }
 

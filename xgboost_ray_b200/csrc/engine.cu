@@ -96,6 +96,16 @@ int b2_launch_dart_margins(const uint8_t*, int64_t, int, const int32_t*, const u
                            const uint32_t*, int, int, int, const float*, const uint8_t*, const float*, float*, float*, int,
                            cudaStream_t);
 int b2_launch_fill(float*, int64_t, float, int, cudaStream_t);
+size_t b2_quantile_hist_elems(int);
+size_t b2_quantile_sel_bytes(int);
+int b2_quantile_passes();
+int b2_launch_gradient_quantile(int, const float*, const float*, const float*, const float*, int64_t, float2*, uint32_t*, int,
+                                cudaStream_t);
+int b2_launch_quantile_metric(int, const float*, const float*, const float*, const float*, int64_t, double*, int, cudaStream_t);
+int b2_launch_quantile_count(int, const uint16_t*, const float*, const float*, int, int, const float2*, int64_t,
+                             const int32_t*, int, const void*, int, unsigned long long*, int, cudaStream_t);
+int b2_launch_quantile_scan(int, const int32_t*, int, int, float, float, unsigned long long*, void*, const B2LeafDev*, float*,
+                            float*, cudaStream_t);
 size_t b2_shap_contribs_smem(int, int, int);
 int b2_launch_shap_contribs(const float*, int64_t, int64_t, int, float, const B2PathElem*, const B2PathInfo*, int, int,
                             const uint32_t*, int, const double*, const float*, float, double*, int, size_t, float*, int, cudaStream_t);
@@ -710,12 +720,13 @@ void bin_matrix(Matrix* m) {
 // objective ids, shared with objective_kernel.cu (the kernels take them as plain ints)
 enum { kObjSquaredError = 0, kObjLogistic = 1, kObjSoftprob = 2, kObjRegLogistic = 3, kObjLogitRaw = 4, kObjSquaredLog = 5,
        kObjPseudoHuber = 6, kObjPoisson = 7, kObjGamma = 8, kObjTweedie = 9, kObjAft = 10, kObjRankPairwise = 11,
-       kObjRankNdcg = 12 };
+       kObjRankNdcg = 12, kObjQuantile = 13 };
 bool obj_log_link(int o) { return o == kObjPoisson || o == kObjGamma || o == kObjTweedie || o == kObjAft; }
 bool obj_sigmoid(int o) { return o == kObjLogistic || o == kObjRegLogistic; }
 bool obj_rank(int o) { return o == kObjRankPairwise || o == kObjRankNdcg; }
-// objectives whose gradient kernel reports non-finite gradient pairs (gradient_param_kernel)
-bool obj_checks_finite(int o) { return o >= kObjSquaredLog; }
+// objectives whose gradient kernel reports non-finite gradient pairs (gradient_param_kernel).  reg:quantileerror's
+// pairs are finite for finite labels and weights (both checked before the first round), so its rounds stay pipelined.
+bool obj_checks_finite(int o) { return o >= kObjSquaredLog && o != kObjQuantile; }
 struct Params {
   int objective = kObjSquaredError;
   std::string objective_name = "reg:squarederror";
@@ -749,6 +760,9 @@ struct Params {
   bool dart_weighted = false;       // sample_type: uniform (false) / weighted
   bool dart_forest = false;         // normalize_type: tree (false) / forest
   bool one_drop = false;
+  // reg:quantileerror: one output (and one tree per round) per alpha
+  std::vector<float> quantile_alpha{0.5f};
+  bool num_class_set = false;
   bool use_cols() const { return colsample_bytree < 1.0f || colsample_bylevel < 1.0f || colsample_bynode < 1.0f; }
 };
 
@@ -934,6 +948,12 @@ struct Booster : HandleBase {
   } dart_next;
   DevBuf<float> dart_drop, dart_prefix, d_dart_w_old, d_dart_w_full, d_dart_w_new;
   DevBuf<uint8_t> d_dart_dropped;
+  // reg:quantileerror: the alphas on the device, and the leaf refresh's digit histograms (zero between passes) and
+  // per-leaf selection state (quantile_kernel.cu).  refresh_leaves: the round being enqueued refreshes its leaves (a
+  // custom objective's rounds keep their Newton leaves).
+  DevBuf<float> d_alpha;
+  DevBuf<unsigned long long> d_qhist; DevBuf<uint8_t> d_qsel; DevBuf<int32_t> d_one;
+  bool refresh_leaves = false;
   // profiling
   Timers t;
   ~Booster() {
@@ -1014,6 +1034,28 @@ std::vector<std::vector<int64_t>> parse_interaction_sets(const std::string& v) {
   return sets;
 }
 
+// quantile_alpha as "a,b,c" (brackets allowed): every alpha finite with 0 < alpha < 1
+std::vector<float> parse_quantile_alpha(std::string v) {
+  for (char& c : v) if (c == '[' || c == ']' || c == '(' || c == ')') c = ' ';
+  std::vector<float> out;
+  size_t pos = 0;
+  while (pos <= v.size()) {
+    size_t comma = v.find(',', pos);
+    if (comma == std::string::npos) comma = v.size();
+    std::string tok = v.substr(pos, comma - pos);
+    const size_t a = tok.find_first_not_of(" \t"), b = tok.find_last_not_of(" \t");
+    tok = a == std::string::npos ? std::string() : tok.substr(a, b - a + 1);
+    char* end = nullptr;
+    const double x = strtod(tok.c_str(), &end);
+    const float f = (float)x;
+    if (tok.empty() || *end != '\0' || !(f > 0.0f && f < 1.0f))
+      fail("quantile_alpha: '%s' is not a number in (0, 1)", tok.c_str());
+    out.push_back(f);
+    pos = comma + 1;
+  }
+  return out;
+}
+
 void parse_params(const char* text, Params* p, int* max_bin_out) {
   std::string s(text ? text : "");
   std::map<std::string, std::string> dart_text;
@@ -1043,10 +1085,12 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
       else if (v == "survival:aft") p->objective = kObjAft;
       else if (v == "rank:pairwise") p->objective = kObjRankPairwise;
       else if (v == "rank:ndcg") p->objective = kObjRankNdcg;
+      else if (v == "reg:quantileerror") p->objective = kObjQuantile;
       else fail("unsupported objective '%s' (supported: reg:squarederror, reg:logistic, binary:logistic, binary:logitraw, "
                 "reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie, survival:aft, "
-                "rank:pairwise, rank:ndcg, multi:softprob, multi:softmax)", v.c_str());
-    } else if (k == "num_class") p->num_class = i();
+                "rank:pairwise, rank:ndcg, reg:quantileerror, multi:softprob, multi:softmax)", v.c_str());
+    } else if (k == "num_class") { p->num_class = i(); p->num_class_set = true; }
+    else if (k == "quantile_alpha") p->quantile_alpha = parse_quantile_alpha(v);
     else if (k == "num_parallel_tree") p->num_parallel_tree = i();
     else if (k == "max_depth") p->max_depth = i();
     else if (k == "eta" || k == "learning_rate") p->eta = f();
@@ -1131,7 +1175,13 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
   }
   if (obj_rank(p->objective) && p->num_class > 1)
     fail("%s has one output per row: num_class must be 1, got %d", p->objective_name.c_str(), p->num_class);
-  if (p->objective != kObjSoftprob) p->num_class = 1;
+  if (p->objective == kObjQuantile) {
+    // rules of this engine (DESIGN.md 2): the outputs are the alphas, the leaf refresh needs the plain gbtree round
+    if (p->num_class_set) fail("reg:quantileerror has one output per quantile_alpha: num_class must not be set");
+    if (p->dart) fail("reg:quantileerror is not supported with booster=dart");
+    if (p->num_parallel_tree > 1) fail("reg:quantileerror needs num_parallel_tree = 1, got %d", p->num_parallel_tree);
+    p->num_class = (int)p->quantile_alpha.size();
+  } else if (p->objective != kObjSoftprob) p->num_class = 1;
   if (p->objective == kObjSoftprob && p->num_class < 2) fail("multi:softprob needs num_class >= 2");
   if (p->max_depth < 1 || p->max_depth > 14) fail("max_depth must be in [1, 14], got %d", p->max_depth);
   if (p->num_parallel_tree < 1 || p->num_parallel_tree > 4096) fail("num_parallel_tree must be in [1, 4096], got %d", p->num_parallel_tree);
@@ -1427,6 +1477,48 @@ void exchange_and_subtract(Booster* b, TreeStats& st, const long long* parent_le
 // enqueues a fixed sequence and the finished tree is copied into pinned block `slot`.
 // With st.capturing the stream is in capture mode: nothing here may allocate, touch pageable host memory or depend on
 // host state that changes from tree to tree (run_tree decides when that holds).
+// reg:quantileerror buffers for up to max_leaves segments, allocated outside any capture; the histograms start zeroed
+// and every scan zeroes what it read
+void ensure_quantile_buffers(Booster* b, int max_leaves) {
+  cudaStream_t s = b->ctx->stream;
+  const size_t elems = b2_quantile_hist_elems(max_leaves);
+  if (b->d_qhist.cap < elems) {
+    b->d_qhist.ensure(elems);
+    CUDA_CHECK(cudaMemsetAsync(b->d_qhist.p, 0, elems * sizeof(unsigned long long), s));
+  }
+  b->d_qsel.ensure(b2_quantile_sel_bytes(max_leaves));
+  if (!b->d_one.p) {
+    const int32_t one = 1;
+    b->d_one.ensure(1);
+    CUDA_CHECK(cudaMemcpyAsync(b->d_one.p, &one, sizeof(one), cudaMemcpyHostToDevice, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+  }
+  if (b->d_alpha.cap < b->p.quantile_alpha.size()) {
+    upload(b->d_alpha, b->p.quantile_alpha, s);
+    CUDA_CHECK(cudaStreamSynchronize(s));
+  }
+}
+
+// The alpha_k-quantile of the residuals y - margin[:, k] (margin nullable: 0) of the rows with a nonzero hessian in each
+// of the *n_leaves segments given by pos (nullable: one segment), exact over all ranks (quantile_kernel.cu).  Writes
+// fp32(q * eta) to leaf_value[leaf] and, with leaves, to tree_value[leaves[leaf].nid]; an empty segment is left as it is.
+// qexp[1] is the exponent of the largest hessian of all ranks (the weights' fixed-point scale).
+int quantile_select(Booster* b, int k, const uint16_t* pos, const float* margin, const float2* gh, const int32_t* qexp,
+                    const int32_t* n_leaves, int max_leaves, float eta, const B2LeafDev* leaves, float* leaf_value,
+                    float* tree_value) {
+  Matrix* m = b->train; cudaStream_t s = b->ctx->stream; const int K = b->p.num_class;
+  const int weighted = m->n_weight > 0 ? 1 : 0;
+  const size_t elems = b2_quantile_hist_elems(max_leaves) / (weighted ? 1 : 2);
+  for (int pass = 0; pass < b2_quantile_passes(); ++pass) {
+    LAUNCH_CHECK(b2_launch_quantile_count(pass, pos, m->label.p, margin, K, k, gh, m->n, qexp, weighted, b->d_qsel.p,
+                                          max_leaves, b->d_qhist.p, b->ctx->num_sms, s));
+    allreduce(b->comm, b->d_qhist.p, elems, kNcclUint64, kNcclSum, s);   // digit counts of all ranks: exact
+    LAUNCH_CHECK(b2_launch_quantile_scan(pass, n_leaves, max_leaves, weighted, b->p.quantile_alpha[k], eta, b->d_qhist.p,
+                                         b->d_qsel.p, leaves, leaf_value, tree_value, s));
+  }
+  return 2 * b2_quantile_passes();
+}
+
 void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   Matrix* m = b->train; Ctx* ctx = b->ctx; cudaStream_t s = ctx->stream; const Params& p = b->p;
   const int64_t n = m->n; const int K = p.num_class; const int G = m->n_groups; const int D = p.max_depth;
@@ -1437,6 +1529,7 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   const bool p2p = multi && b->p2p.enabled;
   static const bool leaf_fused = env_flag("B2_LEAF_FUSED", true);
   if (p.dart && !leaf_fused) fail("booster=dart needs the fused leaf pass (unset B2_LEAF_FUSED)");
+  if (b->refresh_leaves && !leaf_fused) fail("reg:quantileerror needs the fused leaf pass (unset B2_LEAF_FUSED)");
   // leaf sums from a streaming pass over (pos, gh) in row order; needs one shared-memory accumulator per leaf
   const bool leaf_stream = leaf_fused && D >= 1 && D <= b2_leaf_acc_max_depth();
   // sibling subtraction inside eval_splits_kernel (no hist_subtract pass).  The peer-memory exchange subtracts while it
@@ -1647,6 +1740,10 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   if (p2p) { LAUNCH_CHECK(b2_launch_p2p_leaf_sums(&b->p2p.pp, d_n_leaves, b->d_leaf_sums.p, s)); st.kernel_launches++; }
   else allreduce(b->comm, b->d_leaf_sums.p, 4 * lcap, kNcclInt64, kNcclSum, s);   // limb by limb: exact
   LAUNCH_CHECK(b2_launch_leaf_values(b->d_leaves.p, d_n_leaves, b->d_leaf_sums.p, b->d_qexp.p, 40, cp, b->d_leaf_values.p, tree, b->t_qexp.p, s));
+  // reg:quantileerror: the leaf value becomes the alpha_k-quantile of the leaf's residuals at the margin before this tree
+  if (b->refresh_leaves)
+    st.kernel_launches += quantile_select(b, k, b->pos.p, b->margin.p, gh, b->d_qexp.p, d_n_leaves, (int)lcap, cp.eta,
+                                          b->d_leaves.p, b->d_leaf_values.p, tree.leaf_value);
   if (leaf_fused)
     LAUNCH_CHECK(b2_launch_margin_update(b->margin.p, K, k, b->pos.p, b->d_leaf_values.p, p.dart ? b->d_dart_w_new.p : nullptr, n,
                                          ctx->num_sms, s));
@@ -1675,6 +1772,7 @@ void prepare_tree_buffers(Booster* b, int slot) {
   const size_t rows = (size_t)std::max<int64_t>(n, 1);
   b->d_absmax.ensure(2 * (size_t)b->p.num_class); b->d_qexp.ensure(2);
   b->q.ensure(rows); b->ridx[0].ensure(rows); b->ridx[1].ensure(rows); b->pos.ensure(rows);
+  if (b->refresh_leaves) ensure_quantile_buffers(b, 1 << b->p.max_depth);
   if (b->staging_bytes != L.bytes) {
     for (auto& r : b->rb) {
       for (void* h : r.staging) cudaFreeHost(h);
@@ -1919,6 +2017,32 @@ void estimate_base_score(Booster* b) {
   if (!b->trees.empty()) fail("continuing from existing trees needs an explicit base_score (the source model's intercept)");
   if (m->n_label != m->n) fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)m->n);
   const int64_t n = m->n;
+  if (p.objective == kObjQuantile) {
+    // the fp32 mean over k of the weighted alpha_k-quantile of the labels (the leaf refresh's selection, one segment)
+    const int K = p.num_class;
+    ensure_quantile_buffers(b, 1);
+    DevBuf<float2> gq; DevBuf<float> q;
+    gq.ensure((size_t)std::max<int64_t>(n, 1)); q.ensure((size_t)K);
+    b->d_absmax.ensure(2); b->d_qexp.ensure(2);
+    CUDA_CHECK(cudaMemsetAsync(q.p, 0, (size_t)K * sizeof(float), s));
+    for (int k = 0; k < K; ++k) {
+      LAUNCH_CHECK(b2_launch_gradient_quantile(1, b->d_alpha.p + k, nullptr, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
+                                               gq.p, nullptr, b->ctx->num_sms, s));
+      CUDA_CHECK(cudaMemsetAsync(b->d_absmax.p, 0, 2 * sizeof(uint32_t), s));
+      LAUNCH_CHECK(b2_launch_absmax(gq.p, n, b->d_absmax.p, b->ctx->num_sms, s));
+      allreduce(b->comm, b->d_absmax.p, 2, kNcclUint32, kNcclMax, s);
+      LAUNCH_CHECK(b2_launch_quant_exponent(b->d_absmax.p, b->d_qexp.p, s));
+      quantile_select(b, k, nullptr, nullptr, gq.p, b->d_qexp.p, b->d_one.p, 1, 1.0f, nullptr, q.p + k, nullptr);
+    }
+    std::vector<float> h((size_t)K);
+    CUDA_CHECK(cudaMemcpyAsync(h.data(), q.p, (size_t)K * sizeof(float), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    float sum = 0.0f;
+    for (float v : h) sum += v;
+    p.base_score = sum / (float)K;
+    p.base_score_set = true;
+    return;
+  }
   DevBuf<float> zeros; DevBuf<float2> gh; DevBuf<long long> sums;
   zeros.ensure((size_t)std::max<int64_t>(n, 1)); gh.ensure((size_t)std::max<int64_t>(n, 1)); sums.ensure(4);
   CUDA_CHECK(cudaMemsetAsync(zeros.p, 0, (size_t)std::max<int64_t>(n, 1) * sizeof(float), s));
@@ -2055,7 +2179,8 @@ void check_labels(Booster* b) {
       fail("label must be in [0, num_class) for %s, num_class = %d", b->p.objective_name.c_str(), b->p.num_class);
     const char* cond = (o == kObjRegLogistic || o == kObjLogitRaw) ? "label must be in [0, 1]"
                        : o == kObjSquaredLog ? "label must be greater than -1"
-                       : o == kObjGamma ? "label must be positive" : "label must be nonnegative";
+                       : o == kObjGamma ? "label must be positive"
+                       : o == kObjQuantile ? "label must be finite" : "label must be nonnegative";
     fail("%s for %s", cond, b->p.objective_name.c_str());
   }
   b->labels_checked = true;
@@ -2256,6 +2381,7 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
   b->gh.ensure((size_t)std::max<int64_t>(n * K, 1));
   b->d_absmax.ensure(2 * (size_t)K); b->d_qexp.ensure(2);
   b->absmax_fused = false;
+  b->refresh_leaves = !custom_g && b->p.objective == kObjQuantile;
   bool check_finite = false;
   if (custom_g) {
     if (len != n * K) fail("custom gradient has %lld values, expected %lld", (long long)len, (long long)(n * K));
@@ -2280,7 +2406,11 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
                                           b->absmax_fused ? b->d_absmax.p : nullptr, b->d_grad_err.p, b->ctx->num_sms, s));
     else if (obj_rank(b->p.objective))
       rank_gradient(b, gm, b->absmax_fused ? b->d_absmax.p : nullptr, b->d_grad_err.p);
-    else
+    else if (b->p.objective == kObjQuantile) {
+      ensure_quantile_buffers(b, 1 << b->p.max_depth);
+      LAUNCH_CHECK(b2_launch_gradient_quantile(K, b->d_alpha.p, gm, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
+                                               b->gh.p, b->absmax_fused ? b->d_absmax.p : nullptr, b->ctx->num_sms, s));
+    } else
       LAUNCH_CHECK(b2_launch_gradient(b->p.objective, K, gm, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
                                       b->p.scale_pos_weight, objective_param(b->p), b->gh.p,
                                       b->absmax_fused ? b->d_absmax.p : nullptr, check_finite ? b->d_grad_err.p : nullptr,
@@ -2352,6 +2482,7 @@ int metric_id(const char* name, const Params& p, float* param, int* minus) {
   if (s == "mae") return 5;
   if (s == "auc") return 6;
   if (s == "aft-nloglik") return 14;
+  if (s == "quantile") return 19;
   if (s == "interval-regression-accuracy") return 15;
   // ranking metrics: ndcg[@k][-] (16), map[@k][-] (17), pre[@k][-] (18).  *param = k (0: the whole group), *minus = the
   // trailing '-' (a group without relevant rows scores 0 instead of 1)
@@ -2370,7 +2501,7 @@ int metric_id(const char* name, const Params& p, float* param, int* minus) {
   }
   fail("unsupported eval metric '%s' (supported: rmse, mae, logloss, error, auc, mlogloss, merror, rmsle, mape, mphe, "
        "poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy, "
-       "ndcg[@k][-], map[@k][-], pre[@k][-])", s.c_str());
+       "quantile, ndcg[@k][-], map[@k][-], pre[@k][-])", s.c_str());
 }
 
 // margin of matrix m under the current model (cached per matrix, only new trees are applied)
@@ -2943,6 +3074,22 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
   if (aft_metric) {
     LAUNCH_CHECK(b2_launch_aft_metric(b->p.aft_dist, mid, (double)b->p.aft_sigma, margin, m->lower.p, m->upper.p,
                                       m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p, b->ctx->num_sms, s));
+    allreduce(b->comm, b->d_metric.p, 2, kNcclFloat64, kNcclSum, s);
+    double h[2];
+    CUDA_CHECK(cudaMemcpyAsync(h, b->d_metric.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    *out = h[1] > 0 ? h[0] / h[1] : 0.0;
+    return 0;
+  }
+  if (mid == 19) {
+    // pinball loss averaged over the rows and the alphas, weighted (sum, K * sum w summed over the workers)
+    if (b->p.objective != kObjQuantile) fail("metric 'quantile' needs objective reg:quantileerror (it reads quantile_alpha)");
+    if (!b->d_alpha.p || b->d_alpha.cap < b->p.quantile_alpha.size()) {
+      upload(b->d_alpha, b->p.quantile_alpha, s);
+      CUDA_CHECK(cudaStreamSynchronize(s));
+    }
+    LAUNCH_CHECK(b2_launch_quantile_metric(b->p.num_class, b->d_alpha.p, margin, m->label.p, m->n_weight ? m->weight.p : nullptr,
+                                           m->n, b->d_metric.p, b->ctx->num_sms, s));
     allreduce(b->comm, b->d_metric.p, 2, kNcclFloat64, kNcclSum, s);
     double h[2];
     CUDA_CHECK(cudaMemcpyAsync(h, b->d_metric.p, sizeof(h), cudaMemcpyDeviceToHost, s));

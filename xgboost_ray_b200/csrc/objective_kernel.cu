@@ -111,9 +111,9 @@ __device__ double b2_erf(double x) {
 
 // objective ids (engine.cu kObj*): 0 reg:squarederror, 1 binary:logistic, 2 multi:softprob, 3 reg:logistic,
 // 4 binary:logitraw, 5 reg:squaredlogerror, 6 reg:pseudohubererror, 7 count:poisson, 8 reg:gamma, 9 reg:tweedie,
-// 10 survival:aft
+// 10 survival:aft, 13 reg:quantileerror (its kernels are in quantile_kernel.cu)
 constexpr int kObjRegLogistic = 3, kObjLogitRaw = 4, kObjSquaredLog = 5, kObjPseudoHuber = 6, kObjPoisson = 7,
-              kObjGamma = 8, kObjTweedie = 9, kObjAft = 10;
+              kObjGamma = 8, kObjTweedie = 9, kObjAft = 10, kObjQuantile = 13;
 // the parameter of an objective that has one: huber_slope, max_delta_step (Poisson hessian), tweedie_variance_power
 struct ObjParam { float a; };
 
@@ -575,6 +575,7 @@ __global__ void label_check_kernel(int objective, int K, const float* __restrict
     else if (objective == kObjSquaredLog) ok = y > -1.0f;
     else if (objective == kObjPoisson || objective == kObjTweedie) ok = y >= 0.0f;
     else if (objective == kObjGamma) ok = y > 0.0f;
+    else if (objective == kObjQuantile) ok = fabsf(y) <= FLT_MAX;
     any |= !ok;
   }
   if (__any_sync(0xffffffffu, any) && (threadIdx.x & 31) == 0) atomicOr(bad, 1u);

@@ -561,9 +561,44 @@ _OBJECTIVES = {
                                {"aft_loss_distribution": "normal", "aft_loss_distribution_scale": 1}),
     "rank:pairwise": _Objective("ndcg", None, *_LAMBDARANK),
     "rank:ndcg": _Objective("ndcg", None, *_LAMBDARANK),
+    # one output per alpha; the block's value is the alphas' list string (quantile_alpha_text)
+    "reg:quantileerror": _Objective("quantile", None, "reg_quantileerror_param", {"quantile_alpha": "[0.5]"}),
     "multi:softprob": _Objective("mlogloss", "softmax", *_SOFTMAX),
     "multi:softmax": _Objective("mlogloss", "softmax", *_SOFTMAX),
 }
+
+
+def quantile_alphas(value):
+    """reg:quantileerror's quantile_alpha in any form xgboost takes -> float32 array of the alphas.
+
+    value: a number, a list / tuple / numpy array of numbers, or a string such as "0.5" or "[0.1, 0.5, 0.9]"; None gives
+    xgboost's default [0.5].  Every alpha must be finite with 0 < alpha < 1 (as a float32), else XGBoostError names it."""
+    if value is None:
+        return np.array([0.5], np.float32)
+    if isinstance(value, (bytes, bytearray)):
+        value = value.decode()
+    if isinstance(value, str):
+        try:
+            value = ast.literal_eval(value.strip())
+        except (ValueError, SyntaxError) as e:
+            raise XGBoostError("quantile_alpha=%r does not parse as a number or a list of numbers (%s)" % (value, e))
+    items = list(np.ravel(np.asarray(value, dtype=object))) if isinstance(value, (list, tuple, np.ndarray)) else [value]
+    if not items:
+        raise XGBoostError("quantile_alpha must hold at least one alpha")
+    out = []
+    for a in items:
+        if isinstance(a, (bool, np.bool_, str, bytes)) or not isinstance(a, (int, float, np.integer, np.floating)):
+            raise XGBoostError("quantile_alpha: %r is not a number" % (a,))
+        f = np.float32(a)
+        if not (np.isfinite(f) and 0 < f < 1):
+            raise XGBoostError("quantile_alpha: %r is outside (0, 1); every alpha must satisfy 0 < alpha < 1" % (a,))
+        out.append(f)
+    return np.array(out, np.float32)
+
+
+def quantile_alpha_text(alphas):
+    """The alphas as the model and save_config write them: "[0.1, 0.5, 0.9]" (9 significant digits: exact float32)."""
+    return "[" + ", ".join(_num_str(a) for a in quantile_alphas(alphas)) + "]"
 
 
 def _objective(name):
@@ -582,7 +617,7 @@ _ENGINE_KEYS = ("objective", "num_class", "max_depth", "eta", "learning_rate", "
                 "random_state", "num_parallel_tree", "huber_slope", "tweedie_variance_power", "aft_loss_distribution",
                 "aft_loss_distribution_scale", "lambdarank_pair_method", "lambdarank_num_pair_per_sample",
                 "lambdarank_unbiased", "ndcg_exp_gain", "booster", "rate_drop", "skip_drop", "sample_type",
-                "normalize_type", "one_drop")
+                "normalize_type", "one_drop", "quantile_alpha")
 # booster=dart's parameters with xgboost's defaults (save_config's dart_train_param)
 _DART_DEFAULTS = {"rate_drop": 0.0, "skip_drop": 0.0, "sample_type": "uniform", "normalize_type": "tree", "one_drop": 0}
 
@@ -596,7 +631,23 @@ _UNSUPPORTED_NEUTRAL = {
 }
 
 
+def _check_quantile(params):
+    """reg:quantileerror grows one tree per alpha and round on the gbtree path: its outputs are the alphas, so num_class
+    is refused, and so are DART and random forests (num_parallel_tree > 1), whose trees the leaf refresh does not cover."""
+    if params.get("objective") != "reg:quantileerror":
+        return
+    quantile_alphas(params.get("quantile_alpha"))
+    if params.get("num_class") is not None:
+        raise XGBoostError("reg:quantileerror has one output per quantile_alpha: num_class must not be set (got %r)"
+                           % (params["num_class"],))
+    if (params.get("booster") or "gbtree") == "dart":
+        raise XGBoostError("reg:quantileerror is not supported with booster='dart'")
+    if int(params.get("num_parallel_tree", 1) or 1) > 1:
+        raise XGBoostError("reg:quantileerror needs num_parallel_tree = 1 (got %r)" % (params["num_parallel_tree"],))
+
+
 def _check_supported(params):
+    _check_quantile(params)
     mb = params.get("max_bin")
     if mb is not None and not 2 <= int(mb) <= 256:
         raise XGBoostError("parameter max_bin=%r is not supported by the H100 hist engine: the bin matrix is uint8, "
@@ -690,6 +741,8 @@ class Booster:
     def _param_text(self, extra=None):
         _check_supported(self.params)
         p = {k: self.params[k] for k in _ENGINE_KEYS if k in self.params and self.params[k] is not None}
+        if "quantile_alpha" in p:   # the engine takes "a,b,c" with each float32 alpha written exactly
+            p["quantile_alpha"] = ",".join(repr(float(a)) for a in quantile_alphas(p["quantile_alpha"]))
         if extra:
             p.update(extra)
         return "\n".join("%s=%s" % (k, v) for k, v in p.items()).encode()
@@ -781,7 +834,10 @@ class Booster:
 
     @property
     def num_class(self):
+        """Outputs per row: the classes of multi:*, the alphas of reg:quantileerror, else 1."""
         obj = self.params.get("objective", "reg:squarederror")
+        if obj == "reg:quantileerror":
+            return int(quantile_alphas(self.params.get("quantile_alpha")).size)
         return int(self.params.get("num_class", 1)) if obj.startswith("multi:") else 1
 
     @property
@@ -1034,10 +1090,12 @@ class Booster:
             cache.append((self._tree_json(i, src[i], self.n_features), [int(x) for x in src[i]["split_bin"]]))
         trees = [c[0] for c in cache]
         obj = self.params.get("objective", "reg:squarederror")
+        quantile = obj == "reg:quantileerror"   # xgboost counts the alphas as targets, not classes
         spec = _OBJECTIVES.get(obj, _OBJECTIVES["reg:squarederror"])
         obj_block = {"name": obj}
         if spec.block:
             obj_block[spec.block] = {k: str(K) if k == "num_class" else
+                                     quantile_alpha_text(self.params.get(k)) if k == "quantile_alpha" else
                                      _str_param(self.params.get(k, d)) if isinstance(d, str) else _num_str(self.params.get(k, d))
                                      for k, d in spec.block_params.items()}
         attrs = {k: str(v) for k, v in self._attrs.items() if not k.startswith("b2.")}
@@ -1063,8 +1121,8 @@ class Booster:
                 "feature_types": [_xgb_feature_type(x) for x in (self.feature_types or [])],
                 "gradient_booster": gbtree,
                 "learner_model_param": {"base_score": _num_str(self.params.get("base_score", 0.5) if self.params.get("base_score") is not None else 0.5),
-                                        "boost_from_average": "1", "num_class": str(K if K > 1 else 0),
-                                        "num_feature": str(self.n_features), "num_target": "1"},
+                                        "boost_from_average": "1", "num_class": str(K if K > 1 and not quantile else 0),
+                                        "num_feature": str(self.n_features), "num_target": str(K if quantile else 1)},
                 "objective": obj_block,
             },
             "version": [2, 0, 3],
@@ -1194,8 +1252,11 @@ class Booster:
             gbtree = {"name": "dart", "gbtree": gbtree,
                       "dart_train_param": {k: _str_param(self.params.get(k, d)) if isinstance(d, str) else
                                            _num_str(self.params.get(k, d)) for k, d in _DART_DEFAULTS.items()}}
+        objective = {"name": self.params.get("objective", "reg:squarederror")}
+        if objective["name"] == "reg:quantileerror":
+            objective["reg_quantileerror_param"] = {"quantile_alpha": quantile_alpha_text(self.params.get("quantile_alpha"))}
         return json.dumps({"learner": {"gradient_booster": gbtree,
-                                       "objective": {"name": self.params.get("objective", "reg:squarederror")},
+                                       "objective": objective,
                                        "b2_params": {k: v for k, v in self.params.items() if _json_ok(v)}},
                            "version": [2, 0, 3]})
 
@@ -1386,6 +1447,14 @@ def train(params, dtrain, num_boost_round=10, evals=(), obj=None, feval=None, ma
             raise XGBoostError("cannot continue a DART model with booster=%r: its trees carry weights that a gbtree "
                                "model would drop (continue with booster='dart')" % (bst.params.get("booster"),))
         bst._weights = src.get_tree_weights() if bst.is_dart and src.is_dart else None
+        if src.params.get("objective") == "reg:quantileerror" and bst.params.get("objective") == "reg:quantileerror":
+            # the trees of output k were fitted to alpha_k: a continuation keeps the alphas
+            old = quantile_alphas(src.params.get("quantile_alpha"))
+            if bst.params.get("quantile_alpha") is None:
+                bst.params["quantile_alpha"] = [float(a) for a in old]
+            elif quantile_alphas(bst.params["quantile_alpha"]).tobytes() != old.tobytes():
+                raise XGBoostError("cannot continue training with quantile_alpha=%s: the model was trained with %s"
+                                   % (quantile_alpha_text(bst.params["quantile_alpha"]), quantile_alpha_text(old)))
         bst.n_features, bst.feature_names, bst.feature_types = src.n_features, src.feature_names, src.feature_types
         bst._attrs = dict(src._attrs)
         # a restart after an actor failure (main.py sets _freeze_cuts on the unpickled checkpoint) continues with the
