@@ -127,7 +127,7 @@ int b2_launch_lambdarank_gradient(int, const int64_t*, int64_t, int64_t, const u
 int b2_launch_rank_metric(int, int, int, int, const int64_t*, int64_t, const int32_t*, const float*, const uint32_t*,
                           const double*, double*, double*, int, cudaStream_t);
 size_t b2_auc_temp_bytes(int64_t);
-int b2_auc_binary(const float*, const float*, const float*, int64_t, void*, size_t, double*, int, cudaStream_t);
+int b2_auc(int, int, const float*, const float*, const float*, int64_t, void*, size_t, double*, int, cudaStream_t);
 int b2_launch_transform(int, int, float*, int64_t, int, cudaStream_t);
 int b2_extract_batch();
 int b2_launch_extract_keys(const float*, int64_t, int, int, int, float, uint32_t*, int64_t, int, cudaStream_t);
@@ -2481,6 +2481,7 @@ int metric_id(const char* name, const Params& p, float* param, int* minus) {
   if (s == "merror") return 4;
   if (s == "mae") return 5;
   if (s == "auc") return 6;
+  if (s == "aucpr") return 20;
   if (s == "aft-nloglik") return 14;
   if (s == "quantile") return 19;
   if (s == "interval-regression-accuracy") return 15;
@@ -2499,7 +2500,7 @@ int metric_id(const char* name, const Params& p, float* param, int* minus) {
     *param = (float)k;
     return id;
   }
-  fail("unsupported eval metric '%s' (supported: rmse, mae, logloss, error, auc, mlogloss, merror, rmsle, mape, mphe, "
+  fail("unsupported eval metric '%s' (supported: rmse, mae, logloss, error, auc, aucpr, mlogloss, merror, rmsle, mape, mphe, "
        "poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy, "
        "quantile, ndcg[@k][-], map[@k][-], pre[@k][-])", s.c_str());
 }
@@ -3059,14 +3060,54 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
     *out = h[1] > 0 ? h[0] / h[1] : 0.0;
     return 0;
   }
-  // xgboost computes a per-group ranking AUC on a matrix with groups; this engine's auc is the binary one only
-  if (mid == 6 && m->has_qgroups())
-    fail("metric 'auc' on a matrix with query groups (per-group ranking AUC) is not supported; use ndcg or map");
+  const bool auc_metric = mid == 6 || mid == 20;
+  // xgboost computes a per-group ranking AUC on a matrix with groups; this engine's auc / aucpr are binary or
+  // one-vs-rest only
+  if (auc_metric && m->has_qgroups())
+    fail("metric '%s' on a matrix with query groups (per-group ranking AUC) is not supported; use ndcg or map", metric);
+  if (auc_metric && b->p.num_class > 1 && b->p.objective != kObjSoftprob)
+    fail("metric '%s' needs one output per row or a multi:softprob / multi:softmax model; objective '%s' has %d outputs",
+         metric, b->p.objective_name.c_str(), b->p.num_class);
   if (aft_metric && b->p.objective != kObjAft)
     fail("metric '%s' does not fit objective '%s'", metric, b->p.objective_name.c_str());
   if (aft_metric && !m->has_bounds()) fail("metric '%s' needs label_lower_bound and label_upper_bound on the evaluation matrix", metric);
   if (!aft_metric && m->n_label != m->n) fail("evaluation matrix has no labels");
   float* margin = eval_margin(b, m);
+  if (auc_metric) {
+    // ROC / PR AUC on the transformed prediction (auc_kernel.cu; DESIGN.md §2 item 17): per class a worker's triple
+    // (ROC: area, fp*tp, tp; PR: aucpr, 1, 1) plus the count of out-of-range labels, summed over the workers
+    const int K = b->p.num_class;
+    DevBuf<float> pred; DevBuf<uint8_t> tmp;
+    pred.ensure((size_t)std::max<int64_t>(m->n * K, 1));
+    if (m->n > 0) CUDA_CHECK(cudaMemcpyAsync(pred.p, margin, (size_t)(m->n * K) * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    LAUNCH_CHECK(b2_launch_transform(b->p.objective, K, pred.p, m->n, b->ctx->num_sms, s));
+    const size_t tb = b2_auc_temp_bytes(m->n);
+    tmp.ensure(tb);
+    b->d_metric.ensure(3 * (size_t)K + 1);
+    LAUNCH_CHECK(b2_auc(mid == 20 ? 1 : 0, K, pred.p, m->label.p, m->n_weight ? m->weight.p : nullptr, m->n, tmp.p, tb,
+                        b->d_metric.p, b->ctx->num_sms, s));
+    allreduce(b->comm, b->d_metric.p, 3 * (size_t)K + 1, kNcclFloat64, kNcclSum, s);
+    std::vector<double> h(3 * (size_t)K + 1);
+    CUDA_CHECK(cudaMemcpyAsync(h.data(), b->d_metric.p, h.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    if (h[3 * (size_t)K] > 0)
+      fail("metric '%s': label must be in [0, num_class), num_class = %d (%.0f rows outside)", metric, K, h[3 * (size_t)K]);
+    if (K == 1) {
+      // ROC with only one class present: xgboost reports 0.5
+      *out = mid == 6 ? (h[1] > 0 ? h[0] / h[1] : 0.5) : h[0] / h[1];
+      return 0;
+    }
+    // one-vs-rest: sum_c (A_c / L_c) T_c / sum_c T_c; NaN when some class has L_c = 0 or no class has T_c
+    double num = 0.0, den = 0.0;
+    bool defined = true;
+    for (int c = 0; c < K; ++c) {
+      const double A = h[3 * c], L = h[3 * c + 1], T = h[3 * c + 2];
+      if (!(L > 0)) { defined = false; break; }
+      num += A / L * T; den += T;
+    }
+    *out = defined && den > 0 ? num / den : NAN;
+    return 0;
+  }
   b->d_metric.ensure(3);
   CUDA_CHECK(cudaMemsetAsync(b->d_metric.p, 0, 3 * sizeof(double), s));
   if ((mid == 3 || mid == 4) != (b->p.objective == kObjSoftprob))
@@ -3095,24 +3136,6 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
     CUDA_CHECK(cudaMemcpyAsync(h, b->d_metric.p, sizeof(h), cudaMemcpyDeviceToHost, s));
     CUDA_CHECK(cudaStreamSynchronize(s));
     *out = h[1] > 0 ? h[0] / h[1] : 0.0;
-    return 0;
-  }
-  if (mid == 6) {
-    // binary ROC AUC on the transformed prediction (auc_kernel.cu): local (area, fp*tp) pairs summed over the workers
-    if (b->p.objective == kObjSoftprob) fail("metric 'auc' is implemented for binary labels (binary:logistic / regression scores) only");
-    DevBuf<float> pred; DevBuf<uint8_t> tmp;
-    const size_t rows = (size_t)std::max<int64_t>(m->n, 1);
-    pred.ensure(rows);
-    if (m->n > 0) CUDA_CHECK(cudaMemcpyAsync(pred.p, margin, (size_t)m->n * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    LAUNCH_CHECK(b2_launch_transform(b->p.objective, 1, pred.p, m->n, b->ctx->num_sms, s));
-    const size_t tb = b2_auc_temp_bytes(m->n);
-    tmp.ensure(tb);
-    LAUNCH_CHECK(b2_auc_binary(pred.p, m->label.p, m->n_weight ? m->weight.p : nullptr, m->n, tmp.p, tb, b->d_metric.p, b->ctx->num_sms, s));
-    allreduce(b->comm, b->d_metric.p, 2, kNcclFloat64, kNcclSum, s);
-    double h[2];
-    CUDA_CHECK(cudaMemcpyAsync(h, b->d_metric.p, sizeof(h), cudaMemcpyDeviceToHost, s));
-    CUDA_CHECK(cudaStreamSynchronize(s));
-    *out = h[1] > 0 ? h[0] / h[1] : 0.5;   // only one class present: xgboost reports 0.5
     return 0;
   }
   LAUNCH_CHECK(b2_launch_metric(b->p.objective, mid, b->p.num_class, mparam, margin, m->label.p, m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p,

@@ -501,7 +501,7 @@ __global__ void quantize_kernel(const float2* __restrict__ gh, int64_t n, const 
 // metric sums (sum loss*w, sum w, rows with an invalid class label) -> out[3] doubles.  Metrics see the TRANSFORMED prediction (ObjFunction::EvalTransform,
 // src/learner.cc): the probability for binary:logistic / reg:logistic, exp(margin) for the log-link objectives, the raw
 // value otherwise.  metric: 0 rmse, 1 logloss, 2 error, 3 mlogloss, 4 merror, 5 mae, 7 rmsle, 8 mape, 9 mphe (a = huber
-// slope), 10 poisson-nloglik, 11 gamma-nloglik, 12 gamma-deviance, 13 tweedie-nloglik (a = rho); 6 (auc) is auc_kernel.cu.
+// slope), 10 poisson-nloglik, 11 gamma-nloglik, 12 gamma-deviance, 13 tweedie-nloglik (a = rho); 6 (auc) and 20 (aucpr) are auc_kernel.cu.
 // the elementwise metrics of the objectives added after the first three, on the transformed prediction q
 __device__ __forceinline__ double scalar_metric(int metric, float a, double q, double y) {
   if (metric == 7) { const double d = log1p(y) - log1p(fmax(q, -1.0 + 1e-6)); return d * d; }

@@ -1322,9 +1322,9 @@ def _str_param(v):
 
 
 def _maximized(metric):
-    """Metrics where larger is better (early stopping): auc, interval-regression-accuracy and every ndcg / map / pre
-    form (ndcg@5, map-, pre@10, ...)."""
-    if metric in ("auc", "interval-regression-accuracy"):
+    """Metrics where larger is better (early stopping): auc, aucpr, interval-regression-accuracy and every ndcg / map /
+    pre form (ndcg@5, map-, pre@10, ...)."""
+    if metric in ("auc", "aucpr", "interval-regression-accuracy"):
         return True
     return metric.split("@")[0].rstrip("-") in ("ndcg", "map", "pre")
 
