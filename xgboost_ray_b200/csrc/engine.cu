@@ -120,10 +120,10 @@ int b2_rank_order(const float*, int64_t, const int64_t*, int64_t, const int32_t*
                   int, cudaStream_t);
 int b2_launch_rank_disc(double*, int64_t, int, cudaStream_t);
 int b2_launch_rank_inv_idcg(const int64_t*, int64_t, const uint32_t*, const double*, int, int, double*, int, cudaStream_t);
-int b2_launch_rank_label_check(const float*, int64_t, int, uint32_t*, int, cudaStream_t);
+int b2_launch_rank_label_check(const float*, int64_t, int, int, uint32_t*, int, cudaStream_t);
 int b2_launch_lambdarank_gradient(int, const int64_t*, int64_t, int64_t, const uint32_t*, const int32_t*, const float*,
-                                  const double*, const double*, int, int, float*, float*, double*, float2*, uint32_t*, uint32_t*,
-                                  int, cudaStream_t);
+                                  const double*, const double*, int, int, float*, float*, double*, double*, int32_t*, float2*,
+                                  uint32_t*, uint32_t*, int, cudaStream_t);
 int b2_launch_rank_metric(int, int, int, int, const int64_t*, int64_t, const int32_t*, const float*, const uint32_t*,
                           const double*, double*, double*, int, cudaStream_t);
 size_t b2_auc_temp_bytes(int64_t);
@@ -720,10 +720,10 @@ void bin_matrix(Matrix* m) {
 // objective ids, shared with objective_kernel.cu (the kernels take them as plain ints)
 enum { kObjSquaredError = 0, kObjLogistic = 1, kObjSoftprob = 2, kObjRegLogistic = 3, kObjLogitRaw = 4, kObjSquaredLog = 5,
        kObjPseudoHuber = 6, kObjPoisson = 7, kObjGamma = 8, kObjTweedie = 9, kObjAft = 10, kObjRankPairwise = 11,
-       kObjRankNdcg = 12, kObjQuantile = 13 };
+       kObjRankNdcg = 12, kObjQuantile = 13, kObjRankMap = 14 };
 bool obj_log_link(int o) { return o == kObjPoisson || o == kObjGamma || o == kObjTweedie || o == kObjAft; }
 bool obj_sigmoid(int o) { return o == kObjLogistic || o == kObjRegLogistic; }
-bool obj_rank(int o) { return o == kObjRankPairwise || o == kObjRankNdcg; }
+bool obj_rank(int o) { return o == kObjRankPairwise || o == kObjRankNdcg || o == kObjRankMap; }
 // objectives whose gradient kernel reports non-finite gradient pairs (gradient_param_kernel).  reg:quantileerror's
 // pairs are finite for finite labels and weights (both checked before the first round), so its rounds stay pipelined.
 bool obj_checks_finite(int o) { return o >= kObjSquaredLog && o != kObjQuantile; }
@@ -926,11 +926,12 @@ struct Booster : HandleBase {
   std::map<uint64_t, EvalCache*> eval_cache;   // keyed by Matrix::uid
   // learning to rank: the train margins' order (every round), the discount table ln2 / log(r + 2) (grown to the largest
   // group seen), 1/IDCG of the train groups (keyed by matrix, its rank_version, k and the gain) and the stage of the
-  // groups larger than the gradient kernel's shared-memory stage
+  // groups larger than the gradient kernel's shared-memory stage (with rank:map also its hit prefixes A and counts R)
   RankOrder rank_order;
   DevBuf<double> rank_disc; int64_t rank_disc_len = 0;
   DevBuf<double> rank_inv_idcg; uint64_t idcg_uid = 0, idcg_version = 0; int idcg_k = -1, idcg_gain = -1;
   DevBuf<float> rank_scratch_m, rank_scratch_y; DevBuf<double> rank_scratch_p;
+  DevBuf<double> rank_scratch_a; DevBuf<int32_t> rank_scratch_r;
   // DART: the weight of every committed tree (empty for gbtree).  weights_version changes whenever weights of existing
   // trees change (a round that dropped trees, B2_BoosterSetTreeWeights): margins cached from the old weights are stale.
   std::vector<float> tree_w;
@@ -1085,10 +1086,11 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
       else if (v == "survival:aft") p->objective = kObjAft;
       else if (v == "rank:pairwise") p->objective = kObjRankPairwise;
       else if (v == "rank:ndcg") p->objective = kObjRankNdcg;
+      else if (v == "rank:map") p->objective = kObjRankMap;
       else if (v == "reg:quantileerror") p->objective = kObjQuantile;
       else fail("unsupported objective '%s' (supported: reg:squarederror, reg:logistic, binary:logistic, binary:logitraw, "
                 "reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie, survival:aft, "
-                "rank:pairwise, rank:ndcg, reg:quantileerror, multi:softprob, multi:softmax)", v.c_str());
+                "rank:pairwise, rank:ndcg, rank:map, reg:quantileerror, multi:softprob, multi:softmax)", v.c_str());
     } else if (k == "num_class") { p->num_class = i(); p->num_class_set = true; }
     else if (k == "quantile_alpha") p->quantile_alpha = parse_quantile_alpha(v);
     else if (k == "num_parallel_tree") p->num_parallel_tree = i();
@@ -2102,20 +2104,24 @@ void check_bounds(Booster* b) {
   b->labels_checked = true;
 }
 
-// the rank objectives need query groups and labels that are finite, >= 0 and, with the exponential gain, <= 31
+// the rank objectives need query groups and labels that are finite, >= 0 and, with the exponential gain, <= 31;
+// rank:map needs binary relevance (0 or 1) and ignores ndcg_exp_gain
 void check_rank_labels(Booster* b) {
   Matrix* m = b->train; cudaStream_t s = b->ctx->stream;
   if (!m->has_qgroups())
     fail("%s needs query groups on the train matrix: pass qid (or group) to the DMatrix", b->p.objective_name.c_str());
   if (b->labels_checked) return;
   if (m->n_label != m->n) fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)m->n);
-  DevBuf<uint32_t> bad; bad.ensure(2);
-  CUDA_CHECK(cudaMemsetAsync(bad.p, 0, 2 * sizeof(uint32_t), s));
-  LAUNCH_CHECK(b2_launch_rank_label_check(m->label.p, m->n, b->p.ndcg_exp_gain ? 1 : 0, bad.p, b->ctx->num_sms, s));
-  allreduce(b->comm, bad.p, 2, kNcclUint32, kNcclMax, s);
-  uint32_t h[2] = {0, 0};
+  const bool map = b->p.objective == kObjRankMap;
+  DevBuf<uint32_t> bad; bad.ensure(3);
+  CUDA_CHECK(cudaMemsetAsync(bad.p, 0, 3 * sizeof(uint32_t), s));
+  LAUNCH_CHECK(b2_launch_rank_label_check(m->label.p, m->n, !map && b->p.ndcg_exp_gain ? 1 : 0, map ? 1 : 0, bad.p,
+                                          b->ctx->num_sms, s));
+  allreduce(b->comm, bad.p, 3, kNcclUint32, kNcclMax, s);
+  uint32_t h[3] = {0, 0, 0};
   CUDA_CHECK(cudaMemcpyAsync(h, bad.p, sizeof(h), cudaMemcpyDeviceToHost, s));
   CUDA_CHECK(cudaStreamSynchronize(s));
+  if (h[2]) fail("rank:map: labels must be 0 or 1 (binary relevance); use rank:ndcg for graded relevance");
   if (h[0]) fail("%s: labels must be finite and >= 0", b->p.objective_name.c_str());
   if (h[1]) fail("%s: with ndcg_exp_gain the labels must be <= 31 (the gain is 2^label - 1); set ndcg_exp_gain=false "
                  "for larger relevance degrees", b->p.objective_name.c_str());
@@ -2148,15 +2154,18 @@ void rank_gradient(Booster* b, const float* margin, uint32_t* absmax, uint32_t* 
     b->idcg_uid = m->uid; b->idcg_version = m->rank_version; b->idcg_k = p.rank_k; b->idcg_gain = (int)p.ndcg_exp_gain;
   }
   b->rank_order.run(m, margin, sms, s);
+  const bool map = p.objective == kObjRankMap;
   if (m->max_qgroup > b2_rank_stage_rows()) {
     const size_t rows = (size_t)std::max<int64_t>(m->n, 1);
     b->rank_scratch_m.ensure(rows); b->rank_scratch_y.ensure(rows); b->rank_scratch_p.ensure(rows);
+    if (map) { b->rank_scratch_a.ensure(rows); b->rank_scratch_r.ensure(rows); }
   }
-  LAUNCH_CHECK(b2_launch_lambdarank_gradient(ndcg ? 1 : 0, m->qgroup_ptr.p, m->n_qgroups, m->max_qgroup,
+  LAUNCH_CHECK(b2_launch_lambdarank_gradient(map ? 2 : ndcg ? 1 : 0, m->qgroup_ptr.p, m->n_qgroups, m->max_qgroup,
                                              b->rank_order.keys_sorted.p, b->rank_order.rows.p, m->label.p,
                                              ndcg ? b->rank_inv_idcg.p : nullptr, b->rank_disc.p, p.rank_k,
                                              p.ndcg_exp_gain ? 1 : 0, b->rank_scratch_m.p, b->rank_scratch_y.p,
-                                             b->rank_scratch_p.p, b->gh.p, absmax, err, sms, s));
+                                             b->rank_scratch_p.p, map ? b->rank_scratch_a.p : nullptr,
+                                             map ? b->rank_scratch_r.p : nullptr, b->gh.p, absmax, err, sms, s));
 }
 
 // labels outside the objective's domain fail training (xgboost's CheckLabel); once per train matrix, before the first tree

@@ -1,5 +1,5 @@
-// rank_kernel.cu -- learning to rank: the per-group model order, LambdaMART gradients of rank:pairwise / rank:ndcg
-// (xgboost 2.x, lambdarank_pair_method=topk) and the per-group ndcg / map / pre metrics.
+// rank_kernel.cu -- learning to rank: the per-group model order, LambdaMART gradients of rank:pairwise / rank:ndcg /
+// rank:map (xgboost 2.x, lambdarank_pair_method=topk) and the per-group ndcg / map / pre metrics.
 //
 // A query group is a run of rows [gptr[g], gptr[g+1]) of one worker's matrix; the host keeps every group whole on one
 // worker, so nothing here crosses a worker.  The rules (DESIGN.md 2, item 13) are restated operation for operation by
@@ -67,34 +67,52 @@ __global__ void rank_inv_idcg_kernel(const int64_t* __restrict__ gptr, int64_t n
 }
 
 // labels of a rank objective (once per train matrix): bad[0] a label that is NaN, infinite or negative,
-// bad[1] a label above 31 with ndcg_exp_gain (2^y - 1 would not be exact)
-__global__ void rank_label_check_kernel(const float* __restrict__ label, int64_t n, int exp_gain, uint32_t* __restrict__ bad) {
-  bool b0 = false, b1 = false;
+// bad[1] a label above 31 with ndcg_exp_gain (2^y - 1 would not be exact), bad[2] with `binary` (rank:map) a label
+// that is neither 0 nor 1
+__global__ void rank_label_check_kernel(const float* __restrict__ label, int64_t n, int exp_gain, int binary,
+                                        uint32_t* __restrict__ bad) {
+  bool b0 = false, b1 = false, b2 = false;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const float y = label[i];
     b0 |= !(y >= 0.0f) || isinf(y);
     b1 |= exp_gain && y > 31.0f;
+    b2 |= binary && !(y == 0.0f || y == 1.0f);
   }
   if (__any_sync(0xffffffffu, b0) && (threadIdx.x & 31) == 0) atomicOr(&bad[0], 1u);
   if (__any_sync(0xffffffffu, b1) && (threadIdx.x & 31) == 0) atomicOr(&bad[1], 1u);
+  if (__any_sync(0xffffffffu, b2) && (threadIdx.x & 31) == 0) atomicOr(&bad[2], 1u);
 }
 
+// the pair weight of lambdarank_gradient_kernel: 1, |Delta NDCG| or |Delta AP|
+enum RankMode { kRankPairwise = 0, kRankNdcg = 1, kRankMap = 2 };
+
 // the pair (a, b) of model positions ra < rb with different labels: returns (float lambda, float H); *a_high says
-// whether a has the larger label
-template <bool kNdcg>
+// whether a has the larger label.  rank:map reads the group's hit counts R and hit prefixes A (inclusive, by model
+// position) and its hit count n_hits
+template <int kMode>
 __device__ __forceinline__ float2 lambda_pair(float sa, float ya, int ra, float sb, float yb, int rb, bool exp_gain,
-                                              const double* __restrict__ disc, double inv_idcg, bool scale_by_diff,
-                                              bool* a_high) {
+                                              const double* __restrict__ disc, double inv_idcg, const double* A,
+                                              const int32_t* R, double n_hits, bool scale_by_diff, bool* a_high) {
   const bool ah = ya > yb;
   *a_high = ah;
   const float d = ah ? __fadd_rn(sa, -sb) : __fadd_rn(sb, -sa);
   const double sig = (double)b2_sigmoid(d);
   double delta = 1.0;
-  if (kNdcg) {
+  if (kMode == kRankNdcg) {
     const double gh = rank_gain(ah ? ya : yb, exp_gain), gl = rank_gain(ah ? yb : ya, exp_gain);
     const double dh = disc[ah ? ra : rb], dl = disc[ah ? rb : ra];
     const double t = B2_DS(B2_DA(B2_DM(gh, dh), B2_DM(gl, dl)), B2_DA(B2_DM(gl, dh), B2_DM(gh, dl)));
     delta = fabs(B2_DM(t, inv_idcg));
+  } else if (kMode == kRankMap) {
+    // swap of positions ra < rb (DESIGN.md 2, item 13).  ah: the hit at ra moves down to rb,
+    //   N dAP = R_b/(b+1) - R_a/(a+1) - (A_{b-1} - A_a);
+    // else the hit at rb moves up to ra,
+    //   N dAP = (R_a+1)/(a+1) - R_b/(b+1) + (A_{b-1} - A_a)
+    const double ta = B2_DD((double)(ah ? R[ra] : R[ra] + 1), (double)(ra + 1));
+    const double tb = B2_DD((double)R[rb], (double)(rb + 1));
+    const double between = B2_DS(A[rb - 1], A[ra]);
+    const double num = ah ? B2_DS(B2_DS(tb, ta), between) : B2_DA(B2_DS(ta, tb), between);
+    delta = fabs(B2_DD(num, n_hits));
   }
   if (scale_by_diff) delta = B2_DD(delta, B2_DA((double)fabsf(d), 0.01));
   const double lam = B2_DM(B2_DS(sig, 1.0), delta);
@@ -111,13 +129,20 @@ __device__ __forceinline__ float2 lambda_pair(float sa, float ya, int ra, float 
 // -2 lambda(r, j) in binary64, S = sum_r P_r by one thread in r order, then every row is scaled by log2(1 + S) / S when
 // S > 0.  Writes gh[row], the block's |g|, |h| maxima and *err when a
 // pair is not finite (written as (0, 0), like the other gradient kernels).
-template <bool kNdcg>
+//
+// rank:map first builds, for all n positions p of the group, R_p (hits up to p, int32) and A_p (sum of 1/(q + 1) over
+// the hits q <= p, binary64) in a fixed order: thread t sums the chunk [t c, (t + 1) c), c = ceil(n / 128), ascending;
+// thread 0 turns the 128 chunk totals into exclusive carries, ascending; then A_p = carry + local prefix.  Its stage
+// adds A (8 B) and R (4 B) per row after P, M, Y, plus the 128 chunk totals (1.5 KB), which always live in shared
+// memory; A and R of a group above the stage go to scratch_a / scratch_r.
+template <int kMode>
 __global__ void __launch_bounds__(kRankThreads)
 lambdarank_gradient_kernel(const int64_t* __restrict__ gptr, int64_t n_groups, const uint32_t* __restrict__ skeys,
                            const int32_t* __restrict__ srow, const float* __restrict__ label,
                            const double* __restrict__ inv_idcg, const double* __restrict__ disc, int k, int exp_gain,
                            int stage, float* __restrict__ scratch_m, float* __restrict__ scratch_y, double* __restrict__ scratch_p,
-                           float2* __restrict__ gh, uint32_t* __restrict__ absmax, uint32_t* __restrict__ err) {
+                           float2* __restrict__ gh, uint32_t* __restrict__ absmax, uint32_t* __restrict__ err,
+                           double* __restrict__ scratch_a, int32_t* __restrict__ scratch_r) {
   extern __shared__ __align__(16) unsigned char rank_smem[];
   __shared__ double s_norm;
   float mg = 0.0f, mh = 0.0f;
@@ -132,9 +157,45 @@ lambdarank_gradient_kernel(const int64_t* __restrict__ gptr, int64_t n_groups, c
     __syncthreads();                                   // the previous group's readers are done with the stage
     for (int p = threadIdx.x; p < n; p += blockDim.x) { M[p] = rank_key_value(skeys[beg + p]); Y[p] = label[srow[beg + p]]; }
     __syncthreads();
+    const double* A = nullptr;
+    const int32_t* Rh = nullptr;
+    double n_hits = 0.0;
+    if (kMode == kRankMap) {
+      double* tot_a = (double*)(rank_smem + (size_t)stage * 24);
+      int32_t* tot_r = (int32_t*)(rank_smem + (size_t)stage * 28 + kRankThreads * 8);
+      double* Aw = staged ? (double*)(rank_smem + (size_t)stage * 16) : scratch_a + beg;
+      int32_t* Rw = staged ? (int32_t*)(rank_smem + (size_t)stage * 24 + kRankThreads * 8) : scratch_r + beg;
+      const int chunk = (n + kRankThreads - 1) / kRankThreads;
+      const int p0 = min((int)threadIdx.x * chunk, n), p1 = min(p0 + chunk, n);
+      double a = 0.0;
+      int32_t c = 0;
+      for (int p = p0; p < p1; ++p) {
+        if (Y[p] != 0.0f) { ++c; a = B2_DA(a, B2_DD(1.0, (double)(p + 1))); }
+        Aw[p] = a; Rw[p] = c;
+      }
+      tot_a[threadIdx.x] = a; tot_r[threadIdx.x] = c;
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        double ca = 0.0;
+        int32_t cr = 0;
+        for (int t = 0; t < kRankThreads; ++t) {
+          const double ta = tot_a[t];
+          const int32_t tr = tot_r[t];
+          tot_a[t] = ca; tot_r[t] = cr;
+          ca = B2_DA(ca, ta); cr += tr;
+        }
+      }
+      __syncthreads();
+      const double ca = tot_a[threadIdx.x];
+      const int32_t cr = tot_r[threadIdx.x];
+      for (int p = p0; p < p1; ++p) { Aw[p] = B2_DA(ca, Aw[p]); Rw[p] += cr; }
+      __syncthreads();
+      A = Aw; Rh = Rw;
+      n_hits = n > 0 ? (double)Rw[n - 1] : 0.0;
+    }
     const int kk = n < k ? n : k;
     const bool scale = n > 0 && M[0] != M[n - 1];
-    const double inv = kNdcg ? inv_idcg[g] : 0.0;
+    const double inv = kMode == kRankNdcg ? inv_idcg[g] : 0.0;
     for (int r = threadIdx.x; r < n; r += blockDim.x) {
       const float sr = M[r], yr = Y[r];
       float gr = 0.0f, hr = 0.0f;
@@ -143,7 +204,7 @@ lambdarank_gradient_kernel(const int64_t* __restrict__ gptr, int64_t n_groups, c
       for (int i = 0; i < lim; ++i) {
         const float yi = Y[i];
         if (yi == yr) continue;
-        const float2 pg = lambda_pair<kNdcg>(M[i], yi, i, sr, yr, r, exp_gain, disc, inv, scale, &hi);
+        const float2 pg = lambda_pair<kMode>(M[i], yi, i, sr, yr, r, exp_gain, disc, inv, A, Rh, n_hits, scale, &hi);
         gr = __fadd_rn(gr, hi ? -pg.x : pg.x);         // hi: position i is the high member, r the low one
         hr = __fadd_rn(hr, pg.y);
       }
@@ -152,7 +213,7 @@ lambdarank_gradient_kernel(const int64_t* __restrict__ gptr, int64_t n_groups, c
         for (int j = r + 1; j < n; ++j) {
           const float yj = Y[j];
           if (yj == yr) continue;
-          const float2 pg = lambda_pair<kNdcg>(sr, yr, r, M[j], yj, j, exp_gain, disc, inv, scale, &hi);
+          const float2 pg = lambda_pair<kMode>(sr, yr, r, M[j], yj, j, exp_gain, disc, inv, A, Rh, n_hits, scale, &hi);
           gr = __fadd_rn(gr, hi ? pg.x : -pg.x);
           hr = __fadd_rn(hr, pg.y);
           pr = B2_DA(pr, B2_DM(-2.0, (double)pg.x));
@@ -285,29 +346,45 @@ int b2_launch_rank_inv_idcg(const int64_t* gptr, int64_t n_groups, const uint32_
   b2::rank_inv_idcg_kernel<<<rank_grid(n_groups, 128, num_sms), 128, 0, s>>>(gptr, n_groups, lkeys, disc, k, exp_gain, inv_idcg);
   return (int)cudaGetLastError();
 }
-int b2_launch_rank_label_check(const float* label, int64_t n, int exp_gain, uint32_t* bad, int num_sms, cudaStream_t s) {
+// bad: 3 flags (rank_label_check_kernel); binary = 1 for rank:map
+int b2_launch_rank_label_check(const float* label, int64_t n, int exp_gain, int binary, uint32_t* bad, int num_sms,
+                               cudaStream_t s) {
   if (n <= 0) return 0;
-  b2::rank_label_check_kernel<<<rank_grid(n, 256, num_sms), 256, 0, s>>>(label, n, exp_gain, bad);
+  b2::rank_label_check_kernel<<<rank_grid(n, 256, num_sms), 256, 0, s>>>(label, n, exp_gain, binary, bad);
   return (int)cudaGetLastError();
 }
-// max_group: the largest group (sizes the shared-memory stage); scratch_*: [n] when max_group > b2_rank_stage_rows()
-int b2_launch_lambdarank_gradient(int ndcg, const int64_t* gptr, int64_t n_groups, int64_t max_group, const uint32_t* skeys,
+// mode: 0 rank:pairwise, 1 rank:ndcg, 2 rank:map.  max_group: the largest group (sizes the shared-memory stage);
+// scratch_m / y / p: [n] when max_group > b2_rank_stage_rows(), and with mode 2 scratch_a / r too (null otherwise)
+int b2_launch_lambdarank_gradient(int mode, const int64_t* gptr, int64_t n_groups, int64_t max_group, const uint32_t* skeys,
                                   const int32_t* srow, const float* label, const double* inv_idcg, const double* disc, int k,
-                                  int exp_gain, float* scratch_m, float* scratch_y, double* scratch_p, float2* gh,
-                                  uint32_t* absmax, uint32_t* err, int num_sms, cudaStream_t s) {
+                                  int exp_gain, float* scratch_m, float* scratch_y, double* scratch_p, double* scratch_a,
+                                  int32_t* scratch_r, float2* gh, uint32_t* absmax, uint32_t* err, int num_sms, cudaStream_t s) {
   if (n_groups <= 0) return 0;
   const int grid = (int)(n_groups < (int64_t)num_sms * 16 ? n_groups : (int64_t)num_sms * 16);
-  // the stage holds the largest group (up to kRankStageRows rows: at most 32 KB, no opt-in to large shared memory)
+  // the stage holds the largest group, up to kRankStageRows rows: at most 32 KB for pairwise / ndcg (16 B per row, no
+  // opt-in to large shared memory); rank:map adds 12 B per row and the chunk totals, up to 57.5 KB, and opts in
   const int stage = (int)(max_group < b2::kRankStageRows ? (max_group < 1 ? 1 : max_group) : b2::kRankStageRows);
+  if (mode == b2::kRankMap) {
+    const size_t smem = (size_t)stage * (8 + 4 + 4 + 8 + 4) + b2::kRankThreads * (8 + 4);
+    if (smem > 48 * 1024) {
+      const cudaError_t e = cudaFuncSetAttribute(b2::lambdarank_gradient_kernel<b2::kRankMap>,
+                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      if (e != cudaSuccess) return (int)e;
+    }
+    b2::lambdarank_gradient_kernel<b2::kRankMap><<<grid, b2::kRankThreads, smem, s>>>(
+        gptr, n_groups, skeys, srow, label, inv_idcg, disc, k, exp_gain, stage, scratch_m, scratch_y, scratch_p, gh, absmax, err,
+        scratch_a, scratch_r);
+    return (int)cudaGetLastError();
+  }
   const size_t smem = (size_t)stage * (8 + 4 + 4);
-  if (ndcg)
-    b2::lambdarank_gradient_kernel<true><<<grid, b2::kRankThreads, smem, s>>>(gptr, n_groups, skeys, srow, label, inv_idcg, disc, k,
+  if (mode == b2::kRankNdcg)
+    b2::lambdarank_gradient_kernel<b2::kRankNdcg><<<grid, b2::kRankThreads, smem, s>>>(gptr, n_groups, skeys, srow, label, inv_idcg, disc, k,
                                                                             exp_gain, stage, scratch_m, scratch_y, scratch_p, gh,
-                                                                            absmax, err);
+                                                                            absmax, err, nullptr, nullptr);
   else
-    b2::lambdarank_gradient_kernel<false><<<grid, b2::kRankThreads, smem, s>>>(gptr, n_groups, skeys, srow, label, inv_idcg, disc, k,
+    b2::lambdarank_gradient_kernel<b2::kRankPairwise><<<grid, b2::kRankThreads, smem, s>>>(gptr, n_groups, skeys, srow, label, inv_idcg, disc, k,
                                                                              exp_gain, stage, scratch_m, scratch_y, scratch_p, gh,
-                                                                             absmax, err);
+                                                                             absmax, err, nullptr, nullptr);
   return (int)cudaGetLastError();
 }
 // per-group metric values into vals [n_groups], then out[0] = their sum, out[1] = n_groups

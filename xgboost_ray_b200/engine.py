@@ -536,8 +536,8 @@ class _Objective:
     def default_metric(self, params):
         if self.metric == "tweedie-nloglik":   # the metric carries the objective's variance power in its name
             return "tweedie-nloglik@%g" % float(params.get("tweedie_variance_power", 1.5))
-        if self.metric == "ndcg":              # ranking: ndcg at the objective's pair cut-off
-            return "ndcg@%d" % int(params.get("lambdarank_num_pair_per_sample", 32))
+        if self.metric in ("ndcg", "map"):     # ranking: ndcg / map at the objective's pair cut-off
+            return "%s@%d" % (self.metric, int(params.get("lambdarank_num_pair_per_sample", 32)))
         return self.metric
 
 
@@ -561,6 +561,7 @@ _OBJECTIVES = {
                                {"aft_loss_distribution": "normal", "aft_loss_distribution_scale": 1}),
     "rank:pairwise": _Objective("ndcg", None, *_LAMBDARANK),
     "rank:ndcg": _Objective("ndcg", None, *_LAMBDARANK),
+    "rank:map": _Objective("map", None, *_LAMBDARANK),           # binary relevance; ndcg_exp_gain is kept, unused
     # one output per alpha; the block's value is the alphas' list string (quantile_alpha_text)
     "reg:quantileerror": _Objective("quantile", None, "reg_quantileerror_param", {"quantile_alpha": "[0.5]"}),
     "multi:softprob": _Objective("mlogloss", "softmax", *_SOFTMAX),
@@ -1255,6 +1256,9 @@ class Booster:
         objective = {"name": self.params.get("objective", "reg:squarederror")}
         if objective["name"] == "reg:quantileerror":
             objective["reg_quantileerror_param"] = {"quantile_alpha": quantile_alpha_text(self.params.get("quantile_alpha"))}
+        # rank:map reports the model file's lambdarank_param block (rank:pairwise / rank:ndcg keep their name-only entry)
+        if objective["name"] == "rank:map":
+            objective[_LAMBDARANK[0]] = {k: _str_param(self.params.get(k, d)) for k, d in _LAMBDARANK[1].items()}
         return json.dumps({"learner": {"gradient_booster": gbtree,
                                        "objective": objective,
                                        "b2_params": {k: v for k, v in self.params.items() if _json_ok(v)}},
