@@ -88,14 +88,17 @@ int B2_MatrixGetFeatureTypes(B2Handle m, uint8_t* is_cat /*[n_cols]*/);
 int B2_MatrixNumRow(B2Handle m, int64_t* out);
 int B2_MatrixNumCol(B2Handle m, int32_t* out);
 /* GPU quantile sketch (global over `comm`, 0 = single process) + binning into the device uint8
- * matrix.  ref != 0 reuses the cuts of an already quantised matrix.  keep_raw == 0 frees the
+ * matrix.  ref != 0 reuses the cuts of an already quantised matrix; a category code of this matrix
+ * that those cuts do not know is then an error (checked over `comm`).  keep_raw == 0 frees the
  * device copy of the float data afterwards (it is needed again only for Predict on this matrix). */
 int B2_MatrixQuantize(B2Handle m, B2Handle comm, int32_t max_bin, B2Handle ref, int32_t keep_raw);
-/* Quantise with GIVEN cut points (no sketch, no communication): a restart after an actor failure continues with the
+/* Quantise with GIVEN cut points (no sketch): a restart after an actor failure continues with the
  * cuts of the first attempt even when the world size changed, so old and new trees split on the same bins
- * (xgboost_ray/elastic.py:19-178, main.py:1644-1713; SURVEY.md 5 "freeze cuts from attempt 0"). */
-int B2_MatrixQuantizeWithCuts(B2Handle m, const int32_t* ptrs /*[F+1]*/, const float* vals, const float* mins /*[F]*/,
-                              const uint8_t* has_missing /*[F]*/, int32_t max_bin, int32_t keep_raw);
+ * (xgboost_ray/elastic.py:19-178, main.py:1644-1713; SURVEY.md 5 "freeze cuts from attempt 0").  A category code
+ * the cuts do not know is an error; `comm` (0 = single process) only makes that check global. */
+int B2_MatrixQuantizeWithCuts(B2Handle m, B2Handle comm, const int32_t* ptrs /*[F+1]*/, const float* vals,
+                              const float* mins /*[F]*/, const uint8_t* has_missing /*[F]*/, int32_t max_bin,
+                              int32_t keep_raw);
 /* re-upload the float data of a matrix whose device copy was freed (same shape) */
 int B2_MatrixEnsureRaw(B2Handle m, const float* data);
 int B2_MatrixCutsSize(B2Handle m, int32_t* total_cuts);

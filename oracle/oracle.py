@@ -192,6 +192,17 @@ class Cuts:
             lib().or_cuts_set_cat(h, _bp(np.ascontiguousarray(is_cat, np.uint8)))
         return cls(h, f, max_bin)
 
+    def borrowed_by(self, X, missing=np.nan):
+        """The cuts a matrix X trains with when it borrows these ones (DESIGN.md §2 item 6): a categorical feature
+        that has missing values in X is marked has_missing, so that its bin 255 is routed by the default direction
+        (as prediction routes a missing value) rather than as an unknown category.  Numeric features keep theirs."""
+        X = _f32(X)
+        miss = np.isnan(X) if np.isnan(missing) else (np.isnan(X) | (X == np.float32(missing)))
+        hm = self.has_missing | (self.is_cat.astype(bool) & miss.any(axis=0)).astype(np.uint8)
+        if np.array_equal(hm, self.has_missing):
+            return self
+        return Cuts.from_arrays(self.ptrs, self.vals, self.mins, hm, self.max_bin, is_cat=self.is_cat)
+
     def bin(self, X, missing=np.nan):
         X = _f32(X)
         n, f = X.shape
@@ -364,9 +375,12 @@ class Booster:
 
 def train(params, X, y, num_boost_round, weight=None, missing=np.nan, cuts=None, base_margin=None, is_cat=None,
           feature_weights=None):
-    """Convenience: cuts -> bins -> rounds.  Returns (Booster, bins)."""
+    """Convenience: cuts -> bins -> rounds.  Returns (Booster, bins).  `cuts` are borrowed (Cuts.borrowed_by)."""
     X = _f32(X)
-    cuts = cuts or Cuts.from_data(X, int(params.get("max_bin", 256)), missing, is_cat=is_cat, weight=weight)
+    if cuts is not None:
+        cuts = cuts.borrowed_by(X, missing)
+    else:
+        cuts = Cuts.from_data(X, int(params.get("max_bin", 256)), missing, is_cat=is_cat, weight=weight)
     bins = cuts.bin(X, missing)
     bst = Booster(params, cuts)
     if feature_weights is not None:

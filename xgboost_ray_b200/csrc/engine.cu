@@ -19,6 +19,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <climits>
 #include <chrono>
 #include <map>
 #include <mutex>
@@ -567,6 +568,57 @@ void upload_cuts(Matrix* m) {
   CUDA_CHECK(cudaStreamSynchronize(s));
 }
 
+// Categorical features: global {max code, has missing, largest invalid value's key} per entry of m->cat_feats
+// (cat_stats_kernel, allreduce max over the ranks).  Synchronises the stream.
+std::vector<int32_t> category_stats(Matrix* m, Comm* comm) {
+  cudaStream_t s = m->ctx->stream;
+  const int n_cat = (int)m->cat_feats.size();
+  std::vector<int32_t> h_cat((size_t)n_cat * 3);
+  if (n_cat == 0) { CUDA_CHECK(cudaStreamSynchronize(s)); return h_cat; }   // callers read earlier copies after this
+  for (int i = 0; i < n_cat; ++i) { h_cat[i * 3] = -1; h_cat[i * 3 + 1] = 0; h_cat[i * 3 + 2] = INT_MIN; }
+  DevBuf<int32_t> d_cat, d_catf;
+  d_cat.ensure((size_t)n_cat * 3); d_catf.ensure((size_t)n_cat);
+  CUDA_CHECK(cudaMemcpyAsync(d_cat.p, h_cat.data(), (size_t)n_cat * 3 * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  CUDA_CHECK(cudaMemcpyAsync(d_catf.p, m->cat_feats.data(), (size_t)n_cat * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  LAUNCH_CHECK(b2_launch_cat_stats(m->raw.p, m->n, m->F, m->missing, d_catf.p, n_cat, d_cat.p, m->ctx->num_sms, s));
+  allreduce(comm, d_cat.p, (size_t)n_cat * 3, kNcclInt32, kNcclMax, s);
+  CUDA_CHECK(cudaMemcpyAsync(h_cat.data(), d_cat.p, (size_t)n_cat * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  return h_cat;
+}
+// the value behind cat_stats_kernel's signed order-preserving key
+double category_key_value(int32_t key) {
+  const uint32_t k = (uint32_t)key ^ 0x80000000u;
+  const uint32_t u = (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k;
+  float f; memcpy(&f, &u, sizeof(f));
+  return (double)f;
+}
+
+// Borrowed cuts (a ref matrix, or the frozen cuts of a restart) were made from other data.  bin_kernel clamps a code
+// they do not know to their largest code (a negative one to 0), and a code of 255 shares bin 255 with the missing
+// values, while prediction sends every unknown code left: training would see another category than predict().
+// Such codes are refused, as make_cuts refuses codes that are not valid, instead of silently changing the model.
+void check_borrowed_categories(Matrix* m, Comm* comm) {
+  const std::vector<int32_t> h_cat = category_stats(m, comm);
+  for (size_t i = 0; i < m->cat_feats.size(); ++i) {
+    const int f = m->cat_feats[i], mx = h_cat[i * 3], miss = h_cat[i * 3 + 1];
+    const int known = m->cut_ptrs[f + 1] - m->cut_ptrs[f] - 1;   // the cuts of a categorical feature are the codes 0..known
+    if (h_cat[i * 3 + 2] != INT_MIN)
+      fail("categorical feature %d: category codes must be integers in [0, %d], got %.9g", f, known,
+           category_key_value(h_cat[i * 3 + 2]));
+    if (mx > known)
+      fail("categorical feature %d: category code %d is above the largest code %d of the cuts this matrix is binned with",
+           f, mx, known);
+    if (miss && known > 254)
+      fail("categorical feature %d: the feature has missing values, but its cuts use bin 255 (the missing sentinel) for "
+           "category code 255", f);
+    // cuts borrowed from a matrix without missing values: the split scan and partition must still treat bin 255 as
+    // missing (default direction), as prediction does, instead of as an unknown category.  The oracle applies the same
+    // rule when it trains with borrowed cuts (oracle.train(cuts=...), Cuts.borrowed_by).
+    if (miss) m->has_missing[f] = 1;
+  }
+}
+
 // GPU sketch: exact global summary per feature -> cuts (sketch.cu).  No host round trip per feature.
 // Multi-GPU: the column keys of every rank are allgathered (padded to the largest shard); feature f is
 // sorted and pruned only by its owner rank f % world, and the cut tables are merged with one integer
@@ -661,25 +713,14 @@ void make_cuts(Matrix* m, Comm* comm, int max_bin) {
   allreduce(comm, d_tab.p, tab_n, kNcclInt32, kNcclSum, s);
   std::vector<int32_t> h_tab(tab_n);
   CUDA_CHECK(cudaMemcpyAsync(h_tab.data(), d_tab.p, tab_n * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  // categorical features: global max code / has-missing / invalid flags (allreduce max)
   const int n_cat = (int)m->cat_feats.size();
-  std::vector<int32_t> h_cat((size_t)std::max(n_cat, 1) * 3, 0);
-  DevBuf<int32_t> d_cat, d_catf;
-  if (n_cat > 0) {
-    for (int i = 0; i < n_cat; ++i) { h_cat[i * 3] = -1; h_cat[i * 3 + 1] = 0; h_cat[i * 3 + 2] = 0; }
-    d_cat.ensure((size_t)n_cat * 3); d_catf.ensure((size_t)n_cat);
-    CUDA_CHECK(cudaMemcpyAsync(d_cat.p, h_cat.data(), (size_t)n_cat * 3 * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    CUDA_CHECK(cudaMemcpyAsync(d_catf.p, m->cat_feats.data(), (size_t)n_cat * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    LAUNCH_CHECK(b2_launch_cat_stats(m->raw.p, m->n, F, m->missing, d_catf.p, n_cat, d_cat.p, ctx->num_sms, s));
-    allreduce(comm, d_cat.p, (size_t)n_cat * 3, kNcclInt32, kNcclMax, s);
-    CUDA_CHECK(cudaMemcpyAsync(h_cat.data(), d_cat.p, (size_t)n_cat * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  }
-  CUDA_CHECK(cudaStreamSynchronize(s));
+  const std::vector<int32_t> h_cat = category_stats(m, comm);   // synchronises the stream
   for (int i = 0; i < n_cat; ++i) {
     const int f = m->cat_feats[i], mx = h_cat[i * 3], miss = h_cat[i * 3 + 1];
-    if (h_cat[i * 3 + 2] || (miss && mx > 254))
-      fail("categorical feature %d: category codes must be integers in [0, %d]%s", f, miss ? 254 : 255,
-           miss ? " (the feature has missing values; bin 255 is the missing sentinel)" : "");
+    if (h_cat[i * 3 + 2] != INT_MIN || (miss && mx > 254))
+      fail("categorical feature %d: category codes must be integers in [0, %d]%s, got %.9g", f, miss ? 254 : 255,
+           miss ? " (the feature has missing values; bin 255 is the missing sentinel)" : "",
+           h_cat[i * 3 + 2] != INT_MIN ? category_key_value(h_cat[i * 3 + 2]) : (double)mx);
     int32_t* t = h_tab.data();
     float* cuts_f = (float*)t + (size_t)f * 256;
     const int nc = mx < 0 ? 1 : mx + 1;
@@ -2898,6 +2939,7 @@ int B2_MatrixQuantize(B2Handle mh, B2Handle commh, int32_t max_bin, B2Handle ref
     if (r->F != m->F) fail("reference matrix has %d features, this one %d", r->F, m->F);
     m->cut_ptrs = r->cut_ptrs; m->cut_vals = r->cut_vals; m->min_vals = r->min_vals; m->has_missing = r->has_missing; m->max_bin = r->max_bin;
     m->is_cat = r->is_cat; m->cat_feats = r->cat_feats;
+    check_borrowed_categories(m, comm);
   } else {
     make_cuts(m, comm, max_bin);
   }
@@ -2905,11 +2947,12 @@ int B2_MatrixQuantize(B2Handle mh, B2Handle commh, int32_t max_bin, B2Handle ref
   if (!keep_raw) { m->raw.release(); m->has_raw = false; }
   API_END
 }
-int B2_MatrixQuantizeWithCuts(B2Handle mh, const int32_t* ptrs, const float* vals, const float* mins, const uint8_t* has_missing,
-                              int32_t max_bin, int32_t keep_raw) {
+int B2_MatrixQuantizeWithCuts(B2Handle mh, B2Handle commh, const int32_t* ptrs, const float* vals, const float* mins,
+                              const uint8_t* has_missing, int32_t max_bin, int32_t keep_raw) {
   API_BEGIN
   Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
   CUDA_CHECK(cudaSetDevice(m->ctx->device));
+  Comm* comm = commh ? &from_handle<CommH>(commh, kComm, "communicator")->c : nullptr;
   if (!m->has_raw) fail("matrix has no raw data on the device (already quantised without keep_raw?)");
   if (max_bin < 2 || max_bin > 256) fail("max_bin must be in [2, 256] (uint8 bin matrix), got %d", max_bin);
   if (ptrs[0] != 0) fail("cut pointers must start at 0");
@@ -2922,6 +2965,7 @@ int B2_MatrixQuantizeWithCuts(B2Handle mh, const int32_t* ptrs, const float* val
   m->min_vals.assign(mins, mins + m->F);
   m->has_missing.assign(has_missing, has_missing + m->F);
   m->max_bin = max_bin;
+  check_borrowed_categories(m, comm);
   bin_matrix(m);
   if (!keep_raw) { m->raw.release(); m->has_raw = false; }
   API_END

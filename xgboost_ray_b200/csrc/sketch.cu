@@ -192,8 +192,9 @@ prune_cuts_kernel(const float* __restrict__ uval, const long long* __restrict__ 
 }
 
 // Categorical columns (HistogramCuts::AddCategories, src/common/quantile.cc): the cuts are the codes 0..max, so
-// the only statistics needed are the largest code, whether a value is missing and whether a value is not a
-// valid code.  stats [n_cat][3] int32 = {max code (init -1), has_missing, invalid}; merged with an allreduce(max).
+// the only statistics needed are the largest code, whether a value is missing and which values are not valid
+// codes.  stats [n_cat][3] int32 = {max code (init -1), has_missing, largest invalid value (init INT_MIN) as the
+// signed order-preserving key f2key(x) ^ 0x80000000, so the error can name it}; merged with an allreduce(max).
 __global__ void cat_stats_kernel(const float* __restrict__ X, int64_t n, int F, float missing, int missing_is_nan,
                                  const int32_t* __restrict__ cat_feats, int n_cat, int32_t* __restrict__ stats) {
   const int64_t total = n * n_cat;
@@ -201,7 +202,10 @@ __global__ void cat_stats_kernel(const float* __restrict__ X, int64_t n, int F, 
     const int64_t row = e / n_cat; const int ci = (int)(e - row * n_cat);
     const float x = X[row * F + cat_feats[ci]];
     if (is_missing(x, missing, missing_is_nan)) { if (stats[ci * 3 + 1] == 0) atomicMax(&stats[ci * 3 + 1], 1); continue; }
-    if (!(x >= 0.0f) || x > 255.0f || x != (float)(int)x) { atomicMax(&stats[ci * 3 + 2], 1); continue; }
+    if (!(x >= 0.0f) || x > 255.0f || x != (float)(int)x) {
+      atomicMax(&stats[ci * 3 + 2], (int32_t)(f2key(x) ^ 0x80000000u));
+      continue;
+    }
     const int c = (int)x;
     if (stats[ci * 3] < c) atomicMax(&stats[ci * 3], c);
   }
@@ -407,7 +411,7 @@ int b2_launch_bin(const float* X, int64_t n, int F, float missing, const int32_t
                                                         feat_byte, is_cat, row_stride, bins, bins_col, col_stride);
   return (int)cudaGetLastError();
 }
-// stats must be initialised to {-1, 0, 0} per categorical feature
+// stats must be initialised to {-1, 0, INT_MIN} per categorical feature
 int b2_launch_cat_stats(const float* X, int64_t n, int F, float missing, const int32_t* cat_feats, int n_cat, int32_t* stats,
                         int num_sms, cudaStream_t s) {
   if (n <= 0 || n_cat <= 0) return 0;

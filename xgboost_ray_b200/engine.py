@@ -35,6 +35,7 @@ _IP = C.POINTER(C.c_int32)
 _BP = C.POINTER(C.c_uint8)
 _DP = C.POINTER(C.c_double)
 _H = C.c_uint64
+_FLT_MAX = np.finfo(np.float32).max
 
 # name -> (restype, argtypes); every symbol declared in include/b2hist.h
 ABI = {
@@ -61,7 +62,7 @@ ABI = {
     "B2_MatrixNumRow": (C.c_int, [_H, C.POINTER(C.c_int64)]),
     "B2_MatrixNumCol": (C.c_int, [_H, C.POINTER(C.c_int32)]),
     "B2_MatrixQuantize": (C.c_int, [_H, _H, C.c_int32, _H, C.c_int32]),
-    "B2_MatrixQuantizeWithCuts": (C.c_int, [_H, _IP, _FP, _FP, _BP, C.c_int32, C.c_int32]),
+    "B2_MatrixQuantizeWithCuts": (C.c_int, [_H, _H, _IP, _FP, _FP, _BP, C.c_int32, C.c_int32]),
     "B2_MatrixEnsureRaw": (C.c_int, [_H, _FP]),
     "B2_MatrixCutsSize": (C.c_int, [_H, _IP]),
     "B2_MatrixGetCuts": (C.c_int, [_H, _IP, _FP, _FP, _BP]),
@@ -419,7 +420,8 @@ class DMatrix:
                                     np.ascontiguousarray(cuts[3], np.uint8))
             if ptrs.size != self.num_col() + 1:
                 raise XGBoostError("frozen cuts are for %d features, the matrix has %d" % (ptrs.size - 1, self.num_col()))
-            _check(lib().B2_MatrixQuantizeWithCuts(self.handle, _ip(ptrs), _fp(vals), _fp(mins), _bp(hm), mb, 1 if keep_raw else 0))
+            _check(lib().B2_MatrixQuantizeWithCuts(self.handle, _coll.handle, _ip(ptrs), _fp(vals), _fp(mins), _bp(hm), mb,
+                                                   1 if keep_raw else 0))
         else:
             ref_h = 0
             if self.ref is not None:
@@ -1062,8 +1064,14 @@ class Booster:
         # in the arrays above and xgboost does not read the number (RegTree::ExpandCategorical stores NaN, which is not
         # JSON): 0 is written instead
         cond = np.where(leaf, t["value"], np.where(st != 0, np.float32(0.0), t["split_cond"])).astype(np.float32)
+        # a numeric split on +inf (the last cut of a feature whose maximum is +inf or above FLT_MAX / 2) sends every
+        # finite value left.  Strict JSON gets the nearest finite float32 (FLT_MAX), which a stock reader routes alike
+        # except at x = FLT_MAX; the exact condition is returned as [node, "inf"] for the "b2.split_conds" attribute
+        numeric = ~leaf & (st == 0)
+        exact = [[int(nid), str(float(cond[nid]))] for nid in np.nonzero(numeric & ~np.isfinite(cond))[0]]
+        cond = np.where(numeric & ~np.isnan(cond), np.clip(cond, -_FLT_MAX, _FLT_MAX), cond)
         cond = np.where(np.isfinite(cond), cond, np.float32(0.0))
-        return {
+        return exact, {
             "base_weights": [float(x) for x in t["base_weight"]],
             "categories": cats, "categories_nodes": cat_nodes, "categories_segments": cat_segs,
             "categories_sizes": cat_sizes,
@@ -1088,7 +1096,8 @@ class Booster:
         if len(cache) > len(src):
             del cache[:]
         for i in range(len(cache), len(src)):
-            cache.append((self._tree_json(i, src[i], self.n_features), [int(x) for x in src[i]["split_bin"]]))
+            exact, tj = self._tree_json(i, src[i], self.n_features)
+            cache.append((tj, [int(x) for x in src[i]["split_bin"]], exact))
         trees = [c[0] for c in cache]
         obj = self.params.get("objective", "reg:squarederror")
         quantile = obj == "reg:quantileerror"   # xgboost counts the alphas as targets, not classes
@@ -1107,6 +1116,9 @@ class Booster:
             b2p["interaction_constraints"] = str(sets)
         attrs["b2.params"] = json.dumps({k: b2p[k] for k in sorted(b2p)})
         attrs["b2.split_bins"] = json.dumps([c[1] for c in cache], separators=(",", ":"))
+        exact = [[ti, nid, v] for ti, c in enumerate(cache) for nid, v in c[2]]
+        if exact:   # [tree, node, "inf"]: the non-finite numeric conditions, which split_conditions cannot hold
+            attrs["b2.split_conds"] = json.dumps(exact, separators=(",", ":"))
         gbtree = {"model": {
             "gbtree_model_param": {"num_parallel_tree": str(self.num_parallel_tree), "num_trees": str(len(trees))},
             "iteration_indptr": list(range(0, len(trees) + 1, K * self.num_parallel_tree)),
@@ -1149,6 +1161,9 @@ class Booster:
         attrs = dict(L.get("attributes", {}))
         params = dict(json.loads(attrs.pop("b2.params"))) if "b2.params" in attrs else dict(L.get("b2_params", {}))
         split_bins = json.loads(attrs.pop("b2.split_bins")) if "b2.split_bins" in attrs else None
+        exact_conds = {}    # tree -> [(node, condition)]
+        for ti, nid, v in json.loads(attrs.pop("b2.split_conds", "[]")):
+            exact_conds.setdefault(int(ti), []).append((int(nid), np.float32(float(v))))
         params["objective"] = L["objective"]["name"]
         nc = int(L["learner_model_param"].get("num_class", "0"))
         nc = max(nc, int(L["objective"].get("softmax_multiclass_param", {}).get("num_class", "0")))
@@ -1207,6 +1222,8 @@ class Booster:
                 cl = _cat_list(bits[nid])
                 b_ = int(sb[nid]) if sb is not None else (cl[0] if len(cl) == 1 else -1)
                 cond[nid] = np.float32(b_) if b_ >= 0 else np.float32("nan")
+            for nid, v in exact_conds.get(ti, ()):
+                cond[nid] = v
             self._trees.append(dict(
                 split_type=st, cat_bits=bits,
                 left=left, right=np.asarray(t["right_children"], np.int32), parent=parent,

@@ -157,7 +157,10 @@ class RayXGBMixin(BaseEstimator):
         return self
 
     def _predict(self, X, ray_params, ray_dmatrix_params, **kw):
-        data = X if isinstance(X, RayDMatrix) else RayDMatrix(X, **(ray_dmatrix_params or {}))
+        ray_dmatrix_params = dict(ray_dmatrix_params or {})
+        if not (isinstance(self.missing, float) and np.isnan(self.missing)):   # the sentinel the model was fitted with
+            ray_dmatrix_params.setdefault("missing", self.missing)
+        data = X if isinstance(X, RayDMatrix) else RayDMatrix(X, **ray_dmatrix_params)
         return predict(self.get_booster(), data, ray_params=self._ray_params(ray_params), **kw)
 
     def apply(self, X, iteration_range=None, ray_params=None, ray_dmatrix_params=None):
