@@ -74,6 +74,11 @@ int B2_MatrixCreateFromProcessInterleaved(int64_t pid, uint64_t remote_addr, int
  * "label_lower_bound" | "label_upper_bound" (len n_rows, 0 clears): the survival bounds of each row, read by
  * survival:aft only (lower == upper: exact time; upper = +inf: right-censored; lower = 0: left-censored) */
 int B2_MatrixSetFloatInfo(B2Handle m, const char* field, const float* values, int64_t len);
+/* label of T = n_targets columns, row-major [rows][T] (xgboost's 2-D label: multi-target regression, multi-label
+ * classification; xgboost_ray's list of label columns, matrix.py:308-313, 405-416).  rows must equal the matrix's rows,
+ * 1 <= T <= 4096; T = 1 is the same as B2_MatrixSetFloatInfo("label").  T > 1 is refused on a matrix with query
+ * groups or survival bounds.  A booster trained on the matrix grows T trees per round, one per column. */
+int B2_MatrixSetLabel(B2Handle m, const float* values, int64_t rows, int32_t n_targets);
 /* query groups of a ranking matrix (xgb.DMatrix(qid=...) / set_group; the reference sorts rows by qid and ships qid per
  * shard, xgboost_ray/matrix.py:70-100, 300-304, 483, 689 and main.py:371, 399, 431): group g is the next group_sizes[g]
  * rows.  Every size is >= 1 and the sizes sum to the row count; the engine builds the int64 row offsets itself.
@@ -149,6 +154,9 @@ int B2_BoosterResetTrainMargin(B2Handle b);
  * estimated from the labels of all workers before the first tree (xgboost >= 2.0 behaviour, SURVEY.md A.3);
  * is_final = 0 until that has happened. */
 int B2_BoosterGetBaseScore(B2Handle b, float* out, int32_t* is_final);
+/* label columns of the model (1 unless it is multi-target): fixed by the train matrix when the booster is created, or by
+ * num_target=<T> in params (a loaded model; a train matrix must then have T columns) */
+int B2_BoosterNumTargets(B2Handle b, int32_t* out);
 int B2_BoosterNumTrees(B2Handle b, int32_t* out);
 int B2_BoosterTreeNumNodes(B2Handle b, int32_t tree, int32_t* out);
 int B2_BoosterGetTree(B2Handle b, int32_t tree, int32_t* left, int32_t* right, int32_t* parent,

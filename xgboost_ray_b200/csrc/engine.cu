@@ -130,6 +130,10 @@ int b2_launch_rank_metric(int, int, int, int, const int64_t*, int64_t, const int
 size_t b2_auc_temp_bytes(int64_t);
 int b2_auc(int, int, const float*, const float*, const float*, int64_t, void*, size_t, double*, int, cudaStream_t);
 int b2_launch_transform(int, int, float*, int64_t, int, cudaStream_t);
+int b2_launch_gradient_multi_target(int, int, const float*, const float*, const float*, int64_t, float, float, float2*,
+                                    uint32_t*, uint32_t*, int, cudaStream_t);
+int b2_launch_metric_multi_target(int, int, int, float, const float*, const float*, const float*, int64_t, double*, int,
+                                  cudaStream_t);
 int b2_extract_batch();
 int b2_launch_extract_keys(const float*, int64_t, int, int, int, float, uint32_t*, int64_t, int, cudaStream_t);
 size_t b2_sort_temp_bytes(int64_t);
@@ -510,8 +514,10 @@ struct Matrix : HandleBase {
   DevBuf<float> d_cut_vals;
   DevBuf<uint8_t> d_has_missing, d_is_cat;
   bool any_cat() const { return !cat_feats.empty(); }
-  DevBuf<float> label, weight, base_margin;
+  DevBuf<float> label, weight, base_margin;   // label [n][n_targets] row-major
   int64_t n_label = 0, n_weight = 0, n_base_margin = 0;
+  int n_targets = 1;                    // label columns (B2_MatrixSetLabel); > 1: multi-target regression / multi-label
+  bool has_labels(int T) const { return n_targets == T && n_label == n * T; }
   DevBuf<float> lower, upper;          // survival label bounds (label_lower_bound / label_upper_bound), read by survival:aft
   int64_t n_lower = 0, n_upper = 0;
   bool has_bounds() const { return n_lower == n && n_upper == n; }
@@ -768,10 +774,20 @@ bool obj_rank(int o) { return o == kObjRankPairwise || o == kObjRankNdcg || o ==
 // objectives whose gradient kernel reports non-finite gradient pairs (gradient_param_kernel).  reg:quantileerror's
 // pairs are finite for finite labels and weights (both checked before the first round), so its rounds stay pipelined.
 bool obj_checks_finite(int o) { return o >= kObjSquaredLog && o != kObjQuantile; }
+// objectives that take a label of T > 1 columns (xgboost's RegLossObj family and pseudo-Huber, which read labels.Shape(1))
+bool obj_multi_target(int o) {
+  return o == kObjSquaredError || o == kObjLogistic || o == kObjRegLogistic || o == kObjLogitRaw || o == kObjSquaredLog ||
+         o == kObjPseudoHuber;
+}
+constexpr int kMaxTargets = 4096;   // label columns of one matrix (as many trees per round as num_parallel_tree allows)
 struct Params {
   int objective = kObjSquaredError;
   std::string objective_name = "reg:squarederror";
   int num_class = 1;
+  // label columns of a multi-target model (outputs per row; num_class then equals it).  Given as num_target when a model
+  // is loaded, otherwise taken from the train matrix when the booster is created (set_targets)
+  int num_target = 1;
+  bool num_target_set = false;
   int num_parallel_tree = 1;   // trees grown per class and round from the SAME gradients (random forests); leaf values are scaled by eta / n
   int max_depth = 6;
   float eta = 0.3f, gamma = 0.0f, min_child_weight = 1.0f, lambda = 1.0f, alpha = 0.0f, base_score = 0.5f;
@@ -1098,6 +1114,21 @@ std::vector<float> parse_quantile_alpha(std::string v) {
   return out;
 }
 
+// T label columns: one output and one tree per round for each (xgboost's multi_strategy=one_output_per_tree)
+void set_targets(Params* p, int T) {
+  if (T < 1 || T > kMaxTargets) fail("num_target must be in [1, %d], got %d", kMaxTargets, T);
+  if (T > 1) {
+    if (!obj_multi_target(p->objective))
+      fail("objective '%s' does not support a label with %d columns (multi-target objectives: reg:squarederror, "
+           "reg:squaredlogerror, reg:pseudohubererror, reg:logistic, binary:logistic, binary:logitraw)",
+           p->objective_name.c_str(), T);
+    if (p->num_class_set)
+      fail("num_class must not be set with a label of %d columns: a multi-target model has one output per column", T);
+    p->num_class = T;
+  }
+  p->num_target = T;
+}
+
 void parse_params(const char* text, Params* p, int* max_bin_out) {
   std::string s(text ? text : "");
   std::map<std::string, std::string> dart_text;
@@ -1133,6 +1164,7 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
                 "reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie, survival:aft, "
                 "rank:pairwise, rank:ndcg, rank:map, reg:quantileerror, multi:softprob, multi:softmax)", v.c_str());
     } else if (k == "num_class") { p->num_class = i(); p->num_class_set = true; }
+    else if (k == "num_target") { p->num_target = i(); p->num_target_set = true; }
     else if (k == "quantile_alpha") p->quantile_alpha = parse_quantile_alpha(v);
     else if (k == "num_parallel_tree") p->num_parallel_tree = i();
     else if (k == "max_depth") p->max_depth = i();
@@ -1226,6 +1258,7 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     p->num_class = (int)p->quantile_alpha.size();
   } else if (p->objective != kObjSoftprob) p->num_class = 1;
   if (p->objective == kObjSoftprob && p->num_class < 2) fail("multi:softprob needs num_class >= 2");
+  if (p->num_target_set) set_targets(p, p->num_target);
   if (p->max_depth < 1 || p->max_depth > 14) fail("max_depth must be in [1, 14], got %d", p->max_depth);
   if (p->num_parallel_tree < 1 || p->num_parallel_tree > 4096) fail("num_parallel_tree must be in [1, 4096], got %d", p->num_parallel_tree);
   if (p->qbits < 8 || p->qbits > 24) fail("hist_qbits must be in [8, 24], got %d", p->qbits);
@@ -2040,6 +2073,15 @@ const float* device_weights(Booster* b) {
   return b->d_tree_w.p;
 }
 
+// the train matrix holds one label per row and target: a label whose width differs from the model's targets (set after
+// the booster was created) names both
+void check_train_labels(const Booster* b) {
+  const Matrix* m = b->train; const int T = b->p.num_target;
+  if (m->n_label > 0 && m->n_targets != T)
+    fail("the train matrix's label has %d columns, the model has %d targets", m->n_targets, T);
+  if (m->n_label != m->n * T) fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)m->n);
+}
+
 void init_margin(Booster* b, float* margin, Matrix* m) {
   const int K = b->p.num_class; cudaStream_t s = b->ctx->stream;
   if (m->n_base_margin > 0) {
@@ -2058,7 +2100,7 @@ void estimate_base_score(Booster* b) {
   if (p.base_score_set || p.objective == kObjSoftprob) { p.base_score_set = true; return; }
   // existing trees were fitted around the intercept of the model they came from: never assume the default for them
   if (!b->trees.empty()) fail("continuing from existing trees needs an explicit base_score (the source model's intercept)");
-  if (m->n_label != m->n) fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)m->n);
+  check_train_labels(b);
   const int64_t n = m->n;
   if (p.objective == kObjQuantile) {
     // the fp32 mean over k of the weighted alpha_k-quantile of the labels (the leaf refresh's selection, one segment)
@@ -2086,30 +2128,44 @@ void estimate_base_score(Booster* b) {
     p.base_score_set = true;
     return;
   }
+  // T targets (DESIGN.md 2 item 18): one stump per target from its own slice of the class-major pairs, with its own
+  // exponents; the intercept is the fp32 sum over k, in k order, of fp32(stump_k / T) (stump_0 itself for T = 1)
+  const int T = p.num_target;
+  const size_t nt = (size_t)std::max<int64_t>(n * T, 1);
   DevBuf<float> zeros; DevBuf<float2> gh; DevBuf<long long> sums;
-  zeros.ensure((size_t)std::max<int64_t>(n, 1)); gh.ensure((size_t)std::max<int64_t>(n, 1)); sums.ensure(4);
-  CUDA_CHECK(cudaMemsetAsync(zeros.p, 0, (size_t)std::max<int64_t>(n, 1) * sizeof(float), s));
-  LAUNCH_CHECK(b2_launch_gradient(p.objective, 1, zeros.p, m->label.p, m->n_weight ? m->weight.p : nullptr, n, p.scale_pos_weight,
-                                  objective_param(p), gh.p, nullptr, nullptr, b->ctx->num_sms, s));
+  zeros.ensure(nt); gh.ensure(nt); sums.ensure(4);
+  CUDA_CHECK(cudaMemsetAsync(zeros.p, 0, nt * sizeof(float), s));
+  if (T > 1)
+    LAUNCH_CHECK(b2_launch_gradient_multi_target(p.objective, T, zeros.p, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
+                                                 p.scale_pos_weight, objective_param(p), gh.p, nullptr, nullptr,
+                                                 b->ctx->num_sms, s));
+  else
+    LAUNCH_CHECK(b2_launch_gradient(p.objective, 1, zeros.p, m->label.p, m->n_weight ? m->weight.p : nullptr, n, p.scale_pos_weight,
+                                    objective_param(p), gh.p, nullptr, nullptr, b->ctx->num_sms, s));
   b->d_absmax.ensure(2); b->d_qexp.ensure(2);
-  CUDA_CHECK(cudaMemsetAsync(b->d_absmax.p, 0, 2 * sizeof(uint32_t), s));
-  LAUNCH_CHECK(b2_launch_absmax(gh.p, n, b->d_absmax.p, b->ctx->num_sms, s));
-  allreduce(b->comm, b->d_absmax.p, 2, kNcclUint32, kNcclMax, s);
-  LAUNCH_CHECK(b2_launch_quant_exponent(b->d_absmax.p, b->d_qexp.p, s));
-  CUDA_CHECK(cudaMemsetAsync(sums.p, 0, 4 * sizeof(long long), s));
-  LAUNCH_CHECK(b2_launch_sum_fixed(gh.p, n, b->d_qexp.p, 40, sums.p, b->ctx->num_sms, s));
-  allreduce(b->comm, sums.p, 4, kNcclInt64, kNcclSum, s);   // [g, h][hi, lo] limbs (common.cuh): exact over all ranks
-  long long h_s[4]; int32_t h_e[2];
-  CUDA_CHECK(cudaMemcpyAsync(h_s, sums.p, sizeof(h_s), cudaMemcpyDeviceToHost, s));
-  CUDA_CHECK(cudaMemcpyAsync(h_e, b->d_qexp.p, sizeof(h_e), cudaMemcpyDeviceToHost, s));
-  CUDA_CHECK(cudaStreamSynchronize(s));
   auto limbs_to_double = [](long long hi, long long lo) {   // b2_limbs_to_double on the host: one rounding
     hi += lo >> B2_LIMB_SHIFT; lo &= (1ll << B2_LIMB_SHIFT) - 1;
     return (double)hi * (double)(1ll << B2_LIMB_SHIFT) + (double)lo;
   };
-  const double G = limbs_to_double(h_s[0], h_s[1]) / ldexp(1.0, 40 - h_e[0]);
-  const double H = limbs_to_double(h_s[2], h_s[3]) / ldexp(1.0, 40 - h_e[1]);
-  const float stump = H <= 1e-6 ? 0.0f : (float)(-G / H);
+  float stump = 0.0f;
+  for (int k = 0; k < T; ++k) {
+    const float2* ghk = gh.p + (size_t)k * n;
+    CUDA_CHECK(cudaMemsetAsync(b->d_absmax.p, 0, 2 * sizeof(uint32_t), s));
+    LAUNCH_CHECK(b2_launch_absmax(ghk, n, b->d_absmax.p, b->ctx->num_sms, s));
+    allreduce(b->comm, b->d_absmax.p, 2, kNcclUint32, kNcclMax, s);
+    LAUNCH_CHECK(b2_launch_quant_exponent(b->d_absmax.p, b->d_qexp.p, s));
+    CUDA_CHECK(cudaMemsetAsync(sums.p, 0, 4 * sizeof(long long), s));
+    LAUNCH_CHECK(b2_launch_sum_fixed(ghk, n, b->d_qexp.p, 40, sums.p, b->ctx->num_sms, s));
+    allreduce(b->comm, sums.p, 4, kNcclInt64, kNcclSum, s);   // [g, h][hi, lo] limbs (common.cuh): exact over all ranks
+    long long h_s[4]; int32_t h_e[2];
+    CUDA_CHECK(cudaMemcpyAsync(h_s, sums.p, sizeof(h_s), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaMemcpyAsync(h_e, b->d_qexp.p, sizeof(h_e), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    const double G = limbs_to_double(h_s[0], h_s[1]) / ldexp(1.0, 40 - h_e[0]);
+    const double H = limbs_to_double(h_s[2], h_s[3]) / ldexp(1.0, 40 - h_e[1]);
+    const float stump_k = H <= 1e-6 ? 0.0f : (float)(-G / H);
+    stump = k == 0 ? stump_k / (float)T : stump + stump_k / (float)T;
+  }
   if (obj_sigmoid(p.objective) || obj_log_link(p.objective)) {
     // margin -> output space with the engine's own sigmoid / exp (same IEEE sequence as the kernels): evaluated on the device
     DevBuf<float> one; one.ensure(1);
@@ -2152,7 +2208,7 @@ void check_rank_labels(Booster* b) {
   if (!m->has_qgroups())
     fail("%s needs query groups on the train matrix: pass qid (or group) to the DMatrix", b->p.objective_name.c_str());
   if (b->labels_checked) return;
-  if (m->n_label != m->n) fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)m->n);
+  check_train_labels(b);
   const bool map = b->p.objective == kObjRankMap;
   DevBuf<uint32_t> bad; bad.ensure(3);
   CUDA_CHECK(cudaMemsetAsync(bad.p, 0, 3 * sizeof(uint32_t), s));
@@ -2215,10 +2271,10 @@ void check_labels(Booster* b) {
   if (o == kObjAft) { check_bounds(b); return; }
   if (obj_rank(o)) { check_rank_labels(b); return; }
   if (o == kObjSquaredError || o == kObjLogistic || o == kObjPseudoHuber || b->labels_checked) return;
-  if (m->n_label != m->n) fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)m->n);
+  check_train_labels(b);
   DevBuf<uint32_t> bad; bad.ensure(1);
   CUDA_CHECK(cudaMemsetAsync(bad.p, 0, sizeof(uint32_t), s));
-  LAUNCH_CHECK(b2_launch_label_check(o, b->p.num_class, m->label.p, m->n, bad.p, b->ctx->num_sms, s));
+  LAUNCH_CHECK(b2_launch_label_check(o, b->p.num_class, m->label.p, m->n * b->p.num_target, bad.p, b->ctx->num_sms, s));
   allreduce(b->comm, bad.p, 1, kNcclUint32, kNcclMax, s);
   uint32_t h = 0;
   CUDA_CHECK(cudaMemcpyAsync(&h, bad.p, sizeof(h), cudaMemcpyDeviceToHost, s));
@@ -2440,8 +2496,7 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
     CUDA_CHECK(cudaMemcpyAsync(b->d_custom_h.p, custom_h, len * sizeof(float), cudaMemcpyHostToDevice, s));
     LAUNCH_CHECK(b2_launch_pack_custom(b->d_custom_g.p, b->d_custom_h.p, K, n, b->gh.p, b->ctx->num_sms, s));
   } else {
-    if (b->p.objective != kObjAft && m->n_label != n)
-      fail("train matrix has %lld labels for %lld rows", (long long)m->n_label, (long long)n);
+    if (b->p.objective != kObjAft) check_train_labels(b);
     // the |g|,|h| maxima of every class tree come out of the same pass unless rows are dropped afterwards (subsample)
     b->absmax_fused = b->p.subsample >= 1.0f && K <= b2_gradient_fused_max_classes();
     if (b->absmax_fused) CUDA_CHECK(cudaMemsetAsync(b->d_absmax.p, 0, 2 * (size_t)K * sizeof(uint32_t), s));
@@ -2460,7 +2515,12 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
       ensure_quantile_buffers(b, 1 << b->p.max_depth);
       LAUNCH_CHECK(b2_launch_gradient_quantile(K, b->d_alpha.p, gm, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
                                                b->gh.p, b->absmax_fused ? b->d_absmax.p : nullptr, b->ctx->num_sms, s));
-    } else
+    } else if (b->p.num_target > 1)
+      LAUNCH_CHECK(b2_launch_gradient_multi_target(b->p.objective, K, gm, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
+                                                   b->p.scale_pos_weight, objective_param(b->p), b->gh.p,
+                                                   b->absmax_fused ? b->d_absmax.p : nullptr,
+                                                   check_finite ? b->d_grad_err.p : nullptr, b->ctx->num_sms, s));
+    else
       LAUNCH_CHECK(b2_launch_gradient(b->p.objective, K, gm, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
                                       b->p.scale_pos_weight, objective_param(b->p), b->gh.p,
                                       b->absmax_fused ? b->d_absmax.p : nullptr, check_finite ? b->d_grad_err.p : nullptr,
@@ -2857,12 +2917,16 @@ int B2_MatrixSetFloatInfo(B2Handle mh, const char* field, const float* values, i
   CUDA_CHECK(cudaSetDevice(m->ctx->device));
   std::string f(field ? field : "");
   DevBuf<float>* dst = nullptr; int64_t* cnt = nullptr;
-  if (f == "label") { dst = &m->label; cnt = &m->n_label; m->rank_version++; if (len != m->n) fail("label length %lld != rows %lld", (long long)len, (long long)m->n); }
+  if (f == "label") {
+    dst = &m->label; cnt = &m->n_label; m->rank_version++; m->n_targets = 1;
+    if (len != m->n) fail("label length %lld != rows %lld", (long long)len, (long long)m->n);
+  }
   else if (f == "weight") { dst = &m->weight; cnt = &m->n_weight; if (len != m->n && len != 0) fail("weight length %lld != rows %lld", (long long)len, (long long)m->n); }
   else if (f == "label_lower_bound" || f == "label_upper_bound") {
     const bool lo = f == "label_lower_bound";
     dst = lo ? &m->lower : &m->upper; cnt = lo ? &m->n_lower : &m->n_upper;
     if (len != m->n && len != 0) fail("%s length %lld != rows %lld", f.c_str(), (long long)len, (long long)m->n);
+    if (len != 0 && m->n_targets > 1) fail("%s: the matrix has a label of %d columns (survival bounds need one)", f.c_str(), m->n_targets);
   }
   else if (f == "base_margin") { dst = &m->base_margin; cnt = &m->n_base_margin; m->margin_version++; if (len != 0 && (m->n == 0 || len % m->n != 0)) fail("base_margin length %lld is not a multiple of rows %lld", (long long)len, (long long)m->n); }
   else if (f == "feature_weights") {
@@ -2886,11 +2950,31 @@ int B2_MatrixSetFloatInfo(B2Handle mh, const char* field, const float* values, i
   *cnt = len;
   API_END
 }
+int B2_MatrixSetLabel(B2Handle mh, const float* values, int64_t rows, int32_t n_targets) {
+  API_BEGIN
+  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
+  CUDA_CHECK(cudaSetDevice(m->ctx->device));
+  if (rows != m->n) fail("label has %lld rows, the matrix %lld", (long long)rows, (long long)m->n);
+  if (n_targets < 1 || n_targets > kMaxTargets) fail("label columns must be in [1, %d], got %d", kMaxTargets, n_targets);
+  if (n_targets > 1 && m->has_qgroups())
+    fail("a label of %d columns on a matrix with query groups (qid) is not supported", n_targets);
+  if (n_targets > 1 && (m->n_lower > 0 || m->n_upper > 0))
+    fail("a label of %d columns on a matrix with label_lower_bound / label_upper_bound is not supported", n_targets);
+  const int64_t len = rows * n_targets;
+  m->label.ensure((size_t)std::max<int64_t>(len, 1));
+  if (len > 0) CUDA_CHECK(cudaMemcpyAsync(m->label.p, values, len * sizeof(float), cudaMemcpyHostToDevice, m->ctx->stream));
+  CUDA_CHECK(cudaStreamSynchronize(m->ctx->stream));
+  m->n_label = len; m->n_targets = n_targets;
+  m->rank_version++;
+  API_END
+}
 int B2_MatrixSetGroups(B2Handle mh, const int32_t* group_sizes, int64_t n_groups) {
   API_BEGIN
   Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
   CUDA_CHECK(cudaSetDevice(m->ctx->device));
   if (n_groups < 0) fail("query groups: negative group count %lld", (long long)n_groups);
+  if (n_groups > 0 && m->n_targets > 1)
+    fail("query groups (qid) on a matrix with a label of %d columns are not supported", m->n_targets);
   std::vector<int64_t> ptr((size_t)n_groups + 1, 0);
   int64_t mx = 0;
   for (int64_t g = 0; g < n_groups; ++g) {
@@ -3026,6 +3110,10 @@ int B2_BoosterCreate(const char* params, B2Handle trainh, B2Handle commh, B2Hand
   try {
     parse_params(params, &b->p, nullptr);
     if (m) {
+      // the train matrix's label fixes the targets; a loaded model (num_target) must have as many
+      if (b->p.num_target_set && b->p.num_target != m->n_targets)
+        fail("the model has %d targets, the train matrix's label has %d columns", b->p.num_target, m->n_targets);
+      set_targets(&b->p, m->n_targets);
       b->ctx = m->ctx; b->n_features = m->F; CUDA_CHECK(cudaSetDevice(m->ctx->device));
       if (!b->p.interaction_sets.empty()) {   // sets_of[f] bit k: feature f is in set k
         const int W = (int)((b->p.interaction_sets.size() + 63) / 64);
@@ -3118,13 +3206,19 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
   // one-vs-rest only
   if (auc_metric && m->has_qgroups())
     fail("metric '%s' on a matrix with query groups (per-group ranking AUC) is not supported; use ndcg or map", metric);
+  if (auc_metric && b->p.num_target > 1)
+    fail("metric '%s' is not supported for a multi-target model (%d targets); use rmse, mae, logloss or error", metric,
+         b->p.num_target);
   if (auc_metric && b->p.num_class > 1 && b->p.objective != kObjSoftprob)
     fail("metric '%s' needs one output per row or a multi:softprob / multi:softmax model; objective '%s' has %d outputs",
          metric, b->p.objective_name.c_str(), b->p.num_class);
   if (aft_metric && b->p.objective != kObjAft)
     fail("metric '%s' does not fit objective '%s'", metric, b->p.objective_name.c_str());
   if (aft_metric && !m->has_bounds()) fail("metric '%s' needs label_lower_bound and label_upper_bound on the evaluation matrix", metric);
-  if (!aft_metric && m->n_label != m->n) fail("evaluation matrix has no labels");
+  if (!aft_metric && m->n_label > 0 && m->n_targets != b->p.num_target)
+    fail("metric '%s': the evaluation matrix's label has %d columns, the model has %d targets", metric, m->n_targets,
+         b->p.num_target);
+  if (!aft_metric && !m->has_labels(b->p.num_target)) fail("evaluation matrix has no labels");
   float* margin = eval_margin(b, m);
   if (auc_metric) {
     // ROC / PR AUC on the transformed prediction (auc_kernel.cu; DESIGN.md §2 item 17): per class a worker's triple
@@ -3191,8 +3285,16 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
     *out = h[1] > 0 ? h[0] / h[1] : 0.0;
     return 0;
   }
-  LAUNCH_CHECK(b2_launch_metric(b->p.objective, mid, b->p.num_class, mparam, margin, m->label.p, m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p,
-                                b->ctx->num_sms, s));
+  if (b->p.num_target > 1) {
+    // elementwise over the n x T outputs, each with its row's weight (xgboost's EvalEWiseBase)
+    if (!(mid <= 2 || mid == 5 || (mid >= 7 && mid <= 9)))
+      fail("metric '%s' is not supported for a multi-target model (supported: rmse, rmsle, mae, mape, mphe, logloss, error)",
+           metric);
+    LAUNCH_CHECK(b2_launch_metric_multi_target(b->p.objective, mid, b->p.num_target, mparam, margin, m->label.p,
+                                               m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p, b->ctx->num_sms, s));
+  } else
+    LAUNCH_CHECK(b2_launch_metric(b->p.objective, mid, b->p.num_class, mparam, margin, m->label.p, m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p,
+                                  b->ctx->num_sms, s));
   // (sum, wsum, rows with a label outside [0, num_class)): the count travels with the sums, so every rank fails together
   allreduce(b->comm, b->d_metric.p, 3, kNcclFloat64, kNcclSum, s);
   double h[3];
@@ -3361,6 +3463,11 @@ int B2_BoosterGetBaseScore(B2Handle bh, float* out, int32_t* is_final) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
   *out = b->p.base_score; *is_final = b->p.base_score_set ? 1 : 0;
+  API_END
+}
+int B2_BoosterNumTargets(B2Handle bh, int32_t* out) {
+  API_BEGIN
+  *out = from_handle<Booster>(bh, kBooster, "booster")->p.num_target;
   API_END
 }
 int B2_BoosterNumTrees(B2Handle bh, int32_t* out) {

@@ -158,6 +158,29 @@ __device__ __forceinline__ float2 scalar_grad(float p, float y, float a) {
 // the same pass (the fixed-point scale of each class tree needs it; a separate pass re-read 8 bytes per row).
 constexpr int kFusedMaxK = 16;   // classes whose running maxima fit in registers; more classes use absmax_kernel
 
+// (g, h) of one element of reg:squarederror (kObjective 0) or binary:logistic and its variants (1), weight w applied
+// (scale_pos_weight on positive labels, RegLossObj)
+template <int kObjective>
+__device__ __forceinline__ float2 reg_loss_grad(float m, float y, float w, float scale_pos_weight) {
+  if (kObjective == 0) return make_float2(__fmul_rn(__fadd_rn(m, -y), w), w);
+  if (y == 1.0f) w = __fmul_rn(w, scale_pos_weight);   // RegLossObj: positive rows
+  const float p = b2_sigmoid(m);
+  float hh = __fmul_rn(p, __fadd_rn(1.0f, -p));
+  if (hh < 1e-16f) hh = 1e-16f;
+  return make_float2(__fmul_rn(__fadd_rn(p, -y), w), __fmul_rn(hh, w));
+}
+
+// (g, h) of one element of an objective with a parameter, weight applied; a pair that is not finite is returned as
+// (0, 0) with *bad set
+template <int kObjective>
+__device__ __forceinline__ float2 param_grad(float m, float y, float w, float scale_pos_weight, float a, bool* bad) {
+  if (kObjective == kObjSquaredLog && y == 1.0f) w = __fmul_rn(w, scale_pos_weight);   // RegLossObj: positive rows
+  const float2 r = scalar_grad<kObjective>(m, y, a);
+  float2 v = make_float2(__fmul_rn(r.x, w), __fmul_rn(r.y, w));
+  if (!(fabsf(v.x) <= FLT_MAX && fabsf(v.y) <= FLT_MAX)) { *bad = true; v = make_float2(0.0f, 0.0f); }
+  return v;
+}
+
 // scalar objectives (reg:squarederror, binary:logistic and its variants): their own kernel so that the register budget
 // of the softprob path (2 x 16 running maxima) does not cut the occupancy of this streaming loop (72 registers -> 3 blocks
 // per SM made the 10M-row launch take 63 us instead of ~25)
@@ -167,18 +190,9 @@ gradient_scalar_kernel(const float* __restrict__ margin, const float* __restrict
                        int64_t n, float scale_pos_weight, float2* __restrict__ gh, uint32_t* __restrict__ absmax) {
   float mg = 0.0f, mh = 0.0f;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    float w = weight ? weight[i] : 1.0f;
+    const float w = weight ? weight[i] : 1.0f;
     const float y = label[i], m = margin[i];
-    float2 v;
-    if (kObjective == 0) {
-      v = make_float2(__fmul_rn(__fadd_rn(m, -y), w), w);
-    } else {
-      if (y == 1.0f) w = __fmul_rn(w, scale_pos_weight);   // RegLossObj: positive rows
-      const float p = b2_sigmoid(m);
-      float hh = __fmul_rn(p, __fadd_rn(1.0f, -p));
-      if (hh < 1e-16f) hh = 1e-16f;
-      v = make_float2(__fmul_rn(__fadd_rn(p, -y), w), __fmul_rn(hh, w));
-    }
+    const float2 v = reg_loss_grad<kObjective>(m, y, w, scale_pos_weight);
     gh[i] = v;
     mg = fmaxf(mg, fabsf(v.x)); mh = fmaxf(mh, fabsf(v.y));
   }
@@ -196,17 +210,57 @@ gradient_param_kernel(const float* __restrict__ margin, const float* __restrict_
   float mg = 0.0f, mh = 0.0f;
   bool bad = false;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    float w = weight ? weight[i] : 1.0f;
+    const float w = weight ? weight[i] : 1.0f;
     const float y = label[i], m = margin[i];
-    if (kObjective == kObjSquaredLog && y == 1.0f) w = __fmul_rn(w, scale_pos_weight);   // RegLossObj: positive rows
-    const float2 r = scalar_grad<kObjective>(m, y, op.a);
-    float2 v = make_float2(__fmul_rn(r.x, w), __fmul_rn(r.y, w));
-    if (!(fabsf(v.x) <= FLT_MAX && fabsf(v.y) <= FLT_MAX)) { bad = true; v = make_float2(0.0f, 0.0f); }
+    const float2 v = param_grad<kObjective>(m, y, w, scale_pos_weight, op.a, &bad);
     gh[i] = v;
     mg = fmaxf(mg, fabsf(v.x)); mh = fmaxf(mh, fabsf(v.y));
   }
   if (bad && err) atomicOr(err, 1u);
   if (absmax) absmax_publish(mg, mh, absmax);
+}
+
+// multi-target regression / multi-label classification: margin and label [n][T] row-major, one weight per row, gh
+// class-major [T][n] (target k's tree reads a contiguous slice).  Element (i, k) is the scalar kernels' sequence.  kFused
+// (T <= kFusedMaxK): the |g|, |h| maxima of every target come out of the same pass, as in gradient_softprob_kernel.
+// Kept apart from the scalar kernels so that their streaming loop keeps its register budget.
+template <int kObjective, bool kFused>
+__global__ void __launch_bounds__(256)
+gradient_multi_target_kernel(int T, const float* __restrict__ margin, const float* __restrict__ label,
+                             const float* __restrict__ weight, int64_t n, float scale_pos_weight, ObjParam op,
+                             float2* __restrict__ gh, uint32_t* __restrict__ absmax, uint32_t* __restrict__ err) {
+  constexpr int kMax = kFused ? kFusedMaxK : 1;
+  float mg[kMax], mh[kMax];
+#pragma unroll
+  for (int k = 0; k < kMax; ++k) { mg[k] = 0.0f; mh[k] = 0.0f; }
+  bool bad = false;
+  auto elem = [&](int64_t i, int k, float w) {
+    const float y = label[i * T + k], m = margin[i * T + k];
+    float2 v;
+    if constexpr (kObjective <= 1) v = reg_loss_grad<kObjective>(m, y, w, scale_pos_weight);
+    else v = param_grad<kObjective>(m, y, w, scale_pos_weight, op.a, &bad);
+    gh[(int64_t)k * n + i] = v;
+    return v;
+  };
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float w = weight ? weight[i] : 1.0f;
+    if (kFused) {
+#pragma unroll
+      for (int k = 0; k < kMax; ++k)
+        if (k < T) {
+          const float2 v = elem(i, k, w);
+          mg[k] = fmaxf(mg[k], fabsf(v.x)); mh[k] = fmaxf(mh[k], fabsf(v.y));
+        }
+    } else {
+      for (int k = 0; k < T; ++k) elem(i, k, w);
+    }
+  }
+  if (kObjective > 1 && bad && err) atomicOr(err, 1u);
+  if (kFused && absmax) {
+#pragma unroll
+    for (int k = 0; k < kMax; ++k)
+      if (k < T) absmax_publish(mg[k], mh[k], absmax + 2 * k);
+  }
 }
 
 // ---- survival:aft (accelerated failure time).  log y = margin + sigma Z with Z standard normal, logistic or extreme
@@ -514,6 +568,36 @@ __device__ __forceinline__ double scalar_metric(int metric, float a, double q, d
   return -y * pow(q, 1.0 - r) / (1.0 - r) + pow(q, 2.0 - r) / (2.0 - r);
 }
 
+// one element's loss for the elementwise metrics (0-2, 5, 7-13) on the transformed prediction
+__device__ __forceinline__ double elementwise_metric(int objective, int metric, float a, float margin, float y) {
+  const float p = b2_pred_transform(objective, margin);
+  if (metric == 0) { const double d = (double)p - (double)y; return d * d; }
+  if (metric == 5) return fabs((double)p - (double)y);
+  if (metric == 1) {
+    const float eps = 1e-16f;
+    const float pn = 1.0f - p; const float pa = p < eps ? eps : p, pb = pn < eps ? eps : pn;
+    return -((double)y * log((double)pa) + (1.0 - (double)y) * log((double)pb));
+  }
+  if (metric == 2) return ((p > 0.5f) != (y > 0.5f)) ? 1.0 : 0.0;
+  return scalar_metric(metric, a, (double)p, (double)y);
+}
+
+// elementwise metrics of a multi-target model over the n*T elements of margin and label [n][T]: element (i, k) counts
+// with row i's weight, so out = (sum w_i v_ik, T * sum w_i)
+__global__ void metric_multi_target_kernel(int objective, int metric, int T, float a, const float* __restrict__ margin,
+                                           const float* __restrict__ label, const float* __restrict__ weight, int64_t n,
+                                           double* __restrict__ out) {
+  double s = 0.0, ws = 0.0;
+  const int64_t nt = n * T;
+  for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < nt; j += (int64_t)gridDim.x * blockDim.x) {
+    const double w = weight ? (double)weight[j / T] : 1.0;
+    s += elementwise_metric(objective, metric, a, margin[j], label[j]) * w; ws += w;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ws += __shfl_xor_sync(0xffffffffu, ws, o); }
+  if ((threadIdx.x & 31) == 0) { atomicAdd(&out[0], s); atomicAdd(&out[1], ws); }
+}
+
 // a multi-class label is a class index in [0, K): non-integer labels truncate (2.7 -> class 2); NaN is outside
 __device__ __forceinline__ bool b2_class_label_ok(float y, int K) { return y >= 0.0f && y < (float)K; }
 
@@ -527,17 +611,7 @@ __global__ void metric_kernel(int objective, int metric, int K, float a, const f
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const double w = weight ? (double)weight[i] : 1.0;
     double v = 0.0;
-    if (metric <= 2 || metric == 5) {
-      const float p = b2_pred_transform(objective, margin[i]);
-      if (metric == 0) { const double d = (double)p - (double)label[i]; v = d * d; }
-      else if (metric == 5) v = fabs((double)p - (double)label[i]);
-      else if (metric == 1) {
-        const float eps = 1e-16f; const float y = label[i];
-        const float pn = 1.0f - p; const float a = p < eps ? eps : p, b = pn < eps ? eps : pn;
-        v = -((double)y * log((double)a) + (1.0 - (double)y) * log((double)b));
-      } else v = ((p > 0.5f) != (label[i] > 0.5f)) ? 1.0 : 0.0;
-    }
-    else if (metric >= 7) v = scalar_metric(metric, a, (double)b2_pred_transform(objective, margin[i]), (double)label[i]);
+    if (metric <= 2 || metric == 5 || metric >= 7) v = elementwise_metric(objective, metric, a, margin[i], label[i]);
     else {
       const float yf = label[i];
       if (!b2_class_label_ok(yf, K)) { ++bad; continue; }
@@ -651,6 +725,35 @@ int b2_launch_gradient(int objective, int K, const float* margin, const float* l
   }
   return (int)cudaGetLastError();
 }
+// multi-target gradients (T >= 1 label columns): absmax [T][2] (nullable) is filled only when T <= kFusedMaxK
+int b2_launch_gradient_multi_target(int objective, int T, const float* margin, const float* label, const float* weight,
+                                    int64_t n, float scale_pos_weight, float obj_param, float2* gh, uint32_t* absmax,
+                                    uint32_t* err, int num_sms, cudaStream_t s) {
+  if (n <= 0) return 0;
+  const int g = grid_for(n, num_sms);
+  const b2::ObjParam op{obj_param};
+  const bool fused = T <= b2::kFusedMaxK;
+  switch (objective) {
+#define B2_MT(kern_id, id) \
+    case id: \
+      if (fused) b2::gradient_multi_target_kernel<kern_id, true><<<g, 256, 0, s>>>(T, margin, label, weight, n, scale_pos_weight, op, gh, absmax, err); \
+      else b2::gradient_multi_target_kernel<kern_id, false><<<g, 256, 0, s>>>(T, margin, label, weight, n, scale_pos_weight, op, gh, nullptr, err); \
+      break;
+    B2_MT(0, 0) B2_MT(1, 1) B2_MT(1, b2::kObjRegLogistic) B2_MT(1, b2::kObjLogitRaw)
+    B2_MT(b2::kObjSquaredLog, b2::kObjSquaredLog) B2_MT(b2::kObjPseudoHuber, b2::kObjPseudoHuber)
+#undef B2_MT
+    default: return (int)cudaErrorInvalidValue;
+  }
+  return (int)cudaGetLastError();
+}
+int b2_launch_metric_multi_target(int objective, int metric, int T, float metric_param, const float* margin,
+                                  const float* label, const float* weight, int64_t n, double* out, int num_sms,
+                                  cudaStream_t s) {
+  if (n <= 0) return 0;
+  b2::metric_multi_target_kernel<<<grid_for(n * T, num_sms), 256, 0, s>>>(objective, metric, T, metric_param, margin, label,
+                                                                          weight, n, out);
+  return (int)cudaGetLastError();
+}
 int b2_launch_gradient_aft(int dist, double sigma, const float* margin, const float* lower, const float* upper,
                            const float* weight, int64_t n, float2* gh, uint32_t* absmax, uint32_t* err, int num_sms,
                            cudaStream_t s) {
@@ -730,8 +833,10 @@ int b2_launch_fill(float* out, int64_t n, float v, int num_sms, cudaStream_t s) 
   b2::fill_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(out, n, v);
   return (int)cudaGetLastError();
 }
+// m holds n rows of K outputs: softmax runs per row, every other transform over all n * K elements
 int b2_launch_transform(int objective, int K, float* m, int64_t n, int num_sms, cudaStream_t s) {
   if (n <= 0) return 0;
+  if (objective != 2) n *= K;
   b2::transform_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(objective, K, m, n);
   return (int)cudaGetLastError();
 }

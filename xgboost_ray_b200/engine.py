@@ -56,6 +56,7 @@ ABI = {
                                              C.POINTER(_H)]),
     "B2_MatrixSetRows": (C.c_int, [_H, C.c_int64, _FP, C.c_int64]),
     "B2_MatrixSetFloatInfo": (C.c_int, [_H, C.c_char_p, _FP, C.c_int64]),
+    "B2_MatrixSetLabel": (C.c_int, [_H, _FP, C.c_int64, C.c_int32]),
     "B2_MatrixSetGroups": (C.c_int, [_H, _IP, C.c_int64]),
     "B2_MatrixSetFeatureTypes": (C.c_int, [_H, _BP, C.c_int32]),
     "B2_MatrixGetFeatureTypes": (C.c_int, [_H, _BP]),
@@ -79,6 +80,7 @@ ABI = {
     "B2_BoosterGetTrainMargin": (C.c_int, [_H, C.c_int32, _FP, C.c_int64]),
     "B2_BoosterResetTrainMargin": (C.c_int, [_H]),
     "B2_BoosterGetBaseScore": (C.c_int, [_H, _FP, _IP]),
+    "B2_BoosterNumTargets": (C.c_int, [_H, _IP]),
     "B2_BoosterNumTrees": (C.c_int, [_H, _IP]),
     "B2_BoosterTreeNumNodes": (C.c_int, [_H, C.c_int32, _IP]),
     "B2_BoosterGetTree": (C.c_int, [_H, C.c_int32, _IP, _IP, _IP, _IP, _IP, _FP, _BP, _FP, _FP, _FP, _DP]),
@@ -226,11 +228,17 @@ class collective:  # namespace shim: xgb.collective.get_rank() (session.py:73)
 # ----------------------------------------------------------------------------- DMatrix
 class DMatrix:
     """Device matrix.  Float data is uploaded at construction; quantisation (GPU sketch + binning)
-    happens when a Booster first trains on it, because cuts are global over the communicator."""
+    happens when a Booster first trains on it, because cuts are global over the communicator.
+
+    multi_target=True accepts a label of shape (n, T), T > 1: multi-target regression or multi-label classification,
+    one tree per column and round.  Without it a label of several columns is refused, so that a label of the wrong
+    shape (one-hot classes, a target passed twice) is not trained as T independent outputs.  RayDMatrix and the sklearn
+    estimators, whose users ask for several label columns explicitly, set it for them."""
 
     def __init__(self, data, label=None, weight=None, base_margin=None, missing=None, feature_names=None,
                  feature_types=None, nthread=None, enable_categorical=False, max_bin=None, ref=None,
-                 device=None, label_lower_bound=None, label_upper_bound=None, qid=None, group=None, **kwargs):
+                 device=None, label_lower_bound=None, label_upper_bound=None, qid=None, group=None, multi_target=False,
+                 **kwargs):
         if hasattr(data, "values") and not isinstance(data, np.ndarray):  # pandas
             if feature_names is None and hasattr(data, "columns"):
                 feature_names = [str(c) for c in data.columns]
@@ -284,6 +292,7 @@ class DMatrix:
         self.ref = ref
         self._quantized = False
         self._has_raw = True
+        self.multi_target = bool(multi_target)
         self._label = None
         self._weight = None
         self._base_margin = None
@@ -342,7 +351,19 @@ class DMatrix:
                 continue
             if hasattr(v, "values") and not isinstance(v, np.ndarray):
                 v = v.values
-            a = _f32c(np.asarray(v).reshape(-1))
+            a = np.asarray(v)
+            if field == "label" and a.ndim == 2 and a.shape[1] > 1:
+                # T label columns: multi-target regression / multi-label classification, one tree per column and round
+                if not self.multi_target:
+                    raise XGBoostError("label has shape %s: a label of several columns (multi-target regression, "
+                                       "multi-label classification) needs DMatrix(..., multi_target=True)" % (a.shape,))
+                a = _f32c(a)
+                _check(lib().B2_MatrixSetLabel(self.handle, _fp(a), a.shape[0], a.shape[1]))
+                self._label = a
+                continue
+            if field == "label" and a.ndim > 2:
+                raise XGBoostError("label must be 1- or 2-dimensional, got shape %s" % (a.shape,))
+            a = _f32c(a.reshape(-1))
             _check(lib().B2_MatrixSetFloatInfo(self.handle, field.encode(), _fp(a), a.size))
             setattr(self, "_" + field, a)
 
@@ -388,6 +409,7 @@ class DMatrix:
         self.set_info(base_margin=margin)
 
     def get_label(self):
+        """(n,) labels, or (n, T) for a label of T > 1 columns."""
         return self._label if self._label is not None else np.zeros(0, np.float32)
 
     def get_weight(self):
@@ -482,7 +504,8 @@ def _drain_data_iter(it, label, weight, base_margin):
         got["data"].append(np.asarray(data.values if hasattr(data, "values") and not isinstance(data, np.ndarray) else data))
         for k, v in (("label", label), ("weight", weight), ("base_margin", base_margin)):
             if v is not None:
-                got[k].append(np.asarray(v.values if hasattr(v, "values") and not isinstance(v, np.ndarray) else v).reshape(-1))
+                a = np.asarray(v.values if hasattr(v, "values") and not isinstance(v, np.ndarray) else v)
+                got[k].append(a if k == "label" and a.ndim == 2 else a.reshape(-1))   # a 2-D label keeps its columns
 
     it.reset()
     while it.next(input_data):
@@ -620,7 +643,7 @@ _ENGINE_KEYS = ("objective", "num_class", "max_depth", "eta", "learning_rate", "
                 "random_state", "num_parallel_tree", "huber_slope", "tweedie_variance_power", "aft_loss_distribution",
                 "aft_loss_distribution_scale", "lambdarank_pair_method", "lambdarank_num_pair_per_sample",
                 "lambdarank_unbiased", "ndcg_exp_gain", "booster", "rate_drop", "skip_drop", "sample_type",
-                "normalize_type", "one_drop", "quantile_alpha")
+                "normalize_type", "one_drop", "quantile_alpha", "num_target")
 # booster=dart's parameters with xgboost's defaults (save_config's dart_train_param)
 _DART_DEFAULTS = {"rate_drop": 0.0, "skip_drop": 0.0, "sample_type": "uniform", "normalize_type": "tree", "one_drop": 0}
 
@@ -766,9 +789,18 @@ class Booster:
                                       self.feature_names if self.feature_names is not None else dtrain.feature_names)
         # one param line: sets separated by ';', features by ','
         extra = {"interaction_constraints": ";".join(",".join(map(str, s)) for s in sets)} if sets else None
+        if old_trees:   # the trees were grown for the model's targets: the engine checks the matrix's label against them
+            extra = dict(extra or {}, num_target=self._num_target())
         h = _H(0)
         _check(lib().B2_BoosterCreate(self._param_text(extra), dtrain.handle, _coll.handle, C.byref(h)))
         self.handle = h.value
+        # the engine takes the targets from the train matrix's label; the model keeps them for its file and predictions
+        nt = C.c_int32(1)
+        _check(lib().B2_BoosterNumTargets(self.handle, C.byref(nt)))
+        if nt.value > 1:
+            self.params["num_target"] = nt.value
+        else:
+            self.params.pop("num_target", None)
         self._train = dtrain
         self.n_features = dtrain.num_col()
         if self.feature_names is None:
@@ -835,12 +867,19 @@ class Booster:
             return n.value
         return len(self._trees)
 
+    def _num_target(self):
+        """Label columns of the model: T > 1 for multi-target regression / multi-label classification, else 1."""
+        return int(self.params.get("num_target", 1) or 1)
+
     @property
     def num_class(self):
-        """Outputs per row: the classes of multi:*, the alphas of reg:quantileerror, else 1."""
+        """Outputs per row: the classes of multi:*, the alphas of reg:quantileerror, the label columns of a multi-target
+        model, else 1."""
         obj = self.params.get("objective", "reg:squarederror")
         if obj == "reg:quantileerror":
             return int(quantile_alphas(self.params.get("quantile_alpha")).size)
+        if self._num_target() > 1:
+            return self._num_target()
         return int(self.params.get("num_class", 1)) if obj.startswith("multi:") else 1
 
     @property
@@ -1100,7 +1139,7 @@ class Booster:
             cache.append((tj, [int(x) for x in src[i]["split_bin"]], exact))
         trees = [c[0] for c in cache]
         obj = self.params.get("objective", "reg:squarederror")
-        quantile = obj == "reg:quantileerror"   # xgboost counts the alphas as targets, not classes
+        quantile = obj == "reg:quantileerror" or self._num_target() > 1   # alphas and label columns are targets, not classes
         spec = _OBJECTIVES.get(obj, _OBJECTIVES["reg:squarederror"])
         obj_block = {"name": obj}
         if spec.block:
@@ -1110,7 +1149,7 @@ class Booster:
                                      for k, d in spec.block_params.items()}
         attrs = {k: str(v) for k, v in self._attrs.items() if not k.startswith("b2.")}
         b2p = {k: self.params[k] for k in self.params if _json_ok(self.params[k]) and
-               k not in ("objective", "num_class", "base_score", "scale_pos_weight", "num_parallel_tree")}   # those have their own fields
+               k not in ("objective", "num_class", "num_target", "base_score", "scale_pos_weight", "num_parallel_tree")}   # those have their own fields
         sets = self._interaction_sets() if self.n_features is not None else []
         if sets:   # in its resolved string form, which also keeps list / feature-name / numpy inputs
             b2p["interaction_constraints"] = str(sets)
@@ -1193,6 +1232,11 @@ class Booster:
         if npt > 1:
             params["num_parallel_tree"] = npt
         params.update({k: v for k, v in self.params.items() if k not in params})
+        nt = int(L["learner_model_param"].get("num_target", "1"))
+        if nt > 1 and params["objective"] != "reg:quantileerror":   # quantile's targets are its alphas
+            params["num_target"] = nt
+        else:
+            params.pop("num_target", None)
         self.params = params
         self.n_features = int(L["learner_model_param"]["num_feature"])
         self.feature_names = L.get("feature_names") or None
@@ -1468,6 +1512,8 @@ def train(params, dtrain, num_boost_round=10, evals=(), obj=None, feval=None, ma
             raise XGBoostError("cannot continue a DART model with booster=%r: its trees carry weights that a gbtree "
                                "model would drop (continue with booster='dart')" % (bst.params.get("booster"),))
         bst._weights = src.get_tree_weights() if bst.is_dart and src.is_dart else None
+        if src._num_target() > 1:   # the trees of output k were fitted to label column k
+            bst.params["num_target"] = src._num_target()
         if src.params.get("objective") == "reg:quantileerror" and bst.params.get("objective") == "reg:quantileerror":
             # the trees of output k were fitted to alpha_k: a continuation keeps the alphas
             old = quantile_alphas(src.params.get("quantile_alpha"))

@@ -254,12 +254,16 @@ class RemoteBlock:
 
 
 def _column_or_array(frame: LoadedFrame, spec, exclude: set):
-    """`spec` is None, a column name of the loaded frame, or an array-like of row values."""
+    """`spec` is None, a column name of the loaded frame, a list of column names (a label of several columns:
+    multi-target regression / multi-label classification, (n, T) in the given order), or an array-like of row values."""
     if spec is None:
         return None
     if isinstance(spec, str):
         exclude.add(spec)
         return np.ascontiguousarray(frame.column(spec), dtype=np.float32)
+    if isinstance(spec, (list, tuple)) and spec and all(isinstance(c, str) for c in spec):
+        exclude.update(spec)
+        return np.ascontiguousarray(np.stack([np.asarray(frame.column(c)) for c in spec], axis=1), dtype=np.float32)
     if hasattr(spec, "values") and not isinstance(spec, np.ndarray):
         spec = spec.values
     return np.ascontiguousarray(np.asarray(spec), dtype=np.float32)

@@ -189,11 +189,22 @@ class RayXGBClassifier(RayXGBMixin, ClassifierMixin):
                 raise ValueError("When X is a RayDMatrix, set `n_classes_` (or pass num_class=) before fit().")
             self.classes_ = np.arange(n_classes)
             yy = None
+        elif np.ndim(y) == 2 and np.shape(y)[1] > 1:
+            # multi-label classification (xgboost 2.x): a 0/1 label matrix, binary:logistic with one target per column
+            yy = np.asarray(y.values if hasattr(y, "values") and not isinstance(y, np.ndarray) else y, np.float32)
+            if not np.all((yy == 0) | (yy == 1)):
+                raise ValueError("a 2-D label is multi-label classification: every label must be 0 or 1")
+            self.classes_ = np.array([0, 1])
+            self.n_classes_ = 2
+            self._multi_label = True
+            params["objective"] = params["objective"] or "binary:logistic"
+            return self._fit(params, X, yy, sample_weight, base_margin, eval_set, ray_params, ray_dmatrix_params, **kw)
         else:
             self.classes_ = np.unique(np.asarray(y))
             lookup = {c: i for i, c in enumerate(self.classes_)}
             yy = np.asarray([lookup[v] for v in np.asarray(y)], np.float32)
         self.n_classes_ = len(self.classes_)
+        self._multi_label = False
         if self.n_classes_ > 2:
             params["objective"] = "multi:softprob"
             params["num_class"] = self.n_classes_
@@ -203,6 +214,8 @@ class RayXGBClassifier(RayXGBMixin, ClassifierMixin):
 
     def predict_proba(self, X, ray_params=None, ray_dmatrix_params=None, **kw):
         p = self._predict(X, ray_params, ray_dmatrix_params, **kw)
+        if getattr(self, "_multi_label", False):   # (n, T): the probability of label 1 in each column
+            return p
         if p.ndim == 1:
             return np.vstack((1.0 - p, p)).T
         return p
@@ -211,6 +224,8 @@ class RayXGBClassifier(RayXGBMixin, ClassifierMixin):
         if output_margin:
             return self._predict(X, ray_params, ray_dmatrix_params, output_margin=True, **kw)
         proba = self.predict_proba(X, ray_params, ray_dmatrix_params, **kw)
+        if getattr(self, "_multi_label", False):
+            return (proba > 0.5).astype(np.int64)
         return self.classes_[np.argmax(proba, axis=1)]
 
 
