@@ -171,6 +171,11 @@ int B2_BoosterAddTree(B2Handle b, int32_t n_nodes, const int32_t* left, const in
  * after B2_BoosterAddTree when a model with categorical splits is loaded. */
 int B2_BoosterGetTreeCategories(B2Handle b, int32_t tree, uint8_t* split_type /*[n]*/, uint32_t* cat_bits /*[n*8]*/);
 int B2_BoosterSetTreeCategories(B2Handle b, int32_t tree, const uint8_t* split_type, const uint32_t* cat_bits);
+/* vector-leaf tree (multi_strategy=multi_output_tree, T = num_target > 1): v[i*T + k] is node i's value of target k --
+ * a leaf's leaf value, an internal node's eta-scaled weight (model JSON base_weights).  Set is called after
+ * B2_BoosterAddTree on a booster created with multi_strategy=multi_output_tree; Get fails on a single-output tree. */
+int B2_BoosterGetTreeLeafVector(B2Handle b, int32_t tree, float* v /*[n*T]*/, int64_t len);
+int B2_BoosterSetTreeLeafVector(B2Handle b, int32_t tree, const float* v, int64_t len);
 /* booster=dart: the weight of every tree in model order (model JSON gradient_booster.weight_drop); tree t adds
  * fl(w[t] * leaf) to the margin.  Get on a gbtree booster returns 1 for every tree.  Set (after the trees were added
  * with B2_BoosterAddTree; a tree added to a dart booster starts at weight 1) needs finite weights >= 0 and one per

@@ -255,6 +255,9 @@ struct B2DecideArgs {
   B2Interaction ic;                // sets_of != nullptr: write the children's compat entries
   B2CtlParams p;
   int32_t cands_per_node, cand_ranks, cand_rank_stride, can_split, qbits;
+  // vector-leaf tree (eval_splits_vector_kernel): a candidate's left_g / left_h are 0/1 "the left / right child has a
+  // nonzero hessian in some target", and the children's sums and gains come from vector_child_totals_kernel
+  int32_t vector_leaf;
 };
 
 // ---- peer-memory exchange over NVLink / NVSwitch (p2p.cuh, p2p_exchange.cu, control_kernel.cu)

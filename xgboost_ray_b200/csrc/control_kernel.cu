@@ -70,6 +70,27 @@ __global__ void leaf_values_kernel(const B2LeafDev* __restrict__ leaves, const i
   }
 }
 
+// vector-leaf tree: leaf i's value of target k from target k's 40-bit sums (sums + k * sums_stride, exponents qexp[2k..])
+// -> leaf_vec[i][k] (the margin update's table) and tree_vec[nid][k] (the read-back block); also keeps the T exponent
+// pairs in the read-back block (qexp_out)
+__global__ void vector_leaf_values_kernel(const B2LeafDev* __restrict__ leaves, const int32_t* __restrict__ n_leaves,
+                                          const long long* __restrict__ sums, size_t sums_stride, const int32_t* __restrict__ qexp,
+                                          int T, int leaf_bits, B2CtlParams p, float* __restrict__ leaf_vec,
+                                          float* __restrict__ tree_vec, int32_t* __restrict__ qexp_out) {
+  const int n = *n_leaves;
+  if (blockIdx.x == 0)
+    for (int t = threadIdx.x; t < 2 * T; t += blockDim.x) qexp_out[t] = qexp[t];
+  for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < n * T; idx += gridDim.x * blockDim.x) {
+    const int i = idx / T, k = idx - i * T;
+    const long long* s = sums + (size_t)k * sums_stride + 4 * (size_t)i;
+    const double kg = ldexp(1.0, leaf_bits - qexp[2 * k]), kh = ldexp(1.0, leaf_bits - qexp[2 * k + 1]);
+    const double G = __ddiv_rn(b2_limbs_to_double(s[0], s[1]), kg), H = __ddiv_rn(b2_limbs_to_double(s[2], s[3]), kh);
+    const float v = __fmul_rn(c_calc_weight(G, H, p), p.eta);
+    leaf_vec[idx] = v;
+    tree_vec[(size_t)leaves[i].nid * T + k] = v;
+  }
+}
+
 // tree-start reset: root node, counters
 __global__ void tree_init_kernel(B2TreeDev tree, B2LevelCtl* ctl0, B2NodeSeg* seg0, B2EvalNode* ev0, int32_t* n_leaves,
                                  int n_rows, B2HistWork* hist_work0) {
@@ -101,6 +122,13 @@ int b2_launch_leaf_plan(const B2LeafDev* leaves, const int32_t* n_leaves, B2SegW
 int b2_launch_leaf_values(const B2LeafDev* leaves, const int32_t* n_leaves, const long long* sums, const int32_t* qexp,
                           int leaf_bits, B2CtlParams p, float* leaf_value, B2TreeDev tree, int32_t* qexp_out, cudaStream_t s) {
   b2::leaf_values_kernel<<<8, 256, 0, s>>>(leaves, n_leaves, sums, qexp, leaf_bits, p, leaf_value, tree, qexp_out);
+  return (int)cudaGetLastError();
+}
+int b2_launch_vector_leaf_values(const B2LeafDev* leaves, const int32_t* n_leaves, const long long* sums, size_t sums_stride,
+                                 const int32_t* qexp, int T, int leaf_bits, B2CtlParams p, float* leaf_vec, float* tree_vec,
+                                 int32_t* qexp_out, cudaStream_t s) {
+  b2::vector_leaf_values_kernel<<<32, 256, 0, s>>>(leaves, n_leaves, sums, sums_stride, qexp, T, leaf_bits, p, leaf_vec, tree_vec,
+                                                  qexp_out);
   return (int)cudaGetLastError();
 }
 int b2_launch_tree_init(B2TreeDev tree, B2LevelCtl* ctl0, B2NodeSeg* seg0, B2EvalNode* ev0, int32_t* n_leaves, int n_rows,

@@ -126,7 +126,9 @@ __device__ __forceinline__ void decide_block(DecideScratch<kThreads>& sm, const 
       nd = a.ev_cur[i]; sg = a.seg_cur[i];
       if (a.can_split) {
         best = a.cand_best[i];
-        if (best.feature >= 0)
+        if (best.feature >= 0 && a.vector_leaf)
+          expand = best.loss_chg > 1e-6f && best.left_g != 0 && best.left_h != 0 && !(best.loss_chg < p.gamma);
+        else if (best.feature >= 0)
           expand = best.loss_chg > 1e-6f && best.left_h != 0 && (nd.sum_h - best.left_h) != 0 && !(best.loss_chg < p.gamma);
       }
     }
@@ -150,7 +152,8 @@ __device__ __forceinline__ void decide_block(DecideScratch<kThreads>& sm, const 
       }
       tree.left[l] = -1; tree.right[l] = -1; tree.feature[l] = -1; tree.parent[l] = nid;
       tree.left[r] = -1; tree.right[r] = -1; tree.feature[r] = -1; tree.parent[r] = nid;
-      const long long lg = best.left_g, lh = best.left_h, rg = nd.sum_g - lg, rh = nd.sum_h - lh;
+      const long long lg = a.vector_leaf ? 0 : best.left_g, lh = a.vector_leaf ? 0 : best.left_h;
+      const long long rg = a.vector_leaf ? 0 : nd.sum_g - lg, rh = a.vector_leaf ? 0 : nd.sum_h - lh;
       tree.sum_g[l] = lg; tree.sum_h[l] = lh; tree.sum_g[r] = rg; tree.sum_h[r] = rh;
       B2SplitWork sw;
       sw.seg_begin = sg.begin; sw.seg_count = sg.count; sw.feature = best.feature; sw.split_bin = best.bin;

@@ -42,6 +42,20 @@ int b2_launch_eval_splits(const long long*, int, const B2EvalNode*, int, const i
                           int, int, B2ColSample, const B2NodeSeg*, B2SiblingSub, const B2DecideArgs*, uint32_t*, cudaStream_t);
 int b2_eval_ctas_per_node(int, int, int);
 int b2_eval_narrow_max_nodes();
+int b2_launch_eval_splits_vector(const long long*, size_t, int, int, const B2EvalNode*, int, const long long*, const float*,
+                                 const int32_t*, const int32_t*, const int32_t*, const uint8_t*, const int32_t*, int,
+                                 B2TrainParamDev, B2SplitCand*, int, const B2LevelCtl*, B2ColSample, const B2NodeSeg*, cudaStream_t);
+int b2_eval_vector_ctas_per_node(int);
+int b2_launch_vector_root_totals(const long long*, size_t, int, int, const int32_t*, int, B2TrainParamDev, long long*, float*,
+                                 cudaStream_t);
+int b2_launch_vector_child_totals(const long long*, size_t, int, int, int, const B2LevelCtl*, const B2SplitWork*, const int32_t*,
+                                  const B2NodeSeg*, const int32_t*, const int32_t*, const int32_t*, const int32_t*, int,
+                                  B2TrainParamDev, long long*, float*, B2EvalNode*, cudaStream_t);
+int b2_launch_vector_leaf_values(const B2LeafDev*, const int32_t*, const long long*, size_t, const int32_t*, int, int, B2CtlParams,
+                                 float*, float*, int32_t*, cudaStream_t);
+int b2_launch_margin_update_vector(float*, int, const uint16_t*, const float*, int64_t, int, cudaStream_t);
+int b2_launch_predict_vector(const float*, int64_t, int, float, const B2TreeNodeDev*, const int32_t*, const float*, int, int, int,
+                             float*, int, cudaStream_t);
 int b2_launch_subsample(float2*, int64_t, uint32_t, uint32_t, uint32_t, double, int, cudaStream_t);
 int b2_p2p_flag_words(int);
 int b2_launch_p2p_reduce_subtract(const void*, const long long*, long long*, const int32_t*, const B2LevelCtl*, int, int, int64_t, int,
@@ -820,8 +834,13 @@ struct Params {
   // reg:quantileerror: one output (and one tree per round) per alpha
   std::vector<float> quantile_alpha{0.5f};
   bool num_class_set = false;
+  // multi_strategy: 0 one_output_per_tree (one tree per target and round), 1 multi_output_tree (one vector-leaf tree per
+  // round for all targets, DESIGN.md 2 item 19; only with T > 1 targets, ignored otherwise)
+  int multi_strategy = 0;
   bool use_cols() const { return colsample_bytree < 1.0f || colsample_bylevel < 1.0f || colsample_bynode < 1.0f; }
+  bool vector_leaf() const { return multi_strategy == 1 && num_target > 1; }
 };
+constexpr int kMaxVectorTargets = 64;   // vector-leaf trees: the level histograms are T times a scalar tree's
 
 struct TreeHost {
   std::vector<int32_t> left, right, parent, feature, split_bin;
@@ -830,6 +849,8 @@ struct TreeHost {
   std::vector<uint8_t> default_left;
   std::vector<uint8_t> split_type;        // 1 = categorical split
   std::vector<uint32_t> cat_bits;         // [n][8] categories that go right (all zero for numeric nodes)
+  // vector-leaf tree: [n][T] -- a leaf's values, an internal node's eta-scaled weights (empty for a scalar tree)
+  std::vector<float> leaf_vec;
   bool any_cat = false;
   int add(int par) {
     int id = (int)left.size();
@@ -945,6 +966,8 @@ struct Booster : HandleBase {
     uint32_t* h_p2p_err = nullptr;         // pinned copy of the peer-memory error word, written at the end of the round
     std::vector<float> dart_w;             // DART: the weights once this round is committed (trees before it + its own)
     bool dart_dropped = false;             // the round changed weights of earlier trees
+    void* vstaging = nullptr;              // vector-leaf tree: pinned copy of the round's d_vblock
+    size_t vstaging_bytes = 0;
   };
   RoundBuffers rb[2];
   int rb_cur = 0;                          // parity of the next round to enqueue
@@ -1012,6 +1035,12 @@ struct Booster : HandleBase {
   DevBuf<float> d_alpha;
   DevBuf<unsigned long long> d_qhist; DevBuf<uint8_t> d_qsel; DevBuf<int32_t> d_one;
   bool refresh_leaves = false;
+  // vector-leaf trees (grow_vector_tree): T-target level histograms [2][T][half][slice], 40-bit leaf sums [T][leaf][4],
+  // leaf values [leaf][T], and the read-back block d_vblock (VectorLayout: node totals, node vectors, exponents)
+  DevBuf<long long> d_vhist[2], d_vsums;
+  DevBuf<float> d_leaf_vec;
+  DevBuf<uint8_t> d_vblock;
+  DevBuf<float> d_leaf_table; std::vector<float> h_leaf_table;   // prediction: [model nodes][T]
   // profiling
   Timers t;
   ~Booster() {
@@ -1033,6 +1062,7 @@ struct Booster : HandleBase {
       if (r.stop) cudaEventDestroy(r.stop);
       for (void* h : r.staging) cudaFreeHost(h);
       if (r.h_p2p_err) cudaFreeHost(r.h_p2p_err);
+      if (r.vstaging) cudaFreeHost(r.vstaging);
     }
     for (auto& kv : eval_cache) delete kv.second;
     if (h_grad_err) cudaFreeHost(h_grad_err);
@@ -1127,6 +1157,13 @@ void set_targets(Params* p, int T) {
     p->num_class = T;
   }
   p->num_target = T;
+  if (p->vector_leaf()) {   // DESIGN.md 2 item 19: what vector-leaf trees do not cover yet
+    if (T > kMaxVectorTargets)
+      fail("multi_strategy=multi_output_tree supports at most %d targets, the label has %d columns", kMaxVectorTargets, T);
+    if (p->dart) fail("multi_strategy=multi_output_tree is not supported with booster=dart");
+    if (p->num_parallel_tree > 1)
+      fail("multi_strategy=multi_output_tree needs num_parallel_tree = 1, got %d", p->num_parallel_tree);
+  }
 }
 
 void parse_params(const char* text, Params* p, int* max_bin_out) {
@@ -1218,6 +1255,11 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     else if (k == "max_cat_threshold") p->max_cat_threshold = i();
     else if (k == "max_bin") { if (max_bin_out) *max_bin_out = i(); }
     else if (k == "interaction_constraints") p->interaction_sets = parse_interaction_sets(v);
+    else if (k == "multi_strategy") {
+      if (v == "one_output_per_tree") p->multi_strategy = 0;
+      else if (v == "multi_output_tree") p->multi_strategy = 1;
+      else fail("multi_strategy='%s' is not supported (supported: one_output_per_tree, multi_output_tree)", v.c_str());
+    }
     else if (k == "booster") {
       if (v == "gbtree") p->dart = false;
       else if (v == "dart") p->dart = true;
@@ -1258,6 +1300,10 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     p->num_class = (int)p->quantile_alpha.size();
   } else if (p->objective != kObjSoftprob) p->num_class = 1;
   if (p->objective == kObjSoftprob && p->num_class < 2) fail("multi:softprob needs num_class >= 2");
+  if (p->multi_strategy == 1 && p->objective == kObjSoftprob)
+    fail("multi_strategy=multi_output_tree is not supported with objective '%s' (vector-leaf trees take the multi-target "
+         "objectives: reg:squarederror, reg:squaredlogerror, reg:pseudohubererror, reg:logistic, binary:logistic, "
+         "binary:logitraw)", p->objective_name.c_str());
   if (p->num_target_set) set_targets(p, p->num_target);
   if (p->max_depth < 1 || p->max_depth > 14) fail("max_depth must be in [1, 14], got %d", p->max_depth);
   if (p->num_parallel_tree < 1 || p->num_parallel_tree > 4096) fail("num_parallel_tree must be in [1, 4096], got %d", p->num_parallel_tree);
@@ -1458,13 +1504,14 @@ void ensure_ctl_tables(Booster* b) {
   b->node_elems = (size_t)G * B2_GROUP_ELEMS;
   // feature-slot sharding of the histogram exchange: rank r owns slots s with s % shards == r (DESIGN.md 5)
   const int world = b->comm ? b->comm->world : 1;
-  b->shards = (world > 1 && world <= 32 && (32 % world) == 0) ? world : 1;
+  // (vector-leaf trees: every rank scans every slot of the allreduced T-target level buffer, no sharding)
+  b->shards = (world > 1 && world <= 32 && (32 % world) == 0 && !b->p.vector_leaf()) ? world : 1;
   b->log2_shards = 0; while ((1 << b->log2_shards) < b->shards) b->log2_shards++;
   b->sp = B2_GROUP_SLOTS / b->shards;
   b->slice_elems = (size_t)G * 2 * B2_BINS * b->sp;
   b->cpn_num = b2_eval_ctas_per_node(G, b->log2_shards, 1);   // the most numeric candidates per node of any level
   b->cpn = b->cpn_num + (b->train->any_cat() ? b2_cat_ctas() : 0);
-  b->hist[0].ensure(half * b->slice_elems); b->hist[1].ensure(half * b->slice_elems);
+  if (!b->p.vector_leaf()) { b->hist[0].ensure(half * b->slice_elems); b->hist[1].ensure(half * b->slice_elems); }   // vector trees: d_vhist
   if (b->shards > 1) {
     auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
     const size_t build_bytes = up(half * b->node_elems * sizeof(long long));
@@ -1711,7 +1758,7 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
     if (b->ic_words > 0) { ic.sets_of = b->d_ic_sets_of.p; ic.compat = b->d_ic_compat.p; ic.words = b->ic_words; }
     da.ic = ic;
     da.cands_per_node = cpn; da.cand_ranks = b->shards; da.cand_rank_stride = max_nodes_level * cpn;
-    da.can_split = can_split ? 1 : 0; da.qbits = p.qbits;
+    da.can_split = can_split ? 1 : 0; da.qbits = p.qbits; da.vector_leaf = 0;
     // one GPU, numeric features only, levels scanned by the narrow layout: the last CTA of the scan decides the level
     // (no decide launch)
     const bool fold_decide = can_split && !multi && !m->any_cat() && max_nodes_level <= b2_eval_narrow_max_nodes();
@@ -1834,6 +1881,221 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   CUDA_CHECK(cudaMemcpyAsync(stg, b->t_block.p, m->any_cat() ? L.bytes : L.off_cat, cudaMemcpyDeviceToHost, s));
 }
 
+// read-back block of a vector-leaf tree (d_vblock): node totals [max_nodes][T][g, h] int64, node vectors [max_nodes][T]
+// float, the T exponent pairs
+struct VectorLayout { size_t off_vec, off_qexp, bytes; };
+VectorLayout vector_layout(int max_depth, int T) {
+  const size_t mx = (size_t)1 << (max_depth + 1);
+  VectorLayout V;
+  V.off_vec = mx * T * 2 * sizeof(long long);
+  V.off_qexp = V.off_vec + mx * T * sizeof(float);
+  V.bytes = V.off_qexp + 2 * (size_t)T * sizeof(int32_t);
+  return V;
+}
+
+// One vector-leaf tree for all T targets (DESIGN.md 2 item 19), one GPU.  The partition, the leaf plan, sampling and the
+// tree topology are the scalar tree's; per target: the quantisation (own exponents), the level histograms (own slice of
+// d_vhist, siblings by hist_subtract) and the leaf sums.  The split scan sums the targets' gains, the child-totals kernel
+// keeps every node's per-target totals, and the leaves are vectors.
+void grow_vector_tree(Booster* b, int slot, TreeStats& st) {
+  Matrix* m = b->train; Ctx* ctx = b->ctx; cudaStream_t s = ctx->stream; const Params& p = b->p;
+  const int64_t n = m->n; const int T = p.num_target; const int G = m->n_groups; const int D = p.max_depth;
+  ensure_ctl_tables(b);
+  const TreeLayout L = tree_layout(D);
+  const VectorLayout V = vector_layout(D, T);
+  static const bool leaf_fused = env_flag("B2_LEAF_FUSED", true);
+  if (!leaf_fused) fail("multi_strategy=multi_output_tree needs the fused leaf pass (unset B2_LEAF_FUSED)");
+  const bool leaf_stream = D <= b2_leaf_acc_max_depth();
+  mark_phase(b, -1);
+  const uint32_t tree_index = (uint32_t)b->trees.size() + (uint32_t)b->pending_trees + (uint32_t)slot;
+  const size_t lcap = (size_t)1 << D, half = (size_t)1 << (D - 1);
+  const size_t tstride = half * b->slice_elems;   // one target's level buffer
+  long long* vtot = (long long*)b->d_vblock.p;
+  float* tree_vec = (float*)(b->d_vblock.p + V.off_vec);
+  int32_t* qexp_out = (int32_t*)(b->d_vblock.p + V.off_qexp);
+  float* vgain = b->t_f32.p + L.max_nodes;        // the scalar tree's leaf_weight array, unused by vector trees
+  for (int k = 0; k < T; ++k) {
+    float2* ghk = b->gh.p + (size_t)k * n;
+    uint32_t* d_absmax = b->d_absmax.p + 2 * k;
+    if (p.subsample < 1.0f) {   // the same rows in every target: the draw depends on (seed, tree, rank, row) only
+      LAUNCH_CHECK(b2_launch_subsample(ghk, n, (uint32_t)p.seed, tree_index, b->comm ? (uint32_t)b->comm->rank : 0u,
+                                       (double)p.subsample, ctx->num_sms, s));
+      st.kernel_launches++;
+    }
+    if (!b->absmax_fused) {
+      CUDA_CHECK(cudaMemsetAsync(d_absmax, 0, 2 * sizeof(uint32_t), s));
+      LAUNCH_CHECK(b2_launch_absmax(ghk, n, d_absmax, ctx->num_sms, s));
+      st.kernel_launches++;
+    }
+  }
+  allreduce(b->comm, b->d_absmax.p, 2 * (size_t)T, kNcclUint32, kNcclMax, s);   // every target's maxima over all ranks
+  for (int k = 0; k < T; ++k) {
+    float2* ghk = b->gh.p + (size_t)k * n;
+    LAUNCH_CHECK(b2_launch_quant_exponent(b->d_absmax.p + 2 * k, b->d_qexp.p + 2 * k, s));
+    LAUNCH_CHECK(b2_launch_quantize(ghk, n, b->d_qexp.p + 2 * k, p.qbits, b->q.p + (size_t)k * n, ctx->num_sms, s));
+    st.kernel_launches += 2;
+  }
+  std::vector<int> n_level_feats(D, m->F);
+  if (p.use_cols()) {   // one draw per tree, as grow_tree
+    const int F = m->F;
+    const uint32_t* fwq = m->fwq.empty() ? nullptr : m->fwq.data();
+    std::vector<uint8_t> mask_tree(F), masks((size_t)D * F);
+    std::vector<B2ColRank> col_scratch(F);
+    const int n_tree = b2_col_select((uint32_t)p.seed, tree_index, B2_SCOPE_TREE, nullptr, fwq, F,
+                                     b2_sample_count((double)p.colsample_bytree, F), col_scratch.data(), mask_tree.data());
+    for (int d = 0; d < D; ++d)
+      n_level_feats[d] = b2_col_select((uint32_t)p.seed, tree_index, B2_SCOPE_LEVEL(d), mask_tree.data(), fwq, F,
+                                       b2_sample_count((double)p.colsample_bylevel, n_tree), col_scratch.data(),
+                                       masks.data() + (size_t)d * F);
+    b->d_col_masks.ensure(masks.size());
+    CUDA_CHECK(cudaMemcpyAsync(b->d_col_masks.p, masks.data(), masks.size(), cudaMemcpyHostToDevice, s));   // pageable source: staged before return
+  }
+  B2TrainParamDev dp;
+  dp.min_child_weight = (double)p.min_child_weight; dp.lambda = (double)p.lambda; dp.alpha = (double)p.alpha;
+  dp.inv_scale_g = dp.inv_scale_h = 1.0;
+  dp.max_cat_to_onehot = p.max_cat_to_onehot; dp.max_cat_threshold = p.max_cat_threshold;
+  dp.max_delta_step = (double)p.max_delta_step;
+  B2CtlParams cp; cp.mcw = dp.min_child_weight; cp.lambda = dp.lambda; cp.alpha = dp.alpha; cp.max_delta_step = dp.max_delta_step;
+  cp.gamma = p.gamma; cp.eta = p.eta;
+  const bool multi = b->comm && b->comm->world > 1;
+  const double node_bytes = (double)b->node_elems * sizeof(long long);
+  const B2TreeDev tree = tree_dev(b);
+  int32_t* d_n_leaves = tree.n_nodes + 1;
+  long long* d_level_rows = b->t_i64.p + 2 * L.max_nodes;
+  B2LevelCtl* ctl = b->d_ctl.p;
+  const int window = window_rows_for(p.qbits);
+  const int n_streams = std::max(1, ctx->num_sms * 3 / G);
+  const int pchunk = b2_split_chunk_rows(), lchunk = b2_part_chunk_rows();
+  const int max_part_chunks_total = (int)((n + pchunk - 1) / pchunk);
+  const int max_leaf_chunks = (int)((n + lchunk - 1) / lchunk) + (int)lcap;
+  const size_t sums_stride = 4 * lcap;
+  LAUNCH_CHECK(b2_launch_tree_init(tree, ctl, b->d_seg[0].p, b->d_ev[0].p, d_n_leaves, (int)n, b->d_hist_work.p, s));
+  CUDA_CHECK(cudaMemsetAsync(b->d_vsums.p, 0, (size_t)T * sums_stride * sizeof(long long), s));
+  mark_phase(b, 0);
+  {   // root histograms, one per target
+    const int chunk_rows = pick_chunk_rows(b, n);
+    const int chunks = (int)((n + chunk_rows - 1) / chunk_rows);
+    for (int k = 0; k < T; ++k) {
+      long long* tgt = b->d_vhist[0].p + (size_t)k * tstride;
+      CUDA_CHECK(cudaMemsetAsync(tgt, 0, b->node_elems * sizeof(long long), s));
+      if (n > 0) {
+        cudaEvent_t e0 = nullptr, e1 = nullptr;
+        record_hist_launch(b, st, e0, e1, true);
+        LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, b->q.p + (size_t)k * n, nullptr, b->d_hist_work.p, 1, chunks, chunk_rows,
+                                    window, G, tgt, nullptr, 0, 1, ctx->num_sms, s));
+        record_hist_launch(b, st, e0, e1, false);
+        st.hist_launches++; st.kernel_launches++;
+      }
+      allreduce(b->comm, tgt, b->node_elems, kNcclInt64, kNcclSum, s);   // exact: integer sums
+      if (multi) st.allreduce_bytes += node_bytes;
+    }
+  }
+  mark_phase(b, 1);
+  LAUNCH_CHECK(b2_launch_vector_root_totals(b->d_vhist[0].p, tstride, T, G, b->d_qexp.p, p.qbits, dp, vtot, vgain, s));
+  st.kernel_launches++;
+  const int cpn = b2_eval_vector_ctas_per_node(G);
+  int hb = 0;
+  for (int d = 0; d <= D; ++d) {
+    const int cur = d & 1, nxt = cur ^ 1;
+    const int max_nodes_level = 1 << d;
+    const bool can_split = d < D;
+    B2DecideArgs da;
+    da.ctl_cur = ctl + cur; da.ctl_nxt = ctl + nxt; da.seg_cur = b->d_seg[cur].p; da.seg_nxt = b->d_seg[nxt].p;
+    da.ev_cur = b->d_ev[cur].p; da.ev_nxt = b->d_ev[nxt].p;
+    da.cands = b->d_cands.p; da.cand_best = b->d_cand_best.p; da.local_cands = b->d_cands.p;
+    da.tree = tree; da.split_work = b->d_split_work.p; da.pair_parent_hist = b->d_pair_parent.p; da.leaves = b->d_leaves.p;
+    da.n_leaves = d_n_leaves; da.has_missing = m->d_has_missing.p; da.qexp = b->d_qexp.p;
+    da.part_counters = can_split ? b->d_counters.p : nullptr; da.p = cp;
+    B2Interaction ic{nullptr, nullptr, 0};
+    if (b->ic_words > 0) { ic.sets_of = b->d_ic_sets_of.p; ic.compat = b->d_ic_compat.p; ic.words = b->ic_words; }
+    da.ic = ic;
+    da.cands_per_node = cpn; da.cand_ranks = 1; da.cand_rank_stride = max_nodes_level * cpn;
+    da.can_split = can_split ? 1 : 0; da.qbits = p.qbits; da.vector_leaf = 1;
+    if (can_split) {
+      B2ColSample cs;
+      cs.level_mask = p.use_cols() ? b->d_col_masks.p + (size_t)d * m->F : nullptr;
+      cs.fwq = m->fwq.empty() ? nullptr : m->d_fwq.p;
+      cs.bynode = (double)p.colsample_bynode; cs.n_level = n_level_feats[d]; cs.n_features = m->F;
+      cs.seed = (uint32_t)p.seed; cs.tree = p.use_cols() ? tree_index : 0u;
+      cs.ic = ic;
+      LAUNCH_CHECK(b2_launch_eval_splits_vector(b->d_vhist[hb].p, tstride, T, G, b->d_ev[cur].p, max_nodes_level, vtot, vgain,
+                                                m->d_group_first.p, m->d_group_size.p, m->d_nbins.p, m->d_has_missing.p,
+                                                b->d_qexp.p, p.qbits, dp, b->d_cands.p, cpn, ctl + cur, cs, b->d_seg[cur].p, s));
+      st.kernel_launches++;
+    }
+    LAUNCH_CHECK(b2_launch_decide(&da, nullptr, s));
+    st.kernel_launches++;
+    mark_phase(b, 4);
+    if (!can_split) break;
+    // the children's per-target totals, from this level's histograms (still in d_vhist[hb])
+    LAUNCH_CHECK(b2_launch_vector_child_totals(b->d_vhist[hb].p, tstride, T, G, max_nodes_level, ctl + cur, b->d_split_work.p,
+                                               b->d_pair_parent.p, b->d_seg[nxt].p, tree.parent, m->d_feat_byte.p, m->d_nbins.p,
+                                               b->d_qexp.p, p.qbits, dp, vtot, vgain, b->d_ev[nxt].p, s));
+    st.kernel_launches++;
+    const int32_t* ridx_in = d == 0 ? nullptr : b->ridx[cur].p;
+    if (d == D - 1) {   // the children are leaves: every row's leaf index (and without leaf_stream, the leaf sums)
+      LAUNCH_CHECK(b2_launch_leaf_plan(b->d_leaves.p, &ctl[cur].leaf_base_next, b->d_seg_work.p, ctl + 2, s));
+      for (int k = 0; k < (leaf_stream ? 1 : T); ++k) {
+        const float2* ghk = b->gh.p + (size_t)k * n;
+        long long* sums = leaf_stream ? nullptr : b->d_vsums.p + (size_t)k * sums_stride;
+        LAUNCH_CHECK(b2_launch_leaf_sums(ghk, b->ridx[0].p, b->ridx[1].p, b->d_seg_work.p, ctl + 2, max_leaf_chunks,
+                                         b->d_qexp.p + 2 * k, 40, sums, b->pos.p, ctx->num_sms, s));
+        LAUNCH_CHECK(b2_launch_final_assign(m->bins_col.p, m->col_stride, ridx_in, b->d_split_work.p, ctl + cur,
+                                            max_part_chunks_total + max_nodes_level, ghk, b->d_qexp.p + 2 * k, 40, sums, b->pos.p,
+                                            0, ctx->num_sms, s));
+        st.kernel_launches += 2;
+      }
+      st.kernel_launches++;
+      mark_phase(b, 5);
+      continue;
+    }
+    const bool need_hist = d + 1 < D;
+    B2FinalizeArgs fin;
+    fin.ctl_nxt = ctl + nxt; fin.seg_nxt = b->d_seg[nxt].p; fin.ev_nxt = b->d_ev[nxt].p; fin.pair_parent_hist = b->d_pair_parent.p;
+    fin.hist_work = b->d_hist_work.p; fin.triples = b->d_triples.p; fin.stat_rows = d_level_rows + d + 1; fin.done = b->d_part_done.p;
+    fin.max_pairs = max_nodes_level; fin.need_hist = need_hist ? 1 : 0; fin.n_streams = n_streams; fin.window_rows = window;
+    fin.chunk_rows_override = p.hist_chunk_rows;
+    LAUNCH_CHECK(b2_launch_partition(m->bins_col.p, m->col_stride, ridx_in, b->ridx[nxt].p, b->d_split_work.p, ctl + cur,
+                                     max_part_chunks_total + max_nodes_level, b->d_counters.p, 0, fin, ctx->num_sms, s));
+    st.kernel_launches++;
+    mark_phase(b, 5);
+    if (need_hist) {   // per target: built children, then siblings = parent - built over the target's whole slice
+      const int nh = hb ^ 1;
+      for (int k = 0; k < T; ++k) {
+        long long* tgt = b->d_vhist[nh].p + (size_t)k * tstride;
+        CUDA_CHECK(cudaMemsetAsync(tgt, 0, (size_t)max_nodes_level * b->node_elems * sizeof(long long), s));
+        cudaEvent_t e0 = nullptr, e1 = nullptr;
+        record_hist_launch(b, st, e0, e1, true);
+        LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, b->q.p + (size_t)k * n, b->ridx[nxt].p, b->d_hist_work.p, 0, 0, 0, window,
+                                    G, tgt, ctl + nxt, 0, max_nodes_level, ctx->num_sms, s));
+        record_hist_launch(b, st, e0, e1, false);
+        allreduce(b->comm, tgt, (size_t)max_nodes_level * b->node_elems, kNcclInt64, kNcclSum, s);   // the built children
+        if (multi) st.allreduce_bytes += max_nodes_level * node_bytes;
+        LAUNCH_CHECK(b2_launch_hist_subtract(b->d_vhist[hb].p + (size_t)k * tstride, tgt, b->d_triples.p, max_nodes_level,
+                                             (int64_t)b->slice_elems, ctl + nxt, s));
+        st.hist_launches++; st.kernel_launches += 2;
+      }
+      mark_phase(b, 1);
+      hb = nh;
+    }
+  }
+  if (leaf_stream)
+    for (int k = 0; k < T; ++k) {
+      LAUNCH_CHECK(b2_launch_leaf_accumulate(b->gh.p + (size_t)k * n, b->pos.p, n, D, b->d_qexp.p + 2 * k, 40,
+                                             b->d_vsums.p + (size_t)k * sums_stride, ctx->num_sms, s));
+      st.kernel_launches++;
+    }
+  allreduce(b->comm, b->d_vsums.p, (size_t)T * sums_stride, kNcclInt64, kNcclSum, s);   // limb by limb: exact
+  if (multi) st.allreduce_bytes += (double)T * sums_stride * sizeof(long long);
+  LAUNCH_CHECK(b2_launch_vector_leaf_values(b->d_leaves.p, d_n_leaves, b->d_vsums.p, sums_stride, b->d_qexp.p, T, 40, cp,
+                                            b->d_leaf_vec.p, tree_vec, qexp_out, s));
+  LAUNCH_CHECK(b2_launch_margin_update_vector(b->margin.p, T, b->pos.p, b->d_leaf_vec.p, n, ctx->num_sms, s));
+  st.kernel_launches += 2;
+  mark_phase(b, 6);
+  CUDA_CHECK(cudaMemcpyAsync(b->rb[b->rb_cur].staging[slot], b->t_block.p, L.off_cat, cudaMemcpyDeviceToHost, s));
+  CUDA_CHECK(cudaMemcpyAsync(b->rb[b->rb_cur].vstaging, b->d_vblock.p, V.bytes, cudaMemcpyDeviceToHost, s));
+}
+
 void apply_tree_stats(Booster* b, long long hist_launches, long long kernel_launches, double allreduce_bytes,
                       const std::vector<std::pair<cudaEvent_t, cudaEvent_t>>& ev) {
   b->t.hist_launches += hist_launches; b->t.kernel_launches += kernel_launches; b->t.allreduce_bytes += allreduce_bytes;
@@ -1858,6 +2120,30 @@ void prepare_tree_buffers(Booster* b, int slot) {
   }
   std::vector<void*>& staging = b->rb[b->rb_cur].staging;
   while ((int)staging.size() <= slot) { void* h = nullptr; CUDA_CHECK(cudaMallocHost(&h, L.bytes)); staging.push_back(h); }
+  if (b->p.vector_leaf()) {
+    const int T = b->p.num_target, D = b->p.max_depth;
+    const size_t lcap = (size_t)1 << D, half = (size_t)1 << (D - 1);
+    const size_t hist_elems = (size_t)T * half * b->slice_elems;
+    // the level histograms, the quantised pairs and the leaf sums of the T targets
+    const double gib = (2.0 * (double)hist_elems * sizeof(long long) + (double)rows * T * sizeof(int2) +
+                        (double)T * 4 * lcap * sizeof(long long)) / (double)(1ull << 30);
+    if (gib > 48.0)
+      fail("multi_strategy=multi_output_tree with %d targets at max_depth %d needs %.1f GiB of per-target buffers (at most "
+           "48); use fewer targets, a smaller max_depth or multi_strategy=one_output_per_tree", T, D, gib);
+    b->d_vhist[0].ensure(hist_elems); b->d_vhist[1].ensure(hist_elems);
+    b->d_vsums.ensure((size_t)T * 4 * lcap); b->d_leaf_vec.ensure(lcap * T);
+    b->d_absmax.ensure(2 * (size_t)T); b->d_qexp.ensure(2 * (size_t)T);
+    b->q.ensure(rows * T);
+    const VectorLayout V = vector_layout(D, T);
+    b->d_vblock.ensure(V.bytes);
+    Booster::RoundBuffers& R = b->rb[b->rb_cur];
+    if (R.vstaging_bytes != V.bytes) {
+      if (R.vstaging) cudaFreeHost(R.vstaging);
+      R.vstaging = nullptr; R.vstaging_bytes = 0;
+      CUDA_CHECK(cudaMallocHost(&R.vstaging, V.bytes));
+      R.vstaging_bytes = V.bytes;
+    }
+  }
 }
 
 // One class tree: replay its CUDA graph when the launch sequence is the same for every tree (no row / column sampling,
@@ -1872,7 +2158,8 @@ void run_tree(Booster* b, int k, int slot) {
                         p.profile < 2 && p.num_parallel_tree == 1;
   auto direct = [&]() {
     TreeStats st;
-    grow_tree(b, k, slot, st);
+    if (p.vector_leaf()) grow_vector_tree(b, slot, st);
+    else grow_tree(b, k, slot, st);
     apply_tree_stats(b, st.hist_launches, st.kernel_launches, st.allreduce_bytes, st.hist_ev);
     b->direct_trees[k]++;
   };
@@ -1885,7 +2172,7 @@ void run_tree(Booster* b, int k, int slot) {
     cudaGraph_t graph = nullptr; cudaGraphExec_t exec = nullptr;
     bool ok = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
     if (ok) {
-      try { grow_tree(b, k, slot, st); }
+      try { if (p.vector_leaf()) grow_vector_tree(b, slot, st); else grow_tree(b, k, slot, st); }
       catch (const B2Error& e) { cudaStreamEndCapture(s, &graph); if (graph) cudaGraphDestroy(graph); cudaGetLastError(); throw; }
       ok = cudaStreamEndCapture(s, &graph) == cudaSuccess && graph != nullptr;
     }
@@ -1956,8 +2243,70 @@ void materialize_tree(Booster* b, const void* block) {
   b->trees.push_back(std::move(t));
 }
 
+// a vector-leaf tree from its read-back blocks (grow_vector_tree): the scalar block's topology, splits and loss_chg, and
+// the vector block's per-target node totals (sum_hess = sum over the targets of H_k; an internal node's vector holds
+// fp32(fp32(w_k) * eta) of its own sums) and leaf vectors
+void materialize_vector_tree(Booster* b, const void* block, const void* vblock) {
+  Matrix* m = b->train; const Params& p = b->p; const int T = p.num_target;
+  const TreeLayout L = tree_layout(p.max_depth);
+  const VectorLayout V = vector_layout(p.max_depth, T);
+  const char* st = (const char*)block;
+  const int32_t* i32 = (const int32_t*)st; const size_t mx = L.max_nodes;
+  const float* f32 = (const float*)(st + L.off_f32);
+  const long long* vtot = (const long long*)vblock;
+  const float* vec = (const float*)((const char*)vblock + V.off_vec);
+  const int32_t* qexp = (const int32_t*)((const char*)vblock + V.off_qexp);
+  const int nn = i32[7 * mx];
+  if (nn < 1 || (size_t)nn > mx) fail("corrupt tree read-back (n_nodes=%d)", nn);
+  TreeHost t;
+  t.leaf_vec.assign((size_t)nn * T, 0.0f);
+  for (int i = 0; i < nn; ++i) {
+    t.add(i32[2 * mx + i]);
+    t.left[i] = i32[i]; t.right[i] = i32[mx + i]; t.feature[i] = i32[3 * mx + i];
+    double H_sum = 0.0;
+    for (int k = 0; k < T; ++k) {
+      const double G = (double)vtot[((size_t)i * T + k) * 2] * ldexp(1.0, qexp[2 * k] - p.qbits);
+      const double H = (double)vtot[((size_t)i * T + k) * 2 + 1] * ldexp(1.0, qexp[2 * k + 1] - p.qbits);
+      H_sum += H;
+      t.leaf_vec[(size_t)i * T + k] = t.feature[i] >= 0 ? h_calc_weight(p, G, H) * p.eta : vec[(size_t)i * T + k];
+    }
+    t.sum_hess[i] = H_sum;
+    if (t.feature[i] >= 0) {
+      const int f = t.feature[i], bin = i32[4 * mx + i];
+      t.split_bin[i] = bin; t.default_left[i] = (uint8_t)i32[5 * mx + i]; t.loss_chg[i] = f32[i];
+      t.cond[i] = bin < 0 ? m->min_vals[f] : m->cut_vals[m->cut_ptrs[f] + bin];
+    }
+  }
+  const long long* level_rows = (const long long*)(st + L.off_i64) + 2 * mx;
+  long long rows = m->n;
+  for (int d = 1; d < p.max_depth; ++d) rows += level_rows[d];
+  b->t.hist_rows += rows * T;
+  b->trees.push_back(std::move(t));
+}
+
+// every tree of a vector-leaf model has a leaf vector, no tree of a scalar model has one (continuing a model with the
+// other multi_strategy is refused)
+void check_tree_kinds(const Booster* b) {
+  const int T = b->p.num_target;
+  for (size_t i = 0; i < b->trees.size(); ++i) {
+    const TreeHost& t = b->trees[i];
+    if (b->p.vector_leaf() && t.leaf_vec.size() != (size_t)t.size() * T)
+      fail("tree %zu is a single-output tree (multi_strategy=one_output_per_tree); this model uses multi_strategy="
+           "multi_output_tree: a model keeps the strategy it was trained with", i);
+    if (!b->p.vector_leaf() && !t.leaf_vec.empty())
+      fail("tree %zu is a vector-leaf tree (multi_strategy=multi_output_tree); this model uses multi_strategy="
+           "one_output_per_tree: a model keeps the strategy it was trained with", i);
+  }
+}
+
 void sync_device_trees(Booster* b) {
   if (b->d_trees_synced == (int)b->trees.size()) return;
+  check_tree_kinds(b);
+  if (b->p.vector_leaf()) {   // [model nodes][T], in the order of d_nodes
+    b->h_leaf_table.clear();
+    for (auto& t : b->trees) b->h_leaf_table.insert(b->h_leaf_table.end(), t.leaf_vec.begin(), t.leaf_vec.end());
+    upload(b->d_leaf_table, b->h_leaf_table, b->ctx->stream);
+  }
   b->h_nodes.clear(); b->h_tree_offset.clear(); b->h_cat_table.clear();
   for (auto& t : b->trees) {
     b->h_tree_offset.push_back((int32_t)b->h_nodes.size());
@@ -2313,7 +2662,10 @@ void finish_round(Booster* b, Booster::RoundBuffers& R, int n_trees, bool check_
     fail("%s: a gradient or hessian is not finite (the margin left the range where the objective's exp is finite)",
          b->p.objective_name.c_str());
   }
-  for (int slot = 0; slot < n_trees; ++slot) materialize_tree(b, R.staging[slot]);
+  for (int slot = 0; slot < n_trees; ++slot) {
+    if (b->p.vector_leaf()) materialize_vector_tree(b, R.staging[slot], R.vstaging);
+    else materialize_tree(b, R.staging[slot]);
+  }
   if (b->p.dart) {   // the weights are committed with the trees
     b->tree_w = R.dart_w;
     if (R.dart_dropped) b->weights_version++;
@@ -2363,6 +2715,17 @@ void dart_margins(Booster* b, const std::vector<float>& w_old, const std::vector
                                       b->d_dart_w_full.p, drop, full, b->ctx->num_sms, s));
 }
 
+// out += the trees [tree_begin, tree_end) on the raw rows of m (the device trees are in sync)
+void predict_trees(Booster* b, Matrix* m, int tree_begin, int tree_end, float* out) {
+  if (b->p.vector_leaf())
+    LAUNCH_CHECK(b2_launch_predict_vector(m->raw.p, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_leaf_table.p,
+                                          tree_begin, tree_end, b->p.num_target, out, b->ctx->num_sms, b->ctx->stream));
+  else
+    LAUNCH_CHECK(b2_launch_predict(m->raw.p, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, tree_begin,
+                                   tree_end, b->p.num_class, b->p.num_parallel_tree, device_weights(b), out, b->ctx->num_sms,
+                                   b->ctx->stream));
+}
+
 void ensure_train_margin(Booster* b) {
   if (b->margin_ready) return;
   drain_round(b);   // the margin is rebuilt from every tree of the model
@@ -2378,8 +2741,7 @@ void ensure_train_margin(Booster* b) {
   } else if (!b->trees.empty()) {
     if (!m->has_raw) fail("continuing training from existing trees needs the raw data of the train matrix (B2_MatrixEnsureRaw)");
     sync_device_trees(b);
-    LAUNCH_CHECK(b2_launch_predict(m->raw.p, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, 0, (int)b->trees.size(),
-                                   b->p.num_class, b->p.num_parallel_tree, nullptr, b->margin.p, b->ctx->num_sms, b->ctx->stream));
+    predict_trees(b, m, 0, (int)b->trees.size(), b->margin.p);
   }
   b->margin_ready = true;
 }
@@ -2536,6 +2898,9 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
     b->gh_round.ensure((size_t)std::max<int64_t>(n * K, 1));
     CUDA_CHECK(cudaMemcpyAsync(b->gh_round.p, b->gh.p, (size_t)n * K * sizeof(float2), cudaMemcpyDeviceToDevice, s));
   }
+  const int round_trees = b->p.vector_leaf() ? 1 : K * npt;   // a vector-leaf tree covers every target
+  if (b->p.vector_leaf()) run_tree(b, 0, 0);
+  else
   for (int k = 0; k < K; ++k)
     for (int j = 0; j < npt; ++j) {
       if (restore_gh && j > 0)
@@ -2556,7 +2921,7 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
   // this round is queued behind the previous one: make it the pending round, then finish the previous one while the
   // device works (its buffers are the set the next round enqueues into)
   const int prev_trees = b->pending_trees; const bool prev_check = b->pending_check_finite;
-  b->pending_trees = K * npt; b->pending_check_finite = check_finite;
+  b->pending_trees = round_trees; b->pending_check_finite = check_finite;
   b->rb_cur ^= 1;
   if (prev_trees) finish_round(b, b->rb[b->rb_cur], prev_trees, prev_check);
   if (check_finite) drain_round(b);
@@ -2638,8 +3003,7 @@ float* eval_margin(Booster* b, Matrix* m) {
   const int nt = (int)b->trees.size();
   if (c->n_trees_applied < nt) {
     sync_device_trees(b);
-    LAUNCH_CHECK(b2_launch_predict(m->raw.p, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, c->n_trees_applied, nt, K, b->p.num_parallel_tree,
-                                   device_weights(b), c->margin.p, b->ctx->num_sms, b->ctx->stream));
+    predict_trees(b, m, c->n_trees_applied, nt, c->margin.p);
     c->n_trees_applied = nt;
   }
   return c->margin.p;
@@ -3114,6 +3478,9 @@ int B2_BoosterCreate(const char* params, B2Handle trainh, B2Handle commh, B2Hand
       if (b->p.num_target_set && b->p.num_target != m->n_targets)
         fail("the model has %d targets, the train matrix's label has %d columns", b->p.num_target, m->n_targets);
       set_targets(&b->p, m->n_targets);
+      if (b->p.vector_leaf() && m->any_cat())
+        fail("multi_strategy=multi_output_tree is not supported with categorical features (the train matrix has %zu)",
+             m->cat_feats.size());
       b->ctx = m->ctx; b->n_features = m->F; CUDA_CHECK(cudaSetDevice(m->ctx->device));
       if (!b->p.interaction_sets.empty()) {   // sets_of[f] bit k: feature f is in set k
         const int W = (int)((b->p.interaction_sets.size() + 63) / 64);
@@ -3323,8 +3690,7 @@ int B2_BoosterPredict(B2Handle bh, B2Handle mh, int32_t output_margin, int32_t t
   DevBuf<float> tmp; tmp.ensure((size_t)std::max<int64_t>(out_len, 1));
   init_margin(b, tmp.p, m);
   sync_device_trees(b);
-  LAUNCH_CHECK(b2_launch_predict(m->raw.p, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, tree_begin, tree_end, K, b->p.num_parallel_tree,
-                                 device_weights(b), tmp.p, b->ctx->num_sms, s));
+  predict_trees(b, m, tree_begin, tree_end, tmp.p);
   if (!output_margin) LAUNCH_CHECK(b2_launch_transform(b->p.objective, K, tmp.p, m->n, b->ctx->num_sms, s));
   if (out_len > 0) CUDA_CHECK(cudaMemcpyAsync(out, tmp.p, out_len * sizeof(float), cudaMemcpyDeviceToHost, s));
   CUDA_CHECK(cudaStreamSynchronize(s));
@@ -3357,6 +3723,9 @@ int B2_BoosterPredictContribs(B2Handle bh, B2Handle mh, int32_t tree_begin, int3
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
   cudaStream_t s = b->ctx->stream; const int K = b->p.num_class; const int F = m->F;
   const size_t per_row = (size_t)K * (F + 1) * (interactions ? (size_t)(F + 1) : 1);
+  if (b->p.vector_leaf())
+    fail("%s is not supported for vector-leaf trees (multi_strategy=multi_output_tree)",
+         interactions ? "pred_interactions" : "pred_contribs");
   if (out_len != m->n * (int64_t)per_row) fail("output buffer has %lld values, expected %lld", (long long)out_len, (long long)(m->n * (int64_t)per_row));
   check_predict_args(b, m, tree_begin, &tree_end);
   build_paths(b);
@@ -3570,6 +3939,34 @@ int B2_BoosterSetTreeCategories(B2Handle bh, int32_t tree, const uint8_t* split_
     for (int w8 = 0; w8 < 8; ++w8) t.cat_bits[i * 8 + w8] = split_type[i] ? cat_bits[i * 8 + w8] : 0u;
   }
   b->d_trees_synced = 0; b->paths_synced = -1; b->margin_ready = false;
+  for (auto& kv : b->eval_cache) if (kv.second) kv.second->n_trees_applied = 0, kv.second->n = -1;
+  API_END
+}
+int B2_BoosterGetTreeLeafVector(B2Handle bh, int32_t tree, float* out, int64_t len) {
+  API_BEGIN
+  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
+  if (tree < 0 || tree >= (int)b->trees.size()) fail("tree index %d out of range", tree);
+  const TreeHost& t = b->trees[tree];
+  if (t.leaf_vec.empty()) fail("tree %d is not a vector-leaf tree", tree);
+  if (len != (int64_t)t.leaf_vec.size()) fail("leaf vector buffer has %lld values, tree %d has %zu", (long long)len, tree, t.leaf_vec.size());
+  memcpy(out, t.leaf_vec.data(), t.leaf_vec.size() * sizeof(float));
+  API_END
+}
+int B2_BoosterSetTreeLeafVector(B2Handle bh, int32_t tree, const float* v, int64_t len) {
+  API_BEGIN
+  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
+  if (tree < 0 || tree >= (int)b->trees.size()) fail("tree index %d out of range", tree);
+  if (!b->p.vector_leaf())
+    fail("this booster grows single-output trees (multi_strategy=one_output_per_tree, %d target(s)); a vector-leaf tree "
+         "needs multi_strategy=multi_output_tree and num_target > 1", b->p.num_target);
+  TreeHost& t = b->trees[tree];
+  const int64_t want = (int64_t)t.size() * b->p.num_target;
+  if (len != want) fail("leaf vector has %lld values, tree %d needs %lld (%d nodes x %d targets)", (long long)len, tree,
+                        (long long)want, t.size(), b->p.num_target);
+  t.leaf_vec.assign(v, v + len);
+  b->d_trees_synced = 0; b->margin_ready = false;
   for (auto& kv : b->eval_cache) if (kv.second) kv.second->n_trees_applied = 0, kv.second->n = -1;
   API_END
 }

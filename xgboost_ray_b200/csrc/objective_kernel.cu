@@ -674,6 +674,24 @@ __global__ void predict_kernel(const float* __restrict__ X, int64_t n, int F, fl
   }
 }
 
+// vector-leaf trees: each tree adds the leaf vector of the leaf the row reaches (leaf_vec [node][T], the model's nodes
+// in tree order) to the row's T margins, tree by tree as the train margin receives them
+__global__ void predict_vector_kernel(const float* __restrict__ X, int64_t n, int F, float missing, int missing_is_nan,
+                                      const B2TreeNodeDev* __restrict__ nodes, const int32_t* __restrict__ tree_offset,
+                                      const float* __restrict__ leaf_vec, int tree_begin, int tree_end, int T,
+                                      float* __restrict__ out) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float* x = X + i * F;
+    float* o = out + i * T;
+    for (int t = tree_begin; t < tree_end; ++t) {
+      float unused;
+      const int nid = b2_tree_leaf(nodes + tree_offset[t], x, missing, missing_is_nan, nullptr, &unused);
+      const float* v = leaf_vec + ((size_t)tree_offset[t] + nid) * T;
+      for (int k = 0; k < T; ++k) o[k] += __ldg(v + k);
+    }
+  }
+}
+
 __global__ void fill_kernel(float* out, int64_t n, float v) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = v;
 }
@@ -826,6 +844,13 @@ int b2_launch_predict(const float* X, int64_t n, int F, float missing, const B2T
   if (n <= 0 || tree_end <= tree_begin) return 0;
   b2::predict_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(X, n, F, missing, missing != missing ? 1 : 0, nodes, tree_offset,
                                                          cat_table, tree_begin, tree_end, K, npt < 1 ? 1 : npt, weights, out);
+  return (int)cudaGetLastError();
+}
+int b2_launch_predict_vector(const float* X, int64_t n, int F, float missing, const B2TreeNodeDev* nodes, const int32_t* tree_offset,
+                             const float* leaf_vec, int tree_begin, int tree_end, int T, float* out, int num_sms, cudaStream_t s) {
+  if (n <= 0 || tree_end <= tree_begin) return 0;
+  b2::predict_vector_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(X, n, F, missing, missing != missing ? 1 : 0, nodes, tree_offset,
+                                                                 leaf_vec, tree_begin, tree_end, T, out);
   return (int)cudaGetLastError();
 }
 int b2_launch_fill(float* out, int64_t n, float v, int num_sms, cudaStream_t s) {

@@ -328,6 +328,17 @@ margin_update_kernel(float* __restrict__ margin, int K, int k, const uint16_t* _
     margin[i * K + k] += __ldg(leaf_value + pos[i]);
 }
 
+// vector-leaf tree: row i reads its leaf index once and adds the leaf's T values to its T contiguous margins
+__global__ void __launch_bounds__(256)
+margin_update_vector_kernel(float* __restrict__ margin, int T, const uint16_t* __restrict__ pos,
+                            const float* __restrict__ leaf_vec, int64_t n) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float* v = leaf_vec + (size_t)pos[i] * T;
+    float* m = margin + i * T;
+    for (int k = 0; k < T; ++k) m[k] += __ldg(v + k);
+  }
+}
+
 // ---- leaf sums in natural row order: sums[pos[i]] += fixed(gh[i]).  pos and gh stream (10 bytes per row) instead of
 // being gathered per leaf.  The values are the same 40-bit fixed-point integers leaf_sums_kernel / final_assign_kernel
 // add, so the sums are bit-identical in any order.
@@ -466,6 +477,14 @@ int b2_launch_margin_update(float* margin, int K, int k, const uint16_t* pos, co
   int64_t want = (n + 255) / 256;
   int grid = (int)(want < (int64_t)num_sms * 16 ? want : (int64_t)num_sms * 16);
   b2::margin_update_kernel<<<grid, 256, 0, stream>>>(margin, K, k, pos, leaf_value, weight, n);
+  return (int)cudaGetLastError();
+}
+int b2_launch_margin_update_vector(float* margin, int T, const uint16_t* pos, const float* leaf_vec, int64_t n, int num_sms,
+                                   cudaStream_t stream) {
+  if (n <= 0) return 0;
+  int64_t want = (n + 255) / 256;
+  int grid = (int)(want < (int64_t)num_sms * 16 ? want : (int64_t)num_sms * 16);
+  b2::margin_update_vector_kernel<<<grid, 256, 0, stream>>>(margin, T, pos, leaf_vec, n);
   return (int)cudaGetLastError();
 }
 int b2_launch_pred_update(float* margin, int K, int k, const int32_t* ridx0, const int32_t* ridx1, const void* work,

@@ -625,9 +625,268 @@ __global__ void root_totals_kernel(const long long* __restrict__ level_hist, int
   }
 }
 
+// ---------------------------------------------------------------- vector-leaf trees (multi_strategy=multi_output_tree)
+// DESIGN.md 2 item 19.  One tree for T targets: target k has its own quantisation exponents (qexp[2k], qexp[2k + 1]) and
+// its own level histograms at level_hist + k * tstride (the scalar layout, one node slot per hist_index).  vtot holds
+// every node's per-target fixed-point totals [nid][T][g, h] and vgain its fp32 gain(node) = fp32(sum_k CalcGain(G_k, H_k)).
+__device__ __forceinline__ double vector_gain(const long long* __restrict__ tot, int T, const int32_t* __restrict__ qexp, int qbits,
+                                              const B2TrainParamDev& p) {
+  double acc = 0.0;
+  for (int k = 0; k < T; ++k) {
+    const double G = __dmul_rn(__ll2double_rn(tot[2 * k]), ldexp(1.0, qexp[2 * k] - qbits));
+    const double H = __dmul_rn(__ll2double_rn(tot[2 * k + 1]), ldexp(1.0, qexp[2 * k + 1] - qbits));
+    acc = __dadd_rn(acc, calc_gain(G, H, p));
+  }
+  return acc;
+}
+
+// The narrow layout of eval_node_cta for every level (4 slots x 256 bins per CTA, 2 bins per thread), looping over the
+// targets: per target the exact int64 prefix of the thread's bins, then that target's CalcGain terms added, in ascending
+// k, to one double accumulator per (bin, direction, child).  A child "has hessian" when its hessian sum is nonzero in
+// some target; the two bits ride in the candidate's left_g / left_h for decide's expand test.  No min_child_weight
+// filter: a target below it adds 0.  Backward candidates exist when the feature has missing values and, for some
+// target, the node's sums over the real bins differ from its totals.
+__global__ void __launch_bounds__(kEvalThreads, 1)
+eval_splits_vector_kernel(const long long* __restrict__ level_hist, size_t tstride, int T, int n_groups,
+                          const B2EvalNode* __restrict__ nodes, const long long* __restrict__ vtot, const float* __restrict__ vgain,
+                          const int32_t* __restrict__ group_first, const int32_t* __restrict__ group_size,
+                          const int32_t* __restrict__ nbins, const uint8_t* __restrict__ has_missing,
+                          const int32_t* __restrict__ qexp, int qbits, B2TrainParamDev p, B2SplitCand* cands, int cand_stride,
+                          const B2LevelCtl* __restrict__ ctl, B2ColSample cs, const B2NodeSeg* __restrict__ seg) {
+  const int sp = B2_GROUP_SLOTS;
+  const int cpn = eval_ctas_per_node(n_groups, sp, kEvalSlots);
+  const int node = blockIdx.x / cpn, cta_in_node = blockIdx.x % cpn;
+  if (node >= ctl->n_nodes) return;   // uniform over the CTA
+  __shared__ long long s_wg[kEvalWarps][kEvalSlots], s_wh[kEvalWarps][kEvalSlots];
+  __shared__ long long s_tg[kEvalSlots], s_th[kEvalSlots];
+  __shared__ unsigned long long s_key[kEvalWarps];
+  __shared__ uint8_t s_allowed[kEvalSlots];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int s = threadIdx.x & (kEvalSlots - 1), b0 = (threadIdx.x / kEvalSlots) * kEvalBinsPerThread;
+  const int v = cta_in_node * kEvalSlots + s;
+  const bool v_ok = v < n_groups * sp;
+  const int group = v_ok ? v / sp : 0, slot = v_ok ? v % sp : 0;
+  const size_t slice_elems = (size_t)n_groups * 2 * B2_BINS * sp;
+  const B2EvalNode nd = nodes[node];
+  const int nid = seg[node].nid;
+  const size_t in_node = (size_t)nd.hist_index * slice_elems + (size_t)(group * 2) * B2_BINS * sp + slot;
+  const int f = group_first[group] + slot;
+  bool active = v_ok && slot < group_size[group];
+  if (active && cs.level_mask) active = cs.level_mask[f] != 0;
+  if (cs.bynode < 1.0 || cs.ic.sets_of) {
+    if (threadIdx.x < kEvalSlots) {
+      bool ok = active;
+      if (ok && cs.bynode < 1.0)
+        ok = b2_col_selected(cs.seed, cs.tree, B2_SCOPE_NODE(nid), f, cs.level_mask, cs.fwq, cs.n_features,
+                             b2_sample_count(cs.bynode, cs.n_level));
+      if (ok && cs.ic.sets_of) ok = b2_interaction_allowed(cs.ic, nid, f);
+      s_allowed[s] = ok;
+    }
+    __syncthreads();
+    active = active && s_allowed[s];
+  }
+  const int nf = active ? nbins[f] : 0;
+  const bool fmiss = active ? (has_missing[f] != 0) : false;
+  const long long* tot = vtot + (size_t)nid * T * 2;
+  double acc_l[kEvalBinsPerThread][2], acc_r[kEvalBinsPerThread][2];   // [bin][forward, backward]
+  bool nz_l[kEvalBinsPerThread][2], nz_r[kEvalBinsPerThread][2];
+#pragma unroll
+  for (int i = 0; i < kEvalBinsPerThread; ++i)
+#pragma unroll
+    for (int d = 0; d < 2; ++d) { acc_l[i][d] = 0.0; acc_r[i][d] = 0.0; nz_l[i][d] = false; nz_r[i][d] = false; }
+  bool any_missing = false;
+  for (int k = 0; k < T; ++k) {
+    const double inv_g = ldexp(1.0, qexp[2 * k] - qbits), inv_h = ldexp(1.0, qexp[2 * k + 1] - qbits);
+    const long long* hg = level_hist + (size_t)k * tstride + in_node;
+    const long long* hh = hg + (size_t)B2_BINS * sp;
+    long long g[kEvalBinsPerThread], h[kEvalBinsPerThread];
+#pragma unroll
+    for (int i = 0; i < kEvalBinsPerThread; ++i) {
+      const int b = b0 + i;
+      g[i] = 0; h[i] = 0;
+      if (b < nf) { g[i] = hg[b * sp]; h[i] = hh[b * sp]; }
+    }
+    long long tg = 0, th = 0;
+#pragma unroll
+    for (int i = 0; i < kEvalBinsPerThread; ++i) { tg += g[i]; th += h[i]; }
+    long long ig = tg, ih = th;
+#pragma unroll
+    for (int o = kEvalSlots; o < 32; o <<= 1) {
+      const long long ug = __shfl_up_sync(0xffffffffu, ig, o), uh = __shfl_up_sync(0xffffffffu, ih, o);
+      if (lane >= o) { ig += ug; ih += uh; }
+    }
+    __syncthreads();   // the previous target's carries are read
+    if (lane >= 32 - kEvalSlots) { s_wg[warp][s] = ig; s_wh[warp][s] = ih; }
+    __syncthreads();
+    if (threadIdx.x < kEvalSlots) {
+      long long cg = 0, ch = 0;
+      for (int w = 0; w < kEvalWarps; ++w) {
+        const long long a = s_wg[w][threadIdx.x], c = s_wh[w][threadIdx.x];
+        s_wg[w][threadIdx.x] = cg; s_wh[w][threadIdx.x] = ch;
+        cg += a; ch += c;
+      }
+      s_tg[threadIdx.x] = cg; s_th[threadIdx.x] = ch;
+    }
+    __syncthreads();
+    long long pg = s_wg[warp][s] + ig - tg, ph = s_wh[warp][s] + ih - th;
+    const long long real_g = s_tg[s], real_h = s_th[s];
+    const long long tot_g = tot[2 * k], tot_h = tot[2 * k + 1];
+    const double G = __dmul_rn(__ll2double_rn(tot_g), inv_g), H = __dmul_rn(__ll2double_rn(tot_h), inv_h);
+    any_missing = any_missing || (fmiss && (real_g != tot_g || real_h != tot_h));
+#pragma unroll
+    for (int i = 0; i < kEvalBinsPerThread; ++i) {
+      if (b0 + i >= nf) break;
+      const long long eg_excl = pg, eh_excl = ph;
+      pg += g[i]; ph += h[i];
+      {  // forward: left = prefix inclusive, missing -> right
+        const double lh_d = __dmul_rn(__ll2double_rn(ph), inv_h), rh_d = __dadd_rn(H, -lh_d);
+        const double lg_d = __dmul_rn(__ll2double_rn(pg), inv_g), rg_d = __dadd_rn(G, -lg_d);
+        acc_l[i][0] = __dadd_rn(acc_l[i][0], calc_gain(lg_d, lh_d, p));
+        acc_r[i][0] = __dadd_rn(acc_r[i][0], calc_gain(rg_d, rh_d, p));
+        nz_l[i][0] = nz_l[i][0] || ph != 0; nz_r[i][0] = nz_r[i][0] || (tot_h - ph) != 0;
+      }
+      {  // backward at bin b: right = real bins >= b, missing -> left
+        const long long rg_i = real_g - eg_excl, rh_i = real_h - eh_excl;
+        const double rh_d = __dmul_rn(__ll2double_rn(rh_i), inv_h), lh_d = __dadd_rn(H, -rh_d);
+        const double rg_d = __dmul_rn(__ll2double_rn(rg_i), inv_g), lg_d = __dadd_rn(G, -rg_d);
+        acc_l[i][1] = __dadd_rn(acc_l[i][1], calc_gain(lg_d, lh_d, p));
+        acc_r[i][1] = __dadd_rn(acc_r[i][1], calc_gain(rg_d, rh_d, p));
+        nz_l[i][1] = nz_l[i][1] || (tot_h - rh_i) != 0; nz_r[i][1] = nz_r[i][1] || rh_i != 0;
+      }
+    }
+  }
+  const double parent_gain = (double)vgain[nid];
+  Best best; best.key = 0; best.bin = 0; best.default_left = 0; best.lg = 0; best.lh = 0;
+#pragma unroll
+  for (int i = 0; i < kEvalBinsPerThread; ++i) {
+    const int b = b0 + i;
+    if (b >= nf) break;
+    consider(best, __double2float_rn(__dadd_rn(__dadd_rn(acc_l[i][0], acc_r[i][0]), -parent_gain)), (uint32_t)f * 1024u + (uint32_t)b,
+             b, 0, nz_l[i][0] ? 1 : 0, nz_r[i][0] ? 1 : 0);
+    if (any_missing)
+      consider(best, __double2float_rn(__dadd_rn(__dadd_rn(acc_l[i][1], acc_r[i][1]), -parent_gain)),
+               (uint32_t)f * 1024u + 512u + (uint32_t)(255 - b), b - 1, 1, nz_l[i][1] ? 1 : 0, nz_r[i][1] ? 1 : 0);
+  }
+  unsigned long long key = best.key;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long other = __shfl_xor_sync(0xffffffffu, key, o);
+    key = other > key ? other : key;
+  }
+  if (lane == 0) s_key[warp] = key;
+  __syncthreads();
+  unsigned long long kmax = 0;
+#pragma unroll
+  for (int i = 0; i < kEvalWarps; ++i) kmax = s_key[i] > kmax ? s_key[i] : kmax;
+  write_candidate(cands + (size_t)node * cand_stride + cta_in_node, kmax, best, f);
+}
+
+// the root's per-target totals (all 256 bins of slot 0 / group 0 of target k) and its gain
+__global__ void __launch_bounds__(256)
+vector_root_totals_kernel(const long long* __restrict__ level_hist, size_t tstride, int T, int n_groups,
+                          const int32_t* __restrict__ qexp, int qbits, B2TrainParamDev p, long long* __restrict__ vtot,
+                          float* __restrict__ vgain) {
+  __shared__ long long sg[256], sh[256];
+  const int sp = B2_GROUP_SLOTS;
+  for (int k = 0; k < T; ++k) {
+    const long long* hg = level_hist + (size_t)k * tstride;
+    sg[threadIdx.x] = hg[(size_t)threadIdx.x * sp];
+    sh[threadIdx.x] = hg[(size_t)(B2_BINS + threadIdx.x) * sp];
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+      if ((int)threadIdx.x < o) { sg[threadIdx.x] += sg[threadIdx.x + o]; sh[threadIdx.x] += sh[threadIdx.x + o]; }
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) { vtot[2 * k] = sg[0]; vtot[2 * k + 1] = sh[0]; }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) vgain[0] = __double2float_rn(vector_gain(vtot, T, qexp, qbits, p));
+}
+
+// After decide: the per-target totals of the children of split j (one CTA each), from the parent's histogram in the
+// level buffer -- left = the chosen feature's bins 0..split_bin, plus its missing rows (totals minus real bins) when
+// default_left; right = parent - left -- and each child's gain.  ev_nxt's sums get target 0's totals, which pick the
+// child whose histogram is built (level_finalize.cuh).
+__global__ void __launch_bounds__(256)
+vector_child_totals_kernel(const long long* __restrict__ level_hist, size_t tstride, int T, int n_groups,
+                           const B2LevelCtl* __restrict__ ctl, const B2SplitWork* __restrict__ split_work,
+                           const int32_t* __restrict__ pair_parent_hist, const B2NodeSeg* __restrict__ seg_nxt,
+                           const int32_t* __restrict__ tree_parent, const int32_t* __restrict__ feat_byte,
+                           const int32_t* __restrict__ nbins, const int32_t* __restrict__ qexp, int qbits, B2TrainParamDev p,
+                           long long* __restrict__ vtot, float* __restrict__ vgain, B2EvalNode* __restrict__ ev_nxt) {
+  const int j = blockIdx.x;
+  if (j >= ctl->n_split) return;
+  const int sp = B2_GROUP_SLOTS;
+  const size_t slice_elems = (size_t)n_groups * 2 * B2_BINS * sp;
+  const B2SplitWork w = split_work[j];
+  const int l = seg_nxt[2 * j].nid, r = l + 1, par = tree_parent[l];
+  const int fb = feat_byte[w.feature], nf = nbins[w.feature];
+  const size_t off = (size_t)pair_parent_hist[j] * slice_elems + (size_t)((fb >> 5) * 2) * B2_BINS * sp + (fb & 31);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int k = warp; k < T; k += blockDim.x / 32) {
+    const long long* hg = level_hist + (size_t)k * tstride + off;
+    const long long* hh = hg + (size_t)B2_BINS * sp;
+    long long pg = 0, ph = 0, rg = 0, rh = 0;
+    for (int b = lane; b < B2_BINS; b += 32) {
+      if (b >= nf) break;
+      const long long a = hg[b * sp], c = hh[b * sp];
+      rg += a; rh += c;
+      if (b <= w.split_bin) { pg += a; ph += c; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      pg += __shfl_xor_sync(0xffffffffu, pg, o); ph += __shfl_xor_sync(0xffffffffu, ph, o);
+      rg += __shfl_xor_sync(0xffffffffu, rg, o); rh += __shfl_xor_sync(0xffffffffu, rh, o);
+    }
+    if (lane == 0) {
+      const long long tg = vtot[((size_t)par * T + k) * 2], th = vtot[((size_t)par * T + k) * 2 + 1];
+      if (w.default_left) { pg += tg - rg; ph += th - rh; }
+      vtot[((size_t)l * T + k) * 2] = pg; vtot[((size_t)l * T + k) * 2 + 1] = ph;
+      vtot[((size_t)r * T + k) * 2] = tg - pg; vtot[((size_t)r * T + k) * 2 + 1] = th - ph;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < 2) {
+    const int c = threadIdx.x == 0 ? l : r;
+    const long long* t = vtot + (size_t)c * T * 2;
+    vgain[c] = __double2float_rn(vector_gain(t, T, qexp, qbits, p));
+    ev_nxt[2 * j + threadIdx.x].sum_g = t[0]; ev_nxt[2 * j + threadIdx.x].sum_h = t[1];
+  }
+}
+
 }  // namespace b2
 
 extern "C" {
+int b2_launch_eval_splits_vector(const long long* level_hist, size_t tstride, int T, int n_groups, const B2EvalNode* nodes,
+                                 int max_nodes, const long long* vtot, const float* vgain, const int32_t* group_first,
+                                 const int32_t* group_size, const int32_t* nbins, const uint8_t* has_missing,
+                                 const int32_t* qexp, int qbits, B2TrainParamDev p, B2SplitCand* cands, int cand_stride,
+                                 const B2LevelCtl* ctl, B2ColSample cs, const B2NodeSeg* seg, cudaStream_t stream) {
+  if (max_nodes <= 0) return 0;
+  const int cpn = b2::eval_ctas_per_node(n_groups, B2_GROUP_SLOTS, b2::kEvalSlots);
+  b2::eval_splits_vector_kernel<<<max_nodes * cpn, b2::kEvalThreads, 0, stream>>>(level_hist, tstride, T, n_groups, nodes, vtot, vgain,
+                                                                                 group_first, group_size, nbins, has_missing, qexp,
+                                                                                 qbits, p, cands, cand_stride, ctl, cs, seg);
+  return (int)cudaGetLastError();
+}
+// candidates per node of the vector scan (the narrow layout at every level)
+int b2_eval_vector_ctas_per_node(int n_groups) { return b2::eval_ctas_per_node(n_groups, B2_GROUP_SLOTS, b2::kEvalSlots); }
+int b2_launch_vector_root_totals(const long long* level_hist, size_t tstride, int T, int n_groups, const int32_t* qexp, int qbits,
+                                 B2TrainParamDev p, long long* vtot, float* vgain, cudaStream_t stream) {
+  b2::vector_root_totals_kernel<<<1, 256, 0, stream>>>(level_hist, tstride, T, n_groups, qexp, qbits, p, vtot, vgain);
+  return (int)cudaGetLastError();
+}
+int b2_launch_vector_child_totals(const long long* level_hist, size_t tstride, int T, int n_groups, int max_splits,
+                                  const B2LevelCtl* ctl, const B2SplitWork* split_work, const int32_t* pair_parent_hist,
+                                  const B2NodeSeg* seg_nxt, const int32_t* tree_parent, const int32_t* feat_byte,
+                                  const int32_t* nbins, const int32_t* qexp, int qbits, B2TrainParamDev p, long long* vtot,
+                                  float* vgain, B2EvalNode* ev_nxt, cudaStream_t stream) {
+  if (max_splits <= 0) return 0;
+  b2::vector_child_totals_kernel<<<max_splits, 256, 0, stream>>>(level_hist, tstride, T, n_groups, ctl, split_work, pair_parent_hist,
+                                                                 seg_nxt, tree_parent, feat_byte, nbins, qexp, qbits, p, vtot,
+                                                                 vgain, ev_nxt);
+  return (int)cudaGetLastError();
+}
 // candidates per node written by the scan of a level of max_nodes nodes (the layout depends on the node count)
 int b2_eval_ctas_per_node(int n_groups, int log2_shards, int max_nodes) {
   return b2::eval_ctas_per_node(n_groups, B2_GROUP_SLOTS >> log2_shards, max_nodes <= b2::kNarrowMaxNodes ? b2::kEvalSlots : 32);

@@ -87,6 +87,8 @@ ABI = {
     "B2_BoosterAddTree": (C.c_int, [_H, C.c_int32, _IP, _IP, _IP, _IP, _IP, _FP, _BP, _FP, _FP, _FP, _DP]),
     "B2_BoosterGetTreeCategories": (C.c_int, [_H, C.c_int32, _BP, C.POINTER(C.c_uint32)]),
     "B2_BoosterSetTreeCategories": (C.c_int, [_H, C.c_int32, _BP, C.POINTER(C.c_uint32)]),
+    "B2_BoosterGetTreeLeafVector": (C.c_int, [_H, C.c_int32, _FP, C.c_int64]),
+    "B2_BoosterSetTreeLeafVector": (C.c_int, [_H, C.c_int32, _FP, C.c_int64]),
     "B2_BoosterGetTreeWeights": (C.c_int, [_H, _FP, C.c_int64]),
     "B2_BoosterSetTreeWeights": (C.c_int, [_H, _FP, C.c_int64]),
     "B2_BoosterGetTimers": (C.c_int, [_H, C.c_int32, C.c_char_p, C.c_int64]),
@@ -643,7 +645,9 @@ _ENGINE_KEYS = ("objective", "num_class", "max_depth", "eta", "learning_rate", "
                 "random_state", "num_parallel_tree", "huber_slope", "tweedie_variance_power", "aft_loss_distribution",
                 "aft_loss_distribution_scale", "lambdarank_pair_method", "lambdarank_num_pair_per_sample",
                 "lambdarank_unbiased", "ndcg_exp_gain", "booster", "rate_drop", "skip_drop", "sample_type",
-                "normalize_type", "one_drop", "quantile_alpha", "num_target")
+                "normalize_type", "one_drop", "quantile_alpha", "num_target", "multi_strategy")
+# multi_strategy: one tree per target and round (xgboost's default), or one vector-leaf tree per round (DESIGN.md 2 item 19)
+_MULTI_STRATEGIES = ("one_output_per_tree", "multi_output_tree")
 # booster=dart's parameters with xgboost's defaults (save_config's dart_train_param)
 _DART_DEFAULTS = {"rate_drop": 0.0, "skip_drop": 0.0, "sample_type": "uniform", "normalize_type": "tree", "one_drop": 0}
 
@@ -652,7 +656,7 @@ _DART_DEFAULTS = {"rate_drop": 0.0, "skip_drop": 0.0, "sample_type": "uniform", 
 _UNSUPPORTED_NEUTRAL = {
     "sampling_method": ("uniform",), "max_leaves": (0,), "grow_policy": ("depthwise",),
     "monotone_constraints": (None, "", "()", (), []),
-    "multi_strategy": ("one_output_per_tree",), "refresh_leaf": (1, True), "process_type": ("default",),
+    "refresh_leaf": (1, True), "process_type": ("default",),
     "updater": (None, "grow_quantile_histmaker", "grow_gpu_hist"),
 }
 
@@ -672,8 +676,30 @@ def _check_quantile(params):
         raise XGBoostError("reg:quantileerror needs num_parallel_tree = 1 (got %r)" % (params["num_parallel_tree"],))
 
 
+def _check_multi_strategy(params):
+    """multi_strategy names one of the two strategies; vector-leaf trees refuse what they do not cover yet, naming both
+    sides (the engine checks the label width, categorical features and the communicator)."""
+    ms = params.get("multi_strategy")
+    if ms is None:
+        return
+    if ms not in _MULTI_STRATEGIES:
+        raise XGBoostError("multi_strategy=%r is not supported (supported: %s)" % (ms, ", ".join(_MULTI_STRATEGIES)))
+    if ms != "multi_output_tree":
+        return
+    obj = params.get("objective") or "reg:squarederror"
+    if obj.startswith("multi:"):
+        raise XGBoostError("multi_strategy='multi_output_tree' is not supported with objective=%r: vector-leaf trees take "
+                           "the multi-target objectives" % (obj,))
+    if (params.get("booster") or "gbtree") == "dart":
+        raise XGBoostError("multi_strategy='multi_output_tree' is not supported with booster='dart'")
+    if int(params.get("num_parallel_tree", 1) or 1) > 1:
+        raise XGBoostError("multi_strategy='multi_output_tree' needs num_parallel_tree = 1 (got %r)"
+                           % (params["num_parallel_tree"],))
+
+
 def _check_supported(params):
     _check_quantile(params)
+    _check_multi_strategy(params)
     mb = params.get("max_bin")
     if mb is not None and not 2 <= int(mb) <= 256:
         raise XGBoostError("parameter max_bin=%r is not supported by the H100 hist engine: the bin matrix is uint8, "
@@ -841,6 +867,16 @@ class Booster:
                 _check(lib().B2_BoosterSetTreeCategories(
                     self.handle, nt.value - 1, _bp(np.ascontiguousarray(st, np.uint8)),
                     np.ascontiguousarray(t["cat_bits"], np.uint32).ctypes.data_as(C.POINTER(C.c_uint32))))
+            if t.get("leaf_vector") is not None or self.is_vector_leaf:
+                # the engine refuses a vector where it grows single-output trees, and a tree without one where it
+                # grows vector-leaf trees: a model keeps its multi_strategy
+                if t.get("leaf_vector") is None:
+                    raise XGBoostError("multi_strategy='multi_output_tree' cannot continue a model of single-output trees "
+                                       "(multi_strategy='one_output_per_tree')")
+                nt = C.c_int32(0)
+                _check(lib().B2_BoosterNumTrees(self.handle, C.byref(nt)))
+                v = _f32c(np.asarray(t["leaf_vector"]).reshape(-1))
+                _check(lib().B2_BoosterSetTreeLeafVector(self.handle, nt.value - 1, _fp(v), v.size))
         if self.is_dart and trees and weights is not None:
             w = _f32c(weights)
             if w.size != len(trees):
@@ -886,6 +922,15 @@ class Booster:
     def is_dart(self):
         return (self.params.get("booster") or "gbtree") == "dart"
 
+    @property
+    def is_vector_leaf(self):
+        """One vector-leaf tree per round for all targets (multi_strategy='multi_output_tree' with T > 1)."""
+        return self.params.get("multi_strategy") == "multi_output_tree" and self._num_target() > 1
+
+    @property
+    def _trees_per_round(self):
+        return 1 if self.is_vector_leaf else self.num_class * self.num_parallel_tree
+
     def get_tree_weights(self):
         """Per-tree weights (float32, model order): DART's weight_drop; 1 for every gbtree tree."""
         if self.handle:
@@ -902,7 +947,7 @@ class Booster:
         return max(1, int(self.params.get("num_parallel_tree", 1) or 1))
 
     def num_boosted_rounds(self):
-        return self.num_trees() // max(1, self.num_class * self.num_parallel_tree)
+        return self.num_trees() // max(1, self._trees_per_round)
 
     def num_features(self):
         return self.n_features
@@ -923,6 +968,10 @@ class Booster:
                                        _ip(t["split_feature"]), _ip(t["split_bin"]), _fp(t["split_cond"]),
                                        _bp(t["default_left"]), _fp(t["value"]), _fp(t["base_weight"]),
                                        _fp(t["loss_chg"]), t["sum_hess"].ctypes.data_as(_DP)))
+        if self.is_vector_leaf:
+            v = np.zeros((n, self._num_target()), np.float32)
+            _check(lib().B2_BoosterGetTreeLeafVector(self.handle, i, _fp(v), v.size))
+            t["leaf_vector"] = v
         return t
 
     def get_trees(self):
@@ -997,7 +1046,7 @@ class Booster:
     # -- prediction
     def _tree_range(self, iteration_range, ntree_limit):
         """(first tree, end tree) of an iteration_range / ntree_limit; end 0 = all trees."""
-        per_round = self.num_class * self.num_parallel_tree
+        per_round = self._trees_per_round
         tb, te = iteration_range if iteration_range else (0, 0)
         if ntree_limit:
             return 0, int(ntree_limit)
@@ -1030,7 +1079,7 @@ class Booster:
         else:
             data._ensure_raw()
             tb, te = iteration_range if iteration_range else (0, 0)
-            tb_t, te_trees = tb * K * self.num_parallel_tree, te * K * self.num_parallel_tree
+            tb_t, te_trees = tb * self._trees_per_round, te * self._trees_per_round
             if ntree_limit:
                 tb_t, te_trees = 0, ntree_limit
             _check(lib().B2_BoosterPredict(self.handle, data.handle, 1 if output_margin else 0, tb_t, te_trees,
@@ -1061,6 +1110,8 @@ class Booster:
         out = np.zeros((n, max(te - tb, 0)), np.float32)
         _check(lib().B2_BoosterPredictLeaf(self.handle, data.handle, tb, te, _fp(out), out.size))
         if strict_shape:
+            if self.is_vector_leaf:   # one tree per round for all outputs
+                return out.reshape(n, -1, 1, 1)
             return out.reshape(n, -1, self.num_class, self.num_parallel_tree)
         return out
 
@@ -1110,8 +1161,12 @@ class Booster:
         exact = [[int(nid), str(float(cond[nid]))] for nid in np.nonzero(numeric & ~np.isfinite(cond))[0]]
         cond = np.where(numeric & ~np.isnan(cond), np.clip(cond, -_FLT_MAX, _FLT_MAX), cond)
         cond = np.where(np.isfinite(cond), cond, np.float32(0.0))
+        vec = t.get("leaf_vector")
+        if vec is not None:   # vector-leaf tree: node-major [n][T] base weights, a leaf's condition is 0
+            vec = np.asarray(vec, np.float32)
+            cond = np.where(leaf, np.float32(0.0), cond)
         return exact, {
-            "base_weights": [float(x) for x in t["base_weight"]],
+            "base_weights": [float(x) for x in (t["base_weight"] if vec is None else vec.reshape(-1))],
             "categories": cats, "categories_nodes": cat_nodes, "categories_segments": cat_segs,
             "categories_sizes": cat_sizes,
             "default_left": [int(x) for x in t["default_left"]],
@@ -1125,7 +1180,7 @@ class Booster:
             "split_type": [int(x) for x in st],
             "sum_hessian": [float(x) for x in t["sum_hess"]],
             "tree_param": {"num_deleted": "0", "num_feature": str(n_features), "num_nodes": str(n),
-                           "size_leaf_vector": "1"},
+                           "size_leaf_vector": "1" if vec is None else str(vec.shape[1])},
         }
 
     def _model_dict(self):
@@ -1160,8 +1215,8 @@ class Booster:
             attrs["b2.split_conds"] = json.dumps(exact, separators=(",", ":"))
         gbtree = {"model": {
             "gbtree_model_param": {"num_parallel_tree": str(self.num_parallel_tree), "num_trees": str(len(trees))},
-            "iteration_indptr": list(range(0, len(trees) + 1, K * self.num_parallel_tree)),
-            "tree_info": [(i // self.num_parallel_tree) % K for i in range(len(trees))],
+            "iteration_indptr": list(range(0, len(trees) + 1, self._trees_per_round)),
+            "tree_info": [0 if self.is_vector_leaf else (i // self.num_parallel_tree) % K for i in range(len(trees))],
             "trees": trees}, "name": "gbtree"}
         if self.is_dart:   # xgboost's Dart::SaveModel: the gbtree block plus one weight per tree
             gbtree = {"name": "dart", "gbtree": gbtree,
@@ -1237,6 +1292,18 @@ class Booster:
             params["num_target"] = nt
         else:
             params.pop("num_target", None)
+        vsizes = {int(t.get("tree_param", {}).get("size_leaf_vector", "1")) for t in gb["model"]["trees"]}
+        vsizes = {1 if v == 0 else v for v in vsizes}
+        if len(vsizes) > 1:
+            raise XGBoostError("model mixes leaf vector sizes %s: a model keeps one multi_strategy" % sorted(vsizes))
+        if vsizes and max(vsizes) > 1:   # vector-leaf trees, one per round
+            if max(vsizes) != nt:
+                raise XGBoostError("model has leaf vectors of size %d for %d targets" % (max(vsizes), nt))
+            params["multi_strategy"] = "multi_output_tree"
+        elif params.get("multi_strategy") == "multi_output_tree" and gb["model"]["trees"] and nt > 1:
+            # single-output trees for several targets: the model was grown one tree per target (with T = 1 the
+            # strategy is ignored and the recorded parameter is kept)
+            params["multi_strategy"] = "one_output_per_tree"
         self.params = params
         self.n_features = int(L["learner_model_param"]["num_feature"])
         self.feature_names = L.get("feature_names") or None
@@ -1268,15 +1335,22 @@ class Booster:
                 cond[nid] = np.float32(b_) if b_ >= 0 else np.float32("nan")
             for nid, v in exact_conds.get(ti, ()):
                 cond[nid] = v
+            bw = np.asarray(t["base_weights"], np.float32)
+            vec = None
+            if self.is_vector_leaf:   # node-major [n][T]; the scalar fields carry zeros
+                vec = bw.reshape(len(left), nt)
+                bw = np.zeros(len(left), np.float32)
+                sc = np.zeros(len(left), np.float32)
             self._trees.append(dict(
+                leaf_vector=vec,
                 split_type=st, cat_bits=bits,
                 left=left, right=np.asarray(t["right_children"], np.int32), parent=parent,
                 split_feature=np.where(leaf, -1, np.asarray(t["split_indices"], np.int32)).astype(np.int32),
                 split_bin=np.asarray(sb if sb is not None else [-1] * len(left), np.int32),
                 split_cond=cond,
                 default_left=np.asarray(t["default_left"], np.uint8),
-                value=np.where(leaf, sc, np.asarray(t["base_weights"], np.float32)).astype(np.float32),
-                base_weight=np.asarray(t["base_weights"], np.float32),
+                value=np.where(leaf, sc, bw).astype(np.float32),
+                base_weight=bw,
                 loss_chg=np.asarray(t["loss_changes"], np.float32),
                 sum_hess=np.asarray(t["sum_hessian"], np.float64)))
 
@@ -1321,6 +1395,8 @@ class Booster:
         if objective["name"] == "rank:map":
             objective[_LAMBDARANK[0]] = {k: _str_param(self.params.get(k, d)) for k, d in _LAMBDARANK[1].items()}
         return json.dumps({"learner": {"gradient_booster": gbtree,
+                                       "learner_train_param": {
+                                           "multi_strategy": self.params.get("multi_strategy") or "one_output_per_tree"},
                                        "objective": objective,
                                        "b2_params": {k: v for k, v in self.params.items() if _json_ok(v)}},
                            "version": [2, 0, 3]})
@@ -1423,7 +1499,8 @@ def _is_cat_node(t, nid):
 
 def _dump_json(t, nid, depth, names, with_stats):
     if t["split_feature"][nid] < 0:
-        d = {"nodeid": int(nid), "leaf": float(t["value"][nid])}
+        vec = t.get("leaf_vector")
+        d = {"nodeid": int(nid), "leaf": float(t["value"][nid]) if vec is None else [float(x) for x in vec[nid]]}
         if with_stats:
             d["cover"] = float(t["sum_hess"][nid])
         return d
@@ -1446,7 +1523,11 @@ def _dump_json(t, nid, depth, names, with_stats):
 def _dump_text(t, nid, depth, names, with_stats, lines):
     ind = "\t" * depth
     if t["split_feature"][nid] < 0:
-        s = "%s%d:leaf=%.9g" % (ind, nid, float(t["value"][nid]))
+        vec = t.get("leaf_vector")
+        if vec is None:
+            s = "%s%d:leaf=%.9g" % (ind, nid, float(t["value"][nid]))
+        else:   # vector-leaf tree: one value per target
+            s = "%s%d:leaf=[%s]" % (ind, nid, ",".join("%.9g" % float(x) for x in vec[nid]))
         if with_stats:
             s += ",cover=%.9g" % float(t["sum_hess"][nid])
         lines.append(s + "\n")
