@@ -121,6 +121,14 @@ int B2_BoosterCreate(const char* params, B2Handle train, B2Handle comm, B2Handle
 int B2_BoosterUpdateOneIter(B2Handle b, int32_t iter);
 /* custom objective (xgb.train(obj=...), tests/test_xgboost_api.py:77-102): grad/hess [n_rows*num_class] */
 int B2_BoosterBoostOneIter(B2Handle b, const float* grad, const float* hess, int64_t len);
+/* update mode (params process_type=update, updater=refresh, refresh_leaf; xgb.train(xgb_model=...) of xgboost's
+ * TreeRefresher): the trees added with B2_BoosterAddTree / B2_BoosterSetTreeCategories before the first round are the
+ * trees to update, and the model starts empty.  Call r (0-based) takes round r of them (num_class x num_parallel_tree
+ * trees), computes the gradients at the margin of base_score / base_margin plus the rounds already refreshed, re-fits
+ * every node's sum_hess, base_weight and loss_chg (and with refresh_leaf the leaf values) on the raw rows of the train
+ * matrix, and appends the refreshed trees.  grad / hess == NULL: the objective's gradients, else a custom objective's
+ * [n_rows*num_class].  Fails past the model's last round.  B2_BoosterUpdateOneIter / BoostOneIter fail in update mode. */
+int B2_BoosterRefreshOneIter(B2Handle b, const float* grad, const float* hess, int64_t len);
 /* diagnostic: the fp32 gradient pairs of the last round on the train matrix, class-major ([num_class][n_rows]),
  * as the trees of that round saw them (after the weight, before quantisation).  len = n_rows * num_class. */
 int B2_BoosterGetGradients(B2Handle b, float* grad, float* hess, int64_t len);
@@ -183,7 +191,8 @@ int B2_BoosterSetTreeLeafVector(B2Handle b, int32_t tree, const float* v, int64_
 int B2_BoosterGetTreeWeights(B2Handle b, float* out, int64_t len);
 int B2_BoosterSetTreeWeights(B2Handle b, const float* w, int64_t len);
 /* JSON object with accumulated device timings / counters of the hot path (since last reset):
- * hist_ms, hist_launches, hist_rows, hist_bytes, kernel_launches, round_ms, allreduce_bytes ... */
+ * hist_ms, hist_launches, hist_rows, hist_bytes, kernel_launches, round_ms, allreduce_bytes ..., and in update mode
+ * refresh_ms / refresh_launches: the time and count of refresh_kernel launches (B2_BoosterRefreshOneIter) */
 int B2_BoosterGetTimers(B2Handle b, int32_t reset, char* out, int64_t out_cap);
 int B2_BoosterCancel(B2Handle b);
 int B2_BoosterFree(B2Handle b);

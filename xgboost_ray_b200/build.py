@@ -30,6 +30,7 @@ SOURCES = {
     "shap_kernel.cu": [],                      # TreeSHAP contributions / interactions, leaf indices
     "dart_kernel.cu": ["--fmad=false"],        # DART margin rebuild, bit-exact vs the weighted predict and the reference
     "quantile_kernel.cu": ["--fmad=false"],    # quantile gradients, metric and leaf refresh, bit-exact vs the reference
+    "refresh_kernel.cu": ["--fmad=false"],     # refresh updater: leaf sums on raw rows, node statistics bottom-up
     "engine.cu": [],
 }
 

@@ -157,6 +157,10 @@ int b2_launch_weight_absmax(const float*, int64_t, uint32_t*, int, cudaStream_t)
 int b2_launch_weight_quantize(const float*, int64_t, int64_t, const uint32_t*, int32_t*, int, cudaStream_t);
 int b2_launch_bin(const float*, int64_t, int, float, const int32_t*, const float*, const int32_t*, const uint8_t*, int, uint8_t*,
                   uint8_t*, int64_t, int, cudaStream_t);
+int b2_launch_refresh(const float*, int64_t, int, float, const B2TreeNodeDev*, int, const uint32_t*, int, const float2*,
+                      const int32_t*, int, uint16_t*, long long*, int, cudaStream_t);
+int b2_launch_refresh_nodes(const B2TreeNodeDev*, int, const int32_t*, const int32_t*, int, const long long*, const int32_t*, int,
+                            B2CtlParams, int, long long*, unsigned char*, float*, cudaStream_t);
 }
 
 namespace {
@@ -837,6 +841,10 @@ struct Params {
   // multi_strategy: 0 one_output_per_tree (one tree per target and round), 1 multi_output_tree (one vector-leaf tree per
   // round for all targets, DESIGN.md 2 item 19; only with T > 1 targets, ignored otherwise)
   int multi_strategy = 0;
+  // process_type=update with updater=refresh (DESIGN.md 2 item 20): the rounds refresh the trees of an existing model
+  // instead of growing new ones; refresh_leaf = false keeps their leaf values
+  bool update_mode = false, refresh_leaf = true;
+  std::string updater;
   bool use_cols() const { return colsample_bytree < 1.0f || colsample_bylevel < 1.0f || colsample_bynode < 1.0f; }
   bool vector_leaf() const { return multi_strategy == 1 && num_target > 1; }
 };
@@ -867,6 +875,8 @@ struct Timers {
   double hist_ms = 0, round_ms = 0;
   double shap_ms = 0;   // kernel time of pred_contribs / pred_interactions (CUDA events around the SHAP kernels)
   long long shap_rows = 0;
+  double refresh_ms = 0;   // update mode: refresh_kernel time (CUDA events around every launch)
+  long long refresh_launches = 0;
   double phase_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // profile=2: quant, hist, allreduce, subtract, eval+decide, partition+finalize, leaf, other
   long long hist_launches = 0, hist_rows = 0, kernel_launches = 0, rounds = 0;
   double hist_bytes = 0, allreduce_bytes = 0;
@@ -961,6 +971,7 @@ struct Booster : HandleBase {
     std::map<int, TreeGraph> graphs;       // per class slot
     std::vector<cudaEvent_t> ev_pool; size_t ev_used = 0;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> hist_events;
+    std::vector<std::pair<cudaEvent_t, cudaEvent_t>> refresh_events;   // update mode: around every refresh_kernel
     std::vector<std::pair<int, cudaEvent_t>> phase_marks;   // (phase that ENDS at this event)
     cudaEvent_t start = nullptr, stop = nullptr;
     uint32_t* h_p2p_err = nullptr;         // pinned copy of the peer-memory error word, written at the end of the round
@@ -968,6 +979,9 @@ struct Booster : HandleBase {
     bool dart_dropped = false;             // the round changed weights of earlier trees
     void* vstaging = nullptr;              // vector-leaf tree: pinned copy of the round's d_vblock
     size_t vstaging_bytes = 0;
+    bool refresh = false;                  // update mode: the round refreshed the trees to_update[rsrc[slot]]
+    std::vector<void*> rstaging;           // pinned copies of their read-back blocks (refresh_nodes_kernel)
+    std::vector<int> rsrc;
   };
   RoundBuffers rb[2];
   int rb_cur = 0;                          // parity of the next round to enqueue
@@ -1041,6 +1055,15 @@ struct Booster : HandleBase {
   DevBuf<float> d_leaf_vec;
   DevBuf<uint8_t> d_vblock;
   DevBuf<float> d_leaf_table; std::vector<float> h_leaf_table;   // prediction: [model nodes][T]
+  // update mode (refresh_round): the trees added before the first round are moved out of the model into to_update, and
+  // their device copy is built once (nodes with the compact leaf index in pad, category sets, node ids by depth)
+  struct RefreshTree { int32_t node_off, n_nodes, n_leaves, order_off, level_off, n_levels; size_t block_bytes; };
+  std::vector<TreeHost> to_update;
+  std::vector<RefreshTree> rtrees;
+  bool update_started = false;
+  DevBuf<B2TreeNodeDev> d_rnodes; DevBuf<uint32_t> d_rcats; DevBuf<int32_t> d_rorder, d_rlevels;
+  DevBuf<long long> d_rsums, d_rlimbs; DevBuf<float> d_rleaf; DevBuf<uint8_t> d_rblock;
+  size_t rstaging_bytes = 0;               // bytes of every block in rb[].rstaging (the largest tree's)
   // profiling
   Timers t;
   ~Booster() {
@@ -1063,6 +1086,7 @@ struct Booster : HandleBase {
       for (void* h : r.staging) cudaFreeHost(h);
       if (r.h_p2p_err) cudaFreeHost(r.h_p2p_err);
       if (r.vstaging) cudaFreeHost(r.vstaging);
+      for (void* h : r.rstaging) cudaFreeHost(h);
     }
     for (auto& kv : eval_cache) delete kv.second;
     if (h_grad_err) cudaFreeHost(h_grad_err);
@@ -1093,6 +1117,11 @@ void resolve_events(Booster* b, Booster::RoundBuffers& R) {
     if (cudaEventElapsedTime(&ms, pr.first, pr.second) == cudaSuccess) b->t.hist_ms += ms;
   }
   R.hist_events.clear();
+  for (auto& pr : R.refresh_events) {
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, pr.first, pr.second) == cudaSuccess) b->t.refresh_ms += ms;
+  }
+  R.refresh_events.clear();
   R.ev_used = 0;
 }
 
@@ -1161,6 +1190,7 @@ void set_targets(Params* p, int T) {
     if (T > kMaxVectorTargets)
       fail("multi_strategy=multi_output_tree supports at most %d targets, the label has %d columns", kMaxVectorTargets, T);
     if (p->dart) fail("multi_strategy=multi_output_tree is not supported with booster=dart");
+    if (p->update_mode) fail("process_type=update is not supported with multi_strategy=multi_output_tree");
     if (p->num_parallel_tree > 1)
       fail("multi_strategy=multi_output_tree needs num_parallel_tree = 1, got %d", p->num_parallel_tree);
   }
@@ -1267,6 +1297,17 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     }
     else if (k == "rate_drop" || k == "skip_drop" || k == "sample_type" || k == "normalize_type" || k == "one_drop")
       dart_text[k] = v;   // checked below, and only for booster=dart (gbtree ignores them, like xgboost)
+    else if (k == "process_type") {
+      if (v == "default") p->update_mode = false;
+      else if (v == "update") p->update_mode = true;
+      else fail("process_type='%s' is not supported (supported: default, update)", v.c_str());
+    }
+    else if (k == "updater") p->updater = v;
+    else if (k == "refresh_leaf") {
+      if (v == "1" || v == "true" || v == "True") p->refresh_leaf = true;
+      else if (v == "0" || v == "false" || v == "False") p->refresh_leaf = false;
+      else fail("refresh_leaf must be 0 or 1, got '%s'", v.c_str());
+    }
     // unknown keys (nthread, tree_method, verbosity, ...) are accepted and ignored, like xgboost
   }
   if (p->dart) {
@@ -1304,6 +1345,21 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     fail("multi_strategy=multi_output_tree is not supported with objective '%s' (vector-leaf trees take the multi-target "
          "objectives: reg:squarederror, reg:squaredlogerror, reg:pseudohubererror, reg:logistic, binary:logistic, "
          "binary:logitraw)", p->objective_name.c_str());
+  // update mode (DESIGN.md 2 item 20): only the refresh updater, and only where a refreshed leaf is a Newton step
+  if (p->update_mode) {
+    if (p->updater != "refresh")
+      fail("process_type=update needs updater=refresh, got updater='%s' (prune and refresh,prune are not supported)",
+           p->updater.c_str());
+    if (p->dart) fail("process_type=update is not supported with booster=dart");
+    if (p->objective == kObjQuantile)
+      fail("process_type=update is not supported with reg:quantileerror: its leaf values are residual quantiles, which the "
+           "refresh updater does not recompute");
+  } else if (p->updater == "refresh") {
+    fail("updater=refresh needs process_type=update: it refreshes the trees of an existing model (xgb_model)");
+  } else if (!p->updater.empty() && p->updater != "grow_quantile_histmaker" && p->updater != "grow_gpu_hist") {
+    fail("updater='%s' is not supported (supported: grow_quantile_histmaker, grow_gpu_hist, and refresh with "
+         "process_type=update)", p->updater.c_str());
+  }
   if (p->num_target_set) set_targets(p, p->num_target);
   if (p->max_depth < 1 || p->max_depth > 14) fail("max_depth must be in [1, 14], got %d", p->max_depth);
   if (p->num_parallel_tree < 1 || p->num_parallel_tree > 4096) fail("num_parallel_tree must be in [1, 4096], got %d", p->num_parallel_tree);
@@ -2641,6 +2697,24 @@ void check_labels(Booster* b) {
   b->labels_checked = true;
 }
 
+// update mode: tree to_update[src] with the statistics of its refresh_nodes_kernel block.  Structure, splits, default
+// directions and categories are the old tree's; a leaf keeps its loss_chg (xgboost's refresher sets it on splits only).
+void materialize_refreshed(Booster* b, const void* block, int src) {
+  TreeHost t = b->to_update[src];
+  const int nn = t.size();
+  const double* sum_hess = (const double*)block;
+  const float* base_weight = (const float*)((const char*)block + (size_t)nn * 8);
+  const float* loss_chg = base_weight + nn;
+  const float* value = loss_chg + nn;
+  for (int i = 0; i < nn; ++i) {
+    t.sum_hess[i] = sum_hess[i];
+    t.base_weight[i] = base_weight[i];
+    t.value[i] = value[i];
+    if (t.feature[i] >= 0) t.loss_chg[i] = loss_chg[i];
+  }
+  b->trees.push_back(std::move(t));
+}
+
 // Finish an enqueued round: wait for its stop event, resolve its timers, raise a peer-memory or non-finite-gradient
 // error, and turn its read-back blocks into host trees.
 void finish_round(Booster* b, Booster::RoundBuffers& R, int n_trees, bool check_finite) {
@@ -2663,7 +2737,8 @@ void finish_round(Booster* b, Booster::RoundBuffers& R, int n_trees, bool check_
          b->p.objective_name.c_str());
   }
   for (int slot = 0; slot < n_trees; ++slot) {
-    if (b->p.vector_leaf()) materialize_vector_tree(b, R.staging[slot], R.vstaging);
+    if (R.refresh) materialize_refreshed(b, R.rstaging[slot], R.rsrc[slot]);
+    else if (b->p.vector_leaf()) materialize_vector_tree(b, R.staging[slot], R.vstaging);
     else materialize_tree(b, R.staging[slot]);
   }
   if (b->p.dart) {   // the weights are committed with the trees
@@ -2679,6 +2754,78 @@ void drain_round(Booster* b) {
   if (n_trees == 0) return;
   b->pending_trees = 0;
   finish_round(b, b->rb[b->rb_cur ^ 1], n_trees, b->pending_check_finite);
+}
+
+// Update mode, before anything reads the train margin: the trees added so far become the trees to update and the model
+// starts empty (xgboost's gbtree moves them to trees_to_update).  Every tree is checked to be a proper binary tree
+// reachable from node 0 with at most 65,535 leaves, and copied to the device once: B2TreeNodeDev nodes whose pad holds
+// the compact leaf index (leaves numbered in node order), the category sets, and the node ids grouped by depth.
+void begin_update(Booster* b) {
+  if (!b->p.update_mode || b->update_started) return;
+  drain_round(b);
+  b->update_started = true;
+  b->to_update = std::move(b->trees);
+  b->trees.clear();
+  b->d_trees_synced = -1; b->paths_synced = -1; b->margin_ready = false;
+  for (auto& kv : b->eval_cache) if (kv.second) kv.second->n_trees_applied = 0, kv.second->n = -1;
+  std::vector<B2TreeNodeDev> nodes; std::vector<uint32_t> cats; std::vector<int32_t> order, levels;
+  size_t max_leaves = 1, max_nodes = 1, max_block = 8;
+  b->rtrees.clear();
+  for (size_t ti = 0; ti < b->to_update.size(); ++ti) {
+    const TreeHost& t = b->to_update[ti];
+    const int nn = t.size();
+    Booster::RefreshTree rt;
+    rt.node_off = (int32_t)nodes.size(); rt.n_nodes = nn; rt.level_off = (int32_t)levels.size();
+    rt.order_off = (int32_t)order.size();
+    std::vector<int32_t> leaf_of(nn, -1), depth(nn, -1);
+    int n_leaves = 0;
+    for (int i = 0; i < nn; ++i) if (t.feature[i] < 0) leaf_of[i] = n_leaves++;
+    if (n_leaves > 65535) fail("tree %zu has %d leaves; the refresh updater supports at most 65535", ti, n_leaves);
+    // breadth-first from the root: every node reached exactly once, splits with two children, leaves with none
+    std::vector<int32_t> bfs{0}; depth[0] = 0;
+    for (size_t q = 0; q < bfs.size(); ++q) {
+      const int i = bfs[q];
+      if (t.feature[i] < 0) continue;
+      for (int c : {t.left[i], t.right[i]}) {
+        if (c < 0 || c >= nn || depth[c] >= 0)
+          fail("tree %zu is not a binary tree: node %d has child %d (%d nodes)", ti, i, c, nn);
+        depth[c] = depth[i] + 1;
+        bfs.push_back(c);
+      }
+    }
+    if ((int)bfs.size() != nn) fail("tree %zu has %d nodes that the root does not reach", ti, nn - (int)bfs.size());
+    const int n_levels = depth[bfs.back()] + 1;   // BFS order is by depth
+    rt.n_leaves = n_leaves; rt.n_levels = n_levels;
+    int d = -1;
+    for (size_t q = 0; q < bfs.size(); ++q)
+      while (d < depth[bfs[q]]) { levels.push_back((int32_t)(order.size() + q)); ++d; }
+    levels.push_back((int32_t)(order.size() + bfs.size()));
+    order.insert(order.end(), bfs.begin(), bfs.end());
+    for (int i = 0; i < nn; ++i) {
+      int32_t cat_slot = -1;
+      if (t.feature[i] >= 0 && t.split_type[i]) {
+        cat_slot = (int32_t)(cats.size() / 8);
+        cats.insert(cats.end(), t.cat_bits.begin() + (size_t)i * 8, t.cat_bits.begin() + (size_t)i * 8 + 8);
+      }
+      nodes.push_back(B2TreeNodeDev{t.left[i], t.right[i], t.feature[i], t.cond[i], t.value[i], (int32_t)t.default_left[i],
+                                    cat_slot, leaf_of[i]});
+    }
+    rt.block_bytes = (size_t)nn * (8 + 3 * 4);
+    max_leaves = std::max(max_leaves, (size_t)n_leaves); max_nodes = std::max(max_nodes, (size_t)nn);
+    max_block = std::max(max_block, rt.block_bytes);
+    b->rtrees.push_back(rt);
+  }
+  // node ids are relative to the tree, level pointers relative to the tree's segment of the order table
+  for (const Booster::RefreshTree& rt : b->rtrees)
+    for (int l = 0; l <= rt.n_levels; ++l) levels[rt.level_off + l] -= rt.order_off;
+  cudaStream_t s = b->ctx->stream;
+  upload(b->d_rnodes, nodes, s); upload(b->d_rorder, order, s); upload(b->d_rlevels, levels, s);
+  if (cats.empty()) cats.assign(8, 0u);
+  upload(b->d_rcats, cats, s);
+  b->d_rsums.ensure(4 * max_leaves); b->d_rlimbs.ensure(4 * max_nodes); b->d_rleaf.ensure(max_leaves);
+  b->d_rblock.ensure(max_block);
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  b->rstaging_bytes = max_block;
 }
 
 // DART walks the train matrix's bins: every numeric split of a tree must name the bin whose cut is its condition (trees
@@ -2727,6 +2874,7 @@ void predict_trees(Booster* b, Matrix* m, int tree_begin, int tree_end, float* o
 }
 
 void ensure_train_margin(Booster* b) {
+  begin_update(b);
   if (b->margin_ready) return;
   drain_round(b);   // the margin is rebuilt from every tree of the model
   Matrix* m = b->train;
@@ -2818,6 +2966,48 @@ void dart_prepare(Booster* b) {
   dn.r = r;
 }
 
+// Update mode: refresh tree to_update[src] (class k) from gh[k] on the raw train rows, update margin[:, k] with its
+// leaf values and copy its statistics into pinned block `slot` (materialize_refreshed, when the round is drained).
+// Every row counts (no row or column sampling); the leaf sums are the only exchange between the ranks.
+void refresh_tree(Booster* b, int k, int slot, int src) {
+  Matrix* m = b->train; Ctx* ctx = b->ctx; cudaStream_t s = ctx->stream; const Params& p = b->p;
+  const int64_t n = m->n;
+  const Booster::RefreshTree& rt = b->rtrees[src];
+  const float2* gh = b->gh.p + (size_t)k * n;
+  uint32_t* d_absmax = b->d_absmax.p + 2 * k;
+  b->pos.ensure((size_t)std::max<int64_t>(n, 1));
+  Booster::RoundBuffers& R = b->rb[b->rb_cur];
+  while ((int)R.rstaging.size() <= slot) {
+    void* h = nullptr; CUDA_CHECK(cudaMallocHost(&h, b->rstaging_bytes)); R.rstaging.push_back(h);
+  }
+  if (!b->absmax_fused) {
+    CUDA_CHECK(cudaMemsetAsync(d_absmax, 0, 2 * sizeof(uint32_t), s));
+    LAUNCH_CHECK(b2_launch_absmax(gh, n, d_absmax, ctx->num_sms, s));
+    b->t.kernel_launches++;
+  }
+  allreduce(b->comm, d_absmax, 2, kNcclUint32, kNcclMax, s);
+  LAUNCH_CHECK(b2_launch_quant_exponent(d_absmax, b->d_qexp.p, s));
+  CUDA_CHECK(cudaMemsetAsync(b->d_rsums.p, 0, 4 * (size_t)rt.n_leaves * sizeof(long long), s));
+  const B2TreeNodeDev* nodes = b->d_rnodes.p + rt.node_off;
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  if (p.profile) { e0 = get_event(b); e1 = get_event(b); CUDA_CHECK(cudaEventRecord(e0, s)); }
+  LAUNCH_CHECK(b2_launch_refresh(m->raw.p, n, m->F, m->missing, nodes, rt.n_nodes, b->d_rcats.p, rt.n_leaves, gh, b->d_qexp.p, 40,
+                                 b->pos.p, b->d_rsums.p, ctx->num_sms, s));
+  if (p.profile) { CUDA_CHECK(cudaEventRecord(e1, s)); R.refresh_events.push_back({e0, e1}); }
+  b->t.refresh_launches++;
+  allreduce(b->comm, b->d_rsums.p, 4 * (size_t)rt.n_leaves, kNcclInt64, kNcclSum, s);   // limb by limb: exact
+  if (b->comm && b->comm->world > 1) b->t.allreduce_bytes += 4.0 * rt.n_leaves * 8;
+  B2CtlParams cp;
+  cp.mcw = (double)p.min_child_weight; cp.lambda = (double)p.lambda; cp.alpha = (double)p.alpha;
+  cp.max_delta_step = (double)p.max_delta_step; cp.gamma = p.gamma; cp.eta = p.eta / (float)p.num_parallel_tree;
+  LAUNCH_CHECK(b2_launch_refresh_nodes(nodes, rt.n_nodes, b->d_rorder.p + rt.order_off, b->d_rlevels.p + rt.level_off, rt.n_levels,
+                                       b->d_rsums.p, b->d_qexp.p, 40, cp, p.refresh_leaf ? 1 : 0, b->d_rlimbs.p, b->d_rblock.p,
+                                       b->d_rleaf.p, s));
+  LAUNCH_CHECK(b2_launch_margin_update(b->margin.p, p.num_class, k, b->pos.p, b->d_rleaf.p, nullptr, n, ctx->num_sms, s));
+  CUDA_CHECK(cudaMemcpyAsync(R.rstaging[slot], b->d_rblock.p, rt.block_bytes, cudaMemcpyDeviceToHost, s));
+  b->t.kernel_launches += 4;
+}
+
 // One boosting round, pipelined with the previous one: round r+1 (gradients, then its class trees) is enqueued first,
 // round r is drained while the device works on r+1, and r+1 is left pending.  Nothing of r+1 needs the host: the margin
 // it reads was updated on the device by r's margin_update_kernel, in stream order.  A round whose gradient kernel checks
@@ -2828,10 +3018,26 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
   if (b->cancel.load()) { drain_round(b); fail("training cancelled"); }
   Booster::RoundBuffers& R = b->rb[b->rb_cur];   // not pending: the pending round (if any) is in the other set
-  R.hist_events.clear(); R.phase_marks.clear(); R.ev_used = 0;   // left over from a round that failed while enqueuing
+  R.hist_events.clear(); R.refresh_events.clear(); R.phase_marks.clear(); R.ev_used = 0;   // left over from a round that failed while enqueuing
   if (!R.start) { CUDA_CHECK(cudaEventCreate(&R.start)); CUDA_CHECK(cudaEventCreate(&R.stop)); }
   if (b->p.profile) CUDA_CHECK(cudaEventRecord(R.start, s));
   ensure_train_margin(b);
+  // update mode: round r refreshes the r-th round of the model's trees (refresh_tree) instead of growing new ones
+  const bool refresh = b->p.update_mode;
+  int refresh_round_index = 0;
+  if (refresh) {
+    const int per_round = K * b->p.num_parallel_tree;
+    const int64_t have = (int64_t)b->to_update.size();
+    if (have == 0) fail("process_type=update needs the trees of an existing model (xgb_model); this booster has none");
+    if (have % per_round != 0)
+      fail("the model to update has %lld trees, not a whole number of rounds of %d trees", (long long)have, per_round);
+    if (!m->has_raw) fail("process_type=update needs the raw data of the train matrix (B2_MatrixEnsureRaw)");
+    refresh_round_index = (int)(((int64_t)b->trees.size() + b->pending_trees) / per_round);
+    if (refresh_round_index >= have / per_round)
+      fail("the model to update has %lld rounds; process_type=update cannot refresh round %d (num_boost_round must be at "
+           "most %lld)", (long long)(have / per_round), refresh_round_index + 1, (long long)(have / per_round));
+  }
+  R.refresh = refresh;
   // DART: the gradients are taken at the drop margin; the round's trees are added to the full-margin prefix
   const float* gm = b->margin.p;
   if (b->p.dart) {
@@ -2860,7 +3066,7 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
   } else {
     if (b->p.objective != kObjAft) check_train_labels(b);
     // the |g|,|h| maxima of every class tree come out of the same pass unless rows are dropped afterwards (subsample)
-    b->absmax_fused = b->p.subsample >= 1.0f && K <= b2_gradient_fused_max_classes();
+    b->absmax_fused = (b->p.subsample >= 1.0f || refresh) && K <= b2_gradient_fused_max_classes();
     if (b->absmax_fused) CUDA_CHECK(cudaMemsetAsync(b->d_absmax.p, 0, 2 * (size_t)K * sizeof(uint32_t), s));
     check_finite = obj_checks_finite(b->p.objective);
     if (check_finite) {
@@ -2893,13 +3099,19 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
   const int npt = b->p.num_parallel_tree;
   // row sampling zeroes the dropped rows' gradient pairs in place: the parallel trees of a round each sample from the
   // round's ORIGINAL gradients, so those are kept aside and restored in front of every further tree
-  const bool restore_gh = npt > 1 && b->p.subsample < 1.0f;
+  const bool restore_gh = npt > 1 && b->p.subsample < 1.0f && !refresh;
   if (restore_gh) {
     b->gh_round.ensure((size_t)std::max<int64_t>(n * K, 1));
     CUDA_CHECK(cudaMemcpyAsync(b->gh_round.p, b->gh.p, (size_t)n * K * sizeof(float2), cudaMemcpyDeviceToDevice, s));
   }
   const int round_trees = b->p.vector_leaf() ? 1 : K * npt;   // a vector-leaf tree covers every target
-  if (b->p.vector_leaf()) run_tree(b, 0, 0);
+  if (refresh) {
+    R.rsrc.resize(round_trees);
+    for (int slot = 0; slot < round_trees; ++slot) {
+      R.rsrc[slot] = refresh_round_index * round_trees + slot;
+      refresh_tree(b, slot / npt, slot, R.rsrc[slot]);
+    }
+  } else if (b->p.vector_leaf()) run_tree(b, 0, 0);
   else
   for (int k = 0; k < K; ++k)
     for (int j = 0; j < npt; ++j) {
@@ -3506,14 +3718,25 @@ int B2_BoosterUpdateOneIter(B2Handle bh, int32_t iter) {
   API_BEGIN
   (void)iter;
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  if (b->p.update_mode) fail("this booster has process_type=update: its rounds run through B2_BoosterRefreshOneIter");
   boost_round(b, nullptr, nullptr, 0);
   API_END
 }
 int B2_BoosterBoostOneIter(B2Handle bh, const float* grad, const float* hess, int64_t len) {
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  if (b->p.update_mode) fail("this booster has process_type=update: its rounds run through B2_BoosterRefreshOneIter");
   drain_round(b);
   if (!grad || !hess) fail("grad/hess must not be NULL");
+  boost_round(b, grad, hess, len);
+  API_END
+}
+int B2_BoosterRefreshOneIter(B2Handle bh, const float* grad, const float* hess, int64_t len) {
+  API_BEGIN
+  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  if (!b->p.update_mode) fail("B2_BoosterRefreshOneIter needs a booster created with process_type=update");
+  if ((grad == nullptr) != (hess == nullptr)) fail("grad and hess must both be given or both be NULL");
+  if (grad) drain_round(b);   // the caller computed them from the margin of every round so far
   boost_round(b, grad, hess, len);
   API_END
 }
@@ -3876,6 +4099,7 @@ int B2_BoosterAddTree(B2Handle bh, int32_t n_nodes, const int32_t* left, const i
   API_BEGIN
   Booster* b = from_handle<Booster>(bh, kBooster, "booster");
   drain_round(b);
+  if (b->update_started) fail("process_type=update: trees are added before the first refresh round, not after");
   if (n_nodes < 1) fail("a tree needs at least one node");
   TreeHost t;
   for (int i = 0; i < n_nodes; ++i) {
@@ -3979,10 +4203,12 @@ int B2_BoosterGetTimers(B2Handle bh, int32_t reset, char* out, int64_t out_cap) 
            "{\"hist_ms\": %.6f, \"hist_launches\": %lld, \"hist_rows\": %lld, \"hist_bytes\": %.1f, \"kernel_launches\": %lld, "
            "\"round_ms\": %.6f, \"rounds\": %lld, \"allreduce_bytes\": %.1f, \"num_sms\": %d, \"n_groups\": %d, \"row_stride\": %d, "
            "\"phase_ms\": {\"quant\": %.4f, \"hist\": %.4f, \"allreduce\": %.4f, \"subtract\": %.4f, \"eval_decide\": %.4f, "
-           "\"partition_finalize\": %.4f, \"leaf\": %.4f}, \"shap_ms\": %.6f, \"shap_rows\": %lld}",
+           "\"partition_finalize\": %.4f, \"leaf\": %.4f}, \"shap_ms\": %.6f, \"shap_rows\": %lld, \"refresh_ms\": %.6f, "
+           "\"refresh_launches\": %lld}",
            t.hist_ms, t.hist_launches, t.hist_rows, t.hist_bytes, t.kernel_launches, t.round_ms, t.rounds, t.allreduce_bytes,
            b->ctx->num_sms, b->train ? b->train->n_groups : 0, b->train ? b->train->row_stride : 0, t.phase_ms[0], t.phase_ms[1],
-           t.phase_ms[2], t.phase_ms[3], t.phase_ms[4], t.phase_ms[5], t.phase_ms[6], t.shap_ms, t.shap_rows);
+           t.phase_ms[2], t.phase_ms[3], t.phase_ms[4], t.phase_ms[5], t.phase_ms[6], t.shap_ms, t.shap_rows, t.refresh_ms,
+           t.refresh_launches);
   if (reset) b->t.reset();
   API_END
 }

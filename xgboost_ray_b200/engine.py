@@ -72,6 +72,7 @@ ABI = {
     "B2_BoosterCreate": (C.c_int, [C.c_char_p, _H, _H, C.POINTER(_H)]),
     "B2_BoosterUpdateOneIter": (C.c_int, [_H, C.c_int32]),
     "B2_BoosterBoostOneIter": (C.c_int, [_H, _FP, _FP, C.c_int64]),
+    "B2_BoosterRefreshOneIter": (C.c_int, [_H, _FP, _FP, C.c_int64]),
     "B2_BoosterGetGradients": (C.c_int, [_H, _FP, _FP, C.c_int64]),
     "B2_BoosterEvalSet": (C.c_int, [_H, _H, C.c_char_p, _DP]),
     "B2_BoosterPredict": (C.c_int, [_H, _H, C.c_int32, C.c_int32, C.c_int32, _FP, C.c_int64]),
@@ -645,7 +646,8 @@ _ENGINE_KEYS = ("objective", "num_class", "max_depth", "eta", "learning_rate", "
                 "random_state", "num_parallel_tree", "huber_slope", "tweedie_variance_power", "aft_loss_distribution",
                 "aft_loss_distribution_scale", "lambdarank_pair_method", "lambdarank_num_pair_per_sample",
                 "lambdarank_unbiased", "ndcg_exp_gain", "booster", "rate_drop", "skip_drop", "sample_type",
-                "normalize_type", "one_drop", "quantile_alpha", "num_target", "multi_strategy")
+                "normalize_type", "one_drop", "quantile_alpha", "num_target", "multi_strategy", "process_type",
+                "updater", "refresh_leaf")
 # multi_strategy: one tree per target and round (xgboost's default), or one vector-leaf tree per round (DESIGN.md 2 item 19)
 _MULTI_STRATEGIES = ("one_output_per_tree", "multi_output_tree")
 # booster=dart's parameters with xgboost's defaults (save_config's dart_train_param)
@@ -656,9 +658,40 @@ _DART_DEFAULTS = {"rate_drop": 0.0, "skip_drop": 0.0, "sample_type": "uniform", 
 _UNSUPPORTED_NEUTRAL = {
     "sampling_method": ("uniform",), "max_leaves": (0,), "grow_policy": ("depthwise",),
     "monotone_constraints": (None, "", "()", (), []),
-    "refresh_leaf": (1, True), "process_type": ("default",),
-    "updater": (None, "grow_quantile_histmaker", "grow_gpu_hist"),
+    "updater": (None, "grow_quantile_histmaker", "grow_gpu_hist"),   # and "refresh" in update mode (_check_update)
 }
+
+
+def is_update_mode(params):
+    """process_type='update': the rounds refresh the trees of xgb_model instead of growing new ones."""
+    return (params.get("process_type") or "default") == "update"
+
+
+def _check_update(params):
+    """Update mode (DESIGN.md 2 item 20) takes updater='refresh' and nothing else; updater='refresh' needs update mode.
+    DART, vector-leaf trees and reg:quantileerror are refused, naming the parameter."""
+    pt = params.get("process_type") or "default"
+    if pt not in ("default", "update"):
+        raise XGBoostError("process_type=%r is not supported (supported: 'default', 'update')" % (pt,))
+    rl = params.get("refresh_leaf")
+    if rl is not None and rl not in (0, 1, True, False, "0", "1", "true", "false", "True", "False"):
+        raise XGBoostError("refresh_leaf must be 0 or 1, got %r" % (rl,))
+    updater = params.get("updater")
+    if pt != "update":
+        if updater == "refresh":
+            raise XGBoostError("updater='refresh' needs process_type='update': it refreshes the trees of an existing "
+                               "model (xgb_model)")
+        return
+    if updater != "refresh":
+        raise XGBoostError("process_type='update' needs updater='refresh', got updater=%r (updater='prune' and "
+                           "'refresh,prune' are not supported)" % (updater,))
+    if (params.get("booster") or "gbtree") == "dart":
+        raise XGBoostError("process_type='update' is not supported with booster='dart'")
+    if params.get("multi_strategy") == "multi_output_tree" and int(params.get("num_target", 1) or 1) > 1:
+        raise XGBoostError("process_type='update' is not supported with multi_strategy='multi_output_tree'")
+    if params.get("objective") == "reg:quantileerror":
+        raise XGBoostError("process_type='update' is not supported with objective='reg:quantileerror': its leaf values "
+                           "are residual quantiles, which the refresh updater does not recompute")
 
 
 def _check_quantile(params):
@@ -700,6 +733,7 @@ def _check_multi_strategy(params):
 def _check_supported(params):
     _check_quantile(params)
     _check_multi_strategy(params)
+    _check_update(params)
     mb = params.get("max_bin")
     if mb is not None and not 2 <= int(mb) <= 256:
         raise XGBoostError("parameter max_bin=%r is not supported by the H100 hist engine: the bin matrix is uint8, "
@@ -710,6 +744,8 @@ def _check_supported(params):
             if isinstance(v, (list, tuple)) and k == "monotone_constraints" and all(int(x) == 0 for x in v):
                 continue
             if isinstance(v, str) and k == "monotone_constraints" and set(v) <= set("(), 0"):
+                continue
+            if k == "updater" and v == "refresh":   # checked by _check_update
                 continue
             if v not in neutral:
                 raise XGBoostError("parameter %s=%r is not supported by the H100 hist engine (supported: %s)"
@@ -836,7 +872,12 @@ class Booster:
         if old_trees:
             dtrain._ensure_raw()
             self._push_trees(old_trees, old_weights)
-            _check(lib().B2_BoosterResetTrainMargin(self.handle))
+            if is_update_mode(self.params):
+                # the engine takes these as the trees to update; the model starts empty and grows by refreshed rounds
+                self._trees = []
+                self.__dict__.pop("_tree_json_cache", None)
+            else:
+                _check(lib().B2_BoosterResetTrainMargin(self.handle))
 
     def _ensure_predictor(self, device=None):
         if self.handle:
@@ -990,6 +1031,9 @@ class Booster:
             grad, hess = fobj(pred, dtrain)
             self.boost(dtrain, grad, hess)
             return
+        if is_update_mode(self.params):   # refresh round `iteration` of the model's trees (DESIGN.md 2 item 20)
+            _check(lib().B2_BoosterRefreshOneIter(self.handle, None, None, 0))
+            return
         _check(lib().B2_BoosterUpdateOneIter(self.handle, int(iteration)))
         self._sync_base_score()
 
@@ -1009,6 +1053,9 @@ class Booster:
         h = _f32c(np.asarray(hess).reshape(-1))
         if g.size != h.size:
             raise XGBoostError("grad / hess size mismatch")
+        if is_update_mode(self.params):
+            _check(lib().B2_BoosterRefreshOneIter(self.handle, _fp(g), _fp(h), g.size))
+            return
         _check(lib().B2_BoosterBoostOneIter(self.handle, _fp(g), _fp(h), g.size))
         self._sync_base_score()
 
@@ -1384,6 +1431,10 @@ class Booster:
         sets = self._interaction_sets() if self.n_features is not None else []
         if sets:
             gbtree["tree_train_param"] = {"interaction_constraints": str(sets)}
+        if is_update_mode(self.params):   # xgboost's GBTreeTrainParam of an update run
+            gbtree["gbtree_train_param"] = {"process_type": "update", "updater": "refresh",
+                                            "refresh_leaf": _str_param(self.params.get("refresh_leaf", 1) in
+                                                                       (1, True, "1", "true", "True"))}
         if self.is_dart:
             gbtree = {"name": "dart", "gbtree": gbtree,
                       "dart_train_param": {k: _str_param(self.params.get(k, d)) if isinstance(d, str) else
@@ -1579,6 +1630,11 @@ def train(params, dtrain, num_boost_round=10, evals=(), obj=None, feval=None, ma
     feval = custom_metric if custom_metric is not None else feval
     params = _params_dict(params)
     bst = Booster(params)
+    update = is_update_mode(params)
+    if update:
+        _check_update(params)
+        if xgb_model is None:
+            raise XGBoostError("process_type='update' refreshes the trees of an existing model: pass it as xgb_model")
     if xgb_model is not None:
         if isinstance(xgb_model, Booster):
             src = xgb_model
@@ -1614,6 +1670,33 @@ def train(params, dtrain, num_boost_round=10, evals=(), obj=None, feval=None, ma
             if src.params.get("base_score") is None:
                 raise XGBoostError("cannot continue training: the model passed as xgb_model carries no base_score")
             bst.params["base_score"] = float(src.params["base_score"])
+        if update:
+            # the trees keep their shape and their intercept: num_parallel_tree and base_score are the model's own
+            if src.is_vector_leaf:
+                raise XGBoostError("process_type='update' is not supported with multi_strategy='multi_output_tree'")
+            if src.is_dart:
+                raise XGBoostError("process_type='update' is not supported with booster='dart'")
+            if src.params.get("base_score") is None:
+                raise XGBoostError("process_type='update': the model passed as xgb_model carries no base_score")
+            if src.params.get("objective") == "reg:quantileerror":
+                raise XGBoostError("process_type='update' is not supported for a reg:quantileerror model: its leaf "
+                                   "values are residual quantiles, which the refresh updater does not recompute")
+            bst.params["base_score"] = float(src.params["base_score"])
+            bst.params["num_parallel_tree"] = src.num_parallel_tree
+            per_round = src._trees_per_round
+            if bst._trees_per_round != per_round:
+                # round r's trees are cut from the model by its own outputs; the engine refreshes them by the update
+                # call's (its objective, num_class): the two must agree, else trees would be refreshed for other outputs
+                raise XGBoostError("process_type='update': the model has %d trees per round (%d outputs x "
+                                   "num_parallel_tree %d), the update parameters give %d outputs (objective=%r); pass "
+                                   "the model's objective and num_class"
+                                   % (per_round, src.num_class, src.num_parallel_tree, bst.num_class,
+                                      bst.params.get("objective", "reg:squarederror")))
+            rounds = len(bst._trees) // max(1, per_round)
+            if num_boost_round > rounds:
+                raise XGBoostError("process_type='update' refreshes existing rounds: num_boost_round=%d but the model has "
+                                   "%d rounds" % (num_boost_round, rounds))
+            bst._trees = bst._trees[:num_boost_round * per_round]
     bst._attach(dtrain)
     evals = list(evals or [])
     for dm, _ in evals:

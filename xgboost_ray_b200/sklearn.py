@@ -18,7 +18,8 @@ _PARAM_NAMES = ("max_depth", "learning_rate", "gamma", "min_child_weight", "reg_
                 "base_score", "tree_method", "subsample", "colsample_bytree", "colsample_bylevel", "colsample_bynode",
                 "scale_pos_weight", "max_delta_step", "max_cat_to_onehot", "max_cat_threshold", "eval_metric",
                 "tweedie_variance_power", "huber_slope", "interaction_constraints", "booster", "rate_drop", "skip_drop",
-                "sample_type", "normalize_type", "one_drop", "quantile_alpha", "multi_strategy")
+                "sample_type", "normalize_type", "one_drop", "quantile_alpha", "multi_strategy", "process_type", "updater",
+                "refresh_leaf")
 
 
 def _check_if_params_are_ray_dmatrix(X, sample_weight, base_margin, eval_set):
@@ -50,7 +51,8 @@ class RayXGBMixin(BaseEstimator):
                  interaction_constraints=None, booster: Optional[str] = None, rate_drop: Optional[float] = None,
                  skip_drop: Optional[float] = None, sample_type: Optional[str] = None,
                  normalize_type: Optional[str] = None, one_drop: Optional[int] = None, quantile_alpha=None,
-                 multi_strategy: Optional[str] = None):
+                 multi_strategy: Optional[str] = None, process_type: Optional[str] = None,
+                 updater: Optional[str] = None, refresh_leaf: Optional[int] = None):
         self.n_estimators = n_estimators
         self.max_depth = max_depth
         self.learning_rate = learning_rate
@@ -88,6 +90,10 @@ class RayXGBMixin(BaseEstimator):
         self.one_drop = one_drop
         self.quantile_alpha = quantile_alpha   # reg:quantileerror alphas, e.g. [0.05, 0.5, 0.95]; None = 0.5
         self.multi_strategy = multi_strategy   # 2-D y: "one_output_per_tree" (None) or "multi_output_tree" (vector leaves)
+        # "update" with updater="refresh": fit(xgb_model=...) refreshes that model's trees on X (refresh_leaf: new leaves)
+        self.process_type = process_type
+        self.updater = updater
+        self.refresh_leaf = refresh_leaf
 
     def get_xgb_params(self):
         p = {k: getattr(self, k) for k in _PARAM_NAMES if getattr(self, k) is not None}
