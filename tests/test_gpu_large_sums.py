@@ -3,8 +3,8 @@
 
 A row adds up to 2^40 to a 40-bit fixed-point sum, so one int64 sum wraps past 2^23 rows of gradients near the
 maximum and past 2^24 rows of a unit hessian.  These tests drive every writer of the leaf sums (the streaming
-leaf_accumulate_kernel, the gathering leaf_sums_kernel, final_assign_kernel at the last split level, the unfused leaf
-pass, the NCCL and peer-memory exchanges) and the intercept's sum_fixed_kernel with a node of 2^24 + 2^20 rows.
+leaf_accumulate_kernel, the gathering leaf_sums_kernel, final_assign_kernel at the last split level, the NCCL and
+peer-memory exchanges) and the intercept's sum_fixed_kernel with a node of 2^24 + 2^20 rows.
 
 Tolerance: none.  The engine turns the exact integer sums into correctly rounded doubles and then runs the same IEEE
 double / binary32 operations as the reference (calc_weight, times eta, the link), so leaf values, margins and
@@ -12,9 +12,6 @@ base_score must be equal bit for bit.  A wrapped sum is off by 2^64 units and gi
 
 Device memory: at most 12 features x 2^24 rows of bins plus a few per-row arrays, about 2 GB."""
 import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -24,7 +21,6 @@ from tests import fixed_sums_reference as R
 pytestmark = pytest.mark.gpu
 
 F = np.float32
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SQ = "reg:squarederror"
 
 
@@ -86,23 +82,6 @@ def test_root_leaf_exact(eng, depth):
     X, y = R.root_case(R.N_LARGE)
     bst, dm = _train(eng, {"objective": SQ, "max_depth": depth, "eta": 0.3, "base_score": 0.0}, X, y)
     _check_root_leaf(bst, dm, y)
-
-
-def test_root_leaf_exact_unfused_leaf_pass():
-    """B2_LEAF_FUSED=0: the leaf sums come from leaf_sums_kernel after the last level.  The flag is read once per
-    process, so this runs in a process of its own."""
-    code = (
-        "import sys; sys.path.insert(0, %r)\n"
-        "from xgboost_ray_b200 import engine as E\n"
-        "from tests import fixed_sums_reference as R\n"
-        "from tests.test_gpu_large_sums import _check_root_leaf, _train\n"
-        "X, y = R.root_case(R.N_LARGE)\n"
-        "bst, dm = _train(E, {'objective': 'reg:squarederror', 'max_depth': 6, 'eta': 0.3, 'base_score': 0.0}, X, y)\n"
-        "_check_root_leaf(bst, dm, y)\n"
-        "print('unfused ok')\n") % ROOT
-    r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, B2_LEAF_FUSED="0"), capture_output=True,
-                       text=True, timeout=600)
-    assert r.returncode == 0 and "unfused ok" in r.stdout, (r.stdout[-500:], r.stderr[-2500:])
 
 
 # ------------------------------------------------------------------ one skewed split

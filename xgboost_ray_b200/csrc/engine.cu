@@ -84,8 +84,6 @@ int b2_launch_partition(const uint8_t*, int64_t, const int32_t*, int32_t*, const
                         int, B2FinalizeArgs, int, cudaStream_t);
 int b2_launch_leaf_sums(const float2*, const int32_t*, const int32_t*, const void*, const B2LevelCtl*, int, const int32_t*, int,
                         long long*, uint16_t*, int, cudaStream_t);
-int b2_launch_pred_update(float*, int, int, const int32_t*, const int32_t*, const void*, const B2LevelCtl*, int, const float*, int,
-                          cudaStream_t);
 int b2_launch_decide(const B2DecideArgs*, const void*, cudaStream_t);
 int b2_launch_leaf_plan(const B2LeafDev*, const int32_t*, B2SegWork*, B2LevelCtl*, cudaStream_t);
 int b2_launch_leaf_values(const B2LeafDev*, const int32_t*, const long long*, const int32_t*, int, B2CtlParams, float*, B2TreeDev,
@@ -1651,11 +1649,6 @@ void exchange_and_subtract(Booster* b, TreeStats& st, const long long* parent_le
   mark_phase(b, 3);
 }
 
-// Grow one tree for class k from gh[k] (already on device); updates margin[:, k].  No host
-// synchronisation: every data-dependent decision is taken by the control kernels, the host
-// enqueues a fixed sequence and the finished tree is copied into pinned block `slot`.
-// With st.capturing the stream is in capture mode: nothing here may allocate, touch pageable host memory or depend on
-// host state that changes from tree to tree (run_tree decides when that holds).
 // reg:quantileerror buffers for up to max_leaves segments, allocated outside any capture; the histograms start zeroed
 // and every scan zeroes what it read
 void ensure_quantile_buffers(Booster* b, int max_leaves) {
@@ -1698,6 +1691,170 @@ int quantile_select(Booster* b, int k, const uint16_t* pos, const float* margin,
   return 2 * b2_quantile_passes();
 }
 
+B2TrainParamDev train_params(const Params& p) {
+  B2TrainParamDev dp;
+  dp.min_child_weight = (double)p.min_child_weight; dp.lambda = (double)p.lambda; dp.alpha = (double)p.alpha;
+  dp.inv_scale_g = dp.inv_scale_h = 1.0;
+  dp.max_cat_to_onehot = p.max_cat_to_onehot; dp.max_cat_threshold = p.max_cat_threshold;
+  dp.max_delta_step = (double)p.max_delta_step;
+  return dp;
+}
+
+// the leaf values of the num_parallel_tree trees grown from the same gradients are scaled by eta / num_parallel_tree
+B2CtlParams ctl_params(const Params& p) {
+  B2CtlParams cp;
+  cp.mcw = (double)p.min_child_weight; cp.lambda = (double)p.lambda; cp.alpha = (double)p.alpha;
+  cp.max_delta_step = (double)p.max_delta_step; cp.gamma = p.gamma; cp.eta = p.eta / (float)p.num_parallel_tree;
+  return cp;
+}
+
+// Column sampling of one tree: the tree's feature set and one nested set per level are drawn on the host (they depend
+// on (seed, tree, level) only, never on the data) into d_col_masks, the per-node subsets inside the split-scan kernels.
+// Returns the number of features of every level's set.
+std::vector<int> draw_column_masks(Booster* b, uint32_t tree_index) {
+  Matrix* m = b->train; const Params& p = b->p; const int D = p.max_depth, F = m->F;
+  std::vector<int> n_level_feats(D, F);
+  if (!p.use_cols()) return n_level_feats;
+  const uint32_t* fwq = m->fwq.empty() ? nullptr : m->fwq.data();
+  std::vector<uint8_t> mask_tree(F), masks((size_t)D * F);
+  std::vector<B2ColRank> col_scratch(F);
+  const int n_tree = b2_col_select((uint32_t)p.seed, tree_index, B2_SCOPE_TREE, nullptr, fwq, F,
+                                   b2_sample_count((double)p.colsample_bytree, F), col_scratch.data(), mask_tree.data());
+  for (int d = 0; d < D; ++d)
+    n_level_feats[d] = b2_col_select((uint32_t)p.seed, tree_index, B2_SCOPE_LEVEL(d), mask_tree.data(), fwq, F,
+                                     b2_sample_count((double)p.colsample_bylevel, n_tree), col_scratch.data(),
+                                     masks.data() + (size_t)d * F);
+  b->d_col_masks.ensure(masks.size());
+  CUDA_CHECK(cudaMemcpyAsync(b->d_col_masks.p, masks.data(), masks.size(), cudaMemcpyHostToDevice, b->ctx->stream));   // pageable source: staged before return
+  return n_level_feats;
+}
+
+// Fixed-point quantisation of the gradients of targets k0 .. k0 + nt - 1 for one tree, with a global scale per target
+// (the |g|, |h| maxima over the ranks): the target's exponents go to d_qexp[j] and its quantised pairs to q[j] (j: the
+// target's place in the tree).  Row subsampling zeroes the same rows in every target: the draw depends on
+// (seed, tree, rank, row) only.
+void quantise_gradients(Booster* b, TreeStats& st, int k0, int nt, uint32_t tree_index) {
+  const Params& p = b->p; cudaStream_t s = b->ctx->stream; const int64_t n = b->train->n; const int sms = b->ctx->num_sms;
+  const bool p2p = b->comm && b->comm->world > 1 && b->p2p.enabled;
+  uint32_t* absmax = b->d_absmax.p + 2 * k0;
+  for (int j = 0; j < nt; ++j) {
+    float2* gh = b->gh.p + (size_t)(k0 + j) * n;
+    if (p.subsample < 1.0f) {
+      LAUNCH_CHECK(b2_launch_subsample(gh, n, (uint32_t)p.seed, tree_index, b->comm ? (uint32_t)b->comm->rank : 0u,
+                                       (double)p.subsample, sms, s));
+      st.kernel_launches++;
+    }
+    if (!b->absmax_fused) {   // custom objective / row sampling / many classes: |g|,|h| maxima in their own pass
+      CUDA_CHECK(cudaMemsetAsync(absmax + 2 * j, 0, 2 * sizeof(uint32_t), s));
+      LAUNCH_CHECK(b2_launch_absmax(gh, n, absmax + 2 * j, sms, s));
+      st.kernel_launches++;
+    }
+  }
+  if (!p2p) allreduce(b->comm, absmax, 2 * (size_t)nt, kNcclUint32, kNcclMax, s);
+  for (int j = 0; j < nt; ++j) {
+    int32_t* qexp = b->d_qexp.p + 2 * j;
+    if (p2p) LAUNCH_CHECK(b2_launch_p2p_quant_exponent(&b->p2p.pp, absmax + 2 * j, qexp, s));
+    else LAUNCH_CHECK(b2_launch_quant_exponent(absmax + 2 * j, qexp, s));
+    LAUNCH_CHECK(b2_launch_quantize(b->gh.p + (size_t)(k0 + j) * n, n, qexp, p.qbits, b->q.p + (size_t)j * n, sms, s));
+    st.kernel_launches += 2;
+  }
+}
+
+// One histogram build into tgt from the quantised pairs q: the root (ridx == nullptr: every row, in chunks sized on the
+// host; a rank without rows launches nothing) or the `nodes` nodes of ctl's work list over the ordered rows ridx.
+void launch_hist(Booster* b, TreeStats& st, const int2* q, const int32_t* ridx, const B2LevelCtl* ctl, int nodes,
+                 long long* tgt) {
+  Matrix* m = b->train; const int64_t n = m->n;
+  int root = 0, chunks = 0, chunk_rows = 0;
+  if (!ridx) {
+    if (n == 0) return;
+    root = 1; chunk_rows = pick_chunk_rows(b, n); chunks = (int)((n + chunk_rows - 1) / chunk_rows);
+  }
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  record_hist_launch(b, st, e0, e1, true);
+  LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, q, ridx, b->d_hist_work.p, root, chunks, chunk_rows,
+                              window_rows_for(b->p.qbits), m->n_groups, tgt, ctl, b->log2_shards, nodes, b->ctx->num_sms,
+                              b->ctx->stream));
+  record_hist_launch(b, st, e0, e1, false);
+  st.hist_launches++; st.kernel_launches++;
+}
+
+// What decide does at the end of level d's split scan, with cpn candidates per node and rank
+B2DecideArgs decide_args(Booster* b, const B2TreeDev& tree, const B2CtlParams& cp, int d, int cpn) {
+  Matrix* m = b->train; B2LevelCtl* ctl = b->d_ctl.p;
+  const int cur = d & 1, nxt = cur ^ 1;
+  const bool can_split = d < b->p.max_depth;
+  B2DecideArgs da;
+  da.ctl_cur = ctl + cur; da.ctl_nxt = ctl + nxt; da.seg_cur = b->d_seg[cur].p; da.seg_nxt = b->d_seg[nxt].p;
+  da.ev_cur = b->d_ev[cur].p; da.ev_nxt = b->d_ev[nxt].p;
+  da.cands = b->d_cands.p; da.cand_best = b->d_cand_best.p; da.local_cands = b->d_cands.p;
+  da.tree = tree; da.split_work = b->d_split_work.p; da.pair_parent_hist = b->d_pair_parent.p; da.leaves = b->d_leaves.p;
+  da.n_leaves = tree.n_nodes + 1; da.has_missing = m->d_has_missing.p; da.qexp = b->d_qexp.p;
+  da.part_counters = can_split ? b->d_counters.p : nullptr; da.p = cp;
+  B2Interaction ic{nullptr, nullptr, 0};
+  if (b->ic_words > 0) { ic.sets_of = b->d_ic_sets_of.p; ic.compat = b->d_ic_compat.p; ic.words = b->ic_words; }
+  da.ic = ic;
+  da.cands_per_node = cpn; da.cand_ranks = b->shards; da.cand_rank_stride = (1 << d) * cpn;
+  da.can_split = can_split ? 1 : 0; da.qbits = b->p.qbits; da.vector_leaf = 0;
+  return da;
+}
+
+// column sampling of level d's split scan: n_level features in the level's set, filtered per node by ic
+B2ColSample col_sample(Booster* b, int d, int n_level, uint32_t tree_index, const B2Interaction& ic) {
+  Matrix* m = b->train; const Params& p = b->p;
+  B2ColSample cs;
+  cs.level_mask = p.use_cols() ? b->d_col_masks.p + (size_t)d * m->F : nullptr;
+  cs.fwq = m->fwq.empty() ? nullptr : m->d_fwq.p;
+  cs.bynode = (double)p.colsample_bynode; cs.n_level = n_level; cs.n_features = m->F;
+  cs.seed = (uint32_t)p.seed; cs.tree = p.use_cols() ? tree_index : 0u;
+  cs.ic = ic;
+  return cs;
+}
+
+// Rows of level d's nodes (the root's rows are the identity list) and the bound of its split work items
+const int32_t* level_ridx(Booster* b, int d) { return d == 0 ? nullptr : b->ridx[d & 1].p; }
+int split_work_items(Booster* b, int d) {
+  const int64_t n = b->train->n; const int pchunk = b2_split_chunk_rows();
+  return (int)((n + pchunk - 1) / pchunk) + (1 << d);   // chunks of all rows + nodes of the level: an upper bound
+}
+
+// Partition the rows of level d's expanding nodes into the other index list (decide zeroed the counters); the last CTA
+// of the partition finalises the level: child segments, build-child choice, next histogram work list
+void partition_level(Booster* b, TreeStats& st, int d) {
+  Matrix* m = b->train; const Params& p = b->p; B2LevelCtl* ctl = b->d_ctl.p;
+  const int cur = d & 1, nxt = cur ^ 1;
+  B2FinalizeArgs fin;
+  fin.ctl_nxt = ctl + nxt; fin.seg_nxt = b->d_seg[nxt].p; fin.ev_nxt = b->d_ev[nxt].p; fin.pair_parent_hist = b->d_pair_parent.p;
+  fin.hist_work = b->d_hist_work.p; fin.triples = b->d_triples.p; fin.done = b->d_part_done.p;
+  fin.stat_rows = b->t_i64.p + 2 * tree_layout(p.max_depth).max_nodes + d + 1;   // rows per level, after the node sums
+  fin.max_pairs = 1 << d; fin.need_hist = d + 1 < p.max_depth ? 1 : 0;
+  fin.n_streams = std::max(1, b->ctx->num_sms * 3 / m->n_groups); fin.window_rows = window_rows_for(p.qbits);
+  fin.chunk_rows_override = p.hist_chunk_rows;
+  LAUNCH_CHECK(b2_launch_partition(m->bins_col.p, m->col_stride, level_ridx(b, d), b->ridx[nxt].p, b->d_split_work.p,
+                                   ctl + cur, split_work_items(b, d), b->d_counters.p, m->any_cat() ? 1 : 0, fin,
+                                   b->ctx->num_sms, b->ctx->stream));
+  st.kernel_launches++;
+}
+
+// The children of the last split level d are leaves: no ordered index lists any more.  Leaves that stopped earlier get
+// their rows' leaf index (pos) from their segments, rows of the nodes that split here are assigned in one pass
+// (partition_kernel.cu); with sums, both also add gh (quantised by qexp) to the 40-bit fixed-point leaf sums.
+void assign_leaves(Booster* b, TreeStats& st, int d, const float2* gh, const int32_t* qexp, long long* sums) {
+  Matrix* m = b->train; B2LevelCtl* ctl = b->d_ctl.p; cudaStream_t s = b->ctx->stream; const int sms = b->ctx->num_sms;
+  const int lchunk = b2_part_chunk_rows();
+  const int max_leaf_chunks = (int)((m->n + lchunk - 1) / lchunk) + (1 << b->p.max_depth);
+  LAUNCH_CHECK(b2_launch_leaf_sums(gh, b->ridx[0].p, b->ridx[1].p, b->d_seg_work.p, ctl + 2, max_leaf_chunks, qexp, 40, sums,
+                                   b->pos.p, sms, s));
+  LAUNCH_CHECK(b2_launch_final_assign(m->bins_col.p, m->col_stride, level_ridx(b, d), b->d_split_work.p, ctl + (d & 1),
+                                      split_work_items(b, d), gh, qexp, 40, sums, b->pos.p, m->any_cat() ? 1 : 0, sms, s));
+  st.kernel_launches += 2;
+}
+
+// Grow one tree for class k from gh[k] (already on device); updates margin[:, k].  No host
+// synchronisation: every data-dependent decision is taken by the control kernels, the host
+// enqueues a fixed sequence and the finished tree is copied into pinned block `slot`.
+// With st.capturing the stream is in capture mode: nothing here may allocate, touch pageable host memory or depend on
+// host state that changes from tree to tree (run_tree decides when that holds).
 void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   Matrix* m = b->train; Ctx* ctx = b->ctx; cudaStream_t s = ctx->stream; const Params& p = b->p;
   const int64_t n = m->n; const int K = p.num_class; const int G = m->n_groups; const int D = p.max_depth;
@@ -1706,70 +1863,22 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   const TreeLayout L = tree_layout(D);
   const bool multi = b->comm && b->comm->world > 1;
   const bool p2p = multi && b->p2p.enabled;
-  static const bool leaf_fused = env_flag("B2_LEAF_FUSED", true);
-  if (p.dart && !leaf_fused) fail("booster=dart needs the fused leaf pass (unset B2_LEAF_FUSED)");
-  if (b->refresh_leaves && !leaf_fused) fail("reg:quantileerror needs the fused leaf pass (unset B2_LEAF_FUSED)");
   // leaf sums from a streaming pass over (pos, gh) in row order; needs one shared-memory accumulator per leaf
-  const bool leaf_stream = leaf_fused && D >= 1 && D <= b2_leaf_acc_max_depth();
+  const bool leaf_stream = D <= b2_leaf_acc_max_depth();
   // sibling subtraction inside eval_splits_kernel (no hist_subtract pass).  The peer-memory exchange subtracts while it
   // reduces, and the categorical scan reads the sibling slots itself, so both keep the stored siblings.
   const bool sub_in_scan = !p2p && !m->any_cat();
   mark_phase(b, -1);
-  // ---- fixed-point quantisation (global scale via max over the ranks)
   // position of this tree in the model (sampling seed): the trees of a round still pending come before it
   const uint32_t tree_index = (uint32_t)b->trees.size() + (uint32_t)b->pending_trees + (uint32_t)slot;
-  uint32_t* d_absmax = b->d_absmax.p + 2 * k;
-  if (p.subsample < 1.0f) {
-    LAUNCH_CHECK(b2_launch_subsample(b->gh.p + (size_t)k * n, n, (uint32_t)p.seed, tree_index, b->comm ? (uint32_t)b->comm->rank : 0u,
-                                     (double)p.subsample, ctx->num_sms, s));
-    st.kernel_launches++;
-  }
-  // column sampling: the tree's feature set and one nested set per level are drawn on the host (they depend on
-  // (seed, tree, level) only, never on the data), the per-node subsets inside the split-scan kernels
-  std::vector<int> n_level_feats(D > 0 ? D : 1, m->F);
-  if (p.use_cols()) {
-    const int F = m->F;
-    const uint32_t* fwq = m->fwq.empty() ? nullptr : m->fwq.data();
-    std::vector<uint8_t> mask_tree(F), masks((size_t)std::max(D, 1) * F);
-    std::vector<B2ColRank> col_scratch(F);
-    const int n_tree = b2_col_select((uint32_t)p.seed, tree_index, B2_SCOPE_TREE, nullptr, fwq, F,
-                                     b2_sample_count((double)p.colsample_bytree, F), col_scratch.data(), mask_tree.data());
-    for (int d = 0; d < D; ++d)
-      n_level_feats[d] = b2_col_select((uint32_t)p.seed, tree_index, B2_SCOPE_LEVEL(d), mask_tree.data(), fwq, F,
-                                       b2_sample_count((double)p.colsample_bylevel, n_tree), col_scratch.data(),
-                                       masks.data() + (size_t)d * F);
-    b->d_col_masks.ensure(masks.size());
-    CUDA_CHECK(cudaMemcpyAsync(b->d_col_masks.p, masks.data(), masks.size(), cudaMemcpyHostToDevice, s));   // pageable source: staged before return
-  }
-  if (!b->absmax_fused) {   // custom objective / row sampling / many classes: |g|,|h| maxima in their own pass
-    CUDA_CHECK(cudaMemsetAsync(d_absmax, 0, 2 * sizeof(uint32_t), s));
-    LAUNCH_CHECK(b2_launch_absmax(gh, n, d_absmax, ctx->num_sms, s));
-    st.kernel_launches++;
-  }
-  if (p2p) LAUNCH_CHECK(b2_launch_p2p_quant_exponent(&b->p2p.pp, d_absmax, b->d_qexp.p, s));
-  else {
-    allreduce(b->comm, d_absmax, 2, kNcclUint32, kNcclMax, s);
-    LAUNCH_CHECK(b2_launch_quant_exponent(d_absmax, b->d_qexp.p, s));
-  }
-  LAUNCH_CHECK(b2_launch_quantize(gh, n, b->d_qexp.p, p.qbits, b->q.p, ctx->num_sms, s));
-  st.kernel_launches += 2;
-
-  B2TrainParamDev dp;
-  dp.min_child_weight = (double)p.min_child_weight; dp.lambda = (double)p.lambda; dp.alpha = (double)p.alpha;
-  dp.inv_scale_g = dp.inv_scale_h = 1.0;
-  dp.max_cat_to_onehot = p.max_cat_to_onehot; dp.max_cat_threshold = p.max_cat_threshold;
-  dp.max_delta_step = (double)p.max_delta_step;
-  B2CtlParams cp; cp.mcw = dp.min_child_weight; cp.lambda = dp.lambda; cp.alpha = dp.alpha; cp.max_delta_step = dp.max_delta_step; cp.gamma = p.gamma; cp.eta = p.eta / (float)p.num_parallel_tree;
+  quantise_gradients(b, st, k, 1, tree_index);
+  const std::vector<int> n_level_feats = draw_column_masks(b, tree_index);
+  const B2TrainParamDev dp = train_params(p);
+  const B2CtlParams cp = ctl_params(p);
   const B2TreeDev tree = tree_dev(b);
   int32_t* d_n_leaves = tree.n_nodes + 1;
-  long long* d_level_rows = b->t_i64.p + 2 * L.max_nodes;
   B2LevelCtl* ctl = b->d_ctl.p;
-  const int window = window_rows_for(p.qbits);
-  const int n_streams = std::max(1, ctx->num_sms * 3 / G);
-  const int pchunk = b2_split_chunk_rows(), lchunk = b2_part_chunk_rows();
-  const int max_part_chunks_total = (int)((n + pchunk - 1) / pchunk);   // + nodes of the level: upper bound of the split work items
   const size_t lcap = (size_t)1 << D;
-  const int max_leaf_chunks = (int)((n + lchunk - 1) / lchunk) + (int)lcap;
 
   LAUNCH_CHECK(b2_launch_tree_init(tree, ctl, b->d_seg[0].p, b->d_ev[0].p, d_n_leaves, (int)n, b->d_hist_work.p, s));
   CUDA_CHECK(cudaMemsetAsync(b->d_leaf_sums.p, 0, 4 * lcap * sizeof(long long), s));
@@ -1778,18 +1887,7 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   const int sh = b->log2_shards;
   const int shard_rank = b->shards > 1 ? b->comm->rank : 0;
   CUDA_CHECK(cudaMemsetAsync(build_target(b, b->hist[0].p), 0, b->node_elems * sizeof(long long), s));
-  {
-    const int chunk_rows = pick_chunk_rows(b, n);
-    const int chunks = (int)((n + chunk_rows - 1) / chunk_rows);
-    if (n > 0) {
-      cudaEvent_t e0 = nullptr, e1 = nullptr;
-      record_hist_launch(b, st, e0, e1, true);
-      LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, b->q.p, nullptr, b->d_hist_work.p, 1, chunks, chunk_rows, window, G,
-                                  build_target(b, b->hist[0].p), nullptr, sh, 1, ctx->num_sms, s));
-      record_hist_launch(b, st, e0, e1, false);
-      st.hist_launches++; st.kernel_launches++;
-    }
-  }
+  launch_hist(b, st, b->q.p, nullptr, nullptr, 1, build_target(b, b->hist[0].p));
   mark_phase(b, 1);
   exchange_and_subtract(b, st, nullptr, b->hist[0].p, nullptr, nullptr, 1, 1);
   LAUNCH_CHECK(b2_launch_root_totals(b->hist[0].p, G, b->d_ev[0].p, b->d_qexp.p, p.qbits, dp, sh, tree.sum_g, tree.sum_h, s));
@@ -1799,32 +1897,15 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
     const int cur = d & 1, nxt = cur ^ 1;
     const int max_nodes_level = 1 << d;
     const bool can_split = d < D;
-    const bool last_split_level = d == D - 1;
     // candidates per node of this level: the scan's CTAs per node (its layout depends on the node count) + categorical
     const int cpn_num = b2_eval_ctas_per_node(G, sh, max_nodes_level);
     const int cpn = cpn_num + (m->any_cat() ? b2_cat_ctas() : 0);
-    B2DecideArgs da;
-    da.ctl_cur = ctl + cur; da.ctl_nxt = ctl + nxt; da.seg_cur = b->d_seg[cur].p; da.seg_nxt = b->d_seg[nxt].p;
-    da.ev_cur = b->d_ev[cur].p; da.ev_nxt = b->d_ev[nxt].p;
-    da.cands = b->d_cands.p; da.cand_best = b->d_cand_best.p; da.local_cands = b->d_cands.p;
-    da.tree = tree; da.split_work = b->d_split_work.p; da.pair_parent_hist = b->d_pair_parent.p; da.leaves = b->d_leaves.p;
-    da.n_leaves = d_n_leaves; da.has_missing = m->d_has_missing.p; da.qexp = b->d_qexp.p;
-    da.part_counters = can_split ? b->d_counters.p : nullptr; da.p = cp;
-    B2Interaction ic{nullptr, nullptr, 0};
-    if (b->ic_words > 0) { ic.sets_of = b->d_ic_sets_of.p; ic.compat = b->d_ic_compat.p; ic.words = b->ic_words; }
-    da.ic = ic;
-    da.cands_per_node = cpn; da.cand_ranks = b->shards; da.cand_rank_stride = max_nodes_level * cpn;
-    da.can_split = can_split ? 1 : 0; da.qbits = p.qbits; da.vector_leaf = 0;
+    B2DecideArgs da = decide_args(b, tree, cp, d, cpn);
     // one GPU, numeric features only, levels scanned by the narrow layout: the last CTA of the scan decides the level
     // (no decide launch)
     const bool fold_decide = can_split && !multi && !m->any_cat() && max_nodes_level <= b2_eval_narrow_max_nodes();
     if (can_split) {
-      B2ColSample cs;
-      cs.level_mask = p.use_cols() ? b->d_col_masks.p + (size_t)d * m->F : nullptr;
-      cs.fwq = m->fwq.empty() ? nullptr : m->d_fwq.p;
-      cs.bynode = (double)p.colsample_bynode; cs.n_level = n_level_feats[d]; cs.n_features = m->F;
-      cs.seed = (uint32_t)p.seed; cs.tree = p.use_cols() ? tree_index : 0u;
-      cs.ic = ic;
+      const B2ColSample cs = col_sample(b, d, n_level_feats[d], tree_index, da.ic);
       // siblings of this level: parent (previous level buffer) - built, formed in the scan; stored only when the next
       // level takes them as parents
       B2SiblingSub sub{nullptr, nullptr, nullptr, 0};
@@ -1858,48 +1939,23 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
     }
     mark_phase(b, 4);
     if (!can_split) break;
-    const int32_t* ridx_in = d == 0 ? nullptr : b->ridx[cur].p;   // the root's rows are the identity list
-    if (last_split_level && leaf_fused) {
-      // ---- the children of this level are leaves: no ordered index lists any more.  Leaves that stopped earlier get
-      // their rows' leaf index from their segments, rows of the nodes that split here are assigned in one pass
-      // (partition_kernel.cu).  With leaf_stream the sums are left to leaf_accumulate_kernel after the last decide.
-      long long* sums = leaf_stream ? nullptr : b->d_leaf_sums.p;
+    if (d == D - 1) {   // with leaf_stream the sums are left to leaf_accumulate_kernel after the last decide
       LAUNCH_CHECK(b2_launch_leaf_plan(b->d_leaves.p, &ctl[cur].leaf_base_next, b->d_seg_work.p, ctl + 2, s));
-      LAUNCH_CHECK(b2_launch_leaf_sums(gh, b->ridx[0].p, b->ridx[1].p, b->d_seg_work.p, ctl + 2, max_leaf_chunks, b->d_qexp.p, 40,
-                                       sums, b->pos.p, ctx->num_sms, s));
-      LAUNCH_CHECK(b2_launch_final_assign(m->bins_col.p, m->col_stride, ridx_in, b->d_split_work.p, ctl + cur,
-                                          max_part_chunks_total + max_nodes_level, gh, b->d_qexp.p, 40, sums, b->pos.p,
-                                          m->any_cat() ? 1 : 0, ctx->num_sms, s));
-      st.kernel_launches += 3;
+      assign_leaves(b, st, d, gh, b->d_qexp.p, leaf_stream ? nullptr : b->d_leaf_sums.p);
+      st.kernel_launches++;
       mark_phase(b, 5);
       continue;
     }
-    // ---- partition rows of the expanding nodes into the other index list (decide zeroed the counters); the last CTA
-    // of the partition finalises the level: child segments, build-child choice, next histogram work list
-    const bool need_hist = d + 1 < D;
-    B2FinalizeArgs fin;
-    fin.ctl_nxt = ctl + nxt; fin.seg_nxt = b->d_seg[nxt].p; fin.ev_nxt = b->d_ev[nxt].p; fin.pair_parent_hist = b->d_pair_parent.p;
-    fin.hist_work = b->d_hist_work.p; fin.triples = b->d_triples.p; fin.stat_rows = d_level_rows + d + 1; fin.done = b->d_part_done.p;
-    fin.max_pairs = max_nodes_level; fin.need_hist = need_hist ? 1 : 0; fin.n_streams = n_streams; fin.window_rows = window;
-    fin.chunk_rows_override = p.hist_chunk_rows;
-    LAUNCH_CHECK(b2_launch_partition(m->bins_col.p, m->col_stride, ridx_in, b->ridx[nxt].p, b->d_split_work.p, ctl + cur,
-                                     max_part_chunks_total + max_nodes_level, b->d_counters.p, m->any_cat() ? 1 : 0, fin,
-                                     ctx->num_sms, s));
-    st.kernel_launches++;
+    partition_level(b, st, d);
     mark_phase(b, 5);
-    if (need_hist) {
+    if (d + 1 < D) {
       // ---- histograms of level d+1: built children in slots [0, 2^d), siblings in [2^d, 2^(d+1))
       const int nh = hb ^ 1;
       long long* tgt = build_target(b, b->hist[nh].p);
       // (peer-memory exchange: every peer finished reading this rank's build buffer before it published the candidates
       // that the decide kernel above waited for, so the buffer can be zeroed here without another handshake)
       CUDA_CHECK(cudaMemsetAsync(tgt, 0, (size_t)max_nodes_level * b->node_elems * sizeof(long long), s));
-      cudaEvent_t e0 = nullptr, e1 = nullptr;
-      record_hist_launch(b, st, e0, e1, true);
-      LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, b->q.p, b->ridx[nxt].p, b->d_hist_work.p, 0, 0, 0, window, G, tgt,
-                                  ctl + nxt, sh, max_nodes_level, ctx->num_sms, s));
-      record_hist_launch(b, st, e0, e1, false);
-      st.hist_launches++; st.kernel_launches++;
+      launch_hist(b, st, b->q.p, b->ridx[nxt].p, ctl + nxt, max_nodes_level, tgt);
       mark_phase(b, 1);
       exchange_and_subtract(b, st, b->hist[hb].p, b->hist[nh].p, sub_in_scan ? nullptr : b->d_triples.p, ctl + nxt,
                             max_nodes_level, max_nodes_level);
@@ -1907,12 +1963,7 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
     }
   }
   // ---- leaves: 40-bit fixed-point leaf sums -> sum over the ranks -> weights -> margin update
-  if (!leaf_fused) {
-    LAUNCH_CHECK(b2_launch_leaf_plan(b->d_leaves.p, d_n_leaves, b->d_seg_work.p, ctl + 2, s));
-    LAUNCH_CHECK(b2_launch_leaf_sums(gh, b->ridx[0].p, b->ridx[1].p, b->d_seg_work.p, ctl + 2, max_leaf_chunks, b->d_qexp.p, 40,
-                                     b->d_leaf_sums.p, nullptr, ctx->num_sms, s));
-    st.kernel_launches += 2;
-  } else if (leaf_stream) {   // every row's leaf index is in pos: sum the leaves in row order
+  if (leaf_stream) {   // every row's leaf index is in pos: sum the leaves in row order
     LAUNCH_CHECK(b2_launch_leaf_accumulate(gh, b->pos.p, n, D, b->d_qexp.p, 40, b->d_leaf_sums.p, ctx->num_sms, s));
     st.kernel_launches++;
   }
@@ -1923,12 +1974,8 @@ void grow_tree(Booster* b, int k, int slot, TreeStats& st) {
   if (b->refresh_leaves)
     st.kernel_launches += quantile_select(b, k, b->pos.p, b->margin.p, gh, b->d_qexp.p, d_n_leaves, (int)lcap, cp.eta,
                                           b->d_leaves.p, b->d_leaf_values.p, tree.leaf_value);
-  if (leaf_fused)
-    LAUNCH_CHECK(b2_launch_margin_update(b->margin.p, K, k, b->pos.p, b->d_leaf_values.p, p.dart ? b->d_dart_w_new.p : nullptr, n,
-                                         ctx->num_sms, s));
-  else
-    LAUNCH_CHECK(b2_launch_pred_update(b->margin.p, K, k, b->ridx[0].p, b->ridx[1].p, b->d_seg_work.p, ctl + 2, max_leaf_chunks,
-                                       b->d_leaf_values.p, ctx->num_sms, s));
+  LAUNCH_CHECK(b2_launch_margin_update(b->margin.p, K, k, b->pos.p, b->d_leaf_values.p, p.dart ? b->d_dart_w_new.p : nullptr, n,
+                                       ctx->num_sms, s));
   st.kernel_launches += 2;
   mark_phase(b, 6);
   // ---- read the finished tree back (pinned, asynchronous; resolved when the round is drained)
@@ -1959,8 +2006,6 @@ void grow_vector_tree(Booster* b, int slot, TreeStats& st) {
   ensure_ctl_tables(b);
   const TreeLayout L = tree_layout(D);
   const VectorLayout V = vector_layout(D, T);
-  static const bool leaf_fused = env_flag("B2_LEAF_FUSED", true);
-  if (!leaf_fused) fail("multi_strategy=multi_output_tree needs the fused leaf pass (unset B2_LEAF_FUSED)");
   const bool leaf_stream = D <= b2_leaf_acc_max_depth();
   mark_phase(b, -1);
   const uint32_t tree_index = (uint32_t)b->trees.size() + (uint32_t)b->pending_trees + (uint32_t)slot;
@@ -1970,83 +2015,25 @@ void grow_vector_tree(Booster* b, int slot, TreeStats& st) {
   float* tree_vec = (float*)(b->d_vblock.p + V.off_vec);
   int32_t* qexp_out = (int32_t*)(b->d_vblock.p + V.off_qexp);
   float* vgain = b->t_f32.p + L.max_nodes;        // the scalar tree's leaf_weight array, unused by vector trees
-  for (int k = 0; k < T; ++k) {
-    float2* ghk = b->gh.p + (size_t)k * n;
-    uint32_t* d_absmax = b->d_absmax.p + 2 * k;
-    if (p.subsample < 1.0f) {   // the same rows in every target: the draw depends on (seed, tree, rank, row) only
-      LAUNCH_CHECK(b2_launch_subsample(ghk, n, (uint32_t)p.seed, tree_index, b->comm ? (uint32_t)b->comm->rank : 0u,
-                                       (double)p.subsample, ctx->num_sms, s));
-      st.kernel_launches++;
-    }
-    if (!b->absmax_fused) {
-      CUDA_CHECK(cudaMemsetAsync(d_absmax, 0, 2 * sizeof(uint32_t), s));
-      LAUNCH_CHECK(b2_launch_absmax(ghk, n, d_absmax, ctx->num_sms, s));
-      st.kernel_launches++;
-    }
-  }
-  allreduce(b->comm, b->d_absmax.p, 2 * (size_t)T, kNcclUint32, kNcclMax, s);   // every target's maxima over all ranks
-  for (int k = 0; k < T; ++k) {
-    float2* ghk = b->gh.p + (size_t)k * n;
-    LAUNCH_CHECK(b2_launch_quant_exponent(b->d_absmax.p + 2 * k, b->d_qexp.p + 2 * k, s));
-    LAUNCH_CHECK(b2_launch_quantize(ghk, n, b->d_qexp.p + 2 * k, p.qbits, b->q.p + (size_t)k * n, ctx->num_sms, s));
-    st.kernel_launches += 2;
-  }
-  std::vector<int> n_level_feats(D, m->F);
-  if (p.use_cols()) {   // one draw per tree, as grow_tree
-    const int F = m->F;
-    const uint32_t* fwq = m->fwq.empty() ? nullptr : m->fwq.data();
-    std::vector<uint8_t> mask_tree(F), masks((size_t)D * F);
-    std::vector<B2ColRank> col_scratch(F);
-    const int n_tree = b2_col_select((uint32_t)p.seed, tree_index, B2_SCOPE_TREE, nullptr, fwq, F,
-                                     b2_sample_count((double)p.colsample_bytree, F), col_scratch.data(), mask_tree.data());
-    for (int d = 0; d < D; ++d)
-      n_level_feats[d] = b2_col_select((uint32_t)p.seed, tree_index, B2_SCOPE_LEVEL(d), mask_tree.data(), fwq, F,
-                                       b2_sample_count((double)p.colsample_bylevel, n_tree), col_scratch.data(),
-                                       masks.data() + (size_t)d * F);
-    b->d_col_masks.ensure(masks.size());
-    CUDA_CHECK(cudaMemcpyAsync(b->d_col_masks.p, masks.data(), masks.size(), cudaMemcpyHostToDevice, s));   // pageable source: staged before return
-  }
-  B2TrainParamDev dp;
-  dp.min_child_weight = (double)p.min_child_weight; dp.lambda = (double)p.lambda; dp.alpha = (double)p.alpha;
-  dp.inv_scale_g = dp.inv_scale_h = 1.0;
-  dp.max_cat_to_onehot = p.max_cat_to_onehot; dp.max_cat_threshold = p.max_cat_threshold;
-  dp.max_delta_step = (double)p.max_delta_step;
-  B2CtlParams cp; cp.mcw = dp.min_child_weight; cp.lambda = dp.lambda; cp.alpha = dp.alpha; cp.max_delta_step = dp.max_delta_step;
-  cp.gamma = p.gamma; cp.eta = p.eta;
+  quantise_gradients(b, st, 0, T, tree_index);
+  const std::vector<int> n_level_feats = draw_column_masks(b, tree_index);
+  const B2TrainParamDev dp = train_params(p);
+  const B2CtlParams cp = ctl_params(p);
   const bool multi = b->comm && b->comm->world > 1;
-  const double node_bytes = (double)b->node_elems * sizeof(long long);
   const B2TreeDev tree = tree_dev(b);
   int32_t* d_n_leaves = tree.n_nodes + 1;
-  long long* d_level_rows = b->t_i64.p + 2 * L.max_nodes;
   B2LevelCtl* ctl = b->d_ctl.p;
-  const int window = window_rows_for(p.qbits);
-  const int n_streams = std::max(1, ctx->num_sms * 3 / G);
-  const int pchunk = b2_split_chunk_rows(), lchunk = b2_part_chunk_rows();
-  const int max_part_chunks_total = (int)((n + pchunk - 1) / pchunk);
-  const int max_leaf_chunks = (int)((n + lchunk - 1) / lchunk) + (int)lcap;
   const size_t sums_stride = 4 * lcap;
   LAUNCH_CHECK(b2_launch_tree_init(tree, ctl, b->d_seg[0].p, b->d_ev[0].p, d_n_leaves, (int)n, b->d_hist_work.p, s));
   CUDA_CHECK(cudaMemsetAsync(b->d_vsums.p, 0, (size_t)T * sums_stride * sizeof(long long), s));
   mark_phase(b, 0);
-  {   // root histograms, one per target
-    const int chunk_rows = pick_chunk_rows(b, n);
-    const int chunks = (int)((n + chunk_rows - 1) / chunk_rows);
-    for (int k = 0; k < T; ++k) {
-      long long* tgt = b->d_vhist[0].p + (size_t)k * tstride;
-      CUDA_CHECK(cudaMemsetAsync(tgt, 0, b->node_elems * sizeof(long long), s));
-      if (n > 0) {
-        cudaEvent_t e0 = nullptr, e1 = nullptr;
-        record_hist_launch(b, st, e0, e1, true);
-        LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, b->q.p + (size_t)k * n, nullptr, b->d_hist_work.p, 1, chunks, chunk_rows,
-                                    window, G, tgt, nullptr, 0, 1, ctx->num_sms, s));
-        record_hist_launch(b, st, e0, e1, false);
-        st.hist_launches++; st.kernel_launches++;
-      }
-      allreduce(b->comm, tgt, b->node_elems, kNcclInt64, kNcclSum, s);   // exact: integer sums
-      if (multi) st.allreduce_bytes += node_bytes;
-    }
+  for (int k = 0; k < T; ++k) {   // root histograms, one per target
+    long long* tgt = b->d_vhist[0].p + (size_t)k * tstride;
+    CUDA_CHECK(cudaMemsetAsync(tgt, 0, b->node_elems * sizeof(long long), s));
+    launch_hist(b, st, b->q.p + (size_t)k * n, nullptr, nullptr, 1, tgt);
+    mark_phase(b, 1);
+    exchange_and_subtract(b, st, nullptr, tgt, nullptr, nullptr, 1, 1);
   }
-  mark_phase(b, 1);
   LAUNCH_CHECK(b2_launch_vector_root_totals(b->d_vhist[0].p, tstride, T, G, b->d_qexp.p, p.qbits, dp, vtot, vgain, s));
   st.kernel_launches++;
   const int cpn = b2_eval_vector_ctas_per_node(G);
@@ -2055,25 +2042,10 @@ void grow_vector_tree(Booster* b, int slot, TreeStats& st) {
     const int cur = d & 1, nxt = cur ^ 1;
     const int max_nodes_level = 1 << d;
     const bool can_split = d < D;
-    B2DecideArgs da;
-    da.ctl_cur = ctl + cur; da.ctl_nxt = ctl + nxt; da.seg_cur = b->d_seg[cur].p; da.seg_nxt = b->d_seg[nxt].p;
-    da.ev_cur = b->d_ev[cur].p; da.ev_nxt = b->d_ev[nxt].p;
-    da.cands = b->d_cands.p; da.cand_best = b->d_cand_best.p; da.local_cands = b->d_cands.p;
-    da.tree = tree; da.split_work = b->d_split_work.p; da.pair_parent_hist = b->d_pair_parent.p; da.leaves = b->d_leaves.p;
-    da.n_leaves = d_n_leaves; da.has_missing = m->d_has_missing.p; da.qexp = b->d_qexp.p;
-    da.part_counters = can_split ? b->d_counters.p : nullptr; da.p = cp;
-    B2Interaction ic{nullptr, nullptr, 0};
-    if (b->ic_words > 0) { ic.sets_of = b->d_ic_sets_of.p; ic.compat = b->d_ic_compat.p; ic.words = b->ic_words; }
-    da.ic = ic;
-    da.cands_per_node = cpn; da.cand_ranks = 1; da.cand_rank_stride = max_nodes_level * cpn;
-    da.can_split = can_split ? 1 : 0; da.qbits = p.qbits; da.vector_leaf = 1;
+    B2DecideArgs da = decide_args(b, tree, cp, d, cpn);
+    da.vector_leaf = 1;
     if (can_split) {
-      B2ColSample cs;
-      cs.level_mask = p.use_cols() ? b->d_col_masks.p + (size_t)d * m->F : nullptr;
-      cs.fwq = m->fwq.empty() ? nullptr : m->d_fwq.p;
-      cs.bynode = (double)p.colsample_bynode; cs.n_level = n_level_feats[d]; cs.n_features = m->F;
-      cs.seed = (uint32_t)p.seed; cs.tree = p.use_cols() ? tree_index : 0u;
-      cs.ic = ic;
+      const B2ColSample cs = col_sample(b, d, n_level_feats[d], tree_index, da.ic);
       LAUNCH_CHECK(b2_launch_eval_splits_vector(b->d_vhist[hb].p, tstride, T, G, b->d_ev[cur].p, max_nodes_level, vtot, vgain,
                                                 m->d_group_first.p, m->d_group_size.p, m->d_nbins.p, m->d_has_missing.p,
                                                 b->d_qexp.p, p.qbits, dp, b->d_cands.p, cpn, ctl + cur, cs, b->d_seg[cur].p, s));
@@ -2088,50 +2060,27 @@ void grow_vector_tree(Booster* b, int slot, TreeStats& st) {
                                                b->d_pair_parent.p, b->d_seg[nxt].p, tree.parent, m->d_feat_byte.p, m->d_nbins.p,
                                                b->d_qexp.p, p.qbits, dp, vtot, vgain, b->d_ev[nxt].p, s));
     st.kernel_launches++;
-    const int32_t* ridx_in = d == 0 ? nullptr : b->ridx[cur].p;
-    if (d == D - 1) {   // the children are leaves: every row's leaf index (and without leaf_stream, the leaf sums)
+    if (d == D - 1) {   // every row's leaf index (and without leaf_stream, the leaf sums of every target)
       LAUNCH_CHECK(b2_launch_leaf_plan(b->d_leaves.p, &ctl[cur].leaf_base_next, b->d_seg_work.p, ctl + 2, s));
-      for (int k = 0; k < (leaf_stream ? 1 : T); ++k) {
-        const float2* ghk = b->gh.p + (size_t)k * n;
-        long long* sums = leaf_stream ? nullptr : b->d_vsums.p + (size_t)k * sums_stride;
-        LAUNCH_CHECK(b2_launch_leaf_sums(ghk, b->ridx[0].p, b->ridx[1].p, b->d_seg_work.p, ctl + 2, max_leaf_chunks,
-                                         b->d_qexp.p + 2 * k, 40, sums, b->pos.p, ctx->num_sms, s));
-        LAUNCH_CHECK(b2_launch_final_assign(m->bins_col.p, m->col_stride, ridx_in, b->d_split_work.p, ctl + cur,
-                                            max_part_chunks_total + max_nodes_level, ghk, b->d_qexp.p + 2 * k, 40, sums, b->pos.p,
-                                            0, ctx->num_sms, s));
-        st.kernel_launches += 2;
-      }
+      for (int k = 0; k < (leaf_stream ? 1 : T); ++k)
+        assign_leaves(b, st, d, b->gh.p + (size_t)k * n, b->d_qexp.p + 2 * k,
+                      leaf_stream ? nullptr : b->d_vsums.p + (size_t)k * sums_stride);
       st.kernel_launches++;
       mark_phase(b, 5);
       continue;
     }
-    const bool need_hist = d + 1 < D;
-    B2FinalizeArgs fin;
-    fin.ctl_nxt = ctl + nxt; fin.seg_nxt = b->d_seg[nxt].p; fin.ev_nxt = b->d_ev[nxt].p; fin.pair_parent_hist = b->d_pair_parent.p;
-    fin.hist_work = b->d_hist_work.p; fin.triples = b->d_triples.p; fin.stat_rows = d_level_rows + d + 1; fin.done = b->d_part_done.p;
-    fin.max_pairs = max_nodes_level; fin.need_hist = need_hist ? 1 : 0; fin.n_streams = n_streams; fin.window_rows = window;
-    fin.chunk_rows_override = p.hist_chunk_rows;
-    LAUNCH_CHECK(b2_launch_partition(m->bins_col.p, m->col_stride, ridx_in, b->ridx[nxt].p, b->d_split_work.p, ctl + cur,
-                                     max_part_chunks_total + max_nodes_level, b->d_counters.p, 0, fin, ctx->num_sms, s));
-    st.kernel_launches++;
+    partition_level(b, st, d);
     mark_phase(b, 5);
-    if (need_hist) {   // per target: built children, then siblings = parent - built over the target's whole slice
+    if (d + 1 < D) {   // per target: built children, then siblings = parent - built over the target's whole slice
       const int nh = hb ^ 1;
       for (int k = 0; k < T; ++k) {
         long long* tgt = b->d_vhist[nh].p + (size_t)k * tstride;
         CUDA_CHECK(cudaMemsetAsync(tgt, 0, (size_t)max_nodes_level * b->node_elems * sizeof(long long), s));
-        cudaEvent_t e0 = nullptr, e1 = nullptr;
-        record_hist_launch(b, st, e0, e1, true);
-        LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, b->q.p + (size_t)k * n, b->ridx[nxt].p, b->d_hist_work.p, 0, 0, 0, window,
-                                    G, tgt, ctl + nxt, 0, max_nodes_level, ctx->num_sms, s));
-        record_hist_launch(b, st, e0, e1, false);
-        allreduce(b->comm, tgt, (size_t)max_nodes_level * b->node_elems, kNcclInt64, kNcclSum, s);   // the built children
-        if (multi) st.allreduce_bytes += max_nodes_level * node_bytes;
-        LAUNCH_CHECK(b2_launch_hist_subtract(b->d_vhist[hb].p + (size_t)k * tstride, tgt, b->d_triples.p, max_nodes_level,
-                                             (int64_t)b->slice_elems, ctl + nxt, s));
-        st.hist_launches++; st.kernel_launches += 2;
+        launch_hist(b, st, b->q.p + (size_t)k * n, b->ridx[nxt].p, ctl + nxt, max_nodes_level, tgt);
+        mark_phase(b, 1);
+        exchange_and_subtract(b, st, b->d_vhist[hb].p + (size_t)k * tstride, tgt, b->d_triples.p, ctl + nxt, max_nodes_level,
+                              max_nodes_level);
       }
-      mark_phase(b, 1);
       hb = nh;
     }
   }
@@ -2997,9 +2946,7 @@ void refresh_tree(Booster* b, int k, int slot, int src) {
   b->t.refresh_launches++;
   allreduce(b->comm, b->d_rsums.p, 4 * (size_t)rt.n_leaves, kNcclInt64, kNcclSum, s);   // limb by limb: exact
   if (b->comm && b->comm->world > 1) b->t.allreduce_bytes += 4.0 * rt.n_leaves * 8;
-  B2CtlParams cp;
-  cp.mcw = (double)p.min_child_weight; cp.lambda = (double)p.lambda; cp.alpha = (double)p.alpha;
-  cp.max_delta_step = (double)p.max_delta_step; cp.gamma = p.gamma; cp.eta = p.eta / (float)p.num_parallel_tree;
+  const B2CtlParams cp = ctl_params(p);
   LAUNCH_CHECK(b2_launch_refresh_nodes(nodes, rt.n_nodes, b->d_rorder.p + rt.order_off, b->d_rlevels.p + rt.level_off, rt.n_levels,
                                        b->d_rsums.p, b->d_qexp.p, 40, cp, p.refresh_leaf ? 1 : 0, b->d_rlimbs.p, b->d_rblock.p,
                                        b->d_rleaf.p, s));

@@ -209,32 +209,8 @@ leaf_sums_kernel(const float2* __restrict__ gh, const int32_t* __restrict__ ridx
   }
 }
 
-// margin[row*K + k] += leaf_value[leaf]
-__global__ void __launch_bounds__(256)
-pred_update_kernel(float* __restrict__ margin, int K, int k, const int32_t* __restrict__ ridx0,
-                   const int32_t* __restrict__ ridx1, const SegWork* __restrict__ work, const B2LevelCtl* __restrict__ ctl,
-                   const float* __restrict__ leaf_value) {
-  const int n_work = ctl->hist_n_work, total_chunks = ctl->hist_total_chunks;
-  for (int chunk = blockIdx.x; chunk < total_chunks; chunk += gridDim.x) {
-    int lo = 0, hi = n_work - 1;
-    while (lo < hi) {
-      int mid = (lo + hi + 1) >> 1;
-      if (__ldg(&work[mid].chunk_begin) <= chunk) lo = mid; else hi = mid - 1;
-    }
-    const SegWork w = work[lo];
-    const int32_t* ridx = w.pad0 ? nullptr : (w.buf ? ridx1 : ridx0);
-    const int row0 = (chunk - w.chunk_begin) * kPartChunk;
-    const int nrows = min(kPartChunk, w.seg_count - row0);
-    const float v = __ldg(leaf_value + w.id);
-    for (int r = threadIdx.x; r < nrows; r += blockDim.x) {
-      const int64_t row = ridx ? __ldg(ridx + w.seg_begin + row0 + r) : (w.seg_begin + row0 + r);
-      margin[row * K + k] += v;
-    }
-  }
-}
-
 // ---- last split level (d = max_depth - 1): the children are leaves, so their rows need no ordered index list any
-// more.  Instead of partition -> finalize -> leaf_sums -> pred_update (three scattered passes over all rows) one pass
+// more.  Instead of a partition, a leaf-sum pass and a margin pass (three scattered passes over all rows) one pass
 // decides left/right, adds the row's fp32 gradient pair to the 40-bit fixed-point sums of the child LEAF and records
 // the leaf index of the row; the margin is then updated by a streaming kernel (margin_update_kernel).
 // Leaf index of child `side` of split j: leaf_base + 2 j + side -- exactly the index decide_kernel gives the node at
@@ -411,7 +387,7 @@ __global__ void iota_kernel(int32_t* out, int64_t n) {
 }  // namespace b2
 
 extern "C" {
-int b2_part_chunk_rows() { return b2::kPartChunk; }     // leaf-segment work items (leaf_sums / pred_update)
+int b2_part_chunk_rows() { return b2::kPartChunk; }     // leaf-segment work items (leaf_sums)
 int b2_split_chunk_rows() { return b2::kSplitChunk; }   // split-node work items (partition / final_assign)
 
 // partition + finalize of a level: `fin` is what the last CTA writes (level_finalize.cuh)
@@ -485,13 +461,6 @@ int b2_launch_margin_update_vector(float* margin, int T, const uint16_t* pos, co
   int64_t want = (n + 255) / 256;
   int grid = (int)(want < (int64_t)num_sms * 16 ? want : (int64_t)num_sms * 16);
   b2::margin_update_vector_kernel<<<grid, 256, 0, stream>>>(margin, T, pos, leaf_vec, n);
-  return (int)cudaGetLastError();
-}
-int b2_launch_pred_update(float* margin, int K, int k, const int32_t* ridx0, const int32_t* ridx1, const void* work,
-                          const B2LevelCtl* ctl, int max_chunks, const float* leaf_value, int num_sms, cudaStream_t stream) {
-  if (max_chunks <= 0) return 0;
-  int grid = max_chunks < num_sms * 8 ? max_chunks : num_sms * 8;
-  b2::pred_update_kernel<<<grid, 256, 0, stream>>>(margin, K, k, ridx0, ridx1, (const b2::SegWork*)work, ctl, leaf_value);
   return (int)cudaGetLastError();
 }
 int b2_launch_iota(int32_t* out, int64_t n, cudaStream_t stream) {
