@@ -53,7 +53,9 @@ def _select(seed, tree, scope, parent, fwq, n_features, frac):
 class _P:
     """the OrParams fields the growth reads, as the C code sees them (binary32 values widened to double)"""
 
-    def __init__(self, params):
+    def __init__(self, params, rows_sampled=False):
+        """rows_sampled: the caller applies the row draw itself (tests/multi_output_reference.py), so subsample < 1 is
+        accepted; here it raises"""
         p = O.make_params(params)
         self.raw = p
         self.max_depth, self.qbits, self.K = p.max_depth, p.qbits, p.num_class
@@ -62,8 +64,8 @@ class _P:
                                                                             p.max_delta_step))
         self.bytree, self.bylevel, self.bynode = (float(F32(v)) for v in (p.colsample_bytree, p.colsample_bylevel,
                                                                           p.colsample_bynode))
-        self.seed = p.seed
-        if p.subsample < 1.0:
+        self.seed, self.rank, self.subsample = p.seed, p.rank, float(F32(p.subsample))
+        if p.subsample < 1.0 and not rows_sampled:
             raise NotImplementedError("row subsampling is not restated here")
         if self.qbits <= 0:
             raise NotImplementedError("only the fixed-point histograms are restated here")

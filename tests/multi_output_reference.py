@@ -9,9 +9,14 @@ oracle.hist_int per target, or_select_features), restated for T targets with the
     a backward scan on f when f's real-bin sums differ from the node totals for some target;
   * the winner expands when loss_chg > 1e-6, !(loss_chg < gamma) and each child has a nonzero hessian sum in some target;
   * leaf value of target k = fp32(fp32(CalcWeight) * eta) from the 40-bit fixed-point sums of the leaf's rows; an internal
-    node's vector holds the same formula on its qbits sums.
-With T = 1 and min_child_weight = 0 this is the oracle's scalar tree (tests/test_multi_output_reference.py checks it).
-Row subsampling and categorical features are not restated."""
+    node's vector holds the same formula on its qbits sums;
+  * row subsampling (the oracle's draw, restated in row_keep): a row is kept for tree t iff
+    hash4(seed, t, rank, row) < subsample * 2^32; a dropped row keeps its place in the partition and receives the leaf
+    vector, but carries (0, 0) in every target, before the quantisation exponents are taken.
+predict_margin / pred_leaf walk the trees on raw binary32 values: a missing value (NaN, or equal to a non-NaN `missing`)
+follows default_left, any other value goes left when x < split_cond; each tree's leaf vector is added in binary32.
+With T = 1 and min_child_weight = 0 this is the oracle's scalar tree and prediction (tests/test_multi_output_reference.py
+checks both).  Categorical features are not restated."""
 from types import SimpleNamespace
 
 import numpy as np
@@ -19,9 +24,31 @@ import numpy as np
 from oracle import oracle as O
 from tests import multi_target_reference as MT
 from tests.interaction_reference import (LEAF_BITS, MISSING_BIN, RT_EPS, SCOPE_LEVEL0, SCOPE_NODE0, SCOPE_TREE, _P,
-                                         _first_max, _select, allowed_features)
+                                         _select, allowed_features)
 
 F32 = np.float32
+_M64 = (1 << 64) - 1
+
+
+def _mix64(x):
+    """hist_oracle.c mix64 on a uint64 array (wrapping multiplies)"""
+    x = x ^ (x >> np.uint64(30))
+    x = x * np.uint64(0xbf58476d1ce4e5b9)
+    x = x ^ (x >> np.uint64(27))
+    x = x * np.uint64(0x94d049bb133111eb)
+    return x ^ (x >> np.uint64(31))
+
+
+def row_keep(seed, tree, rank, n, subsample):
+    """the oracle's row draw for one tree: keep row i iff hash4(seed, tree, rank, i) < subsample * 2^32 (subsample as
+    binary32 widened to double; a threshold at or past 2^32 - 1 keeps every row)"""
+    thr_d = float(F32(subsample)) * 4294967296.0
+    thr = 0xFFFFFFFF if thr_d >= 4294967295.0 else int(thr_d)
+    h0 = ((seed & 0xFFFFFFFF) * 0x9e3779b97f4a7c15 + (tree & 0xFFFFFFFF)) & _M64
+    h = _mix64(np.full(n, h0, np.uint64))
+    h = _mix64(h + np.uint64(rank & 0xFFFFFFFF))
+    h = _mix64(h + np.arange(n, dtype=np.uint64))
+    return (h >> np.uint64(32)) < np.uint64(thr)
 
 
 def node_gain(p, G, H):
@@ -41,47 +68,65 @@ def _acc_gain(p, Gs, Hs):
 
 
 def best_split(p, cuts, hists, sg, sh, inv_g, inv_h, feats):
-    """the first candidate of the largest finite loss_chg > 0 (feature ascending; forward bins ascending, backward bins
-    descending); hists[k] = target k's integer histogram [F][256][2]"""
+    """the first candidate of the largest finite loss_chg > 0 in enumeration order (feature ascending; per feature the
+    forward bins ascending, then the backward bins descending); hists[k] = target k's integer histogram [F][256][2].
+    Every feature's candidates are formed at once as [features][256] arrays, element by element with the operations of
+    the per-feature scan, so each loss_chg is the same binary32 value; the enumeration order is the flattened order of
+    [forward bins | backward bins reversed] per feature, and np.argmax keeps the first of equal maxima."""
     T = len(hists)
     G = [sg[k] * inv_g[k] for k in range(T)]
     H = [sh[k] * inv_h[k] for k in range(T)]
     parent_gain = float(F32(node_gain(p, G, H)))
-    best = None
-    for f in sorted(feats):
-        nf = int(cuts.ptrs[f + 1] - cuts.ptrs[f])
-        if nf <= 0:
-            continue
-        cg = [np.cumsum(hists[k][f, :nf, 0]) for k in range(T)]
-        ch = [np.cumsum(hists[k][f, :nf, 1]) for k in range(T)]
+    fa = np.array(sorted(feats), np.int64)
+    if fa.size == 0:
+        return None
+    nf = (cuts.ptrs[fa + 1] - cuts.ptrs[fa]).astype(np.int64)
+    fa, nf = fa[nf > 0], nf[nf > 0]
+    if fa.size == 0:
+        return None
+    real = np.arange(256)[None, :] < nf[:, None]               # the feature's real bins
+    hg = [np.where(real, hists[k][fa, :, 0], 0) for k in range(T)]
+    hh = [np.where(real, hists[k][fa, :, 1], 0) for k in range(T)]
+    cg = [np.cumsum(a, axis=1) for a in hg]
+    ch = [np.cumsum(a, axis=1) for a in hh]
+    tg = [a[:, -1:] for a in cg]                                # sums over the real bins
+    th = [a[:, -1:] for a in ch]
+    with np.errstate(all="ignore"):
         # forward: left = bins <= i, missing -> right
         lg = [cg[k] * inv_g[k] for k in range(T)]
         lh = [ch[k] * inv_h[k] for k in range(T)]
-        chg = ((_acc_gain(p, lg, lh) + _acc_gain(p, [G[k] - lg[k] for k in range(T)],
-                                                  [H[k] - lh[k] for k in range(T)])) - parent_gain).astype(F32)
-        nz_l = np.any([ch[k] != 0 for k in range(T)], axis=0)
-        nz_r = np.any([(sh[k] - ch[k]) != 0 for k in range(T)], axis=0)
-        i = _first_max(chg, np.ones(nf, bool))
-        if i is not None and (best is None or chg[i] > best["chg"]):
-            best = dict(chg=chg[i], feature=f, bin=i, cond=float(cuts.vals[cuts.ptrs[f] + i]), default_left=0,
-                        nz_l=bool(nz_l[i]), nz_r=bool(nz_r[i]))
-        if any(cg[k][-1] != sg[k] or ch[k][-1] != sh[k] for k in range(T)):   # backward: missing -> left
-            bgi = [cg[k][-1] - np.concatenate([[0], cg[k][:-1]]) for k in range(T)]
-            bhi = [ch[k][-1] - np.concatenate([[0], ch[k][:-1]]) for k in range(T)]
-            rg = [bgi[k] * inv_g[k] for k in range(T)]
-            rh = [bhi[k] * inv_h[k] for k in range(T)]
-            chg = ((_acc_gain(p, [G[k] - rg[k] for k in range(T)], [H[k] - rh[k] for k in range(T)])
-                    + _acc_gain(p, rg, rh)) - parent_gain).astype(F32)
-            nz_l = np.any([(sh[k] - bhi[k]) != 0 for k in range(T)], axis=0)
-            nz_r = np.any([bhi[k] != 0 for k in range(T)], axis=0)
-            j = _first_max(chg[::-1], np.ones(nf, bool))
-            if j is not None:
-                i = nf - 1 - j
-                if best is None or chg[i] > best["chg"]:
-                    cond = float(cuts.mins[f]) if i == 0 else float(cuts.vals[cuts.ptrs[f] + i - 1])
-                    best = dict(chg=chg[i], feature=f, bin=i - 1, cond=cond, default_left=1, nz_l=bool(nz_l[i]),
-                                nz_r=bool(nz_r[i]))
-    return best
+        chg_f = ((_acc_gain(p, lg, lh) + _acc_gain(p, [G[k] - lg[k] for k in range(T)],
+                                                    [H[k] - lh[k] for k in range(T)])) - parent_gain).astype(F32)
+        nzl_f = np.any([ch[k] != 0 for k in range(T)], axis=0)
+        nzr_f = np.any([(sh[k] - ch[k]) != 0 for k in range(T)], axis=0)
+        # backward at bin i: right = real bins >= i, missing -> left; only where some target has missing sums
+        bgi = [tg[k] - (cg[k] - hg[k]) for k in range(T)]
+        bhi = [th[k] - (ch[k] - hh[k]) for k in range(T)]
+        rg = [bgi[k] * inv_g[k] for k in range(T)]
+        rh = [bhi[k] * inv_h[k] for k in range(T)]
+        chg_b = ((_acc_gain(p, [G[k] - rg[k] for k in range(T)], [H[k] - rh[k] for k in range(T)])
+                  + _acc_gain(p, rg, rh)) - parent_gain).astype(F32)
+        nzl_b = np.any([(sh[k] - bhi[k]) != 0 for k in range(T)], axis=0)
+        nzr_b = np.any([bhi[k] != 0 for k in range(T)], axis=0)
+    back = np.any([(tg[k][:, 0] != sg[k]) | (th[k][:, 0] != sh[k]) for k in range(T)], axis=0)
+
+    def usable(chg, ok):
+        return np.where(ok & np.isfinite(chg) & (chg > F32(0.0)), chg.astype(np.float64), -np.inf)
+
+    cand = np.concatenate([usable(chg_f, real), usable(chg_b, real & back[:, None])[:, ::-1]], axis=1)
+    flat = int(np.argmax(cand))
+    j, c = divmod(flat, 512)
+    if cand[j, c] == -np.inf:
+        return None
+    f = int(fa[j])
+    if c < 256:
+        i = c
+        return dict(chg=chg_f[j, i], feature=f, bin=i, cond=float(cuts.vals[cuts.ptrs[f] + i]), default_left=0,
+                    nz_l=bool(nzl_f[j, i]), nz_r=bool(nzr_f[j, i]))
+    i = 511 - c
+    cond = float(cuts.mins[f]) if i == 0 else float(cuts.vals[cuts.ptrs[f] + i - 1])
+    return dict(chg=chg_b[j, i], feature=f, bin=i - 1, cond=cond, default_left=1, nz_l=bool(nzl_b[j, i]),
+                nz_r=bool(nzr_b[j, i]))
 
 
 def grow_tree(p, cuts, bins, g, h, sets, tree_index, fwq=None):
@@ -89,6 +134,9 @@ def grow_tree(p, cuts, bins, g, h, sets, tree_index, fwq=None):
     n, F = bins.shape
     T = g.shape[1]
     g, h = np.ascontiguousarray(g, F32), np.ascontiguousarray(h, F32)
+    if p.subsample < 1.0:   # one draw for the tree: the dropped rows carry (0, 0) in every target
+        keep = row_keep(p.seed, tree_index, p.rank, n, p.subsample)[:, None]
+        g, h = np.where(keep, g, F32(0.0)), np.where(keep, h, F32(0.0))
     q = [(O.quantize(g[:, k], p.qbits), O.quantize(h[:, k], p.qbits)) for k in range(T)]
     qg, qh = [a[0][0] for a in q], [a[1][0] for a in q]
     eg, eh = [a[0][1] for a in q], [a[1][1] for a in q]
@@ -187,8 +235,10 @@ def grow_tree(p, cuts, bins, g, h, sets, tree_index, fwq=None):
 
 
 class Model:
-    def __init__(self, trees, margin, base_score):
-        self._trees, self.margin, self.base_score = trees, margin, base_score
+    """the trees, the train margins [n][T], base_score and the margin every row starts from (base_value)"""
+
+    def __init__(self, trees, margin, base_score, base_value):
+        self._trees, self.margin, self.base_score, self.base_value = trees, margin, base_score, base_value
 
     @property
     def num_trees(self):
@@ -198,10 +248,49 @@ class Model:
         return self._trees[i]
 
 
+def _tree_range(model, iteration_range):
+    if iteration_range is None or tuple(iteration_range) == (0, 0):
+        return 0, model.num_trees
+    return int(iteration_range[0]), int(iteration_range[1])
+
+
+def pred_leaf(model, X, missing=np.nan, iteration_range=None):
+    """[n][trees] leaf node ids of the raw binary32 rows X: a missing value (NaN, or == missing when missing is not NaN;
+    -0.0 == 0.0) follows default_left, any other value goes left when x < split_cond"""
+    X = np.ascontiguousarray(X, F32)
+    n = X.shape[0]
+    rows = np.arange(n)
+    b, e = _tree_range(model, iteration_range)
+    out = np.zeros((n, e - b), np.int32)
+    for j, t in enumerate(model._trees[b:e]):
+        nid = np.zeros(n, np.int64)
+        while True:
+            inner = t.split_feature[nid] >= 0
+            if not inner.any():
+                break
+            x = X[rows, np.maximum(t.split_feature[nid], 0)]
+            miss = np.isnan(x) if np.isnan(missing) else (np.isnan(x) | (x == F32(missing)))
+            left = np.where(miss, t.default_left[nid] != 0, x < t.split_cond[nid])
+            nid = np.where(inner, np.where(left, t.left[nid], t.right[nid]), nid)
+        out[:, j] = nid
+    return out
+
+
+def predict_margin(model, X, missing=np.nan, iteration_range=None):
+    """[n][T] margins: base_value plus each tree's leaf vector, added in binary32 one tree at a time in tree order"""
+    leaves = pred_leaf(model, X, missing, iteration_range)
+    b, _ = _tree_range(model, iteration_range)
+    T = model.tree(0).leaf_vector.shape[1]
+    out = np.full((leaves.shape[0], T), F32(model.base_value), F32)
+    for j in range(leaves.shape[1]):
+        out = (out + model.tree(b + j).leaf_vector[leaves[:, j]]).astype(F32)
+    return out
+
+
 def train(params, X, Y, rounds, weight=None, sets=None, feature_weights=None, gradients=None, base_margin=None):
     """`rounds` vector-leaf trees on numeric X with the label Y [n][T] (one of the multi-target objectives of
     tests/multi_target_reference.py), or with gradients(margin [n][T]) -> (g, h) [n][T] (a custom objective)."""
-    p = _P({k: v for k, v in params.items() if k not in ("multi_strategy", "objective", "base_score")})
+    p = _P({k: v for k, v in params.items() if k not in ("multi_strategy", "objective", "base_score")}, rows_sampled=True)
     X = np.ascontiguousarray(X, F32)
     Y = np.ascontiguousarray(Y, F32)
     n, T = Y.shape
@@ -214,10 +303,11 @@ def train(params, X, Y, rounds, weight=None, sets=None, feature_weights=None, gr
     if feature_weights is not None:
         qf = np.asarray(feature_weights, np.float64) * 65536.0
         fwq = np.where(qf >= 4294967295.0, 0xFFFFFFFF, np.rint(qf)).astype(np.uint32)
+    base_value = F32(b) if gradients is not None else F32(MT.base_margin_of(obj, b))
     if base_margin is not None:
         margin = np.array(np.asarray(base_margin, F32).reshape(n, T), F32)
     else:
-        margin = np.full((n, T), F32(b) if gradients is not None else MT.base_margin_of(obj, b), F32)
+        margin = np.full((n, T), base_value, F32)
     trees = []
     for r in range(rounds):
         if gradients is None:
@@ -229,7 +319,7 @@ def train(params, X, Y, rounds, weight=None, sets=None, feature_weights=None, gr
                                r, fwq)
         trees.append(tree)
         margin = (margin + leaf).astype(F32)
-    return Model(trees, margin, b)
+    return Model(trees, margin, b, base_value)
 
 
 def assert_engine_matches(bst, ref, leaf_tol=1e-5):

@@ -74,6 +74,90 @@ def test_duplicated_targets_double_the_oracle(extra, weighted):
         assert np.array_equal(r.leaf_vector[leaf, 1], o.value[leaf])
 
 
+SAMPLED = [
+    {"subsample": 0.5, "seed": 11},
+    {"subsample": 0.8, "colsample_bynode": 0.6, "seed": 4},
+]
+
+
+@pytest.mark.parametrize("extra", SAMPLED)
+def test_one_target_subsampled_is_the_oracle_tree(extra):
+    X, y = data(n=4000, seed=9)
+    params = dict({"objective": "reg:squarederror", "max_depth": 6, "eta": 0.3, "min_child_weight": 0,
+                   "base_score": 0.5}, **extra)
+    obst, _ = O.train(params, X, y, 4)
+    ref = R.train(params, X, y[:, None], 4)
+    for i in range(4):
+        o, r = obst.tree(i), ref.tree(i)
+        same_tree(o, r)
+        assert np.array_equal(o.loss_chg, r.loss_chg)
+        leaf = o.split_feature < 0
+        assert np.max(np.abs(o.value[leaf] - r.leaf_vector[leaf, 0])) <= 1e-6
+    assert np.max(np.abs(obst.margin.reshape(-1) - ref.margin[:, 0])) <= 1e-6
+    # the draw drops rows: a tree without it is a different tree
+    full = R.train(dict(params, subsample=1.0), X, y[:, None], 1)
+    assert full.tree(0).n_nodes != ref.tree(0).n_nodes or not np.array_equal(full.tree(0).loss_chg, ref.tree(0).loss_chg)
+
+
+def test_row_draw_keeps_the_fraction():
+    keep = R.row_keep(7, 3, 0, 200000, 0.3)
+    assert abs(keep.mean() - 0.3) < 0.005
+    assert not np.array_equal(keep, R.row_keep(7, 4, 0, 200000, 0.3))   # a new draw per tree
+    assert R.row_keep(7, 3, 0, 1000, 1.0).all()
+
+
+def held_out_rows(trees, n=3000, f=8, seed=31):
+    """rows with NaN, +-inf and every split condition of the trees placed in its feature (and next to it)"""
+    X, _ = data(n=n, f=f, seed=seed, nan_frac=0.05)
+    rng = np.random.RandomState(seed)
+    X[rng.uniform(size=X.shape) < 0.03] = np.inf
+    X[rng.uniform(size=X.shape) < 0.03] = -np.inf
+    i = 0
+    for t in trees:
+        for nid in np.nonzero(t.split_feature >= 0)[0]:
+            c = F32(t.split_cond[nid])
+            for v in (c, np.nextafter(c, F32(-np.inf)), np.nextafter(c, F32(np.inf))):
+                X[i % n, t.split_feature[nid]] = v
+                i += 1
+    return X
+
+
+@pytest.mark.parametrize("missing", [np.nan, -999.0])
+def test_one_target_predict_is_the_oracle_predict(missing):
+    X, y = data(n=4000, seed=12)
+    params = {"objective": "reg:squarederror", "max_depth": 6, "eta": 0.3, "min_child_weight": 0, "base_score": 0.5}
+    obst, _ = O.train(params, X, y, 4)
+    ref = R.train(params, X, y[:, None], 4)
+    Xt = held_out_rows([ref.tree(i) for i in range(4)])
+    if not np.isnan(missing):
+        Xt[np.random.RandomState(2).uniform(size=Xt.shape) < 0.05] = missing
+    want = obst.predict_margin(Xt, missing=missing)
+    got = R.predict_margin(ref, Xt, missing=missing)
+    assert np.array_equal(got.view(np.uint32), want.view(np.uint32))
+    for b, e in ((0, 2), (2, 4)):
+        assert np.array_equal(R.predict_margin(ref, Xt, missing=missing, iteration_range=(b, e)).view(np.uint32),
+                              obst.predict_margin(Xt, missing=missing, tree_begin=b, tree_end=e).view(np.uint32))
+    leaves = R.pred_leaf(ref, Xt, missing=missing)
+    assert leaves.shape == (len(Xt), 4)
+    assert all((ref.tree(i).split_feature[leaves[:, i]] < 0).all() for i in range(4))
+
+
+def test_duplicated_targets_subsampled_double_inside_the_reference():
+    X, y = data(seed=17)
+    params = {"objective": "reg:squarederror", "max_depth": 6, "eta": 0.3, "min_child_weight": 0, "gamma": 0,
+              "base_score": 0.5, "subsample": 0.6, "seed": 8}
+    one = R.train(params, X, y[:, None], 3)
+    two = R.train(params, X, np.stack([y, y], 1), 3)
+    for i in range(3):
+        o, r = one.tree(i), two.tree(i)
+        assert not np.any((o.loss_chg > 5e-7) & (o.loss_chg <= 1e-6))
+        same_tree(o, r)
+        assert np.array_equal(r.loss_chg, F32(2) * o.loss_chg)
+        assert np.array_equal(r.leaf_vector[:, 0], o.leaf_vector[:, 0])
+        assert np.array_equal(r.leaf_vector[:, 1], o.leaf_vector[:, 0])
+    assert np.array_equal(two.margin[:, 0], one.margin[:, 0]) and np.array_equal(two.margin[:, 1], one.margin[:, 0])
+
+
 def test_hand_computed_two_targets():
     # one feature, four rows with values 0..3; target 0 wants the split 0|123, target 1 the split 012|3; summed, the
     # first of the two tied best candidates wins (hand computation below); squared error at margin 0, lambda = 0, eta = 1
