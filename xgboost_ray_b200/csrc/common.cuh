@@ -105,7 +105,7 @@ struct B2TreeNodeDev {
 // one path: element 0 is the bias (feature -1), then one element per DISTINCT feature on the root -> leaf path, the
 // repeated splits on it merged: numeric splits into an interval, categorical splits into an intersected category set,
 // missing values into one flag (missing follows the path only if every merged split sends it that way).
-#define B2_SHAP_MAX_PATH 16            // bias + at most 14 distinct features (max_depth <= 14) + slack
+#define B2_SHAP_MAX_PATH 32            // bias + at most 31 distinct features: one warp (max_depth <= 16 needs 17)
 #define B2_PATH_MISSING_OK 1u          // a missing value follows the path
 #define B2_PATH_HAS_HI 2u              // numeric: x < hi is required
 #define B2_PATH_OUTSIDE_OK 4u          // categorical: a value outside [0, 256) follows the path

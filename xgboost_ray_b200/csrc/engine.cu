@@ -1359,7 +1359,8 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
          "process_type=update)", p->updater.c_str());
   }
   if (p->num_target_set) set_targets(p, p->num_target);
-  if (p->max_depth < 1 || p->max_depth > 14) fail("max_depth must be in [1, 14], got %d", p->max_depth);
+  // 16: a leaf index must fit the uint16_t row -> leaf map pos (2^16 leaves), DESIGN.md 9
+  if (p->max_depth < 1 || p->max_depth > 16) fail("max_depth must be in [1, 16], got %d", p->max_depth);
   if (p->num_parallel_tree < 1 || p->num_parallel_tree > 4096) fail("num_parallel_tree must be in [1, 4096], got %d", p->num_parallel_tree);
   if (p->qbits < 8 || p->qbits > 24) fail("hist_qbits must be in [8, 24], got %d", p->qbits);
   for (float v : {p->subsample, p->colsample_bytree, p->colsample_bylevel, p->colsample_bynode})
@@ -1526,6 +1527,34 @@ void p2p_setup(Booster* b) {
   st.enabled = true;
 }
 
+// feature-slot sharding of the histogram exchange: rank r owns slots s with s % shards == r (DESIGN.md 5)
+// (vector-leaf trees: every rank scans every slot of the allreduced T-target level buffer, no sharding)
+int hist_shards(const Booster* b) {
+  const int world = b->comm ? b->comm->world : 1;
+  return (world > 1 && world <= 32 && (32 % world) == 0 && !b->p.vector_leaf()) ? world : 1;
+}
+
+// The two level buffers hold 2^(D-1) nodes x n_groups x 128 KiB split over the shards, and a sharded exchange adds a
+// build buffer of 2^(D-1) nodes x n_groups x 128 KiB: 8 GiB at max_depth 16 with one feature group, far more for a
+// wide matrix.  A booster whose buffers do not fit in the device memory free now (the pool's cached blocks count as
+// free) is refused when it is created, before anything is allocated for it, rather than failing in cudaMalloc partway
+// through its first tree.  Vector-leaf trees have their own check (prepare_tree_buffers); update mode grows nothing.
+void check_level_memory(const Booster* b) {
+  if (b->p.vector_leaf() || b->p.update_mode) return;
+  const int D = b->p.max_depth, G = b->train->n_groups, shards = hist_shards(b);
+  const double half = (double)((size_t)1 << (D - 1)), node_bytes = (double)G * B2_GROUP_ELEMS * sizeof(long long);
+  const double need = 2.0 * half * node_bytes / shards + (shards > 1 ? half * node_bytes : 0.0);
+  size_t free_bytes = 0, total_bytes = 0;
+  CUDA_CHECK(cudaMemGetInfo(&free_bytes, &total_bytes));
+  int dev = 0; CUDA_CHECK(cudaGetDevice(&dev));
+  size_t cached = 0;
+  if (dev >= 0 && dev < 64) { std::lock_guard<std::mutex> lk(g_dev_pool[dev].mu); cached = g_dev_pool[dev].cached; }
+  const double avail = (double)free_bytes + (double)cached;
+  if (need > avail)
+    fail("max_depth %d with %d feature groups needs %.1f GiB of level histograms, and %.1f GiB of device memory is free; "
+         "use a smaller max_depth or fewer features", D, G, need / (double)(1ull << 30), avail / (double)(1ull << 30));
+}
+
 void ensure_ctl_tables(Booster* b) {
   const int D = b->p.max_depth; const int G = b->train->n_groups;
   if (b->ctl_depth == D) return;
@@ -1556,10 +1585,7 @@ void ensure_ctl_tables(Booster* b) {
   b->d_leaf_sums.ensure(4 * lcap); b->d_leaf_values.ensure(lcap);   // [leaf][g, h][hi, lo] limbs (common.cuh)
   if (b->ic_words > 0) b->d_ic_compat.ensure(L.max_nodes * (size_t)b->ic_words);
   b->node_elems = (size_t)G * B2_GROUP_ELEMS;
-  // feature-slot sharding of the histogram exchange: rank r owns slots s with s % shards == r (DESIGN.md 5)
-  const int world = b->comm ? b->comm->world : 1;
-  // (vector-leaf trees: every rank scans every slot of the allreduced T-target level buffer, no sharding)
-  b->shards = (world > 1 && world <= 32 && (32 % world) == 0 && !b->p.vector_leaf()) ? world : 1;
+  b->shards = hist_shards(b);
   b->log2_shards = 0; while ((1 << b->log2_shards) < b->shards) b->log2_shards++;
   b->sp = B2_GROUP_SLOTS / b->shards;
   b->slice_elems = (size_t)G * 2 * B2_BINS * b->sp;
@@ -2345,7 +2371,7 @@ void walk_paths(const TreeHost& t, int nid, std::vector<PathBuildElem>& path, in
                 std::vector<B2PathElem>& elems, std::vector<B2PathInfo>& infos, std::vector<uint32_t>& cats, double* expected) {
   if (t.feature[nid] < 0) {
     if (path.size() + 1 > B2_SHAP_MAX_PATH)
-      fail("tree %d has a leaf below %d distinct features; TreeSHAP supports at most %d (max_depth <= 14)", tree,
+      fail("tree %d has a leaf below %d distinct features; TreeSHAP supports at most %d distinct features on a path", tree,
            (int)path.size(), B2_SHAP_MAX_PATH - 1);
     B2PathInfo pi{(int32_t)elems.size(), (int32_t)path.size() + 1, cls, 0, (double)t.value[nid]};
     elems.push_back(B2PathElem{-1, -1, 0.f, 0.f, 0u, 0u, 1.0});
@@ -2707,8 +2733,9 @@ void drain_round(Booster* b) {
 
 // Update mode, before anything reads the train margin: the trees added so far become the trees to update and the model
 // starts empty (xgboost's gbtree moves them to trees_to_update).  Every tree is checked to be a proper binary tree
-// reachable from node 0 with at most 65,535 leaves, and copied to the device once: B2TreeNodeDev nodes whose pad holds
-// the compact leaf index (leaves numbered in node order), the category sets, and the node ids grouped by depth.
+// reachable from node 0 with at most 65,536 leaves (compact indices 0..65,535 fit pos), and copied to the device once:
+// B2TreeNodeDev nodes whose pad holds the compact leaf index (leaves numbered in node order), the category sets, and
+// the node ids grouped by depth.
 void begin_update(Booster* b) {
   if (!b->p.update_mode || b->update_started) return;
   drain_round(b);
@@ -2729,7 +2756,7 @@ void begin_update(Booster* b) {
     std::vector<int32_t> leaf_of(nn, -1), depth(nn, -1);
     int n_leaves = 0;
     for (int i = 0; i < nn; ++i) if (t.feature[i] < 0) leaf_of[i] = n_leaves++;
-    if (n_leaves > 65535) fail("tree %zu has %d leaves; the refresh updater supports at most 65535", ti, n_leaves);
+    if (n_leaves > 65536) fail("tree %zu has %d leaves; the refresh updater supports at most 65536", ti, n_leaves);
     // breadth-first from the root: every node reached exactly once, splits with two children, leaves with none
     std::vector<int32_t> bfs{0}; depth[0] = 0;
     for (size_t q = 0; q < bfs.size(); ++q) {
@@ -3641,6 +3668,7 @@ int B2_BoosterCreate(const char* params, B2Handle trainh, B2Handle commh, B2Hand
         fail("multi_strategy=multi_output_tree is not supported with categorical features (the train matrix has %zu)",
              m->cat_feats.size());
       b->ctx = m->ctx; b->n_features = m->F; CUDA_CHECK(cudaSetDevice(m->ctx->device));
+      check_level_memory(b);
       if (!b->p.interaction_sets.empty()) {   // sets_of[f] bit k: feature f is in set k
         const int W = (int)((b->p.interaction_sets.size() + 63) / 64);
         std::vector<unsigned long long> sets_of((size_t)m->F * W, 0ull);

@@ -8,8 +8,11 @@
 // its elements, the EXTEND recurrence runs across them with shuffles, and every lane then UNWINDS its own element.
 //
 // Warp mapping and determinism (DESIGN.md 4.6): a warp owns one row at a time and walks the path list of the tree
-// range in order, two paths at once (half-warps of 16 lanes).  Contributions are accumulated in double in the warp's
-// own accumulator -- shared memory for pred_contribs, the row's slice of a global scratch block for interactions (up to
+// range in order.  Paths of at most 16 elements go two at a time (half-warps of 16 lanes); a path of 17..32 elements
+// (max_depth 16, or a deep model loaded from JSON) takes the whole warp on its own, and so does a short path whose
+// successor is long.  Which width a path runs at depends only on the path table, and a path's values do not depend on
+// it: lanes past its length never change the recurrences.  Contributions are accumulated in double in the warp's own
+// accumulator -- shared memory for pred_contribs, the row's slice of a global scratch block for interactions (up to
 // K (F+1)^2 doubles, far beyond shared memory) -- by plain read-modify-writes in a fixed order (half 0 before half 1,
 // path after path), so the result is bit-identical from call to call and independent of how rows are sharded.  There
 // are no atomics; each output value is written once per row.
@@ -41,15 +44,16 @@ __device__ __forceinline__ double path_one_fraction(const B2PathElem& e, const f
   return (v >= e.lo && (!(e.flags & B2_PATH_HAS_HI) || v < e.hi)) ? 1.0 : 0.0;
 }
 
-// EXTEND over elements 1..L-1 of this half-warp's path (element 0, the bias, starts the path with weight 1), leaving
+// EXTEND over elements 1..L-1 of this W-lane group's path (element 0, the bias, starts the path with weight 1), leaving
 // out element `skip` (-1: none).  Lane s returns the permutation weight of position s; positions are compacted past
-// `skip`.  Every lane of the warp calls this with the same Lmax = max(L) of the two halves.
+// `skip`.  Every lane of the warp calls this with the same Lmax = max(L) of the warp's groups.
+template <int W>
 __device__ __forceinline__ double path_extend(int sub, int L, int Lmax, double z, double o, int skip) {
   double w = sub == 0 ? 1.0 : 0.0;
   int pos = 0;
   for (int l = 1; l < Lmax; ++l) {
-    const double zl = __shfl_sync(kFull, z, l, kHalf), ol = __shfl_sync(kFull, o, l, kHalf);
-    const double wl = __shfl_up_sync(kFull, w, 1, kHalf);
+    const double zl = __shfl_sync(kFull, z, l, W), ol = __shfl_sync(kFull, o, l, W);
+    const double wl = __shfl_up_sync(kFull, w, 1, W);
     if (l < L && l != skip) {
       ++pos;
       if (sub <= pos)
@@ -61,12 +65,13 @@ __device__ __forceinline__ double path_extend(int sub, int L, int Lmax, double z
 
 // UNWOUND_PATH_SUM: total permutation weight of the path with this lane's element (z, o) removed, given the weights
 // w of the Lp positions.  A lane whose element has o = z = 0 contributes nothing and returns 0 (never 0/0).
+template <int W>
 __device__ __forceinline__ double path_unwound_sum(int Lp, int Lpmax, double w, double z, double o, bool active) {
   const int l = Lp - 1;
-  double next = __shfl_sync(kFull, w, l < 0 ? 0 : l, kHalf);
+  double next = __shfl_sync(kFull, w, l < 0 ? 0 : l, W);
   double total = 0.0;
   for (int j = Lpmax - 2; j >= 0; --j) {
-    const double wj = __shfl_sync(kFull, w, j, kHalf);
+    const double wj = __shfl_sync(kFull, w, j, W);
     if (active && j < l) {
       if (o != 0.0) {
         const double t = next * (double)(l + 1) / ((double)(j + 1) * o);
@@ -104,6 +109,70 @@ __device__ __forceinline__ PathLane load_path_lane(const B2PathElem* __restrict_
   return r;
 }
 
+// How the warp takes the paths from p on: 0 = path p alone on the full warp (more than 16 elements), 2 = paths p and
+// p + 1 on the two half-warps, 1 = path p on half 0 alone (the next path is long, or p is the last).  Warp-uniform.
+__device__ __forceinline__ int path_step(const B2PathInfo* __restrict__ paths, int p, int p_end) {
+  if (paths[p].len > kHalf) return 0;
+  return p + 1 < p_end && paths[p + 1].len <= kHalf ? 2 : 1;
+}
+
+// phi of one path per W-lane group (W = 16: group `part` of the warp holds path q; W = 32: part 0, the whole warp),
+// added to the row accumulator group by group in path order
+template <int W>
+__device__ __forceinline__ void contribs_path(double* acc, int F1, const B2PathElem* __restrict__ elems,
+                                              const B2PathInfo* __restrict__ paths, int q, int q_end, int sub, int part,
+                                              const float* __restrict__ x, float missing, int missing_is_nan,
+                                              const uint32_t* __restrict__ cat_table) {
+  const PathLane pl = load_path_lane(elems, paths, q, q_end, sub, x, missing, missing_is_nan, cat_table);
+  const int Lmax = W == 32 ? pl.L : max(pl.L, __shfl_xor_sync(kFull, pl.L, 16));
+  const double w = path_extend<W>(sub, pl.L, Lmax, pl.z, pl.o, -1);
+  const bool mine = sub > 0 && sub < pl.L;
+  const double s = path_unwound_sum<W>(pl.L, Lmax, w, pl.z, pl.o, mine);
+  const double c = s * (pl.o - pl.z) * pl.v;
+#pragma unroll
+  for (int h = 0; h < 32 / W; ++h) {
+    if (part == h && mine) acc[pl.cls * F1 + pl.e.feature] += c;
+    __syncwarp();
+  }
+}
+
+// Phi_ij of one path per W-lane group, as contribs_path: phi_i on the diagonal, then the conditioning elements in order
+template <int W>
+__device__ __forceinline__ void interactions_path(double* acc, size_t mat, int F1, const B2PathElem* __restrict__ elems,
+                                                  const B2PathInfo* __restrict__ paths, int q, int q_end, int sub, int part,
+                                                  const float* __restrict__ x, float missing, int missing_is_nan,
+                                                  const uint32_t* __restrict__ cat_table) {
+  const PathLane pl = load_path_lane(elems, paths, q, q_end, sub, x, missing, missing_is_nan, cat_table);
+  const int Lmax = W == 32 ? pl.L : max(pl.L, __shfl_xor_sync(kFull, pl.L, 16));
+  const bool mine = sub > 0 && sub < pl.L;
+  double* accc = acc + (size_t)pl.cls * mat;
+  {   // phi_i of the full path, kept on the diagonal until the final correction
+    const double w = path_extend<W>(sub, pl.L, Lmax, pl.z, pl.o, -1);
+    const double c = path_unwound_sum<W>(pl.L, Lmax, w, pl.z, pl.o, mine) * (pl.o - pl.z) * pl.v;
+#pragma unroll
+    for (int h = 0; h < 32 / W; ++h) {
+      if (part == h && mine) accc[(size_t)pl.e.feature * F1 + pl.e.feature] += c;
+      __syncwarp();
+    }
+  }
+  for (int cc = 1; cc < Lmax; ++cc) {
+    const bool has_c = cc < pl.L;
+    const double zc = __shfl_sync(kFull, pl.z, cc, W), oc = __shfl_sync(kFull, pl.o, cc, W);
+    const int fc = __shfl_sync(kFull, pl.e.feature, cc, W);
+    const int Lp = has_c ? pl.L - 1 : 0;
+    const int Lpmax = W == 32 ? Lp : max(Lp, __shfl_xor_sync(kFull, Lp, 16));
+    const double w = path_extend<W>(sub, has_c ? pl.L : 0, Lmax, pl.z, pl.o, cc);
+    const bool act = has_c && mine && sub != cc;
+    const double s = path_unwound_sum<W>(Lp, Lpmax, w, pl.z, pl.o, act);
+    const double val = 0.5 * s * (pl.o - pl.z) * pl.v * (oc - zc);
+#pragma unroll
+    for (int h = 0; h < 32 / W; ++h) {
+      if (part == h && act) accc[(size_t)fc * F1 + pl.e.feature] += val;
+      __syncwarp();
+    }
+  }
+}
+
 // pred_contribs: out [rows][K][F+1] (float), row r of the block is global row row0 + r
 __global__ void __launch_bounds__(256) shap_contribs_kernel(
     const float* __restrict__ X, int64_t row0, int64_t rows, int F, float missing, int missing_is_nan,
@@ -123,17 +192,14 @@ __global__ void __launch_bounds__(256) shap_contribs_kernel(
       acc[i] = f == F ? (double)(base_margin ? base_margin[row * K + k] : base_value) + bias_k[k] : 0.0;
     }
     __syncwarp();
-    for (int p = p_begin; p < p_end; p += 2) {
-      const PathLane pl = load_path_lane(elems, paths, p + half, p_end, sub, x, missing, missing_is_nan, cat_table);
-      const int Lmax = max(pl.L, __shfl_xor_sync(kFull, pl.L, 16));
-      const double w = path_extend(sub, pl.L, Lmax, pl.z, pl.o, -1);
-      const bool mine = sub > 0 && sub < pl.L;
-      const double s = path_unwound_sum(pl.L, Lmax, w, pl.z, pl.o, mine);
-      const double c = s * (pl.o - pl.z) * pl.v;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (half == h && mine) acc[pl.cls * F1 + pl.e.feature] += c;
-        __syncwarp();
+    for (int p = p_begin; p < p_end;) {
+      const int step = path_step(paths, p, p_end);
+      if (step == 0) {
+        contribs_path<32>(acc, F1, elems, paths, p, p + 1, lane, 0, x, missing, missing_is_nan, cat_table);
+        p += 1;
+      } else {
+        contribs_path<kHalf>(acc, F1, elems, paths, p + half, p + step, sub, half, x, missing, missing_is_nan, cat_table);
+        p += step;
       }
     }
     for (int i = lane; i < stride; i += 32) out[r * stride + i] = (float)acc[i];
@@ -163,35 +229,15 @@ __global__ void __launch_bounds__(256) shap_interactions_kernel(
     for (int k = lane; k < K; k += 32)
       acc[k * mat + (size_t)F * F1 + F] = (double)(base_margin ? base_margin[row * K + k] : base_value) + bias_k[k];
     __syncwarp();
-    for (int p = p_begin; p < p_end; p += 2) {
-      const PathLane pl = load_path_lane(elems, paths, p + half, p_end, sub, x, missing, missing_is_nan, cat_table);
-      const int Lmax = max(pl.L, __shfl_xor_sync(kFull, pl.L, 16));
-      const bool mine = sub > 0 && sub < pl.L;
-      double* accc = acc + (size_t)pl.cls * mat;
-      {   // phi_i of the full path, kept on the diagonal until the final correction
-        const double w = path_extend(sub, pl.L, Lmax, pl.z, pl.o, -1);
-        const double c = path_unwound_sum(pl.L, Lmax, w, pl.z, pl.o, mine) * (pl.o - pl.z) * pl.v;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (half == h && mine) accc[(size_t)pl.e.feature * F1 + pl.e.feature] += c;
-          __syncwarp();
-        }
-      }
-      for (int cc = 1; cc < Lmax; ++cc) {
-        const bool has_c = cc < pl.L;
-        const double zc = __shfl_sync(kFull, pl.z, cc, kHalf), oc = __shfl_sync(kFull, pl.o, cc, kHalf);
-        const int fc = __shfl_sync(kFull, pl.e.feature, cc, kHalf);
-        const int Lp = has_c ? pl.L - 1 : 0;
-        const int Lpmax = max(Lp, __shfl_xor_sync(kFull, Lp, 16));
-        const double w = path_extend(sub, has_c ? pl.L : 0, Lmax, pl.z, pl.o, cc);
-        const bool act = has_c && mine && sub != cc;
-        const double s = path_unwound_sum(Lp, Lpmax, w, pl.z, pl.o, act);
-        const double val = 0.5 * s * (pl.o - pl.z) * pl.v * (oc - zc);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (half == h && act) accc[(size_t)fc * F1 + pl.e.feature] += val;
-          __syncwarp();
-        }
+    for (int p = p_begin; p < p_end;) {
+      const int step = path_step(paths, p, p_end);
+      if (step == 0) {
+        interactions_path<32>(acc, mat, F1, elems, paths, p, p + 1, lane, 0, x, missing, missing_is_nan, cat_table);
+        p += 1;
+      } else {
+        interactions_path<kHalf>(acc, mat, F1, elems, paths, p + half, p + step, sub, half, x, missing, missing_is_nan,
+                                 cat_table);
+        p += step;
       }
     }
     for (int i = lane; i < K * F; i += 32) {
