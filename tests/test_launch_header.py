@@ -1,0 +1,88 @@
+"""The kernel launchers are declared once, in csrc/launch.h, and both sides compile against it.
+
+The launchers have C linkage, so a prototype kept apart from its definition links even when the two disagree, and the
+kernel then reads shifted arguments at run time.  With one header included by engine.cu and by every defining file, a
+mismatch is a compile error.  These checks keep it that way: every b2_* function a kernel file defines for the host is
+declared in the header and nowhere else."""
+import os
+import re
+
+CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "xgboost_ray_b200", "csrc")
+HEADER = "launch.h"
+
+
+def _source(name):
+    text = open(os.path.join(CSRC, name)).read()
+    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
+    return re.sub(r"//[^\n]*", "", text)
+
+
+def _extern_c_blocks(text):
+    for m in re.finditer(r'extern\s+"C"\s*\{', text):
+        depth, i = 1, m.end()
+        while depth:
+            depth += {"{": 1, "}": -1}.get(text[i], 0)
+            i += 1
+        yield text[m.end():i - 1]
+
+
+def _top_level(block):
+    """the text of an extern "C" block outside every function body"""
+    out, depth = [], 0
+    for c in block:
+        if c == "}":
+            depth -= 1
+        if depth == 0:
+            out.append(c)
+        if c == "{":
+            depth += 1
+    return "".join(out)
+
+
+def _defined(text):
+    names = set()
+    for block in _extern_c_blocks(text):
+        names.update(re.findall(r"\b(b2_\w+)\s*\([^;{}]*\)\s*\{", _top_level(block)))
+    return names
+
+
+def _declared(text):
+    names = set()
+    for block in _extern_c_blocks(text):
+        names.update(re.findall(r"\b(b2_\w+)\s*\([^;{}]*\)\s*;", _top_level(block)))
+    return names
+
+
+def _kernel_files():
+    return sorted(f for f in os.listdir(CSRC) if f.endswith(".cu"))
+
+
+def test_header_declares_exactly_the_defined_launchers():
+    defined = {}
+    for f in _kernel_files():
+        for name in _defined(_source(f)):
+            assert name not in defined, "%s is defined in both %s and %s" % (name, defined[name], f)
+            defined[name] = f
+    declared = _declared(_source(HEADER))
+    assert len(defined) >= 80
+    missing = sorted(set(defined) - declared)
+    assert not missing, "defined in an extern \"C\" block but not declared in %s: %s" % (
+        HEADER, ", ".join("%s (%s)" % (n, defined[n]) for n in missing))
+    stale = sorted(declared - set(defined))
+    assert not stale, "declared in %s but defined by no kernel file: %s" % (HEADER, ", ".join(stale))
+
+
+def test_defining_files_and_engine_include_the_header():
+    include = re.compile(r'^\s*#\s*include\s+"%s"' % re.escape(HEADER), re.M)
+    users = [f for f in _kernel_files() if _defined(_source(f))] + ["engine.cu"]
+    for f in users:
+        assert include.search(_source(f)), "%s does not include %s" % (f, HEADER)
+
+
+def test_engine_keeps_no_launcher_prototypes():
+    text = _source("engine.cu")
+    local = sorted(_declared(text) | _defined(text))
+    assert not local, "engine.cu declares launchers of its own: %s" % ", ".join(local)
+    # the only extern "C" block of engine.cu is the C ABI of include/b2hist.h
+    blocks = list(_extern_c_blocks(text))
+    assert len(blocks) == 1 and re.search(r"\bint\s+B2_BoosterCreate\s*\(", blocks[0])

@@ -4,6 +4,7 @@
 
 The .so and the object files are build products and stay out of git.
 """
+import glob
 import os
 import subprocess
 import sys
@@ -44,7 +45,9 @@ def _stale(target, deps):
 
 def build(force=False, verbose=False):
     os.makedirs(OBJ_DIR, exist_ok=True)
-    headers = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "hist_common.cuh"), os.path.join(CSRC, "sampling.cuh"), os.path.join(CSRC, "p2p.cuh"), os.path.join(CSRC, "level_finalize.cuh"), os.path.join(CSRC, "decide.cuh"), os.path.join(CSRC, "objective_common.cuh"), os.path.join(HERE, "..", "include", "b2hist.h"), __file__]
+    # every object is rebuilt when any header changes: launch.h declares the launchers of every file
+    headers = sorted(glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h")))
+    headers += [os.path.join(HERE, "..", "include", "b2hist.h"), __file__]
     jobs = []
     objs = []
     for src, extra in SOURCES.items():

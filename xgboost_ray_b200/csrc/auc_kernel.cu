@@ -12,6 +12,7 @@
 #include <cub/device/device_scan.cuh>
 
 #include "common.cuh"
+#include "launch.h"
 
 namespace b2 {
 

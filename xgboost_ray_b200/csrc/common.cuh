@@ -267,6 +267,7 @@ struct B2DecideArgs {
 // exchange of a slot is epoch n on every rank.  The epoch counters live in device memory and are advanced by the
 // kernels themselves, which keeps the whole tree capturable in a CUDA graph.
 #define B2_P2P_MAX_WORLD 8
+// kSlotClose is reserved: no kernel exchanges on it (engine.cu ~Booster says why there is no teardown barrier)
 enum { kSlotHist = 0, kSlotCand = 1, kSlotAbsmax = 2, kSlotLeaf = 3, kSlotClose = 4, kP2PSlots = 5 };
 struct B2P2P {
   long long* build[B2_P2P_MAX_WORLD];      // hist_build of rank w ([shards][node_cap][slice]); own pointer for w == rank
@@ -280,6 +281,14 @@ struct B2P2P {
   int32_t world, rank;
   int32_t cand_cap, misc_stride;
   long long spin_limit;                    // polls (each ~0.25 us) before a wait gives up
+};
+// the row blocks of the interleaved ingest (p2p_exchange.cu gather_interleaved_rows_kernel): base[w] = device pointer of
+// rank w's block (own pointer for w == rank), which holds global rows [start[w], start[w + 1])
+struct B2RowBlocks {
+  const float* base[B2_P2P_MAX_WORLD];
+  long long start[B2_P2P_MAX_WORLD + 1];   // first global row of every block; start[W] = n_total
+  int world, rank, n_cols;
+  long long n_mine;
 };
 
 struct B2TrainParamDev {

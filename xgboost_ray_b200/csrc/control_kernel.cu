@@ -11,6 +11,7 @@
 
 #include "common.cuh"
 #include "decide.cuh"
+#include "launch.h"
 
 namespace b2 {
 
@@ -109,9 +110,9 @@ __global__ void tree_init_kernel(B2TreeDev tree, B2LevelCtl* ctl0, B2NodeSeg* se
 }  // namespace b2
 
 extern "C" {
-int b2_launch_decide(const B2DecideArgs* a, const void* p2p, cudaStream_t s) {
+int b2_launch_decide(const B2DecideArgs* a, const B2P2P* p2p, cudaStream_t s) {
   B2P2P pp;
-  if (p2p) pp = *reinterpret_cast<const B2P2P*>(p2p); else memset(&pp, 0, sizeof(pp));
+  if (p2p) pp = *p2p; else memset(&pp, 0, sizeof(pp));
   b2::decide_kernel<<<1, b2::kCtlThreads, 0, s>>>(*a, p2p ? 1 : 0, pp);
   return (int)cudaGetLastError();
 }

@@ -17,6 +17,7 @@
 #include <stdint.h>
 
 #include "common.cuh"
+#include "launch.h"
 
 namespace b2 {
 

@@ -30,136 +30,8 @@
 
 #include "../../include/b2hist.h"
 #include "common.cuh"
+#include "launch.h"
 #include "sampling.cuh"
-
-// ---------------------------------------------------------------- kernel launchers (other TUs)
-extern "C" {
-int b2_launch_hist(const uint8_t*, int, const int2*, const int32_t*, const B2HistWork*, int, int, int, int, int, long long*,
-                   const B2LevelCtl*, int, int, int, cudaStream_t);
-int b2_launch_hist_subtract(const long long*, long long*, const int32_t*, int, int64_t, const B2LevelCtl*, cudaStream_t);
-int b2_launch_eval_splits(const long long*, int, const B2EvalNode*, int, const int32_t*, const int32_t*, const int32_t*,
-                          const uint8_t*, const uint8_t*, const int32_t*, int, B2TrainParamDev, B2SplitCand*, int, const B2LevelCtl*,
-                          int, int, B2ColSample, const B2NodeSeg*, B2SiblingSub, const B2DecideArgs*, uint32_t*, cudaStream_t);
-int b2_eval_ctas_per_node(int, int, int);
-int b2_eval_narrow_max_nodes();
-int b2_launch_eval_splits_vector(const long long*, size_t, int, int, const B2EvalNode*, int, const long long*, const float*,
-                                 const int32_t*, const int32_t*, const int32_t*, const uint8_t*, const int32_t*, int,
-                                 B2TrainParamDev, B2SplitCand*, int, const B2LevelCtl*, B2ColSample, const B2NodeSeg*, cudaStream_t);
-int b2_eval_vector_ctas_per_node(int);
-int b2_launch_vector_root_totals(const long long*, size_t, int, int, const int32_t*, int, B2TrainParamDev, long long*, float*,
-                                 cudaStream_t);
-int b2_launch_vector_child_totals(const long long*, size_t, int, int, int, const B2LevelCtl*, const B2SplitWork*, const int32_t*,
-                                  const B2NodeSeg*, const int32_t*, const int32_t*, const int32_t*, const int32_t*, int,
-                                  B2TrainParamDev, long long*, float*, B2EvalNode*, cudaStream_t);
-int b2_launch_vector_leaf_values(const B2LeafDev*, const int32_t*, const long long*, size_t, const int32_t*, int, int, B2CtlParams,
-                                 float*, float*, int32_t*, cudaStream_t);
-int b2_launch_margin_update_vector(float*, int, const uint16_t*, const float*, int64_t, int, cudaStream_t);
-int b2_launch_predict_vector(const float*, int64_t, int, float, const B2TreeNodeDev*, const int32_t*, const float*, int, int, int,
-                             float*, int, cudaStream_t);
-int b2_launch_subsample(float2*, int64_t, uint32_t, uint32_t, uint32_t, double, int, cudaStream_t);
-int b2_p2p_flag_words(int);
-int b2_launch_p2p_reduce_subtract(const void*, const long long*, long long*, const int32_t*, const B2LevelCtl*, int, int, int64_t, int,
-                                  cudaStream_t);
-int b2_launch_p2p_quant_exponent(const void*, const uint32_t*, int32_t*, cudaStream_t);
-int b2_launch_p2p_leaf_sums(const void*, const int32_t*, long long*, cudaStream_t);
-int b2_launch_p2p_close(const void*, cudaStream_t);
-int b2_launch_gather_interleaved_rows(const void*, float*, int, cudaStream_t);
-int b2_launch_final_assign(const uint8_t*, int64_t, const int32_t*, const B2SplitWork*, const B2LevelCtl*, int, const float2*,
-                           const int32_t*, int, long long*, uint16_t*, int, int, cudaStream_t);
-int b2_launch_margin_update(float*, int, int, const uint16_t*, const float*, const float*, int64_t, int, cudaStream_t);
-int b2_leaf_acc_max_depth();
-int b2_launch_leaf_accumulate(const float2*, const uint16_t*, int64_t, int, const int32_t*, int, long long*, int, cudaStream_t);
-int b2_gradient_fused_max_classes();
-int b2_launch_sum_fixed(const float2*, int64_t, const int32_t*, int, long long*, int, cudaStream_t);
-int b2_cat_ctas();
-int b2_launch_eval_cat_splits(const long long*, int, const B2EvalNode*, int, const int32_t*, int, const int32_t*, const int32_t*,
-                              const int32_t*, int, B2TrainParamDev, B2SplitCand*, int, int, const B2LevelCtl*, int, int,
-                              B2ColSample, const B2NodeSeg*, cudaStream_t);
-int b2_launch_cat_stats(const float*, int64_t, int, float, const int32_t*, int, int32_t*, int, cudaStream_t);
-int b2_launch_root_totals(const long long*, int, B2EvalNode*, const int32_t*, int, B2TrainParamDev, int, long long*, long long*,
-                          cudaStream_t);
-int b2_part_chunk_rows();
-int b2_split_chunk_rows();
-int b2_launch_partition(const uint8_t*, int64_t, const int32_t*, int32_t*, const B2SplitWork*, const B2LevelCtl*, int, int32_t*,
-                        int, B2FinalizeArgs, int, cudaStream_t);
-int b2_launch_leaf_sums(const float2*, const int32_t*, const int32_t*, const void*, const B2LevelCtl*, int, const int32_t*, int,
-                        long long*, uint16_t*, int, cudaStream_t);
-int b2_launch_decide(const B2DecideArgs*, const void*, cudaStream_t);
-int b2_launch_leaf_plan(const B2LeafDev*, const int32_t*, B2SegWork*, B2LevelCtl*, cudaStream_t);
-int b2_launch_leaf_values(const B2LeafDev*, const int32_t*, const long long*, const int32_t*, int, B2CtlParams, float*, B2TreeDev,
-                          int32_t*, cudaStream_t);
-int b2_launch_tree_init(B2TreeDev, B2LevelCtl*, B2NodeSeg*, B2EvalNode*, int32_t*, int, B2HistWork*, cudaStream_t);
-int b2_launch_iota(int32_t*, int64_t, cudaStream_t);
-int b2_launch_gradient(int, int, const float*, const float*, const float*, int64_t, float, float, float2*, uint32_t*, uint32_t*, int,
-                       cudaStream_t);
-int b2_launch_label_check(int, int, const float*, int64_t, uint32_t*, int, cudaStream_t);
-int b2_launch_gradient_aft(int, double, const float*, const float*, const float*, const float*, int64_t, float2*, uint32_t*,
-                           uint32_t*, int, cudaStream_t);
-int b2_launch_aft_bounds_check(const float*, const float*, int64_t, uint32_t*, int, cudaStream_t);
-int b2_launch_aft_metric(int, int, double, const float*, const float*, const float*, const float*, int64_t, double*, int,
-                         cudaStream_t);
-int b2_launch_pack_custom(const float*, const float*, int, int64_t, float2*, int, cudaStream_t);
-int b2_launch_absmax(const float2*, int64_t, uint32_t*, int, cudaStream_t);
-int b2_launch_quant_exponent(const uint32_t*, int32_t*, cudaStream_t);
-int b2_launch_quantize(const float2*, int64_t, const int32_t*, int, int2*, int, cudaStream_t);
-int b2_launch_metric(int, int, int, float, const float*, const float*, const float*, int64_t, double*, int, cudaStream_t);
-int b2_launch_predict(const float*, int64_t, int, float, const B2TreeNodeDev*, const int32_t*, const uint32_t*, int, int, int, int,
-                      const float*, float*, int, cudaStream_t);
-int b2_launch_dart_margins(const uint8_t*, int64_t, int, const int32_t*, const uint8_t*, const B2TreeNodeDev*, const int32_t*,
-                           const uint32_t*, int, int, int, const float*, const uint8_t*, const float*, float*, float*, int,
-                           cudaStream_t);
-int b2_launch_fill(float*, int64_t, float, int, cudaStream_t);
-size_t b2_quantile_hist_elems(int);
-size_t b2_quantile_sel_bytes(int);
-int b2_quantile_passes();
-int b2_launch_gradient_quantile(int, const float*, const float*, const float*, const float*, int64_t, float2*, uint32_t*, int,
-                                cudaStream_t);
-int b2_launch_quantile_metric(int, const float*, const float*, const float*, const float*, int64_t, double*, int, cudaStream_t);
-int b2_launch_quantile_count(int, const uint16_t*, const float*, const float*, int, int, const float2*, int64_t,
-                             const int32_t*, int, const void*, int, unsigned long long*, int, cudaStream_t);
-int b2_launch_quantile_scan(int, const int32_t*, int, int, float, float, unsigned long long*, void*, const B2LeafDev*, float*,
-                            float*, cudaStream_t);
-size_t b2_shap_contribs_smem(int, int, int);
-int b2_launch_shap_contribs(const float*, int64_t, int64_t, int, float, const B2PathElem*, const B2PathInfo*, int, int,
-                            const uint32_t*, int, const double*, const float*, float, double*, int, size_t, float*, int, cudaStream_t);
-int b2_launch_shap_interactions(const float*, int64_t, int64_t, int, float, const B2PathElem*, const B2PathInfo*, int, int,
-                                const uint32_t*, int, const double*, const float*, float, double*, float*, int, cudaStream_t);
-int b2_launch_leaf_index(const float*, int64_t, int64_t, int, float, const B2TreeNodeDev*, const int32_t*, const uint32_t*, int, int,
-                         float*, int, cudaStream_t);
-int b2_rank_stage_rows();
-size_t b2_rank_order_temp_bytes(int64_t, int64_t);
-int b2_launch_rank_iota(int32_t*, int64_t, int, cudaStream_t);
-int b2_rank_order(const float*, int64_t, const int64_t*, int64_t, const int32_t*, uint32_t*, uint32_t*, int32_t*, void*, size_t,
-                  int, cudaStream_t);
-int b2_launch_rank_disc(double*, int64_t, int, cudaStream_t);
-int b2_launch_rank_inv_idcg(const int64_t*, int64_t, const uint32_t*, const double*, int, int, double*, int, cudaStream_t);
-int b2_launch_rank_label_check(const float*, int64_t, int, int, uint32_t*, int, cudaStream_t);
-int b2_launch_lambdarank_gradient(int, const int64_t*, int64_t, int64_t, const uint32_t*, const int32_t*, const float*,
-                                  const double*, const double*, int, int, float*, float*, double*, double*, int32_t*, float2*,
-                                  uint32_t*, uint32_t*, int, cudaStream_t);
-int b2_launch_rank_metric(int, int, int, int, const int64_t*, int64_t, const int32_t*, const float*, const uint32_t*,
-                          const double*, double*, double*, int, cudaStream_t);
-size_t b2_auc_temp_bytes(int64_t);
-int b2_auc(int, int, const float*, const float*, const float*, int64_t, void*, size_t, double*, int, cudaStream_t);
-int b2_launch_transform(int, int, float*, int64_t, int, cudaStream_t);
-int b2_launch_gradient_multi_target(int, int, const float*, const float*, const float*, int64_t, float, float, float2*,
-                                    uint32_t*, uint32_t*, int, cudaStream_t);
-int b2_launch_metric_multi_target(int, int, int, float, const float*, const float*, const float*, int64_t, double*, int,
-                                  cudaStream_t);
-int b2_extract_batch();
-int b2_launch_extract_keys(const float*, int64_t, int, int, int, float, uint32_t*, int64_t, int, cudaStream_t);
-size_t b2_sort_temp_bytes(int64_t);
-int b2_sketch_column(const uint32_t*, const int32_t*, uint32_t*, int32_t*, long long*, int64_t, long long, void*, size_t, int32_t*,
-                     int32_t*, float*, long long*, int32_t*, long long*, int, float*, int32_t*, float*, int32_t*, int, cudaStream_t);
-int b2_launch_weight_absmax(const float*, int64_t, uint32_t*, int, cudaStream_t);
-int b2_launch_weight_quantize(const float*, int64_t, int64_t, const uint32_t*, int32_t*, int, cudaStream_t);
-int b2_launch_bin(const float*, int64_t, int, float, const int32_t*, const float*, const int32_t*, const uint8_t*, int, uint8_t*,
-                  uint8_t*, int64_t, int, cudaStream_t);
-int b2_launch_refresh(const float*, int64_t, int, float, const B2TreeNodeDev*, int, const uint32_t*, int, const float2*,
-                      const int32_t*, int, uint16_t*, long long*, int, cudaStream_t);
-int b2_launch_refresh_nodes(const B2TreeNodeDev*, int, const int32_t*, const int32_t*, int, const long long*, const int32_t*, int,
-                            B2CtlParams, int, long long*, unsigned char*, float*, cudaStream_t);
-}
 
 namespace {
 
@@ -780,10 +652,6 @@ void bin_matrix(Matrix* m) {
 }
 
 // ---------------------------------------------------------------- booster
-// objective ids, shared with objective_kernel.cu (the kernels take them as plain ints)
-enum { kObjSquaredError = 0, kObjLogistic = 1, kObjSoftprob = 2, kObjRegLogistic = 3, kObjLogitRaw = 4, kObjSquaredLog = 5,
-       kObjPseudoHuber = 6, kObjPoisson = 7, kObjGamma = 8, kObjTweedie = 9, kObjAft = 10, kObjRankPairwise = 11,
-       kObjRankNdcg = 12, kObjQuantile = 13, kObjRankMap = 14 };
 bool obj_log_link(int o) { return o == kObjPoisson || o == kObjGamma || o == kObjTweedie || o == kObjAft; }
 bool obj_sigmoid(int o) { return o == kObjLogistic || o == kObjRegLogistic; }
 bool obj_rank(int o) { return o == kObjRankPairwise || o == kObjRankNdcg || o == kObjRankMap; }
@@ -817,7 +685,7 @@ struct Params {
   bool max_delta_step_set = false;             // false: count:poisson uses 0.7 (xgboost's Learner::ConfigureObjective)
   float huber_slope = 1.0f;                    // reg:pseudohubererror delta (also the mphe metric's)
   float tweedie_variance_power = 1.5f;         // reg:tweedie rho in [1, 2)
-  int aft_dist = 0;                            // survival:aft distribution: 0 normal, 1 logistic, 2 extreme
+  int aft_dist = kAftNormal;                   // survival:aft distribution (B2AftDist)
   float aft_sigma = 1.0f;                      // survival:aft scale sigma > 0
   int rank_k = 32;                             // lambdarank_num_pair_per_sample (topk pairs: the first k model positions)
   bool ndcg_exp_gain = true;                   // ndcg gain 2^y - 1 (true) or y (rank:ndcg and the ndcg metrics)
@@ -1254,9 +1122,9 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     else if (k == "huber_slope") p->huber_slope = f();
     else if (k == "tweedie_variance_power") p->tweedie_variance_power = f();
     else if (k == "aft_loss_distribution") {
-      if (v == "normal") p->aft_dist = 0;
-      else if (v == "logistic") p->aft_dist = 1;
-      else if (v == "extreme") p->aft_dist = 2;
+      if (v == "normal") p->aft_dist = kAftNormal;
+      else if (v == "logistic") p->aft_dist = kAftLogistic;
+      else if (v == "extreme") p->aft_dist = kAftExtreme;
       else fail("aft_loss_distribution must be normal, logistic or extreme, got '%s'", v.c_str());
     }
     else if (k == "aft_loss_distribution_scale") p->aft_sigma = f();
@@ -2637,7 +2505,8 @@ void rank_gradient(Booster* b, const float* margin, uint32_t* absmax, uint32_t* 
     b->rank_scratch_m.ensure(rows); b->rank_scratch_y.ensure(rows); b->rank_scratch_p.ensure(rows);
     if (map) { b->rank_scratch_a.ensure(rows); b->rank_scratch_r.ensure(rows); }
   }
-  LAUNCH_CHECK(b2_launch_lambdarank_gradient(map ? 2 : ndcg ? 1 : 0, m->qgroup_ptr.p, m->n_qgroups, m->max_qgroup,
+  const B2RankMode mode = map ? kRankMap : ndcg ? kRankNdcg : kRankPairwise;
+  LAUNCH_CHECK(b2_launch_lambdarank_gradient(mode, m->qgroup_ptr.p, m->n_qgroups, m->max_qgroup,
                                              b->rank_order.keys_sorted.p, b->rank_order.rows.p, m->label.p,
                                              ndcg ? b->rank_inv_idcg.p : nullptr, b->rank_disc.p, p.rank_k,
                                              p.ndcg_exp_gain ? 1 : 0, b->rank_scratch_m.p, b->rank_scratch_y.p,
@@ -3114,15 +2983,15 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
 }
 
 // metric id of an eval_metric name; *param receives the metric's parameter (rho of tweedie-nloglik@rho, huber_slope for mphe)
-int metric_id(const char* name, const Params& p, float* param, int* minus) {
+B2Metric metric_id(const char* name, const Params& p, float* param, int* minus) {
   std::string s(name ? name : "");
   *param = 0.0f; *minus = 0;
-  if (s == "rmsle") return 7;
-  if (s == "mape") return 8;
-  if (s == "mphe") { *param = p.huber_slope; return 9; }
-  if (s == "poisson-nloglik") return 10;
-  if (s == "gamma-nloglik") return 11;
-  if (s == "gamma-deviance") return 12;
+  if (s == "rmsle") return kMetricRmsle;
+  if (s == "mape") return kMetricMape;
+  if (s == "mphe") { *param = p.huber_slope; return kMetricMphe; }
+  if (s == "poisson-nloglik") return kMetricPoissonNloglik;
+  if (s == "gamma-nloglik") return kMetricGammaNloglik;
+  if (s == "gamma-deviance") return kMetricGammaDeviance;
   if (s.rfind("tweedie-nloglik", 0) == 0) {
     *param = 1.5f;   // xgboost's default when the name carries no @rho
     if (s.size() > 15) {
@@ -3133,23 +3002,23 @@ int metric_id(const char* name, const Params& p, float* param, int* minus) {
         fail("eval metric '%s': the Tweedie power must be given as tweedie-nloglik@rho with rho in [1, 2)", s.c_str());
       *param = (float)v;
     }
-    return 13;
+    return kMetricTweedieNloglik;
   }
-  if (s == "rmse") return 0;
-  if (s == "logloss") return 1;
-  if (s == "error") return 2;
-  if (s == "mlogloss") return 3;
-  if (s == "merror") return 4;
-  if (s == "mae") return 5;
-  if (s == "auc") return 6;
-  if (s == "aucpr") return 20;
-  if (s == "aft-nloglik") return 14;
-  if (s == "quantile") return 19;
-  if (s == "interval-regression-accuracy") return 15;
-  // ranking metrics: ndcg[@k][-] (16), map[@k][-] (17), pre[@k][-] (18).  *param = k (0: the whole group), *minus = the
-  // trailing '-' (a group without relevant rows scores 0 instead of 1)
-  for (int id = 16; id <= 18; ++id) {
-    const std::string base = id == 16 ? "ndcg" : id == 17 ? "map" : "pre";
+  if (s == "rmse") return kMetricRmse;
+  if (s == "logloss") return kMetricLogloss;
+  if (s == "error") return kMetricError;
+  if (s == "mlogloss") return kMetricMlogloss;
+  if (s == "merror") return kMetricMerror;
+  if (s == "mae") return kMetricMae;
+  if (s == "auc") return kMetricAuc;
+  if (s == "aucpr") return kMetricAucPr;
+  if (s == "aft-nloglik") return kMetricAftNloglik;
+  if (s == "quantile") return kMetricQuantile;
+  if (s == "interval-regression-accuracy") return kMetricIntervalAccuracy;
+  // ranking metrics: ndcg[@k][-], map[@k][-], pre[@k][-].  *param = k (0: the whole group), *minus = the trailing '-'
+  // (a group without relevant rows scores 0 instead of 1)
+  for (const B2Metric id : {kMetricNdcg, kMetricMap, kMetricPre}) {
+    const std::string base = id == kMetricNdcg ? "ndcg" : id == kMetricMap ? "map" : "pre";
     if (s.compare(0, base.size(), base) != 0) continue;
     std::string rest = s.substr(base.size());
     if (!rest.empty() && rest.back() == '-') { *minus = 1; rest.pop_back(); }
@@ -3193,6 +3062,15 @@ float* eval_margin(Booster* b, Matrix* m) {
     c->n_trees_applied = nt;
   }
   return c->margin.p;
+}
+
+// the first n doubles of b->d_metric summed over the workers, on the host (synchronises the stream)
+std::vector<double> metric_sums(Booster* b, size_t n, cudaStream_t s) {
+  allreduce(b->comm, b->d_metric.p, n, kNcclFloat64, kNcclSum, s);
+  std::vector<double> h(n);
+  CUDA_CHECK(cudaMemcpyAsync(h.data(), b->d_metric.p, n * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  return h;
 }
 
 }  // namespace
@@ -3327,13 +3205,6 @@ int B2_MatrixCreateFromProcess(int64_t pid, uint64_t remote_addr, int64_t remote
   *out = (B2Handle)m;
   API_END
 }
-// host mirror of b2::B2RowBlocks (p2p_exchange.cu)
-struct RowBlocksHost {
-  const float* base[B2_P2P_MAX_WORLD];
-  long long start[B2_P2P_MAX_WORLD + 1];
-  int world, rank, n_cols;
-  long long n_mine;
-};
 // Staging block of the interleaved ingest: persistent per device (grow-only), exported ONCE; the peers keep their mapping
 // of it across calls (mapping / unmapping a multi-GB allocation costs more than moving the rows).  A block that had to
 // grow is retired and freed only after the call's closing barrier, when every peer has dropped its mapping of it.
@@ -3361,7 +3232,7 @@ int B2_MatrixCreateFromProcessInterleaved(int64_t pid, uint64_t remote_addr, int
   };
   std::lock_guard<std::mutex> ingest_lock(g_ingest_mu);
   // contiguous block of this rank (BATCH split of the global rows) and the rows it finally owns (INTERLEAVED)
-  RowBlocksHost rb; memset(&rb, 0, sizeof(rb));
+  B2RowBlocks rb; memset(&rb, 0, sizeof(rb));
   const int64_t per = n_total_rows / W, extra = n_total_rows % W;
   for (int w = 0; w <= W; ++w) rb.start[w] = (long long)(w * per + std::min<int64_t>(w, extra));
   const int64_t b0 = rb.start[rank], bn = rb.start[rank + 1] - b0;
@@ -3739,9 +3610,9 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
   cudaStream_t s = b->ctx->stream;
   float mparam = 0.0f;
   int minus = 0;
-  const int mid = metric_id(metric, b->p, &mparam, &minus);
-  const bool aft_metric = mid == 14 || mid == 15;
-  if (mid >= 16 && mid <= 18) {
+  const B2Metric mid = metric_id(metric, b->p, &mparam, &minus);
+  const bool aft_metric = mid == kMetricAftNloglik || mid == kMetricIntervalAccuracy;
+  if (mid >= kMetricNdcg && mid <= kMetricPre) {
     // ndcg / map / pre: per query group on the prediction order (rank_kernel.cu), averaged over the groups of all workers
     if (b->p.num_class > 1) fail("metric '%s' needs a single-output objective", metric);
     if (!m->has_qgroups()) fail("metric '%s' needs query groups (qid) on the evaluation matrix", metric);
@@ -3752,21 +3623,18 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
     if (m->n > 0) CUDA_CHECK(cudaMemcpyAsync(pred.p, margin, (size_t)m->n * sizeof(float), cudaMemcpyDeviceToDevice, s));
     LAUNCH_CHECK(b2_launch_transform(b->p.objective, 1, pred.p, m->n, b->ctx->num_sms, s));
     po.run(m, pred.p, b->ctx->num_sms, s);
-    if (mid == 16) lo.run(m, m->label.p, b->ctx->num_sms, s);
+    if (mid == kMetricNdcg) lo.run(m, m->label.p, b->ctx->num_sms, s);
     ensure_rank_disc(b, m->max_qgroup);
     vals.ensure((size_t)std::max<int64_t>(m->n_qgroups, 1));
     b->d_metric.ensure(2);
     LAUNCH_CHECK(b2_launch_rank_metric(mid, (int)mparam, minus, b->p.ndcg_exp_gain ? 1 : 0, m->qgroup_ptr.p, m->n_qgroups,
-                                       po.rows.p, m->label.p, mid == 16 ? lo.keys_sorted.p : nullptr, b->rank_disc.p, vals.p,
-                                       b->d_metric.p, b->ctx->num_sms, s));
-    allreduce(b->comm, b->d_metric.p, 2, kNcclFloat64, kNcclSum, s);
-    double h[2];
-    CUDA_CHECK(cudaMemcpyAsync(h, b->d_metric.p, sizeof(h), cudaMemcpyDeviceToHost, s));
-    CUDA_CHECK(cudaStreamSynchronize(s));
+                                       po.rows.p, m->label.p, mid == kMetricNdcg ? lo.keys_sorted.p : nullptr, b->rank_disc.p,
+                                       vals.p, b->d_metric.p, b->ctx->num_sms, s));
+    const std::vector<double> h = metric_sums(b, 2, s);
     *out = h[1] > 0 ? h[0] / h[1] : 0.0;
     return 0;
   }
-  const bool auc_metric = mid == 6 || mid == 20;
+  const bool auc_metric = mid == kMetricAuc || mid == kMetricAucPr;
   // xgboost computes a per-group ranking AUC on a matrix with groups; this engine's auc / aucpr are binary or
   // one-vs-rest only
   if (auc_metric && m->has_qgroups())
@@ -3796,17 +3664,14 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
     const size_t tb = b2_auc_temp_bytes(m->n);
     tmp.ensure(tb);
     b->d_metric.ensure(3 * (size_t)K + 1);
-    LAUNCH_CHECK(b2_auc(mid == 20 ? 1 : 0, K, pred.p, m->label.p, m->n_weight ? m->weight.p : nullptr, m->n, tmp.p, tb,
-                        b->d_metric.p, b->ctx->num_sms, s));
-    allreduce(b->comm, b->d_metric.p, 3 * (size_t)K + 1, kNcclFloat64, kNcclSum, s);
-    std::vector<double> h(3 * (size_t)K + 1);
-    CUDA_CHECK(cudaMemcpyAsync(h.data(), b->d_metric.p, h.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-    CUDA_CHECK(cudaStreamSynchronize(s));
+    LAUNCH_CHECK(b2_auc(mid == kMetricAucPr ? 1 : 0, K, pred.p, m->label.p, m->n_weight ? m->weight.p : nullptr, m->n,
+                        tmp.p, tb, b->d_metric.p, b->ctx->num_sms, s));
+    const std::vector<double> h = metric_sums(b, 3 * (size_t)K + 1, s);
     if (h[3 * (size_t)K] > 0)
       fail("metric '%s': label must be in [0, num_class), num_class = %d (%.0f rows outside)", metric, K, h[3 * (size_t)K]);
     if (K == 1) {
       // ROC with only one class present: xgboost reports 0.5
-      *out = mid == 6 ? (h[1] > 0 ? h[0] / h[1] : 0.5) : h[0] / h[1];
+      *out = mid == kMetricAuc ? (h[1] > 0 ? h[0] / h[1] : 0.5) : h[0] / h[1];
       return 0;
     }
     // one-vs-rest: sum_c (A_c / L_c) T_c / sum_c T_c; NaN when some class has L_c = 0 or no class has T_c
@@ -3822,19 +3687,16 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
   }
   b->d_metric.ensure(3);
   CUDA_CHECK(cudaMemsetAsync(b->d_metric.p, 0, 3 * sizeof(double), s));
-  if ((mid == 3 || mid == 4) != (b->p.objective == kObjSoftprob))
+  if ((mid == kMetricMlogloss || mid == kMetricMerror) != (b->p.objective == kObjSoftprob))
     fail("metric '%s' does not fit objective '%s'", metric, b->p.objective_name.c_str());
   if (aft_metric) {
     LAUNCH_CHECK(b2_launch_aft_metric(b->p.aft_dist, mid, (double)b->p.aft_sigma, margin, m->lower.p, m->upper.p,
                                       m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p, b->ctx->num_sms, s));
-    allreduce(b->comm, b->d_metric.p, 2, kNcclFloat64, kNcclSum, s);
-    double h[2];
-    CUDA_CHECK(cudaMemcpyAsync(h, b->d_metric.p, sizeof(h), cudaMemcpyDeviceToHost, s));
-    CUDA_CHECK(cudaStreamSynchronize(s));
+    const std::vector<double> h = metric_sums(b, 2, s);
     *out = h[1] > 0 ? h[0] / h[1] : 0.0;
     return 0;
   }
-  if (mid == 19) {
+  if (mid == kMetricQuantile) {
     // pinball loss averaged over the rows and the alphas, weighted (sum, K * sum w summed over the workers)
     if (b->p.objective != kObjQuantile) fail("metric 'quantile' needs objective reg:quantileerror (it reads quantile_alpha)");
     if (!b->d_alpha.p || b->d_alpha.cap < b->p.quantile_alpha.size()) {
@@ -3843,16 +3705,13 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
     }
     LAUNCH_CHECK(b2_launch_quantile_metric(b->p.num_class, b->d_alpha.p, margin, m->label.p, m->n_weight ? m->weight.p : nullptr,
                                            m->n, b->d_metric.p, b->ctx->num_sms, s));
-    allreduce(b->comm, b->d_metric.p, 2, kNcclFloat64, kNcclSum, s);
-    double h[2];
-    CUDA_CHECK(cudaMemcpyAsync(h, b->d_metric.p, sizeof(h), cudaMemcpyDeviceToHost, s));
-    CUDA_CHECK(cudaStreamSynchronize(s));
+    const std::vector<double> h = metric_sums(b, 2, s);
     *out = h[1] > 0 ? h[0] / h[1] : 0.0;
     return 0;
   }
   if (b->p.num_target > 1) {
     // elementwise over the n x T outputs, each with its row's weight (xgboost's EvalEWiseBase)
-    if (!(mid <= 2 || mid == 5 || (mid >= 7 && mid <= 9)))
+    if (!(mid <= kMetricError || mid == kMetricMae || (mid >= kMetricRmsle && mid <= kMetricMphe)))
       fail("metric '%s' is not supported for a multi-target model (supported: rmse, rmsle, mae, mape, mphe, logloss, error)",
            metric);
     LAUNCH_CHECK(b2_launch_metric_multi_target(b->p.objective, mid, b->p.num_target, mparam, margin, m->label.p,
@@ -3861,14 +3720,11 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
     LAUNCH_CHECK(b2_launch_metric(b->p.objective, mid, b->p.num_class, mparam, margin, m->label.p, m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p,
                                   b->ctx->num_sms, s));
   // (sum, wsum, rows with a label outside [0, num_class)): the count travels with the sums, so every rank fails together
-  allreduce(b->comm, b->d_metric.p, 3, kNcclFloat64, kNcclSum, s);
-  double h[3];
-  CUDA_CHECK(cudaMemcpyAsync(h, b->d_metric.p, sizeof(h), cudaMemcpyDeviceToHost, s));
-  CUDA_CHECK(cudaStreamSynchronize(s));
+  const std::vector<double> h = metric_sums(b, 3, s);
   if (h[2] > 0)
     fail("metric '%s': label must be in [0, num_class), num_class = %d (%.0f rows outside)", metric, b->p.num_class, h[2]);
   double v = h[1] > 0 ? h[0] / h[1] : 0.0;
-  *out = (mid == 0 || mid == 7) ? sqrt(v) : v;
+  *out = (mid == kMetricRmse || mid == kMetricRmsle) ? sqrt(v) : v;
   API_END
 }
 int B2_BoosterPredict(B2Handle bh, B2Handle mh, int32_t output_margin, int32_t tree_begin, int32_t tree_end, float* out,

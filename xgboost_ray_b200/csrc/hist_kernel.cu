@@ -21,6 +21,7 @@
 //    2^30 (none for well spread bins), which is what keeps the int32 cells from overflowing.
 //  * Rows of a node are addressed through the row-index segment list (gather) except at the root.
 #include "hist_common.cuh"
+#include "launch.h"
 
 namespace b2 {
 

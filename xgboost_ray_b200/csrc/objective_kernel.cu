@@ -10,6 +10,7 @@
 #include "common.cuh"
 #include "sampling.cuh"
 #include "objective_common.cuh"
+#include "launch.h"
 
 namespace b2 {
 
@@ -109,17 +110,12 @@ __device__ double b2_erf(double x) {
   return hx >= 0 ? B2_DS(1.0, B2_DD(r, ax)) : B2_DS(B2_DD(r, ax), 1.0);
 }
 
-// objective ids (engine.cu kObj*): 0 reg:squarederror, 1 binary:logistic, 2 multi:softprob, 3 reg:logistic,
-// 4 binary:logitraw, 5 reg:squaredlogerror, 6 reg:pseudohubererror, 7 count:poisson, 8 reg:gamma, 9 reg:tweedie,
-// 10 survival:aft, 13 reg:quantileerror (its kernels are in quantile_kernel.cu)
-constexpr int kObjRegLogistic = 3, kObjLogitRaw = 4, kObjSquaredLog = 5, kObjPseudoHuber = 6, kObjPoisson = 7,
-              kObjGamma = 8, kObjTweedie = 9, kObjAft = 10, kObjQuantile = 13;
 // the parameter of an objective that has one: huber_slope, max_delta_step (Poisson hessian), tweedie_variance_power
 struct ObjParam { float a; };
 
 // margin -> prediction of one scalar output (ObjFunction::PredTransform): sigmoid, exp or identity
 __device__ __forceinline__ float b2_pred_transform(int objective, float m) {
-  if (objective == 1 || objective == kObjRegLogistic) return b2_sigmoid(m);
+  if (objective == kObjLogistic || objective == kObjRegLogistic) return b2_sigmoid(m);
   if (objective == kObjPoisson || objective == kObjGamma || objective == kObjTweedie || objective == kObjAft) return b2_expf(m);
   return m;
 }
@@ -158,11 +154,11 @@ __device__ __forceinline__ float2 scalar_grad(float p, float y, float a) {
 // the same pass (the fixed-point scale of each class tree needs it; a separate pass re-read 8 bytes per row).
 constexpr int kFusedMaxK = 16;   // classes whose running maxima fit in registers; more classes use absmax_kernel
 
-// (g, h) of one element of reg:squarederror (kObjective 0) or binary:logistic and its variants (1), weight w applied
-// (scale_pos_weight on positive labels, RegLossObj)
+// (g, h) of one element of reg:squarederror (kObjSquaredError) or binary:logistic and its variants (kObjLogistic), weight w
+// applied (scale_pos_weight on positive labels, RegLossObj)
 template <int kObjective>
 __device__ __forceinline__ float2 reg_loss_grad(float m, float y, float w, float scale_pos_weight) {
-  if (kObjective == 0) return make_float2(__fmul_rn(__fadd_rn(m, -y), w), w);
+  if (kObjective == kObjSquaredError) return make_float2(__fmul_rn(__fadd_rn(m, -y), w), w);
   if (y == 1.0f) w = __fmul_rn(w, scale_pos_weight);   // RegLossObj: positive rows
   const float p = b2_sigmoid(m);
   float hh = __fmul_rn(p, __fadd_rn(1.0f, -p));
@@ -237,7 +233,7 @@ gradient_multi_target_kernel(int T, const float* __restrict__ margin, const floa
   auto elem = [&](int64_t i, int k, float w) {
     const float y = label[i * T + k], m = margin[i * T + k];
     float2 v;
-    if constexpr (kObjective <= 1) v = reg_loss_grad<kObjective>(m, y, w, scale_pos_weight);
+    if constexpr (kObjective <= kObjLogistic) v = reg_loss_grad<kObjective>(m, y, w, scale_pos_weight);
     else v = param_grad<kObjective>(m, y, w, scale_pos_weight, op.a, &bad);
     gh[(int64_t)k * n + i] = v;
     return v;
@@ -255,7 +251,7 @@ gradient_multi_target_kernel(int T, const float* __restrict__ margin, const floa
       for (int k = 0; k < T; ++k) elem(i, k, w);
     }
   }
-  if (kObjective > 1 && bad && err) atomicOr(err, 1u);
+  if (kObjective > kObjLogistic && bad && err) atomicOr(err, 1u);
   if (kFused && absmax) {
 #pragma unroll
     for (int k = 0; k < kMax; ++k)
@@ -272,7 +268,6 @@ gradient_multi_target_kernel(int T, const float* __restrict__ margin, const floa
 // in binary64 (tests/survival_reference.py replays the sequence).  A quotient that is not finite while its denominator
 // is below kEps takes its limit as the margin goes to -inf (z > 0; z_u > 0 or z_l > 0 for censored rows) or +inf; then
 // g is clipped to [-15, 15] and h to [1e-16, 15].
-constexpr int kAftNormal = 0, kAftLogistic = 1, kAftExtreme = 2;
 constexpr double kAftEps = 1e-12;
 struct AftDensity { double pdf, cdf, dpdf, d2pdf; };
 
@@ -411,10 +406,10 @@ __global__ void aft_bounds_check_kernel(const float* __restrict__ lower, const f
   if (__any_sync(0xffffffffu, b3) && (threadIdx.x & 31) == 0) atomicOr(&bad[3], 1u);
 }
 
-// aft-nloglik (metric 14) and interval-regression-accuracy (metric 15): (sum w v, sum w) in double
+// aft-nloglik and interval-regression-accuracy: (sum w v, sum w) in double
 template <int kDist>
 __device__ __forceinline__ double aft_metric_value(int metric, float m, float lower, float upper, double sigma) {
-  if (metric == 14) return aft_loss<kDist>((double)m, lower, upper, sigma);
+  if (metric == kMetricAftNloglik) return aft_loss<kDist>((double)m, lower, upper, sigma);
   const double p = b2_exp((double)m);
   return ((double)lower <= p && p <= (double)upper) ? 1.0 : 0.0;
 }
@@ -554,31 +549,31 @@ __global__ void quantize_kernel(const float2* __restrict__ gh, int64_t n, const 
 
 // metric sums (sum loss*w, sum w, rows with an invalid class label) -> out[3] doubles.  Metrics see the TRANSFORMED prediction (ObjFunction::EvalTransform,
 // src/learner.cc): the probability for binary:logistic / reg:logistic, exp(margin) for the log-link objectives, the raw
-// value otherwise.  metric: 0 rmse, 1 logloss, 2 error, 3 mlogloss, 4 merror, 5 mae, 7 rmsle, 8 mape, 9 mphe (a = huber
-// slope), 10 poisson-nloglik, 11 gamma-nloglik, 12 gamma-deviance, 13 tweedie-nloglik (a = rho); 6 (auc) and 20 (aucpr) are auc_kernel.cu.
+// value otherwise.  a: huber_slope of mphe, rho of tweedie-nloglik.  auc and aucpr are auc_kernel.cu.
 // the elementwise metrics of the objectives added after the first three, on the transformed prediction q
 __device__ __forceinline__ double scalar_metric(int metric, float a, double q, double y) {
-  if (metric == 7) { const double d = log1p(y) - log1p(fmax(q, -1.0 + 1e-6)); return d * d; }
-  if (metric == 8) return fabs((y - q) / y);
-  if (metric == 9) { const double z = (y - q) / (double)a; return (double)a * (double)a * (sqrt(1.0 + z * z) - 1.0); }
-  if (metric == 10) { const double qq = fmax(q, 1e-16); return lgamma(y + 1.0) + qq - y * log(qq); }
-  if (metric == 11) return y / q + log(q);
-  if (metric == 12) { const double qq = q + 1e-6, yy = y + 1e-6; return 2.0 * (log(qq / yy) + yy / qq - 1.0); }
+  if (metric == kMetricRmsle) { const double d = log1p(y) - log1p(fmax(q, -1.0 + 1e-6)); return d * d; }
+  if (metric == kMetricMape) return fabs((y - q) / y);
+  if (metric == kMetricMphe) { const double z = (y - q) / (double)a; return (double)a * (double)a * (sqrt(1.0 + z * z) - 1.0); }
+  if (metric == kMetricPoissonNloglik) { const double qq = fmax(q, 1e-16); return lgamma(y + 1.0) + qq - y * log(qq); }
+  if (metric == kMetricGammaNloglik) return y / q + log(q);
+  if (metric == kMetricGammaDeviance) { const double qq = q + 1e-6, yy = y + 1e-6; return 2.0 * (log(qq / yy) + yy / qq - 1.0); }
   const double r = (double)a;
   return -y * pow(q, 1.0 - r) / (1.0 - r) + pow(q, 2.0 - r) / (2.0 - r);
 }
 
-// one element's loss for the elementwise metrics (0-2, 5, 7-13) on the transformed prediction
+// one element's loss for the elementwise metrics (rmse, logloss, error, mae, rmsle .. tweedie-nloglik) on the transformed
+// prediction
 __device__ __forceinline__ double elementwise_metric(int objective, int metric, float a, float margin, float y) {
   const float p = b2_pred_transform(objective, margin);
-  if (metric == 0) { const double d = (double)p - (double)y; return d * d; }
-  if (metric == 5) return fabs((double)p - (double)y);
-  if (metric == 1) {
+  if (metric == kMetricRmse) { const double d = (double)p - (double)y; return d * d; }
+  if (metric == kMetricMae) return fabs((double)p - (double)y);
+  if (metric == kMetricLogloss) {
     const float eps = 1e-16f;
     const float pn = 1.0f - p; const float pa = p < eps ? eps : p, pb = pn < eps ? eps : pn;
     return -((double)y * log((double)pa) + (1.0 - (double)y) * log((double)pb));
   }
-  if (metric == 2) return ((p > 0.5f) != (y > 0.5f)) ? 1.0 : 0.0;
+  if (metric == kMetricError) return ((p > 0.5f) != (y > 0.5f)) ? 1.0 : 0.0;
   return scalar_metric(metric, a, (double)p, (double)y);
 }
 
@@ -611,13 +606,14 @@ __global__ void metric_kernel(int objective, int metric, int K, float a, const f
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const double w = weight ? (double)weight[i] : 1.0;
     double v = 0.0;
-    if (metric <= 2 || metric == 5 || metric >= 7) v = elementwise_metric(objective, metric, a, margin[i], label[i]);
+    if (metric <= kMetricError || metric == kMetricMae || metric >= kMetricRmsle)
+      v = elementwise_metric(objective, metric, a, margin[i], label[i]);
     else {
       const float yf = label[i];
       if (!b2_class_label_ok(yf, K)) { ++bad; continue; }
       const float* r = margin + i * K; const int y = (int)yf; float mx = r[0]; int am = 0;
       for (int k = 1; k < K; ++k) if (r[k] > mx) { mx = r[k]; am = k; }
-      if (metric == 4) v = (am != y) ? 1.0 : 0.0;
+      if (metric == kMetricMerror) v = (am != y) ? 1.0 : 0.0;
       else {
         float ssum = 0.0f;
         for (int k = 0; k < K; ++k) ssum = __fadd_rn(ssum, b2_expf(__fadd_rn(r[k], -mx)));
@@ -644,7 +640,7 @@ __global__ void label_check_kernel(int objective, int K, const float* __restrict
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const float y = label[i];
     bool ok = true;
-    if (objective == 2) ok = b2_class_label_ok(y, K);
+    if (objective == kObjSoftprob) ok = b2_class_label_ok(y, K);
     else if (objective == kObjRegLogistic || objective == kObjLogitRaw) ok = y >= 0.0f && y <= 1.0f;
     else if (objective == kObjSquaredLog) ok = y > -1.0f;
     else if (objective == kObjPoisson || objective == kObjTweedie) ok = y >= 0.0f;
@@ -699,7 +695,7 @@ __global__ void fill_kernel(float* out, int64_t n, float v) {
 // margin -> prediction transform in place (sigmoid / exp / softmax)
 __global__ void transform_kernel(int objective, int K, float* __restrict__ m, int64_t n) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    if (objective == 2) {
+    if (objective == kObjSoftprob) {
       float* r = m + i * K; float mx = r[0];
       for (int k = 1; k < K; ++k) if (r[k] > mx) mx = r[k];
       float s = 0.0f;
@@ -730,14 +726,16 @@ int b2_launch_gradient(int objective, int K, const float* margin, const float* l
   const int g = grid_for(n, num_sms);
   const b2::ObjParam op{obj_param};
   switch (objective) {
-    case 0: b2::gradient_scalar_kernel<0><<<g, 256, 0, s>>>(margin, label, weight, n, scale_pos_weight, gh, absmax); break;
-    case 1: case b2::kObjRegLogistic: case b2::kObjLogitRaw:   // the logistic variants differ only in the transform
-      b2::gradient_scalar_kernel<1><<<g, 256, 0, s>>>(margin, label, weight, n, scale_pos_weight, gh, absmax); break;
-    case 2: b2::gradient_softprob_kernel<<<g, 256, 0, s>>>(K, margin, label, weight, n, gh, absmax); break;
+    case kObjSquaredError:
+      b2::gradient_scalar_kernel<kObjSquaredError><<<g, 256, 0, s>>>(margin, label, weight, n, scale_pos_weight, gh, absmax);
+      break;
+    case kObjLogistic: case kObjRegLogistic: case kObjLogitRaw:   // the logistic variants differ only in the transform
+      b2::gradient_scalar_kernel<kObjLogistic><<<g, 256, 0, s>>>(margin, label, weight, n, scale_pos_weight, gh, absmax); break;
+    case kObjSoftprob: b2::gradient_softprob_kernel<<<g, 256, 0, s>>>(K, margin, label, weight, n, gh, absmax); break;
 #define B2_PARAM_OBJ(id) \
     case id: b2::gradient_param_kernel<id><<<g, 256, 0, s>>>(margin, label, weight, n, scale_pos_weight, op, gh, absmax, err); break;
-    B2_PARAM_OBJ(b2::kObjSquaredLog) B2_PARAM_OBJ(b2::kObjPseudoHuber) B2_PARAM_OBJ(b2::kObjPoisson)
-    B2_PARAM_OBJ(b2::kObjGamma) B2_PARAM_OBJ(b2::kObjTweedie)
+    B2_PARAM_OBJ(kObjSquaredLog) B2_PARAM_OBJ(kObjPseudoHuber) B2_PARAM_OBJ(kObjPoisson) B2_PARAM_OBJ(kObjGamma)
+    B2_PARAM_OBJ(kObjTweedie)
 #undef B2_PARAM_OBJ
     default: return (int)cudaErrorInvalidValue;
   }
@@ -757,8 +755,8 @@ int b2_launch_gradient_multi_target(int objective, int T, const float* margin, c
       if (fused) b2::gradient_multi_target_kernel<kern_id, true><<<g, 256, 0, s>>>(T, margin, label, weight, n, scale_pos_weight, op, gh, absmax, err); \
       else b2::gradient_multi_target_kernel<kern_id, false><<<g, 256, 0, s>>>(T, margin, label, weight, n, scale_pos_weight, op, gh, nullptr, err); \
       break;
-    B2_MT(0, 0) B2_MT(1, 1) B2_MT(1, b2::kObjRegLogistic) B2_MT(1, b2::kObjLogitRaw)
-    B2_MT(b2::kObjSquaredLog, b2::kObjSquaredLog) B2_MT(b2::kObjPseudoHuber, b2::kObjPseudoHuber)
+    B2_MT(kObjSquaredError, kObjSquaredError) B2_MT(kObjLogistic, kObjLogistic) B2_MT(kObjLogistic, kObjRegLogistic)
+    B2_MT(kObjLogistic, kObjLogitRaw) B2_MT(kObjSquaredLog, kObjSquaredLog) B2_MT(kObjPseudoHuber, kObjPseudoHuber)
 #undef B2_MT
     default: return (int)cudaErrorInvalidValue;
   }
@@ -780,7 +778,7 @@ int b2_launch_gradient_aft(int dist, double sigma, const float* margin, const fl
   switch (dist) {
 #define B2_AFT(d) \
     case d: b2::gradient_aft_kernel<d><<<g, 256, 0, s>>>(margin, lower, upper, weight, n, sigma, gh, absmax, err); break;
-    B2_AFT(b2::kAftNormal) B2_AFT(b2::kAftLogistic) B2_AFT(b2::kAftExtreme)
+    B2_AFT(kAftNormal) B2_AFT(kAftLogistic) B2_AFT(kAftExtreme)
 #undef B2_AFT
     default: return (int)cudaErrorInvalidValue;
   }
@@ -861,7 +859,7 @@ int b2_launch_fill(float* out, int64_t n, float v, int num_sms, cudaStream_t s) 
 // m holds n rows of K outputs: softmax runs per row, every other transform over all n * K elements
 int b2_launch_transform(int objective, int K, float* m, int64_t n, int num_sms, cudaStream_t s) {
   if (n <= 0) return 0;
-  if (objective != 2) n *= K;
+  if (objective != kObjSoftprob) n *= K;
   b2::transform_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(objective, K, m, n);
   return (int)cudaGetLastError();
 }

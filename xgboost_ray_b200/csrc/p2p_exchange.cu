@@ -11,6 +11,7 @@
 // The split candidates travel the other way: decide_kernel (control_kernel.cu) stores this rank's candidates into
 // every peer's table before it decides.  No NCCL call is left inside a tree.
 #include "p2p.cuh"
+#include "launch.h"
 
 namespace b2 {
 
@@ -97,13 +98,7 @@ p2p_leaf_sums_kernel(B2P2P pp, const int32_t* __restrict__ n_leaves, long long* 
 // INTERLEAVED sharding without host-side amplification: every rank uploads ONE contiguous block of the driver's matrix
 // (rows [start_w, start_w + count_w) on rank w, BATCH-style split) and then pulls the rows it owns -- global rows
 // rank, rank + W, rank + 2W, ... -- out of the peers' blocks over NVLink.  One warp per row, coalesced float4 / float
-// copies.  blocks[w] = device pointer of rank w's block (own pointer for w == rank).
-struct B2RowBlocks {
-  const float* base[B2_P2P_MAX_WORLD];
-  long long start[B2_P2P_MAX_WORLD + 1];   // first global row of every block; start[W] = n_total
-  int world, rank, n_cols;
-  long long n_mine;
-};
+// copies.
 __global__ void __launch_bounds__(256)
 gather_interleaved_rows_kernel(B2RowBlocks rb, float* __restrict__ out) {
   const int lane = threadIdx.x & 31;
@@ -119,19 +114,11 @@ gather_interleaved_rows_kernel(B2RowBlocks rb, float* __restrict__ out) {
   }
 }
 
-// teardown barrier: nobody frees a mapped buffer while a peer may still be reading it
-__global__ void p2p_close_kernel(B2P2P pp) {
-  const uint32_t epoch = p2p_next_epoch(pp, kSlotClose);
-  p2p_signal(pp, kSlotClose, epoch);
-  p2p_wait(pp, kSlotClose, epoch);
-  p2p_finish_single(pp, kSlotClose, epoch);
-}
-
 }  // namespace b2
 
 extern "C" {
 int b2_p2p_flag_words(int world) { return kP2PSlots * world; }
-int b2_launch_p2p_reduce_subtract(const void* pp, const long long* parent_level, long long* level, const int32_t* triples,
+int b2_launch_p2p_reduce_subtract(const B2P2P* pp, const long long* parent_level, long long* level, const int32_t* triples,
                                   const B2LevelCtl* ctl, int max_pairs, int node_cap, int64_t slice_elems, int num_sms,
                                   cudaStream_t s) {
   if (max_pairs <= 0 || slice_elems <= 0) return 0;
@@ -142,29 +129,23 @@ int b2_launch_p2p_reduce_subtract(const void* pp, const long long* parent_level,
   if (bx > cap) bx = cap;
   if (bx < 1) bx = 1;
   dim3 grid(bx, max_pairs);
-  b2::p2p_reduce_subtract_kernel<<<grid, 256, 0, s>>>(*reinterpret_cast<const B2P2P*>(pp), parent_level, level, triples, ctl,
-                                                     node_cap, slice_elems);
+  b2::p2p_reduce_subtract_kernel<<<grid, 256, 0, s>>>(*pp, parent_level, level, triples, ctl, node_cap, slice_elems);
   return (int)cudaGetLastError();
 }
-int b2_launch_p2p_quant_exponent(const void* pp, const uint32_t* absmax, int32_t* qexp, cudaStream_t s) {
-  b2::p2p_quant_exponent_kernel<<<1, 32, 0, s>>>(*reinterpret_cast<const B2P2P*>(pp), absmax, qexp);
+int b2_launch_p2p_quant_exponent(const B2P2P* pp, const uint32_t* absmax, int32_t* qexp, cudaStream_t s) {
+  b2::p2p_quant_exponent_kernel<<<1, 32, 0, s>>>(*pp, absmax, qexp);
   return (int)cudaGetLastError();
 }
-int b2_launch_p2p_leaf_sums(const void* pp, const int32_t* n_leaves, long long* sums, cudaStream_t s) {
-  b2::p2p_leaf_sums_kernel<<<1, 1024, 0, s>>>(*reinterpret_cast<const B2P2P*>(pp), n_leaves, sums);
+int b2_launch_p2p_leaf_sums(const B2P2P* pp, const int32_t* n_leaves, long long* sums, cudaStream_t s) {
+  b2::p2p_leaf_sums_kernel<<<1, 1024, 0, s>>>(*pp, n_leaves, sums);
   return (int)cudaGetLastError();
 }
-int b2_launch_gather_interleaved_rows(const void* blocks, float* out, int num_sms, cudaStream_t s) {
-  const b2::B2RowBlocks& rb = *reinterpret_cast<const b2::B2RowBlocks*>(blocks);
+int b2_launch_gather_interleaved_rows(const B2RowBlocks* blocks, float* out, int num_sms, cudaStream_t s) {
+  const B2RowBlocks& rb = *blocks;
   if (rb.n_mine <= 0) return 0;
   long long want = (rb.n_mine * 32 + 255) / 256;
   int grid = (int)(want < (long long)num_sms * 16 ? want : (long long)num_sms * 16);
   b2::gather_interleaved_rows_kernel<<<grid, 256, 0, s>>>(rb, out);
-  return (int)cudaGetLastError();
-}
-int b2_row_blocks_bytes() { return (int)sizeof(b2::B2RowBlocks); }
-int b2_launch_p2p_close(const void* pp, cudaStream_t s) {
-  b2::p2p_close_kernel<<<1, 32, 0, s>>>(*reinterpret_cast<const B2P2P*>(pp));
   return (int)cudaGetLastError();
 }
 }

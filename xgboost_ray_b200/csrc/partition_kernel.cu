@@ -9,6 +9,7 @@
 
 #include "common.cuh"
 #include "level_finalize.cuh"
+#include "launch.h"
 
 namespace b2 {
 
@@ -380,10 +381,6 @@ leaf_accumulate_kernel(const float2* __restrict__ gh, const uint16_t* __restrict
   }
 }
 
-__global__ void iota_kernel(int32_t* out, int64_t n) {
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = (int32_t)i;
-}
-
 }  // namespace b2
 
 extern "C" {
@@ -406,12 +403,12 @@ int b2_launch_partition(const uint8_t* bins_col, int64_t col_stride, const int32
 #undef B2_PART_LAUNCH
   return (int)cudaGetLastError();
 }
-int b2_launch_leaf_sums(const float2* gh, const int32_t* ridx0, const int32_t* ridx1, const void* work, const B2LevelCtl* ctl,
-                        int max_chunks, const int32_t* qexp, int leaf_bits, long long* sums, uint16_t* pos, int num_sms,
-                        cudaStream_t stream) {
+int b2_launch_leaf_sums(const float2* gh, const int32_t* ridx0, const int32_t* ridx1, const B2SegWork* work,
+                        const B2LevelCtl* ctl, int max_chunks, const int32_t* qexp, int leaf_bits, long long* sums,
+                        uint16_t* pos, int num_sms, cudaStream_t stream) {
   if (max_chunks <= 0) return 0;
   int grid = max_chunks < num_sms * 8 ? max_chunks : num_sms * 8;
-  b2::leaf_sums_kernel<<<grid, 256, 0, stream>>>(gh, ridx0, ridx1, (const b2::SegWork*)work, ctl, qexp, leaf_bits, sums, pos);
+  b2::leaf_sums_kernel<<<grid, 256, 0, stream>>>(gh, ridx0, ridx1, work, ctl, qexp, leaf_bits, sums, pos);
   return (int)cudaGetLastError();
 }
 int b2_launch_final_assign(const uint8_t* bins_col, int64_t col_stride, const int32_t* ridx_in, const B2SplitWork* work,
@@ -461,13 +458,6 @@ int b2_launch_margin_update_vector(float* margin, int T, const uint16_t* pos, co
   int64_t want = (n + 255) / 256;
   int grid = (int)(want < (int64_t)num_sms * 16 ? want : (int64_t)num_sms * 16);
   b2::margin_update_vector_kernel<<<grid, 256, 0, stream>>>(margin, T, pos, leaf_vec, n);
-  return (int)cudaGetLastError();
-}
-int b2_launch_iota(int32_t* out, int64_t n, cudaStream_t stream) {
-  if (n <= 0) return 0;
-  int grid = (int)((n + 1023) / 1024);
-  if (grid > 4096) grid = 4096;
-  b2::iota_kernel<<<grid, 256, 0, stream>>>(out, n);
   return (int)cudaGetLastError();
 }
 }

@@ -12,6 +12,7 @@
 #include <cub/block/block_scan.cuh>
 #include "common.cuh"
 #include "objective_common.cuh"
+#include "launch.h"
 
 namespace b2 {
 

@@ -14,6 +14,7 @@
 #include <cfloat>
 #include "common.cuh"
 #include "objective_common.cuh"
+#include "launch.h"
 
 namespace b2 {
 
@@ -82,9 +83,6 @@ __global__ void rank_label_check_kernel(const float* __restrict__ label, int64_t
   if (__any_sync(0xffffffffu, b1) && (threadIdx.x & 31) == 0) atomicOr(&bad[1], 1u);
   if (__any_sync(0xffffffffu, b2) && (threadIdx.x & 31) == 0) atomicOr(&bad[2], 1u);
 }
-
-// the pair weight of lambdarank_gradient_kernel: 1, |Delta NDCG| or |Delta AP|
-enum RankMode { kRankPairwise = 0, kRankNdcg = 1, kRankMap = 2 };
 
 // the pair (a, b) of model positions ra < rb with different labels: returns (float lambda, float H); *a_high says
 // whether a has the larger label.  rank:map reads the group's hit counts R and hit prefixes A (inclusive, by model
@@ -244,7 +242,7 @@ lambdarank_gradient_kernel(const int64_t* __restrict__ gptr, int64_t n_groups, c
   if (absmax) absmax_publish(mg, mh, absmax);
 }
 
-// metric ids (engine.cu): 16 ndcg, 17 map, 18 pre; k = 0 means the whole group; minus: the score of a group without a
+// metric: ndcg, map or pre; k = 0 means the whole group; minus: the score of a group without a
 // relevant row (IDCG = 0 / no label != 0) is 0 instead of 1.  One thread per group, positions ascending, binary64.
 __global__ void rank_metric_kernel(int metric, int k, int minus, int exp_gain, const int64_t* __restrict__ gptr,
                                    int64_t n_groups, const int32_t* __restrict__ prow, const float* __restrict__ label,
@@ -253,14 +251,14 @@ __global__ void rank_metric_kernel(int metric, int k, int minus, int exp_gain, c
   for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n_groups; g += (int64_t)gridDim.x * blockDim.x) {
     const int64_t b = gptr[g], n = gptr[g + 1] - b, kk = k > 0 ? k : n, t_end = n < kk ? n : kk;
     double v;
-    if (metric == 16) {
+    if (metric == kMetricNdcg) {
       double dcg = 0.0, idcg = 0.0;
       for (int64_t t = 0; t < t_end; ++t) {
         dcg = B2_DA(dcg, B2_DM(rank_gain(label[prow[b + t]], exp_gain), disc[t]));
         idcg = B2_DA(idcg, B2_DM(rank_gain(rank_key_value(lkeys[b + t]), exp_gain), disc[t]));
       }
       v = idcg == 0.0 ? (minus ? 0.0 : 1.0) : B2_DD(dcg, idcg);
-    } else if (metric == 17) {
+    } else if (metric == kMetricMap) {
       int64_t rel = 0;
       for (int64_t t = 0; t < n; ++t) rel += label[b + t] != 0.0f;
       if (rel == 0) {
@@ -353,8 +351,8 @@ int b2_launch_rank_label_check(const float* label, int64_t n, int exp_gain, int 
   b2::rank_label_check_kernel<<<rank_grid(n, 256, num_sms), 256, 0, s>>>(label, n, exp_gain, binary, bad);
   return (int)cudaGetLastError();
 }
-// mode: 0 rank:pairwise, 1 rank:ndcg, 2 rank:map.  max_group: the largest group (sizes the shared-memory stage);
-// scratch_m / y / p: [n] when max_group > b2_rank_stage_rows(), and with mode 2 scratch_a / r too (null otherwise)
+// mode: B2RankMode.  max_group: the largest group (sizes the shared-memory stage);
+// scratch_m / y / p: [n] when max_group > b2_rank_stage_rows(), and with kRankMap scratch_a / r too (null otherwise)
 int b2_launch_lambdarank_gradient(int mode, const int64_t* gptr, int64_t n_groups, int64_t max_group, const uint32_t* skeys,
                                   const int32_t* srow, const float* label, const double* inv_idcg, const double* disc, int k,
                                   int exp_gain, float* scratch_m, float* scratch_y, double* scratch_p, double* scratch_a,
@@ -364,25 +362,25 @@ int b2_launch_lambdarank_gradient(int mode, const int64_t* gptr, int64_t n_group
   // the stage holds the largest group, up to kRankStageRows rows: at most 32 KB for pairwise / ndcg (16 B per row, no
   // opt-in to large shared memory); rank:map adds 12 B per row and the chunk totals, up to 57.5 KB, and opts in
   const int stage = (int)(max_group < b2::kRankStageRows ? (max_group < 1 ? 1 : max_group) : b2::kRankStageRows);
-  if (mode == b2::kRankMap) {
+  if (mode == kRankMap) {
     const size_t smem = (size_t)stage * (8 + 4 + 4 + 8 + 4) + b2::kRankThreads * (8 + 4);
     if (smem > 48 * 1024) {
-      const cudaError_t e = cudaFuncSetAttribute(b2::lambdarank_gradient_kernel<b2::kRankMap>,
+      const cudaError_t e = cudaFuncSetAttribute(b2::lambdarank_gradient_kernel<kRankMap>,
                                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return (int)e;
     }
-    b2::lambdarank_gradient_kernel<b2::kRankMap><<<grid, b2::kRankThreads, smem, s>>>(
+    b2::lambdarank_gradient_kernel<kRankMap><<<grid, b2::kRankThreads, smem, s>>>(
         gptr, n_groups, skeys, srow, label, inv_idcg, disc, k, exp_gain, stage, scratch_m, scratch_y, scratch_p, gh, absmax, err,
         scratch_a, scratch_r);
     return (int)cudaGetLastError();
   }
   const size_t smem = (size_t)stage * (8 + 4 + 4);
-  if (mode == b2::kRankNdcg)
-    b2::lambdarank_gradient_kernel<b2::kRankNdcg><<<grid, b2::kRankThreads, smem, s>>>(gptr, n_groups, skeys, srow, label, inv_idcg, disc, k,
+  if (mode == kRankNdcg)
+    b2::lambdarank_gradient_kernel<kRankNdcg><<<grid, b2::kRankThreads, smem, s>>>(gptr, n_groups, skeys, srow, label, inv_idcg, disc, k,
                                                                             exp_gain, stage, scratch_m, scratch_y, scratch_p, gh,
                                                                             absmax, err, nullptr, nullptr);
   else
-    b2::lambdarank_gradient_kernel<b2::kRankPairwise><<<grid, b2::kRankThreads, smem, s>>>(gptr, n_groups, skeys, srow, label, inv_idcg, disc, k,
+    b2::lambdarank_gradient_kernel<kRankPairwise><<<grid, b2::kRankThreads, smem, s>>>(gptr, n_groups, skeys, srow, label, inv_idcg, disc, k,
                                                                              exp_gain, stage, scratch_m, scratch_y, scratch_p, gh,
                                                                              absmax, err, nullptr, nullptr);
   return (int)cudaGetLastError();

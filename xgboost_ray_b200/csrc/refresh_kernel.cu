@@ -10,6 +10,7 @@
 // The sums use the round's quantisation exponents (max |g|, |h| over all ranks), so they are exact integers that do not
 // depend on row order or sharding: only the leaf sums are exchanged, every rank derives the rest itself.
 #include "common.cuh"
+#include "launch.h"
 
 namespace b2 {
 

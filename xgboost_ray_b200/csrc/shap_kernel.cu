@@ -21,6 +21,7 @@
 #include <stdint.h>
 
 #include "common.cuh"
+#include "launch.h"
 
 namespace b2 {
 

@@ -13,6 +13,7 @@
 #include <cub/cub.cuh>
 
 #include "common.cuh"
+#include "launch.h"
 
 namespace b2 {
 

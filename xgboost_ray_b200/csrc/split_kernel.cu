@@ -12,6 +12,7 @@
 #include "common.cuh"
 #include "decide.cuh"
 #include "sampling.cuh"
+#include "launch.h"
 
 namespace b2 {
 
