@@ -1,7 +1,7 @@
 """DART (booster="dart") on top of the oracle: the drop draw, the weight normalisation and the weighted margins in
 NumPy, the trees grown by the oracle (`train`) from gradients taken at the drop margin.
 
-What the engine implements (csrc/engine.cu dart_drop_set / dart_prepare, csrc/dart_kernel.cu; DESIGN.md 2), written out
+What the engine implements (csrc/round.cu dart_drop_set / dart_prepare, csrc/dart_kernel.cu; DESIGN.md 2), written out
 independently so that the GPU tests can replay a trained model round by round:
   * draw u_j = hash4(seed, r, j, SCOPE_DART) / 2^32 (the counter-based hash of csrc/sampling.cuh), r = rounds already
     in the model; j = 0xFFFFFFFF decides skip_drop, j = 0xFFFFFFFE the one_drop pick;

@@ -1,7 +1,7 @@
 """Multi-target regression and multi-label classification (a label of T > 1 columns) on top of the oracle.
 
 What the engine implements (csrc/objective_kernel.cu gradient_multi_target_kernel / metric_multi_target_kernel,
-csrc/engine.cu estimate_base_score; DESIGN.md 2 item 18), written out per column so that the GPU tests can replay a
+csrc/round.cu estimate_base_score; DESIGN.md 2 item 18), written out per column so that the GPU tests can replay a
 trained model round by round:
   * the gradients of column k are the single-target binary32 sequence of tests/objective_reference.py on margin[:, k] and
     label[:, k], with the row's weight (scale_pos_weight applies per element where y == 1);

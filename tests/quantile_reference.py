@@ -1,8 +1,8 @@
 """reg:quantileerror on top of the oracle: pinball gradients and the leaf refresh in NumPy, the trees grown by the oracle
 from those gradients as custom gradients.
 
-What the engine implements (csrc/quantile_kernel.cu, csrc/engine.cu quantile_select / estimate_base_score; DESIGN.md 2),
-written out literally with np.sort so that the GPU tests can replay a trained model round by round:
+What the engine implements (csrc/quantile_kernel.cu, csrc/tree.cu quantile_select, csrc/round.cu estimate_base_score;
+DESIGN.md 2), written out literally with np.sort so that the GPU tests can replay a trained model round by round:
   * gradients of output k at margin m: d = fp32(m_k - y), g = fp32((d >= 0 ? fp32(1 - alpha_k) : -alpha_k) * w), h = w;
   * after tree k of a round is grown, every leaf value becomes fp32(q * eta), q the alpha_k-quantile of the residuals
     r = fp32(y - m_k) of the leaf's rows with a nonzero hessian (`leaf_quantile`); a leaf without such rows keeps the

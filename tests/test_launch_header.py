@@ -1,9 +1,10 @@
 """The kernel launchers are declared once, in csrc/launch.h, and both sides compile against it.
 
 The launchers have C linkage, so a prototype kept apart from its definition links even when the two disagree, and the
-kernel then reads shifted arguments at run time.  With one header included by engine.cu and by every defining file, a
-mismatch is a compile error.  These checks keep it that way: every b2_* function a kernel file defines for the host is
-declared in the header and nowhere else."""
+kernel then reads shifted arguments at run time.  With one header included by every host file that calls a launcher and
+by every defining file, a mismatch is a compile error.  These checks keep it that way: every b2_* function a kernel file
+defines for the host is declared in the header and nowhere else.  The host files are host.h and the .cu files that
+include it (engine.cu, tree.cu, ...)."""
 import os
 import re
 
@@ -57,6 +58,20 @@ def _kernel_files():
     return sorted(f for f in os.listdir(CSRC) if f.endswith(".cu"))
 
 
+def _includes(text, name):
+    return re.search(r'^\s*#\s*include\s+"%s"' % re.escape(name), text, re.M) is not None
+
+
+def _host_files():
+    files = ["host.h"] + [f for f in _kernel_files() if _includes(_source(f), "host.h")]
+    assert "engine.cu" in files and len(files) >= 8, files
+    return files
+
+
+def _calls_launcher(text, launchers):
+    return any(name in launchers for name in re.findall(r"\b(b2_\w+)\s*\(", text))
+
+
 def test_header_declares_exactly_the_defined_launchers():
     defined = {}
     for f in _kernel_files():
@@ -73,16 +88,21 @@ def test_header_declares_exactly_the_defined_launchers():
 
 
 def test_defining_files_and_engine_include_the_header():
-    include = re.compile(r'^\s*#\s*include\s+"%s"' % re.escape(HEADER), re.M)
-    users = [f for f in _kernel_files() if _defined(_source(f))] + ["engine.cu"]
+    launchers = _declared(_source(HEADER))
+    users = [f for f in _kernel_files() if _defined(_source(f))]
+    users += [f for f in _host_files() if _calls_launcher(_source(f), launchers)]
+    assert "engine.cu" in users and "tree.cu" in users
     for f in users:
-        assert include.search(_source(f)), "%s does not include %s" % (f, HEADER)
+        assert _includes(_source(f), HEADER), "%s does not include %s" % (f, HEADER)
 
 
 def test_engine_keeps_no_launcher_prototypes():
-    text = _source("engine.cu")
-    local = sorted(_declared(text) | _defined(text))
-    assert not local, "engine.cu declares launchers of its own: %s" % ", ".join(local)
-    # the only extern "C" block of engine.cu is the C ABI of include/b2hist.h
-    blocks = list(_extern_c_blocks(text))
-    assert len(blocks) == 1 and re.search(r"\bint\s+B2_BoosterCreate\s*\(", blocks[0])
+    abi = []
+    for f in _host_files():
+        text = _source(f)
+        local = sorted(_declared(text) | _defined(text) | set(re.findall(r'extern\s+"C"\s+[^{;]*?\b(b2_\w+)\s*\(', text)))
+        assert not local, "%s declares launchers of its own: %s" % (f, ", ".join(local))
+        abi += [(f, block) for block in _extern_c_blocks(text)]
+    # the only extern "C" block of the host files is the C ABI of include/b2hist.h, in engine.cu
+    assert len(abi) == 1 and abi[0][0] == "engine.cu", [f for f, _ in abi]
+    assert re.search(r"\bint\s+B2_BoosterCreate\s*\(", abi[0][1])

@@ -32,6 +32,13 @@ SOURCES = {
     "dart_kernel.cu": ["--fmad=false"],        # DART margin rebuild, bit-exact vs the weighted predict and the reference
     "quantile_kernel.cu": ["--fmad=false"],    # quantile gradients, metric and leaf refresh, bit-exact vs the reference
     "refresh_kernel.cu": ["--fmad=false"],     # refresh updater: leaf sums on raw rows, node statistics bottom-up
+    # host side (host.h): no device code
+    "device.cu": [],
+    "matrix.cu": [],
+    "params.cu": [],
+    "tree.cu": [],
+    "round.cu": [],
+    "predict.cu": [],
     "engine.cu": [],
 }
 

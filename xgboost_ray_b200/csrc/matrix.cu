@@ -1,0 +1,243 @@
+// matrix.cu -- the matrix registry, the feature -> group layout of the bin matrix, the GPU sketch that makes the cuts,
+// the checks of categorical codes, and the binning of the raw values.
+#include <string.h>
+
+#include <climits>
+
+#include "host.h"
+#include "launch.h"
+
+namespace b2host __attribute__((visibility("hidden"))) {
+
+// ids of the matrices that are alive: a Booster's evaluation cache is keyed by the id, never by the address (a freed
+// matrix and a new one of the same shape can share an address)
+std::mutex g_matrix_mu;
+std::set<uint64_t> g_live_matrices;
+uint64_t g_next_matrix_uid = 1;
+
+// Feature -> (group, slot) layout of the bin matrix: the features are spread EVENLY over ceil(F / 32) groups, so that
+// every CTA type of the histogram kernel (one pair of groups) costs the same and the types walk the chunk list in lock
+// step -- the CTAs that read the two 64-byte halves of a row do it at the same time and the row is fetched from DRAM
+// once.  (Packing the F mod 32 leftover features into a narrow last group saves padding-slot atomics, but the types then
+// differ in cost, drift apart and read the halves of a row at different times; DESIGN.md 4.1.)
+void setup_groups(Matrix* m) {
+  const int F = m->F;
+  m->n_groups = (F + B2_GROUP_SLOTS - 1) / B2_GROUP_SLOTS;
+  if (m->n_groups < 1) m->n_groups = 1;
+  m->row_stride = m->n_groups * B2_GROUP_SLOTS;
+  m->group_first.assign(m->n_groups, 0);
+  m->group_size.assign(m->n_groups, 0);
+  m->feat_byte.assign(F, 0);
+  const int base = F / m->n_groups, rem = F % m->n_groups;
+  int f = 0;
+  for (int g = 0; g < m->n_groups; ++g) {
+    const int sz = base + (g < rem ? 1 : 0);
+    m->group_first[g] = f; m->group_size[g] = sz;
+    for (int s = 0; s < sz; ++s) m->feat_byte[f + s] = g * B2_GROUP_SLOTS + s;
+    f += sz;
+  }
+}
+
+void upload_cuts(Matrix* m) {
+  cudaStream_t s = m->ctx->stream;
+  m->nbins.resize(m->F);
+  for (int f = 0; f < m->F; ++f) m->nbins[f] = m->cut_ptrs[f + 1] - m->cut_ptrs[f];
+  upload(m->d_group_first, m->group_first, s); upload(m->d_group_size, m->group_size, s);
+  upload(m->d_feat_byte, m->feat_byte, s); upload(m->d_cut_ptrs, m->cut_ptrs, s);
+  upload(m->d_cut_vals, m->cut_vals, s); upload(m->d_nbins, m->nbins, s);
+  upload(m->d_has_missing, m->has_missing, s);
+  if (m->is_cat.empty()) m->is_cat.assign(m->F, 0);
+  upload(m->d_is_cat, m->is_cat, s); upload(m->d_cat_feats, m->cat_feats, s);
+  CUDA_CHECK(cudaStreamSynchronize(s));
+}
+
+// Categorical features: global {max code, has missing, largest invalid value's key} per entry of m->cat_feats
+// (cat_stats_kernel, allreduce max over the ranks).  Synchronises the stream.
+std::vector<int32_t> category_stats(Matrix* m, Comm* comm) {
+  cudaStream_t s = m->ctx->stream;
+  const int n_cat = (int)m->cat_feats.size();
+  std::vector<int32_t> h_cat((size_t)n_cat * 3);
+  if (n_cat == 0) { CUDA_CHECK(cudaStreamSynchronize(s)); return h_cat; }   // callers read earlier copies after this
+  for (int i = 0; i < n_cat; ++i) { h_cat[i * 3] = -1; h_cat[i * 3 + 1] = 0; h_cat[i * 3 + 2] = INT_MIN; }
+  DevBuf<int32_t> d_cat, d_catf;
+  d_cat.ensure((size_t)n_cat * 3); d_catf.ensure((size_t)n_cat);
+  CUDA_CHECK(cudaMemcpyAsync(d_cat.p, h_cat.data(), (size_t)n_cat * 3 * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  CUDA_CHECK(cudaMemcpyAsync(d_catf.p, m->cat_feats.data(), (size_t)n_cat * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  LAUNCH_CHECK(b2_launch_cat_stats(m->raw.p, m->n, m->F, m->missing, d_catf.p, n_cat, d_cat.p, m->ctx->num_sms, s));
+  allreduce(comm, d_cat.p, (size_t)n_cat * 3, kNcclInt32, kNcclMax, s);
+  CUDA_CHECK(cudaMemcpyAsync(h_cat.data(), d_cat.p, (size_t)n_cat * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  return h_cat;
+}
+// the value behind cat_stats_kernel's signed order-preserving key
+double category_key_value(int32_t key) {
+  const uint32_t k = (uint32_t)key ^ 0x80000000u;
+  const uint32_t u = (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k;
+  float f; memcpy(&f, &u, sizeof(f));
+  return (double)f;
+}
+
+// Borrowed cuts (a ref matrix, or the frozen cuts of a restart) were made from other data.  bin_kernel clamps a code
+// they do not know to their largest code (a negative one to 0), and a code of 255 shares bin 255 with the missing
+// values, while prediction sends every unknown code left: training would see another category than predict().
+// Such codes are refused, as make_cuts refuses codes that are not valid, instead of silently changing the model.
+void check_borrowed_categories(Matrix* m, Comm* comm) {
+  const std::vector<int32_t> h_cat = category_stats(m, comm);
+  for (size_t i = 0; i < m->cat_feats.size(); ++i) {
+    const int f = m->cat_feats[i], mx = h_cat[i * 3], miss = h_cat[i * 3 + 1];
+    const int known = m->cut_ptrs[f + 1] - m->cut_ptrs[f] - 1;   // the cuts of a categorical feature are the codes 0..known
+    if (h_cat[i * 3 + 2] != INT_MIN)
+      fail("categorical feature %d: category codes must be integers in [0, %d], got %.9g", f, known,
+           category_key_value(h_cat[i * 3 + 2]));
+    if (mx > known)
+      fail("categorical feature %d: category code %d is above the largest code %d of the cuts this matrix is binned with",
+           f, mx, known);
+    if (miss && known > 254)
+      fail("categorical feature %d: the feature has missing values, but its cuts use bin 255 (the missing sentinel) for "
+           "category code 255", f);
+    // cuts borrowed from a matrix without missing values: the split scan and partition must still treat bin 255 as
+    // missing (default direction), as prediction does, instead of as an unknown category.  The oracle applies the same
+    // rule when it trains with borrowed cuts (oracle.train(cuts=...), Cuts.borrowed_by).
+    if (miss) m->has_missing[f] = 1;
+  }
+}
+
+// GPU sketch: exact global summary per feature -> cuts (sketch.cu).  No host round trip per feature.
+// Multi-GPU: the column keys of every rank are allgathered (padded to the largest shard); feature f is
+// sorted and pruned only by its owner rank f % world, and the cut tables are merged with one integer
+// allreduce (non-owners contribute zeros), so every rank ends up with identical global cuts.
+void make_cuts(Matrix* m, Comm* comm, int max_bin) {
+  Ctx* ctx = m->ctx; cudaStream_t s = ctx->stream;
+  if (max_bin < 2 || max_bin > 256) fail("max_bin must be in [2, 256] (uint8 bin matrix), got %d", max_bin);
+  if (!m->has_raw) fail("matrix has no raw data to sketch");
+  const int world = comm ? comm->world : 1, rank = comm ? comm->rank : 0;
+  // largest shard and global row count
+  DevBuf<long long> d_cnt; d_cnt.ensure(2);
+  long long h_cnt[2] = {m->n, m->n};
+  if (world > 1) {
+    CUDA_CHECK(cudaMemcpyAsync(d_cnt.p, h_cnt, sizeof(h_cnt), cudaMemcpyHostToDevice, s));
+    allreduce(comm, d_cnt.p, 1, kNcclInt64, kNcclMax, s);
+    allreduce(comm, d_cnt.p + 1, 1, kNcclInt64, kNcclSum, s);
+    CUDA_CHECK(cudaMemcpyAsync(h_cnt, d_cnt.p, sizeof(h_cnt), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+  }
+  const int64_t n_pad = h_cnt[0], n_total = n_pad * world; const long long n_global = h_cnt[1];
+  const int B = b2_extract_batch(); const int F = m->F;
+  DevBuf<uint32_t> keys_local, keys_all, keys_sorted;
+  DevBuf<int32_t> flags, idx, m_scratch; DevBuf<float> uval; DevBuf<long long> rmin, nvalid;
+  DevBuf<int32_t> d_tab;   // [F*256 cut bits][F n_cuts][F min bits][F has_missing]
+  DevBuf<uint8_t> temp;
+  const size_t nt = (size_t)std::max<int64_t>(n_total, 1);
+  keys_local.ensure((size_t)std::max<int64_t>(n_pad, 1) * B);
+  if (world > 1) keys_all.ensure(nt);
+  keys_sorted.ensure(nt); flags.ensure(nt); idx.ensure(nt); uval.ensure(nt); rmin.ensure(nt); m_scratch.ensure(1); nvalid.ensure(2);
+  // sample weights make the sketch a weighted one (xgboost SketchContainer pushes info.weights_): quantise them to
+  // integers with a global power-of-two scale so that the weighted ranks are exact and identical on every rank
+  DevBuf<int32_t> wq_local, wq_all, wq_sorted; DevBuf<long long> wpre; DevBuf<uint32_t> d_wmax;
+  const int32_t* wq = nullptr;
+  {
+    long long h_has[1] = {m->n_weight > 0 ? 1 : 0};
+    if (world > 1) {   // a rank whose shard came without weights while others have them would desynchronise the collectives
+      CUDA_CHECK(cudaMemcpyAsync(d_cnt.p, h_has, sizeof(h_has), cudaMemcpyHostToDevice, s));
+      allreduce(comm, d_cnt.p, 1, kNcclInt64, kNcclMax, s);
+      CUDA_CHECK(cudaMemcpyAsync(h_has, d_cnt.p, sizeof(h_has), cudaMemcpyDeviceToHost, s));
+      CUDA_CHECK(cudaStreamSynchronize(s));
+    }
+    if (h_has[0]) {
+      if (m->n_weight != m->n) fail("sample weights are set on some ranks only (this rank has %lld for %lld rows)", (long long)m->n_weight, (long long)m->n);
+      d_wmax.ensure(2);
+      CUDA_CHECK(cudaMemsetAsync(d_wmax.p, 0, 2 * sizeof(uint32_t), s));
+      LAUNCH_CHECK(b2_launch_weight_absmax(m->weight.p, m->n, d_wmax.p, ctx->num_sms, s));
+      allreduce(comm, d_wmax.p, 2, kNcclUint32, kNcclMax, s);
+      uint32_t h_w[2];
+      CUDA_CHECK(cudaMemcpyAsync(h_w, d_wmax.p, sizeof(h_w), cudaMemcpyDeviceToHost, s));
+      CUDA_CHECK(cudaStreamSynchronize(s));
+      if (h_w[1]) fail("sample weights must be finite and non-negative");
+      wq_local.ensure((size_t)std::max<int64_t>(n_pad, 1));
+      LAUNCH_CHECK(b2_launch_weight_quantize(m->weight.p, m->n, n_pad, d_wmax.p, wq_local.p, ctx->num_sms, s));
+      wq = wq_local.p;
+      if (world > 1) {
+        wq_all.ensure(nt);
+        NCCL_CHECK(nccl()->AllGather(wq_local.p, wq_all.p, (size_t)n_pad, kNcclInt32, comm->comm, s));
+        wq = wq_all.p;
+      }
+      wq_sorted.ensure(nt); wpre.ensure(nt);
+    }
+  }
+  const size_t temp_bytes = b2_sort_temp_bytes(n_total > 0 ? n_total : 1);
+  temp.ensure(temp_bytes ? temp_bytes : 1);
+  const size_t tab_n = (size_t)F * 256 + 3 * (size_t)F;
+  d_tab.ensure(tab_n);
+  CUDA_CHECK(cudaMemsetAsync(d_tab.p, 0, tab_n * sizeof(int32_t), s));
+  float* d_cuts = (float*)d_tab.p; int32_t* d_ncuts = d_tab.p + (size_t)F * 256;
+  float* d_mins = (float*)(d_ncuts + F); int32_t* d_hasmiss = d_ncuts + 2 * (size_t)F;
+  if (m->is_cat.empty()) m->is_cat.assign(F, 0);
+  for (int f0 = 0; f0 < F; f0 += B) {
+    const int nf = std::min(B, F - f0);
+    bool any_numeric = false;
+    for (int j = 0; j < nf; ++j) any_numeric = any_numeric || !m->is_cat[f0 + j];
+    if (!any_numeric) continue;
+    LAUNCH_CHECK(b2_launch_extract_keys(m->raw.p, m->n, F, f0, nf, m->missing, keys_local.p, n_pad, ctx->num_sms, s));
+    for (int j = 0; j < nf; ++j) {
+      const int f = f0 + j;
+      if (m->is_cat[f]) continue;   // categorical: cuts are the codes 0..max (below)
+      const uint32_t* kin = keys_local.p + (size_t)j * n_pad;
+      if (world > 1) {
+        NCCL_CHECK(nccl()->AllGather(kin, keys_all.p, (size_t)n_pad, kNcclUint32, comm->comm, s));
+        kin = keys_all.p;
+        if (f % world != rank) continue;   // the owner rank sketches this feature
+      }
+      LAUNCH_CHECK(b2_sketch_column(kin, wq, keys_sorted.p, wq_sorted.p, wpre.p, n_total, n_global, temp.p, temp_bytes, flags.p, idx.p, uval.p, rmin.p,
+                                    m_scratch.p, nvalid.p, max_bin, d_cuts + (size_t)f * 256, d_ncuts + f, d_mins + f,
+                                    d_hasmiss + f, ctx->num_sms, s));
+    }
+  }
+  // merge the per-owner tables: exact because every entry is written by exactly one rank (others hold 0 bits)
+  allreduce(comm, d_tab.p, tab_n, kNcclInt32, kNcclSum, s);
+  std::vector<int32_t> h_tab(tab_n);
+  CUDA_CHECK(cudaMemcpyAsync(h_tab.data(), d_tab.p, tab_n * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  const int n_cat = (int)m->cat_feats.size();
+  const std::vector<int32_t> h_cat = category_stats(m, comm);   // synchronises the stream
+  for (int i = 0; i < n_cat; ++i) {
+    const int f = m->cat_feats[i], mx = h_cat[i * 3], miss = h_cat[i * 3 + 1];
+    if (h_cat[i * 3 + 2] != INT_MIN || (miss && mx > 254))
+      fail("categorical feature %d: category codes must be integers in [0, %d]%s, got %.9g", f, miss ? 254 : 255,
+           miss ? " (the feature has missing values; bin 255 is the missing sentinel)" : "",
+           h_cat[i * 3 + 2] != INT_MIN ? category_key_value(h_cat[i * 3 + 2]) : (double)mx);
+    int32_t* t = h_tab.data();
+    float* cuts_f = (float*)t + (size_t)f * 256;
+    const int nc = mx < 0 ? 1 : mx + 1;
+    for (int k = 0; k < nc; ++k) cuts_f[k] = (float)k;
+    t[(size_t)F * 256 + f] = nc;
+    ((float*)(t + (size_t)F * 256 + F))[f] = -1e-5f;
+    t[(size_t)F * 256 + 2 * (size_t)F + f] = miss;
+  }
+  const float* h_cuts = (const float*)h_tab.data(); const int32_t* h_nc = h_tab.data() + (size_t)F * 256;
+  const float* h_mins = (const float*)(h_nc + F); const int32_t* h_hm = h_nc + 2 * (size_t)F;
+  m->cut_ptrs.assign(F + 1, 0);
+  m->cut_vals.clear(); m->min_vals.assign(h_mins, h_mins + F); m->has_missing.assign(F, 0);
+  for (int f = 0; f < F; ++f) {
+    if (h_nc[f] < 1 || h_nc[f] > 256) fail("sketch produced %d cuts for feature %d", h_nc[f], f);
+    m->cut_ptrs[f + 1] = m->cut_ptrs[f] + h_nc[f];
+    m->cut_vals.insert(m->cut_vals.end(), h_cuts + (size_t)f * 256, h_cuts + (size_t)f * 256 + h_nc[f]);
+    m->has_missing[f] = h_hm[f] ? 1 : 0;
+  }
+  m->max_bin = max_bin;
+}
+
+void bin_matrix(Matrix* m) {
+  Ctx* ctx = m->ctx; cudaStream_t s = ctx->stream;
+  setup_groups(m);
+  upload_cuts(m);
+  m->bins.ensure((size_t)std::max<int64_t>(m->n, 1) * m->row_stride);
+  CUDA_CHECK(cudaMemsetAsync(m->bins.p, 0, (size_t)std::max<int64_t>(m->n, 1) * m->row_stride, s));
+  m->col_stride = (std::max<int64_t>(m->n, 1) + 127) & ~(int64_t)127;
+  m->bins_col.ensure((size_t)m->col_stride * m->F);
+  LAUNCH_CHECK(b2_launch_bin(m->raw.p, m->n, m->F, m->missing, m->d_cut_ptrs.p, m->d_cut_vals.p, m->d_feat_byte.p,
+                             m->any_cat() ? m->d_is_cat.p : nullptr, m->row_stride, m->bins.p, m->bins_col.p, m->col_stride,
+                             ctx->num_sms, s));
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  m->quantized = true;
+}
+
+}  // namespace b2host

@@ -1,0 +1,367 @@
+// params.cu -- the booster parameters: parsing and checking the "key=value" text of B2_BoosterCreate, the objective
+// predicates, the host replicas of the leaf-weight formula, and the eval_metric names.
+#include <math.h>
+#include <stdlib.h>
+
+#include "host.h"
+
+namespace b2host __attribute__((visibility("hidden"))) {
+
+bool obj_log_link(int o) { return o == kObjPoisson || o == kObjGamma || o == kObjTweedie || o == kObjAft; }
+bool obj_sigmoid(int o) { return o == kObjLogistic || o == kObjRegLogistic; }
+bool obj_rank(int o) { return o == kObjRankPairwise || o == kObjRankNdcg || o == kObjRankMap; }
+// objectives whose gradient kernel reports non-finite gradient pairs (gradient_param_kernel).  reg:quantileerror's
+// pairs are finite for finite labels and weights (both checked before the first round), so its rounds stay pipelined.
+bool obj_checks_finite(int o) { return o >= kObjSquaredLog && o != kObjQuantile; }
+// objectives that take a label of T > 1 columns (xgboost's RegLossObj family and pseudo-Huber, which read labels.Shape(1))
+bool obj_multi_target(int o) {
+  return o == kObjSquaredError || o == kObjLogistic || o == kObjRegLogistic || o == kObjLogitRaw || o == kObjSquaredLog ||
+         o == kObjPseudoHuber;
+}
+constexpr int kMaxVectorTargets = 64;   // vector-leaf trees: the level histograms are T times a scalar tree's
+
+// "0,1;2,3,4" -> {{0, 1}, {2, 3, 4}}; empty sets are dropped, the indices are checked against F in B2_BoosterCreate
+std::vector<std::vector<int64_t>> parse_interaction_sets(const std::string& v) {
+  std::vector<std::vector<int64_t>> sets;
+  size_t pos = 0;
+  while (pos <= v.size()) {
+    size_t semi = v.find(';', pos);
+    if (semi == std::string::npos) semi = v.size();
+    std::vector<int64_t> set;
+    size_t q = pos;
+    while (q < semi) {
+      size_t comma = v.find(',', q);
+      if (comma == std::string::npos || comma > semi) comma = semi;
+      const std::string tok = v.substr(q, comma - q);
+      char* end = nullptr;
+      const long long f = strtoll(tok.c_str(), &end, 10);
+      if (tok.empty() || *end != '\0' || f < 0)
+        fail("interaction_constraints: '%s' is not a feature index (expected sets like 0,1;2,3,4)", tok.c_str());
+      set.push_back(f);
+      q = comma + 1;
+    }
+    if (!set.empty()) sets.push_back(set);
+    pos = semi + 1;
+  }
+  return sets;
+}
+
+// quantile_alpha as "a,b,c" (brackets allowed): every alpha finite with 0 < alpha < 1
+std::vector<float> parse_quantile_alpha(std::string v) {
+  for (char& c : v) if (c == '[' || c == ']' || c == '(' || c == ')') c = ' ';
+  std::vector<float> out;
+  size_t pos = 0;
+  while (pos <= v.size()) {
+    size_t comma = v.find(',', pos);
+    if (comma == std::string::npos) comma = v.size();
+    std::string tok = v.substr(pos, comma - pos);
+    const size_t a = tok.find_first_not_of(" \t"), b = tok.find_last_not_of(" \t");
+    tok = a == std::string::npos ? std::string() : tok.substr(a, b - a + 1);
+    char* end = nullptr;
+    const double x = strtod(tok.c_str(), &end);
+    const float f = (float)x;
+    if (tok.empty() || *end != '\0' || !(f > 0.0f && f < 1.0f))
+      fail("quantile_alpha: '%s' is not a number in (0, 1)", tok.c_str());
+    out.push_back(f);
+    pos = comma + 1;
+  }
+  return out;
+}
+
+// T label columns: one output and one tree per round for each (xgboost's multi_strategy=one_output_per_tree)
+void set_targets(Params* p, int T) {
+  if (T < 1 || T > kMaxTargets) fail("num_target must be in [1, %d], got %d", kMaxTargets, T);
+  if (T > 1) {
+    if (!obj_multi_target(p->objective))
+      fail("objective '%s' does not support a label with %d columns (multi-target objectives: reg:squarederror, "
+           "reg:squaredlogerror, reg:pseudohubererror, reg:logistic, binary:logistic, binary:logitraw)",
+           p->objective_name.c_str(), T);
+    if (p->num_class_set)
+      fail("num_class must not be set with a label of %d columns: a multi-target model has one output per column", T);
+    p->num_class = T;
+  }
+  p->num_target = T;
+  if (p->vector_leaf()) {   // DESIGN.md 2 item 19: what vector-leaf trees do not cover yet
+    if (T > kMaxVectorTargets)
+      fail("multi_strategy=multi_output_tree supports at most %d targets, the label has %d columns", kMaxVectorTargets, T);
+    if (p->dart) fail("multi_strategy=multi_output_tree is not supported with booster=dart");
+    if (p->update_mode) fail("process_type=update is not supported with multi_strategy=multi_output_tree");
+    if (p->num_parallel_tree > 1)
+      fail("multi_strategy=multi_output_tree needs num_parallel_tree = 1, got %d", p->num_parallel_tree);
+  }
+}
+
+void parse_params(const char* text, Params* p, int* max_bin_out) {
+  std::string s(text ? text : "");
+  std::map<std::string, std::string> dart_text;
+  size_t pos = 0;
+  while (pos < s.size()) {
+    size_t nl = s.find('\n', pos);
+    if (nl == std::string::npos) nl = s.size();
+    std::string line = s.substr(pos, nl - pos);
+    pos = nl + 1;
+    size_t eq = line.find('=');
+    if (eq == std::string::npos) continue;
+    std::string k = line.substr(0, eq), v = line.substr(eq + 1);
+    auto f = [&]() { return (float)atof(v.c_str()); };
+    auto i = [&]() { return atoi(v.c_str()); };
+    if (k == "objective") {
+      p->objective_name = v;
+      if (v == "reg:squarederror" || v == "reg:linear") p->objective = kObjSquaredError;
+      else if (v == "binary:logistic") p->objective = kObjLogistic;
+      else if (v == "multi:softprob" || v == "multi:softmax") p->objective = kObjSoftprob;
+      else if (v == "reg:logistic") p->objective = kObjRegLogistic;
+      else if (v == "binary:logitraw") p->objective = kObjLogitRaw;
+      else if (v == "reg:squaredlogerror") p->objective = kObjSquaredLog;
+      else if (v == "reg:pseudohubererror") p->objective = kObjPseudoHuber;
+      else if (v == "count:poisson") p->objective = kObjPoisson;
+      else if (v == "reg:gamma") p->objective = kObjGamma;
+      else if (v == "reg:tweedie") p->objective = kObjTweedie;
+      else if (v == "survival:aft") p->objective = kObjAft;
+      else if (v == "rank:pairwise") p->objective = kObjRankPairwise;
+      else if (v == "rank:ndcg") p->objective = kObjRankNdcg;
+      else if (v == "rank:map") p->objective = kObjRankMap;
+      else if (v == "reg:quantileerror") p->objective = kObjQuantile;
+      else fail("unsupported objective '%s' (supported: reg:squarederror, reg:logistic, binary:logistic, binary:logitraw, "
+                "reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie, survival:aft, "
+                "rank:pairwise, rank:ndcg, rank:map, reg:quantileerror, multi:softprob, multi:softmax)", v.c_str());
+    } else if (k == "num_class") { p->num_class = i(); p->num_class_set = true; }
+    else if (k == "num_target") { p->num_target = i(); p->num_target_set = true; }
+    else if (k == "quantile_alpha") p->quantile_alpha = parse_quantile_alpha(v);
+    else if (k == "num_parallel_tree") p->num_parallel_tree = i();
+    else if (k == "max_depth") p->max_depth = i();
+    else if (k == "eta" || k == "learning_rate") p->eta = f();
+    else if (k == "gamma" || k == "min_split_loss") p->gamma = f();
+    else if (k == "min_child_weight") p->min_child_weight = f();
+    else if (k == "lambda" || k == "reg_lambda") p->lambda = f();
+    else if (k == "alpha" || k == "reg_alpha") p->alpha = f();
+    else if (k == "base_score") { p->base_score = f(); p->base_score_set = true; }
+    else if (k == "hist_qbits") p->qbits = i();
+    else if (k == "hist_chunk_rows") p->hist_chunk_rows = i();
+    else if (k == "profile") p->profile = i();
+    else if (k == "num_feature") p->num_feature = i();
+    else if (k == "device") p->device = i();
+    else if (k == "subsample") p->subsample = f();
+    else if (k == "colsample_bytree") p->colsample_bytree = f();
+    else if (k == "colsample_bylevel") p->colsample_bylevel = f();
+    else if (k == "colsample_bynode") p->colsample_bynode = f();
+    else if (k == "seed" || k == "random_state") p->seed = i();
+    else if (k == "scale_pos_weight") p->scale_pos_weight = f();
+    else if (k == "max_delta_step") { p->max_delta_step = f(); p->max_delta_step_set = true; }
+    else if (k == "huber_slope") p->huber_slope = f();
+    else if (k == "tweedie_variance_power") p->tweedie_variance_power = f();
+    else if (k == "aft_loss_distribution") {
+      if (v == "normal") p->aft_dist = kAftNormal;
+      else if (v == "logistic") p->aft_dist = kAftLogistic;
+      else if (v == "extreme") p->aft_dist = kAftExtreme;
+      else fail("aft_loss_distribution must be normal, logistic or extreme, got '%s'", v.c_str());
+    }
+    else if (k == "aft_loss_distribution_scale") p->aft_sigma = f();
+    else if (k == "lambdarank_pair_method") {
+      if (v != "topk") fail("lambdarank_pair_method='%s' is not supported (supported: topk; random pair sampling "
+                            "(mean) is not implemented)", v.c_str());
+    }
+    else if (k == "lambdarank_num_pair_per_sample") {
+      char* end = nullptr;
+      const long long kv = strtoll(v.c_str(), &end, 10);
+      if (v.empty() || *end != '\0' || kv < 1 || kv > INT32_MAX)
+        fail("lambdarank_num_pair_per_sample must be an integer >= 1, got '%s'", v.c_str());
+      p->rank_k = (int)kv;
+    }
+    else if (k == "lambdarank_unbiased" || k == "ndcg_exp_gain") {
+      bool on;
+      if (v == "1" || v == "true" || v == "True") on = true;
+      else if (v == "0" || v == "false" || v == "False") on = false;
+      else fail("%s must be a boolean, got '%s'", k.c_str(), v.c_str());
+      if (k == "ndcg_exp_gain") p->ndcg_exp_gain = on;
+      else if (on) fail("lambdarank_unbiased=true is not supported (position-bias estimation is not implemented)");
+    }
+    else if (k == "max_cat_to_onehot") p->max_cat_to_onehot = i();
+    else if (k == "max_cat_threshold") p->max_cat_threshold = i();
+    else if (k == "max_bin") { if (max_bin_out) *max_bin_out = i(); }
+    else if (k == "interaction_constraints") p->interaction_sets = parse_interaction_sets(v);
+    else if (k == "multi_strategy") {
+      if (v == "one_output_per_tree") p->multi_strategy = 0;
+      else if (v == "multi_output_tree") p->multi_strategy = 1;
+      else fail("multi_strategy='%s' is not supported (supported: one_output_per_tree, multi_output_tree)", v.c_str());
+    }
+    else if (k == "booster") {
+      if (v == "gbtree") p->dart = false;
+      else if (v == "dart") p->dart = true;
+      else fail("booster='%s' is not supported (supported: gbtree, dart)", v.c_str());
+    }
+    else if (k == "rate_drop" || k == "skip_drop" || k == "sample_type" || k == "normalize_type" || k == "one_drop")
+      dart_text[k] = v;   // checked below, and only for booster=dart (gbtree ignores them, like xgboost)
+    else if (k == "process_type") {
+      if (v == "default") p->update_mode = false;
+      else if (v == "update") p->update_mode = true;
+      else fail("process_type='%s' is not supported (supported: default, update)", v.c_str());
+    }
+    else if (k == "updater") p->updater = v;
+    else if (k == "refresh_leaf") {
+      if (v == "1" || v == "true" || v == "True") p->refresh_leaf = true;
+      else if (v == "0" || v == "false" || v == "False") p->refresh_leaf = false;
+      else fail("refresh_leaf must be 0 or 1, got '%s'", v.c_str());
+    }
+    // unknown keys (nthread, tree_method, verbosity, ...) are accepted and ignored, like xgboost
+  }
+  if (p->dart) {
+    for (const auto& kv : dart_text) {
+      const std::string& k = kv.first; const std::string& v = kv.second;
+      if (k == "sample_type") {
+        if (v != "uniform" && v != "weighted") fail("sample_type must be uniform or weighted, got '%s'", v.c_str());
+        p->dart_weighted = v == "weighted";
+      } else if (k == "normalize_type") {
+        if (v != "tree" && v != "forest") fail("normalize_type must be tree or forest, got '%s'", v.c_str());
+        p->dart_forest = v == "forest";
+      } else if (k == "one_drop") {
+        if (v == "1" || v == "true" || v == "True") p->one_drop = true;
+        else if (v == "0" || v == "false" || v == "False") p->one_drop = false;
+        else fail("one_drop must be 0 or 1, got '%s'", v.c_str());
+      } else {
+        char* end = nullptr;
+        const double x = strtod(v.c_str(), &end);
+        if (v.empty() || *end != '\0' || !(x >= 0.0 && x <= 1.0)) fail("%s must be a number in [0, 1], got '%s'", k.c_str(), v.c_str());
+        (k == "rate_drop" ? p->rate_drop : p->skip_drop) = x;
+      }
+    }
+  }
+  if (obj_rank(p->objective) && p->num_class > 1)
+    fail("%s has one output per row: num_class must be 1, got %d", p->objective_name.c_str(), p->num_class);
+  if (p->objective == kObjQuantile) {
+    // rules of this engine (DESIGN.md 2): the outputs are the alphas, the leaf refresh needs the plain gbtree round
+    if (p->num_class_set) fail("reg:quantileerror has one output per quantile_alpha: num_class must not be set");
+    if (p->dart) fail("reg:quantileerror is not supported with booster=dart");
+    if (p->num_parallel_tree > 1) fail("reg:quantileerror needs num_parallel_tree = 1, got %d", p->num_parallel_tree);
+    p->num_class = (int)p->quantile_alpha.size();
+  } else if (p->objective != kObjSoftprob) p->num_class = 1;
+  if (p->objective == kObjSoftprob && p->num_class < 2) fail("multi:softprob needs num_class >= 2");
+  if (p->multi_strategy == 1 && p->objective == kObjSoftprob)
+    fail("multi_strategy=multi_output_tree is not supported with objective '%s' (vector-leaf trees take the multi-target "
+         "objectives: reg:squarederror, reg:squaredlogerror, reg:pseudohubererror, reg:logistic, binary:logistic, "
+         "binary:logitraw)", p->objective_name.c_str());
+  // update mode (DESIGN.md 2 item 20): only the refresh updater, and only where a refreshed leaf is a Newton step
+  if (p->update_mode) {
+    if (p->updater != "refresh")
+      fail("process_type=update needs updater=refresh, got updater='%s' (prune and refresh,prune are not supported)",
+           p->updater.c_str());
+    if (p->dart) fail("process_type=update is not supported with booster=dart");
+    if (p->objective == kObjQuantile)
+      fail("process_type=update is not supported with reg:quantileerror: its leaf values are residual quantiles, which the "
+           "refresh updater does not recompute");
+  } else if (p->updater == "refresh") {
+    fail("updater=refresh needs process_type=update: it refreshes the trees of an existing model (xgb_model)");
+  } else if (!p->updater.empty() && p->updater != "grow_quantile_histmaker" && p->updater != "grow_gpu_hist") {
+    fail("updater='%s' is not supported (supported: grow_quantile_histmaker, grow_gpu_hist, and refresh with "
+         "process_type=update)", p->updater.c_str());
+  }
+  if (p->num_target_set) set_targets(p, p->num_target);
+  // 16: a leaf index must fit the uint16_t row -> leaf map pos (2^16 leaves), DESIGN.md 9
+  if (p->max_depth < 1 || p->max_depth > 16) fail("max_depth must be in [1, 16], got %d", p->max_depth);
+  if (p->num_parallel_tree < 1 || p->num_parallel_tree > 4096) fail("num_parallel_tree must be in [1, 4096], got %d", p->num_parallel_tree);
+  if (p->qbits < 8 || p->qbits > 24) fail("hist_qbits must be in [8, 24], got %d", p->qbits);
+  for (float v : {p->subsample, p->colsample_bytree, p->colsample_bylevel, p->colsample_bynode})
+    if (!(v > 0.0f && v <= 1.0f)) fail("subsample / colsample_* must be in (0, 1], got %g", (double)v);
+  if (p->max_cat_to_onehot < 1) fail("max_cat_to_onehot must be >= 1, got %d", p->max_cat_to_onehot);
+  if (p->max_cat_threshold < 1) fail("max_cat_threshold must be >= 1, got %d", p->max_cat_threshold);
+  if (p->objective == kObjPoisson) {
+    if (!p->max_delta_step_set) p->max_delta_step = 0.7f;   // both the hessian's shift and the leaf-step clamp
+    if (!(p->max_delta_step >= 0.0f)) fail("max_delta_step must be >= 0 for count:poisson, got %g", (double)p->max_delta_step);
+  }
+  if (p->objective == kObjPseudoHuber && !(p->huber_slope > 0.0f))
+    fail("huber_slope must be > 0 for reg:pseudohubererror, got %g", (double)p->huber_slope);
+  if (p->objective == kObjTweedie && !(p->tweedie_variance_power >= 1.0f && p->tweedie_variance_power < 2.0f))
+    fail("tweedie_variance_power must be in [1, 2), got %g", (double)p->tweedie_variance_power);
+  if (!(p->aft_sigma > 0.0f) || std::isinf(p->aft_sigma))
+    fail("aft_loss_distribution_scale must be finite and > 0, got %g", (double)p->aft_sigma);
+  // survival:aft fits no intercept: base_score defaults to 0.5 (margin log 0.5) and is never estimated
+  if (p->objective == kObjAft && !p->base_score_set) { p->base_score = 0.5f; p->base_score_set = true; }
+  // the rank objectives neither: their margin is the score itself (identity transform)
+  if (obj_rank(p->objective) && !p->base_score_set) { p->base_score = 0.5f; p->base_score_set = true; }
+  if (p->base_score_set) {
+    if (p->objective == kObjRegLogistic && !(p->base_score > 0.0f && p->base_score < 1.0f))
+      fail("base_score must be in (0, 1) for reg:logistic, got %g", (double)p->base_score);
+    if (obj_log_link(p->objective) && !(p->base_score > 0.0f))
+      fail("base_score must be > 0 for %s, got %g", p->objective_name.c_str(), (double)p->base_score);
+  }
+}
+
+// the parameter that the gradient kernel of an objective takes (gradient_param_kernel)
+float objective_param(const Params& p) {
+  if (p.objective == kObjPseudoHuber) return p.huber_slope;
+  if (p.objective == kObjPoisson) return p.max_delta_step;
+  if (p.objective == kObjTweedie) return p.tweedie_variance_power;
+  return 0.0f;
+}
+
+// margin of base_score (the inverse of the prediction transform), evaluated on the host with libm's logf
+float base_margin_value(const Params& p) {
+  if (obj_sigmoid(p.objective)) return -logf(1.0f / p.base_score - 1.0f);
+  if (obj_log_link(p.objective)) return logf(p.base_score);
+  return p.base_score;
+}
+
+// -- host replicas of the gain / weight formulas (A.6, A.7); same IEEE sequence as the kernels
+double h_thr_l1(double g, double a) { if (g > a) return g - a; if (g < -a) return g + a; return 0.0; }
+float h_calc_weight(const Params& p, double G, double H) {
+  if (H < (double)p.min_child_weight || H <= 0.0) return 0.0f;
+  double t = p.alpha == 0.0f ? G : h_thr_l1(G, (double)p.alpha);
+  double dw = -t / (H + (double)p.lambda);
+  if (p.max_delta_step != 0.0f && fabs(dw) > (double)p.max_delta_step) dw = copysign((double)p.max_delta_step, dw);
+  return (float)dw;
+}
+
+// metric id of an eval_metric name; *param receives the metric's parameter (rho of tweedie-nloglik@rho, huber_slope for mphe)
+B2Metric metric_id(const char* name, const Params& p, float* param, int* minus) {
+  std::string s(name ? name : "");
+  *param = 0.0f; *minus = 0;
+  if (s == "rmsle") return kMetricRmsle;
+  if (s == "mape") return kMetricMape;
+  if (s == "mphe") { *param = p.huber_slope; return kMetricMphe; }
+  if (s == "poisson-nloglik") return kMetricPoissonNloglik;
+  if (s == "gamma-nloglik") return kMetricGammaNloglik;
+  if (s == "gamma-deviance") return kMetricGammaDeviance;
+  if (s.rfind("tweedie-nloglik", 0) == 0) {
+    *param = 1.5f;   // xgboost's default when the name carries no @rho
+    if (s.size() > 15) {
+      char* end = nullptr;
+      const std::string r = s.substr(16);
+      const double v = s[15] == '@' ? strtod(r.c_str(), &end) : NAN;
+      if (s[15] != '@' || r.empty() || *end != '\0' || !(v >= 1.0 && v < 2.0))
+        fail("eval metric '%s': the Tweedie power must be given as tweedie-nloglik@rho with rho in [1, 2)", s.c_str());
+      *param = (float)v;
+    }
+    return kMetricTweedieNloglik;
+  }
+  if (s == "rmse") return kMetricRmse;
+  if (s == "logloss") return kMetricLogloss;
+  if (s == "error") return kMetricError;
+  if (s == "mlogloss") return kMetricMlogloss;
+  if (s == "merror") return kMetricMerror;
+  if (s == "mae") return kMetricMae;
+  if (s == "auc") return kMetricAuc;
+  if (s == "aucpr") return kMetricAucPr;
+  if (s == "aft-nloglik") return kMetricAftNloglik;
+  if (s == "quantile") return kMetricQuantile;
+  if (s == "interval-regression-accuracy") return kMetricIntervalAccuracy;
+  // ranking metrics: ndcg[@k][-], map[@k][-], pre[@k][-].  *param = k (0: the whole group), *minus = the trailing '-'
+  // (a group without relevant rows scores 0 instead of 1)
+  for (const B2Metric id : {kMetricNdcg, kMetricMap, kMetricPre}) {
+    const std::string base = id == kMetricNdcg ? "ndcg" : id == kMetricMap ? "map" : "pre";
+    if (s.compare(0, base.size(), base) != 0) continue;
+    std::string rest = s.substr(base.size());
+    if (!rest.empty() && rest.back() == '-') { *minus = 1; rest.pop_back(); }
+    if (rest.empty()) return id;
+    char* end = nullptr;
+    const long long k = rest[0] == '@' && rest.size() > 1 ? strtoll(rest.c_str() + 1, &end, 10) : -1;
+    if (rest[0] != '@' || rest.size() < 2 || *end != '\0' || k < 1 || k > (1 << 24))
+      fail("eval metric '%s': the cut-off must be given as %s@k with an integer k >= 1", s.c_str(), base.c_str());
+    *param = (float)k;
+    return id;
+  }
+  fail("unsupported eval metric '%s' (supported: rmse, mae, logloss, error, auc, aucpr, mlogloss, merror, rmsle, mape, mphe, "
+       "poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy, "
+       "quantile, ndcg[@k][-], map[@k][-], pre[@k][-])", s.c_str());
+}
+
+}  // namespace b2host

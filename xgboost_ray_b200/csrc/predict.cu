@@ -1,0 +1,154 @@
+// predict.cu -- prediction on the device model: the TreeSHAP path table, margins of a range of trees, the cached
+// evaluation margins of a matrix, and metric sums over the workers.
+#include <math.h>
+
+#include "host.h"
+#include "launch.h"
+
+namespace b2host __attribute__((visibility("hidden"))) {
+
+// ---- TreeSHAP path table (common.cuh B2PathElem / B2PathInfo; shap_kernel.cu).  Walks every tree root -> leaf; on the
+// way each split is merged into the element of its feature (appended the first time the feature is seen): the interval
+// of a numeric feature narrows, the category set of a categorical feature is intersected with the side taken (keeping
+// predict_kernel's rule that a category outside [0, 256) goes left), the missing flag is AND-ed with "the default
+// direction is the side taken", and zero_fraction is multiplied by cover(child) / cover(parent) (0 for a zero-cover
+// parent, never NaN).  The tree's expected value, sum over leaves of value * prod zero_fraction, is its SHAP bias.
+struct PathBuildElem {
+  int32_t feature; bool is_cat; float lo, hi; uint32_t flags; uint32_t bits[8]; double z;
+};
+void walk_paths(const TreeHost& t, int nid, std::vector<PathBuildElem>& path, int tree, int cls, Booster* b,
+                std::vector<B2PathElem>& elems, std::vector<B2PathInfo>& infos, std::vector<uint32_t>& cats, double* expected) {
+  if (t.feature[nid] < 0) {
+    if (path.size() + 1 > B2_SHAP_MAX_PATH)
+      fail("tree %d has a leaf below %d distinct features; TreeSHAP supports at most %d distinct features on a path", tree,
+           (int)path.size(), B2_SHAP_MAX_PATH - 1);
+    B2PathInfo pi{(int32_t)elems.size(), (int32_t)path.size() + 1, cls, 0, (double)t.value[nid]};
+    elems.push_back(B2PathElem{-1, -1, 0.f, 0.f, 0u, 0u, 1.0});
+    double zprod = 1.0;
+    for (const PathBuildElem& e : path) {
+      int32_t slot = -1;
+      if (e.is_cat) { slot = (int32_t)(cats.size() / 8); cats.insert(cats.end(), e.bits, e.bits + 8); }
+      elems.push_back(B2PathElem{e.feature, slot, e.lo, e.hi, e.flags, 0u, e.z});
+      zprod *= e.z;
+    }
+    *expected += (double)t.value[nid] * zprod;
+    infos.push_back(pi);
+    return;
+  }
+  const int f = t.feature[nid];
+  const bool is_cat = t.split_type[nid] != 0;
+  const double cover = t.sum_hess[nid];
+  for (int side = 0; side < 2; ++side) {
+    const int child = side == 0 ? t.left[nid] : t.right[nid];
+    const bool left = side == 0;
+    std::vector<PathBuildElem> next = path;
+    PathBuildElem* e = nullptr;
+    for (auto& x : next) if (x.feature == f) e = &x;
+    if (!e) {
+      PathBuildElem ne;
+      ne.feature = f; ne.is_cat = is_cat; ne.lo = -INFINITY; ne.hi = INFINITY;
+      ne.flags = B2_PATH_MISSING_OK | B2_PATH_OUTSIDE_OK; ne.z = 1.0;
+      for (int w = 0; w < 8; ++w) ne.bits[w] = 0xffffffffu;
+      next.push_back(ne); e = &next.back();
+    }
+    e->z *= cover > 0.0 ? t.sum_hess[child] / cover : 0.0;
+    if ((t.default_left[nid] != 0) != left) e->flags &= ~B2_PATH_MISSING_OK;
+    if (is_cat) {
+      e->is_cat = true;
+      for (int w = 0; w < 8; ++w) e->bits[w] &= left ? ~t.cat_bits[(size_t)nid * 8 + w] : t.cat_bits[(size_t)nid * 8 + w];
+      if (!left) e->flags &= ~B2_PATH_OUTSIDE_OK;
+    } else if (left) {
+      if (!(e->flags & B2_PATH_HAS_HI) || t.cond[nid] < e->hi) e->hi = t.cond[nid];
+      e->flags |= B2_PATH_HAS_HI;
+    } else if (t.cond[nid] > e->lo) {
+      e->lo = t.cond[nid];
+    }
+    walk_paths(t, child, next, tree, cls, b, elems, infos, cats, expected);
+  }
+}
+
+void build_paths(Booster* b) {
+  if (b->paths_synced == (int)b->trees.size() && b->paths_weights_version == (int)b->weights_version) return;
+  std::vector<B2PathElem> elems; std::vector<B2PathInfo> infos; std::vector<uint32_t> cats;
+  b->tree_path_offset.assign(1, 0); b->tree_expected.clear();
+  const int K = b->p.num_class, npt = std::max(1, b->p.num_parallel_tree);
+  for (int t = 0; t < (int)b->trees.size(); ++t) {
+    std::vector<PathBuildElem> path;
+    double expected = 0.0;
+    const int32_t first = (int32_t)infos.size();
+    walk_paths(b->trees[t], 0, path, t, (t / npt) % K, b, elems, infos, cats, &expected);
+    if (b->p.dart) {   // DART: the tree's leaves count with its weight
+      const double w = (double)b->tree_w[t];
+      for (size_t i = first; i < infos.size(); ++i) infos[i].value *= w;
+      expected *= w;
+    }
+    b->tree_path_offset.push_back((int32_t)infos.size());
+    b->tree_expected.push_back(expected);
+  }
+  cudaStream_t s = b->ctx->stream;
+  upload(b->d_path_elems, elems, s); upload(b->d_paths, infos, s); upload(b->d_path_cats, cats, s);
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  b->paths_synced = (int)b->trees.size();
+  b->paths_weights_version = (int)b->weights_version;
+}
+
+// DART: the tree weights on the device (nullptr for gbtree: the kernels then add the plain leaf values)
+const float* device_weights(Booster* b) {
+  if (!b->p.dart) return nullptr;
+  if (b->d_tree_w_version != b->weights_version || b->d_tree_w_count != b->tree_w.size()) {
+    upload(b->d_tree_w, b->tree_w, b->ctx->stream);   // pageable source: staged before return
+    b->d_tree_w_version = b->weights_version; b->d_tree_w_count = b->tree_w.size();
+  }
+  return b->d_tree_w.p;
+}
+
+// out += the trees [tree_begin, tree_end) on the raw rows of m (the device trees are in sync)
+void predict_trees(Booster* b, Matrix* m, int tree_begin, int tree_end, float* out) {
+  if (b->p.vector_leaf())
+    LAUNCH_CHECK(b2_launch_predict_vector(m->raw.p, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_leaf_table.p,
+                                          tree_begin, tree_end, b->p.num_target, out, b->ctx->num_sms, b->ctx->stream));
+  else
+    LAUNCH_CHECK(b2_launch_predict(m->raw.p, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, tree_begin,
+                                   tree_end, b->p.num_class, b->p.num_parallel_tree, device_weights(b), out, b->ctx->num_sms,
+                                   b->ctx->stream));
+}
+
+// margin of matrix m under the current model (cached per matrix, only new trees are applied)
+float* eval_margin(Booster* b, Matrix* m) {
+  if (b->train && m == b->train) { ensure_train_margin(b); return b->margin.p; }
+  if (!m->has_raw) fail("evaluation / prediction matrix has no raw data on the device");
+  if (m->F != b->n_features) fail("feature count mismatch: matrix has %d, model has %d", m->F, b->n_features);
+  {   // drop the cached margins of matrices that were freed since the last call
+    std::lock_guard<std::mutex> lk(g_matrix_mu);
+    for (auto it = b->eval_cache.begin(); it != b->eval_cache.end();) {
+      if (!g_live_matrices.count(it->first)) { delete it->second; it = b->eval_cache.erase(it); } else ++it;
+    }
+  }
+  if (!m->uid) fail("evaluation matrix is not a registered matrix handle");
+  EvalCache*& c = b->eval_cache[m->uid];
+  const int K = b->p.num_class;
+  if (!c || c->n != m->n || c->margin_version != m->margin_version || c->weights_version != b->weights_version) {
+    delete c; c = new EvalCache(); c->n = m->n; c->margin_version = m->margin_version; c->weights_version = b->weights_version;
+    c->margin.ensure((size_t)std::max<int64_t>(m->n * K, 1));
+    init_margin(b, c->margin.p, m);
+    c->n_trees_applied = 0;
+  }
+  const int nt = (int)b->trees.size();
+  if (c->n_trees_applied < nt) {
+    sync_device_trees(b);
+    predict_trees(b, m, c->n_trees_applied, nt, c->margin.p);
+    c->n_trees_applied = nt;
+  }
+  return c->margin.p;
+}
+
+// the first n doubles of b->d_metric summed over the workers, on the host (synchronises the stream)
+std::vector<double> metric_sums(Booster* b, size_t n, cudaStream_t s) {
+  allreduce(b->comm, b->d_metric.p, n, kNcclFloat64, kNcclSum, s);
+  std::vector<double> h(n);
+  CUDA_CHECK(cudaMemcpyAsync(h.data(), b->d_metric.p, n * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  return h;
+}
+
+}  // namespace b2host
