@@ -4,6 +4,8 @@ otherwise, categories in the stored set go RIGHT, missing follows default_left."
 import numpy as np
 import pytest
 
+from tests import categorical_reference as CR
+
 P1 = {"objective": "reg:squarederror", "max_depth": 1, "eta": 1.0, "base_score": 0.0, "lambda": 0.0}
 
 
@@ -112,3 +114,50 @@ def test_mixed_numeric_and_categorical_multiclass(oracle):
     for t in b.trees():
         used |= {(int(f), int(st)) for f, st in zip(t.split_feature, t.split_type) if f >= 0}
     assert (3, 1) in used and (4, 1) in used and (0, 0) in used      # one-hot, partition and numeric splits all occur
+
+
+# ------------------------------------------------------------------ the oracle against tests/categorical_reference.py
+ROOT = {"objective": "reg:squarederror", "max_depth": 1, "eta": 1.0, "base_score": 0.0}
+F32 = np.float32
+CARDS = [1, 2, 3, 4, 5, 31, 32, 33, 64, 65, 128, 224, 225, 255, 256]
+
+
+def _root_against_reference(oracle, params, X, y, w=None):
+    params = dict(ROOT, **params)
+    b, _ = oracle.train(params, X, y, 1, weight=w, is_cat=[1] * X.shape[1])
+    g = (F32(0.0) - y).astype(F32) * (F32(1.0) if w is None else w)
+    h = np.ones_like(g) if w is None else w.astype(F32)
+    split, hist = CR.root_split(X, g.astype(F32), h, int(params.get("hist_qbits", 18)), params)
+    CR.root_matches(vars(b.tree(0)), split, hist)
+    return split, hist
+
+
+@pytest.mark.parametrize("seed,params,nan_frac,weighted", [
+    (0, {}, 0.0, False),
+    (1, {"max_cat_to_onehot": 257}, 0.1, False),               # every feature one-hot, candidate keys up to 2 * 255 + 1
+    (2, {"max_cat_threshold": 1}, 0.1, True),                  # no partition candidate: only the one-hot features split
+    (3, {"max_cat_threshold": 2, "hist_qbits": 8}, 0.1, False),
+    (4, {"max_cat_threshold": 300, "hist_qbits": 24, "lambda": 0.0}, 0.0, True),
+    (5, {"max_cat_to_onehot": 33, "alpha": 2.0, "min_child_weight": 40.0}, 0.1, False),
+    (6, {"max_cat_to_onehot": 1, "max_delta_step": 0.4, "lambda": 3.0}, 0.1, True),
+])
+def test_reference_root_scan_matches_oracle_random(oracle, seed, params, nan_frac, weighted):
+    X, y, w = CR.random_case(seed, CARDS, 6000, nan_frac, weighted)
+    split, _ = _root_against_reference(oracle, params, X, y, w)
+    if params.get("max_cat_threshold") == 1:
+        assert split["kind"] == "onehot"
+
+
+@pytest.mark.parametrize("values,thr,kind", [
+    ((0.5, 1.0, 2.0, 4.0), 2, "backward"), ((0.5, 1.0, 2.0, 4.0), 6, "backward"),
+    ((3.0, 3.5, 4.0), 4, "forward"), ((3.0, 3.5, 4.0), 6, "forward"),
+])
+def test_reference_root_scan_matches_oracle_ties(oracle, values, thr, kind):
+    X, y = CR.tie_case(0, values=values)
+    params = {"lambda": 0.5, "min_child_weight": 3.0, "max_cat_threshold": thr}
+    split, hist = _root_against_reference(oracle, params, X, y)
+    assert split["feature"] == 0 and split["kind"] == kind
+    # the chosen set cuts through categories of equal weight (-0.0, +0.0 of empty and light categories included):
+    # only the stable order decides which of them go right
+    cat_g, cat_h, nf, _, _, sg, sh = hist
+    assert CR.tied_across(split, cat_g, cat_h, nf, sg, sh, params)
