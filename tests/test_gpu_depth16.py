@@ -135,16 +135,28 @@ def test_dart_depth16(eng, oracle):
     assert_deep_shape(bst, 16)
 
 
-def test_quantile_depth16(eng, oracle):
+def quantile_depth16(eng, oracle, weighted):
     X, y = deep_data(400_000, 16, 37, cat=False)
     params = {"objective": "reg:quantileerror", "quantile_alpha": [0.3, 0.7], "max_depth": 16, "min_child_weight": 0}
-    bst = eng.train(params, eng.DMatrix(X, label=y), num_boost_round=2, verbose_eval=False)
-    ref = QR.train(oracle, params, X, y, 2)
+    w = np.random.RandomState(38).randint(0, 4, size=len(y)).astype(F32) if weighted else None
+    bst = eng.train(params, eng.DMatrix(X, label=y, weight=w), num_boost_round=2, verbose_eval=False)
+    ref = QR.train(oracle, params, X, y, 2, weight=w)
     assert_same_model(bst, ref)
     for i, t in enumerate(bst.get_trees()):
         leaf = t["split_feature"] < 0
         assert t["value"][leaf].tobytes() == ref.tree(i).value[leaf].tobytes(), "tree %d leaf values" % i
     assert_deep_shape(bst, 16, min_leaves=1 << 14)     # pinball gradients stop more nodes early
+
+
+def test_quantile_depth16(eng, oracle):
+    quantile_depth16(eng, oracle, False)
+
+
+@pytest.mark.timeout(900)
+def test_quantile_depth16_weighted(eng, oracle):
+    """integer weights 0-3: rows of hessian 0 are skipped, the others count by fixed-point mass in the global-memory
+    histograms of the weighted count pass"""
+    quantile_depth16(eng, oracle, True)
 
 
 def test_refresh_depth16_is_identity(eng):

@@ -61,10 +61,15 @@ def test_matches_reference(eng, oracle, alpha, depth):
     assert bst.num_boosted_rounds() == 8 and bst.num_trees() == 8 * T
 
 
-@pytest.mark.parametrize("variant", ["int_weights", "frac_weights", "nan_categorical", "sampling"])
-def test_variants_match_reference(eng, oracle, variant):
+VARIANTS = ["int_weights", "frac_weights", "nan_categorical", "sampling"]
+
+
+# depth 6 and 7 sit on either side of the weighted count pass's shared-memory limit (quantile_kernel.cu)
+@pytest.mark.parametrize("variant,depth", [(v, 6) for v in VARIANTS] + [(v, 7) for v in VARIANTS],
+                         ids=VARIANTS + [v + "-depth7" for v in VARIANTS])
+def test_variants_match_reference(eng, oracle, variant, depth):
     rng = np.random.RandomState(3)
-    params = {"objective": "reg:quantileerror", "quantile_alpha": [0.2, 0.8], "max_depth": 6, "eta": 0.4}
+    params = {"objective": "reg:quantileerror", "quantile_alpha": [0.2, 0.8], "max_depth": depth, "eta": 0.4}
     is_cat, kw, w = None, {}, None
     if variant == "nan_categorical":
         X, y, rng = make_cat_data(8000, 5, nan_frac=0.05)
@@ -181,10 +186,11 @@ def test_two_gpus_and_two_actors_same_model(eng):
     from xgboost_ray_b200 import RayDMatrix, RayParams, train
     X, y = dataset(n=30001, seed=15, nan_frac=0.05)
     w = np.random.RandomState(3).uniform(0.5, 2, size=len(y)).astype(F32)
-    params = {"objective": "reg:quantileerror", "quantile_alpha": [0.1, 0.5, 0.9], "max_depth": 6}
-    b1 = train(params, RayDMatrix(X, y, weight=w), num_boost_round=5, ray_params=RayParams(num_actors=1))
-    b2 = train(params, RayDMatrix(X, y, weight=w), num_boost_round=5, ray_params=RayParams(num_actors=2))
-    assert bytes(b1.save_raw()) == bytes(b2.save_raw())
+    for depth in (6, 8):          # weighted counts in shared memory, then in global memory
+        params = {"objective": "reg:quantileerror", "quantile_alpha": [0.1, 0.5, 0.9], "max_depth": depth}
+        b1 = train(params, RayDMatrix(X, y, weight=w), num_boost_round=5, ray_params=RayParams(num_actors=1))
+        b2 = train(params, RayDMatrix(X, y, weight=w), num_boost_round=5, ray_params=RayParams(num_actors=2))
+        assert bytes(b1.save_raw()) == bytes(b2.save_raw()), "max_depth %d" % depth
 
 
 @pytest.mark.parametrize("extra,match", [({"num_class": 2}, "num_class"), ({"booster": "dart"}, "dart"),

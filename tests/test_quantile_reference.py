@@ -50,6 +50,95 @@ def test_weighted_rule_by_hand():
     assert R.leaf_quantile(r, 0.7, np.zeros(4, np.int64)) == F32(1.0)
 
 
+def bits(v):
+    return np.array([v], F32).tobytes()
+
+
+def test_radix_select_by_hand():
+    r = np.array([3.0, 1.0, 2.0], F32)
+    # n = 3: alpha = 1/(n+1) = 0.25 is the minimum and 3/(n+1) = 0.75 the maximum by equality, with one target
+    assert R.radix_select(r, 0.25) == (F32(1.0), None)
+    assert R.radix_select(r, 0.75) == (F32(3.0), None)
+    # frac = 0: alpha (n + 1) = 2 is an integer, so q is v_1 itself; the targets are 2.0 and 3.0, keys 0xc0000000 and
+    # 0xc0400000, which part in the second byte
+    assert R.radix_select(r, 0.5) == (F32(2.0), 1)
+    assert R.leaf_quantile(r, 0.5) == F32(2.0)
+    # -0 and +0 are one key: the targets never split, and the answer is +0
+    q, split = R.radix_select(np.array([-0.0, 0.0, -0.0, 0.0], F32), 0.5)
+    assert bits(q) == bits(0.0) and split is None
+    # weighted: masses 2^31 each (max weight 1) sum to 2^33; alpha = 0.5 puts the target exactly at the end of 2.0's
+    # cumulative weight, so 2.0 is picked and not 3.0
+    r4 = np.array([4.0, 1.0, 3.0, 2.0], F32)
+    m = R.fixed_mass(np.ones(4, F32), R.frexp_exponent(1.0))
+    assert m.tolist() == [2 ** 31] * 4
+    assert R.radix_select(r4, 0.5, m) == (F32(2.0), None) and R.leaf_quantile(r4, 0.5, m) == F32(2.0)
+    assert R.radix_select(r4, np.nextafter(F32(0.5), F32(1)), m)[0] == F32(3.0)
+    # half-way masses with max weight 1 (e = 1, scale 2^31): 2^-32 -> 0.5 -> 0 and 3 * 2^-32 -> 1.5 -> 2, ties to even
+    w = np.array([1.0, 2.0 ** -32, 3 * 2.0 ** -32, 5 * 2.0 ** -32], F32)
+    assert R.fixed_mass(w, R.frexp_exponent(w.max())).tolist() == [2 ** 31, 0, 2, 2]
+    # a row of mass 0 is never the answer of the weighted rule, even as the smallest value: W = 2^31 + 4, so alpha =
+    # 1e-10 gives the target 1, first reached by 2.0 (mass 2)
+    m = R.fixed_mass(w, 1)
+    r = np.array([5.0, -1.0, 2.0, 3.0], F32)
+    assert R.radix_select(r, 1e-10, m) == (F32(2.0), None) and R.leaf_quantile(r, 1e-10, m) == F32(2.0)
+    # every mass 0 (weights 2^-32 where the tree's largest is 1): ceil(alpha W) = 0, the minimum by count
+    m0 = R.fixed_mass(np.full(3, 2.0 ** -32, F32), 1)
+    assert m0.tolist() == [0, 0, 0]
+    assert R.radix_select(r[1:], 0.9, m0) == (F32(-1.0), None) and R.leaf_quantile(r[1:], 0.9, m0) == F32(-1.0)
+
+
+def weighted_inputs(y, w):
+    keep = w != 0
+    return y[keep], R.fixed_mass(w[keep], R.frexp_exponent(w.max()))
+
+
+@pytest.mark.parametrize("n", [1, 2, 3, 4, 255, 256, 257, 20000])
+def test_radix_select_is_the_sort_on_boundary_sets(n):
+    """The kernel's four-pass selection, replayed, gives leaf_quantile's value bit for bit on every boundary set, and
+    each pair set splits its targets in the pass its keys say"""
+    rng = np.random.RandomState(n)
+    splits = set()
+    checked = 0
+    for name, y, alphas in R.boundary_sets(n):
+        for a in alphas:
+            q, split = R.radix_select(y, a)
+            assert bits(q) == bits(R.leaf_quantile(y, a)), (name, float(a))
+            splits.add(split)
+            if name.startswith("pair") and n > 2:
+                assert split == int(name[-2]), (name, split)
+            for kind in ("int", "half", "pow2"):
+                w = R.boundary_weights(kind, n, rng)
+                yw, m = weighted_inputs(y, w)
+                aw = [a]
+                if kind == "pow2":          # no zero weights: yw is y
+                    aw.append(R.boundary_alpha(y, w, rng) or a)
+                for b in aw:
+                    qw, sw = R.radix_select(yw, b, m)
+                    assert bits(qw) == bits(R.leaf_quantile(yw, b, m)) and sw is None, (name, kind, float(b))
+            checked += 1
+    assert checked >= len(R.SPLIT_PAIRS)
+    if n > 1:
+        assert splits >= {0, 1, 2, 3, None}, splits
+
+
+def test_weighted_target_on_a_cumulative_boundary():
+    rng = np.random.RandomState(5)
+    for n in (2, 3, 5, 100, 257):
+        y = rng.choice(R.POOL, n)
+        w = R.boundary_weights("pow2", n, rng)
+        a = R.boundary_alpha(y, w, rng)
+        if a is None:
+            continue
+        m = R.fixed_mass(w, R.frexp_exponent(w.max()))
+        yn = np.where(y == 0, F32(0.0), y).astype(F32)
+        order = np.argsort(yn, kind="stable")
+        cum = np.cumsum(m[order])
+        target = int(np.ceil(float(a) * float(cum[-1])))
+        i = int(np.nonzero(cum == target)[0][0])          # the target is exactly a cumulative sum
+        assert yn[order][i] < yn[order][i + 1]
+        assert R.leaf_quantile(y, a, m) == yn[order][i] == R.radix_select(y, a, m)[0]
+
+
 @pytest.mark.parametrize("seed", range(6))
 def test_rules_agree_with_numpy(seed):
     rng = np.random.RandomState(seed)
