@@ -53,6 +53,15 @@ int B2_MatrixCreateFromDense(const float* data, int64_t n_rows, int32_t n_cols, 
  * per Ray object / file, xgboost_ray/matrix.py:127-196, main.py:387-418): allocate the device matrix once, then
  * upload each block at its row offset -- no host-side concatenation (matrix.py:65-67). */
 int B2_MatrixCreate(int64_t n_rows, int32_t n_cols, float missing, int device, B2Handle* out);
+/* A scipy.sparse matrix (xgb.DMatrix(csr), reached through xgboost_ray/main.py:437): row i stores entries
+ * [indptr[i], indptr[i+1]) of indices / values; an entry a row does not store is missing, a stored one follows the
+ * dense rules (NaN or `missing` is missing).  indptr is only read.  The arrays are checked on the device: indptr[0] = 0,
+ * indptr non-decreasing, indptr[n_rows] = nnz, every column in [0, n_cols) and strictly increasing within its row; the
+ * first row that breaks a rule fails the call and is named.  The device keeps the CSR (8 (n_rows + 1) + 8 nnz bytes),
+ * never an n_rows x n_cols float copy: the kernels that read raw rows get them densified tile by tile.  Bins, cuts,
+ * models and predictions equal those of the dense matrix with NaN in every absent cell. */
+int B2_MatrixCreateFromCSR(int64_t* indptr, const int32_t* indices, const float* values, int64_t n_rows, int32_t n_cols,
+                           int64_t nnz, float missing, int device, B2Handle* out);
 int B2_MatrixSetRows(B2Handle m, int64_t row_begin, const float* data, int64_t n_rows);
 /* The shard lives in ANOTHER process (the driver that holds the user's matrix): rows of n_cols floats, remote_row_stride
  * bytes apart starting at remote_addr in process `pid`, are read with process_vm_readv straight into the pinned upload
@@ -106,6 +115,10 @@ int B2_MatrixQuantizeWithCuts(B2Handle m, B2Handle comm, const int32_t* ptrs /*[
                               int32_t keep_raw);
 /* re-upload the float data of a matrix whose device copy was freed (same shape) */
 int B2_MatrixEnsureRaw(B2Handle m, const float* data);
+/* the same for a matrix created with B2_MatrixCreateFromCSR: re-upload (and check) its CSR arrays (xgboost_ray/main.py:437) */
+int B2_MatrixEnsureRawCSR(B2Handle m, int64_t* indptr, const int32_t* indices, const float* values);
+/* device bytes the matrix owns: the capacities of its raw (dense or CSR), bin and info buffers (xgboost_ray/main.py:437) */
+int B2_MatrixDeviceBytes(B2Handle m, int64_t* out);
 int B2_MatrixCutsSize(B2Handle m, int32_t* total_cuts);
 int B2_MatrixGetCuts(B2Handle m, int32_t* ptrs /*[F+1]*/, float* vals /*[total]*/, float* mins /*[F]*/,
                      uint8_t* has_missing /*[F]*/);

@@ -32,6 +32,7 @@ SOURCES = {
     "dart_kernel.cu": ["--fmad=false"],        # DART margin rebuild, bit-exact vs the weighted predict and the reference
     "quantile_kernel.cu": ["--fmad=false"],    # quantile gradients, metric and leaf refresh, bit-exact vs the reference
     "refresh_kernel.cu": ["--fmad=false"],     # refresh updater: leaf sums on raw rows, node statistics bottom-up
+    "sparse_kernel.cu": [],                    # CSR raw values: validation, dense row tiles, sketch keys
     # host side (host.h): no device code
     "device.cu": [],
     "matrix.cu": [],

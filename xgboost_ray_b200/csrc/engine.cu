@@ -138,6 +138,19 @@ int B2_MatrixCreateFromDense(const float* data, int64_t n_rows, int32_t n_cols, 
   *out = (B2Handle)m;
   API_END
 }
+int B2_MatrixCreateFromCSR(int64_t* indptr, const int32_t* indices, const float* values, int64_t n_rows, int32_t n_cols,
+                           int64_t nnz, float missing, int device, B2Handle* out) {
+  API_BEGIN
+  if (n_rows < 0 || n_cols <= 0 || nnz < 0) fail("invalid CSR matrix %lld x %d with %lld entries", (long long)n_rows, n_cols, (long long)nnz);
+  if (n_rows >= (1LL << 31)) fail("at most 2^31-1 rows per GPU shard (row ids are int32), got %lld", (long long)n_rows);
+  Ctx* ctx = get_ctx(device);
+  Matrix* m = new Matrix(); m->kind = kMatrix; m->ctx = ctx; m->n = n_rows; m->F = n_cols; m->missing = missing;
+  m->csr = true; m->nnz = nnz;
+  try { upload_csr(m, indptr, indices, values); } catch (...) { delete m; throw; }
+  { std::lock_guard<std::mutex> lk(g_matrix_mu); m->uid = g_next_matrix_uid++; g_live_matrices.insert(m->uid); }
+  *out = (B2Handle)m;
+  API_END
+}
 int B2_MatrixCreate(int64_t n_rows, int32_t n_cols, float missing, int device, B2Handle* out) {
   API_BEGIN
   if (n_rows < 0 || n_cols <= 0) fail("invalid matrix shape %lld x %d", (long long)n_rows, n_cols);
@@ -290,6 +303,7 @@ int B2_MatrixSetRows(B2Handle mh, int64_t row_begin, const float* data, int64_t 
   Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
   CUDA_CHECK(cudaSetDevice(m->ctx->device));
   if (m->quantized || !m->has_raw) fail("rows can only be set before the matrix is quantised");
+  if (m->csr) fail("rows of a matrix created from CSR arrays cannot be set");
   if (row_begin < 0 || n_rows < 0 || row_begin + n_rows > m->n) fail("row block [%lld, %lld) outside the matrix (%lld rows)",
                                                                      (long long)row_begin, (long long)(row_begin + n_rows), (long long)m->n);
   upload_pipelined(m->ctx, m->raw.p + (size_t)row_begin * m->F, data, (size_t)n_rows * m->F * sizeof(float));
@@ -412,7 +426,7 @@ int B2_MatrixQuantize(B2Handle mh, B2Handle commh, int32_t max_bin, B2Handle ref
     make_cuts(m, comm, max_bin);
   }
   bin_matrix(m);
-  if (!keep_raw) { m->raw.release(); m->has_raw = false; }
+  if (!keep_raw) release_raw(m);
   API_END
 }
 int B2_MatrixQuantizeWithCuts(B2Handle mh, B2Handle commh, const int32_t* ptrs, const float* vals, const float* mins,
@@ -435,7 +449,7 @@ int B2_MatrixQuantizeWithCuts(B2Handle mh, B2Handle commh, const int32_t* ptrs, 
   m->max_bin = max_bin;
   check_borrowed_categories(m, comm);
   bin_matrix(m);
-  if (!keep_raw) { m->raw.release(); m->has_raw = false; }
+  if (!keep_raw) release_raw(m);
   API_END
 }
 int B2_MatrixEnsureRaw(B2Handle mh, const float* data) {
@@ -443,9 +457,24 @@ int B2_MatrixEnsureRaw(B2Handle mh, const float* data) {
   Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
   CUDA_CHECK(cudaSetDevice(m->ctx->device));
   if (m->has_raw) return 0;
+  if (m->csr) fail("the matrix was created from CSR arrays: re-upload them with B2_MatrixEnsureRawCSR");
   m->raw.ensure((size_t)std::max<int64_t>(m->n * m->F, 1));
   upload_pipelined(m->ctx, m->raw.p, data, (size_t)m->n * m->F * sizeof(float));
   m->has_raw = true;
+  API_END
+}
+int B2_MatrixEnsureRawCSR(B2Handle mh, int64_t* indptr, const int32_t* indices, const float* values) {
+  API_BEGIN
+  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
+  CUDA_CHECK(cudaSetDevice(m->ctx->device));
+  if (m->has_raw) return 0;
+  if (!m->csr) fail("the matrix was created from dense rows: re-upload them with B2_MatrixEnsureRaw");
+  upload_csr(m, indptr, indices, values);
+  API_END
+}
+int B2_MatrixDeviceBytes(B2Handle mh, int64_t* out) {
+  API_BEGIN
+  *out = (int64_t)matrix_device_bytes(from_handle<Matrix>(mh, kMatrix, "matrix"));
   API_END
 }
 int B2_MatrixCutsSize(B2Handle mh, int32_t* total) {
@@ -761,8 +790,8 @@ int B2_BoosterPredictContribs(B2Handle bh, B2Handle mh, int32_t tree_begin, int3
     if (smem > (size_t)200 * 1024) { smem = 0; warps = 8; }
   }
   const bool gscratch = interactions || smem == 0;
-  const int64_t blk = rows_per_block(m->n, per_row * (sizeof(float) + (gscratch ? sizeof(double) : 0)));
-  DevBuf<float> d_out; DevBuf<double> d_acc;
+  const int64_t blk = std::min(rows_per_block(m->n, per_row * (sizeof(float) + (gscratch ? sizeof(double) : 0))), raw_tile_rows(m));
+  DevBuf<float> d_out, tile; DevBuf<double> d_acc;
   d_out.ensure((size_t)std::max<int64_t>(blk, 1) * per_row);
   if (gscratch) d_acc.ensure((size_t)std::max<int64_t>(blk, 1) * per_row);
   std::vector<cudaEvent_t> ev;
@@ -770,14 +799,16 @@ int B2_BoosterPredictContribs(B2Handle bh, B2Handle mh, int32_t tree_begin, int3
     const int64_t rows = std::min<int64_t>(blk, m->n - r0);
     cudaEvent_t e0, e1; CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
     ev.push_back(e0); ev.push_back(e1);
+    const float* X = raw_rows(m, r0, rows, tile);   // row 0 of X is row r0 of the matrix
+    const float* bm_rows = bm ? bm + (size_t)r0 * K : nullptr;
     CUDA_CHECK(cudaEventRecord(e0, s));
     if (interactions)
-      LAUNCH_CHECK(b2_launch_shap_interactions(m->raw.p, r0, rows, F, m->missing, b->d_path_elems.p, b->d_paths.p, p_begin, p_end,
-                                               b->d_path_cats.p, K, d_bias.p, bm, base_value, d_acc.p, d_out.p, b->ctx->num_sms, s));
+      LAUNCH_CHECK(b2_launch_shap_interactions(X, 0, rows, F, m->missing, b->d_path_elems.p, b->d_paths.p, p_begin, p_end,
+                                               b->d_path_cats.p, K, d_bias.p, bm_rows, base_value, d_acc.p, d_out.p, b->ctx->num_sms, s));
     else
-      LAUNCH_CHECK(b2_launch_shap_contribs(m->raw.p, r0, rows, F, m->missing, b->d_path_elems.p, b->d_paths.p, p_begin, p_end,
-                                           b->d_path_cats.p, K, d_bias.p, bm, base_value, gscratch ? d_acc.p : nullptr, warps, smem,
-                                           d_out.p, b->ctx->num_sms, s));
+      LAUNCH_CHECK(b2_launch_shap_contribs(X, 0, rows, F, m->missing, b->d_path_elems.p, b->d_paths.p, p_begin, p_end,
+                                           b->d_path_cats.p, K, d_bias.p, bm_rows, base_value, gscratch ? d_acc.p : nullptr, warps,
+                                           smem, d_out.p, b->ctx->num_sms, s));
     CUDA_CHECK(cudaEventRecord(e1, s));
     CUDA_CHECK(cudaMemcpyAsync(out + (size_t)r0 * per_row, d_out.p, (size_t)rows * per_row * sizeof(float), cudaMemcpyDeviceToHost, s));
   }
@@ -803,12 +834,12 @@ int B2_BoosterPredictLeaf(B2Handle bh, B2Handle mh, int32_t tree_begin, int32_t 
   if (out_len != m->n * T) fail("output buffer has %lld values, expected %lld", (long long)out_len, (long long)(m->n * T));
   if (T == 0 || m->n == 0) return 0;
   sync_device_trees(b);
-  const int64_t blk = rows_per_block(m->n, (size_t)T * sizeof(float));
-  DevBuf<float> d_out; d_out.ensure((size_t)blk * T);
+  const int64_t blk = std::min(rows_per_block(m->n, (size_t)T * sizeof(float)), raw_tile_rows(m));
+  DevBuf<float> d_out, tile; d_out.ensure((size_t)blk * T);
   for (int64_t r0 = 0; r0 < m->n; r0 += blk) {
     const int64_t rows = std::min<int64_t>(blk, m->n - r0);
-    LAUNCH_CHECK(b2_launch_leaf_index(m->raw.p, r0, rows, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p,
-                                      tree_begin, tree_end, d_out.p, b->ctx->num_sms, s));
+    LAUNCH_CHECK(b2_launch_leaf_index(raw_rows(m, r0, rows, tile), 0, rows, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p,
+                                      b->d_cat_table.p, tree_begin, tree_end, d_out.p, b->ctx->num_sms, s));
     CUDA_CHECK(cudaMemcpyAsync(out + (size_t)r0 * T, d_out.p, (size_t)rows * T * sizeof(float), cudaMemcpyDeviceToHost, s));
   }
   CUDA_CHECK(cudaStreamSynchronize(s));

@@ -169,7 +169,13 @@ struct Matrix : HandleBase {
   int F = 0;
   float missing = NAN;
   DevBuf<float> raw;     // [n][F], optional
-  bool has_raw = false;
+  // CSR raw values instead of raw (B2_MatrixCreateFromCSR): row i stores entries [indptr[i], indptr[i+1]) of indices /
+  // values, columns strictly increasing; an entry a row does not store is missing.  Kernels get raw rows through
+  // raw_rows / for_raw_tiles, never from these buffers directly.
+  bool csr = false;
+  int64_t nnz = 0;
+  DevBuf<int64_t> csr_indptr; DevBuf<int32_t> csr_indices; DevBuf<float> csr_values;
+  bool has_raw = false;  // raw, or the CSR buffers, are on the device
   DevBuf<uint8_t> bins;  // [n][row_stride]
   DevBuf<uint8_t> bins_col;  // [F][col_stride] feature-major copy for the row partition
   int64_t col_stride = 0;
@@ -209,6 +215,30 @@ void upload(DevBuf<T>& d, const std::vector<T>& h, cudaStream_t s) {
   d.ensure(h.size() ? h.size() : 1);
   if (!h.empty()) CUDA_CHECK(cudaMemcpyAsync(d.p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, s));
 }
+
+// ---- raw rows (matrix.cu): the one place that knows whether a matrix holds its raw values dense or as CSR
+constexpr size_t kRawTileBytes = (size_t)256 << 20;   // largest dense tile densified from a CSR matrix
+// rows of one raw tile: all rows of a dense matrix; for CSR floor(kRawTileBytes / (4 F)) rounded down to a multiple of
+// 128 (at least 128), so every tile starts on the 128-row alignment of bins_col's column stride
+int64_t raw_tile_rows(const Matrix* m);
+// dense float rows [r0, r0 + rows) x [0, F): a pointer into raw, or `tile` filled from the CSR (rows <= raw_tile_rows)
+const float* raw_rows(Matrix* m, int64_t r0, int64_t rows, DevBuf<float>& tile);
+// fn(X, r0, rows) over consecutive raw tiles covering every row (once with rows = 0 for an empty matrix).  A dense
+// matrix is one call with X = raw: the kernels run exactly as on a plain dense matrix.
+template <typename Fn>
+void for_raw_tiles(Matrix* m, Fn fn) {
+  DevBuf<float> tile;
+  const int64_t step = raw_tile_rows(m);
+  int64_t r0 = 0;
+  do {
+    const int64_t rows = std::min<int64_t>(step, m->n - r0);
+    fn(raw_rows(m, r0, rows, tile), r0, rows);
+    r0 += step;
+  } while (r0 < m->n);
+}
+void upload_csr(Matrix* m, const int64_t* indptr, const int32_t* indices, const float* values);
+void release_raw(Matrix* m);
+size_t matrix_device_bytes(const Matrix* m);
 
 void setup_groups(Matrix* m);
 void check_borrowed_categories(Matrix* m, Comm* comm);

@@ -227,6 +227,14 @@ int b2_launch_bin(const float* X, int64_t n, int F, float missing, const int32_t
 int b2_launch_cat_stats(const float* X, int64_t n, int F, float missing, const int32_t* cat_feats, int n_cat, int32_t* stats,
                         int num_sms, cudaStream_t s);
 
+// sparse_kernel.cu (CSR raw values: indptr [n+1], indices / values [nnz])
+int b2_launch_csr_validate(const int64_t* indptr, const int32_t* indices, int64_t n, int F, int64_t nnz, unsigned long long* bad,
+                           int num_sms, cudaStream_t s);
+int b2_launch_csr_densify(const int64_t* indptr, const int32_t* indices, const float* values, int64_t r0, int64_t rows, int F,
+                          float* out, int num_sms, cudaStream_t s);
+int b2_launch_csr_extract_keys(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int f0, int nf,
+                               float missing, uint32_t* keys, int64_t n_padded, int num_sms, cudaStream_t s);
+
 // refresh_kernel.cu
 int b2_launch_refresh(const float* X, int64_t n, int F, float missing, const B2TreeNodeDev* nodes, int n_nodes,
                       const uint32_t* cat_table, int n_leaves, const float2* gh, const int32_t* qexp, int leaf_bits,

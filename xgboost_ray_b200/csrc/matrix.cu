@@ -38,6 +38,87 @@ void setup_groups(Matrix* m) {
   }
 }
 
+int64_t raw_tile_rows(const Matrix* m) {
+  if (!m->csr) return std::max<int64_t>(m->n, 1);
+  const int64_t rows = (int64_t)(kRawTileBytes / (4 * (size_t)m->F)) & ~(int64_t)127;
+  return std::max<int64_t>(rows, 128);
+}
+
+const float* raw_rows(Matrix* m, int64_t r0, int64_t rows, DevBuf<float>& tile) {
+  if (!m->has_raw) fail("matrix has no raw data on the device");
+  if (!m->csr) return m->raw.p + (size_t)r0 * m->F;
+  tile.ensure((size_t)std::max<int64_t>(rows, 1) * m->F);
+  LAUNCH_CHECK(b2_launch_csr_densify(m->csr_indptr.p, m->csr_indices.p, m->csr_values.p, r0, rows, m->F, tile.p, m->ctx->num_sms,
+                                     m->ctx->stream));
+  return tile.p;
+}
+
+// Uploads the CSR arrays of m (n rows, F columns and nnz set) and checks them on the device in one pass; the first row
+// that breaks a rule is named, with the rule read back from the caller's arrays.  The check guards the C ABI: an
+// out-of-range column would be written outside a densified tile.
+void upload_csr(Matrix* m, const int64_t* indptr, const int32_t* indices, const float* values) {
+  Ctx* ctx = m->ctx; cudaStream_t s = ctx->stream;
+  const int64_t n = m->n, nnz = m->nnz;
+  m->csr_indptr.ensure((size_t)n + 1); m->csr_indices.ensure((size_t)nnz); m->csr_values.ensure((size_t)nnz);
+  upload_pipelined(ctx, m->csr_indptr.p, indptr, ((size_t)n + 1) * sizeof(int64_t));
+  upload_pipelined(ctx, m->csr_indices.p, indices, (size_t)nnz * sizeof(int32_t));
+  upload_pipelined(ctx, m->csr_values.p, values, (size_t)nnz * sizeof(float));
+  if (n == 0) {
+    if (indptr[0] != 0 || nnz != 0) fail("CSR matrix without rows: indptr[0] = %lld and nnz = %lld must be 0", (long long)indptr[0], (long long)nnz);
+    m->has_raw = true;
+    return;
+  }
+  DevBuf<unsigned long long> d_bad; d_bad.ensure(1);
+  LAUNCH_CHECK(b2_launch_csr_validate(m->csr_indptr.p, m->csr_indices.p, n, m->F, nnz, d_bad.p, ctx->num_sms, s));
+  unsigned long long bad = 0;
+  CUDA_CHECK(cudaMemcpyAsync(&bad, d_bad.p, sizeof(bad), cudaMemcpyDeviceToHost, s));
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  if (bad != ~0ull) {
+    const int64_t i = (int64_t)bad, b = indptr[i], e = indptr[i + 1];
+    if (i == 0 && b != 0) fail("CSR row 0: indptr[0] = %lld, must be 0", (long long)b);
+    if (b > e) fail("CSR row %lld: indptr decreases (indptr[%lld] = %lld > indptr[%lld] = %lld)", (long long)i, (long long)i,
+                    (long long)b, (long long)(i + 1), (long long)e);
+    if (b < 0 || e > nnz) fail("CSR row %lld: entries [%lld, %lld) outside the %lld stored entries", (long long)i, (long long)b,
+                               (long long)e, (long long)nnz);
+    for (int64_t k = b; k < e; ++k) {
+      const int c = indices[k];
+      if (c < 0 || c >= m->F) fail("CSR row %lld: column %d is outside [0, %d)", (long long)i, c, m->F);
+      if (k > b && c == indices[k - 1]) fail("CSR row %lld: column %d is stored twice", (long long)i, c);
+      if (k > b && c < indices[k - 1])
+        fail("CSR row %lld: column %d follows column %d (the columns of a row must increase)", (long long)i, c, indices[k - 1]);
+    }
+    fail("CSR row %lld: indptr[%lld] = %lld, must equal nnz = %lld", (long long)i, (long long)(i + 1), (long long)e, (long long)nnz);
+  }
+  m->has_raw = true;
+}
+
+void release_raw(Matrix* m) {
+  m->raw.release();
+  m->csr_indptr.release(); m->csr_indices.release(); m->csr_values.release();
+  m->has_raw = false;
+}
+
+template <typename T>
+static size_t buf_bytes(const DevBuf<T>& d) { return d.cap * sizeof(T); }
+size_t matrix_device_bytes(const Matrix* m) {
+  return buf_bytes(m->raw) + buf_bytes(m->csr_indptr) + buf_bytes(m->csr_indices) + buf_bytes(m->csr_values) +
+         buf_bytes(m->bins) + buf_bytes(m->bins_col) + buf_bytes(m->d_group_first) + buf_bytes(m->d_group_size) +
+         buf_bytes(m->d_feat_byte) + buf_bytes(m->d_cut_ptrs) + buf_bytes(m->d_nbins) + buf_bytes(m->d_cat_feats) +
+         buf_bytes(m->d_cut_vals) + buf_bytes(m->d_has_missing) + buf_bytes(m->d_is_cat) + buf_bytes(m->label) +
+         buf_bytes(m->weight) + buf_bytes(m->base_margin) + buf_bytes(m->lower) + buf_bytes(m->upper) +
+         buf_bytes(m->qgroup_ptr) + buf_bytes(m->d_fwq);
+}
+
+// sketch keys [kExtractBatch][n_pad] of features [f0, f0 + nf) (missing values and padding rows: 0xffffffff)
+static void extract_keys(Matrix* m, int f0, int nf, uint32_t* keys, int64_t n_pad) {
+  Ctx* ctx = m->ctx;
+  if (m->csr)
+    LAUNCH_CHECK(b2_launch_csr_extract_keys(m->csr_indptr.p, m->csr_indices.p, m->csr_values.p, m->n, f0, nf, m->missing, keys,
+                                            n_pad, ctx->num_sms, ctx->stream));
+  else
+    LAUNCH_CHECK(b2_launch_extract_keys(m->raw.p, m->n, m->F, f0, nf, m->missing, keys, n_pad, ctx->num_sms, ctx->stream));
+}
+
 void upload_cuts(Matrix* m) {
   cudaStream_t s = m->ctx->stream;
   m->nbins.resize(m->F);
@@ -63,7 +144,9 @@ std::vector<int32_t> category_stats(Matrix* m, Comm* comm) {
   d_cat.ensure((size_t)n_cat * 3); d_catf.ensure((size_t)n_cat);
   CUDA_CHECK(cudaMemcpyAsync(d_cat.p, h_cat.data(), (size_t)n_cat * 3 * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   CUDA_CHECK(cudaMemcpyAsync(d_catf.p, m->cat_feats.data(), (size_t)n_cat * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-  LAUNCH_CHECK(b2_launch_cat_stats(m->raw.p, m->n, m->F, m->missing, d_catf.p, n_cat, d_cat.p, m->ctx->num_sms, s));
+  for_raw_tiles(m, [&](const float* X, int64_t, int64_t rows) {   // the stats are maxima: they accumulate over the tiles
+    LAUNCH_CHECK(b2_launch_cat_stats(X, rows, m->F, m->missing, d_catf.p, n_cat, d_cat.p, m->ctx->num_sms, s));
+  });
   allreduce(comm, d_cat.p, (size_t)n_cat * 3, kNcclInt32, kNcclMax, s);
   CUDA_CHECK(cudaMemcpyAsync(h_cat.data(), d_cat.p, (size_t)n_cat * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   CUDA_CHECK(cudaStreamSynchronize(s));
@@ -177,7 +260,7 @@ void make_cuts(Matrix* m, Comm* comm, int max_bin) {
     bool any_numeric = false;
     for (int j = 0; j < nf; ++j) any_numeric = any_numeric || !m->is_cat[f0 + j];
     if (!any_numeric) continue;
-    LAUNCH_CHECK(b2_launch_extract_keys(m->raw.p, m->n, F, f0, nf, m->missing, keys_local.p, n_pad, ctx->num_sms, s));
+    extract_keys(m, f0, nf, keys_local.p, n_pad);
     for (int j = 0; j < nf; ++j) {
       const int f = f0 + j;
       if (m->is_cat[f]) continue;   // categorical: cuts are the codes 0..max (below)
@@ -233,9 +316,13 @@ void bin_matrix(Matrix* m) {
   CUDA_CHECK(cudaMemsetAsync(m->bins.p, 0, (size_t)std::max<int64_t>(m->n, 1) * m->row_stride, s));
   m->col_stride = (std::max<int64_t>(m->n, 1) + 127) & ~(int64_t)127;
   m->bins_col.ensure((size_t)m->col_stride * m->F);
-  LAUNCH_CHECK(b2_launch_bin(m->raw.p, m->n, m->F, m->missing, m->d_cut_ptrs.p, m->d_cut_vals.p, m->d_feat_byte.p,
-                             m->any_cat() ? m->d_is_cat.p : nullptr, m->row_stride, m->bins.p, m->bins_col.p, m->col_stride,
-                             ctx->num_sms, s));
+  // both bin kernels write rows [0, rows) of the bins / bins_col they are given and nothing else, so a tile writes its
+  // own rows only
+  for_raw_tiles(m, [&](const float* X, int64_t r0, int64_t rows) {
+    LAUNCH_CHECK(b2_launch_bin(X, rows, m->F, m->missing, m->d_cut_ptrs.p, m->d_cut_vals.p, m->d_feat_byte.p,
+                               m->any_cat() ? m->d_is_cat.p : nullptr, m->row_stride, m->bins.p + (size_t)r0 * m->row_stride,
+                               m->bins_col.p + r0, m->col_stride, ctx->num_sms, s));
+  });
   CUDA_CHECK(cudaStreamSynchronize(s));
   m->quantized = true;
 }

@@ -104,13 +104,17 @@ const float* device_weights(Booster* b) {
 
 // out += the trees [tree_begin, tree_end) on the raw rows of m (the device trees are in sync)
 void predict_trees(Booster* b, Matrix* m, int tree_begin, int tree_end, float* out) {
-  if (b->p.vector_leaf())
-    LAUNCH_CHECK(b2_launch_predict_vector(m->raw.p, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_leaf_table.p,
-                                          tree_begin, tree_end, b->p.num_target, out, b->ctx->num_sms, b->ctx->stream));
-  else
-    LAUNCH_CHECK(b2_launch_predict(m->raw.p, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, tree_begin,
-                                   tree_end, b->p.num_class, b->p.num_parallel_tree, device_weights(b), out, b->ctx->num_sms,
-                                   b->ctx->stream));
+  const float* w = b->p.vector_leaf() ? nullptr : device_weights(b);
+  for_raw_tiles(m, [&](const float* X, int64_t r0, int64_t rows) {
+    if (b->p.vector_leaf())
+      LAUNCH_CHECK(b2_launch_predict_vector(X, rows, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_leaf_table.p,
+                                            tree_begin, tree_end, b->p.num_target, out + (size_t)r0 * b->p.num_target,
+                                            b->ctx->num_sms, b->ctx->stream));
+    else
+      LAUNCH_CHECK(b2_launch_predict(X, rows, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, tree_begin,
+                                     tree_end, b->p.num_class, b->p.num_parallel_tree, w, out + (size_t)r0 * b->p.num_class,
+                                     b->ctx->num_sms, b->ctx->stream));
+  });
 }
 
 // margin of matrix m under the current model (cached per matrix, only new trees are applied)

@@ -14,20 +14,9 @@
 
 #include "common.cuh"
 #include "launch.h"
+#include "raw_keys.cuh"
 
 namespace b2 {
-
-__device__ __forceinline__ uint32_t f2key(float f) {
-  uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key2f(uint32_t k) {
-  uint32_t u = (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k;
-  return __uint_as_float(u);
-}
-__device__ __forceinline__ bool is_missing(float x, float missing, int missing_is_nan) {
-  return isnan(x) || (!missing_is_nan && x == missing);
-}
 
 // keys of kBatch consecutive feature columns in one pass: thread (row, j) reads X[row][f0+j], so a warp
 // reads 4 rows x 32 contiguous bytes (whole sectors) instead of one float per 4*F-byte row.
@@ -41,7 +30,7 @@ __global__ void extract_keys_kernel(const float* __restrict__ X, int64_t n, int 
     uint32_t k = 0xffffffffu;
     if (i < n) {
       float x = X[i * F + f0 + j];
-      if (!is_missing(x, missing, missing_is_nan)) { if (x == 0.0f) x = 0.0f; k = f2key(x); }
+      if (!is_missing(x, missing, missing_is_nan)) k = sketch_key(x);
     }
     keys[(int64_t)j * n_padded + i] = k;
   }

@@ -1,0 +1,124 @@
+// sparse_kernel.cu -- the raw values of a CSR matrix (B2_MatrixCreateFromCSR): validation of the three arrays, dense
+// row tiles for the kernels that read raw rows, and the sketch keys of a batch of features read straight from the CSR.
+//
+// An entry a row does not store is missing.  A stored entry is copied bit for bit, so every kernel that reads a tile
+// sees exactly the floats of the matrix's dense twin (the same matrix with NaN in every absent cell).
+#include <stdint.h>
+
+#include <algorithm>
+
+#include "common.cuh"
+#include "launch.h"
+#include "raw_keys.cuh"
+
+namespace b2 {
+
+constexpr int kSparseThreads = 256;
+constexpr int kDensifyCells = 4096;      // cells of one CTA step (rows * F), so that narrow matrices fill the CTA
+constexpr int kDensifyMaxRows = 1024;    // rows of one CTA step (the row pointers staged in shared memory)
+
+// bad = smallest row that breaks a rule: indptr[0] = 0, indptr[n] = nnz, indptr non-decreasing and inside [0, nnz],
+// every column in [0, F) and the columns of a row strictly increasing (no duplicates).  One thread per row.
+__global__ void __launch_bounds__(kSparseThreads)
+csr_validate_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, int64_t n, int F, int64_t nnz,
+                    unsigned long long* __restrict__ bad) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t b = indptr[i], e = indptr[i + 1];
+    bool ok = b >= 0 && b <= e && e <= nnz && (i != 0 || b == 0) && (i != n - 1 || e == nnz);
+    for (int64_t k = b, prev = -1; ok && k < e; ++k) {
+      const int c = indices[k];
+      ok = c > prev && c < F;   // prev = -1 first: a negative column fails too
+      prev = c;
+    }
+    if (!ok) atomicMin(bad, (unsigned long long)i);
+  }
+}
+
+// out [rows][F] = rows [r0, r0 + rows) of the CSR, NaN where a row stores nothing.  A CTA step covers `step` rows: it
+// fills their cells with NaN, then scatters their stored entries (one thread per entry, its row found by a binary
+// search of the step's row pointers in shared memory).  The entries of a step are contiguous in indices / values, so
+// both phases read and write whole sectors.
+__global__ void __launch_bounds__(kSparseThreads)
+csr_densify_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, const uint32_t* __restrict__ values,
+                   int64_t r0, int64_t rows, int F, int step, uint32_t* __restrict__ out) {
+  __shared__ int64_t sptr[kDensifyMaxRows + 1];
+  const int64_t n_steps = (rows + step - 1) / step;
+  for (int64_t blk = blockIdx.x; blk < n_steps; blk += gridDim.x) {
+    const int64_t lr0 = blk * step;
+    const int nr = (int)min((int64_t)step, rows - lr0);
+    uint32_t* dst = out + lr0 * F;
+    const int64_t cells = (int64_t)nr * F;
+    for (int64_t c = threadIdx.x; c < cells; c += blockDim.x) dst[c] = 0x7fc00000u;   // NaN
+    for (int i = threadIdx.x; i <= nr; i += blockDim.x) sptr[i] = indptr[r0 + lr0 + i];
+    __syncthreads();
+    const int64_t e1 = sptr[nr];
+    for (int64_t e = sptr[0] + threadIdx.x; e < e1; e += blockDim.x) {
+      int lo = 0, hi = nr;   // the last row of the step whose first entry is <= e
+      while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (sptr[mid] <= e) lo = mid; else hi = mid; }
+      dst[(int64_t)lo * F + __ldg(indices + e)] = __ldg(values + e);
+    }
+    __syncthreads();
+  }
+}
+
+// keys [kExtractBatch][n_padded] of features [f0, f0 + nf), the layout of extract_keys_kernel (sketch.cu); the caller
+// sets every key to the missing sentinel 0xffffffff first.  One thread per row: a binary search finds the row's first
+// column >= f0, then the row's entries in the window are keyed.
+__global__ void __launch_bounds__(kSparseThreads)
+csr_extract_keys_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, const float* __restrict__ values,
+                        int64_t n, int f0, int nf, float missing, int missing_is_nan, uint32_t* __restrict__ keys,
+                        int64_t n_padded) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t end = indptr[i + 1];
+    int64_t lo = indptr[i], hi = end;
+    while (lo < hi) { const int64_t mid = (lo + hi) >> 1; if (__ldg(indices + mid) < f0) lo = mid + 1; else hi = mid; }
+    for (int64_t e = lo; e < end; ++e) {
+      const int j = __ldg(indices + e) - f0;
+      if (j >= nf) break;
+      const float x = __ldg(values + e);
+      if (!is_missing(x, missing, missing_is_nan)) keys[(int64_t)j * n_padded + i] = sketch_key(x);
+    }
+  }
+}
+
+}  // namespace b2
+
+static inline int sparse_grid(int64_t work, int num_sms) {
+  int64_t g = (work + b2::kSparseThreads - 1) / b2::kSparseThreads, cap = (int64_t)num_sms * 8;
+  if (g > cap) g = cap;
+  if (g < 1) g = 1;
+  return (int)g;
+}
+
+extern "C" {
+
+int b2_launch_csr_validate(const int64_t* indptr, const int32_t* indices, int64_t n, int F, int64_t nnz, unsigned long long* bad,
+                           int num_sms, cudaStream_t s) {
+  cudaError_t e = cudaMemsetAsync(bad, 0xff, sizeof(unsigned long long), s);
+  if (e != cudaSuccess || n <= 0) return (int)e;
+  b2::csr_validate_kernel<<<sparse_grid(n, num_sms), b2::kSparseThreads, 0, s>>>(indptr, indices, n, F, nnz, bad);
+  return (int)cudaGetLastError();
+}
+
+int b2_launch_csr_densify(const int64_t* indptr, const int32_t* indices, const float* values, int64_t r0, int64_t rows, int F,
+                          float* out, int num_sms, cudaStream_t s) {
+  if (rows <= 0) return 0;
+  const int step = F >= b2::kDensifyCells ? 1 : std::min(b2::kDensifyMaxRows, b2::kDensifyCells / F);
+  const int64_t n_steps = (rows + step - 1) / step;
+  const int grid = (int)std::min<int64_t>(n_steps, (int64_t)num_sms * 8);
+  b2::csr_densify_kernel<<<grid, b2::kSparseThreads, 0, s>>>(indptr, indices, reinterpret_cast<const uint32_t*>(values), r0, rows,
+                                                            F, step, reinterpret_cast<uint32_t*>(out));
+  return (int)cudaGetLastError();
+}
+
+int b2_launch_csr_extract_keys(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int f0, int nf,
+                               float missing, uint32_t* keys, int64_t n_padded, int num_sms, cudaStream_t s) {
+  if (n_padded <= 0) return 0;
+  cudaError_t e = cudaMemsetAsync(keys, 0xff, (size_t)nf * n_padded * sizeof(uint32_t), s);
+  if (e != cudaSuccess || n <= 0) return (int)e;
+  b2::csr_extract_keys_kernel<<<sparse_grid(n, num_sms), b2::kSparseThreads, 0, s>>>(indptr, indices, values, n, f0, nf, missing,
+                                                                                   missing != missing ? 1 : 0, keys, n_padded);
+  return (int)cudaGetLastError();
+}
+
+}  // extern "C"

@@ -1,4 +1,4 @@
-"""Data-source adapters for RayDMatrix: numpy, pandas, CSV, Parquet (single file or list of files).
+"""Data-source adapters for RayDMatrix: numpy, pandas, scipy.sparse, CSV, Parquet (single file or list of files).
 
 Mirrors the adapter registry of the reference (xgboost_ray/data_sources/__init__.py:13-24,
 data_source.py:22-155, numpy.py:13-33, pandas.py:8-30, csv.py:9-47, parquet.py:9-48).  The
@@ -193,14 +193,41 @@ class Parquet(DataSource):
         return 1 if isinstance(data, str) else len(data)
 
 
-data_sources = [Numpy, Pandas, CSV, Parquet]
+class Sparse(DataSource):
+    """A scipy.sparse matrix or array (CSR, CSC, COO), loaded centrally.  RayDMatrix keeps it in CSR form and shards
+    it by rows; it is never densified on the host."""
+    needs_partitions = True
+
+    @staticmethod
+    def is_data_type(data, filetype=None):
+        from xgboost_ray_b200.engine import is_sparse
+        return is_sparse(data)
+
+    @staticmethod
+    def load_data(data, ignore=None, indices=None, **kwargs):
+        from xgboost_ray_b200.engine import canonical_csr
+        if ignore:
+            raise ValueError("`ignore` names columns, but a scipy.sparse matrix has none (got %r)" % (ignore,))
+        return canonical_csr(data)
+
+    @staticmethod
+    def get_n(data):
+        return data.shape[0]
+
+
+data_sources = [Numpy, Pandas, Sparse, CSV, Parquet]
 
 
 def resolve_data_source(data, filetype=None):
+    if _is_path_like(data, ".libsvm") or _is_path_like(data, ".svm"):
+        raise ValueError("LIBSVM text files are not supported (%r): load them with "
+                         "sklearn.datasets.load_svmlight_file and pass the scipy.sparse matrix" % (data,))
+    if isinstance(data, (list, tuple)) and data and any(Sparse.is_data_type(d) for d in data):
+        raise ValueError("a list of scipy.sparse row blocks is not supported: pass one matrix (scipy.sparse.vstack)")
     for src in data_sources:
         if src.is_data_type(data, filetype):
             return src
     raise ValueError(
         "Unknown data source type: %s with FileType: %s.\nFIX THIS by passing a numpy array, a pandas "
-        "DataFrame/Series, or CSV / Parquet file name(s) (Modin/Dask/Petastorm/Ray datasets are out of scope "
+        "DataFrame/Series, a scipy.sparse matrix, or CSV / Parquet file name(s) (Modin/Dask/Petastorm/Ray datasets are out of scope "
         "of the single-node H100 build)." % (type(data), filetype))

@@ -13,6 +13,7 @@ import ast
 import ctypes as C
 import json
 import os
+import sys
 import threading
 
 import numpy as np
@@ -34,6 +35,7 @@ _FP = C.POINTER(C.c_float)
 _IP = C.POINTER(C.c_int32)
 _BP = C.POINTER(C.c_uint8)
 _DP = C.POINTER(C.c_double)
+_LP = C.POINTER(C.c_int64)
 _H = C.c_uint64
 _FLT_MAX = np.finfo(np.float32).max
 
@@ -50,6 +52,8 @@ ABI = {
     "B2_CommFree": (C.c_int, [_H]),
     "B2_MatrixCreateFromDense": (C.c_int, [_FP, C.c_int64, C.c_int32, C.c_float, C.c_int, C.POINTER(_H)]),
     "B2_MatrixCreate": (C.c_int, [C.c_int64, C.c_int32, C.c_float, C.c_int, C.POINTER(_H)]),
+    "B2_MatrixCreateFromCSR": (C.c_int, [_LP, _IP, _FP, C.c_int64, C.c_int32, C.c_int64, C.c_float, C.c_int,
+                                         C.POINTER(_H)]),
     "B2_MatrixCreateFromProcessInterleaved": (C.c_int, [C.c_int64, C.c_uint64, C.c_int64, C.c_int32, C.c_int32, _H,
                                                         C.c_float, C.c_int, C.POINTER(_H)]),
     "B2_MatrixCreateFromProcess": (C.c_int, [C.c_int64, C.c_uint64, C.c_int64, C.c_int64, C.c_int32, C.c_float, C.c_int,
@@ -65,6 +69,8 @@ ABI = {
     "B2_MatrixQuantize": (C.c_int, [_H, _H, C.c_int32, _H, C.c_int32]),
     "B2_MatrixQuantizeWithCuts": (C.c_int, [_H, _H, _IP, _FP, _FP, _BP, C.c_int32, C.c_int32]),
     "B2_MatrixEnsureRaw": (C.c_int, [_H, _FP]),
+    "B2_MatrixEnsureRawCSR": (C.c_int, [_H, _LP, _IP, _FP]),
+    "B2_MatrixDeviceBytes": (C.c_int, [_H, C.POINTER(C.c_int64)]),
     "B2_MatrixCutsSize": (C.c_int, [_H, _IP]),
     "B2_MatrixGetCuts": (C.c_int, [_H, _IP, _FP, _FP, _BP]),
     "B2_MatrixGetBins": (C.c_int, [_H, _BP]),
@@ -228,6 +234,85 @@ class collective:  # namespace shim: xgb.collective.get_rank() (session.py:73)
         return a
 
 
+# ----------------------------------------------------------------------------- sparse input
+def is_sparse(data):
+    """True for a scipy.sparse matrix or array.  scipy is never imported here: a caller holding one has imported it."""
+    sp = sys.modules.get("scipy.sparse")
+    return sp is not None and sp.issparse(data)
+
+
+class CSRArrays:
+    """The canonical CSR form of a sparse input: int64 `indptr` [n+1], int32 `indices` and float32 `values` [nnz], the
+    columns of every row strictly increasing, and the input's `shape` (trailing columns that store nothing count)."""
+
+    def __init__(self, indptr, indices, values, shape):
+        self.indptr, self.indices, self.values = indptr, indices, values
+        self.shape = (int(shape[0]), int(shape[1]))
+        self.ndim = 2
+
+    @property
+    def nnz(self):
+        return int(self.indices.size)
+
+
+RAW_TILE_BYTES = 256 << 20   # host.h kRawTileBytes
+
+
+def raw_tile_rows(n_cols):
+    """Rows of one dense tile the device densifies from a CSR matrix of n_cols columns (host.h raw_tile_rows): at most
+    RAW_TILE_BYTES of float32, a multiple of 128 rows, at least 128."""
+    return max(RAW_TILE_BYTES // (4 * int(n_cols)) // 128 * 128, 128)
+
+
+def _cast(a, dtype):
+    """`a` C-contiguous with `dtype`; the array itself when it already is (no copy)."""
+    return np.ascontiguousarray(a, dtype=dtype)
+
+
+def canonical_csr(X):
+    """CSR / CSC / COO (matrix or array) -> CSRArrays.  The caller's matrix is never modified: a conversion or a sort
+    of the columns works on a copy.  A (row, column) stored twice is refused (a COO matrix is converted without summing
+    its duplicates, so they are refused too)."""
+    if X.ndim != 2:
+        raise XGBoostError("DMatrix data must be 2-dimensional, got a sparse input of shape %s" % (X.shape,))
+    n, f = X.shape
+    if X.format == "coo":
+        row, col = np.asarray(X.row, np.int64), np.asarray(X.col, np.int64)
+        order = np.lexsort((col, row))
+        indptr = np.zeros(n + 1, np.int64)
+        np.cumsum(np.bincount(row, minlength=n), out=indptr[1:])
+        indices, values = _cast(col[order], np.int32), _cast(np.asarray(X.data)[order], np.float32)
+    else:
+        X = X.tocsr()   # CSC: a transposed copy; CSR: the matrix itself
+        indptr, indices, values = _cast(X.indptr, np.int64), _cast(X.indices, np.int32), _cast(X.data, np.float32)
+        if indptr.size != n + 1 or indices.size != int(indptr[-1]) or values.size != indices.size:
+            raise XGBoostError("sparse input: inconsistent CSR arrays (%d row pointers, %d columns, %d values for %d rows)"
+                               % (indptr.size, indices.size, values.size, n))
+        step = _row_steps(indptr, indices)
+        if step.size and step.min() < 0:   # unsorted columns within a row: sort a copy
+            Xs = X.sorted_indices()
+            indices, values = _cast(Xs.indices, np.int32), _cast(Xs.data, np.float32)
+    step = _row_steps(indptr, indices)
+    if step.size and step.min() <= 0:
+        k = int(np.flatnonzero(step <= 0)[0])
+        r = int(np.searchsorted(indptr, k, side="right")) - 1
+        raise XGBoostError("sparse input: row %d stores column %d twice" % (r, int(indices[k])))
+    if indices.size and (int(indices.min()) < 0 or int(indices.max()) >= f):
+        raise XGBoostError("sparse input: a column index is outside [0, %d)" % f)
+    return CSRArrays(indptr, indices, values, (n, f))
+
+
+def _row_steps(indptr, indices):
+    """indices[k + 1] - indices[k] for the consecutive entries k, k + 1 of one row (positions that end a row hold 1)."""
+    if indices.size < 2:
+        return np.zeros(0, np.int64)
+    step = np.diff(indices.astype(np.int64))
+    ends = indptr[1:-1]
+    ends = ends[(ends > 0) & (ends < indices.size)] - 1
+    step[ends] = 1
+    return step
+
+
 # ----------------------------------------------------------------------------- DMatrix
 class DMatrix:
     """Device matrix.  Float data is uploaded at construction; quantisation (GPU sketch + binning)
@@ -242,7 +327,13 @@ class DMatrix:
                  feature_types=None, nthread=None, enable_categorical=False, max_bin=None, ref=None,
                  device=None, label_lower_bound=None, label_upper_bound=None, qid=None, group=None, multi_target=False,
                  **kwargs):
-        if hasattr(data, "values") and not isinstance(data, np.ndarray):  # pandas
+        if is_sparse(data):
+            data = canonical_csr(data)
+        elif hasattr(data, "values") and not isinstance(data, np.ndarray):  # pandas
+            dtypes = list(data.dtypes) if hasattr(data, "columns") else [getattr(data, "dtype", None)]
+            if any(str(dt).startswith("Sparse") for dt in dtypes):
+                raise XGBoostError("pandas columns with a SparseDtype are not supported: pass "
+                                   "scipy.sparse.csr_matrix(df.sparse.to_coo()) instead")
             if feature_names is None and hasattr(data, "columns"):
                 feature_names = [str(c) for c in data.columns]
             cat_cols = [str(dt) == "category" for dt in data.dtypes] if hasattr(data, "columns") else []
@@ -265,13 +356,16 @@ class DMatrix:
                 data = data.values
         blocks = None
         remote = data if (hasattr(data, "pid") and hasattr(data, "row_stride") and hasattr(data, "addr")) else None
-        if remote is not None:                                     # rows of another process (matrix.RemoteBlock)
-            data = remote
+        if remote is not None or isinstance(data, CSRArrays):     # rows of another process (matrix.RemoteBlock) / CSR
+            pass
         elif hasattr(data, "next") and hasattr(data, "reset"):       # xgboost.DataIter protocol (matrix.py:127-196)
             blocks, label, weight, base_margin = _drain_data_iter(data, label, weight, base_margin)
         elif isinstance(data, (list, tuple)) and data and all(hasattr(b, "shape") for b in data):
+            if any(is_sparse(b) for b in data):
+                raise XGBoostError("a list of sparse row blocks is not supported: pass one scipy.sparse matrix "
+                                   "(scipy.sparse.vstack(blocks))")
             blocks = [np.asarray(b.values if hasattr(b, "values") and not isinstance(b, np.ndarray) else b) for b in data]
-        if remote is not None:
+        if remote is not None or isinstance(data, CSRArrays):
             pass
         elif blocks is not None:
             blocks = [b.reshape(-1, 1) if b.ndim == 1 else b for b in blocks]
@@ -318,6 +412,12 @@ class DMatrix:
             # the shard lives in the driver process: read it straight into the pinned upload buffers
             _check(lib().B2_MatrixCreateFromProcess(remote.pid, remote.addr, remote.row_stride, n, f, self.missing, self.device,
                                                     C.byref(h)))
+            self.handle = h.value
+        elif isinstance(self._host, CSRArrays):
+            # the device keeps the CSR: absent entries are missing, kernels read densified tiles of it
+            c = self._host
+            _check(lib().B2_MatrixCreateFromCSR(c.indptr.ctypes.data_as(_LP), _ip(c.indices), _fp(c.values), n, f, c.nnz,
+                                                self.missing, self.device, C.byref(h)))
             self.handle = h.value
         elif isinstance(self._host, _BlockList):
             # several row blocks (multi-file shard / DataIter): one device allocation, each block uploaded at its row
@@ -458,12 +558,23 @@ class DMatrix:
 
     def _ensure_raw(self):
         if not self._has_raw:
+            if isinstance(self._host, CSRArrays):
+                c = self._host
+                _check(lib().B2_MatrixEnsureRawCSR(self.handle, c.indptr.ctypes.data_as(_LP), _ip(c.indices), _fp(c.values)))
+                self._has_raw = True
+                return
             if isinstance(self._host, _BlockList):   # rare (predicting on a block-built training matrix): one host copy
                 self._host = np.concatenate(self._host.blocks, axis=0)
             elif not isinstance(self._host, np.ndarray):   # rows of another process: fetch them once
                 self._host = _f32c(np.asarray(self._host))
             _check(lib().B2_MatrixEnsureRaw(self.handle, _fp(self._host)))
             self._has_raw = True
+
+    def device_bytes(self):
+        """Device bytes this matrix owns (raw values dense or CSR, bins, cuts and info arrays)."""
+        out = C.c_int64(0)
+        _check(lib().B2_MatrixDeviceBytes(self.handle, C.byref(out)))
+        return out.value
 
     def get_cuts(self):
         tot = C.c_int32(0)
@@ -504,6 +615,9 @@ def _drain_data_iter(it, label, weight, base_margin):
     got = {"data": [], "label": [], "weight": [], "base_margin": []}
 
     def input_data(data=None, label=None, weight=None, base_margin=None, **kw):
+        if is_sparse(data):
+            raise XGBoostError("a DataIter batch that is a scipy.sparse matrix is not supported: pass the whole matrix "
+                               "to DMatrix as one scipy.sparse matrix")
         got["data"].append(np.asarray(data.values if hasattr(data, "values") and not isinstance(data, np.ndarray) else data))
         for k, v in (("label", label), ("weight", weight), ("base_margin", base_margin)):
             if v is not None:

@@ -22,7 +22,8 @@ from typing import Dict, Iterable, List, Optional, Sequence
 
 import numpy as np
 
-from xgboost_ray_b200.data_sources import LoadedFrame, RayFileType, resolve_data_source  # noqa: F401
+from xgboost_ray_b200.data_sources import LoadedFrame, RayFileType, Sparse, resolve_data_source  # noqa: F401
+from xgboost_ray_b200.engine import CSRArrays
 
 
 class RayShardingMode(Enum):
@@ -156,8 +157,8 @@ def _parallel_copy(dst: np.ndarray, src: np.ndarray):
     list(pool.map(lambda i: np.copyto(dst[i:i + step], src[i:i + step], casting="unsafe"), range(0, n, step)))
 
 
-def _shared_copy(src: Optional[np.ndarray], tag: str):
-    """Copy `src` (any strided view) into a float32 .npy file under /dev/shm; returns (array view, ('shm', path)).
+def _shared_copy(src: Optional[np.ndarray], tag: str, dtype=np.float32):
+    """Copy `src` (any strided view) into a .npy file of `dtype` under /dev/shm; returns (array view, ('shm', path)).
     Without a usable /dev/shm the copy stays in process memory and travels by pickle."""
     if src is None:
         return None, None
@@ -165,16 +166,16 @@ def _shared_copy(src: Optional[np.ndarray], tag: str):
     if d is not None:
         try:
             st = os.statvfs(d)
-            if st.f_bavail * st.f_frsize < src.size * 4 + (64 << 20):
+            if st.f_bavail * st.f_frsize < src.size * np.dtype(dtype).itemsize + (64 << 20):
                 d = None
         except OSError:
             d = None
     if d is None:
-        a = np.empty(src.shape, np.float32)
+        a = np.empty(src.shape, dtype)
         _parallel_copy(a, src)
         return a, a
     path = os.path.join(d, "b2x_%d_%s_%s.npy" % (os.getpid(), tag, uuid.uuid4().hex[:12]))
-    a = np.lib.format.open_memmap(path, mode="w+", dtype=np.float32, shape=tuple(src.shape))
+    a = np.lib.format.open_memmap(path, mode="w+", dtype=dtype, shape=tuple(src.shape))
     with _SHM_LOCK:
         _SHM_FILES.add(path)
     _parallel_copy(a, src)
@@ -251,6 +252,34 @@ class RemoteBlock:
                 if got != k * row_bytes:
                     raise OSError(ctypes.get_errno(), "process_vm_readv failed: %s" % os.strerror(ctypes.get_errno()))
         return out if dtype is None else out.astype(dtype, copy=False)
+
+
+def csr_take_rows(c: CSRArrays, rows) -> CSRArrays:
+    """Rows `rows` (a slice or an index array) of a canonical CSR, in that order."""
+    n = c.shape[0]
+    if isinstance(rows, slice) and rows.step in (None, 1):
+        r0, r1, _ = rows.indices(n)
+        r1 = max(r0, r1)
+        e0, e1 = int(c.indptr[r0]), int(c.indptr[r1])
+        return CSRArrays(c.indptr[r0:r1 + 1] - e0, c.indices[e0:e1], c.values[e0:e1], (r1 - r0, c.shape[1]))
+    rows = np.arange(n)[rows] if isinstance(rows, slice) else np.asarray(rows, np.int64)
+    starts = c.indptr[rows]
+    lens = c.indptr[rows + 1] - starts
+    indptr = np.zeros(len(rows) + 1, np.int64)
+    np.cumsum(lens, out=indptr[1:])
+    pos = np.repeat(starts - indptr[:-1], lens) + np.arange(int(indptr[-1]), dtype=np.int64)
+    return CSRArrays(indptr, c.indices[pos], c.values[pos], (len(rows), c.shape[1]))
+
+
+def _shared_csr(c: CSRArrays, tag: str):
+    """A CSR shard as three /dev/shm .npy files (indptr int64, indices int32, values float32); returns (CSRArrays of
+    the copies, ('csr', indptr, indices, values, n_rows, n_cols) with a descriptor per array)."""
+    arrays, descs = [], []
+    for name, a, dt in (("indptr", c.indptr, np.int64), ("indices", c.indices, np.int32), ("values", c.values, np.float32)):
+        ref, desc = _shared_copy(a, tag + "_" + name, dt)
+        arrays.append(ref)
+        descs.append(desc)
+    return CSRArrays(*arrays, c.shape), ("csr",) + tuple(descs) + c.shape
 
 
 def _column_or_array(frame: LoadedFrame, spec, exclude: set):
@@ -401,6 +430,8 @@ class RayDMatrix:
                 total += sum(len(b) for b in blocks)
             self.n = total if rank is None else self.n
             self.sharding = RayShardingMode.FIXED
+        elif self.data_source is Sparse:
+            self._load_sparse(W)
         else:
             n_src = self.data_source.get_n(self.data)
             if W > n_src and self.data_source.needs_partitions:
@@ -467,6 +498,60 @@ class RayDMatrix:
             self._row_index.append(rows)
         self.n = n
 
+    def _load_sparse(self, W: int):
+        """Central loading of a scipy.sparse matrix: the canonical CSR is sharded by rows (INTERLEAVED / BATCH as for
+        dense data, whole query groups with qid) and every shard travels as three /dev/shm files; it is never
+        densified.  The side columns must be arrays (the matrix has no named columns), the features are f0, f1, ..."""
+        c = self.data_source.load_data(self.data, ignore=self.ignore)
+        n = c.shape[0]
+        if W > n:
+            raise RuntimeError(f"Trying to shard data for {W} actors, but the maximum number of shards "
+                               f"(i.e. the number of data rows) is {n}. Consider using fewer actors.")
+        side = {}
+        for name in ("label", "weight", "base_margin", "label_lower_bound", "label_upper_bound", "qid"):
+            spec = getattr(self, name)
+            if isinstance(spec, str) or (isinstance(spec, (list, tuple)) and spec and all(isinstance(x, str) for x in spec)):
+                raise ValueError(f"`{name}` names the column(s) {spec!r}, but a scipy.sparse matrix has no named columns."
+                                 f"\nFIX THIS by passing `{name}` as an array with one value per row.")
+            if name == "qid":
+                continue
+            side[name] = _column_or_array(None, spec, set())
+            if side[name] is not None and len(side[name]) != n:
+                raise ValueError(f"`{name}` has {len(side[name])} rows but the data has {n}")
+        fw = None if self.feature_weights is None else np.asarray(self.feature_weights, np.float32)
+        self._columns = ["f%d" % i for i in range(c.shape[1])]
+        tag = lambda r: "%x_%d_" % (self._uid & 0xffffffff, r)  # noqa: E731
+        if self.qid is not None:
+            q = np.asarray(self.qid.values if hasattr(self.qid, "values") and not isinstance(self.qid, np.ndarray)
+                           else self.qid).reshape(-1)
+            if len(q) != n:
+                raise ValueError(f"`qid` has {len(q)} rows but the data has {n}")
+            order = None if n < 2 or not np.any(q[1:] < q[:-1]) else np.argsort(q, kind="mergesort")
+            qs = q if order is None else q[order]
+            offsets = group_offsets(qs)
+            self._row_index = []
+            for r in range(W):
+                rows = group_sharding_rows(self.sharding, r, W, offsets)
+                src = rows if order is None else order[rows]
+                ref, shared = {"feature_weights": fw}, {"feature_weights": fw}
+                ref["data"], shared["data"] = _shared_csr(csr_take_rows(c, src), tag(r) + "data")
+                for name, a in side.items():
+                    ref[name], shared[name] = _shared_copy(None if a is None else a[src], tag(r) + name)
+                local = group_offsets(qs[rows])
+                gid = np.repeat(np.arange(len(local) - 1), np.diff(local)).astype(np.float32)
+                ref["qid"], shared["qid"] = _shared_copy(gid, tag(r) + "qid")
+                self.refs[r], self._shared[r] = ref, shared
+                self._row_index.append(rows)
+        else:
+            for r in range(W):
+                sl = _get_sharding_indices(self.sharding, r, W, n)
+                ref, shared = {"feature_weights": fw, "qid": None}, {"feature_weights": fw, "qid": None}
+                ref["data"], shared["data"] = _shared_csr(csr_take_rows(c, sl), tag(r) + "data")
+                for name, a in side.items():
+                    ref[name], shared[name] = _shared_copy(None if a is None else a[sl], tag(r) + name)
+                self.refs[r], self._shared[r] = ref, shared
+        self.n = n
+
     def get_data(self, rank: int, num_actors: Optional[int] = None) -> Dict[str, Optional[np.ndarray]]:
         self.load_data(num_actors=num_actors, rank=rank if (self.distributed and rank not in self.refs) else None)
         if rank not in self.refs:
@@ -488,13 +573,15 @@ class RayDMatrix:
     def unload_data(self):
         for sh in self._shared.values():
             for v in sh.values():
-                if isinstance(v, tuple) and len(v) == 2 and v[0] == "shm":
-                    with _SHM_LOCK:
-                        _SHM_FILES.discard(v[1])
-                    try:
-                        os.unlink(v[1])
-                    except OSError:
-                        pass
+                files = [v] if not (isinstance(v, tuple) and v and v[0] == "csr") else list(v[1:4])   # CSR: three files
+                for f in files:
+                    if isinstance(f, tuple) and len(f) == 2 and f[0] == "shm":
+                        with _SHM_LOCK:
+                            _SHM_FILES.discard(f[1])
+                        try:
+                            os.unlink(f[1])
+                        except OSError:
+                            pass
         self.refs, self._shared = {}, {}
         self._keep_alive = None
         self.loaded = False
