@@ -84,6 +84,11 @@ struct B2SplitCand {
   int32_t is_cat;        // categorical candidate: bin = category for a one-hot split, -1 for a partition split
   uint32_t cat_bits[8];  // categories that go right
 };
+// the candidate of a scan that found no split (cat_bits are not read)
+__device__ __forceinline__ void b2_no_candidate(B2SplitCand& c) {
+  c.loss_chg = 0.0f; c.feature = -1; c.bin = 0; c.default_left = 0; c.left_g = 0; c.left_h = 0;
+  c.order = 0xffffffffu; c.is_cat = 0;
+}
 
 struct B2EvalNode {
   int64_t sum_g, sum_h;  // node totals (fixed point)

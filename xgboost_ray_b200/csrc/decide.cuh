@@ -117,8 +117,8 @@ __device__ __forceinline__ void decide_block(DecideScratch<kThreads>& sm, const 
   for (int base = 0; base < n; base += kThreads) {
     const int i = base + threadIdx.x;
     const bool in = i < n;
-    B2SplitCand best; best.feature = -1; best.loss_chg = 0.f; best.order = 0xffffffffu; best.bin = 0; best.default_left = 0;
-    best.left_g = 0; best.left_h = 0; best.is_cat = 0;
+    B2SplitCand best;
+    b2_no_candidate(best);
     B2EvalNode nd; nd.sum_g = 0; nd.sum_h = 0; nd.hist_index = 0; nd.root_gain = 0.f;
     B2NodeSeg sg; sg.nid = 0; sg.begin = 0; sg.count = 0; sg.buf = 0;
     bool expand = false;
