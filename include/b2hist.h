@@ -27,6 +27,10 @@ typedef uint64_t B2Handle;
 const char* B2_GetLastError(void);
 int B2_GetVersion(void);
 int B2_DeviceCount(int* out);
+/* Check the params text of B2_BoosterCreate without a device: the same parsing and every rule about which parameters go
+ * together.  The rules that need the label width apply when the text gives num_target=<T>; what needs the train matrix
+ * itself (feature count, categorical features) does not.  A broken rule fails with B2_BoosterCreate's message. */
+int B2_CheckParams(const char* params);
 
 /* ---- communicator: replaces the Rabit bridge.
  * xgboost_ray/main.py:256-283 (_start_rabit_tracker -> rabit_args env) becomes B2_GetUniqueId on

@@ -68,7 +68,14 @@ def test_names_need_feature_names():
         E.interaction_sets([["a", "b"]], 6, None)
 
 
-def test_parameter_is_no_longer_rejected():
+@pytest.fixture(scope="module")
+def built():
+    """libb2hist.so: the engine checks the parameters (B2_CheckParams needs no device)."""
+    from xgboost_ray_b200 import build
+    return build.build()
+
+
+def test_parameter_is_no_longer_rejected(built):
     E._check_supported({"interaction_constraints": "[[0, 1], [2, 3, 4]]"})
     with pytest.raises(E.XGBoostError):     # its neighbours still are
         E._check_supported({"monotone_constraints": "(1,0)"})

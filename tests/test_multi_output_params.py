@@ -8,19 +8,26 @@ import pytest
 from xgboost_ray_b200 import engine
 
 
+@pytest.fixture(scope="module")
+def built():
+    """libb2hist.so: the engine checks the parameters (B2_CheckParams needs no device)."""
+    from xgboost_ray_b200 import build
+    return build.build()
+
+
 @pytest.mark.parametrize("params,match", [
     ({"multi_strategy": "bogus"}, "multi_strategy='bogus'"),
     ({"multi_strategy": "multi_output_tree", "objective": "multi:softprob"}, "multi_output_tree.*multi:softprob"),
     ({"multi_strategy": "multi_output_tree", "booster": "dart"}, "multi_output_tree.*dart"),
     ({"multi_strategy": "multi_output_tree", "num_parallel_tree": 3}, "multi_output_tree.*num_parallel_tree"),
 ])
-def test_refused(params, match):
+def test_refused(built, params, match):
     with pytest.raises(engine.XGBoostError, match=match):
         engine._check_supported(params)
 
 
 @pytest.mark.parametrize("ms", [None, "one_output_per_tree", "multi_output_tree"])
-def test_accepted(ms):
+def test_accepted(built, ms):
     engine._check_supported({"multi_strategy": ms, "objective": "binary:logistic"})
 
 

@@ -13,6 +13,13 @@ from xgboost_ray_b200 import engine as E
 F32 = np.float32
 
 
+@pytest.fixture(scope="module")
+def built():
+    """libb2hist.so: the engine checks the parameters (B2_CheckParams needs no device)."""
+    from xgboost_ray_b200 import build
+    return build.build()
+
+
 def test_unweighted_rule_by_hand():
     assert R.leaf_quantile([], 0.5) is None
     # n = 1: every alpha gives the single value
@@ -213,7 +220,7 @@ def test_quantile_alpha_error_names_the_value():
 @pytest.mark.parametrize("extra,match", [({"num_class": 3}, "num_class"), ({"booster": "dart"}, "dart"),
                                          ({"num_parallel_tree": 2}, "num_parallel_tree"),
                                          ({"quantile_alpha": 2.0}, "quantile_alpha")])
-def test_rejected_combinations(extra, match):
+def test_rejected_combinations(built, extra, match):
     params = dict({"objective": "reg:quantileerror"}, **extra)
     with pytest.raises(E.XGBoostError, match=match):
         E._check_supported(params)

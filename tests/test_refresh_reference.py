@@ -33,6 +33,13 @@ def data(n=4000, seed=0):
 PARAMS = {"eta": 0.3, "lambda": 1.0, "min_child_weight": 0.0}
 
 
+@pytest.fixture(scope="module")
+def built():
+    """libb2hist.so: the engine checks the parameters (B2_CheckParams needs no device)."""
+    from xgboost_ray_b200 import build
+    return build.build()
+
+
 def test_traversal_rules():
     t = hand_tree()
     X = np.array([[0.0, -1.0], [0.0, 1.0], [0.9, 0.0], [np.nan, 2.0]], F32)
@@ -95,20 +102,20 @@ def test_parallel_tree_scaling():
     ({"process_type": "update", "updater": "refresh", "refresh_leaf": 2}, "refresh_leaf"),
     ({"updater": "prune"}, "updater='prune'"),
 ])
-def test_parameter_checks(params, match):
+def test_parameter_checks(built, params, match):
     from xgboost_ray_b200 import engine
     with pytest.raises(engine.XGBoostError, match=match):
         engine._check_supported(params)
 
 
-def test_accepted_parameters():
+def test_accepted_parameters(built):
     from xgboost_ray_b200 import engine
     engine._check_supported({"process_type": "update", "updater": "refresh", "refresh_leaf": 0})
     engine._check_supported({"process_type": "default", "refresh_leaf": 1})
     engine._check_supported({"updater": "grow_gpu_hist"})
 
 
-def test_update_without_model_is_refused():
+def test_update_without_model_is_refused(built):
     from xgboost_ray_b200 import engine
     with pytest.raises(engine.XGBoostError, match="xgb_model"):
         engine.train({"process_type": "update", "updater": "refresh"}, None, 1)

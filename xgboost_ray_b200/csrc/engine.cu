@@ -43,6 +43,12 @@ extern "C" {
 
 const char* B2_GetLastError(void) { return g_last_error.c_str(); }
 int B2_GetVersion(void) { return 100; }
+int B2_CheckParams(const char* params) {
+  API_BEGIN
+  Params p;
+  parse_params(params, &p, nullptr);
+  API_END
+}
 int B2_DeviceCount(int* out) {
   API_BEGIN
   int n = 0;

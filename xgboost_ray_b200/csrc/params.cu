@@ -1,5 +1,6 @@
-// params.cu -- the booster parameters: parsing and checking the "key=value" text of B2_BoosterCreate, the objective
-// predicates, the host replicas of the leaf-weight formula, and the eval_metric names.
+// params.cu -- the booster parameters: parsing the "key=value" text of B2_BoosterCreate and B2_CheckParams with every
+// rule about which parameters go together, the objective predicates, the host replicas of the leaf-weight formula, and
+// the eval_metric names.
 #include <math.h>
 #include <stdlib.h>
 
@@ -81,13 +82,10 @@ void set_targets(Params* p, int T) {
     p->num_class = T;
   }
   p->num_target = T;
-  if (p->vector_leaf()) {   // DESIGN.md 2 item 19: what vector-leaf trees do not cover yet
+  if (p->vector_leaf()) {   // DESIGN.md 2 item 19: the vector-leaf rules that need the label width
     if (T > kMaxVectorTargets)
-      fail("multi_strategy=multi_output_tree supports at most %d targets, the label has %d columns", kMaxVectorTargets, T);
-    if (p->dart) fail("multi_strategy=multi_output_tree is not supported with booster=dart");
-    if (p->update_mode) fail("process_type=update is not supported with multi_strategy=multi_output_tree");
-    if (p->num_parallel_tree > 1)
-      fail("multi_strategy=multi_output_tree needs num_parallel_tree = 1, got %d", p->num_parallel_tree);
+      fail("multi_strategy='multi_output_tree' supports at most %d targets, the label has %d columns", kMaxVectorTargets, T);
+    if (p->update_mode) fail("process_type='update' is not supported with multi_strategy='multi_output_tree'");
   }
 }
 
@@ -195,9 +193,14 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     else if (k == "process_type") {
       if (v == "default") p->update_mode = false;
       else if (v == "update") p->update_mode = true;
-      else fail("process_type='%s' is not supported (supported: default, update)", v.c_str());
+      else fail("process_type='%s' is not supported (supported: 'default', 'update')", v.c_str());
     }
-    else if (k == "updater") p->updater = v;
+    else if (k == "updater") {
+      if (v != "refresh" && v != "grow_quantile_histmaker" && v != "grow_gpu_hist")
+        fail("updater='%s' is not supported (supported: grow_quantile_histmaker, grow_gpu_hist, and refresh with "
+             "process_type='update')", v.c_str());
+      p->updater = v;
+    }
     else if (k == "refresh_leaf") {
       if (v == "1" || v == "true" || v == "True") p->refresh_leaf = true;
       else if (v == "0" || v == "false" || v == "False") p->refresh_leaf = false;
@@ -230,30 +233,34 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     fail("%s has one output per row: num_class must be 1, got %d", p->objective_name.c_str(), p->num_class);
   if (p->objective == kObjQuantile) {
     // rules of this engine (DESIGN.md 2): the outputs are the alphas, the leaf refresh needs the plain gbtree round
-    if (p->num_class_set) fail("reg:quantileerror has one output per quantile_alpha: num_class must not be set");
-    if (p->dart) fail("reg:quantileerror is not supported with booster=dart");
-    if (p->num_parallel_tree > 1) fail("reg:quantileerror needs num_parallel_tree = 1, got %d", p->num_parallel_tree);
+    if (p->num_class_set)
+      fail("reg:quantileerror has one output per quantile_alpha: num_class must not be set (got %d)", p->num_class);
+    if (p->dart) fail("reg:quantileerror is not supported with booster='dart'");
+    if (p->num_parallel_tree > 1) fail("reg:quantileerror needs num_parallel_tree = 1 (got %d)", p->num_parallel_tree);
     p->num_class = (int)p->quantile_alpha.size();
   } else if (p->objective != kObjSoftprob) p->num_class = 1;
+  // vector-leaf trees (DESIGN.md 2 item 19): what they do not cover yet, refused for any number of targets
+  if (p->multi_strategy == 1) {
+    if (p->objective == kObjSoftprob)
+      fail("multi_strategy='multi_output_tree' is not supported with objective='%s': vector-leaf trees take the "
+           "multi-target objectives (reg:squarederror, reg:squaredlogerror, reg:pseudohubererror, reg:logistic, "
+           "binary:logistic, binary:logitraw)", p->objective_name.c_str());
+    if (p->dart) fail("multi_strategy='multi_output_tree' is not supported with booster='dart'");
+    if (p->num_parallel_tree > 1)
+      fail("multi_strategy='multi_output_tree' needs num_parallel_tree = 1 (got %d)", p->num_parallel_tree);
+  }
   if (p->objective == kObjSoftprob && p->num_class < 2) fail("multi:softprob needs num_class >= 2");
-  if (p->multi_strategy == 1 && p->objective == kObjSoftprob)
-    fail("multi_strategy=multi_output_tree is not supported with objective '%s' (vector-leaf trees take the multi-target "
-         "objectives: reg:squarederror, reg:squaredlogerror, reg:pseudohubererror, reg:logistic, binary:logistic, "
-         "binary:logitraw)", p->objective_name.c_str());
   // update mode (DESIGN.md 2 item 20): only the refresh updater, and only where a refreshed leaf is a Newton step
   if (p->update_mode) {
     if (p->updater != "refresh")
-      fail("process_type=update needs updater=refresh, got updater='%s' (prune and refresh,prune are not supported)",
-           p->updater.c_str());
-    if (p->dart) fail("process_type=update is not supported with booster=dart");
+      fail("process_type='update' needs updater='refresh', got updater='%s' (updater='prune' and 'refresh,prune' are "
+           "not supported)", p->updater.c_str());
+    if (p->dart) fail("process_type='update' is not supported with booster='dart'");
     if (p->objective == kObjQuantile)
-      fail("process_type=update is not supported with reg:quantileerror: its leaf values are residual quantiles, which the "
-           "refresh updater does not recompute");
+      fail("process_type='update' is not supported with objective='reg:quantileerror': its leaf values are residual "
+           "quantiles, which the refresh updater does not recompute");
   } else if (p->updater == "refresh") {
-    fail("updater=refresh needs process_type=update: it refreshes the trees of an existing model (xgb_model)");
-  } else if (!p->updater.empty() && p->updater != "grow_quantile_histmaker" && p->updater != "grow_gpu_hist") {
-    fail("updater='%s' is not supported (supported: grow_quantile_histmaker, grow_gpu_hist, and refresh with "
-         "process_type=update)", p->updater.c_str());
+    fail("updater='refresh' needs process_type='update': it refreshes the trees of an existing model (xgb_model)");
   }
   if (p->num_target_set) set_targets(p, p->num_target);
   // 16: a leaf index must fit the uint16_t row -> leaf map pos (2^16 leaves), DESIGN.md 9

@@ -43,6 +43,7 @@ _FLT_MAX = np.finfo(np.float32).max
 ABI = {
     "B2_GetLastError": (C.c_char_p, []),
     "B2_GetVersion": (C.c_int, []),
+    "B2_CheckParams": (C.c_int, [C.c_char_p]),
     "B2_DeviceCount": (C.c_int, [C.POINTER(C.c_int)]),
     "B2_GetUniqueId": (C.c_int, [_BP]),
     "B2_CommCreate": (C.c_int, [_BP, C.c_int, C.c_int, C.c_int, C.POINTER(_H)]),
@@ -762,17 +763,15 @@ _ENGINE_KEYS = ("objective", "num_class", "max_depth", "eta", "learning_rate", "
                 "lambdarank_unbiased", "ndcg_exp_gain", "booster", "rate_drop", "skip_drop", "sample_type",
                 "normalize_type", "one_drop", "quantile_alpha", "num_target", "multi_strategy", "process_type",
                 "updater", "refresh_leaf")
-# multi_strategy: one tree per target and round (xgboost's default), or one vector-leaf tree per round (DESIGN.md 2 item 19)
-_MULTI_STRATEGIES = ("one_output_per_tree", "multi_output_tree")
 # booster=dart's parameters with xgboost's defaults (save_config's dart_train_param)
 _DART_DEFAULTS = {"rate_drop": 0.0, "skip_drop": 0.0, "sample_type": "uniform", "normalize_type": "tree", "one_drop": 0}
 
-# xgboost parameters that change the trained model and that this engine does not implement: a value different
-# from the neutral one is an error, never silently ignored (a drop-in must not train a different model quietly)
+# xgboost parameters that change the trained model and that this engine does not implement (its parameter parser
+# ignores them as unknown keys): a value different from the neutral one is an error, never silently ignored (a drop-in
+# must not train a different model quietly)
 _UNSUPPORTED_NEUTRAL = {
     "sampling_method": ("uniform",), "max_leaves": (0,), "grow_policy": ("depthwise",),
     "monotone_constraints": (None, "", "()", (), []),
-    "updater": (None, "grow_quantile_histmaker", "grow_gpu_hist"),   # and "refresh" in update mode (_check_update)
 }
 
 
@@ -781,73 +780,19 @@ def is_update_mode(params):
     return (params.get("process_type") or "default") == "update"
 
 
-def _check_update(params):
-    """Update mode (DESIGN.md 2 item 20) takes updater='refresh' and nothing else; updater='refresh' needs update mode.
-    DART, vector-leaf trees and reg:quantileerror are refused, naming the parameter."""
-    pt = params.get("process_type") or "default"
-    if pt not in ("default", "update"):
-        raise XGBoostError("process_type=%r is not supported (supported: 'default', 'update')" % (pt,))
-    rl = params.get("refresh_leaf")
-    if rl is not None and rl not in (0, 1, True, False, "0", "1", "true", "false", "True", "False"):
-        raise XGBoostError("refresh_leaf must be 0 or 1, got %r" % (rl,))
-    updater = params.get("updater")
-    if pt != "update":
-        if updater == "refresh":
-            raise XGBoostError("updater='refresh' needs process_type='update': it refreshes the trees of an existing "
-                               "model (xgb_model)")
-        return
-    if updater != "refresh":
-        raise XGBoostError("process_type='update' needs updater='refresh', got updater=%r (updater='prune' and "
-                           "'refresh,prune' are not supported)" % (updater,))
-    if (params.get("booster") or "gbtree") == "dart":
-        raise XGBoostError("process_type='update' is not supported with booster='dart'")
-    if params.get("multi_strategy") == "multi_output_tree" and int(params.get("num_target", 1) or 1) > 1:
-        raise XGBoostError("process_type='update' is not supported with multi_strategy='multi_output_tree'")
-    if params.get("objective") == "reg:quantileerror":
-        raise XGBoostError("process_type='update' is not supported with objective='reg:quantileerror': its leaf values "
-                           "are residual quantiles, which the refresh updater does not recompute")
+def _engine_text(params, extra=None):
+    """The params text of B2_BoosterCreate / B2_CheckParams: the engine's keys of `params` (None: not given), then
+    `extra`.  quantile_alpha goes as "a,b,c" with each float32 alpha written exactly."""
+    p = {k: params[k] for k in _ENGINE_KEYS if params.get(k) is not None}
+    if "quantile_alpha" in p:
+        p["quantile_alpha"] = ",".join(repr(float(a)) for a in quantile_alphas(p["quantile_alpha"]))
+    if extra:
+        p.update(extra)
+    return "\n".join("%s=%s" % (k, v) for k, v in p.items()).encode()
 
 
-def _check_quantile(params):
-    """reg:quantileerror grows one tree per alpha and round on the gbtree path: its outputs are the alphas, so num_class
-    is refused, and so are DART and random forests (num_parallel_tree > 1), whose trees the leaf refresh does not cover."""
-    if params.get("objective") != "reg:quantileerror":
-        return
-    quantile_alphas(params.get("quantile_alpha"))
-    if params.get("num_class") is not None:
-        raise XGBoostError("reg:quantileerror has one output per quantile_alpha: num_class must not be set (got %r)"
-                           % (params["num_class"],))
-    if (params.get("booster") or "gbtree") == "dart":
-        raise XGBoostError("reg:quantileerror is not supported with booster='dart'")
-    if int(params.get("num_parallel_tree", 1) or 1) > 1:
-        raise XGBoostError("reg:quantileerror needs num_parallel_tree = 1 (got %r)" % (params["num_parallel_tree"],))
-
-
-def _check_multi_strategy(params):
-    """multi_strategy names one of the two strategies; vector-leaf trees refuse what they do not cover yet, naming both
-    sides (the engine checks the label width, categorical features and the communicator)."""
-    ms = params.get("multi_strategy")
-    if ms is None:
-        return
-    if ms not in _MULTI_STRATEGIES:
-        raise XGBoostError("multi_strategy=%r is not supported (supported: %s)" % (ms, ", ".join(_MULTI_STRATEGIES)))
-    if ms != "multi_output_tree":
-        return
-    obj = params.get("objective") or "reg:squarederror"
-    if obj.startswith("multi:"):
-        raise XGBoostError("multi_strategy='multi_output_tree' is not supported with objective=%r: vector-leaf trees take "
-                           "the multi-target objectives" % (obj,))
-    if (params.get("booster") or "gbtree") == "dart":
-        raise XGBoostError("multi_strategy='multi_output_tree' is not supported with booster='dart'")
-    if int(params.get("num_parallel_tree", 1) or 1) > 1:
-        raise XGBoostError("multi_strategy='multi_output_tree' needs num_parallel_tree = 1 (got %r)"
-                           % (params["num_parallel_tree"],))
-
-
-def _check_supported(params):
-    _check_quantile(params)
-    _check_multi_strategy(params)
-    _check_update(params)
+def _check_python_forms(params):
+    """The checks only Python can make: max_bin's range, and the keys the engine ignores, in their Python forms."""
     mb = params.get("max_bin")
     if mb is not None and not 2 <= int(mb) <= 256:
         raise XGBoostError("parameter max_bin=%r is not supported by the H100 hist engine: the bin matrix is uint8, "
@@ -859,11 +804,15 @@ def _check_supported(params):
                 continue
             if isinstance(v, str) and k == "monotone_constraints" and set(v) <= set("(), 0"):
                 continue
-            if k == "updater" and v == "refresh":   # checked by _check_update
-                continue
             if v not in neutral:
                 raise XGBoostError("parameter %s=%r is not supported by the H100 hist engine (supported: %s)"
                                    % (k, v, ", ".join(repr(x) for x in neutral[:4])))
+
+
+def _check_supported(params):
+    """Every parameter rule, without a device: the Python-only checks, then the engine's (params.cu) on its text."""
+    _check_python_forms(params)
+    _check(lib().B2_CheckParams(_engine_text(params)))
 
 
 def interaction_sets(value, n_features, feature_names=None):
@@ -906,11 +855,7 @@ def interaction_sets(value, n_features, feature_names=None):
 
 
 def _params_dict(params):
-    if params is None:
-        return {}
-    if isinstance(params, (list, tuple)):
-        return dict(params)
-    return dict(params)
+    return {} if params is None else dict(params)
 
 
 class Booster:
@@ -941,13 +886,9 @@ class Booster:
 
     # -- engine object management
     def _param_text(self, extra=None):
-        _check_supported(self.params)
-        p = {k: self.params[k] for k in _ENGINE_KEYS if k in self.params and self.params[k] is not None}
-        if "quantile_alpha" in p:   # the engine takes "a,b,c" with each float32 alpha written exactly
-            p["quantile_alpha"] = ",".join(repr(float(a)) for a in quantile_alphas(p["quantile_alpha"]))
-        if extra:
-            p.update(extra)
-        return "\n".join("%s=%s" % (k, v) for k, v in p.items()).encode()
+        """The text B2_BoosterCreate parses, which applies the engine's parameter rules itself."""
+        _check_python_forms(self.params)
+        return _engine_text(self.params, extra)
 
     def _interaction_sets(self, n_features=None, feature_names=None):
         return interaction_sets(self.params.get("interaction_constraints"),
@@ -1239,12 +1180,8 @@ class Booster:
                 out = _transform(self.params.get("objective", "reg:squarederror"), out.reshape(n, K)).reshape(-1)
         else:
             data._ensure_raw()
-            tb, te = iteration_range if iteration_range else (0, 0)
-            tb_t, te_trees = tb * self._trees_per_round, te * self._trees_per_round
-            if ntree_limit:
-                tb_t, te_trees = 0, ntree_limit
-            _check(lib().B2_BoosterPredict(self.handle, data.handle, 1 if output_margin else 0, tb_t, te_trees,
-                                           _fp(out), out.size))
+            tb, te = self._tree_range(iteration_range, ntree_limit)
+            _check(lib().B2_BoosterPredict(self.handle, data.handle, 1 if output_margin else 0, tb, te, _fp(out), out.size))
         if K == 1:
             return out
         out = out.reshape(n, K)
@@ -1488,7 +1425,6 @@ class Booster:
             sb = t.get("split_bins") if split_bins is None else split_bins[ti]
             cat_split = (st != 0) & ~leaf
             # a categorical node: one-hot splits keep their category as the condition, set splits have none (NaN)
-            ncat = np.array([bin(int(w)).count("1") for w in bits.reshape(len(left), -1).astype(np.uint64).sum(axis=1)]) if False else None
             cond = np.where(leaf, 0, sc).astype(np.float32)
             for nid in np.nonzero(cat_split)[0]:
                 cl = _cat_list(bits[nid])
@@ -1746,7 +1682,7 @@ def train(params, dtrain, num_boost_round=10, evals=(), obj=None, feval=None, ma
     bst = Booster(params)
     update = is_update_mode(params)
     if update:
-        _check_update(params)
+        _check_supported(params)
         if xgb_model is None:
             raise XGBoostError("process_type='update' refreshes the trees of an existing model: pass it as xgb_model")
     if xgb_model is not None:
@@ -1787,9 +1723,10 @@ def train(params, dtrain, num_boost_round=10, evals=(), obj=None, feval=None, ma
         if update:
             # the trees keep their shape and their intercept: num_parallel_tree and base_score are the model's own
             if src.is_vector_leaf:
-                raise XGBoostError("process_type='update' is not supported with multi_strategy='multi_output_tree'")
+                raise XGBoostError("process_type='update' is not supported for a multi_strategy='multi_output_tree' "
+                                   "model")
             if src.is_dart:
-                raise XGBoostError("process_type='update' is not supported with booster='dart'")
+                raise XGBoostError("process_type='update' is not supported for a booster='dart' model")
             if src.params.get("base_score") is None:
                 raise XGBoostError("process_type='update': the model passed as xgb_model carries no base_score")
             if src.params.get("objective") == "reg:quantileerror":
@@ -1813,9 +1750,6 @@ def train(params, dtrain, num_boost_round=10, evals=(), obj=None, feval=None, ma
             bst._trees = bst._trees[:num_boost_round * per_round]
     bst._attach(dtrain)
     evals = list(evals or [])
-    for dm, _ in evals:
-        if dm is not dtrain and dm.ref is None and not dm._quantized:
-            pass  # evaluation matrices are traversed on raw floats; no quantisation needed
     evals_log = {}
     for cb in callbacks:
         r = cb.before_training(bst)
