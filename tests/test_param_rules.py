@@ -33,6 +33,11 @@ REFUSED = [
     (dict(UPD, num_target=3, **VEC), "process_type='update' is not supported with multi_strategy='multi_output_tree'"),
     # parse_params: one value at a time
     ({"objective": "reg:absoluteerror"}, "unsupported objective 'reg:absoluteerror'"),
+    ({"objective": "survival:cox"},
+     "^" + re.escape("unsupported objective 'survival:cox' (supported: reg:squarederror, reg:logistic, binary:logistic, "
+                     "binary:logitraw, reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie, "
+                     "survival:aft, rank:pairwise, rank:ndcg, rank:map, reg:quantileerror, multi:softprob, "
+                     "multi:softmax)") + "$"),
     ({"aft_loss_distribution": "cauchy"}, "aft_loss_distribution must be normal, logistic or extreme, got 'cauchy'"),
     ({"lambdarank_pair_method": "mean"}, "lambdarank_pair_method='mean' is not supported"),
     ({"lambdarank_num_pair_per_sample": 0}, "lambdarank_num_pair_per_sample must be an integer >= 1, got '0'"),
@@ -113,6 +118,11 @@ def test_refusal_of_engine_text(built, text, match):
     dict(UPD, refresh_leaf="false"), {"updater": "grow_quantile_histmaker"}, {"booster": "dart", "rate_drop": 0.1},
     {"objective": "reg:quantileerror", "quantile_alpha": [0.1, 0.9]}, {"objective": "rank:map"},
     {"booster": "gbtree", "sample_type": "x"},   # DART's parameters are ignored by gbtree, like xgboost
+    # every other accepted objective name
+    *({"objective": o} for o in ("reg:squarederror", "reg:linear", "reg:logistic", "binary:logistic", "binary:logitraw",
+                                 "reg:squaredlogerror", "reg:pseudohubererror", "count:poisson", "reg:gamma",
+                                 "reg:tweedie", "survival:aft", "rank:pairwise", "rank:ndcg")),
+    {"objective": "multi:softmax", "num_class": 3},
 ])
 def test_accepted(built, params):
     E._check_supported(params)

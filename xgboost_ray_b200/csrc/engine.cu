@@ -605,124 +605,7 @@ int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out)
   drain_round(b);
   Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
-  cudaStream_t s = b->ctx->stream;
-  float mparam = 0.0f;
-  int minus = 0;
-  const B2Metric mid = metric_id(metric, b->p, &mparam, &minus);
-  const bool aft_metric = mid == kMetricAftNloglik || mid == kMetricIntervalAccuracy;
-  if (mid >= kMetricNdcg && mid <= kMetricPre) {
-    // ndcg / map / pre: per query group on the prediction order (rank_kernel.cu), averaged over the groups of all workers
-    if (b->p.num_class > 1) fail("metric '%s' needs a single-output objective", metric);
-    if (!m->has_qgroups()) fail("metric '%s' needs query groups (qid) on the evaluation matrix", metric);
-    if (m->n_label != m->n) fail("evaluation matrix has no labels");
-    float* margin = eval_margin(b, m);
-    DevBuf<float> pred; DevBuf<double> vals; RankOrder po, lo;
-    pred.ensure((size_t)std::max<int64_t>(m->n, 1));
-    if (m->n > 0) CUDA_CHECK(cudaMemcpyAsync(pred.p, margin, (size_t)m->n * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    LAUNCH_CHECK(b2_launch_transform(b->p.objective, 1, pred.p, m->n, b->ctx->num_sms, s));
-    po.run(m, pred.p, b->ctx->num_sms, s);
-    if (mid == kMetricNdcg) lo.run(m, m->label.p, b->ctx->num_sms, s);
-    ensure_rank_disc(b, m->max_qgroup);
-    vals.ensure((size_t)std::max<int64_t>(m->n_qgroups, 1));
-    b->d_metric.ensure(2);
-    LAUNCH_CHECK(b2_launch_rank_metric(mid, (int)mparam, minus, b->p.ndcg_exp_gain ? 1 : 0, m->qgroup_ptr.p, m->n_qgroups,
-                                       po.rows.p, m->label.p, mid == kMetricNdcg ? lo.keys_sorted.p : nullptr, b->rank_disc.p,
-                                       vals.p, b->d_metric.p, b->ctx->num_sms, s));
-    const std::vector<double> h = metric_sums(b, 2, s);
-    *out = h[1] > 0 ? h[0] / h[1] : 0.0;
-    return 0;
-  }
-  const bool auc_metric = mid == kMetricAuc || mid == kMetricAucPr;
-  // xgboost computes a per-group ranking AUC on a matrix with groups; this engine's auc / aucpr are binary or
-  // one-vs-rest only
-  if (auc_metric && m->has_qgroups())
-    fail("metric '%s' on a matrix with query groups (per-group ranking AUC) is not supported; use ndcg or map", metric);
-  if (auc_metric && b->p.num_target > 1)
-    fail("metric '%s' is not supported for a multi-target model (%d targets); use rmse, mae, logloss or error", metric,
-         b->p.num_target);
-  if (auc_metric && b->p.num_class > 1 && b->p.objective != kObjSoftprob)
-    fail("metric '%s' needs one output per row or a multi:softprob / multi:softmax model; objective '%s' has %d outputs",
-         metric, b->p.objective_name.c_str(), b->p.num_class);
-  if (aft_metric && b->p.objective != kObjAft)
-    fail("metric '%s' does not fit objective '%s'", metric, b->p.objective_name.c_str());
-  if (aft_metric && !m->has_bounds()) fail("metric '%s' needs label_lower_bound and label_upper_bound on the evaluation matrix", metric);
-  if (!aft_metric && m->n_label > 0 && m->n_targets != b->p.num_target)
-    fail("metric '%s': the evaluation matrix's label has %d columns, the model has %d targets", metric, m->n_targets,
-         b->p.num_target);
-  if (!aft_metric && !m->has_labels(b->p.num_target)) fail("evaluation matrix has no labels");
-  float* margin = eval_margin(b, m);
-  if (auc_metric) {
-    // ROC / PR AUC on the transformed prediction (auc_kernel.cu; DESIGN.md §2 item 17): per class a worker's triple
-    // (ROC: area, fp*tp, tp; PR: aucpr, 1, 1) plus the count of out-of-range labels, summed over the workers
-    const int K = b->p.num_class;
-    DevBuf<float> pred; DevBuf<uint8_t> tmp;
-    pred.ensure((size_t)std::max<int64_t>(m->n * K, 1));
-    if (m->n > 0) CUDA_CHECK(cudaMemcpyAsync(pred.p, margin, (size_t)(m->n * K) * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    LAUNCH_CHECK(b2_launch_transform(b->p.objective, K, pred.p, m->n, b->ctx->num_sms, s));
-    const size_t tb = b2_auc_temp_bytes(m->n);
-    tmp.ensure(tb);
-    b->d_metric.ensure(3 * (size_t)K + 1);
-    LAUNCH_CHECK(b2_auc(mid == kMetricAucPr ? 1 : 0, K, pred.p, m->label.p, m->n_weight ? m->weight.p : nullptr, m->n,
-                        tmp.p, tb, b->d_metric.p, b->ctx->num_sms, s));
-    const std::vector<double> h = metric_sums(b, 3 * (size_t)K + 1, s);
-    if (h[3 * (size_t)K] > 0)
-      fail("metric '%s': label must be in [0, num_class), num_class = %d (%.0f rows outside)", metric, K, h[3 * (size_t)K]);
-    if (K == 1) {
-      // ROC with only one class present: xgboost reports 0.5
-      *out = mid == kMetricAuc ? (h[1] > 0 ? h[0] / h[1] : 0.5) : h[0] / h[1];
-      return 0;
-    }
-    // one-vs-rest: sum_c (A_c / L_c) T_c / sum_c T_c; NaN when some class has L_c = 0 or no class has T_c
-    double num = 0.0, den = 0.0;
-    bool defined = true;
-    for (int c = 0; c < K; ++c) {
-      const double A = h[3 * c], L = h[3 * c + 1], T = h[3 * c + 2];
-      if (!(L > 0)) { defined = false; break; }
-      num += A / L * T; den += T;
-    }
-    *out = defined && den > 0 ? num / den : NAN;
-    return 0;
-  }
-  b->d_metric.ensure(3);
-  CUDA_CHECK(cudaMemsetAsync(b->d_metric.p, 0, 3 * sizeof(double), s));
-  if ((mid == kMetricMlogloss || mid == kMetricMerror) != (b->p.objective == kObjSoftprob))
-    fail("metric '%s' does not fit objective '%s'", metric, b->p.objective_name.c_str());
-  if (aft_metric) {
-    LAUNCH_CHECK(b2_launch_aft_metric(b->p.aft_dist, mid, (double)b->p.aft_sigma, margin, m->lower.p, m->upper.p,
-                                      m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p, b->ctx->num_sms, s));
-    const std::vector<double> h = metric_sums(b, 2, s);
-    *out = h[1] > 0 ? h[0] / h[1] : 0.0;
-    return 0;
-  }
-  if (mid == kMetricQuantile) {
-    // pinball loss averaged over the rows and the alphas, weighted (sum, K * sum w summed over the workers)
-    if (b->p.objective != kObjQuantile) fail("metric 'quantile' needs objective reg:quantileerror (it reads quantile_alpha)");
-    if (!b->d_alpha.p || b->d_alpha.cap < b->p.quantile_alpha.size()) {
-      upload(b->d_alpha, b->p.quantile_alpha, s);
-      CUDA_CHECK(cudaStreamSynchronize(s));
-    }
-    LAUNCH_CHECK(b2_launch_quantile_metric(b->p.num_class, b->d_alpha.p, margin, m->label.p, m->n_weight ? m->weight.p : nullptr,
-                                           m->n, b->d_metric.p, b->ctx->num_sms, s));
-    const std::vector<double> h = metric_sums(b, 2, s);
-    *out = h[1] > 0 ? h[0] / h[1] : 0.0;
-    return 0;
-  }
-  if (b->p.num_target > 1) {
-    // elementwise over the n x T outputs, each with its row's weight (xgboost's EvalEWiseBase)
-    if (!(mid <= kMetricError || mid == kMetricMae || (mid >= kMetricRmsle && mid <= kMetricMphe)))
-      fail("metric '%s' is not supported for a multi-target model (supported: rmse, rmsle, mae, mape, mphe, logloss, error)",
-           metric);
-    LAUNCH_CHECK(b2_launch_metric_multi_target(b->p.objective, mid, b->p.num_target, mparam, margin, m->label.p,
-                                               m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p, b->ctx->num_sms, s));
-  } else
-    LAUNCH_CHECK(b2_launch_metric(b->p.objective, mid, b->p.num_class, mparam, margin, m->label.p, m->n_weight ? m->weight.p : nullptr, m->n, b->d_metric.p,
-                                  b->ctx->num_sms, s));
-  // (sum, wsum, rows with a label outside [0, num_class)): the count travels with the sums, so every rank fails together
-  const std::vector<double> h = metric_sums(b, 3, s);
-  if (h[2] > 0)
-    fail("metric '%s': label must be in [0, num_class), num_class = %d (%.0f rows outside)", metric, b->p.num_class, h[2]);
-  double v = h[1] > 0 ? h[0] / h[1] : 0.0;
-  *out = (mid == kMetricRmse || mid == kMetricRmsle) ? sqrt(v) : v;
+  *out = eval_metric(b, m, metric);
   API_END
 }
 int B2_BoosterPredict(B2Handle bh, B2Handle mh, int32_t output_margin, int32_t tree_begin, int32_t tree_end, float* out,

@@ -9,10 +9,10 @@
 //
 // device.cu   device context, memory pool, pinned upload pipeline, NCCL
 // matrix.cu   matrix registry, cuts, binning
-// params.cu   parameter parsing, objective predicates, metric names
+// params.cu   parameter parsing, the objective table (kObjectives), metric names
 // tree.cu     growing one tree (scalar or vector-leaf) and reading it back
-// round.cu    a boosting round: gradients, base_score, DART, refresh, the round pipeline
-// predict.cu  TreeSHAP paths, prediction and evaluation margins
+// round.cu    a boosting round: label checks, gradients, base_score, DART, refresh, the round pipeline
+// predict.cu  TreeSHAP paths, prediction, evaluation margins and eval metrics
 // engine.cu   the C ABI (include/b2hist.h)
 //
 // Everything is in namespace b2host, and every file opens it with hidden visibility, so the library exports no symbol
@@ -246,14 +246,10 @@ void make_cuts(Matrix* m, Comm* comm, int max_bin);
 void bin_matrix(Matrix* m);
 
 // ---------------------------------------------------------------- booster
-bool obj_log_link(int o);
-bool obj_sigmoid(int o);
-bool obj_rank(int o);
-bool obj_checks_finite(int o);
-
 constexpr int kMaxTargets = 4096;   // label columns of one matrix (as many trees per round as num_parallel_tree allows)
 struct Params {
   int objective = kObjSquaredError;
+  int objective_index = 0;   // its row of params.cu kObjectives (objective_row)
   std::string objective_name = "reg:squarederror";
   int num_class = 1;
   // label columns of a multi-target model (outputs per row; num_class then equals it).  Given as num_target when a model
@@ -302,6 +298,28 @@ struct Params {
   bool use_cols() const { return colsample_bytree < 1.0f || colsample_bylevel < 1.0f || colsample_bynode < 1.0f; }
   bool vector_leaf() const { return multi_strategy == 1 && num_target > 1; }
 };
+
+// What an objective is on the host: one row of params.cu kObjectives per accepted name (DESIGN.md 4.4)
+enum ObjLink { kLinkIdentity, kLinkSigmoid, kLinkExp, kLinkSoftmax };
+enum ObjGrad { kGradScalar, kGradSoftprob, kGradAft, kGradRank, kGradQuantile };
+enum ObjLabels { kLabelsAny, kLabelsDomain, kLabelsBounds, kLabelsRank };
+enum ObjIntercept { kInterceptStump, kInterceptQuantile, kInterceptFixed, kInterceptNone };
+struct Objective {
+  const char* name;
+  B2Objective id;
+  ObjLink link;
+  ObjGrad grad;
+  float Params::*param;   // the gradient kernel's parameter, nullptr: none
+  bool multi_target, checks_finite;
+  ObjLabels labels;
+  ObjIntercept intercept;
+  const char* label_rule = nullptr;   // kLabelsDomain: fail() format taking the objective's name and num_class
+};
+const Objective& objective_row(const Params& p);
+
+// An eval_metric name (params.cu kMetrics); the family picks eval_metric's rules, launch and finish
+enum MetricFamily { kEvalElementwise, kEvalClass, kEvalAuc, kEvalAft, kEvalQuantile, kEvalRank };
+struct Metric { const char* name; B2Metric id; MetricFamily family; bool multi_target; };
 
 struct TreeHost {
   std::vector<int32_t> left, right, parent, feature, split_bin;
@@ -549,10 +567,9 @@ struct Booster : HandleBase {
 // ---------------------------------------------------------------- params.cu
 void set_targets(Params* p, int T);
 void parse_params(const char* text, Params* p, int* max_bin_out);
-float objective_param(const Params& p);
 float base_margin_value(const Params& p);
 float h_calc_weight(const Params& p, double G, double H);
-B2Metric metric_id(const char* name, const Params& p, float* param, int* minus);
+const Metric& metric_id(const char* name, const Params& p, float* param, int* minus);
 
 // ---------------------------------------------------------------- tree.cu
 void check_level_memory(const Booster* b);
@@ -580,6 +597,6 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
 void build_paths(Booster* b);
 void predict_trees(Booster* b, Matrix* m, int tree_begin, int tree_end, float* out);
 float* eval_margin(Booster* b, Matrix* m);
-std::vector<double> metric_sums(Booster* b, size_t n, cudaStream_t s);
+double eval_metric(Booster* b, Matrix* m, const char* name);
 
 }  // namespace b2host

@@ -1,24 +1,45 @@
 // params.cu -- the booster parameters: parsing the "key=value" text of B2_BoosterCreate and B2_CheckParams with every
-// rule about which parameters go together, the objective predicates, the host replicas of the leaf-weight formula, and
-// the eval_metric names.
+// rule about which parameters go together, the objective table, the host replicas of the leaf-weight formula, and the
+// eval_metric names.
 #include <math.h>
 #include <stdlib.h>
+#include <string.h>
 
 #include "host.h"
 
 namespace b2host __attribute__((visibility("hidden"))) {
 
-bool obj_log_link(int o) { return o == kObjPoisson || o == kObjGamma || o == kObjTweedie || o == kObjAft; }
-bool obj_sigmoid(int o) { return o == kObjLogistic || o == kObjRegLogistic; }
-bool obj_rank(int o) { return o == kObjRankPairwise || o == kObjRankNdcg || o == kObjRankMap; }
-// objectives whose gradient kernel reports non-finite gradient pairs (gradient_param_kernel).  reg:quantileerror's
-// pairs are finite for finite labels and weights (both checked before the first round), so its rounds stay pipelined.
-bool obj_checks_finite(int o) { return o >= kObjSquaredLog && o != kObjQuantile; }
-// objectives that take a label of T > 1 columns (xgboost's RegLossObj family and pseudo-Huber, which read labels.Shape(1))
-bool obj_multi_target(int o) {
-  return o == kObjSquaredError || o == kObjLogistic || o == kObjRegLogistic || o == kObjLogitRaw || o == kObjSquaredLog ||
-         o == kObjPseudoHuber;
-}
+// the label_rule messages; a class label is an index (non-integer labels truncate like xgboost's, NaN is rejected)
+constexpr char kIn01[] = "label must be in [0, 1] for %s", kNonneg[] = "label must be nonnegative for %s",
+               kAboveMinus1[] = "label must be greater than -1 for %s", kPositive[] = "label must be positive for %s",
+               kFinite[] = "label must be finite for %s",
+               kClassIndex[] = "label must be in [0, num_class) for %s, num_class = %d";
+
+// Every accepted objective name.  reg:quantileerror's gradient pairs are finite for finite labels and weights (both
+// checked before the first round), so its rounds stay pipelined.
+constexpr Objective kObjectives[] = {
+  // name, id, link, grad, param, multi_target, checks_finite, labels, intercept[, label_rule]
+  {"reg:squarederror", kObjSquaredError, kLinkIdentity, kGradScalar, nullptr, true, false, kLabelsAny, kInterceptStump},
+  {"reg:linear", kObjSquaredError, kLinkIdentity, kGradScalar, nullptr, true, false, kLabelsAny, kInterceptStump},
+  {"reg:logistic", kObjRegLogistic, kLinkSigmoid, kGradScalar, nullptr, true, false, kLabelsDomain, kInterceptStump, kIn01},
+  {"binary:logistic", kObjLogistic, kLinkSigmoid, kGradScalar, nullptr, true, false, kLabelsAny, kInterceptStump},
+  {"binary:logitraw", kObjLogitRaw, kLinkIdentity, kGradScalar, nullptr, true, false, kLabelsDomain, kInterceptStump, kIn01},
+  {"reg:squaredlogerror", kObjSquaredLog, kLinkIdentity, kGradScalar, nullptr, true, true, kLabelsDomain, kInterceptStump, kAboveMinus1},
+  {"reg:pseudohubererror", kObjPseudoHuber, kLinkIdentity, kGradScalar, &Params::huber_slope, true, true, kLabelsAny, kInterceptStump},
+  {"count:poisson", kObjPoisson, kLinkExp, kGradScalar, &Params::max_delta_step, false, true, kLabelsDomain, kInterceptStump, kNonneg},
+  {"reg:gamma", kObjGamma, kLinkExp, kGradScalar, nullptr, false, true, kLabelsDomain, kInterceptStump, kPositive},
+  {"reg:tweedie", kObjTweedie, kLinkExp, kGradScalar, &Params::tweedie_variance_power, false, true, kLabelsDomain, kInterceptStump, kNonneg},
+  {"survival:aft", kObjAft, kLinkExp, kGradAft, nullptr, false, true, kLabelsBounds, kInterceptFixed},
+  {"rank:pairwise", kObjRankPairwise, kLinkIdentity, kGradRank, nullptr, false, true, kLabelsRank, kInterceptFixed},
+  {"rank:ndcg", kObjRankNdcg, kLinkIdentity, kGradRank, nullptr, false, true, kLabelsRank, kInterceptFixed},
+  {"rank:map", kObjRankMap, kLinkIdentity, kGradRank, nullptr, false, true, kLabelsRank, kInterceptFixed},
+  {"reg:quantileerror", kObjQuantile, kLinkIdentity, kGradQuantile, nullptr, false, false, kLabelsDomain, kInterceptQuantile, kFinite},
+  {"multi:softprob", kObjSoftprob, kLinkSoftmax, kGradSoftprob, nullptr, false, false, kLabelsDomain, kInterceptNone, kClassIndex},
+  {"multi:softmax", kObjSoftprob, kLinkSoftmax, kGradSoftprob, nullptr, false, false, kLabelsDomain, kInterceptNone, kClassIndex},
+};
+
+const Objective& objective_row(const Params& p) { return kObjectives[p.objective_index]; }
+
 constexpr int kMaxVectorTargets = 64;   // vector-leaf trees: the level histograms are T times a scalar tree's
 
 // "0,1;2,3,4" -> {{0, 1}, {2, 3, 4}}; empty sets are dropped, the indices are checked against F in B2_BoosterCreate
@@ -73,7 +94,7 @@ std::vector<float> parse_quantile_alpha(std::string v) {
 void set_targets(Params* p, int T) {
   if (T < 1 || T > kMaxTargets) fail("num_target must be in [1, %d], got %d", kMaxTargets, T);
   if (T > 1) {
-    if (!obj_multi_target(p->objective))
+    if (!objective_row(*p).multi_target)
       fail("objective '%s' does not support a label with %d columns (multi-target objectives: reg:squarederror, "
            "reg:squaredlogerror, reg:pseudohubererror, reg:logistic, binary:logistic, binary:logitraw)",
            p->objective_name.c_str(), T);
@@ -105,24 +126,14 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     auto i = [&]() { return atoi(v.c_str()); };
     if (k == "objective") {
       p->objective_name = v;
-      if (v == "reg:squarederror" || v == "reg:linear") p->objective = kObjSquaredError;
-      else if (v == "binary:logistic") p->objective = kObjLogistic;
-      else if (v == "multi:softprob" || v == "multi:softmax") p->objective = kObjSoftprob;
-      else if (v == "reg:logistic") p->objective = kObjRegLogistic;
-      else if (v == "binary:logitraw") p->objective = kObjLogitRaw;
-      else if (v == "reg:squaredlogerror") p->objective = kObjSquaredLog;
-      else if (v == "reg:pseudohubererror") p->objective = kObjPseudoHuber;
-      else if (v == "count:poisson") p->objective = kObjPoisson;
-      else if (v == "reg:gamma") p->objective = kObjGamma;
-      else if (v == "reg:tweedie") p->objective = kObjTweedie;
-      else if (v == "survival:aft") p->objective = kObjAft;
-      else if (v == "rank:pairwise") p->objective = kObjRankPairwise;
-      else if (v == "rank:ndcg") p->objective = kObjRankNdcg;
-      else if (v == "rank:map") p->objective = kObjRankMap;
-      else if (v == "reg:quantileerror") p->objective = kObjQuantile;
-      else fail("unsupported objective '%s' (supported: reg:squarederror, reg:logistic, binary:logistic, binary:logitraw, "
-                "reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie, survival:aft, "
-                "rank:pairwise, rank:ndcg, rank:map, reg:quantileerror, multi:softprob, multi:softmax)", v.c_str());
+      const Objective* row = std::find_if(std::begin(kObjectives), std::end(kObjectives),
+                                          [&](const Objective& o) { return v == o.name; });
+      if (row == std::end(kObjectives))
+        fail("unsupported objective '%s' (supported: reg:squarederror, reg:logistic, binary:logistic, binary:logitraw, "
+             "reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie, survival:aft, "
+             "rank:pairwise, rank:ndcg, rank:map, reg:quantileerror, multi:softprob, multi:softmax)", v.c_str());
+      p->objective_index = (int)(row - kObjectives);
+      p->objective = row->id;
     } else if (k == "num_class") { p->num_class = i(); p->num_class_set = true; }
     else if (k == "num_target") { p->num_target = i(); p->num_target_set = true; }
     else if (k == "quantile_alpha") p->quantile_alpha = parse_quantile_alpha(v);
@@ -229,19 +240,20 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
       }
     }
   }
-  if (obj_rank(p->objective) && p->num_class > 1)
+  const Objective& obj = objective_row(*p);
+  if (obj.grad == kGradRank && p->num_class > 1)
     fail("%s has one output per row: num_class must be 1, got %d", p->objective_name.c_str(), p->num_class);
-  if (p->objective == kObjQuantile) {
+  if (obj.grad == kGradQuantile) {
     // rules of this engine (DESIGN.md 2): the outputs are the alphas, the leaf refresh needs the plain gbtree round
     if (p->num_class_set)
       fail("reg:quantileerror has one output per quantile_alpha: num_class must not be set (got %d)", p->num_class);
     if (p->dart) fail("reg:quantileerror is not supported with booster='dart'");
     if (p->num_parallel_tree > 1) fail("reg:quantileerror needs num_parallel_tree = 1 (got %d)", p->num_parallel_tree);
     p->num_class = (int)p->quantile_alpha.size();
-  } else if (p->objective != kObjSoftprob) p->num_class = 1;
+  } else if (obj.grad != kGradSoftprob) p->num_class = 1;
   // vector-leaf trees (DESIGN.md 2 item 19): what they do not cover yet, refused for any number of targets
   if (p->multi_strategy == 1) {
-    if (p->objective == kObjSoftprob)
+    if (obj.grad == kGradSoftprob)
       fail("multi_strategy='multi_output_tree' is not supported with objective='%s': vector-leaf trees take the "
            "multi-target objectives (reg:squarederror, reg:squaredlogerror, reg:pseudohubererror, reg:logistic, "
            "binary:logistic, binary:logitraw)", p->objective_name.c_str());
@@ -249,14 +261,14 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     if (p->num_parallel_tree > 1)
       fail("multi_strategy='multi_output_tree' needs num_parallel_tree = 1 (got %d)", p->num_parallel_tree);
   }
-  if (p->objective == kObjSoftprob && p->num_class < 2) fail("multi:softprob needs num_class >= 2");
+  if (obj.grad == kGradSoftprob && p->num_class < 2) fail("multi:softprob needs num_class >= 2");
   // update mode (DESIGN.md 2 item 20): only the refresh updater, and only where a refreshed leaf is a Newton step
   if (p->update_mode) {
     if (p->updater != "refresh")
       fail("process_type='update' needs updater='refresh', got updater='%s' (updater='prune' and 'refresh,prune' are "
            "not supported)", p->updater.c_str());
     if (p->dart) fail("process_type='update' is not supported with booster='dart'");
-    if (p->objective == kObjQuantile)
+    if (obj.grad == kGradQuantile)
       fail("process_type='update' is not supported with objective='reg:quantileerror': its leaf values are residual "
            "quantiles, which the refresh updater does not recompute");
   } else if (p->updater == "refresh") {
@@ -281,31 +293,22 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     fail("tweedie_variance_power must be in [1, 2), got %g", (double)p->tweedie_variance_power);
   if (!(p->aft_sigma > 0.0f) || std::isinf(p->aft_sigma))
     fail("aft_loss_distribution_scale must be finite and > 0, got %g", (double)p->aft_sigma);
-  // survival:aft fits no intercept: base_score defaults to 0.5 (margin log 0.5) and is never estimated
-  if (p->objective == kObjAft && !p->base_score_set) { p->base_score = 0.5f; p->base_score_set = true; }
-  // the rank objectives neither: their margin is the score itself (identity transform)
-  if (obj_rank(p->objective) && !p->base_score_set) { p->base_score = 0.5f; p->base_score_set = true; }
+  // survival:aft fits no intercept (margin log 0.5), and the rank objectives' margin is the score itself (identity
+  // transform): base_score defaults to 0.5 and is never estimated
+  if (obj.intercept == kInterceptFixed && !p->base_score_set) { p->base_score = 0.5f; p->base_score_set = true; }
   if (p->base_score_set) {
     if (p->objective == kObjRegLogistic && !(p->base_score > 0.0f && p->base_score < 1.0f))
       fail("base_score must be in (0, 1) for reg:logistic, got %g", (double)p->base_score);
-    if (obj_log_link(p->objective) && !(p->base_score > 0.0f))
+    if (obj.link == kLinkExp && !(p->base_score > 0.0f))
       fail("base_score must be > 0 for %s, got %g", p->objective_name.c_str(), (double)p->base_score);
   }
 }
 
-// the parameter that the gradient kernel of an objective takes (gradient_param_kernel)
-float objective_param(const Params& p) {
-  if (p.objective == kObjPseudoHuber) return p.huber_slope;
-  if (p.objective == kObjPoisson) return p.max_delta_step;
-  if (p.objective == kObjTweedie) return p.tweedie_variance_power;
-  return 0.0f;
-}
-
 // margin of base_score (the inverse of the prediction transform), evaluated on the host with libm's logf
 float base_margin_value(const Params& p) {
-  if (obj_sigmoid(p.objective)) return -logf(1.0f / p.base_score - 1.0f);
-  if (obj_log_link(p.objective)) return logf(p.base_score);
-  return p.base_score;
+  if (objective_row(p).link == kLinkSigmoid) return -logf(1.0f / p.base_score - 1.0f);
+  if (objective_row(p).link == kLinkExp) return logf(p.base_score);
+  return p.base_score;   // identity, and every class of a softmax
 }
 
 // -- host replicas of the gain / weight formulas (A.6, A.7); same IEEE sequence as the kernels
@@ -318,53 +321,62 @@ float h_calc_weight(const Params& p, double G, double H) {
   return (float)dw;
 }
 
-// metric id of an eval_metric name; *param receives the metric's parameter (rho of tweedie-nloglik@rho, huber_slope for mphe)
-B2Metric metric_id(const char* name, const Params& p, float* param, int* minus) {
-  std::string s(name ? name : "");
+// Every eval_metric name.  A name is matched whole, except tweedie-nloglik[@rho] and the ranking metrics ndcg / map /
+// pre[@k][-]; those come last, so that "mape" is not read as map@k.
+constexpr Metric kMetrics[] = {
+  {"rmse", kMetricRmse, kEvalElementwise, true},
+  {"rmsle", kMetricRmsle, kEvalElementwise, true},
+  {"mae", kMetricMae, kEvalElementwise, true},
+  {"mape", kMetricMape, kEvalElementwise, true},
+  {"mphe", kMetricMphe, kEvalElementwise, true},
+  {"logloss", kMetricLogloss, kEvalElementwise, true},
+  {"error", kMetricError, kEvalElementwise, true},
+  {"poisson-nloglik", kMetricPoissonNloglik, kEvalElementwise, false},
+  {"gamma-nloglik", kMetricGammaNloglik, kEvalElementwise, false},
+  {"gamma-deviance", kMetricGammaDeviance, kEvalElementwise, false},
+  {"mlogloss", kMetricMlogloss, kEvalClass, false},
+  {"merror", kMetricMerror, kEvalClass, false},
+  {"auc", kMetricAuc, kEvalAuc, false},
+  {"aucpr", kMetricAucPr, kEvalAuc, false},
+  {"aft-nloglik", kMetricAftNloglik, kEvalAft, false},
+  {"interval-regression-accuracy", kMetricIntervalAccuracy, kEvalAft, false},
+  {"quantile", kMetricQuantile, kEvalQuantile, false},
+  {"tweedie-nloglik", kMetricTweedieNloglik, kEvalElementwise, false},
+  {"ndcg", kMetricNdcg, kEvalRank, false},
+  {"map", kMetricMap, kEvalRank, false},
+  {"pre", kMetricPre, kEvalRank, false},
+};
+
+// the row of an eval_metric name; *param receives its parameter (tweedie-nloglik@rho, mphe's huber_slope, k of a ranking
+// metric's @k, 0: the whole group), *minus a ranking metric's trailing '-' (groups without relevant rows score 0, not 1)
+const Metric& metric_id(const char* name, const Params& p, float* param, int* minus) {
+  const std::string s(name ? name : "");
   *param = 0.0f; *minus = 0;
-  if (s == "rmsle") return kMetricRmsle;
-  if (s == "mape") return kMetricMape;
-  if (s == "mphe") { *param = p.huber_slope; return kMetricMphe; }
-  if (s == "poisson-nloglik") return kMetricPoissonNloglik;
-  if (s == "gamma-nloglik") return kMetricGammaNloglik;
-  if (s == "gamma-deviance") return kMetricGammaDeviance;
-  if (s.rfind("tweedie-nloglik", 0) == 0) {
-    *param = 1.5f;   // xgboost's default when the name carries no @rho
-    if (s.size() > 15) {
+  for (const Metric& r : kMetrics) {
+    if (s.compare(0, strlen(r.name), r.name) != 0) continue;
+    std::string rest = s.substr(strlen(r.name));
+    if (r.id == kMetricTweedieNloglik) {
+      *param = 1.5f;   // xgboost's default when the name carries no @rho
+      if (rest.empty()) return r;
       char* end = nullptr;
-      const std::string r = s.substr(16);
-      const double v = s[15] == '@' ? strtod(r.c_str(), &end) : NAN;
-      if (s[15] != '@' || r.empty() || *end != '\0' || !(v >= 1.0 && v < 2.0))
+      const double v = rest[0] == '@' ? strtod(rest.c_str() + 1, &end) : NAN;
+      if (rest[0] != '@' || rest.size() < 2 || *end != '\0' || !(v >= 1.0 && v < 2.0))
         fail("eval metric '%s': the Tweedie power must be given as tweedie-nloglik@rho with rho in [1, 2)", s.c_str());
       *param = (float)v;
+    } else if (r.family == kEvalRank) {
+      if (!rest.empty() && rest.back() == '-') { *minus = 1; rest.pop_back(); }
+      if (rest.empty()) return r;
+      char* end = nullptr;
+      const long long k = rest[0] == '@' && rest.size() > 1 ? strtoll(rest.c_str() + 1, &end, 10) : -1;
+      if (rest[0] != '@' || rest.size() < 2 || *end != '\0' || k < 1 || k > (1 << 24))
+        fail("eval metric '%s': the cut-off must be given as %s@k with an integer k >= 1", s.c_str(), r.name);
+      *param = (float)k;
+    } else if (!rest.empty()) {
+      continue;
+    } else if (r.id == kMetricMphe) {
+      *param = p.huber_slope;
     }
-    return kMetricTweedieNloglik;
-  }
-  if (s == "rmse") return kMetricRmse;
-  if (s == "logloss") return kMetricLogloss;
-  if (s == "error") return kMetricError;
-  if (s == "mlogloss") return kMetricMlogloss;
-  if (s == "merror") return kMetricMerror;
-  if (s == "mae") return kMetricMae;
-  if (s == "auc") return kMetricAuc;
-  if (s == "aucpr") return kMetricAucPr;
-  if (s == "aft-nloglik") return kMetricAftNloglik;
-  if (s == "quantile") return kMetricQuantile;
-  if (s == "interval-regression-accuracy") return kMetricIntervalAccuracy;
-  // ranking metrics: ndcg[@k][-], map[@k][-], pre[@k][-].  *param = k (0: the whole group), *minus = the trailing '-'
-  // (a group without relevant rows scores 0 instead of 1)
-  for (const B2Metric id : {kMetricNdcg, kMetricMap, kMetricPre}) {
-    const std::string base = id == kMetricNdcg ? "ndcg" : id == kMetricMap ? "map" : "pre";
-    if (s.compare(0, base.size(), base) != 0) continue;
-    std::string rest = s.substr(base.size());
-    if (!rest.empty() && rest.back() == '-') { *minus = 1; rest.pop_back(); }
-    if (rest.empty()) return id;
-    char* end = nullptr;
-    const long long k = rest[0] == '@' && rest.size() > 1 ? strtoll(rest.c_str() + 1, &end, 10) : -1;
-    if (rest[0] != '@' || rest.size() < 2 || *end != '\0' || k < 1 || k > (1 << 24))
-      fail("eval metric '%s': the cut-off must be given as %s@k with an integer k >= 1", s.c_str(), base.c_str());
-    *param = (float)k;
-    return id;
+    return r;
   }
   fail("unsupported eval metric '%s' (supported: rmse, mae, logloss, error, auc, aucpr, mlogloss, merror, rmsle, mape, mphe, "
        "poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy, "

@@ -1,5 +1,5 @@
 // predict.cu -- prediction on the device model: the TreeSHAP path table, margins of a range of trees, the cached
-// evaluation margins of a matrix, and metric sums over the workers.
+// evaluation margins of a matrix, and the eval metrics over the workers.
 #include <math.h>
 
 #include "host.h"
@@ -147,12 +147,117 @@ float* eval_margin(Booster* b, Matrix* m) {
 }
 
 // the first n doubles of b->d_metric summed over the workers, on the host (synchronises the stream)
-std::vector<double> metric_sums(Booster* b, size_t n, cudaStream_t s) {
+static std::vector<double> metric_sums(Booster* b, size_t n, cudaStream_t s) {
   allreduce(b->comm, b->d_metric.p, n, kNcclFloat64, kNcclSum, s);
   std::vector<double> h(n);
   CUDA_CHECK(cudaMemcpyAsync(h.data(), b->d_metric.p, n * sizeof(double), cudaMemcpyDeviceToHost, s));
   CUDA_CHECK(cudaStreamSynchronize(s));
   return h;
+}
+
+// eval_metric `name` on matrix m over every worker; the class, quantile and multi-target rules come after the margin
+double eval_metric(Booster* b, Matrix* m, const char* name) {
+  const Params& p = b->p; cudaStream_t s = b->ctx->stream; const int sms = b->ctx->num_sms, K = p.num_class;
+  float mparam; int minus;
+  const Metric& mt = metric_id(name, p, &mparam, &minus);
+  const ObjGrad grad = objective_row(p).grad;
+  const char* obj = p.objective_name.c_str();
+  const bool rank = mt.family == kEvalRank, auc = mt.family == kEvalAuc, aft = mt.family == kEvalAft;
+  if (rank && K > 1) fail("metric '%s' needs a single-output objective", name);
+  if (rank && !m->has_qgroups()) fail("metric '%s' needs query groups (qid) on the evaluation matrix", name);
+  // xgboost computes a per-group ranking AUC on a matrix with groups; this engine's auc / aucpr are binary or one-vs-rest
+  if (auc && m->has_qgroups())
+    fail("metric '%s' on a matrix with query groups (per-group ranking AUC) is not supported; use ndcg or map", name);
+  if (auc && p.num_target > 1)
+    fail("metric '%s' is not supported for a multi-target model (%d targets); use rmse, mae, logloss or error", name,
+         p.num_target);
+  if (auc && K > 1 && grad != kGradSoftprob)
+    fail("metric '%s' needs one output per row or a multi:softprob / multi:softmax model; objective '%s' has %d outputs",
+         name, obj, K);
+  if (aft && grad != kGradAft) fail("metric '%s' does not fit objective '%s'", name, obj);
+  if (aft && !m->has_bounds()) fail("metric '%s' needs label_lower_bound and label_upper_bound on the evaluation matrix", name);
+  if (!aft && m->n_label > 0 && m->n_targets != p.num_target)
+    fail("metric '%s': the evaluation matrix's label has %d columns, the model has %d targets", name, m->n_targets,
+         p.num_target);
+  if (!aft && !m->has_labels(p.num_target)) fail("evaluation matrix has no labels");
+  float* margin = eval_margin(b, m);
+  if (!auc && (mt.family == kEvalClass) != (grad == kGradSoftprob)) fail("metric '%s' does not fit objective '%s'", name, obj);
+  if (mt.family == kEvalQuantile && grad != kGradQuantile)
+    fail("metric 'quantile' needs objective reg:quantileerror (it reads quantile_alpha)");
+  if (p.num_target > 1 && !mt.multi_target)
+    fail("metric '%s' is not supported for a multi-target model (supported: rmse, rmsle, mae, mape, mphe, logloss, error)",
+         name);
+  const float* w = m->n_weight ? m->weight.p : nullptr;
+  b->d_metric.ensure(3 * (size_t)K + 1);
+  CUDA_CHECK(cudaMemsetAsync(b->d_metric.p, 0, 3 * sizeof(double), s));   // the aft, quantile and elementwise sums
+  DevBuf<float> pred;   // the ranking and AUC metrics read the transformed prediction
+  if (rank || auc) {
+    pred.ensure((size_t)std::max<int64_t>(m->n * K, 1));
+    if (m->n > 0) CUDA_CHECK(cudaMemcpyAsync(pred.p, margin, (size_t)(m->n * K) * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    LAUNCH_CHECK(b2_launch_transform(p.objective, K, pred.p, m->n, sms, s));
+  }
+  switch (mt.family) {
+    case kEvalRank: {
+      // ndcg / map / pre: per query group on the prediction order (rank_kernel.cu), averaged over the groups of all workers
+      DevBuf<double> vals; RankOrder po, lo;
+      po.run(m, pred.p, sms, s);
+      if (mt.id == kMetricNdcg) lo.run(m, m->label.p, sms, s);
+      ensure_rank_disc(b, m->max_qgroup);
+      vals.ensure((size_t)std::max<int64_t>(m->n_qgroups, 1));
+      LAUNCH_CHECK(b2_launch_rank_metric(mt.id, (int)mparam, minus, p.ndcg_exp_gain ? 1 : 0, m->qgroup_ptr.p, m->n_qgroups,
+                                         po.rows.p, m->label.p, mt.id == kMetricNdcg ? lo.keys_sorted.p : nullptr,
+                                         b->rank_disc.p, vals.p, b->d_metric.p, sms, s));
+      break;
+    }
+    case kEvalAuc: {
+      // ROC / PR AUC (auc_kernel.cu; DESIGN.md §2 item 17): per class a worker's triple (ROC: area, fp*tp, tp; PR: aucpr,
+      // 1, 1) plus the count of out-of-range labels, summed over the workers
+      DevBuf<uint8_t> tmp;
+      const size_t tb = b2_auc_temp_bytes(m->n);
+      tmp.ensure(tb);
+      LAUNCH_CHECK(b2_auc(mt.id == kMetricAucPr ? 1 : 0, K, pred.p, m->label.p, w, m->n, tmp.p, tb, b->d_metric.p, sms, s));
+      const std::vector<double> h = metric_sums(b, 3 * (size_t)K + 1, s);
+      if (h[3 * (size_t)K] > 0)
+        fail("metric '%s': label must be in [0, num_class), num_class = %d (%.0f rows outside)", name, K, h[3 * (size_t)K]);
+      // ROC with only one class present: xgboost reports 0.5
+      if (K == 1) return mt.id == kMetricAuc ? (h[1] > 0 ? h[0] / h[1] : 0.5) : h[0] / h[1];
+      // one-vs-rest: sum_c (A_c / L_c) T_c / sum_c T_c; NaN when some class has L_c = 0 or no class has T_c
+      double num = 0.0, den = 0.0;
+      for (int c = 0; c < K; ++c) {
+        const double A = h[3 * c], L = h[3 * c + 1], T = h[3 * c + 2];
+        if (!(L > 0)) return NAN;
+        num += A / L * T; den += T;
+      }
+      return den > 0 ? num / den : NAN;
+    }
+    case kEvalAft:
+      LAUNCH_CHECK(b2_launch_aft_metric(p.aft_dist, mt.id, (double)p.aft_sigma, margin, m->lower.p, m->upper.p, w, m->n,
+                                        b->d_metric.p, sms, s));
+      break;
+    case kEvalQuantile:
+      // pinball loss averaged over the rows and the alphas, weighted (sum, K * sum w summed over the workers)
+      if (!b->d_alpha.p || b->d_alpha.cap < p.quantile_alpha.size()) {
+        upload(b->d_alpha, p.quantile_alpha, s);
+        CUDA_CHECK(cudaStreamSynchronize(s));
+      }
+      LAUNCH_CHECK(b2_launch_quantile_metric(K, b->d_alpha.p, margin, m->label.p, w, m->n, b->d_metric.p, sms, s));
+      break;
+    default: {
+      // elementwise (over the n x T outputs of a multi-target model, each with its row's weight: xgboost's EvalEWiseBase)
+      // and class metrics: (sum, wsum, rows with a label outside [0, num_class)), so every rank fails together
+      if (p.num_target > 1)
+        LAUNCH_CHECK(b2_launch_metric_multi_target(p.objective, mt.id, p.num_target, mparam, margin, m->label.p, w, m->n,
+                                                   b->d_metric.p, sms, s));
+      else
+        LAUNCH_CHECK(b2_launch_metric(p.objective, mt.id, K, mparam, margin, m->label.p, w, m->n, b->d_metric.p, sms, s));
+      const std::vector<double> h = metric_sums(b, 3, s);
+      if (h[2] > 0) fail("metric '%s': label must be in [0, num_class), num_class = %d (%.0f rows outside)", name, K, h[2]);
+      const double v = h[1] > 0 ? h[0] / h[1] : 0.0;
+      return (mt.id == kMetricRmse || mt.id == kMetricRmsle) ? sqrt(v) : v;
+    }
+  }
+  const std::vector<double> h = metric_sums(b, 2, s);   // ranking, aft and quantile: (sum, weight sum)
+  return h[1] > 0 ? h[0] / h[1] : 0.0;
 }
 
 }  // namespace b2host

@@ -59,108 +59,29 @@ void init_margin(Booster* b, float* margin, Matrix* m) {
   }
 }
 
-// base_score when the user gave none (xgboost >= 2.0: ObjFunction::InitEstimation -> FitIntercept, tree::FitStump;
-// SURVEY.md A.3): one Newton step of a stump at margin 0, -sum(g)/sum(h) over ALL workers, then the inverse link.
-// Sums are 40-bit fixed-point integers (exact below 2^31 rows), so every rank (and the oracle) computes the same value.
-void estimate_base_score(Booster* b) {
-  Matrix* m = b->train; cudaStream_t s = b->ctx->stream; Params& p = b->p;
-  if (p.base_score_set || p.objective == kObjSoftprob) { p.base_score_set = true; return; }
-  // existing trees were fitted around the intercept of the model they came from: never assume the default for them
-  if (!b->trees.empty()) fail("continuing from existing trees needs an explicit base_score (the source model's intercept)");
-  check_train_labels(b);
-  const int64_t n = m->n;
-  if (p.objective == kObjQuantile) {
-    // the fp32 mean over k of the weighted alpha_k-quantile of the labels (the leaf refresh's selection, one segment)
-    const int K = p.num_class;
-    ensure_quantile_buffers(b, 1);
-    DevBuf<float2> gq; DevBuf<float> q;
-    gq.ensure((size_t)std::max<int64_t>(n, 1)); q.ensure((size_t)K);
-    b->d_absmax.ensure(2); b->d_qexp.ensure(2);
-    CUDA_CHECK(cudaMemsetAsync(q.p, 0, (size_t)K * sizeof(float), s));
-    for (int k = 0; k < K; ++k) {
-      LAUNCH_CHECK(b2_launch_gradient_quantile(1, b->d_alpha.p + k, nullptr, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
-                                               gq.p, nullptr, b->ctx->num_sms, s));
-      CUDA_CHECK(cudaMemsetAsync(b->d_absmax.p, 0, 2 * sizeof(uint32_t), s));
-      LAUNCH_CHECK(b2_launch_absmax(gq.p, n, b->d_absmax.p, b->ctx->num_sms, s));
-      allreduce(b->comm, b->d_absmax.p, 2, kNcclUint32, kNcclMax, s);
-      LAUNCH_CHECK(b2_launch_quant_exponent(b->d_absmax.p, b->d_qexp.p, s));
-      quantile_select(b, k, nullptr, nullptr, gq.p, b->d_qexp.p, b->d_one.p, 1, 1.0f, nullptr, q.p + k, nullptr);
-    }
-    std::vector<float> h((size_t)K);
-    CUDA_CHECK(cudaMemcpyAsync(h.data(), q.p, (size_t)K * sizeof(float), cudaMemcpyDeviceToHost, s));
-    CUDA_CHECK(cudaStreamSynchronize(s));
-    float sum = 0.0f;
-    for (float v : h) sum += v;
-    p.base_score = sum / (float)K;
-    p.base_score_set = true;
-    return;
-  }
-  // T targets (DESIGN.md 2 item 18): one stump per target from its own slice of the class-major pairs, with its own
-  // exponents; the intercept is the fp32 sum over k, in k order, of fp32(stump_k / T) (stump_0 itself for T = 1)
-  const int T = p.num_target;
-  const size_t nt = (size_t)std::max<int64_t>(n * T, 1);
-  DevBuf<float> zeros; DevBuf<float2> gh; DevBuf<long long> sums;
-  zeros.ensure(nt); gh.ensure(nt); sums.ensure(4);
-  CUDA_CHECK(cudaMemsetAsync(zeros.p, 0, nt * sizeof(float), s));
-  if (T > 1)
-    LAUNCH_CHECK(b2_launch_gradient_multi_target(p.objective, T, zeros.p, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
-                                                 p.scale_pos_weight, objective_param(p), gh.p, nullptr, nullptr,
-                                                 b->ctx->num_sms, s));
-  else
-    LAUNCH_CHECK(b2_launch_gradient(p.objective, 1, zeros.p, m->label.p, m->n_weight ? m->weight.p : nullptr, n, p.scale_pos_weight,
-                                    objective_param(p), gh.p, nullptr, nullptr, b->ctx->num_sms, s));
-  b->d_absmax.ensure(2); b->d_qexp.ensure(2);
-  auto limbs_to_double = [](long long hi, long long lo) {   // b2_limbs_to_double on the host: one rounding
-    hi += lo >> B2_LIMB_SHIFT; lo &= (1ll << B2_LIMB_SHIFT) - 1;
-    return (double)hi * (double)(1ll << B2_LIMB_SHIFT) + (double)lo;
-  };
-  float stump = 0.0f;
-  for (int k = 0; k < T; ++k) {
-    const float2* ghk = gh.p + (size_t)k * n;
-    CUDA_CHECK(cudaMemsetAsync(b->d_absmax.p, 0, 2 * sizeof(uint32_t), s));
-    LAUNCH_CHECK(b2_launch_absmax(ghk, n, b->d_absmax.p, b->ctx->num_sms, s));
-    allreduce(b->comm, b->d_absmax.p, 2, kNcclUint32, kNcclMax, s);
-    LAUNCH_CHECK(b2_launch_quant_exponent(b->d_absmax.p, b->d_qexp.p, s));
-    CUDA_CHECK(cudaMemsetAsync(sums.p, 0, 4 * sizeof(long long), s));
-    LAUNCH_CHECK(b2_launch_sum_fixed(ghk, n, b->d_qexp.p, 40, sums.p, b->ctx->num_sms, s));
-    allreduce(b->comm, sums.p, 4, kNcclInt64, kNcclSum, s);   // [g, h][hi, lo] limbs (common.cuh): exact over all ranks
-    long long h_s[4]; int32_t h_e[2];
-    CUDA_CHECK(cudaMemcpyAsync(h_s, sums.p, sizeof(h_s), cudaMemcpyDeviceToHost, s));
-    CUDA_CHECK(cudaMemcpyAsync(h_e, b->d_qexp.p, sizeof(h_e), cudaMemcpyDeviceToHost, s));
-    CUDA_CHECK(cudaStreamSynchronize(s));
-    const double G = limbs_to_double(h_s[0], h_s[1]) / ldexp(1.0, 40 - h_e[0]);
-    const double H = limbs_to_double(h_s[2], h_s[3]) / ldexp(1.0, 40 - h_e[1]);
-    const float stump_k = H <= 1e-6 ? 0.0f : (float)(-G / H);
-    stump = k == 0 ? stump_k / (float)T : stump + stump_k / (float)T;
-  }
-  if (obj_sigmoid(p.objective) || obj_log_link(p.objective)) {
-    // margin -> output space with the engine's own sigmoid / exp (same IEEE sequence as the kernels): evaluated on the device
-    DevBuf<float> one; one.ensure(1);
-    CUDA_CHECK(cudaMemcpyAsync(one.p, &stump, sizeof(float), cudaMemcpyHostToDevice, s));
-    LAUNCH_CHECK(b2_launch_transform(p.objective, 1, one.p, 1, b->ctx->num_sms, s));
-    float prob = 0.5f;
-    CUDA_CHECK(cudaMemcpyAsync(&prob, one.p, sizeof(float), cudaMemcpyDeviceToHost, s));
-    CUDA_CHECK(cudaStreamSynchronize(s));
-    p.base_score = prob;
-  } else {
-    p.base_score = stump;
-  }
-  p.base_score_set = true;
+// the n flags launch(bad) sets, maxed over the ranks so that every rank fails together (synchronises the stream)
+template <typename Launch>
+std::vector<uint32_t> check_flags(Booster* b, int n, Launch launch) {
+  cudaStream_t s = b->ctx->stream;
+  DevBuf<uint32_t> bad; bad.ensure(n);
+  CUDA_CHECK(cudaMemsetAsync(bad.p, 0, n * sizeof(uint32_t), s));
+  LAUNCH_CHECK(launch(bad.p));
+  allreduce(b->comm, bad.p, n, kNcclUint32, kNcclMax, s);
+  std::vector<uint32_t> h(n);
+  CUDA_CHECK(cudaMemcpyAsync(h.data(), bad.p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  return h;
 }
 
 // survival:aft reads the label bounds instead of the label: both present, no NaN, 0 <= lower (finite) <= upper, and an
 // uncensored row (lower == upper) needs y > 0.  Once per train matrix, like check_labels.
 void check_bounds(Booster* b) {
-  Matrix* m = b->train; cudaStream_t s = b->ctx->stream;
+  Matrix* m = b->train;
   if (b->labels_checked) return;
   if (!m->has_bounds()) fail("survival:aft needs label_lower_bound and label_upper_bound");
-  DevBuf<uint32_t> bad; bad.ensure(4);
-  CUDA_CHECK(cudaMemsetAsync(bad.p, 0, 4 * sizeof(uint32_t), s));
-  LAUNCH_CHECK(b2_launch_aft_bounds_check(m->lower.p, m->upper.p, m->n, bad.p, b->ctx->num_sms, s));
-  allreduce(b->comm, bad.p, 4, kNcclUint32, kNcclMax, s);
-  uint32_t h[4] = {0, 0, 0, 0};
-  CUDA_CHECK(cudaMemcpyAsync(h, bad.p, sizeof(h), cudaMemcpyDeviceToHost, s));
-  CUDA_CHECK(cudaStreamSynchronize(s));
+  const std::vector<uint32_t> h = check_flags(b, 4, [&](uint32_t* bad) {
+    return b2_launch_aft_bounds_check(m->lower.p, m->upper.p, m->n, bad, b->ctx->num_sms, b->ctx->stream);
+  });
   if (h[0]) fail("survival:aft: label bounds must not be NaN");
   if (h[1]) fail("survival:aft: label_lower_bound must be finite and >= 0");
   if (h[2]) fail("survival:aft: label_upper_bound must be >= label_lower_bound");
@@ -171,20 +92,16 @@ void check_bounds(Booster* b) {
 // the rank objectives need query groups and labels that are finite, >= 0 and, with the exponential gain, <= 31;
 // rank:map needs binary relevance (0 or 1) and ignores ndcg_exp_gain
 void check_rank_labels(Booster* b) {
-  Matrix* m = b->train; cudaStream_t s = b->ctx->stream;
+  Matrix* m = b->train;
   if (!m->has_qgroups())
     fail("%s needs query groups on the train matrix: pass qid (or group) to the DMatrix", b->p.objective_name.c_str());
   if (b->labels_checked) return;
   check_train_labels(b);
   const bool map = b->p.objective == kObjRankMap;
-  DevBuf<uint32_t> bad; bad.ensure(3);
-  CUDA_CHECK(cudaMemsetAsync(bad.p, 0, 3 * sizeof(uint32_t), s));
-  LAUNCH_CHECK(b2_launch_rank_label_check(m->label.p, m->n, !map && b->p.ndcg_exp_gain ? 1 : 0, map ? 1 : 0, bad.p,
-                                          b->ctx->num_sms, s));
-  allreduce(b->comm, bad.p, 3, kNcclUint32, kNcclMax, s);
-  uint32_t h[3] = {0, 0, 0};
-  CUDA_CHECK(cudaMemcpyAsync(h, bad.p, sizeof(h), cudaMemcpyDeviceToHost, s));
-  CUDA_CHECK(cudaStreamSynchronize(s));
+  const std::vector<uint32_t> h = check_flags(b, 3, [&](uint32_t* bad) {
+    return b2_launch_rank_label_check(m->label.p, m->n, !map && b->p.ndcg_exp_gain ? 1 : 0, map ? 1 : 0, bad,
+                                      b->ctx->num_sms, b->ctx->stream);
+  });
   if (h[2]) fail("rank:map: labels must be 0 or 1 (binary relevance); use rank:ndcg for graded relevance");
   if (h[0]) fail("%s: labels must be finite and >= 0", b->p.objective_name.c_str());
   if (h[1]) fail("%s: with ndcg_exp_gain the labels must be <= 31 (the gain is 2^label - 1); set ndcg_exp_gain=false "
@@ -202,7 +119,7 @@ void ensure_rank_disc(Booster* b, int64_t len) {
 }
 
 // LambdaMART gradients of the train matrix (rank_kernel.cu): order the margins per group, then one pass over the groups
-void rank_gradient(Booster* b, const float* margin, uint32_t* absmax, uint32_t* err) {
+void rank_gradient(Booster* b, const float* margin, float2* gh, uint32_t* absmax, uint32_t* err) {
   Matrix* m = b->train; cudaStream_t s = b->ctx->stream; const Params& p = b->p; const int sms = b->ctx->num_sms;
   ensure_rank_disc(b, m->max_qgroup);
   const bool ndcg = p.objective == kObjRankNdcg;
@@ -230,34 +147,127 @@ void rank_gradient(Booster* b, const float* margin, uint32_t* absmax, uint32_t* 
                                              ndcg ? b->rank_inv_idcg.p : nullptr, b->rank_disc.p, p.rank_k,
                                              p.ndcg_exp_gain ? 1 : 0, b->rank_scratch_m.p, b->rank_scratch_y.p,
                                              b->rank_scratch_p.p, map ? b->rank_scratch_a.p : nullptr,
-                                             map ? b->rank_scratch_r.p : nullptr, b->gh.p, absmax, err, sms, s));
+                                             map ? b->rank_scratch_r.p : nullptr, gh, absmax, err, sms, s));
 }
 
 // labels outside the objective's domain fail training (xgboost's CheckLabel); once per train matrix, before the first tree
 void check_labels(Booster* b) {
-  Matrix* m = b->train; const int o = b->p.objective; cudaStream_t s = b->ctx->stream;
-  if (o == kObjAft) { check_bounds(b); return; }
-  if (obj_rank(o)) { check_rank_labels(b); return; }
-  if (o == kObjSquaredError || o == kObjLogistic || o == kObjPseudoHuber || b->labels_checked) return;
+  Matrix* m = b->train; const Params& p = b->p; const Objective& o = objective_row(p);
+  if (o.labels == kLabelsBounds) { check_bounds(b); return; }
+  if (o.labels == kLabelsRank) { check_rank_labels(b); return; }
+  if (o.labels == kLabelsAny || b->labels_checked) return;
   check_train_labels(b);
-  DevBuf<uint32_t> bad; bad.ensure(1);
-  CUDA_CHECK(cudaMemsetAsync(bad.p, 0, sizeof(uint32_t), s));
-  LAUNCH_CHECK(b2_launch_label_check(o, b->p.num_class, m->label.p, m->n * b->p.num_target, bad.p, b->ctx->num_sms, s));
-  allreduce(b->comm, bad.p, 1, kNcclUint32, kNcclMax, s);
-  uint32_t h = 0;
-  CUDA_CHECK(cudaMemcpyAsync(&h, bad.p, sizeof(h), cudaMemcpyDeviceToHost, s));
-  CUDA_CHECK(cudaStreamSynchronize(s));
-  if (h) {
-    // a class index; non-integer labels truncate like xgboost's, NaN is rejected (xgboost lets it through)
-    if (o == kObjSoftprob)
-      fail("label must be in [0, num_class) for %s, num_class = %d", b->p.objective_name.c_str(), b->p.num_class);
-    const char* cond = (o == kObjRegLogistic || o == kObjLogitRaw) ? "label must be in [0, 1]"
-                       : o == kObjSquaredLog ? "label must be greater than -1"
-                       : o == kObjGamma ? "label must be positive"
-                       : o == kObjQuantile ? "label must be finite" : "label must be nonnegative";
-    fail("%s for %s", cond, b->p.objective_name.c_str());
-  }
+  const std::vector<uint32_t> h = check_flags(b, 1, [&](uint32_t* bad) {
+    return b2_launch_label_check(p.objective, p.num_class, m->label.p, m->n * p.num_target, bad, b->ctx->num_sms,
+                                 b->ctx->stream);
+  });
+  if (h[0]) fail(o.label_rule, p.objective_name.c_str(), p.num_class);
   b->labels_checked = true;
+}
+
+// the gradient pairs at margin [n][K] into gh [K][n]; nullable absmax (|g|, |h| maxima per class) and err (non-finite)
+void objective_gradient(Booster* b, const float* margin, float2* gh, uint32_t* absmax, uint32_t* err) {
+  Matrix* m = b->train; const Params& p = b->p; const Objective& o = objective_row(p);
+  const float* w = m->n_weight ? m->weight.p : nullptr;
+  const float param = o.param ? p.*o.param : 0.0f;
+  const int K = p.num_class, sms = b->ctx->num_sms; cudaStream_t s = b->ctx->stream;
+  if (o.grad == kGradRank)
+    rank_gradient(b, margin, gh, absmax, err);
+  else if (o.grad == kGradAft)
+    LAUNCH_CHECK(b2_launch_gradient_aft(p.aft_dist, (double)p.aft_sigma, margin, m->lower.p, m->upper.p, w, m->n, gh,
+                                        absmax, err, sms, s));
+  else if (o.grad == kGradQuantile) {
+    ensure_quantile_buffers(b, 1 << p.max_depth);
+    LAUNCH_CHECK(b2_launch_gradient_quantile(K, b->d_alpha.p, margin, m->label.p, w, m->n, gh, absmax, sms, s));
+  } else if (p.num_target > 1) {   // kGradScalar, one column per target
+    LAUNCH_CHECK(b2_launch_gradient_multi_target(p.objective, K, margin, m->label.p, w, m->n, p.scale_pos_weight, param,
+                                                 gh, absmax, err, sms, s));
+  } else {   // kGradScalar and kGradSoftprob, one column per class
+    LAUNCH_CHECK(b2_launch_gradient(p.objective, K, margin, m->label.p, w, m->n, p.scale_pos_weight, param, gh, absmax, err,
+                                    sms, s));
+  }
+}
+
+// base_score when the user gave none (xgboost >= 2.0: ObjFunction::InitEstimation -> FitIntercept, tree::FitStump;
+// SURVEY.md A.3): one Newton step of a stump at margin 0, -sum(g)/sum(h) over ALL workers, then the inverse link.
+// Sums are 40-bit fixed-point integers (exact below 2^31 rows), so every rank (and the oracle) computes the same value.
+void estimate_base_score(Booster* b) {
+  Matrix* m = b->train; cudaStream_t s = b->ctx->stream; Params& p = b->p; const Objective& o = objective_row(p);
+  if (p.base_score_set || o.intercept == kInterceptNone) { p.base_score_set = true; return; }
+  // existing trees were fitted around the intercept of the model they came from: never assume the default for them
+  if (!b->trees.empty()) fail("continuing from existing trees needs an explicit base_score (the source model's intercept)");
+  check_train_labels(b);
+  const int64_t n = m->n;
+  b->d_absmax.ensure(2); b->d_qexp.ensure(2);
+  if (o.intercept == kInterceptQuantile) {
+    // the fp32 mean over k of the weighted alpha_k-quantile of the labels (the leaf refresh's selection, one segment)
+    const int K = p.num_class;
+    ensure_quantile_buffers(b, 1);
+    DevBuf<float2> gq; DevBuf<float> q;
+    gq.ensure((size_t)std::max<int64_t>(n, 1)); q.ensure((size_t)K);
+    CUDA_CHECK(cudaMemsetAsync(q.p, 0, (size_t)K * sizeof(float), s));
+    for (int k = 0; k < K; ++k) {
+      LAUNCH_CHECK(b2_launch_gradient_quantile(1, b->d_alpha.p + k, nullptr, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
+                                               gq.p, nullptr, b->ctx->num_sms, s));
+      CUDA_CHECK(cudaMemsetAsync(b->d_absmax.p, 0, 2 * sizeof(uint32_t), s));
+      LAUNCH_CHECK(b2_launch_absmax(gq.p, n, b->d_absmax.p, b->ctx->num_sms, s));
+      allreduce(b->comm, b->d_absmax.p, 2, kNcclUint32, kNcclMax, s);
+      LAUNCH_CHECK(b2_launch_quant_exponent(b->d_absmax.p, b->d_qexp.p, s));
+      quantile_select(b, k, nullptr, nullptr, gq.p, b->d_qexp.p, b->d_one.p, 1, 1.0f, nullptr, q.p + k, nullptr);
+    }
+    std::vector<float> h((size_t)K);
+    CUDA_CHECK(cudaMemcpyAsync(h.data(), q.p, (size_t)K * sizeof(float), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    float sum = 0.0f;
+    for (float v : h) sum += v;
+    p.base_score = sum / (float)K;
+    p.base_score_set = true;
+    return;
+  }
+  // T targets (DESIGN.md 2 item 18): one stump per target from its own slice of the class-major pairs, with its own
+  // exponents; the intercept is the fp32 sum over k, in k order, of fp32(stump_k / T) (stump_0 itself for T = 1)
+  const int T = p.num_target;
+  const size_t nt = (size_t)std::max<int64_t>(n * T, 1);
+  DevBuf<float> zeros; DevBuf<float2> gh; DevBuf<long long> sums;
+  zeros.ensure(nt); gh.ensure(nt); sums.ensure(4);
+  CUDA_CHECK(cudaMemsetAsync(zeros.p, 0, nt * sizeof(float), s));
+  objective_gradient(b, zeros.p, gh.p, nullptr, nullptr);
+  auto limbs_to_double = [](long long hi, long long lo) {   // b2_limbs_to_double on the host: one rounding
+    hi += lo >> B2_LIMB_SHIFT; lo &= (1ll << B2_LIMB_SHIFT) - 1;
+    return (double)hi * (double)(1ll << B2_LIMB_SHIFT) + (double)lo;
+  };
+  float stump = 0.0f;
+  for (int k = 0; k < T; ++k) {
+    const float2* ghk = gh.p + (size_t)k * n;
+    CUDA_CHECK(cudaMemsetAsync(b->d_absmax.p, 0, 2 * sizeof(uint32_t), s));
+    LAUNCH_CHECK(b2_launch_absmax(ghk, n, b->d_absmax.p, b->ctx->num_sms, s));
+    allreduce(b->comm, b->d_absmax.p, 2, kNcclUint32, kNcclMax, s);
+    LAUNCH_CHECK(b2_launch_quant_exponent(b->d_absmax.p, b->d_qexp.p, s));
+    CUDA_CHECK(cudaMemsetAsync(sums.p, 0, 4 * sizeof(long long), s));
+    LAUNCH_CHECK(b2_launch_sum_fixed(ghk, n, b->d_qexp.p, 40, sums.p, b->ctx->num_sms, s));
+    allreduce(b->comm, sums.p, 4, kNcclInt64, kNcclSum, s);   // [g, h][hi, lo] limbs (common.cuh): exact over all ranks
+    long long h_s[4]; int32_t h_e[2];
+    CUDA_CHECK(cudaMemcpyAsync(h_s, sums.p, sizeof(h_s), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaMemcpyAsync(h_e, b->d_qexp.p, sizeof(h_e), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    const double G = limbs_to_double(h_s[0], h_s[1]) / ldexp(1.0, 40 - h_e[0]);
+    const double H = limbs_to_double(h_s[2], h_s[3]) / ldexp(1.0, 40 - h_e[1]);
+    const float stump_k = H <= 1e-6 ? 0.0f : (float)(-G / H);
+    stump = k == 0 ? stump_k / (float)T : stump + stump_k / (float)T;
+  }
+  if (o.link == kLinkSigmoid || o.link == kLinkExp) {
+    // margin -> output space with the engine's own sigmoid / exp (same IEEE sequence as the kernels): evaluated on the device
+    DevBuf<float> one; one.ensure(1);
+    CUDA_CHECK(cudaMemcpyAsync(one.p, &stump, sizeof(float), cudaMemcpyHostToDevice, s));
+    LAUNCH_CHECK(b2_launch_transform(p.objective, 1, one.p, 1, b->ctx->num_sms, s));
+    float prob = 0.5f;
+    CUDA_CHECK(cudaMemcpyAsync(&prob, one.p, sizeof(float), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    p.base_score = prob;
+  } else {
+    p.base_score = stump;
+  }
+  p.base_score_set = true;
 }
 
 // update mode: tree to_update[src] with the statistics of its refresh_nodes_kernel block.  Structure, splits, default
@@ -609,7 +619,8 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
   b->gh.ensure((size_t)std::max<int64_t>(n * K, 1));
   b->d_absmax.ensure(2 * (size_t)K); b->d_qexp.ensure(2);
   b->absmax_fused = false;
-  b->refresh_leaves = !custom_g && b->p.objective == kObjQuantile;
+  const Objective& o = objective_row(b->p);
+  b->refresh_leaves = !custom_g && o.grad == kGradQuantile;
   bool check_finite = false;
   if (custom_g) {
     if (len != n * K) fail("custom gradient has %lld values, expected %lld", (long long)len, (long long)(n * K));
@@ -618,35 +629,16 @@ void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64
     CUDA_CHECK(cudaMemcpyAsync(b->d_custom_h.p, custom_h, len * sizeof(float), cudaMemcpyHostToDevice, s));
     LAUNCH_CHECK(b2_launch_pack_custom(b->d_custom_g.p, b->d_custom_h.p, K, n, b->gh.p, b->ctx->num_sms, s));
   } else {
-    if (b->p.objective != kObjAft) check_train_labels(b);
+    if (o.labels != kLabelsBounds) check_train_labels(b);
     // the |g|,|h| maxima of every class tree come out of the same pass unless rows are dropped afterwards (subsample)
     b->absmax_fused = (b->p.subsample >= 1.0f || refresh) && K <= b2_gradient_fused_max_classes();
     if (b->absmax_fused) CUDA_CHECK(cudaMemsetAsync(b->d_absmax.p, 0, 2 * (size_t)K * sizeof(uint32_t), s));
-    check_finite = obj_checks_finite(b->p.objective);
+    check_finite = o.checks_finite;
     if (check_finite) {
       if (!b->h_grad_err) { CUDA_CHECK(cudaMallocHost(&b->h_grad_err, sizeof(uint32_t))); b->d_grad_err.ensure(1); }
       CUDA_CHECK(cudaMemsetAsync(b->d_grad_err.p, 0, sizeof(uint32_t), s));
     }
-    if (b->p.objective == kObjAft)
-      LAUNCH_CHECK(b2_launch_gradient_aft(b->p.aft_dist, (double)b->p.aft_sigma, gm, m->lower.p, m->upper.p,
-                                          m->n_weight ? m->weight.p : nullptr, n, b->gh.p,
-                                          b->absmax_fused ? b->d_absmax.p : nullptr, b->d_grad_err.p, b->ctx->num_sms, s));
-    else if (obj_rank(b->p.objective))
-      rank_gradient(b, gm, b->absmax_fused ? b->d_absmax.p : nullptr, b->d_grad_err.p);
-    else if (b->p.objective == kObjQuantile) {
-      ensure_quantile_buffers(b, 1 << b->p.max_depth);
-      LAUNCH_CHECK(b2_launch_gradient_quantile(K, b->d_alpha.p, gm, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
-                                               b->gh.p, b->absmax_fused ? b->d_absmax.p : nullptr, b->ctx->num_sms, s));
-    } else if (b->p.num_target > 1)
-      LAUNCH_CHECK(b2_launch_gradient_multi_target(b->p.objective, K, gm, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
-                                                   b->p.scale_pos_weight, objective_param(b->p), b->gh.p,
-                                                   b->absmax_fused ? b->d_absmax.p : nullptr,
-                                                   check_finite ? b->d_grad_err.p : nullptr, b->ctx->num_sms, s));
-    else
-      LAUNCH_CHECK(b2_launch_gradient(b->p.objective, K, gm, m->label.p, m->n_weight ? m->weight.p : nullptr, n,
-                                      b->p.scale_pos_weight, objective_param(b->p), b->gh.p,
-                                      b->absmax_fused ? b->d_absmax.p : nullptr, check_finite ? b->d_grad_err.p : nullptr,
-                                      b->ctx->num_sms, s));
+    objective_gradient(b, gm, b->gh.p, b->absmax_fused ? b->d_absmax.p : nullptr, check_finite ? b->d_grad_err.p : nullptr);
   }
   b->gh_ready = true;
   b->t.kernel_launches++;
