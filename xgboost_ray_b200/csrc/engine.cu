@@ -3,12 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
-#include <chrono>
-#include <map>
-#include <mutex>
 #include <string>
 #include <vector>
 
@@ -33,6 +29,41 @@ thread_local std::string g_last_error;
   return 0;
 
 struct CommH : HandleBase { Comm c; };
+Comm* comm_of(B2Handle h) { return h ? &from_handle<CommH>(h, kComm, "communicator")->c : nullptr; }   // 0: single process
+
+// the matrix of handle mh, its device made current
+Matrix* matrix_of(B2Handle mh) {
+  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
+  CUDA_CHECK(cudaSetDevice(m->ctx->device));
+  return m;
+}
+// the booster of handle bh with its pending round finished: every entry that reads or changes the model opens with this
+Booster* drained(B2Handle bh) {
+  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
+  drain_round(b);
+  return b;
+}
+TreeHost& tree_at(Booster* b, int tree) {
+  if (tree < 0 || tree >= (int)b->trees.size()) fail("tree index %d out of range", tree);
+  return b->trees[tree];
+}
+
+// n host values into a device field of m, copied before return (the caller may reuse its array); n < 0 copies none
+template <typename T>
+void set_field(Matrix* m, DevBuf<T>& d, const T* values, int64_t n) {
+  upload(d, values, (size_t)std::max<int64_t>(n, 0), m->ctx->stream);
+  CUDA_CHECK(cudaStreamSynchronize(m->ctx->stream));
+}
+// an entry that reads matrix mh under the model of booster bh: its pending round drained, the booster's device current
+template <typename Fn>
+int with_matrix(B2Handle bh, B2Handle mh, Fn fn) {
+  API_BEGIN
+  Booster* b = drained(bh);
+  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
+  CUDA_CHECK(cudaSetDevice(b->ctx->device));
+  fn(b, m);
+  API_END
+}
 
 }  // namespace b2host
 
@@ -131,183 +162,52 @@ int B2_CommFree(B2Handle comm) {
 
 int B2_MatrixCreateFromDense(const float* data, int64_t n_rows, int32_t n_cols, float missing, int device, B2Handle* out) {
   API_BEGIN
-  if (n_rows < 0 || n_cols <= 0) fail("invalid matrix shape %lld x %d", (long long)n_rows, n_cols);
-  if (n_rows >= (1LL << 31)) fail("at most 2^31-1 rows per GPU shard (row ids are int32), got %lld", (long long)n_rows);
-  Ctx* ctx = get_ctx(device);
-  Matrix* m = new Matrix(); m->kind = kMatrix; m->ctx = ctx; m->n = n_rows; m->F = n_cols; m->missing = missing;
-  try {
-    m->raw.ensure((size_t)std::max<int64_t>(n_rows * n_cols, 1));
-    upload_pipelined(ctx, m->raw.p, data, (size_t)n_rows * n_cols * sizeof(float));
-  } catch (...) { delete m; throw; }
-  m->has_raw = true;
-  { std::lock_guard<std::mutex> lk(g_matrix_mu); m->uid = g_next_matrix_uid++; g_live_matrices.insert(m->uid); }
-  *out = (B2Handle)m;
+  std::unique_ptr<Matrix> m = new_matrix(n_rows, n_cols, missing);
+  m->ctx = get_ctx(device);
+  upload_raw(m.get(), UploadSource{data});
+  *out = register_matrix(std::move(m));
   API_END
 }
 int B2_MatrixCreateFromCSR(int64_t* indptr, const int32_t* indices, const float* values, int64_t n_rows, int32_t n_cols,
                            int64_t nnz, float missing, int device, B2Handle* out) {
   API_BEGIN
   if (n_rows < 0 || n_cols <= 0 || nnz < 0) fail("invalid CSR matrix %lld x %d with %lld entries", (long long)n_rows, n_cols, (long long)nnz);
-  if (n_rows >= (1LL << 31)) fail("at most 2^31-1 rows per GPU shard (row ids are int32), got %lld", (long long)n_rows);
-  Ctx* ctx = get_ctx(device);
-  Matrix* m = new Matrix(); m->kind = kMatrix; m->ctx = ctx; m->n = n_rows; m->F = n_cols; m->missing = missing;
-  m->csr = true; m->nnz = nnz;
-  try { upload_csr(m, indptr, indices, values); } catch (...) { delete m; throw; }
-  { std::lock_guard<std::mutex> lk(g_matrix_mu); m->uid = g_next_matrix_uid++; g_live_matrices.insert(m->uid); }
-  *out = (B2Handle)m;
+  std::unique_ptr<Matrix> m = new_matrix(n_rows, n_cols, missing);
+  m->ctx = get_ctx(device); m->csr = true; m->nnz = nnz;
+  upload_csr(m.get(), indptr, indices, values);
+  *out = register_matrix(std::move(m));
   API_END
 }
 int B2_MatrixCreate(int64_t n_rows, int32_t n_cols, float missing, int device, B2Handle* out) {
   API_BEGIN
-  if (n_rows < 0 || n_cols <= 0) fail("invalid matrix shape %lld x %d", (long long)n_rows, n_cols);
-  if (n_rows >= (1LL << 31)) fail("at most 2^31-1 rows per GPU shard (row ids are int32), got %lld", (long long)n_rows);
-  Ctx* ctx = get_ctx(device);
-  Matrix* m = new Matrix(); m->kind = kMatrix; m->ctx = ctx; m->n = n_rows; m->F = n_cols; m->missing = missing;
-  try { m->raw.ensure((size_t)std::max<int64_t>(n_rows * n_cols, 1)); } catch (...) { delete m; throw; }
+  std::unique_ptr<Matrix> m = new_matrix(n_rows, n_cols, missing);
+  m->ctx = get_ctx(device);
+  m->raw.ensure((size_t)std::max<int64_t>(n_rows * n_cols, 1));   // filled by B2_MatrixSetRows
   m->has_raw = true;
-  { std::lock_guard<std::mutex> lk(g_matrix_mu); m->uid = g_next_matrix_uid++; g_live_matrices.insert(m->uid); }
-  *out = (B2Handle)m;
+  *out = register_matrix(std::move(m));
   API_END
 }
 int B2_MatrixCreateFromProcess(int64_t pid, uint64_t remote_addr, int64_t remote_row_stride_bytes, int64_t n_rows, int32_t n_cols,
                                float missing, int device, B2Handle* out) {
   API_BEGIN
-  if (n_rows < 0 || n_cols <= 0) fail("invalid matrix shape %lld x %d", (long long)n_rows, n_cols);
-  if (n_rows >= (1LL << 31)) fail("at most 2^31-1 rows per GPU shard (row ids are int32), got %lld", (long long)n_rows);
+  std::unique_ptr<Matrix> m = new_matrix(n_rows, n_cols, missing);
   if (pid <= 0 || remote_row_stride_bytes < (int64_t)n_cols * 4) fail("invalid remote source (pid %lld, row stride %lld)", (long long)pid, (long long)remote_row_stride_bytes);
-  Ctx* ctx = get_ctx(device);
-  Matrix* m = new Matrix(); m->kind = kMatrix; m->ctx = ctx; m->n = n_rows; m->F = n_cols; m->missing = missing;
-  try {
-    m->raw.ensure((size_t)std::max<int64_t>(n_rows * n_cols, 1));
-    UploadSource u; u.pid = pid; u.remote_addr = remote_addr; u.row_bytes = (size_t)n_cols * 4; u.row_stride = (size_t)remote_row_stride_bytes;
-    upload_pipelined(ctx, m->raw.p, u, (size_t)n_rows * n_cols * sizeof(float));
-  } catch (...) { delete m; throw; }
-  m->has_raw = true;
-  { std::lock_guard<std::mutex> lk(g_matrix_mu); m->uid = g_next_matrix_uid++; g_live_matrices.insert(m->uid); }
-  *out = (B2Handle)m;
+  m->ctx = get_ctx(device);
+  UploadSource u; u.pid = pid; u.remote_addr = remote_addr; u.row_bytes = (size_t)n_cols * 4; u.row_stride = (size_t)remote_row_stride_bytes;
+  upload_raw(m.get(), u);
+  *out = register_matrix(std::move(m));
   API_END
 }
-// Staging block of the interleaved ingest: persistent per device (grow-only), exported ONCE; the peers keep their mapping
-// of it across calls (mapping / unmapping a multi-GB allocation costs more than moving the rows).  A block that had to
-// grow is retired and freed only after the call's closing barrier, when every peer has dropped its mapping of it.
-struct IngestStage { float* p = nullptr; size_t bytes = 0; cudaIpcMemHandle_t h; bool exported = false; };
-IngestStage g_ingest_stage[64];
-std::map<std::string, void*> g_peer_stage;      // handle bytes -> mapped pointer (this process)
-std::mutex g_ingest_mu;
-double wall_seconds() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-
 int B2_MatrixCreateFromProcessInterleaved(int64_t pid, uint64_t remote_addr, int64_t n_total_rows, int32_t n_cols, int32_t shard_rank,
                                           B2Handle commh, float missing, int device, B2Handle* out) {
   API_BEGIN
   if (n_total_rows < 0 || n_cols <= 0 || pid <= 0) fail("invalid remote matrix (%lld x %d, pid %lld)", (long long)n_total_rows, n_cols, (long long)pid);
-  Comm* c = commh ? &from_handle<CommH>(commh, kComm, "communicator")->c : nullptr;
-  if (!c || c->world < 2 || c->world > B2_P2P_MAX_WORLD) fail("interleaved remote ingest needs a communicator of 2..%d ranks", B2_P2P_MAX_WORLD);
-  const int W = c->world, rank = c->rank;
-  Ctx* ctx = get_ctx(device); cudaStream_t s = ctx->stream;
-  static const bool timing = getenv("B2_INGEST_TIMING") && atoi(getenv("B2_INGEST_TIMING")) != 0;
-  double t0 = wall_seconds(), t_prev = t0;
-  auto lap = [&](const char* what) {
-    if (!timing) return;
-    const double t = wall_seconds();
-    fprintf(stderr, "[b2 ingest rank %d] %-28s %.4f s\n", rank, what, t - t_prev);
-    t_prev = t;
-  };
-  std::lock_guard<std::mutex> ingest_lock(g_ingest_mu);
-  // contiguous block of this rank (BATCH split of the global rows) and the rows it finally owns (INTERLEAVED)
-  B2RowBlocks rb; memset(&rb, 0, sizeof(rb));
-  const int64_t per = n_total_rows / W, extra = n_total_rows % W;
-  for (int w = 0; w <= W; ++w) rb.start[w] = (long long)(w * per + std::min<int64_t>(w, extra));
-  const int64_t b0 = rb.start[rank], bn = rb.start[rank + 1] - b0;
-  const int64_t n_mine = rank < n_total_rows ? (n_total_rows - rank + W - 1) / W : 0;
-  if (n_mine >= (1LL << 31)) fail("at most 2^31-1 rows per GPU shard (row ids are int32), got %lld", (long long)n_mine);
-  rb.world = W; rb.rank = rank; rb.n_cols = n_cols; rb.n_mine = (long long)n_mine;
-  DevBuf<int32_t> d_flag; d_flag.ensure(1);
-  auto any_rank = [&](int32_t mine) {   // max over the ranks of a flag
-    CUDA_CHECK(cudaMemcpyAsync(d_flag.p, &mine, sizeof(mine), cudaMemcpyHostToDevice, s));
-    allreduce(c, d_flag.p, 1, kNcclInt32, kNcclMax, s);
-    CUDA_CHECK(cudaMemcpyAsync(&mine, d_flag.p, sizeof(mine), cudaMemcpyDeviceToHost, s));
-    CUDA_CHECK(cudaStreamSynchronize(s));
-    return mine;
-  };
-  // collective call: every rank must hold the shard of its own rank, or all of them fail together
-  if (any_rank(shard_rank == rank ? 0 : 1))
-    fail("interleaved remote ingest: shard %d handed to rank %d (or a mismatch on another rank)", shard_rank, rank);
-  lap("agreement");
-  Matrix* m = new Matrix(); m->kind = kMatrix; m->ctx = ctx; m->n = n_mine; m->F = n_cols; m->missing = missing;
-  void* retired = nullptr;
-  try {
-    IngestStage& st = g_ingest_stage[(device >= 0 && device < 64) ? device : 0];
-    const size_t need = (size_t)std::max<int64_t>(bn * n_cols, 1) * sizeof(float);
-    int ok = 1;
-    if (st.bytes < need) {
-      retired = st.p; st.p = nullptr; st.bytes = 0; st.exported = false;
-      const size_t want = (need + need / 16 + ((size_t)1 << 20)) & ~(((size_t)1 << 20) - 1);
-      void* q = nullptr;
-      if (cudaMalloc(&q, want) != cudaSuccess) {
-        cudaGetLastError();
-        { std::lock_guard<std::mutex> lk(g_dev_pool[(device >= 0 && device < 64) ? device : 0].mu); pool_trim(g_dev_pool[(device >= 0 && device < 64) ? device : 0], 0); }
-        if (cudaMalloc(&q, want) != cudaSuccess) { cudaGetLastError(); fail("cudaMalloc of the %zu-byte ingest staging block failed", want); }
-      }
-      st.p = (float*)q; st.bytes = want;
-    }
-    if (!st.exported) {
-      if (cudaIpcGetMemHandle(&st.h, st.p) == cudaSuccess) st.exported = true;
-      else { ok = 0; cudaGetLastError(); memset(&st.h, 0, sizeof(st.h)); }
-    }
-    lap("staging block");
-    UploadSource u; u.pid = pid; u.remote_addr = remote_addr + (uint64_t)b0 * (uint64_t)n_cols * 4u; u.row_bytes = (size_t)n_cols * 4; u.row_stride = u.row_bytes;
-    upload_pipelined(ctx, st.p, u, (size_t)bn * n_cols * sizeof(float));
-    lap("read block from the driver");
-    m->raw.ensure((size_t)std::max<int64_t>(n_mine * n_cols, 1));
-    // exchange the IPC handles of the staging blocks (also: every rank's block is uploaded)
-    DevBuf<uint8_t> d_mine, d_all; d_mine.ensure(sizeof(st.h)); d_all.ensure(sizeof(st.h) * (size_t)W);
-    CUDA_CHECK(cudaMemcpyAsync(d_mine.p, &st.h, sizeof(st.h), cudaMemcpyHostToDevice, s));
-    NCCL_CHECK(nccl()->AllGather(d_mine.p, d_all.p, sizeof(st.h), kNcclUint8, c->comm, s));
-    std::vector<cudaIpcMemHandle_t> all((size_t)W);
-    CUDA_CHECK(cudaMemcpyAsync(all.data(), d_all.p, sizeof(st.h) * (size_t)W, cudaMemcpyDeviceToHost, s));
-    CUDA_CHECK(cudaStreamSynchronize(s));
-    lap("handle exchange");
-    // drop mappings of blocks that no peer exports any more (a peer's block grew), then map what is new
-    std::set<std::string> current;
-    for (int w = 0; w < W; ++w) if (w != rank) current.insert(std::string((const char*)&all[w], sizeof(all[w])));
-    for (auto it = g_peer_stage.begin(); it != g_peer_stage.end();) {
-      if (!current.count(it->first)) { cudaIpcCloseMemHandle(it->second); it = g_peer_stage.erase(it); } else ++it;
-    }
-    for (int w = 0; w < W && ok; ++w) {
-      if (w == rank) { rb.base[w] = st.p; continue; }
-      const std::string key((const char*)&all[w], sizeof(all[w]));
-      auto it = g_peer_stage.find(key);
-      if (it == g_peer_stage.end()) {
-        void* q = nullptr;
-        if (cudaIpcOpenMemHandle(&q, all[w], cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { ok = 0; cudaGetLastError(); break; }
-        it = g_peer_stage.emplace(key, q).first;
-      }
-      rb.base[w] = (const float*)it->second;
-    }
-    lap("peer mappings");
-    if (any_rank(ok ? 0 : 1)) {
-      // no peer mapping on some rank (no NVLink / IPC): every rank reads its own strided shard from the driver instead
-      UploadSource us; us.pid = pid; us.remote_addr = remote_addr + (uint64_t)rank * (uint64_t)n_cols * 4u;
-      us.row_bytes = (size_t)n_cols * 4; us.row_stride = us.row_bytes * (size_t)W;
-      upload_pipelined(ctx, m->raw.p, us, (size_t)n_mine * n_cols * sizeof(float));
-    } else {
-      LAUNCH_CHECK(b2_launch_gather_interleaved_rows(&rb, m->raw.p, ctx->num_sms, s));
-    }
-    // nobody overwrites (next call) or frees (a retired block) its staging block while a peer may still pull rows out of it
-    any_rank(0);
-    lap("row gather + closing barrier");
-    if (retired) { cudaFree(retired); retired = nullptr; }
-  } catch (...) { if (retired) cudaFree(retired); delete m; throw; }
-  m->has_raw = true;
-  { std::lock_guard<std::mutex> lk(g_matrix_mu); m->uid = g_next_matrix_uid++; g_live_matrices.insert(m->uid); }
-  *out = (B2Handle)m;
-  if (timing) fprintf(stderr, "[b2 ingest rank %d] total %.4f s (%lld of %lld rows x %d)\n", rank, wall_seconds() - t0, (long long)n_mine, (long long)n_total_rows, n_cols);
+  *out = ingest_interleaved(comm_of(commh), pid, remote_addr, n_total_rows, n_cols, shard_rank, missing, device);
   API_END
 }
 int B2_MatrixSetRows(B2Handle mh, int64_t row_begin, const float* data, int64_t n_rows) {
   API_BEGIN
-  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
-  CUDA_CHECK(cudaSetDevice(m->ctx->device));
+  Matrix* m = matrix_of(mh);
   if (m->quantized || !m->has_raw) fail("rows can only be set before the matrix is quantised");
   if (m->csr) fail("rows of a matrix created from CSR arrays cannot be set");
   if (row_begin < 0 || n_rows < 0 || row_begin + n_rows > m->n) fail("row block [%lld, %lld) outside the matrix (%lld rows)",
@@ -317,8 +217,7 @@ int B2_MatrixSetRows(B2Handle mh, int64_t row_begin, const float* data, int64_t 
 }
 int B2_MatrixSetFloatInfo(B2Handle mh, const char* field, const float* values, int64_t len) {
   API_BEGIN
-  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
-  CUDA_CHECK(cudaSetDevice(m->ctx->device));
+  Matrix* m = matrix_of(mh);
   std::string f(field ? field : "");
   DevBuf<float>* dst = nullptr; int64_t* cnt = nullptr;
   if (f == "label") {
@@ -342,22 +241,17 @@ int B2_MatrixSetFloatInfo(B2Handle mh, const char* field, const float* values, i
       const double q = (double)values[i] * 65536.0;
       m->fwq.push_back(q >= 4294967295.0 ? 0xffffffffu : (uint32_t)llrint(q));
     }
-    m->d_fwq.ensure((size_t)std::max<int64_t>(len, 1));
-    if (len > 0) CUDA_CHECK(cudaMemcpyAsync(m->d_fwq.p, m->fwq.data(), len * sizeof(uint32_t), cudaMemcpyHostToDevice, m->ctx->stream));
-    CUDA_CHECK(cudaStreamSynchronize(m->ctx->stream));
+    set_field(m, m->d_fwq, m->fwq.data(), len);
     return 0;
   }
   else fail("unknown float info field '%s'", f.c_str());
-  dst->ensure((size_t)std::max<int64_t>(len, 1));
-  if (len > 0) CUDA_CHECK(cudaMemcpyAsync(dst->p, values, len * sizeof(float), cudaMemcpyHostToDevice, m->ctx->stream));
-  CUDA_CHECK(cudaStreamSynchronize(m->ctx->stream));
+  set_field(m, *dst, values, len);
   *cnt = len;
   API_END
 }
 int B2_MatrixSetLabel(B2Handle mh, const float* values, int64_t rows, int32_t n_targets) {
   API_BEGIN
-  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
-  CUDA_CHECK(cudaSetDevice(m->ctx->device));
+  Matrix* m = matrix_of(mh);
   if (rows != m->n) fail("label has %lld rows, the matrix %lld", (long long)rows, (long long)m->n);
   if (n_targets < 1 || n_targets > kMaxTargets) fail("label columns must be in [1, %d], got %d", kMaxTargets, n_targets);
   if (n_targets > 1 && m->has_qgroups())
@@ -365,17 +259,14 @@ int B2_MatrixSetLabel(B2Handle mh, const float* values, int64_t rows, int32_t n_
   if (n_targets > 1 && (m->n_lower > 0 || m->n_upper > 0))
     fail("a label of %d columns on a matrix with label_lower_bound / label_upper_bound is not supported", n_targets);
   const int64_t len = rows * n_targets;
-  m->label.ensure((size_t)std::max<int64_t>(len, 1));
-  if (len > 0) CUDA_CHECK(cudaMemcpyAsync(m->label.p, values, len * sizeof(float), cudaMemcpyHostToDevice, m->ctx->stream));
-  CUDA_CHECK(cudaStreamSynchronize(m->ctx->stream));
+  set_field(m, m->label, values, len);
   m->n_label = len; m->n_targets = n_targets;
   m->rank_version++;
   API_END
 }
 int B2_MatrixSetGroups(B2Handle mh, const int32_t* group_sizes, int64_t n_groups) {
   API_BEGIN
-  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
-  CUDA_CHECK(cudaSetDevice(m->ctx->device));
+  Matrix* m = matrix_of(mh);
   if (n_groups < 0) fail("query groups: negative group count %lld", (long long)n_groups);
   if (n_groups > 0 && m->n_targets > 1)
     fail("query groups (qid) on a matrix with a label of %d columns are not supported", m->n_targets);
@@ -388,9 +279,7 @@ int B2_MatrixSetGroups(B2Handle mh, const int32_t* group_sizes, int64_t n_groups
   }
   if (n_groups > 0 && ptr[n_groups] != m->n)
     fail("query groups cover %lld rows, the matrix has %lld", (long long)ptr[n_groups], (long long)m->n);
-  m->qgroup_ptr.ensure(ptr.size());
-  CUDA_CHECK(cudaMemcpyAsync(m->qgroup_ptr.p, ptr.data(), ptr.size() * sizeof(int64_t), cudaMemcpyHostToDevice, m->ctx->stream));
-  CUDA_CHECK(cudaStreamSynchronize(m->ctx->stream));
+  set_field(m, m->qgroup_ptr, ptr.data(), (int64_t)ptr.size());
   m->h_qgroup_ptr = std::move(ptr);
   m->n_qgroups = n_groups; m->max_qgroup = mx;
   m->rank_version++;
@@ -417,9 +306,8 @@ int B2_MatrixNumCol(B2Handle mh, int32_t* out) { API_BEGIN *out = from_handle<Ma
 
 int B2_MatrixQuantize(B2Handle mh, B2Handle commh, int32_t max_bin, B2Handle refh, int32_t keep_raw) {
   API_BEGIN
-  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
-  CUDA_CHECK(cudaSetDevice(m->ctx->device));
-  Comm* comm = commh ? &from_handle<CommH>(commh, kComm, "communicator")->c : nullptr;
+  Matrix* m = matrix_of(mh);
+  Comm* comm = comm_of(commh);
   if (!m->has_raw) fail("matrix has no raw data on the device (already quantised without keep_raw?)");
   if (refh) {
     Matrix* r = from_handle<Matrix>(refh, kMatrix, "matrix");
@@ -427,20 +315,15 @@ int B2_MatrixQuantize(B2Handle mh, B2Handle commh, int32_t max_bin, B2Handle ref
     if (r->F != m->F) fail("reference matrix has %d features, this one %d", r->F, m->F);
     m->cut_ptrs = r->cut_ptrs; m->cut_vals = r->cut_vals; m->min_vals = r->min_vals; m->has_missing = r->has_missing; m->max_bin = r->max_bin;
     m->is_cat = r->is_cat; m->cat_feats = r->cat_feats;
-    check_borrowed_categories(m, comm);
-  } else {
-    make_cuts(m, comm, max_bin);
   }
-  bin_matrix(m);
-  if (!keep_raw) release_raw(m);
+  quantize_matrix(m, comm, max_bin, refh != 0, keep_raw != 0);
   API_END
 }
 int B2_MatrixQuantizeWithCuts(B2Handle mh, B2Handle commh, const int32_t* ptrs, const float* vals, const float* mins,
                               const uint8_t* has_missing, int32_t max_bin, int32_t keep_raw) {
   API_BEGIN
-  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
-  CUDA_CHECK(cudaSetDevice(m->ctx->device));
-  Comm* comm = commh ? &from_handle<CommH>(commh, kComm, "communicator")->c : nullptr;
+  Matrix* m = matrix_of(mh);
+  Comm* comm = comm_of(commh);
   if (!m->has_raw) fail("matrix has no raw data on the device (already quantised without keep_raw?)");
   if (max_bin < 2 || max_bin > 256) fail("max_bin must be in [2, 256] (uint8 bin matrix), got %d", max_bin);
   if (ptrs[0] != 0) fail("cut pointers must start at 0");
@@ -453,26 +336,20 @@ int B2_MatrixQuantizeWithCuts(B2Handle mh, B2Handle commh, const int32_t* ptrs, 
   m->min_vals.assign(mins, mins + m->F);
   m->has_missing.assign(has_missing, has_missing + m->F);
   m->max_bin = max_bin;
-  check_borrowed_categories(m, comm);
-  bin_matrix(m);
-  if (!keep_raw) release_raw(m);
+  quantize_matrix(m, comm, max_bin, true, keep_raw != 0);
   API_END
 }
 int B2_MatrixEnsureRaw(B2Handle mh, const float* data) {
   API_BEGIN
-  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
-  CUDA_CHECK(cudaSetDevice(m->ctx->device));
+  Matrix* m = matrix_of(mh);
   if (m->has_raw) return 0;
   if (m->csr) fail("the matrix was created from CSR arrays: re-upload them with B2_MatrixEnsureRawCSR");
-  m->raw.ensure((size_t)std::max<int64_t>(m->n * m->F, 1));
-  upload_pipelined(m->ctx, m->raw.p, data, (size_t)m->n * m->F * sizeof(float));
-  m->has_raw = true;
+  upload_raw(m, UploadSource{data});
   API_END
 }
 int B2_MatrixEnsureRawCSR(B2Handle mh, int64_t* indptr, const int32_t* indices, const float* values) {
   API_BEGIN
-  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
-  CUDA_CHECK(cudaSetDevice(m->ctx->device));
+  Matrix* m = matrix_of(mh);
   if (m->has_raw) return 0;
   if (!m->csr) fail("the matrix was created from dense rows: re-upload them with B2_MatrixEnsureRaw");
   upload_csr(m, indptr, indices, values);
@@ -502,8 +379,7 @@ int B2_MatrixGetCuts(B2Handle mh, int32_t* ptrs, float* vals, float* mins, uint8
 }
 int B2_MatrixGetBins(B2Handle mh, uint8_t* out) {
   API_BEGIN
-  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
-  CUDA_CHECK(cudaSetDevice(m->ctx->device));
+  Matrix* m = matrix_of(mh);
   if (!m->quantized) fail("matrix is not quantised");
   std::vector<uint8_t> h((size_t)m->n * m->row_stride);
   if (m->n > 0) CUDA_CHECK(cudaMemcpy(h.data(), m->bins.p, h.size(), cudaMemcpyDeviceToHost));
@@ -515,8 +391,7 @@ int B2_MatrixFree(B2Handle mh) {
   API_BEGIN
   Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
   cudaSetDevice(m->ctx->device);
-  { std::lock_guard<std::mutex> lk(g_matrix_mu); g_live_matrices.erase(m->uid); }
-  delete m;
+  free_matrix(m);
   API_END
 }
 
@@ -524,38 +399,7 @@ int B2_BoosterCreate(const char* params, B2Handle trainh, B2Handle commh, B2Hand
   API_BEGIN
   Matrix* m = trainh ? from_handle<Matrix>(trainh, kMatrix, "matrix") : nullptr;
   if (m && !m->quantized) fail("train matrix must be quantised (B2_MatrixQuantize) before B2_BoosterCreate");
-  Booster* b = new Booster(); b->kind = kBooster; b->train = m;
-  b->comm = commh ? &from_handle<CommH>(commh, kComm, "communicator")->c : nullptr;
-  try {
-    parse_params(params, &b->p, nullptr);
-    if (m) {
-      // the train matrix's label fixes the targets; a loaded model (num_target) must have as many
-      if (b->p.num_target_set && b->p.num_target != m->n_targets)
-        fail("the model has %d targets, the train matrix's label has %d columns", b->p.num_target, m->n_targets);
-      set_targets(&b->p, m->n_targets);
-      if (b->p.vector_leaf() && m->any_cat())
-        fail("multi_strategy=multi_output_tree is not supported with categorical features (the train matrix has %zu)",
-             m->cat_feats.size());
-      b->ctx = m->ctx; b->n_features = m->F; CUDA_CHECK(cudaSetDevice(m->ctx->device));
-      check_level_memory(b);
-      if (!b->p.interaction_sets.empty()) {   // sets_of[f] bit k: feature f is in set k
-        const int W = (int)((b->p.interaction_sets.size() + 63) / 64);
-        std::vector<unsigned long long> sets_of((size_t)m->F * W, 0ull);
-        for (size_t k = 0; k < b->p.interaction_sets.size(); ++k)
-          for (int64_t f : b->p.interaction_sets[k]) {
-            if (f >= m->F) fail("interaction_constraints: feature index %lld is out of range for %d features", (long long)f, m->F);
-            sets_of[(size_t)f * W + k / 64] |= 1ull << (k % 64);
-          }
-        upload(b->d_ic_sets_of, sets_of, m->ctx->stream);   // pageable source: staged before return
-        b->ic_words = W;
-      }
-    }
-    else {  // prediction-only booster (model loaded with B2_BoosterAddTree)
-      if (b->p.num_feature <= 0) fail("a booster without a train matrix needs num_feature=<n> in params");
-      b->ctx = get_ctx(b->p.device); b->n_features = b->p.num_feature;
-    }
-  } catch (...) { delete b; throw; }
-  *out = (B2Handle)b;
+  *out = (B2Handle)new_booster(params, m, comm_of(commh));
   API_END
 }
 int B2_BoosterUpdateOneIter(B2Handle bh, int32_t iter) {
@@ -586,8 +430,7 @@ int B2_BoosterRefreshOneIter(B2Handle bh, const float* grad, const float* hess, 
 }
 int B2_BoosterGetGradients(B2Handle bh, float* grad, float* hess, int64_t len) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
+  Booster* b = drained(bh);
   if (!b->train) fail("this booster has no train matrix (prediction-only)");
   const int64_t nk = b->train->n * b->p.num_class;
   if (len != nk) fail("gradient buffers have %lld values, expected %lld", (long long)len, (long long)nk);
@@ -600,145 +443,24 @@ int B2_BoosterGetGradients(B2Handle bh, float* grad, float* hess, int64_t len) {
   API_END
 }
 int B2_BoosterEvalSet(B2Handle bh, B2Handle mh, const char* metric, double* out) {
-  API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
-  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
-  CUDA_CHECK(cudaSetDevice(b->ctx->device));
-  *out = eval_metric(b, m, metric);
-  API_END
+  return with_matrix(bh, mh, [&](Booster* b, Matrix* m) { *out = eval_metric(b, m, metric); });
 }
 int B2_BoosterPredict(B2Handle bh, B2Handle mh, int32_t output_margin, int32_t tree_begin, int32_t tree_end, float* out,
                       int64_t out_len) {
-  API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
-  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
-  CUDA_CHECK(cudaSetDevice(b->ctx->device));
-  cudaStream_t s = b->ctx->stream; const int K = b->p.num_class;
-  if (out_len != m->n * K) fail("output buffer has %lld values, expected %lld", (long long)out_len, (long long)(m->n * K));
-  if (!m->has_raw) fail("prediction matrix has no raw data on the device (B2_MatrixEnsureRaw)");
-  if (m->F != b->n_features) fail("feature count mismatch: matrix has %d, model has %d", m->F, b->n_features);
-  const int nt = (int)b->trees.size();
-  if (tree_end <= 0 || tree_end > nt) tree_end = nt;
-  if (tree_begin < 0 || tree_begin > tree_end) fail("invalid tree range [%d, %d)", tree_begin, tree_end);
-  DevBuf<float> tmp; tmp.ensure((size_t)std::max<int64_t>(out_len, 1));
-  init_margin(b, tmp.p, m);
-  sync_device_trees(b);
-  predict_trees(b, m, tree_begin, tree_end, tmp.p);
-  if (!output_margin) LAUNCH_CHECK(b2_launch_transform(b->p.objective, K, tmp.p, m->n, b->ctx->num_sms, s));
-  if (out_len > 0) CUDA_CHECK(cudaMemcpyAsync(out, tmp.p, out_len * sizeof(float), cudaMemcpyDeviceToHost, s));
-  CUDA_CHECK(cudaStreamSynchronize(s));
-  API_END
+  return with_matrix(bh, mh, [&](Booster* b, Matrix* m) { predict(b, m, output_margin != 0, tree_begin, tree_end, out, out_len); });
 }
-// Common checks of the SHAP / leaf entries (the same as B2_BoosterPredict); resolves tree_end == 0 to all trees
-static void check_predict_args(Booster* b, Matrix* m, int32_t tree_begin, int32_t* tree_end) {
-  if (!m->has_raw) fail("prediction matrix has no raw data on the device (B2_MatrixEnsureRaw)");
-  if (m->F != b->n_features) fail("feature count mismatch: matrix has %d, model has %d", m->F, b->n_features);
-  const int nt = (int)b->trees.size();
-  if (*tree_end <= 0 || *tree_end > nt) *tree_end = nt;
-  if (tree_begin < 0 || tree_begin > *tree_end) fail("invalid tree range [%d, %d)", tree_begin, *tree_end);
-  if (m->n_base_margin > 0 && m->n_base_margin != m->n * b->p.num_class)
-    fail("base_margin has %lld values, expected %lld", (long long)m->n_base_margin, (long long)(m->n * b->p.num_class));
-}
-
-// rows per output block so that the device scratch of one block stays within 1 GiB whatever the row count
-static int64_t rows_per_block(int64_t n, size_t bytes_per_row) {
-  const size_t budget = (size_t)1 << 30;
-  int64_t r = (int64_t)std::max<size_t>(1, budget / std::max<size_t>(bytes_per_row, 1));
-  return std::max<int64_t>(1, std::min<int64_t>(r, n));
-}
-
 int B2_BoosterPredictContribs(B2Handle bh, B2Handle mh, int32_t tree_begin, int32_t tree_end, int32_t interactions, float* out,
                               int64_t out_len) {
-  API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
-  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
-  CUDA_CHECK(cudaSetDevice(b->ctx->device));
-  cudaStream_t s = b->ctx->stream; const int K = b->p.num_class; const int F = m->F;
-  const size_t per_row = (size_t)K * (F + 1) * (interactions ? (size_t)(F + 1) : 1);
-  if (b->p.vector_leaf())
-    fail("%s is not supported for vector-leaf trees (multi_strategy=multi_output_tree)",
-         interactions ? "pred_interactions" : "pred_contribs");
-  if (out_len != m->n * (int64_t)per_row) fail("output buffer has %lld values, expected %lld", (long long)out_len, (long long)(m->n * (int64_t)per_row));
-  check_predict_args(b, m, tree_begin, &tree_end);
-  build_paths(b);
-  std::vector<double> bias(K, 0.0);   // sum of the expected values of the trees in range, in tree order
-  for (int t = tree_begin; t < tree_end; ++t) bias[(t / std::max(1, b->p.num_parallel_tree)) % K] += b->tree_expected[t];
-  DevBuf<double> d_bias; upload(d_bias, bias, s);
-  const int p_begin = b->tree_path_offset[tree_begin], p_end = b->tree_path_offset[tree_end];
-  const float* bm = m->n_base_margin > 0 ? m->base_margin.p : nullptr;
-  const float base_value = base_margin_value(b->p);
-  // contributions: the row accumulators live in shared memory (up to 8 warps of K (F+1) doubles in <= 200 KiB),
-  // otherwise in global scratch; interactions always accumulate in global scratch
-  int warps = 8; size_t smem = 0;
-  if (!interactions) {
-    while (warps > 1 && b2_shap_contribs_smem(K, F, warps) > (size_t)200 * 1024) warps /= 2;
-    smem = b2_shap_contribs_smem(K, F, warps);
-    if (smem > (size_t)200 * 1024) { smem = 0; warps = 8; }
-  }
-  const bool gscratch = interactions || smem == 0;
-  const int64_t blk = std::min(rows_per_block(m->n, per_row * (sizeof(float) + (gscratch ? sizeof(double) : 0))), raw_tile_rows(m));
-  DevBuf<float> d_out, tile; DevBuf<double> d_acc;
-  d_out.ensure((size_t)std::max<int64_t>(blk, 1) * per_row);
-  if (gscratch) d_acc.ensure((size_t)std::max<int64_t>(blk, 1) * per_row);
-  std::vector<cudaEvent_t> ev;
-  for (int64_t r0 = 0; r0 < m->n; r0 += blk) {
-    const int64_t rows = std::min<int64_t>(blk, m->n - r0);
-    cudaEvent_t e0, e1; CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
-    ev.push_back(e0); ev.push_back(e1);
-    const float* X = raw_rows(m, r0, rows, tile);   // row 0 of X is row r0 of the matrix
-    const float* bm_rows = bm ? bm + (size_t)r0 * K : nullptr;
-    CUDA_CHECK(cudaEventRecord(e0, s));
-    if (interactions)
-      LAUNCH_CHECK(b2_launch_shap_interactions(X, 0, rows, F, m->missing, b->d_path_elems.p, b->d_paths.p, p_begin, p_end,
-                                               b->d_path_cats.p, K, d_bias.p, bm_rows, base_value, d_acc.p, d_out.p, b->ctx->num_sms, s));
-    else
-      LAUNCH_CHECK(b2_launch_shap_contribs(X, 0, rows, F, m->missing, b->d_path_elems.p, b->d_paths.p, p_begin, p_end,
-                                           b->d_path_cats.p, K, d_bias.p, bm_rows, base_value, gscratch ? d_acc.p : nullptr, warps,
-                                           smem, d_out.p, b->ctx->num_sms, s));
-    CUDA_CHECK(cudaEventRecord(e1, s));
-    CUDA_CHECK(cudaMemcpyAsync(out + (size_t)r0 * per_row, d_out.p, (size_t)rows * per_row * sizeof(float), cudaMemcpyDeviceToHost, s));
-  }
-  CUDA_CHECK(cudaStreamSynchronize(s));
-  for (size_t i = 0; i < ev.size(); i += 2) {
-    float ms = 0; cudaEventElapsedTime(&ms, ev[i], ev[i + 1]);
-    b->t.shap_ms += ms;
-    cudaEventDestroy(ev[i]); cudaEventDestroy(ev[i + 1]);
-  }
-  b->t.shap_rows += m->n;
-  API_END
+  return with_matrix(bh, mh, [&](Booster* b, Matrix* m) {
+    predict_contribs(b, m, tree_begin, tree_end, interactions != 0, out, out_len);
+  });
 }
-
 int B2_BoosterPredictLeaf(B2Handle bh, B2Handle mh, int32_t tree_begin, int32_t tree_end, float* out, int64_t out_len) {
-  API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
-  Matrix* m = from_handle<Matrix>(mh, kMatrix, "matrix");
-  CUDA_CHECK(cudaSetDevice(b->ctx->device));
-  cudaStream_t s = b->ctx->stream;
-  check_predict_args(b, m, tree_begin, &tree_end);
-  const int T = tree_end - tree_begin;
-  if (out_len != m->n * T) fail("output buffer has %lld values, expected %lld", (long long)out_len, (long long)(m->n * T));
-  if (T == 0 || m->n == 0) return 0;
-  sync_device_trees(b);
-  const int64_t blk = std::min(rows_per_block(m->n, (size_t)T * sizeof(float)), raw_tile_rows(m));
-  DevBuf<float> d_out, tile; d_out.ensure((size_t)blk * T);
-  for (int64_t r0 = 0; r0 < m->n; r0 += blk) {
-    const int64_t rows = std::min<int64_t>(blk, m->n - r0);
-    LAUNCH_CHECK(b2_launch_leaf_index(raw_rows(m, r0, rows, tile), 0, rows, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p,
-                                      b->d_cat_table.p, tree_begin, tree_end, d_out.p, b->ctx->num_sms, s));
-    CUDA_CHECK(cudaMemcpyAsync(out + (size_t)r0 * T, d_out.p, (size_t)rows * T * sizeof(float), cudaMemcpyDeviceToHost, s));
-  }
-  CUDA_CHECK(cudaStreamSynchronize(s));
-  API_END
+  return with_matrix(bh, mh, [&](Booster* b, Matrix* m) { predict_leaf(b, m, tree_begin, tree_end, out, out_len); });
 }
-
 int B2_BoosterGetTrainMargin(B2Handle bh, int32_t full, float* out, int64_t out_len) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
+  Booster* b = drained(bh);
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
   if (!b->train) fail("this booster has no train matrix (prediction-only)");
   const int64_t want = b->train->n * b->p.num_class;
@@ -754,8 +476,7 @@ int B2_BoosterGetTrainMargin(B2Handle bh, int32_t full, float* out, int64_t out_
 }
 int B2_BoosterResetTrainMargin(B2Handle bh) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
+  Booster* b = drained(bh);
   CUDA_CHECK(cudaSetDevice(b->ctx->device));
   if (!b->train) fail("this booster has no train matrix (prediction-only)");
   b->margin_ready = false;
@@ -778,27 +499,21 @@ int B2_BoosterNumTargets(B2Handle bh, int32_t* out) {
 }
 int B2_BoosterNumTrees(B2Handle bh, int32_t* out) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
+  Booster* b = drained(bh);
   *out = (int32_t)b->trees.size();
   API_END
 }
 int B2_BoosterTreeNumNodes(B2Handle bh, int32_t tree, int32_t* out) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
-  if (tree < 0 || tree >= (int)b->trees.size()) fail("tree index %d out of range", tree);
-  *out = b->trees[tree].size();
+  *out = tree_at(drained(bh), tree).size();
   API_END
 }
 int B2_BoosterGetTree(B2Handle bh, int32_t tree, int32_t* left, int32_t* right, int32_t* parent, int32_t* split_feature,
                       int32_t* split_bin, float* split_cond, uint8_t* default_left, float* value, float* base_weight,
                       float* loss_chg, double* sum_hess) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
-  if (tree < 0 || tree >= (int)b->trees.size()) fail("tree index %d out of range", tree);
-  const TreeHost& t = b->trees[tree]; const size_t n = t.size();
+  Booster* b = drained(bh);
+  const TreeHost& t = tree_at(b, tree); const size_t n = t.size();
   memcpy(left, t.left.data(), n * 4); memcpy(right, t.right.data(), n * 4); memcpy(parent, t.parent.data(), n * 4);
   memcpy(split_feature, t.feature.data(), n * 4); memcpy(split_bin, t.split_bin.data(), n * 4);
   memcpy(split_cond, t.cond.data(), n * 4); memcpy(default_left, t.default_left.data(), n);
@@ -811,8 +526,7 @@ int B2_BoosterAddTree(B2Handle bh, int32_t n_nodes, const int32_t* left, const i
                       const uint8_t* default_left, const float* value, const float* base_weight, const float* loss_chg,
                       const double* sum_hess) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
+  Booster* b = drained(bh);
   if (b->update_started) fail("process_type=update: trees are added before the first refresh round, not after");
   if (n_nodes < 1) fail("a tree needs at least one node");
   TreeHost t;
@@ -832,16 +546,14 @@ int B2_BoosterAddTree(B2Handle bh, int32_t n_nodes, const int32_t* left, const i
 }
 int B2_BoosterGetTreeWeights(B2Handle bh, float* out, int64_t len) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
+  Booster* b = drained(bh);
   if (len != (int64_t)b->trees.size()) fail("weight buffer has %lld values for %zu trees", (long long)len, b->trees.size());
   for (int64_t t = 0; t < len; ++t) out[t] = b->p.dart ? b->tree_w[t] : 1.0f;
   API_END
 }
 int B2_BoosterSetTreeWeights(B2Handle bh, const float* w, int64_t len) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
+  Booster* b = drained(bh);
   if (!b->p.dart) fail("tree weights belong to booster=dart; this booster is gbtree");
   if (len != (int64_t)b->trees.size()) fail("%lld tree weights for %zu trees", (long long)len, b->trees.size());
   float S = 0.0f;   // the binary32 sum sample_type=weighted divides by (dart_drop_set)
@@ -858,34 +570,27 @@ int B2_BoosterSetTreeWeights(B2Handle bh, const float* w, int64_t len) {
 }
 int B2_BoosterGetTreeCategories(B2Handle bh, int32_t tree, uint8_t* split_type, uint32_t* cat_bits) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
-  if (tree < 0 || tree >= (int)b->trees.size()) fail("tree index %d out of range", tree);
-  const TreeHost& t = b->trees[tree]; const size_t n = t.size();
+  Booster* b = drained(bh);
+  const TreeHost& t = tree_at(b, tree); const size_t n = t.size();
   memcpy(split_type, t.split_type.data(), n); memcpy(cat_bits, t.cat_bits.data(), n * 8 * sizeof(uint32_t));
   API_END
 }
 int B2_BoosterSetTreeCategories(B2Handle bh, int32_t tree, const uint8_t* split_type, const uint32_t* cat_bits) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
-  if (tree < 0 || tree >= (int)b->trees.size()) fail("tree index %d out of range", tree);
-  TreeHost& t = b->trees[tree]; const size_t n = t.size();
+  Booster* b = drained(bh);
+  TreeHost& t = tree_at(b, tree); const size_t n = t.size();
   for (size_t i = 0; i < n; ++i) {
     t.split_type[i] = split_type[i] ? 1 : 0;
     if (t.split_type[i]) t.any_cat = true;
     for (int w8 = 0; w8 < 8; ++w8) t.cat_bits[i * 8 + w8] = split_type[i] ? cat_bits[i * 8 + w8] : 0u;
   }
-  b->d_trees_synced = 0; b->paths_synced = -1; b->margin_ready = false;
-  for (auto& kv : b->eval_cache) if (kv.second) kv.second->n_trees_applied = 0, kv.second->n = -1;
+  trees_edited(b);
   API_END
 }
 int B2_BoosterGetTreeLeafVector(B2Handle bh, int32_t tree, float* out, int64_t len) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
-  if (tree < 0 || tree >= (int)b->trees.size()) fail("tree index %d out of range", tree);
-  const TreeHost& t = b->trees[tree];
+  Booster* b = drained(bh);
+  const TreeHost& t = tree_at(b, tree);
   if (t.leaf_vec.empty()) fail("tree %d is not a vector-leaf tree", tree);
   if (len != (int64_t)t.leaf_vec.size()) fail("leaf vector buffer has %lld values, tree %d has %zu", (long long)len, tree, t.leaf_vec.size());
   memcpy(out, t.leaf_vec.data(), t.leaf_vec.size() * sizeof(float));
@@ -893,25 +598,21 @@ int B2_BoosterGetTreeLeafVector(B2Handle bh, int32_t tree, float* out, int64_t l
 }
 int B2_BoosterSetTreeLeafVector(B2Handle bh, int32_t tree, const float* v, int64_t len) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
-  if (tree < 0 || tree >= (int)b->trees.size()) fail("tree index %d out of range", tree);
+  Booster* b = drained(bh);
+  TreeHost& t = tree_at(b, tree);
   if (!b->p.vector_leaf())
     fail("this booster grows single-output trees (multi_strategy=one_output_per_tree, %d target(s)); a vector-leaf tree "
          "needs multi_strategy=multi_output_tree and num_target > 1", b->p.num_target);
-  TreeHost& t = b->trees[tree];
   const int64_t want = (int64_t)t.size() * b->p.num_target;
   if (len != want) fail("leaf vector has %lld values, tree %d needs %lld (%d nodes x %d targets)", (long long)len, tree,
                         (long long)want, t.size(), b->p.num_target);
   t.leaf_vec.assign(v, v + len);
-  b->d_trees_synced = 0; b->margin_ready = false;
-  for (auto& kv : b->eval_cache) if (kv.second) kv.second->n_trees_applied = 0, kv.second->n = -1;
+  trees_edited(b);
   API_END
 }
 int B2_BoosterGetTimers(B2Handle bh, int32_t reset, char* out, int64_t out_cap) {
   API_BEGIN
-  Booster* b = from_handle<Booster>(bh, kBooster, "booster");
-  drain_round(b);
+  Booster* b = drained(bh);
   const Timers& t = b->t;
   snprintf(out, (size_t)out_cap,
            "{\"hist_ms\": %.6f, \"hist_launches\": %lld, \"hist_rows\": %lld, \"hist_bytes\": %.1f, \"kernel_launches\": %lld, "

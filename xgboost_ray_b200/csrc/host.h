@@ -8,12 +8,12 @@
 //   smaller-child hist -> allreduce -> sibling subtraction -> ... -> leaf sums -> margin update.
 //
 // device.cu   device context, memory pool, pinned upload pipeline, NCCL
-// matrix.cu   matrix registry, cuts, binning
+// matrix.cu   matrix construction, registry and interleaved NVLink ingest, cuts, binning
 // params.cu   parameter parsing, the objective table (kObjectives), metric names
 // tree.cu     growing one tree (scalar or vector-leaf) and reading it back
-// round.cu    a boosting round: label checks, gradients, base_score, DART, refresh, the round pipeline
-// predict.cu  TreeSHAP paths, prediction, evaluation margins and eval metrics
-// engine.cu   the C ABI (include/b2hist.h)
+// round.cu    booster setup and a boosting round: label checks, gradients, base_score, DART, refresh, the round pipeline
+// predict.cu  model caches, TreeSHAP paths, prediction, contributions, leaf indices, evaluation margins, eval metrics
+// engine.cu   the C ABI (include/b2hist.h): handle lookups, then one call into the files above
 //
 // Everything is in namespace b2host, and every file opens it with hidden visibility, so the library exports no symbol
 // of the host layer: only the C ABI of engine.cu reaches it.
@@ -25,6 +25,7 @@
 #include <algorithm>
 #include <atomic>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <set>
 #include <string>
@@ -156,11 +157,6 @@ T* from_handle(B2Handle h, int kind, const char* what) {
   return reinterpret_cast<T*>(h);
 }
 
-// the matrix registry (matrix.cu)
-extern std::mutex g_matrix_mu;
-extern std::set<uint64_t> g_live_matrices;
-extern uint64_t g_next_matrix_uid;
-
 struct Matrix : HandleBase {
   uint64_t margin_version = 0;   // bumped when base_margin changes (cached evaluation margins start from it)
   uint64_t uid = 0;       // unique for the life of the process; 0 = not registered (stack temporaries)
@@ -211,10 +207,22 @@ struct Matrix : HandleBase {
 };
 
 template <typename T>
-void upload(DevBuf<T>& d, const std::vector<T>& h, cudaStream_t s) {
-  d.ensure(h.size() ? h.size() : 1);
-  if (!h.empty()) CUDA_CHECK(cudaMemcpyAsync(d.p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, s));
+void upload(DevBuf<T>& d, const T* h, size_t n, cudaStream_t s) {
+  d.ensure(n ? n : 1);
+  if (n) CUDA_CHECK(cudaMemcpyAsync(d.p, h, n * sizeof(T), cudaMemcpyHostToDevice, s));
 }
+template <typename T>
+void upload(DevBuf<T>& d, const std::vector<T>& h, cudaStream_t s) { upload(d, h.data(), h.size(), s); }
+
+// ---- matrix lifecycle (matrix.cu).  new_matrix refuses a bad shape or more rows than int32 ids; the caller sets ctx
+std::unique_ptr<Matrix> new_matrix(int64_t n, int F, float missing);
+B2Handle register_matrix(std::unique_ptr<Matrix> m);   // gives m its uid; the handle is released by free_matrix
+void free_matrix(Matrix* m);
+bool matrix_alive(uint64_t uid);
+void upload_raw(Matrix* m, const UploadSource& u);    // raw: the n x F values of u
+// B2_MatrixCreateFromProcessInterleaved: rows r = rank (mod world) of a remote matrix, exchanged over NVLink when it can
+B2Handle ingest_interleaved(Comm* c, int64_t pid, uint64_t remote_addr, int64_t n_total_rows, int n_cols, int shard_rank,
+                            float missing, int device);
 
 // ---- raw rows (matrix.cu): the one place that knows whether a matrix holds its raw values dense or as CSR
 constexpr size_t kRawTileBytes = (size_t)256 << 20;   // largest dense tile densified from a CSR matrix
@@ -223,12 +231,12 @@ constexpr size_t kRawTileBytes = (size_t)256 << 20;   // largest dense tile dens
 int64_t raw_tile_rows(const Matrix* m);
 // dense float rows [r0, r0 + rows) x [0, F): a pointer into raw, or `tile` filled from the CSR (rows <= raw_tile_rows)
 const float* raw_rows(Matrix* m, int64_t r0, int64_t rows, DevBuf<float>& tile);
-// fn(X, r0, rows) over consecutive raw tiles covering every row (once with rows = 0 for an empty matrix).  A dense
-// matrix is one call with X = raw: the kernels run exactly as on a plain dense matrix.
+// fn(X, r0, rows) over consecutive raw tiles of at most max_rows rows covering every row (once with rows = 0 for an
+// empty matrix).  Uncapped, a dense matrix is one call with X = raw: the kernels run as on a plain dense matrix.
 template <typename Fn>
-void for_raw_tiles(Matrix* m, Fn fn) {
+void for_raw_tiles(Matrix* m, Fn fn, int64_t max_rows = INT64_MAX) {
   DevBuf<float> tile;
-  const int64_t step = raw_tile_rows(m);
+  const int64_t step = std::min(raw_tile_rows(m), max_rows);
   int64_t r0 = 0;
   do {
     const int64_t rows = std::min<int64_t>(step, m->n - r0);
@@ -237,13 +245,11 @@ void for_raw_tiles(Matrix* m, Fn fn) {
   } while (r0 < m->n);
 }
 void upload_csr(Matrix* m, const int64_t* indptr, const int32_t* indices, const float* values);
-void release_raw(Matrix* m);
 size_t matrix_device_bytes(const Matrix* m);
 
 void setup_groups(Matrix* m);
-void check_borrowed_categories(Matrix* m, Comm* comm);
-void make_cuts(Matrix* m, Comm* comm, int max_bin);
-void bin_matrix(Matrix* m);
+// cuts (sketched, or borrowed ones checked against the categorical codes), the bin matrix, raw released unless keep_raw
+void quantize_matrix(Matrix* m, Comm* comm, int max_bin, bool borrowed_cuts, bool keep_raw);
 
 // ---------------------------------------------------------------- booster
 constexpr int kMaxTargets = 4096;   // label columns of one matrix (as many trees per round as num_parallel_tree allows)
@@ -385,10 +391,11 @@ struct Booster : HandleBase {
   std::vector<TreeHost> trees;
   std::atomic<bool> cancel{false};
   // device model cache for prediction
+  // d_trees_synced / paths_synced: the number of trees a cache was built from, -1 = stale (trees_edited)
   DevBuf<B2TreeNodeDev> d_nodes; DevBuf<int32_t> d_tree_offset; int d_trees_synced = 0;
   std::vector<B2TreeNodeDev> h_nodes; std::vector<int32_t> h_tree_offset;
   DevBuf<uint32_t> d_cat_table; std::vector<uint32_t> h_cat_table;   // [categorical nodes][8]
-  // TreeSHAP path table (build_paths), rebuilt when the tree set changes (paths_synced = trees it was built from, -1 = stale)
+  // TreeSHAP path table (build_paths), rebuilt when the tree set changes
   DevBuf<B2PathElem> d_path_elems; DevBuf<B2PathInfo> d_paths; DevBuf<uint32_t> d_path_cats;
   std::vector<int32_t> tree_path_offset;   // [trees + 1]: paths of tree t are [offset[t], offset[t+1])
   std::vector<double> tree_expected;       // [trees] cover-weighted mean of the leaves (the tree's SHAP bias)
@@ -591,12 +598,19 @@ void ensure_rank_disc(Booster* b, int64_t len);
 void drain_round(Booster* b);
 void ensure_train_margin(Booster* b);
 void dart_prepare(Booster* b);
+Booster* new_booster(const char* params, Matrix* m, Comm* comm);
 void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64_t len);
 
 // ---------------------------------------------------------------- predict.cu
+// an existing tree changed: every cache derived from b->trees is stale (-1, never a tree count; appends are incremental)
+void trees_edited(Booster* b);
 void build_paths(Booster* b);
 void predict_trees(Booster* b, Matrix* m, int tree_begin, int tree_end, float* out);
 float* eval_margin(Booster* b, Matrix* m);
 double eval_metric(Booster* b, Matrix* m, const char* name);
+// B2_BoosterPredict, B2_BoosterPredictContribs, B2_BoosterPredictLeaf: tree_end <= 0 means every tree
+void predict(Booster* b, Matrix* m, bool output_margin, int tree_begin, int tree_end, float* out, int64_t out_len);
+void predict_contribs(Booster* b, Matrix* m, int tree_begin, int tree_end, bool interactions, float* out, int64_t out_len);
+void predict_leaf(Booster* b, Matrix* m, int tree_begin, int tree_end, float* out, int64_t out_len);
 
 }  // namespace b2host

@@ -1,7 +1,11 @@
-// matrix.cu -- the matrix registry, the feature -> group layout of the bin matrix, the GPU sketch that makes the cuts,
-// the checks of categorical codes, and the binning of the raw values.
+// matrix.cu -- the matrix lifecycle (construction, the registry, the interleaved NVLink ingest), the feature -> group
+// layout of the bin matrix, the GPU sketch that makes the cuts, the checks of categorical codes, and the binning of the
+// raw values.
+#include <stdio.h>
+#include <stdlib.h>
 #include <string.h>
 
+#include <chrono>
 #include <climits>
 
 #include "host.h"
@@ -11,9 +15,145 @@ namespace b2host __attribute__((visibility("hidden"))) {
 
 // ids of the matrices that are alive: a Booster's evaluation cache is keyed by the id, never by the address (a freed
 // matrix and a new one of the same shape can share an address)
-std::mutex g_matrix_mu;
-std::set<uint64_t> g_live_matrices;
-uint64_t g_next_matrix_uid = 1;
+static std::mutex g_matrix_mu;
+static std::set<uint64_t> g_live_matrices;
+static uint64_t g_next_matrix_uid = 1;
+std::unique_ptr<Matrix> new_matrix(int64_t n, int F, float missing) {
+  if (n < 0 || F <= 0) fail("invalid matrix shape %lld x %d", (long long)n, F);
+  if (n >= (1LL << 31)) fail("at most 2^31-1 rows per GPU shard (row ids are int32), got %lld", (long long)n);
+  std::unique_ptr<Matrix> m(new Matrix());
+  m->kind = kMatrix; m->n = n; m->F = F; m->missing = missing;
+  return m;
+}
+B2Handle register_matrix(std::unique_ptr<Matrix> m) {
+  { std::lock_guard<std::mutex> lk(g_matrix_mu); m->uid = g_next_matrix_uid++; g_live_matrices.insert(m->uid); }
+  return (B2Handle)m.release();
+}
+void free_matrix(Matrix* m) {
+  { std::lock_guard<std::mutex> lk(g_matrix_mu); g_live_matrices.erase(m->uid); }
+  delete m;
+}
+bool matrix_alive(uint64_t uid) { std::lock_guard<std::mutex> lk(g_matrix_mu); return g_live_matrices.count(uid) != 0; }
+
+void upload_raw(Matrix* m, const UploadSource& u) {
+  m->raw.ensure((size_t)std::max<int64_t>(m->n * m->F, 1));
+  upload_pipelined(m->ctx, m->raw.p, u, (size_t)m->n * m->F * sizeof(float));
+  m->has_raw = true;
+}
+
+// Staging block of the interleaved ingest: persistent per device (grow-only), exported ONCE; the peers keep their mapping
+// of it across calls (mapping / unmapping a multi-GB allocation costs more than moving the rows).  A block that had to
+// grow is retired and freed only after the call's closing barrier, when every peer has dropped its mapping of it.
+struct IngestStage { float* p = nullptr; size_t bytes = 0; cudaIpcMemHandle_t h; bool exported = false; };
+static IngestStage g_ingest_stage[64];
+static std::map<std::string, void*> g_peer_stage;      // handle bytes -> mapped pointer (this process)
+static std::mutex g_ingest_mu;
+static double wall_seconds() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+
+B2Handle ingest_interleaved(Comm* c, int64_t pid, uint64_t remote_addr, int64_t n_total_rows, int n_cols, int shard_rank,
+                            float missing, int device) {
+  if (!c || c->world < 2 || c->world > B2_P2P_MAX_WORLD) fail("interleaved remote ingest needs a communicator of 2..%d ranks", B2_P2P_MAX_WORLD);
+  const int W = c->world, rank = c->rank;
+  Ctx* ctx = get_ctx(device); cudaStream_t s = ctx->stream;
+  static const bool timing = getenv("B2_INGEST_TIMING") && atoi(getenv("B2_INGEST_TIMING")) != 0;
+  double t0 = wall_seconds(), t_prev = t0;
+  auto lap = [&](const char* what) {
+    if (!timing) return;
+    const double t = wall_seconds();
+    fprintf(stderr, "[b2 ingest rank %d] %-28s %.4f s\n", rank, what, t - t_prev);
+    t_prev = t;
+  };
+  std::lock_guard<std::mutex> ingest_lock(g_ingest_mu);
+  // contiguous block of this rank (BATCH split of the global rows) and the rows it finally owns (INTERLEAVED)
+  B2RowBlocks rb; memset(&rb, 0, sizeof(rb));
+  const int64_t per = n_total_rows / W, extra = n_total_rows % W;
+  for (int w = 0; w <= W; ++w) rb.start[w] = (long long)(w * per + std::min<int64_t>(w, extra));
+  const int64_t b0 = rb.start[rank], bn = rb.start[rank + 1] - b0;
+  const int64_t n_mine = rank < n_total_rows ? (n_total_rows - rank + W - 1) / W : 0;
+  std::unique_ptr<Matrix> m = new_matrix(n_mine, n_cols, missing);
+  m->ctx = ctx;
+  rb.world = W; rb.rank = rank; rb.n_cols = n_cols; rb.n_mine = (long long)n_mine;
+  DevBuf<int32_t> d_flag; d_flag.ensure(1);
+  auto any_rank = [&](int32_t mine) {   // max over the ranks of a flag
+    CUDA_CHECK(cudaMemcpyAsync(d_flag.p, &mine, sizeof(mine), cudaMemcpyHostToDevice, s));
+    allreduce(c, d_flag.p, 1, kNcclInt32, kNcclMax, s);
+    CUDA_CHECK(cudaMemcpyAsync(&mine, d_flag.p, sizeof(mine), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    return mine;
+  };
+  // collective call: every rank must hold the shard of its own rank, or all of them fail together
+  if (any_rank(shard_rank == rank ? 0 : 1))
+    fail("interleaved remote ingest: shard %d handed to rank %d (or a mismatch on another rank)", shard_rank, rank);
+  lap("agreement");
+  void* retired = nullptr;
+  try {
+    IngestStage& st = g_ingest_stage[(device >= 0 && device < 64) ? device : 0];
+    const size_t need = (size_t)std::max<int64_t>(bn * n_cols, 1) * sizeof(float);
+    int ok = 1;
+    if (st.bytes < need) {
+      retired = st.p; st.p = nullptr; st.bytes = 0; st.exported = false;
+      const size_t want = (need + need / 16 + ((size_t)1 << 20)) & ~(((size_t)1 << 20) - 1);
+      void* q = nullptr;
+      if (cudaMalloc(&q, want) != cudaSuccess) {
+        cudaGetLastError();
+        { std::lock_guard<std::mutex> lk(g_dev_pool[(device >= 0 && device < 64) ? device : 0].mu); pool_trim(g_dev_pool[(device >= 0 && device < 64) ? device : 0], 0); }
+        if (cudaMalloc(&q, want) != cudaSuccess) { cudaGetLastError(); fail("cudaMalloc of the %zu-byte ingest staging block failed", want); }
+      }
+      st.p = (float*)q; st.bytes = want;
+    }
+    if (!st.exported) {
+      if (cudaIpcGetMemHandle(&st.h, st.p) == cudaSuccess) st.exported = true;
+      else { ok = 0; cudaGetLastError(); memset(&st.h, 0, sizeof(st.h)); }
+    }
+    lap("staging block");
+    UploadSource u; u.pid = pid; u.remote_addr = remote_addr + (uint64_t)b0 * (uint64_t)n_cols * 4u; u.row_bytes = (size_t)n_cols * 4; u.row_stride = u.row_bytes;
+    upload_pipelined(ctx, st.p, u, (size_t)bn * n_cols * sizeof(float));
+    lap("read block from the driver");
+    m->raw.ensure((size_t)std::max<int64_t>(n_mine * n_cols, 1));
+    // exchange the IPC handles of the staging blocks (also: every rank's block is uploaded)
+    DevBuf<uint8_t> d_mine, d_all; d_mine.ensure(sizeof(st.h)); d_all.ensure(sizeof(st.h) * (size_t)W);
+    CUDA_CHECK(cudaMemcpyAsync(d_mine.p, &st.h, sizeof(st.h), cudaMemcpyHostToDevice, s));
+    NCCL_CHECK(nccl()->AllGather(d_mine.p, d_all.p, sizeof(st.h), kNcclUint8, c->comm, s));
+    std::vector<cudaIpcMemHandle_t> all((size_t)W);
+    CUDA_CHECK(cudaMemcpyAsync(all.data(), d_all.p, sizeof(st.h) * (size_t)W, cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    lap("handle exchange");
+    // drop mappings of blocks that no peer exports any more (a peer's block grew), then map what is new
+    std::set<std::string> current;
+    for (int w = 0; w < W; ++w) if (w != rank) current.insert(std::string((const char*)&all[w], sizeof(all[w])));
+    for (auto it = g_peer_stage.begin(); it != g_peer_stage.end();) {
+      if (!current.count(it->first)) { cudaIpcCloseMemHandle(it->second); it = g_peer_stage.erase(it); } else ++it;
+    }
+    for (int w = 0; w < W && ok; ++w) {
+      if (w == rank) { rb.base[w] = st.p; continue; }
+      const std::string key((const char*)&all[w], sizeof(all[w]));
+      auto it = g_peer_stage.find(key);
+      if (it == g_peer_stage.end()) {
+        void* q = nullptr;
+        if (cudaIpcOpenMemHandle(&q, all[w], cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { ok = 0; cudaGetLastError(); break; }
+        it = g_peer_stage.emplace(key, q).first;
+      }
+      rb.base[w] = (const float*)it->second;
+    }
+    lap("peer mappings");
+    if (any_rank(ok ? 0 : 1)) {
+      // no peer mapping on some rank (no NVLink / IPC): every rank reads its own strided shard from the driver instead
+      UploadSource us; us.pid = pid; us.remote_addr = remote_addr + (uint64_t)rank * (uint64_t)n_cols * 4u;
+      us.row_bytes = (size_t)n_cols * 4; us.row_stride = us.row_bytes * (size_t)W;
+      upload_pipelined(ctx, m->raw.p, us, (size_t)n_mine * n_cols * sizeof(float));
+    } else {
+      LAUNCH_CHECK(b2_launch_gather_interleaved_rows(&rb, m->raw.p, ctx->num_sms, s));
+    }
+    // nobody overwrites (next call) or frees (a retired block) its staging block while a peer may still pull rows out of it
+    any_rank(0);
+    lap("row gather + closing barrier");
+    if (retired) { cudaFree(retired); retired = nullptr; }
+  } catch (...) { if (retired) cudaFree(retired); throw; }
+  m->has_raw = true;
+  const B2Handle h = register_matrix(std::move(m));
+  if (timing) fprintf(stderr, "[b2 ingest rank %d] total %.4f s (%lld of %lld rows x %d)\n", rank, wall_seconds() - t0, (long long)n_mine, (long long)n_total_rows, n_cols);
+  return h;
+}
 
 // Feature -> (group, slot) layout of the bin matrix: the features are spread EVENLY over ceil(F / 32) groups, so that
 // every CTA type of the histogram kernel (one pair of groups) costs the same and the types walk the chunk list in lock
@@ -92,7 +232,7 @@ void upload_csr(Matrix* m, const int64_t* indptr, const int32_t* indices, const 
   m->has_raw = true;
 }
 
-void release_raw(Matrix* m) {
+static void release_raw(Matrix* m) {
   m->raw.release();
   m->csr_indptr.release(); m->csr_indices.release(); m->csr_values.release();
   m->has_raw = false;
@@ -164,7 +304,7 @@ double category_key_value(int32_t key) {
 // they do not know to their largest code (a negative one to 0), and a code of 255 shares bin 255 with the missing
 // values, while prediction sends every unknown code left: training would see another category than predict().
 // Such codes are refused, as make_cuts refuses codes that are not valid, instead of silently changing the model.
-void check_borrowed_categories(Matrix* m, Comm* comm) {
+static void check_borrowed_categories(Matrix* m, Comm* comm) {
   const std::vector<int32_t> h_cat = category_stats(m, comm);
   for (size_t i = 0; i < m->cat_feats.size(); ++i) {
     const int f = m->cat_feats[i], mx = h_cat[i * 3], miss = h_cat[i * 3 + 1];
@@ -189,7 +329,7 @@ void check_borrowed_categories(Matrix* m, Comm* comm) {
 // Multi-GPU: the column keys of every rank are allgathered (padded to the largest shard); feature f is
 // sorted and pruned only by its owner rank f % world, and the cut tables are merged with one integer
 // allreduce (non-owners contribute zeros), so every rank ends up with identical global cuts.
-void make_cuts(Matrix* m, Comm* comm, int max_bin) {
+static void make_cuts(Matrix* m, Comm* comm, int max_bin) {
   Ctx* ctx = m->ctx; cudaStream_t s = ctx->stream;
   if (max_bin < 2 || max_bin > 256) fail("max_bin must be in [2, 256] (uint8 bin matrix), got %d", max_bin);
   if (!m->has_raw) fail("matrix has no raw data to sketch");
@@ -308,7 +448,7 @@ void make_cuts(Matrix* m, Comm* comm, int max_bin) {
   m->max_bin = max_bin;
 }
 
-void bin_matrix(Matrix* m) {
+static void bin_matrix(Matrix* m) {
   Ctx* ctx = m->ctx; cudaStream_t s = ctx->stream;
   setup_groups(m);
   upload_cuts(m);
@@ -325,6 +465,13 @@ void bin_matrix(Matrix* m) {
   });
   CUDA_CHECK(cudaStreamSynchronize(s));
   m->quantized = true;
+}
+
+void quantize_matrix(Matrix* m, Comm* comm, int max_bin, bool borrowed_cuts, bool keep_raw) {
+  if (borrowed_cuts) check_borrowed_categories(m, comm);
+  else make_cuts(m, comm, max_bin);
+  bin_matrix(m);
+  if (!keep_raw) release_raw(m);
 }
 
 }  // namespace b2host

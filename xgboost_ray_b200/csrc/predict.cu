@@ -7,6 +7,11 @@
 
 namespace b2host __attribute__((visibility("hidden"))) {
 
+void trees_edited(Booster* b) {
+  b->d_trees_synced = -1; b->paths_synced = -1; b->margin_ready = false;
+  for (auto& kv : b->eval_cache) if (kv.second) kv.second->n_trees_applied = 0, kv.second->n = -1;
+}
+
 // ---- TreeSHAP path table (common.cuh B2PathElem / B2PathInfo; shap_kernel.cu).  Walks every tree root -> leaf; on the
 // way each split is merged into the element of its feature (appended the first time the feature is seen): the interval
 // of a numeric feature narrows, the category set of a categorical feature is intersected with the side taken (keeping
@@ -102,8 +107,9 @@ const float* device_weights(Booster* b) {
   return b->d_tree_w.p;
 }
 
-// out += the trees [tree_begin, tree_end) on the raw rows of m (the device trees are in sync)
+// out += the trees [tree_begin, tree_end) on the raw rows of m
 void predict_trees(Booster* b, Matrix* m, int tree_begin, int tree_end, float* out) {
+  sync_device_trees(b);
   const float* w = b->p.vector_leaf() ? nullptr : device_weights(b);
   for_raw_tiles(m, [&](const float* X, int64_t r0, int64_t rows) {
     if (b->p.vector_leaf())
@@ -122,11 +128,9 @@ float* eval_margin(Booster* b, Matrix* m) {
   if (b->train && m == b->train) { ensure_train_margin(b); return b->margin.p; }
   if (!m->has_raw) fail("evaluation / prediction matrix has no raw data on the device");
   if (m->F != b->n_features) fail("feature count mismatch: matrix has %d, model has %d", m->F, b->n_features);
-  {   // drop the cached margins of matrices that were freed since the last call
-    std::lock_guard<std::mutex> lk(g_matrix_mu);
-    for (auto it = b->eval_cache.begin(); it != b->eval_cache.end();) {
-      if (!g_live_matrices.count(it->first)) { delete it->second; it = b->eval_cache.erase(it); } else ++it;
-    }
+  // drop the cached margins of matrices that were freed since the last call
+  for (auto it = b->eval_cache.begin(); it != b->eval_cache.end();) {
+    if (!matrix_alive(it->first)) { delete it->second; it = b->eval_cache.erase(it); } else ++it;
   }
   if (!m->uid) fail("evaluation matrix is not a registered matrix handle");
   EvalCache*& c = b->eval_cache[m->uid];
@@ -139,7 +143,6 @@ float* eval_margin(Booster* b, Matrix* m) {
   }
   const int nt = (int)b->trees.size();
   if (c->n_trees_applied < nt) {
-    sync_device_trees(b);
     predict_trees(b, m, c->n_trees_applied, nt, c->margin.p);
     c->n_trees_applied = nt;
   }
@@ -258,6 +261,108 @@ double eval_metric(Booster* b, Matrix* m, const char* name) {
   }
   const std::vector<double> h = metric_sums(b, 2, s);   // ranking, aft and quantile: (sum, weight sum)
   return h[1] > 0 ? h[0] / h[1] : 0.0;
+}
+
+// the checks every prediction entry makes (each checks its output length where it can); resolves tree_end <= 0 to all trees
+static void check_predict_args(Booster* b, Matrix* m, int tree_begin, int* tree_end) {
+  if (!m->has_raw) fail("prediction matrix has no raw data on the device (B2_MatrixEnsureRaw)");
+  if (m->F != b->n_features) fail("feature count mismatch: matrix has %d, model has %d", m->F, b->n_features);
+  const int nt = (int)b->trees.size();
+  if (*tree_end <= 0 || *tree_end > nt) *tree_end = nt;
+  if (tree_begin < 0 || tree_begin > *tree_end) fail("invalid tree range [%d, %d)", tree_begin, *tree_end);
+  if (m->n_base_margin > 0 && m->n_base_margin != m->n * b->p.num_class)
+    fail("base_margin has %lld values, expected %lld", (long long)m->n_base_margin, (long long)(m->n * b->p.num_class));
+}
+
+// rows per output block, so that the device scratch of one block stays within 1 GiB whatever the row count, and within
+// one raw tile
+static int64_t rows_per_block(Matrix* m, size_t bytes_per_row) {
+  const size_t budget = (size_t)1 << 30;
+  int64_t r = (int64_t)std::max<size_t>(1, budget / std::max<size_t>(bytes_per_row, 1));
+  return std::min(std::max<int64_t>(1, std::min<int64_t>(r, m->n)), raw_tile_rows(m));
+}
+
+void predict(Booster* b, Matrix* m, bool output_margin, int tree_begin, int tree_end, float* out, int64_t out_len) {
+  cudaStream_t s = b->ctx->stream; const int K = b->p.num_class;
+  if (out_len != m->n * K) fail("output buffer has %lld values, expected %lld", (long long)out_len, (long long)(m->n * K));
+  check_predict_args(b, m, tree_begin, &tree_end);
+  DevBuf<float> tmp; tmp.ensure((size_t)std::max<int64_t>(out_len, 1));
+  init_margin(b, tmp.p, m);
+  predict_trees(b, m, tree_begin, tree_end, tmp.p);
+  if (!output_margin) LAUNCH_CHECK(b2_launch_transform(b->p.objective, K, tmp.p, m->n, b->ctx->num_sms, s));
+  if (out_len > 0) CUDA_CHECK(cudaMemcpyAsync(out, tmp.p, out_len * sizeof(float), cudaMemcpyDeviceToHost, s));
+  CUDA_CHECK(cudaStreamSynchronize(s));
+}
+
+void predict_contribs(Booster* b, Matrix* m, int tree_begin, int tree_end, bool interactions, float* out, int64_t out_len) {
+  cudaStream_t s = b->ctx->stream; const int K = b->p.num_class; const int F = m->F;
+  const size_t per_row = (size_t)K * (F + 1) * (interactions ? (size_t)(F + 1) : 1);
+  if (b->p.vector_leaf())
+    fail("%s is not supported for vector-leaf trees (multi_strategy=multi_output_tree)",
+         interactions ? "pred_interactions" : "pred_contribs");
+  if (out_len != m->n * (int64_t)per_row) fail("output buffer has %lld values, expected %lld", (long long)out_len, (long long)(m->n * (int64_t)per_row));
+  check_predict_args(b, m, tree_begin, &tree_end);
+  build_paths(b);
+  std::vector<double> bias(K, 0.0);   // sum of the expected values of the trees in range, in tree order
+  for (int t = tree_begin; t < tree_end; ++t) bias[(t / std::max(1, b->p.num_parallel_tree)) % K] += b->tree_expected[t];
+  DevBuf<double> d_bias; upload(d_bias, bias, s);
+  const int p_begin = b->tree_path_offset[tree_begin], p_end = b->tree_path_offset[tree_end];
+  const float* bm = m->n_base_margin > 0 ? m->base_margin.p : nullptr;
+  const float base_value = base_margin_value(b->p);
+  // contributions: the row accumulators live in shared memory (up to 8 warps of K (F+1) doubles in <= 200 KiB),
+  // otherwise in global scratch; interactions always accumulate in global scratch
+  int warps = 8; size_t smem = 0;
+  if (!interactions) {
+    while (warps > 1 && b2_shap_contribs_smem(K, F, warps) > (size_t)200 * 1024) warps /= 2;
+    smem = b2_shap_contribs_smem(K, F, warps);
+    if (smem > (size_t)200 * 1024) { smem = 0; warps = 8; }
+  }
+  const bool gscratch = interactions || smem == 0;
+  if (m->n == 0) { CUDA_CHECK(cudaStreamSynchronize(s)); return; }   // for_raw_tiles calls once, with no rows
+  const int64_t blk = rows_per_block(m, per_row * (sizeof(float) + (gscratch ? sizeof(double) : 0)));
+  DevBuf<float> d_out; DevBuf<double> d_acc;
+  d_out.ensure((size_t)blk * per_row);
+  if (gscratch) d_acc.ensure((size_t)blk * per_row);
+  std::vector<cudaEvent_t> ev;
+  for_raw_tiles(m, [&](const float* X, int64_t r0, int64_t rows) {   // row 0 of X is row r0 of the matrix
+    cudaEvent_t e0, e1; CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
+    ev.push_back(e0); ev.push_back(e1);
+    const float* bm_rows = bm ? bm + (size_t)r0 * K : nullptr;
+    CUDA_CHECK(cudaEventRecord(e0, s));
+    if (interactions)
+      LAUNCH_CHECK(b2_launch_shap_interactions(X, 0, rows, F, m->missing, b->d_path_elems.p, b->d_paths.p, p_begin, p_end,
+                                               b->d_path_cats.p, K, d_bias.p, bm_rows, base_value, d_acc.p, d_out.p, b->ctx->num_sms, s));
+    else
+      LAUNCH_CHECK(b2_launch_shap_contribs(X, 0, rows, F, m->missing, b->d_path_elems.p, b->d_paths.p, p_begin, p_end,
+                                           b->d_path_cats.p, K, d_bias.p, bm_rows, base_value, gscratch ? d_acc.p : nullptr, warps,
+                                           smem, d_out.p, b->ctx->num_sms, s));
+    CUDA_CHECK(cudaEventRecord(e1, s));
+    CUDA_CHECK(cudaMemcpyAsync(out + (size_t)r0 * per_row, d_out.p, (size_t)rows * per_row * sizeof(float), cudaMemcpyDeviceToHost, s));
+  }, blk);
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  for (size_t i = 0; i < ev.size(); i += 2) {
+    float ms = 0; cudaEventElapsedTime(&ms, ev[i], ev[i + 1]);
+    b->t.shap_ms += ms;
+    cudaEventDestroy(ev[i]); cudaEventDestroy(ev[i + 1]);
+  }
+  b->t.shap_rows += m->n;
+}
+
+void predict_leaf(Booster* b, Matrix* m, int tree_begin, int tree_end, float* out, int64_t out_len) {
+  cudaStream_t s = b->ctx->stream;
+  check_predict_args(b, m, tree_begin, &tree_end);
+  const int T = tree_end - tree_begin;
+  if (out_len != m->n * T) fail("output buffer has %lld values, expected %lld", (long long)out_len, (long long)(m->n * T));
+  if (T == 0 || m->n == 0) return;
+  sync_device_trees(b);
+  const int64_t blk = rows_per_block(m, (size_t)T * sizeof(float));
+  DevBuf<float> d_out; d_out.ensure((size_t)blk * T);
+  for_raw_tiles(m, [&](const float* X, int64_t r0, int64_t rows) {
+    LAUNCH_CHECK(b2_launch_leaf_index(X, 0, rows, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p,
+                                      tree_begin, tree_end, d_out.p, b->ctx->num_sms, s));
+    CUDA_CHECK(cudaMemcpyAsync(out + (size_t)r0 * T, d_out.p, (size_t)rows * T * sizeof(float), cudaMemcpyDeviceToHost, s));
+  }, blk);
+  CUDA_CHECK(cudaStreamSynchronize(s));
 }
 
 }  // namespace b2host

@@ -329,6 +329,39 @@ void drain_round(Booster* b) {
   finish_round(b, b->rb[b->rb_cur ^ 1], n_trees, b->pending_check_finite);
 }
 
+// B2_BoosterCreate: a booster that trains on m, or without m a prediction-only one (num_feature=<n> in params)
+Booster* new_booster(const char* params, Matrix* m, Comm* comm) {
+  std::unique_ptr<Booster> b(new Booster()); b->kind = kBooster; b->train = m; b->comm = comm;
+  parse_params(params, &b->p, nullptr);
+  if (m) {
+    // the train matrix's label fixes the targets; a loaded model (num_target) must have as many
+    if (b->p.num_target_set && b->p.num_target != m->n_targets)
+      fail("the model has %d targets, the train matrix's label has %d columns", b->p.num_target, m->n_targets);
+    set_targets(&b->p, m->n_targets);
+    if (b->p.vector_leaf() && m->any_cat())
+      fail("multi_strategy=multi_output_tree is not supported with categorical features (the train matrix has %zu)",
+           m->cat_feats.size());
+    b->ctx = m->ctx; b->n_features = m->F; CUDA_CHECK(cudaSetDevice(m->ctx->device));
+    check_level_memory(b.get());
+    if (!b->p.interaction_sets.empty()) {   // sets_of[f] bit k: feature f is in set k
+      const int W = (int)((b->p.interaction_sets.size() + 63) / 64);
+      std::vector<unsigned long long> sets_of((size_t)m->F * W, 0ull);
+      for (size_t k = 0; k < b->p.interaction_sets.size(); ++k)
+        for (int64_t f : b->p.interaction_sets[k]) {
+          if (f >= m->F) fail("interaction_constraints: feature index %lld is out of range for %d features", (long long)f, m->F);
+          sets_of[(size_t)f * W + k / 64] |= 1ull << (k % 64);
+        }
+      upload(b->d_ic_sets_of, sets_of, m->ctx->stream);   // pageable source: staged before return
+      b->ic_words = W;
+    }
+  }
+  else {  // prediction-only booster (model loaded with B2_BoosterAddTree)
+    if (b->p.num_feature <= 0) fail("a booster without a train matrix needs num_feature=<n> in params");
+    b->ctx = get_ctx(b->p.device); b->n_features = b->p.num_feature;
+  }
+  return b.release();
+}
+
 // Update mode, before anything reads the train margin: the trees added so far become the trees to update and the model
 // starts empty (xgboost's gbtree moves them to trees_to_update).  Every tree is checked to be a proper binary tree
 // reachable from node 0 with at most 65,536 leaves (compact indices 0..65,535 fit pos), and copied to the device once:
@@ -340,8 +373,7 @@ void begin_update(Booster* b) {
   b->update_started = true;
   b->to_update = std::move(b->trees);
   b->trees.clear();
-  b->d_trees_synced = -1; b->paths_synced = -1; b->margin_ready = false;
-  for (auto& kv : b->eval_cache) if (kv.second) kv.second->n_trees_applied = 0, kv.second->n = -1;
+  trees_edited(b);
   std::vector<B2TreeNodeDev> nodes; std::vector<uint32_t> cats; std::vector<int32_t> order, levels;
   size_t max_leaves = 1, max_nodes = 1, max_block = 8;
   b->rtrees.clear();
@@ -451,7 +483,6 @@ void ensure_train_margin(Booster* b) {
     dart_margins(b, {}, {}, b->tree_w, nullptr, b->margin.p);
   } else if (!b->trees.empty()) {
     if (!m->has_raw) fail("continuing training from existing trees needs the raw data of the train matrix (B2_MatrixEnsureRaw)");
-    sync_device_trees(b);
     predict_trees(b, m, 0, (int)b->trees.size(), b->margin.p);
   }
   b->margin_ready = true;
