@@ -135,6 +135,13 @@ int B2_MatrixFree(B2Handle m);
  * max_depth, eta, gamma, min_child_weight, lambda, alpha, max_bin, base_score, hist_qbits,
  * eval_metric).  train must be quantised.  comm may be 0. */
 int B2_BoosterCreate(const char* params, B2Handle train, B2Handle comm, B2Handle* out);
+/* Change parameters between boosting rounds (xgboost's Booster.set_param during training, e.g. a learning-rate schedule):
+ * the same "key=value" lines as B2_BoosterCreate.  eta / learning_rate, gamma / min_split_loss, min_child_weight,
+ * lambda / reg_lambda, alpha / reg_alpha, max_delta_step, subsample, colsample_bytree / bylevel / bynode,
+ * max_cat_to_onehot and max_cat_threshold take effect from the next round, each checked by its B2_BoosterCreate rule.
+ * Any other key the engine knows may only repeat its value (a new one fails, naming the key); unknown keys are ignored.
+ * Either every key is applied or, on failure, none.  A round still in flight is finished with the old values first. */
+int B2_BoosterSetParam(B2Handle b, const char* params);
 int B2_BoosterUpdateOneIter(B2Handle b, int32_t iter);
 /* custom objective (xgb.train(obj=...), tests/test_xgboost_api.py:77-102): grad/hess [n_rows*num_class] */
 int B2_BoosterBoostOneIter(B2Handle b, const float* grad, const float* hess, int64_t len);
@@ -209,7 +216,9 @@ int B2_BoosterGetTreeWeights(B2Handle b, float* out, int64_t len);
 int B2_BoosterSetTreeWeights(B2Handle b, const float* w, int64_t len);
 /* JSON object with accumulated device timings / counters of the hot path (since last reset):
  * hist_ms, hist_launches, hist_rows, hist_bytes, kernel_launches, round_ms, allreduce_bytes ..., and in update mode
- * refresh_ms / refresh_launches: the time and count of refresh_kernel launches (B2_BoosterRefreshOneIter) */
+ * refresh_ms / refresh_launches: the time and count of refresh_kernel launches (B2_BoosterRefreshOneIter), and
+ * graph_update_ms / graph_updates / graph_reinstantiations: the host time of re-capturing a tree whose graph a
+ * B2_BoosterSetParam change made stale, the updates of its graph in place, and the updates refused (instantiated anew) */
 int B2_BoosterGetTimers(B2Handle b, int32_t reset, char* out, int64_t out_cap);
 int B2_BoosterCancel(B2Handle b);
 int B2_BoosterFree(B2Handle b);

@@ -402,6 +402,11 @@ int B2_BoosterCreate(const char* params, B2Handle trainh, B2Handle commh, B2Hand
   *out = (B2Handle)new_booster(params, m, comm_of(commh));
   API_END
 }
+int B2_BoosterSetParam(B2Handle bh, const char* params) {
+  API_BEGIN
+  set_booster_params(from_handle<Booster>(bh, kBooster, "booster"), params);
+  API_END
+}
 int B2_BoosterUpdateOneIter(B2Handle bh, int32_t iter) {
   API_BEGIN
   (void)iter;
@@ -619,11 +624,11 @@ int B2_BoosterGetTimers(B2Handle bh, int32_t reset, char* out, int64_t out_cap) 
            "\"round_ms\": %.6f, \"rounds\": %lld, \"allreduce_bytes\": %.1f, \"num_sms\": %d, \"n_groups\": %d, \"row_stride\": %d, "
            "\"phase_ms\": {\"quant\": %.4f, \"hist\": %.4f, \"allreduce\": %.4f, \"subtract\": %.4f, \"eval_decide\": %.4f, "
            "\"partition_finalize\": %.4f, \"leaf\": %.4f}, \"shap_ms\": %.6f, \"shap_rows\": %lld, \"refresh_ms\": %.6f, "
-           "\"refresh_launches\": %lld}",
+           "\"refresh_launches\": %lld, \"graph_update_ms\": %.6f, \"graph_updates\": %lld, \"graph_reinstantiations\": %lld}",
            t.hist_ms, t.hist_launches, t.hist_rows, t.hist_bytes, t.kernel_launches, t.round_ms, t.rounds, t.allreduce_bytes,
            b->ctx->num_sms, b->train ? b->train->n_groups : 0, b->train ? b->train->row_stride : 0, t.phase_ms[0], t.phase_ms[1],
            t.phase_ms[2], t.phase_ms[3], t.phase_ms[4], t.phase_ms[5], t.phase_ms[6], t.shap_ms, t.shap_rows, t.refresh_ms,
-           t.refresh_launches);
+           t.refresh_launches, t.graph_update_ms, t.graph_updates, t.graph_reinstantiations);
   if (reset) b->t.reset();
   API_END
 }

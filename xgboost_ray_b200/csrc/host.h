@@ -354,6 +354,10 @@ struct Timers {
   long long shap_rows = 0;
   double refresh_ms = 0;   // update mode: refresh_kernel time (CUDA events around every launch)
   long long refresh_launches = 0;
+  // B2_BoosterSetParam changed a value the tree graphs bake in: host time of re-capturing a tree and applying it to its
+  // graph (cudaGraphExecUpdate), and how often the update was refused and the graph instantiated again instead
+  double graph_update_ms = 0;
+  long long graph_updates = 0, graph_reinstantiations = 0;
   double phase_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // profile=2: quant, hist, allreduce, subtract, eval+decide, partition+finalize, leaf, other
   long long hist_launches = 0, hist_rows = 0, kernel_launches = 0, rounds = 0;
   double hist_bytes = 0, allreduce_bytes = 0;
@@ -434,9 +438,11 @@ struct Booster : HandleBase {
     int cand_cap = 0;
   } p2p;
   // CUDA graphs of the per-tree launch sequence, one per class tree of a round (grow_tree is sync-free and its
-  // arguments are the same for every tree, so the sequence is captured once and replayed)
+  // arguments are the same for every tree, so the sequence is captured once and replayed; B2_BoosterSetParam marks them
+  // stale when it changes an argument, and run_tree captures the sequence again and updates the graph in place)
   struct TreeGraph {
     cudaGraphExec_t exec = nullptr;
+    bool stale = false;                    // B2_BoosterSetParam changed a kernel argument baked into it (run_tree)
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> hist_ev;   // owned; recorded by the graph (external event nodes)
     long long hist_launches = 0, kernel_launches = 0;
     double allreduce_bytes = 0;
@@ -544,13 +550,16 @@ struct Booster : HandleBase {
   size_t rstaging_bytes = 0;               // bytes of every block in rb[].rstaging (the largest tree's)
   // profiling
   Timers t;
+  // the one teardown of a tree graph: its executable graph and the events its nodes record
+  static void destroy_graph(TreeGraph& g) {
+    if (g.exec) cudaGraphExecDestroy(g.exec);
+    for (auto& pr : g.hist_ev) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
+    g.exec = nullptr; g.hist_ev.clear();
+  }
   ~Booster() {
     // (a pending round is not drained: the stream synchronisation below waits for it and its trees are dropped)
     for (auto& r : rb)
-      for (auto& kv : r.graphs) {
-        if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-        for (auto& pr : kv.second.hist_ev) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
-      }
+      for (auto& kv : r.graphs) destroy_graph(kv.second);
     // No barrier with the peers here: a peer touches this rank's arena only inside the exchange kernels of a round, and
     // every one of those accesses happens-before a flag that this rank waited for before ITS round completed -- once the
     // last round is synchronised the arena is quiescent.  (A barrier in the destructor made a rank whose peer keeps its
@@ -574,6 +583,7 @@ struct Booster : HandleBase {
 // ---------------------------------------------------------------- params.cu
 void set_targets(Params* p, int T);
 void parse_params(const char* text, Params* p, int* max_bin_out);
+Params changed_params(const Params& live, const char* text);
 float base_margin_value(const Params& p);
 float h_calc_weight(const Params& p, double G, double H);
 const Metric& metric_id(const char* name, const Params& p, float* param, int* minus);
@@ -585,6 +595,7 @@ int quantile_select(Booster* b, int k, const uint16_t* pos, const float* margin,
                     const int32_t* n_leaves, int max_leaves, float eta, const B2LeafDev* leaves, float* leaf_value,
                     float* tree_value);
 B2CtlParams ctl_params(const Params& p);
+void tree_params_changed(Booster* b, const Params& old);
 void run_tree(Booster* b, int k, int slot);
 void materialize_tree(Booster* b, const void* block);
 void materialize_vector_tree(Booster* b, const void* block, const void* vblock);
@@ -599,6 +610,7 @@ void drain_round(Booster* b);
 void ensure_train_margin(Booster* b);
 void dart_prepare(Booster* b);
 Booster* new_booster(const char* params, Matrix* m, Comm* comm);
+void set_booster_params(Booster* b, const char* params);
 void boost_round(Booster* b, const float* custom_g, const float* custom_h, int64_t len);
 
 // ---------------------------------------------------------------- predict.cu

@@ -5,6 +5,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <tuple>
+
 #include "host.h"
 
 namespace b2host __attribute__((visibility("hidden"))) {
@@ -110,115 +112,126 @@ void set_targets(Params* p, int T) {
   }
 }
 
-void parse_params(const char* text, Params* p, int* max_bin_out) {
-  std::string s(text ? text : "");
-  std::map<std::string, std::string> dart_text;
+// the "key=value" lines of a params text, in order; a line without '=' is skipped
+std::vector<std::pair<std::string, std::string>> param_lines(const char* text) {
+  std::vector<std::pair<std::string, std::string>> out;
+  const std::string s(text ? text : "");
   size_t pos = 0;
   while (pos < s.size()) {
     size_t nl = s.find('\n', pos);
     if (nl == std::string::npos) nl = s.size();
-    std::string line = s.substr(pos, nl - pos);
+    const std::string line = s.substr(pos, nl - pos);
     pos = nl + 1;
-    size_t eq = line.find('=');
-    if (eq == std::string::npos) continue;
-    std::string k = line.substr(0, eq), v = line.substr(eq + 1);
-    auto f = [&]() { return (float)atof(v.c_str()); };
-    auto i = [&]() { return atoi(v.c_str()); };
-    if (k == "objective") {
-      p->objective_name = v;
-      const Objective* row = std::find_if(std::begin(kObjectives), std::end(kObjectives),
-                                          [&](const Objective& o) { return v == o.name; });
-      if (row == std::end(kObjectives))
-        fail("unsupported objective '%s' (supported: reg:squarederror, reg:logistic, binary:logistic, binary:logitraw, "
-             "reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie, survival:aft, "
-             "rank:pairwise, rank:ndcg, rank:map, reg:quantileerror, multi:softprob, multi:softmax)", v.c_str());
-      p->objective_index = (int)(row - kObjectives);
-      p->objective = row->id;
-    } else if (k == "num_class") { p->num_class = i(); p->num_class_set = true; }
-    else if (k == "num_target") { p->num_target = i(); p->num_target_set = true; }
-    else if (k == "quantile_alpha") p->quantile_alpha = parse_quantile_alpha(v);
-    else if (k == "num_parallel_tree") p->num_parallel_tree = i();
-    else if (k == "max_depth") p->max_depth = i();
-    else if (k == "eta" || k == "learning_rate") p->eta = f();
-    else if (k == "gamma" || k == "min_split_loss") p->gamma = f();
-    else if (k == "min_child_weight") p->min_child_weight = f();
-    else if (k == "lambda" || k == "reg_lambda") p->lambda = f();
-    else if (k == "alpha" || k == "reg_alpha") p->alpha = f();
-    else if (k == "base_score") { p->base_score = f(); p->base_score_set = true; }
-    else if (k == "hist_qbits") p->qbits = i();
-    else if (k == "hist_chunk_rows") p->hist_chunk_rows = i();
-    else if (k == "profile") p->profile = i();
-    else if (k == "num_feature") p->num_feature = i();
-    else if (k == "device") p->device = i();
-    else if (k == "subsample") p->subsample = f();
-    else if (k == "colsample_bytree") p->colsample_bytree = f();
-    else if (k == "colsample_bylevel") p->colsample_bylevel = f();
-    else if (k == "colsample_bynode") p->colsample_bynode = f();
-    else if (k == "seed" || k == "random_state") p->seed = i();
-    else if (k == "scale_pos_weight") p->scale_pos_weight = f();
-    else if (k == "max_delta_step") { p->max_delta_step = f(); p->max_delta_step_set = true; }
-    else if (k == "huber_slope") p->huber_slope = f();
-    else if (k == "tweedie_variance_power") p->tweedie_variance_power = f();
-    else if (k == "aft_loss_distribution") {
-      if (v == "normal") p->aft_dist = kAftNormal;
-      else if (v == "logistic") p->aft_dist = kAftLogistic;
-      else if (v == "extreme") p->aft_dist = kAftExtreme;
-      else fail("aft_loss_distribution must be normal, logistic or extreme, got '%s'", v.c_str());
-    }
-    else if (k == "aft_loss_distribution_scale") p->aft_sigma = f();
-    else if (k == "lambdarank_pair_method") {
-      if (v != "topk") fail("lambdarank_pair_method='%s' is not supported (supported: topk; random pair sampling "
-                            "(mean) is not implemented)", v.c_str());
-    }
-    else if (k == "lambdarank_num_pair_per_sample") {
-      char* end = nullptr;
-      const long long kv = strtoll(v.c_str(), &end, 10);
-      if (v.empty() || *end != '\0' || kv < 1 || kv > INT32_MAX)
-        fail("lambdarank_num_pair_per_sample must be an integer >= 1, got '%s'", v.c_str());
-      p->rank_k = (int)kv;
-    }
-    else if (k == "lambdarank_unbiased" || k == "ndcg_exp_gain") {
-      bool on;
-      if (v == "1" || v == "true" || v == "True") on = true;
-      else if (v == "0" || v == "false" || v == "False") on = false;
-      else fail("%s must be a boolean, got '%s'", k.c_str(), v.c_str());
-      if (k == "ndcg_exp_gain") p->ndcg_exp_gain = on;
-      else if (on) fail("lambdarank_unbiased=true is not supported (position-bias estimation is not implemented)");
-    }
-    else if (k == "max_cat_to_onehot") p->max_cat_to_onehot = i();
-    else if (k == "max_cat_threshold") p->max_cat_threshold = i();
-    else if (k == "max_bin") { if (max_bin_out) *max_bin_out = i(); }
-    else if (k == "interaction_constraints") p->interaction_sets = parse_interaction_sets(v);
-    else if (k == "multi_strategy") {
-      if (v == "one_output_per_tree") p->multi_strategy = 0;
-      else if (v == "multi_output_tree") p->multi_strategy = 1;
-      else fail("multi_strategy='%s' is not supported (supported: one_output_per_tree, multi_output_tree)", v.c_str());
-    }
-    else if (k == "booster") {
-      if (v == "gbtree") p->dart = false;
-      else if (v == "dart") p->dart = true;
-      else fail("booster='%s' is not supported (supported: gbtree, dart)", v.c_str());
-    }
-    else if (k == "rate_drop" || k == "skip_drop" || k == "sample_type" || k == "normalize_type" || k == "one_drop")
-      dart_text[k] = v;   // checked below, and only for booster=dart (gbtree ignores them, like xgboost)
-    else if (k == "process_type") {
-      if (v == "default") p->update_mode = false;
-      else if (v == "update") p->update_mode = true;
-      else fail("process_type='%s' is not supported (supported: 'default', 'update')", v.c_str());
-    }
-    else if (k == "updater") {
-      if (v != "refresh" && v != "grow_quantile_histmaker" && v != "grow_gpu_hist")
-        fail("updater='%s' is not supported (supported: grow_quantile_histmaker, grow_gpu_hist, and refresh with "
-             "process_type='update')", v.c_str());
-      p->updater = v;
-    }
-    else if (k == "refresh_leaf") {
-      if (v == "1" || v == "true" || v == "True") p->refresh_leaf = true;
-      else if (v == "0" || v == "false" || v == "False") p->refresh_leaf = false;
-      else fail("refresh_leaf must be 0 or 1, got '%s'", v.c_str());
-    }
-    // unknown keys (nthread, tree_method, verbosity, ...) are accepted and ignored, like xgboost
+    const size_t eq = line.find('=');
+    if (eq != std::string::npos) out.push_back({line.substr(0, eq), line.substr(eq + 1)});
   }
+  return out;
+}
+
+// One key into p.  The DART keys go to dart_text (checked once booster=dart is known); max_bin to *max_bin_out.
+// Returns false for a key the engine does not know.
+bool apply_param(Params* p, const std::string& k, const std::string& v, std::map<std::string, std::string>* dart_text,
+                 int* max_bin_out) {
+  auto f = [&]() { return (float)atof(v.c_str()); };
+  auto i = [&]() { return atoi(v.c_str()); };
+  if (k == "objective") {
+    p->objective_name = v;
+    const Objective* row = std::find_if(std::begin(kObjectives), std::end(kObjectives),
+                                        [&](const Objective& o) { return v == o.name; });
+    if (row == std::end(kObjectives))
+      fail("unsupported objective '%s' (supported: reg:squarederror, reg:logistic, binary:logistic, binary:logitraw, "
+           "reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie, survival:aft, "
+           "rank:pairwise, rank:ndcg, rank:map, reg:quantileerror, multi:softprob, multi:softmax)", v.c_str());
+    p->objective_index = (int)(row - kObjectives);
+    p->objective = row->id;
+  } else if (k == "num_class") { p->num_class = i(); p->num_class_set = true; }
+  else if (k == "num_target") { p->num_target = i(); p->num_target_set = true; }
+  else if (k == "quantile_alpha") p->quantile_alpha = parse_quantile_alpha(v);
+  else if (k == "num_parallel_tree") p->num_parallel_tree = i();
+  else if (k == "max_depth") p->max_depth = i();
+  else if (k == "eta" || k == "learning_rate") p->eta = f();
+  else if (k == "gamma" || k == "min_split_loss") p->gamma = f();
+  else if (k == "min_child_weight") p->min_child_weight = f();
+  else if (k == "lambda" || k == "reg_lambda") p->lambda = f();
+  else if (k == "alpha" || k == "reg_alpha") p->alpha = f();
+  else if (k == "base_score") { p->base_score = f(); p->base_score_set = true; }
+  else if (k == "hist_qbits") p->qbits = i();
+  else if (k == "hist_chunk_rows") p->hist_chunk_rows = i();
+  else if (k == "profile") p->profile = i();
+  else if (k == "num_feature") p->num_feature = i();
+  else if (k == "device") p->device = i();
+  else if (k == "subsample") p->subsample = f();
+  else if (k == "colsample_bytree") p->colsample_bytree = f();
+  else if (k == "colsample_bylevel") p->colsample_bylevel = f();
+  else if (k == "colsample_bynode") p->colsample_bynode = f();
+  else if (k == "seed" || k == "random_state") p->seed = i();
+  else if (k == "scale_pos_weight") p->scale_pos_weight = f();
+  else if (k == "max_delta_step") { p->max_delta_step = f(); p->max_delta_step_set = true; }
+  else if (k == "huber_slope") p->huber_slope = f();
+  else if (k == "tweedie_variance_power") p->tweedie_variance_power = f();
+  else if (k == "aft_loss_distribution") {
+    if (v == "normal") p->aft_dist = kAftNormal;
+    else if (v == "logistic") p->aft_dist = kAftLogistic;
+    else if (v == "extreme") p->aft_dist = kAftExtreme;
+    else fail("aft_loss_distribution must be normal, logistic or extreme, got '%s'", v.c_str());
+  }
+  else if (k == "aft_loss_distribution_scale") p->aft_sigma = f();
+  else if (k == "lambdarank_pair_method") {
+    if (v != "topk") fail("lambdarank_pair_method='%s' is not supported (supported: topk; random pair sampling "
+                          "(mean) is not implemented)", v.c_str());
+  }
+  else if (k == "lambdarank_num_pair_per_sample") {
+    char* end = nullptr;
+    const long long kv = strtoll(v.c_str(), &end, 10);
+    if (v.empty() || *end != '\0' || kv < 1 || kv > INT32_MAX)
+      fail("lambdarank_num_pair_per_sample must be an integer >= 1, got '%s'", v.c_str());
+    p->rank_k = (int)kv;
+  }
+  else if (k == "lambdarank_unbiased" || k == "ndcg_exp_gain") {
+    bool on;
+    if (v == "1" || v == "true" || v == "True") on = true;
+    else if (v == "0" || v == "false" || v == "False") on = false;
+    else fail("%s must be a boolean, got '%s'", k.c_str(), v.c_str());
+    if (k == "ndcg_exp_gain") p->ndcg_exp_gain = on;
+    else if (on) fail("lambdarank_unbiased=true is not supported (position-bias estimation is not implemented)");
+  }
+  else if (k == "max_cat_to_onehot") p->max_cat_to_onehot = i();
+  else if (k == "max_cat_threshold") p->max_cat_threshold = i();
+  else if (k == "max_bin") { if (max_bin_out) *max_bin_out = i(); }
+  else if (k == "interaction_constraints") p->interaction_sets = parse_interaction_sets(v);
+  else if (k == "multi_strategy") {
+    if (v == "one_output_per_tree") p->multi_strategy = 0;
+    else if (v == "multi_output_tree") p->multi_strategy = 1;
+    else fail("multi_strategy='%s' is not supported (supported: one_output_per_tree, multi_output_tree)", v.c_str());
+  }
+  else if (k == "booster") {
+    if (v == "gbtree") p->dart = false;
+    else if (v == "dart") p->dart = true;
+    else fail("booster='%s' is not supported (supported: gbtree, dart)", v.c_str());
+  }
+  else if (k == "rate_drop" || k == "skip_drop" || k == "sample_type" || k == "normalize_type" || k == "one_drop")
+    (*dart_text)[k] = v;   // checked by apply_dart_params, and only for booster=dart (gbtree ignores them, like xgboost)
+  else if (k == "process_type") {
+    if (v == "default") p->update_mode = false;
+    else if (v == "update") p->update_mode = true;
+    else fail("process_type='%s' is not supported (supported: 'default', 'update')", v.c_str());
+  }
+  else if (k == "updater") {
+    if (v != "refresh" && v != "grow_quantile_histmaker" && v != "grow_gpu_hist")
+      fail("updater='%s' is not supported (supported: grow_quantile_histmaker, grow_gpu_hist, and refresh with "
+           "process_type='update')", v.c_str());
+    p->updater = v;
+  }
+  else if (k == "refresh_leaf") {
+    if (v == "1" || v == "true" || v == "True") p->refresh_leaf = true;
+    else if (v == "0" || v == "false" || v == "False") p->refresh_leaf = false;
+    else fail("refresh_leaf must be 0 or 1, got '%s'", v.c_str());
+  }
+  else return false;   // unknown keys (nthread, tree_method, verbosity, ...) are accepted and ignored, like xgboost
+  return true;
+}
+
+void apply_dart_params(Params* p, const std::map<std::string, std::string>& dart_text) {
   if (p->dart) {
     for (const auto& kv : dart_text) {
       const std::string& k = kv.first; const std::string& v = kv.second;
@@ -240,6 +253,25 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
       }
     }
   }
+}
+
+// The range rules of the keys that may change between rounds (round_param_key): B2_BoosterCreate and
+// B2_BoosterSetParam apply the same ones.  count:poisson's max_delta_step defaults to 0.7 until one is given.
+void check_round_params(Params* p) {
+  for (float v : {p->subsample, p->colsample_bytree, p->colsample_bylevel, p->colsample_bynode})
+    if (!(v > 0.0f && v <= 1.0f)) fail("subsample / colsample_* must be in (0, 1], got %g", (double)v);
+  if (p->max_cat_to_onehot < 1) fail("max_cat_to_onehot must be >= 1, got %d", p->max_cat_to_onehot);
+  if (p->max_cat_threshold < 1) fail("max_cat_threshold must be >= 1, got %d", p->max_cat_threshold);
+  if (p->objective == kObjPoisson) {
+    if (!p->max_delta_step_set) p->max_delta_step = 0.7f;   // both the hessian's shift and the leaf-step clamp
+    if (!(p->max_delta_step >= 0.0f)) fail("max_delta_step must be >= 0 for count:poisson, got %g", (double)p->max_delta_step);
+  }
+}
+
+void parse_params(const char* text, Params* p, int* max_bin_out) {
+  std::map<std::string, std::string> dart_text;
+  for (const auto& kv : param_lines(text)) apply_param(p, kv.first, kv.second, &dart_text, max_bin_out);
+  apply_dart_params(p, dart_text);
   const Objective& obj = objective_row(*p);
   if (obj.grad == kGradRank && p->num_class > 1)
     fail("%s has one output per row: num_class must be 1, got %d", p->objective_name.c_str(), p->num_class);
@@ -279,14 +311,7 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
   if (p->max_depth < 1 || p->max_depth > 16) fail("max_depth must be in [1, 16], got %d", p->max_depth);
   if (p->num_parallel_tree < 1 || p->num_parallel_tree > 4096) fail("num_parallel_tree must be in [1, 4096], got %d", p->num_parallel_tree);
   if (p->qbits < 8 || p->qbits > 24) fail("hist_qbits must be in [8, 24], got %d", p->qbits);
-  for (float v : {p->subsample, p->colsample_bytree, p->colsample_bylevel, p->colsample_bynode})
-    if (!(v > 0.0f && v <= 1.0f)) fail("subsample / colsample_* must be in (0, 1], got %g", (double)v);
-  if (p->max_cat_to_onehot < 1) fail("max_cat_to_onehot must be >= 1, got %d", p->max_cat_to_onehot);
-  if (p->max_cat_threshold < 1) fail("max_cat_threshold must be >= 1, got %d", p->max_cat_threshold);
-  if (p->objective == kObjPoisson) {
-    if (!p->max_delta_step_set) p->max_delta_step = 0.7f;   // both the hessian's shift and the leaf-step clamp
-    if (!(p->max_delta_step >= 0.0f)) fail("max_delta_step must be >= 0 for count:poisson, got %g", (double)p->max_delta_step);
-  }
+  check_round_params(p);
   if (p->objective == kObjPseudoHuber && !(p->huber_slope > 0.0f))
     fail("huber_slope must be > 0 for reg:pseudohubererror, got %g", (double)p->huber_slope);
   if (p->objective == kObjTweedie && !(p->tweedie_variance_power >= 1.0f && p->tweedie_variance_power < 2.0f))
@@ -302,6 +327,53 @@ void parse_params(const char* text, Params* p, int* max_bin_out) {
     if (obj.link == kLinkExp && !(p->base_score > 0.0f))
       fail("base_score must be > 0 for %s, got %g", p->objective_name.c_str(), (double)p->base_score);
   }
+}
+
+// The keys B2_BoosterSetParam applies between rounds (DESIGN.md 2 item 22): they enter a round's gradients, split scan,
+// sampling and leaf values only, never the model's shape or the size of a device buffer
+bool round_param_key(const std::string& k) {
+  static const std::set<std::string> keys{
+      "eta", "learning_rate", "gamma", "min_split_loss", "min_child_weight", "lambda", "reg_lambda", "alpha",
+      "reg_alpha", "max_delta_step", "subsample", "colsample_bytree", "colsample_bylevel", "colsample_bynode",
+      "max_cat_to_onehot", "max_cat_threshold"};
+  return keys.count(k) != 0;
+}
+
+// every field a key outside round_param_key sets (not the *_set bookkeeping): equal when such a key kept its value
+bool same_fixed_params(const Params& a, const Params& b) {
+  return std::tie(a.objective_name, a.num_class, a.num_target, a.num_parallel_tree, a.max_depth, a.base_score, a.qbits,
+                  a.hist_chunk_rows, a.profile, a.num_feature, a.device, a.scale_pos_weight, a.huber_slope,
+                  a.tweedie_variance_power, a.aft_dist, a.aft_sigma, a.rank_k, a.ndcg_exp_gain, a.seed,
+                  a.interaction_sets, a.dart, a.rate_drop, a.skip_drop, a.dart_weighted, a.dart_forest, a.one_drop,
+                  a.quantile_alpha, a.multi_strategy, a.update_mode, a.refresh_leaf, a.updater) ==
+         std::tie(b.objective_name, b.num_class, b.num_target, b.num_parallel_tree, b.max_depth, b.base_score, b.qbits,
+                  b.hist_chunk_rows, b.profile, b.num_feature, b.device, b.scale_pos_weight, b.huber_slope,
+                  b.tweedie_variance_power, b.aft_dist, b.aft_sigma, b.rank_k, b.ndcg_exp_gain, b.seed,
+                  b.interaction_sets, b.dart, b.rate_drop, b.skip_drop, b.dart_weighted, b.dart_forest, b.one_drop,
+                  b.quantile_alpha, b.multi_strategy, b.update_mode, b.refresh_leaf, b.updater);
+}
+
+// B2_BoosterSetParam's rules: `live` with the round keys of text applied, each checked by its B2_BoosterCreate rule.
+// Any other key the engine knows must keep its value; unknown keys are ignored.  Fails before anything is applied.
+Params changed_params(const Params& live, const char* text) {
+  Params q = live;
+  for (const auto& kv : param_lines(text)) {
+    const std::string& k = kv.first;
+    if (round_param_key(k)) { apply_param(&q, k, kv.second, nullptr, nullptr); continue; }
+    Params r = live;
+    std::map<std::string, std::string> dart_text;
+    if (!apply_param(&r, k, kv.second, &dart_text, nullptr)) continue;
+    apply_dart_params(&r, dart_text);
+    if (!same_fixed_params(r, live))
+      fail("parameter %s cannot change after training started: %s; pass it to train()", k.c_str(),
+           k == "max_depth" ? "the level buffers and read-back blocks are sized by it"
+           : k == "objective" || k == "num_class" || k == "num_target" || k == "quantile_alpha" ||
+                   k == "multi_strategy" || k == "num_parallel_tree"
+               ? "it sets the model's outputs and the trees of a round"
+               : "it is fixed when the booster is created");
+  }
+  check_round_params(&q);
+  return q;
 }
 
 // margin of base_score (the inverse of the prediction transform), evaluated on the host with libm's logf

@@ -362,6 +362,20 @@ Booster* new_booster(const char* params, Matrix* m, Comm* comm) {
   return b.release();
 }
 
+// B2_BoosterSetParam (DESIGN.md 2 item 22).  Every rule is checked before anything changes.  The pending round was
+// enqueued with the old values and its host-side finish reads them (materialize_tree's base weights, the vector leaves'
+// eta), so it is finished first; the next round is the first one to use the new values.
+void set_booster_params(Booster* b, const char* params) {
+  const Params q = changed_params(b->p, params);
+  if (!b->train) { b->p = q; return; }   // prediction-only: nothing is pending or captured
+  CUDA_CHECK(cudaSetDevice(b->ctx->device));
+  drain_round(b);
+  const Params old = b->p;
+  b->p = q;
+  if (q.eta != old.eta) b->dart_next.r = -1;   // DART's next-round weights normalise by eta
+  tree_params_changed(b, old);
+}
+
 // Update mode, before anything reads the train margin: the trees added so far become the trees to update and the model
 // starts empty (xgboost's gbtree moves them to trees_to_update).  Every tree is checked to be a proper binary tree
 // reachable from node 0 with at most 65,536 leaves (compact indices 0..65,535 fit pos), and copied to the device once:

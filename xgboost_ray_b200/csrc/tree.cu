@@ -6,6 +6,9 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <chrono>
+#include <tuple>
+
 #include "host.h"
 #include "launch.h"
 #include "sampling.cuh"
@@ -158,10 +161,7 @@ void ensure_ctl_tables(Booster* b) {
   if (b->ctl_depth == D) return;
   if (b->ctl_depth != 0 && b->p2p.enabled) fail("max_depth cannot change while the peer-memory exchange is mapped");
   for (auto& r : b->rb) {   // captured launch sequences hold the old table addresses
-    for (auto& kv : r.graphs) {
-      if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-      for (auto& pr : kv.second.hist_ev) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
-    }
+    for (auto& kv : r.graphs) Booster::destroy_graph(kv.second);
     r.graphs.clear();
   }
   b->direct_trees.clear();
@@ -330,6 +330,19 @@ B2CtlParams ctl_params(const Params& p) {
   cp.mcw = (double)p.min_child_weight; cp.lambda = (double)p.lambda; cp.alpha = (double)p.alpha;
   cp.max_delta_step = (double)p.max_delta_step; cp.gamma = p.gamma; cp.eta = p.eta / (float)p.num_parallel_tree;
   return cp;
+}
+
+// B2_BoosterSetParam changed b->p from old: the tree graphs of both round-buffer sets are stale when a value that
+// train_params or ctl_params pass to the kernels by value changed (run_tree captures them again on their next use)
+void tree_params_changed(Booster* b, const Params& old) {
+  const Params& p = b->p;
+  if (std::tie(p.eta, p.gamma, p.min_child_weight, p.lambda, p.alpha, p.max_delta_step, p.max_cat_to_onehot,
+               p.max_cat_threshold) ==
+      std::tie(old.eta, old.gamma, old.min_child_weight, old.lambda, old.alpha, old.max_delta_step,
+               old.max_cat_to_onehot, old.max_cat_threshold))
+    return;
+  for (auto& r : b->rb)
+    for (auto& kv : r.graphs) kv.second.stale = true;
 }
 
 // Column sampling of one tree: the tree's feature set and one nested set per level are drawn on the host (they depend
@@ -779,6 +792,8 @@ void prepare_tree_buffers(Booster* b, int slot) {
 // fused |g|,|h| maxima, no per-phase profiling), otherwise enqueue the kernels one by one.  The first tree of a class
 // slot always runs with direct launches (it allocates); the next two are captured, one graph per round parity (each
 // copies into its own read-back block and records its own events), and the following ones replay them alternately.
+// A stale graph (tree_params_changed) is captured again and applied to its executable graph with cudaGraphExecUpdate:
+// the topology is the same, only kernel arguments differ.  It is instantiated again only when the update is refused.
 void run_tree(Booster* b, int k, int slot) {
   cudaStream_t s = b->ctx->stream; const Params& p = b->p;
   prepare_tree_buffers(b, slot);
@@ -795,18 +810,39 @@ void run_tree(Booster* b, int k, int slot) {
   if (!eligible) { direct(); return; }
   std::map<int, Booster::TreeGraph>& graphs = b->rb[b->rb_cur].graphs;
   auto it = graphs.find(k);
-  if (it == graphs.end()) {
-    if (b->direct_trees[k] == 0) { direct(); return; }
+  if (it == graphs.end() || it->second.stale) {
+    if (it == graphs.end() && b->direct_trees[k] == 0) { direct(); return; }
+    const auto t0 = std::chrono::steady_clock::now();
     TreeStats st; st.capturing = true;
     cudaGraph_t graph = nullptr; cudaGraphExec_t exec = nullptr;
     bool ok = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
     if (ok) {
       try { if (p.vector_leaf()) grow_vector_tree(b, slot, st); else grow_tree(b, k, slot, st); }
-      catch (const B2Error& e) { cudaStreamEndCapture(s, &graph); if (graph) cudaGraphDestroy(graph); cudaGetLastError(); throw; }
+      catch (const B2Error& e) {
+        cudaStreamEndCapture(s, &graph); if (graph) cudaGraphDestroy(graph); cudaGetLastError();
+        for (auto& pr : st.hist_ev) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
+        throw;
+      }
       ok = cudaStreamEndCapture(s, &graph) == cudaSuccess && graph != nullptr;
     }
-    if (ok) ok = cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess;
+    if (ok && it != graphs.end()) {
+      cudaGraphExecUpdateResultInfo info;
+      if (cudaGraphExecUpdate(it->second.exec, graph, &info) == cudaSuccess) {
+        exec = it->second.exec;
+        it->second.exec = nullptr;   // moved to the new entry; the old one keeps only its events
+        b->t.graph_updates++;
+      } else {
+        cudaGetLastError();
+        b->t.graph_reinstantiations++;
+      }
+    }
+    if (ok && !exec) ok = cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess;
     if (graph) cudaGraphDestroy(graph);
+    if (it != graphs.end()) {
+      Booster::destroy_graph(it->second);
+      graphs.erase(it);
+      b->t.graph_update_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    }
     if (!ok) {
       cudaGetLastError();
       for (auto& pr : st.hist_ev) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }

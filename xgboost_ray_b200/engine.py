@@ -77,6 +77,7 @@ ABI = {
     "B2_MatrixGetBins": (C.c_int, [_H, _BP]),
     "B2_MatrixFree": (C.c_int, [_H]),
     "B2_BoosterCreate": (C.c_int, [C.c_char_p, _H, _H, C.POINTER(_H)]),
+    "B2_BoosterSetParam": (C.c_int, [_H, C.c_char_p]),
     "B2_BoosterUpdateOneIter": (C.c_int, [_H, C.c_int32]),
     "B2_BoosterBoostOneIter": (C.c_int, [_H, _FP, _FP, C.c_int64]),
     "B2_BoosterRefreshOneIter": (C.c_int, [_H, _FP, _FP, C.c_int64]),
@@ -664,8 +665,36 @@ class EarlyStopException(Exception):
         self.best_iteration = best_iteration
 
 
-class callback:  # namespace shim: xgb.callback.TrainingCallback
+class LearningRateScheduler(TrainingCallback):
+    """xgboost.callback.LearningRateScheduler: a learning rate per boosting round.
+
+    learning_rates: a sequence of rates, or a callable that takes the epoch and returns the rate.  After round `epoch`
+    the callback calls ``model.set_param("learning_rate", rate)`` with rate ``learning_rates[epoch]`` (or
+    ``learning_rates(epoch)``), so rate i applies from round i + 1 and the first round trains with the params' eta.
+    That is the after_iteration hook xgboost 1.3-2.x uses as far as recalled; it could not be checked against
+    xgboost's source.  Epochs restart at 0 in every train() call, also when it continues from xgb_model.
+
+    Actors receive their callbacks pickled: a sequence is stored as a tuple of floats, so the callback pickles; a
+    callable must be picklable itself (a module-level function, not a lambda)."""
+
+    def __init__(self, learning_rates):
+        if callable(learning_rates):
+            self.learning_rates = learning_rates
+        elif isinstance(learning_rates, (list, tuple, np.ndarray)):
+            self.learning_rates = tuple(float(r) for r in np.asarray(learning_rates, np.float64).reshape(-1))
+        else:
+            raise TypeError("learning_rates must be a sequence of rates or a callable of the epoch, got %r"
+                            % (type(learning_rates).__name__,))
+
+    def after_iteration(self, model, epoch, evals_log):
+        rates = self.learning_rates
+        model.set_param("learning_rate", rates(epoch) if callable(rates) else rates[epoch])
+        return False
+
+
+class callback:  # namespace shim: xgb.callback.TrainingCallback, xgb.callback.LearningRateScheduler
     TrainingCallback = TrainingCallback
+    LearningRateScheduler = LearningRateScheduler
 
 
 # ----------------------------------------------------------------------------- Booster
@@ -763,6 +792,10 @@ _ENGINE_KEYS = ("objective", "num_class", "max_depth", "eta", "learning_rate", "
                 "lambdarank_unbiased", "ndcg_exp_gain", "booster", "rate_drop", "skip_drop", "sample_type",
                 "normalize_type", "one_drop", "quantile_alpha", "num_target", "multi_strategy", "process_type",
                 "updater", "refresh_leaf")
+# xgboost's parameter aliases among the engine's keys
+_ALIASES = {"eta": ("learning_rate",), "learning_rate": ("eta",), "gamma": ("min_split_loss",),
+            "min_split_loss": ("gamma",), "lambda": ("reg_lambda",), "reg_lambda": ("lambda",), "alpha": ("reg_alpha",),
+            "reg_alpha": ("alpha",), "seed": ("random_state",), "random_state": ("seed",)}
 # booster=dart's parameters with xgboost's defaults (save_config's dart_train_param)
 _DART_DEFAULTS = {"rate_drop": 0.0, "skip_drop": 0.0, "sample_type": "uniform", "normalize_type": "tree", "one_drop": 0}
 
@@ -911,6 +944,7 @@ class Booster:
         h = _H(0)
         _check(lib().B2_BoosterCreate(self._param_text(extra), dtrain.handle, _coll.handle, C.byref(h)))
         self.handle = h.value
+        self._trained = False   # set_param takes effect through the engine once a round has run
         # the engine takes the targets from the train matrix's label; the model keeps them for its file and predictions
         nt = C.c_int32(1)
         _check(lib().B2_BoosterNumTargets(self.handle, C.byref(nt)))
@@ -1088,8 +1122,10 @@ class Booster:
             return
         if is_update_mode(self.params):   # refresh round `iteration` of the model's trees (DESIGN.md 2 item 20)
             _check(lib().B2_BoosterRefreshOneIter(self.handle, None, None, 0))
+            self._trained = True
             return
         _check(lib().B2_BoosterUpdateOneIter(self.handle, int(iteration)))
+        self._trained = True
         self._sync_base_score()
 
     def _sync_base_score(self):
@@ -1110,8 +1146,10 @@ class Booster:
             raise XGBoostError("grad / hess size mismatch")
         if is_update_mode(self.params):
             _check(lib().B2_BoosterRefreshOneIter(self.handle, _fp(g), _fp(h), g.size))
+            self._trained = True
             return
         _check(lib().B2_BoosterBoostOneIter(self.handle, _fp(g), _fp(h), g.size))
+        self._trained = True
         self._sync_base_score()
 
     def _metric_names(self):
@@ -1231,9 +1269,32 @@ class Booster:
         return dict(self._attrs)
 
     def set_param(self, params, value=None):
+        """Booster.set_param.  Once the device booster has trained a round, the engine's keys of the change go to the
+        engine (B2_BoosterSetParam): the keys a round may change apply from the next round, any other engine key may
+        only repeat its value, and a refused change raises XGBoostError and changes nothing.  Before the first round the
+        next update() creates the device booster from the new parameters.  Other keys only update the dict."""
         if isinstance(params, str):
             params = {params: value}
-        self.params.update(_params_dict(params))
+        params = _params_dict(params)
+        engine = {k: v for k, v in params.items() if k in _ENGINE_KEYS or k == "interaction_constraints"}
+        if engine and self.handle and self._train is not None:
+            if getattr(self, "_trained", False):
+                sets = engine.pop("interaction_constraints", None)
+                extra = None
+                if sets is not None:
+                    sets = interaction_sets(sets, self.n_features, self.feature_names)
+                    extra = {"interaction_constraints": ";".join(",".join(map(str, s)) for s in sets)}
+                _check(lib().B2_BoosterSetParam(self.handle, _engine_text(engine, extra)))
+                # the model's params now say what the next rounds are grown with: an alias given earlier would
+                # otherwise win over the new value when the booster is created again (_attach, checkpoints)
+                for k in engine:
+                    for alias in _ALIASES.get(k, ()):
+                        self.params.pop(alias, None)
+            else:
+                self.get_trees()
+                self.get_tree_weights()
+                self._free()
+        self.params.update(params)
 
     # -- (de)serialisation: XGBoost's JSON model format (doc/model.schema of dmlc/xgboost 2.x; SURVEY.md 8f-1).  Everything
     # a stock xgboost needs is where it expects it (objective parameter block, learner_model_param, gbtree_model_param,
