@@ -18,7 +18,7 @@ import threading
 import uuid
 from concurrent.futures import ThreadPoolExecutor
 from enum import Enum
-from typing import Dict, Iterable, List, Optional, Sequence
+from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -330,13 +330,18 @@ class RayDMatrix:
             raise ValueError(f"Distributed data loading is not supported for input data of type {type(data)}. "
                              f"\nFIX THIS by passing file names or setting `distributed=False`.")
         self.distributed = bool(distributed)
-        if self.distributed and qid is not None:
-            raise ValueError("ranking (qid) with distributed loading (a list of files read by the actors) is not "
-                             "supported: a query group may span files.\nFIX THIS by loading the data centrally "
-                             "(`distributed=False`).")
-        self._row_index: Optional[List[np.ndarray]] = None   # qid: rows of every rank in the qid-sorted order
+        if self.distributed and qid is not None and not isinstance(qid, str):
+            raise ValueError("with distributed loading (a list of files read by the actors) `qid` must be the name of a "
+                             "column of the files: an array of ids cannot be split among the files, whose row counts "
+                             "only the actors that read them know.\nFIX THIS by storing the query id as a column of "
+                             "every file and passing its name, or by loading the data centrally (`distributed=False`).")
+        self._row_index: Optional[List[np.ndarray]] = None   # qid: rows of every rank in the prediction order
+        # distributed qid: file index -> (row count, sorted distinct qids) of every file read so far
+        self._file_groups: Dict[int, Tuple[int, np.ndarray]] = {}
         if self.distributed:
             self.sharding = RayShardingMode.FIXED if sharding == RayShardingMode.FIXED else sharding
+        # how a file list is dealt to the ranks: BATCH, otherwise INTERLEAVED (file i to rank i mod W)
+        self._file_sharding = RayShardingMode.BATCH if sharding == RayShardingMode.BATCH else RayShardingMode.INTERLEAVED
         self.refs: Dict[int, Dict[str, Optional[np.ndarray]]] = {}
         self._shared: Dict[int, Dict] = {}      # rank -> {field: ('shm', path) | ndarray | None}: what an actor is sent
         self.n = None
@@ -386,6 +391,54 @@ class RayDMatrix:
                 self._inferred_types = list(x.feature_types)
         return x, y, w, fw, b, ll, lu
 
+    def _rank_files(self, rank: int, num_actors: int, n_files: int) -> List[int]:
+        """Indices of the files that `rank` reads (distributed loading)."""
+        return list(range(n_files))[_get_sharding_indices(self._file_sharding, rank, num_actors, n_files)]
+
+    def _file_name(self, i: int) -> str:
+        return self.data if isinstance(self.data, str) else str(self.data[i])
+
+    def _sort_file_by_qid(self, i: int, part, q: np.ndarray):
+        """The rows of file `i` stably sorted by qid (merge sort, skipped when the file is already non-decreasing), and
+        the sizes of its query groups.  Records the file's row count and sorted distinct ids for check_file_groups."""
+        x, y, w, fw, b, ll, lu = part
+        order = None if len(q) < 2 or not np.any(q[1:] < q[:-1]) else np.argsort(q, kind="mergesort")
+        qs = q if order is None else q[order]
+        offsets = group_offsets(qs)
+        self._file_groups[i] = (len(qs), qs[offsets[:-1]])
+        if order is not None:
+            x = LoadedFrame(x.values[order], x.columns, x.feature_types)
+            y, w, b, ll, lu = (None if a is None else a[order] for a in (y, w, b, ll, lu))
+        return (x, y, w, fw, b, ll, lu), np.diff(offsets)
+
+    def check_file_groups(self, num_actors: int):
+        """Distributed qid, once the files have been read: refuse a query id that appears in two files (every group
+        must lie in exactly one file, the unit the actors read), and set the prediction order -- the files in list
+        order, each file's rows in its stable qid order -- for any number of actors."""
+        idx = sorted(self._file_groups)
+        ids = [self._file_groups[i][1] for i in idx]
+        if ids:
+            owner = np.repeat(np.asarray(idx, np.int64), [len(v) for v in ids])
+            ids = np.concatenate(ids)
+            order = np.argsort(ids, kind="mergesort")       # stable: of two equal ids the lower file index comes first
+            ids, owner = ids[order], owner[order]
+            dup = np.flatnonzero(ids[1:] == ids[:-1])
+            if dup.size:
+                j = int(dup[0])
+                v = float(ids[j])
+                raise ValueError(f"query id {int(v) if v.is_integer() else v} appears in two files, "
+                                 f"{self._file_name(int(owner[j]))!r} and {self._file_name(int(owner[j + 1]))!r}: with "
+                                 f"distributed loading every query group must lie in exactly one file.\nFIX THIS by "
+                                 f"writing all rows of each query group into one file, or by loading the data centrally "
+                                 f"(`distributed=False`).")
+        n_files = self.data_source.get_n(self.data)
+        if len(idx) != n_files:
+            return
+        start = np.r_[0, np.cumsum([self._file_groups[i][0] for i in range(n_files)])].astype(np.int64)
+        self._row_index = [np.concatenate([np.arange(start[i], start[i + 1]) for i in files]).astype(np.int64)
+                           if files else np.zeros(0, np.int64)
+                           for files in (self._rank_files(r, num_actors, n_files) for r in range(num_actors))]
+
     def load_data(self, num_actors: Optional[int] = None, rank: Optional[int] = None, transport: Optional[str] = None):
         """Central loading (matrix.py:431-487): read once, shard per rank.  Distributed (file lists,
         matrix.py:614-693): rank r reads files r, r+W, ... itself.  transport = "remote": the feature matrix is NOT
@@ -413,23 +466,36 @@ class RayDMatrix:
             total = 0
             cat = lambda parts: None if parts[0] is None else np.concatenate(parts)  # noqa: E731
             for r in ranks:
-                idx = list(range(n_files))[_get_sharding_indices(
-                    RayShardingMode.INTERLEAVED if self.sharding != RayShardingMode.BATCH else RayShardingMode.BATCH,
-                    r, W, n_files)]
+                idx = self._rank_files(r, W, n_files)
                 # one row block per file (matrix.py:127-196: the shards of an actor stay separate and go to the device
                 # matrix one by one); only the small side columns are concatenated
-                parts = [self._split(self.data_source.load_data(self.data, ignore=self.ignore, indices=[i], **self.kwargs))
-                         for i in idx]
+                parts, sizes = [], []
+                for i in idx:
+                    part = self._split(self.data_source.load_data(self.data, ignore=self.ignore, indices=[i], **self.kwargs))
+                    if self._qid_rows is not None:
+                        part, group_sizes = self._sort_file_by_qid(i, part, self._qid_rows)
+                        sizes.append(group_sizes)
+                    parts.append(part)
                 self._columns = parts[0][0].columns
                 blocks = [p[0].values for p in parts]
                 self.refs[r] = {"data": blocks if len(blocks) > 1 else blocks[0], "label": cat([p[1] for p in parts]),
                                 "weight": cat([p[2] for p in parts]), "feature_weights": parts[0][3],
                                 "base_margin": cat([p[4] for p in parts]), "label_lower_bound": cat([p[5] for p in parts]),
                                 "label_upper_bound": cat([p[6] for p in parts]), "qid": None}
+                if self.qid is not None:
+                    # no group spans files, so the sorted blocks of this rank keep every group contiguous: its qid is
+                    # the rank-local group number, as in _load_groups (exact in float32 up to 2^24 groups)
+                    sizes = np.concatenate(sizes)
+                    if len(sizes) > (1 << 24):
+                        raise ValueError(f"rank {r} holds {len(sizes)} query groups; at most 2^24 fit the float32 "
+                                         f"group numbers of a shard.\nFIX THIS by using more actors.")
+                    self.refs[r]["qid"] = np.repeat(np.arange(len(sizes)), sizes).astype(np.float32)
                 self._shared[r] = dict(self.refs[r])
                 total += sum(len(b) for b in blocks)
             self.n = total if rank is None else self.n
             self.sharding = RayShardingMode.FIXED
+            if self.qid is not None and rank is None:
+                self.check_file_groups(W)
         elif self.data_source is Sparse:
             self._load_sparse(W)
         else:
@@ -568,6 +634,7 @@ class RayDMatrix:
         (distributed loading, matrix.py:614-693)."""
         m = copy.copy(self)
         m.refs, m._shared, m.loaded = {}, {}, False
+        m._file_groups, m._row_index = {}, None
         return m
 
     def unload_data(self):
