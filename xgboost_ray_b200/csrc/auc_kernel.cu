@@ -22,21 +22,6 @@ __device__ __forceinline__ uint32_t desc_key(float v) {
   return ~u;                                        // descending
 }
 
-// sum of v over the CTA in a fixed order (butterfly within each warp, then warp 0 over the warp sums); every thread
-// must call it; the result is valid in thread 0
-__device__ __forceinline__ double block_sum_fixed(double v, double* sh /* [32] */) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    v = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0.0;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  }
-  return v;
-}
-
 // keys of class c: pred is [n, K] row-major
 __global__ void auc_keys_kernel(const float* __restrict__ pred, int K, int c, int64_t n, uint32_t* __restrict__ keys,
                                 int32_t* __restrict__ idx) {
@@ -93,7 +78,7 @@ __global__ void auc_area_kernel(int pr, const double* __restrict__ tp, const dou
     const double tp0 = prev >= 0 ? tp[prev] : 0.0, fp0 = prev >= 0 ? fp[prev] : 0.0;
     area += pr ? pr_segment(tp0, fp0, tp[p], fp[p], P) : fabs(fp[p] - fp0) * (tp[p] + tp0) * 0.5;
   }
-  area = block_sum_fixed(area, sh);
+  area = b2_block_sum_fixed(area, sh);
   if (threadIdx.x == 0) partial[blockIdx.x] = area;
 }
 // one CTA: the class's contribution out3 = ROC (area, fp * tp, tp) or PR (aucpr, 1, 1), aucpr NaN without positive or
@@ -103,7 +88,7 @@ __global__ void auc_finish_kernel(int pr, const double* __restrict__ partial, in
   __shared__ double sh[32];
   double s = 0.0;
   for (int i = threadIdx.x; i < g; i += blockDim.x) s += partial[i];
-  s = block_sum_fixed(s, sh);
+  s = b2_block_sum_fixed(s, sh);
   if (threadIdx.x == 0) {
     const double P = n > 0 ? tp[n - 1] : 0.0, N = n > 0 ? fp[n - 1] : 0.0;
     if (pr) { out3[0] = (P > 0.0 && N > 0.0) ? s : __longlong_as_double(0x7ff8000000000000LL); out3[1] = 1.0; out3[2] = 1.0; }

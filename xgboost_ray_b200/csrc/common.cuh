@@ -37,6 +37,30 @@ __device__ __forceinline__ double b2_limbs_to_double(long long hi, long long lo)
   return __dadd_rn(__dmul_rn(__ll2double_rn(hi), (double)(1ll << B2_LIMB_SHIFT)), __ll2double_rn(lo));
 }
 
+// ---- double sums in a fixed order (AUC areas, eval metrics): the same bits on every call, no floating-point atomics.
+// Sum of v over the CTA: butterfly within each warp, then warp 0 over the warp sums.  Every thread must call it; the
+// result is valid in thread 0.
+__device__ __forceinline__ double b2_block_sum_fixed(double v, double* sh /* [32] */) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    v = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0.0;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  }
+  return v;
+}
+// a metric kernel's CTA: its threads' (sum w v, sum w) summed in a fixed order into partial[2 blockIdx.x + {0, 1}],
+// which b2_launch_metric_sum then adds up in CTA order
+__device__ __forceinline__ void b2_metric_partial(double s, double ws, double* __restrict__ partial) {
+  __shared__ double sh_s[32], sh_w[32];
+  s = b2_block_sum_fixed(s, sh_s);
+  ws = b2_block_sum_fixed(ws, sh_w);
+  if (threadIdx.x == 0) { partial[2 * blockIdx.x] = s; partial[2 * blockIdx.x + 1] = ws; }
+}
+
 // ---- fixed-point quantisation scale.  e is frexpf's exponent of a non-negative binary32 max (2^(e-1) <= max < 2^e,
 // 0 for 0), from its bit pattern: a subnormal max = m * 2^-149 with bit_length(m) = L lies in [2^(L-150), 2^(L-149)),
 // so e = L - 149, from -148 (m = 1) to -126 (the largest subnormal).  Used for gradients, hessians and sketch weights.

@@ -121,15 +121,21 @@ int b2_launch_gradient(int objective, int K, const float* margin, const float* l
 int b2_launch_gradient_multi_target(int objective, int T, const float* margin, const float* label, const float* weight,
                                     int64_t n, float scale_pos_weight, float obj_param, float2* gh, uint32_t* absmax,
                                     uint32_t* err, int num_sms, cudaStream_t s);
+// The metric launchers (metric, metric_multi_target, aft_metric, quantile_metric) write out[0..1] = (sum w v, sum w)
+// in a fixed order, so the same model and matrix give the same bits on every call on one GPU model: each CTA's sums go
+// to partial, b2_metric_partial_doubles(num_sms) doubles of device scratch, and b2_launch_metric_sum adds the first g
+// pairs of it in CTA order.  n <= 0 launches nothing and leaves out as it is.
+size_t b2_metric_partial_doubles(int num_sms);
+int b2_launch_metric_sum(const double* partial, int g, double* out, cudaStream_t s);
 int b2_launch_metric_multi_target(int objective, int metric, int T, float metric_param, const float* margin,
-                                  const float* label, const float* weight, int64_t n, double* out, int num_sms,
-                                  cudaStream_t s);
+                                  const float* label, const float* weight, int64_t n, double* partial, double* out,
+                                  int num_sms, cudaStream_t s);
 int b2_launch_gradient_aft(int dist, double sigma, const float* margin, const float* lower, const float* upper,
                            const float* weight, int64_t n, float2* gh, uint32_t* absmax, uint32_t* err, int num_sms,
                            cudaStream_t s);
 int b2_launch_aft_bounds_check(const float* lower, const float* upper, int64_t n, uint32_t* bad, int num_sms, cudaStream_t s);
 int b2_launch_aft_metric(int dist, int metric, double sigma, const float* margin, const float* lower, const float* upper,
-                         const float* weight, int64_t n, double* out, int num_sms, cudaStream_t s);
+                         const float* weight, int64_t n, double* partial, double* out, int num_sms, cudaStream_t s);
 int b2_launch_label_check(int objective, int K, const float* label, int64_t n, uint32_t* bad, int num_sms, cudaStream_t s);
 int b2_launch_subsample(float2* gh, int64_t n, uint32_t seed, uint32_t tree, uint32_t rank, double subsample, int num_sms,
                         cudaStream_t s);
@@ -138,8 +144,9 @@ int b2_launch_pack_custom(const float* g, const float* h, int K, int64_t n, floa
 int b2_launch_absmax(const float2* gh, int64_t n, uint32_t* absmax, int num_sms, cudaStream_t s);
 int b2_launch_quant_exponent(const uint32_t* absmax, int32_t* qexp, cudaStream_t s);
 int b2_launch_quantize(const float2* gh, int64_t n, const int32_t* qexp, int qbits, int2* q, int num_sms, cudaStream_t s);
+// out[2] += the rows of mlogloss / merror whose label is not a class index
 int b2_launch_metric(int objective, int metric, int K, float metric_param, const float* margin, const float* label,
-                     const float* weight, int64_t n, double* out, int num_sms, cudaStream_t s);
+                     const float* weight, int64_t n, double* partial, double* out, int num_sms, cudaStream_t s);
 int b2_launch_predict(const float* X, int64_t n, int F, float missing, const B2TreeNodeDev* nodes, const int32_t* tree_offset,
                       const uint32_t* cat_table, int tree_begin, int tree_end, int K, int npt, const float* weights, float* out,
                       int num_sms, cudaStream_t s);
@@ -156,7 +163,7 @@ int b2_quantile_passes();
 int b2_launch_gradient_quantile(int K, const float* alpha, const float* margin, const float* label, const float* weight,
                                 int64_t n, float2* gh, uint32_t* absmax, int num_sms, cudaStream_t s);
 int b2_launch_quantile_metric(int K, const float* alpha, const float* margin, const float* label, const float* weight,
-                              int64_t n, double* out, int num_sms, cudaStream_t s);
+                              int64_t n, double* partial, double* out, int num_sms, cudaStream_t s);
 int b2_launch_quantile_count(int pass, const uint16_t* pos, const float* label, const float* margin, int K, int k,
                              const float2* gh, int64_t n, const int32_t* qexp, int weighted, const void* sel,
                              int max_leaves, unsigned long long* hist, int num_sms, cudaStream_t s);

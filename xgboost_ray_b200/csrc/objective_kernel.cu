@@ -406,7 +406,7 @@ __global__ void aft_bounds_check_kernel(const float* __restrict__ lower, const f
   if (__any_sync(0xffffffffu, b3) && (threadIdx.x & 31) == 0) atomicOr(&bad[3], 1u);
 }
 
-// aft-nloglik and interval-regression-accuracy: (sum w v, sum w) in double
+// aft-nloglik and interval-regression-accuracy: each CTA's (sum w v, sum w) in double
 template <int kDist>
 __device__ __forceinline__ double aft_metric_value(int metric, float m, float lower, float upper, double sigma) {
   if (metric == kMetricAftNloglik) return aft_loss<kDist>((double)m, lower, upper, sigma);
@@ -415,7 +415,7 @@ __device__ __forceinline__ double aft_metric_value(int metric, float m, float lo
 }
 __global__ void aft_metric_kernel(int dist, int metric, double sigma, const float* __restrict__ margin,
                                   const float* __restrict__ lower, const float* __restrict__ upper,
-                                  const float* __restrict__ weight, int64_t n, double* __restrict__ out) {
+                                  const float* __restrict__ weight, int64_t n, double* __restrict__ partial) {
   double s = 0.0, ws = 0.0;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const double w = weight ? (double)weight[i] : 1.0;
@@ -424,9 +424,7 @@ __global__ void aft_metric_kernel(int dist, int metric, double sigma, const floa
                    : aft_metric_value<kAftExtreme>(metric, margin[i], lower[i], upper[i], sigma);
     s += v * w; ws += w;
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ws += __shfl_xor_sync(0xffffffffu, ws, o); }
-  if ((threadIdx.x & 31) == 0) { atomicAdd(&out[0], s); atomicAdd(&out[1], ws); }
+  b2_metric_partial(s, ws, partial);
 }
 
 __global__ void gradient_softprob_kernel(int K, const float* __restrict__ margin, const float* __restrict__ label,
@@ -547,7 +545,9 @@ __global__ void quantize_kernel(const float2* __restrict__ gh, int64_t n, const 
   }
 }
 
-// metric sums (sum loss*w, sum w, rows with an invalid class label) -> out[3] doubles.  Metrics see the TRANSFORMED prediction (ObjFunction::EvalTransform,
+// metric sums (sum loss*w, sum w, rows with an invalid class label) -> out[3] doubles: the metric kernels write each
+// CTA's (sum loss*w, sum w) to partial, metric_sum_kernel adds them in CTA order, so a value has the same bits on every
+// call on the same GPU model.  Metrics see the TRANSFORMED prediction (ObjFunction::EvalTransform,
 // src/learner.cc): the probability for binary:logistic / reg:logistic, exp(margin) for the log-link objectives, the raw
 // value otherwise.  a: huber_slope of mphe, rho of tweedie-nloglik.  auc and aucpr are auc_kernel.cu.
 // the elementwise metrics of the objectives added after the first three, on the transformed prediction q
@@ -578,19 +578,17 @@ __device__ __forceinline__ double elementwise_metric(int objective, int metric, 
 }
 
 // elementwise metrics of a multi-target model over the n*T elements of margin and label [n][T]: element (i, k) counts
-// with row i's weight, so out = (sum w_i v_ik, T * sum w_i)
+// with row i's weight, so the sums are (sum w_i v_ik, T * sum w_i)
 __global__ void metric_multi_target_kernel(int objective, int metric, int T, float a, const float* __restrict__ margin,
                                            const float* __restrict__ label, const float* __restrict__ weight, int64_t n,
-                                           double* __restrict__ out) {
+                                           double* __restrict__ partial) {
   double s = 0.0, ws = 0.0;
   const int64_t nt = n * T;
   for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < nt; j += (int64_t)gridDim.x * blockDim.x) {
     const double w = weight ? (double)weight[j / T] : 1.0;
     s += elementwise_metric(objective, metric, a, margin[j], label[j]) * w; ws += w;
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ws += __shfl_xor_sync(0xffffffffu, ws, o); }
-  if ((threadIdx.x & 31) == 0) { atomicAdd(&out[0], s); atomicAdd(&out[1], ws); }
+  b2_metric_partial(s, ws, partial);
 }
 
 // a multi-class label is a class index in [0, K): non-integer labels truncate (2.7 -> class 2); NaN is outside
@@ -600,7 +598,7 @@ __device__ __forceinline__ bool b2_class_label_ok(float y, int K) { return y >= 
 // never read for them) and the caller fails the evaluation
 __global__ void metric_kernel(int objective, int metric, int K, float a, const float* __restrict__ margin,
                               const float* __restrict__ label, const float* __restrict__ weight, int64_t n,
-                              double* __restrict__ out) {
+                              double* __restrict__ partial, double* __restrict__ out) {
   double s = 0.0, ws = 0.0;
   unsigned bad = 0;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -624,13 +622,19 @@ __global__ void metric_kernel(int objective, int metric, int K, float a, const f
     }
     s += v * w; ws += w;
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ws += __shfl_xor_sync(0xffffffffu, ws, o); }
+  b2_metric_partial(s, ws, partial);
   bad = __reduce_add_sync(0xffffffffu, bad);
-  if ((threadIdx.x & 31) == 0) {
-    atomicAdd(&out[0], s); atomicAdd(&out[1], ws);
-    if (bad) atomicAdd(&out[2], (double)bad);
-  }
+  if ((threadIdx.x & 31) == 0 && bad) atomicAdd(&out[2], (double)bad);   // integer counts: exact in any order
+}
+
+// one CTA: out[0..1] = the g CTA partials (sum, weight sum) of a metric kernel, added in a fixed order
+__global__ void __launch_bounds__(256) metric_sum_kernel(const double* __restrict__ partial, int g, double* __restrict__ out) {
+  __shared__ double sh_s[32], sh_w[32];
+  double s = 0.0, ws = 0.0;
+  for (int i = threadIdx.x; i < g; i += blockDim.x) { s += partial[2 * i]; ws += partial[2 * i + 1]; }
+  s = b2_block_sum_fixed(s, sh_s);
+  ws = b2_block_sum_fixed(ws, sh_w);
+  if (threadIdx.x == 0) { out[0] = s; out[1] = ws; }
 }
 
 // label domain of an objective (checked once per train matrix): *bad |= 1 when some label is outside it (NaN included);
@@ -709,9 +713,10 @@ __global__ void transform_kernel(int objective, int K, float* __restrict__ m, in
 
 }  // namespace b2
 
+static constexpr int kMaxCtasPerSm = 16;
 static inline int grid_for(int64_t n, int num_sms) {
   int64_t g = (n + 255) / 256;
-  int64_t cap = (int64_t)num_sms * 16;
+  int64_t cap = (int64_t)num_sms * kMaxCtasPerSm;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
   return (int)g;
@@ -762,13 +767,18 @@ int b2_launch_gradient_multi_target(int objective, int T, const float* margin, c
   }
   return (int)cudaGetLastError();
 }
-int b2_launch_metric_multi_target(int objective, int metric, int T, float metric_param, const float* margin,
-                                  const float* label, const float* weight, int64_t n, double* out, int num_sms,
-                                  cudaStream_t s) {
-  if (n <= 0) return 0;
-  b2::metric_multi_target_kernel<<<grid_for(n * T, num_sms), 256, 0, s>>>(objective, metric, T, metric_param, margin, label,
-                                                                          weight, n, out);
+size_t b2_metric_partial_doubles(int num_sms) { return 2 * (size_t)num_sms * kMaxCtasPerSm; }
+int b2_launch_metric_sum(const double* partial, int g, double* out, cudaStream_t s) {
+  b2::metric_sum_kernel<<<1, 256, 0, s>>>(partial, g, out);
   return (int)cudaGetLastError();
+}
+int b2_launch_metric_multi_target(int objective, int metric, int T, float metric_param, const float* margin,
+                                  const float* label, const float* weight, int64_t n, double* partial, double* out,
+                                  int num_sms, cudaStream_t s) {
+  if (n <= 0) return 0;
+  const int g = grid_for(n * T, num_sms);
+  b2::metric_multi_target_kernel<<<g, 256, 0, s>>>(objective, metric, T, metric_param, margin, label, weight, n, partial);
+  return b2_launch_metric_sum(partial, g, out, s);
 }
 int b2_launch_gradient_aft(int dist, double sigma, const float* margin, const float* lower, const float* upper,
                            const float* weight, int64_t n, float2* gh, uint32_t* absmax, uint32_t* err, int num_sms,
@@ -790,10 +800,11 @@ int b2_launch_aft_bounds_check(const float* lower, const float* upper, int64_t n
   return (int)cudaGetLastError();
 }
 int b2_launch_aft_metric(int dist, int metric, double sigma, const float* margin, const float* lower, const float* upper,
-                         const float* weight, int64_t n, double* out, int num_sms, cudaStream_t s) {
+                         const float* weight, int64_t n, double* partial, double* out, int num_sms, cudaStream_t s) {
   if (n <= 0) return 0;
-  b2::aft_metric_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(dist, metric, sigma, margin, lower, upper, weight, n, out);
-  return (int)cudaGetLastError();
+  const int g = grid_for(n, num_sms);
+  b2::aft_metric_kernel<<<g, 256, 0, s>>>(dist, metric, sigma, margin, lower, upper, weight, n, partial);
+  return b2_launch_metric_sum(partial, g, out, s);
 }
 int b2_launch_label_check(int objective, int K, const float* label, int64_t n, uint32_t* bad, int num_sms, cudaStream_t s) {
   if (n <= 0) return 0;
@@ -831,10 +842,11 @@ int b2_launch_quantize(const float2* gh, int64_t n, const int32_t* qexp, int qbi
   return (int)cudaGetLastError();
 }
 int b2_launch_metric(int objective, int metric, int K, float metric_param, const float* margin, const float* label,
-                     const float* weight, int64_t n, double* out, int num_sms, cudaStream_t s) {
+                     const float* weight, int64_t n, double* partial, double* out, int num_sms, cudaStream_t s) {
   if (n <= 0) return 0;
-  b2::metric_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(objective, metric, K, metric_param, margin, label, weight, n, out);
-  return (int)cudaGetLastError();
+  const int g = grid_for(n, num_sms);
+  b2::metric_kernel<<<g, 256, 0, s>>>(objective, metric, K, metric_param, margin, label, weight, n, partial, out);
+  return b2_launch_metric_sum(partial, g, out, s);
 }
 int b2_launch_predict(const float* X, int64_t n, int F, float missing, const B2TreeNodeDev* nodes,
                       const int32_t* tree_offset, const uint32_t* cat_table, int tree_begin, int tree_end, int K, int npt,

@@ -191,8 +191,10 @@ double eval_metric(Booster* b, Matrix* m, const char* name) {
     fail("metric '%s' is not supported for a multi-target model (supported: rmse, rmsle, mae, mape, mphe, logloss, error)",
          name);
   const float* w = m->n_weight ? m->weight.p : nullptr;
-  b->d_metric.ensure(3 * (size_t)K + 1);
-  CUDA_CHECK(cudaMemsetAsync(b->d_metric.p, 0, 3 * sizeof(double), s));   // the aft, quantile and elementwise sums
+  // d_metric: the AUC triples, or the aft, quantile and elementwise sums followed by their per-CTA partials
+  b->d_metric.ensure(std::max(3 * (size_t)K + 1, 3 + b2_metric_partial_doubles(sms)));
+  CUDA_CHECK(cudaMemsetAsync(b->d_metric.p, 0, 3 * sizeof(double), s));
+  double* partial = b->d_metric.p + 3;
   DevBuf<float> pred;   // the ranking and AUC metrics read the transformed prediction
   if (rank || auc) {
     pred.ensure((size_t)std::max<int64_t>(m->n * K, 1));
@@ -235,7 +237,7 @@ double eval_metric(Booster* b, Matrix* m, const char* name) {
     }
     case kEvalAft:
       LAUNCH_CHECK(b2_launch_aft_metric(p.aft_dist, mt.id, (double)p.aft_sigma, margin, m->lower.p, m->upper.p, w, m->n,
-                                        b->d_metric.p, sms, s));
+                                        partial, b->d_metric.p, sms, s));
       break;
     case kEvalQuantile:
       // pinball loss averaged over the rows and the alphas, weighted (sum, K * sum w summed over the workers)
@@ -243,16 +245,17 @@ double eval_metric(Booster* b, Matrix* m, const char* name) {
         upload(b->d_alpha, p.quantile_alpha, s);
         CUDA_CHECK(cudaStreamSynchronize(s));
       }
-      LAUNCH_CHECK(b2_launch_quantile_metric(K, b->d_alpha.p, margin, m->label.p, w, m->n, b->d_metric.p, sms, s));
+      LAUNCH_CHECK(b2_launch_quantile_metric(K, b->d_alpha.p, margin, m->label.p, w, m->n, partial, b->d_metric.p, sms, s));
       break;
     default: {
       // elementwise (over the n x T outputs of a multi-target model, each with its row's weight: xgboost's EvalEWiseBase)
       // and class metrics: (sum, wsum, rows with a label outside [0, num_class)), so every rank fails together
       if (p.num_target > 1)
         LAUNCH_CHECK(b2_launch_metric_multi_target(p.objective, mt.id, p.num_target, mparam, margin, m->label.p, w, m->n,
-                                                   b->d_metric.p, sms, s));
+                                                   partial, b->d_metric.p, sms, s));
       else
-        LAUNCH_CHECK(b2_launch_metric(p.objective, mt.id, K, mparam, margin, m->label.p, w, m->n, b->d_metric.p, sms, s));
+        LAUNCH_CHECK(b2_launch_metric(p.objective, mt.id, K, mparam, margin, m->label.p, w, m->n, partial, b->d_metric.p,
+                                      sms, s));
       const std::vector<double> h = metric_sums(b, 3, s);
       if (h[2] > 0) fail("metric '%s': label must be in [0, num_class), num_class = %d (%.0f rows outside)", name, K, h[2]);
       const double v = h[1] > 0 ? h[0] / h[1] : 0.0;

@@ -71,10 +71,11 @@ gradient_quantile_kernel(int K, const float* __restrict__ alpha, const float* __
   }
 }
 
-// ---- the quantile metric: (sum_i w_i sum_k rho_{alpha_k}(y_i - p_ik), K sum_i w_i), rho_a(u) = u (a - [u < 0])
+// ---- the quantile metric: (sum_i w_i sum_k rho_{alpha_k}(y_i - p_ik), K sum_i w_i), rho_a(u) = u (a - [u < 0]), one
+// pair per CTA in partial (b2_metric_partial)
 __global__ void quantile_metric_kernel(int K, const float* __restrict__ alpha, const float* __restrict__ margin,
                                        const float* __restrict__ label, const float* __restrict__ weight, int64_t n,
-                                       double* __restrict__ out) {
+                                       double* __restrict__ partial) {
   double s = 0.0, ws = 0.0;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const double w = weight ? (double)weight[i] : 1.0, y = (double)label[i];
@@ -85,9 +86,7 @@ __global__ void quantile_metric_kernel(int K, const float* __restrict__ alpha, c
     }
     s += v * w; ws += w * (double)K;
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ws += __shfl_xor_sync(0xffffffffu, ws, o); }
-  if ((threadIdx.x & 31) == 0) { atomicAdd(&out[0], s); atomicAdd(&out[1], ws); }
+  b2_metric_partial(s, ws, partial);
 }
 
 // ---- count pass.  hist: count[L][2][256] then (weighted) mass[L][2][256], uint64.  Slot 1 holds the second target's
@@ -273,10 +272,11 @@ int b2_launch_gradient_quantile(int K, const float* alpha, const float* margin, 
 }
 
 int b2_launch_quantile_metric(int K, const float* alpha, const float* margin, const float* label, const float* weight,
-                              int64_t n, double* out, int num_sms, cudaStream_t s) {
+                              int64_t n, double* partial, double* out, int num_sms, cudaStream_t s) {
   if (n <= 0) return 0;
-  b2::quantile_metric_kernel<<<q_grid(n, num_sms), 256, 0, s>>>(K, alpha, margin, label, weight, n, out);
-  return (int)cudaGetLastError();
+  const int g = q_grid(n, num_sms);
+  b2::quantile_metric_kernel<<<g, 256, 0, s>>>(K, alpha, margin, label, weight, n, partial);
+  return b2_launch_metric_sum(partial, g, out, s);
 }
 
 // one pass of the selection: count (hist_reduce, nullable, is called between count and scan to sum the histograms over
