@@ -12,6 +12,8 @@ compute call raises ``XGBoostError``.
 import ast
 import ctypes as C
 import json
+import numbers
+import operator
 import os
 import sys
 import threading
@@ -692,9 +694,67 @@ class LearningRateScheduler(TrainingCallback):
         return False
 
 
-class callback:  # namespace shim: xgb.callback.TrainingCallback, xgb.callback.LearningRateScheduler
+class EarlyStopping(TrainingCallback):
+    """xgboost.callback.EarlyStopping: stop training once `rounds` rounds in a row have not improved a metric.
+
+    It watches metric `metric_name` of the eval set `data_name`; by default the last eval set of `evals` and its last
+    metric.  An unknown name raises ValueError naming it.  `maximize` defaults to the direction train(...,
+    early_stopping_rounds=) uses for the metric.  A round improves when `score - min_delta > best` (maximising) or
+    `best - min_delta > score` (minimising), so an equal score does not improve.  After every improving round the
+    model's best_iteration and best_score are set; best_iteration counts the model's rounds, those of xgb_model
+    included.  With save_best=True, after_training returns ``model[: best_iteration + 1]`` carrying both attributes
+    again.  These rules are recalled from xgboost 2.x's callback.py, not checked against its source (DESIGN.md 2
+    item 23).
+
+    The history starts again in before_training, so one instance can serve several train() calls.  Actors receive the
+    callback pickled; every rank sees the same allreduced metric values and stops at the same round.  An actor restart
+    re-sends the callbacks, so the history starts again at the checkpoint's round."""
+
+    def __init__(self, rounds, metric_name=None, data_name=None, maximize=None, save_best=False, min_delta=0.0):
+        if min_delta < 0:
+            raise ValueError("min_delta must be >= 0, got %r" % (min_delta,))
+        self.rounds = int(rounds)
+        self.metric_name, self.data_name, self.maximize = metric_name, data_name, maximize
+        self.save_best, self.min_delta = bool(save_best), float(min_delta)
+        self.starting_round, self.best, self.stale = 0, None, 0
+
+    def before_training(self, model):
+        self.starting_round, self.best, self.stale = model.num_boosted_rounds(), None, 0
+        return model
+
+    def after_iteration(self, model, epoch, evals_log):
+        if not evals_log:
+            raise ValueError("EarlyStopping needs at least one eval set (evals=)")
+        data = self.data_name if self.data_name is not None else list(evals_log)[-1]
+        if data not in evals_log:
+            raise ValueError("EarlyStopping: no eval set named %r (eval sets: %s)" % (data, ", ".join(evals_log)))
+        log = evals_log[data]
+        metric = self.metric_name if self.metric_name is not None else list(log)[-1]
+        if metric not in log:
+            raise ValueError("EarlyStopping: eval set %r has no metric named %r (metrics: %s)"
+                             % (data, metric, ", ".join(log)))
+        score = float(log[metric][-1])
+        mx = self.maximize if self.maximize is not None else _maximized(metric)
+        if self.best is None or (score - self.min_delta > self.best if mx else self.best - self.min_delta > score):
+            self.best, self.stale = score, 0
+            model.best_iteration, model.best_score = self.starting_round + epoch, score
+        else:
+            self.stale += 1
+        return self.stale >= self.rounds
+
+    def after_training(self, model):
+        if not self.save_best or model.best_iteration is None:
+            return model
+        best_iteration, best_score = model.best_iteration, model.best_score
+        model = model[: best_iteration + 1]
+        model.best_iteration, model.best_score = best_iteration, best_score
+        return model
+
+
+class callback:  # namespace shim: xgb.callback.TrainingCallback, LearningRateScheduler, EarlyStopping
     TrainingCallback = TrainingCallback
     LearningRateScheduler = LearningRateScheduler
+    EarlyStopping = EarlyStopping
 
 
 # ----------------------------------------------------------------------------- Booster
@@ -1536,6 +1596,53 @@ class Booster:
         b = Booster.__new__(Booster)
         b.__setstate__(self.__getstate__())
         return b
+
+    def __getitem__(self, val):
+        """bst[start:stop:step] / bst[i]: a new Booster with boosting rounds start, start + step, ... < stop.
+
+        A round is _trees_per_round consecutive trees.  An int i is i:i + 1; start None is 0, stop None or 0 is
+        num_boosted_rounds(), step None is 1.  A negative index, stop < start or step < 1 raises ValueError, a tuple
+        ValueError, another type TypeError, and start >= num_boosted_rounds() or stop > num_boosted_rounds() IndexError
+        (recalled from xgboost 2.x's Booster.__getitem__, DESIGN.md 2 item 23).  The slice keeps the params, the
+        features, the attributes and each kept tree unchanged (DART: its weight too); it drops best_iteration /
+        best_score, which index this model's rounds, and the frozen restart cuts.  It is built on the host: its device
+        predictor is created when it first predicts, and this booster keeps its device state and can train on."""
+        if isinstance(val, numbers.Integral):
+            val = slice(val, val + 1)
+        if isinstance(val, tuple):
+            raise ValueError("Booster slicing supports only 1 dimension, got %r" % (val,))
+        if not isinstance(val, slice):
+            raise TypeError("Booster indices must be an int or a slice of rounds, got %s" % type(val).__name__)
+        rounds = self.num_boosted_rounds()
+        start = 0 if val.start is None else operator.index(val.start)
+        stop = 0 if val.stop is None else operator.index(val.stop)
+        step = 1 if val.step is None else operator.index(val.step)
+        if start < 0 or stop < 0:
+            raise ValueError("Booster slicing takes no negative index, got %r" % (val,))
+        if stop == 0:
+            stop = rounds
+        elif stop < start:
+            raise ValueError("Booster slice %r ends before it starts" % (val,))
+        if step < 1:
+            raise ValueError("Booster slice step must be >= 1, got %d" % step)
+        if start >= rounds or stop > rounds:
+            raise IndexError("Booster slice %r is out of range: the model has %d rounds" % (val, rounds))
+        per = self._trees_per_round
+        keep = [r * per + j for r in range(start, stop, step) for j in range(per)]
+        trees = self.get_trees()
+        out = Booster(self.params)
+        out._trees = [{k: v.copy() if isinstance(v, np.ndarray) else v for k, v in trees[i].items()} for i in keep]
+        out._weights = self.get_tree_weights()[keep] if self.is_dart else None
+        out._attrs = dict(self._attrs)
+        out.n_features = self.n_features
+        out.feature_names = list(self.feature_names) if self.feature_names is not None else None
+        out.feature_types = list(self.feature_types) if self.feature_types is not None else None
+        return out
+
+    def __iter__(self):
+        """One Booster per boosting round, in model order: self[i] for i in range(num_boosted_rounds())."""
+        for i in range(self.num_boosted_rounds()):
+            yield self[i]
 
     def save_config(self):
         gbtree = {"name": "gbtree"}
