@@ -121,6 +121,13 @@ int B2_MatrixQuantizeWithCuts(B2Handle m, B2Handle comm, const int32_t* ptrs /*[
 int B2_MatrixEnsureRaw(B2Handle m, const float* data);
 /* the same for a matrix created with B2_MatrixCreateFromCSR: re-upload (and check) its CSR arrays (xgboost_ray/main.py:437) */
 int B2_MatrixEnsureRawCSR(B2Handle m, int64_t* indptr, const int32_t* indices, const float* values);
+/* xgboost's DMatrix.slice(rindex): a new matrix of rows rows[0..n_rows) of m, in that order (duplicates allowed), built
+ * on m's device from m's device data: raw values (dense, or CSR kept as CSR), the label ([rows][T]), weight, base_margin
+ * ([rows][K]) and label bounds gathered, missing, the feature types and feature_weights copied.  The slice is not quantised
+ * and has no query groups: it is sketched with its own cuts like a matrix built from those rows.  m needs its raw data on
+ * the device (B2_MatrixEnsureRaw / EnsureRawCSR) and is not changed.  n_rows >= 1, every index in [0, m's rows); rows is
+ * only read. */
+int B2_MatrixSlice(B2Handle m, int64_t* rows, int64_t n_rows, B2Handle* out);
 /* device bytes the matrix owns: the capacities of its raw (dense or CSR), bin and info buffers (xgboost_ray/main.py:437) */
 int B2_MatrixDeviceBytes(B2Handle m, int64_t* out);
 int B2_MatrixCutsSize(B2Handle m, int32_t* total_cuts);

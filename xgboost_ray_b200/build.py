@@ -33,6 +33,7 @@ SOURCES = {
     "quantile_kernel.cu": ["--fmad=false"],    # quantile gradients, metric and leaf refresh, bit-exact vs the reference
     "refresh_kernel.cu": ["--fmad=false"],     # refresh updater: leaf sums on raw rows, node statistics bottom-up
     "sparse_kernel.cu": [],                    # CSR raw values: validation, dense row tiles, sketch keys
+    "slice_kernel.cu": [],                     # DMatrix.slice: row gathers of dense / CSR values and side arrays
     # host side (host.h): no device code
     "device.cu": [],
     "matrix.cu": [],

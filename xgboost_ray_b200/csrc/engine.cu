@@ -355,6 +355,11 @@ int B2_MatrixEnsureRawCSR(B2Handle mh, int64_t* indptr, const int32_t* indices, 
   upload_csr(m, indptr, indices, values);
   API_END
 }
+int B2_MatrixSlice(B2Handle mh, int64_t* rows, int64_t n_rows, B2Handle* out) {
+  API_BEGIN
+  *out = slice_matrix(matrix_of(mh), rows, n_rows);
+  API_END
+}
 int B2_MatrixDeviceBytes(B2Handle mh, int64_t* out) {
   API_BEGIN
   *out = (int64_t)matrix_device_bytes(from_handle<Matrix>(mh, kMatrix, "matrix"));

@@ -247,6 +247,9 @@ void for_raw_tiles(Matrix* m, Fn fn, int64_t max_rows = INT64_MAX) {
 void upload_csr(Matrix* m, const int64_t* indptr, const int32_t* indices, const float* values);
 size_t matrix_device_bytes(const Matrix* m);
 
+// B2_MatrixSlice: a new unquantised matrix of parent rows rows[0..n) (host array), gathered on the device
+B2Handle slice_matrix(Matrix* parent, const int64_t* rows, int64_t n);
+
 void setup_groups(Matrix* m);
 // cuts (sketched, or borrowed ones checked against the categorical codes), the bin matrix, raw released unless keep_raw
 void quantize_matrix(Matrix* m, Comm* comm, int max_bin, bool borrowed_cuts, bool keep_raw);

@@ -242,6 +242,19 @@ int b2_launch_csr_densify(const int64_t* indptr, const int32_t* indices, const f
 int b2_launch_csr_extract_keys(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int f0, int nf,
                                float missing, uint32_t* keys, int64_t n_padded, int num_sms, cudaStream_t s);
 
+// slice_kernel.cu (B2_MatrixSlice: rows[0..n) of a parent matrix, in that order, duplicates allowed; every row index is
+// in range, checked by the caller)
+// dst [n][width] = src [rows[i]][width]: dense raw values and the per-row side arrays
+int b2_launch_gather_rows(const float* src, int64_t width, const int64_t* rows, int64_t n, float* dst, int num_sms,
+                          cudaStream_t s);
+size_t b2_csr_slice_temp_bytes(int64_t n);
+// out_indptr [n+1] of the slice (lengths: n scratch int64, temp: b2_csr_slice_temp_bytes(n) bytes of CUB scratch)
+int b2_launch_csr_slice_indptr(const int64_t* indptr, const int64_t* rows, int64_t n, int64_t* lengths, int64_t* out_indptr,
+                               void* temp, size_t temp_bytes, int num_sms, cudaStream_t s);
+int b2_launch_csr_slice_entries(const int64_t* indptr, const int32_t* indices, const float* values, const int64_t* rows,
+                                int64_t n, const int64_t* out_indptr, int32_t* out_indices, float* out_values, int num_sms,
+                                cudaStream_t s);
+
 // refresh_kernel.cu
 int b2_launch_refresh(const float* X, int64_t n, int F, float missing, const B2TreeNodeDev* nodes, int n_nodes,
                       const uint32_t* cat_table, int n_leaves, const float2* gh, const int32_t* qexp, int leaf_bits,

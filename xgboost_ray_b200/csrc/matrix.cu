@@ -232,6 +232,58 @@ void upload_csr(Matrix* m, const int64_t* indptr, const int32_t* indices, const 
   m->has_raw = true;
 }
 
+// The slice holds raw values (dense or CSR, as the parent) and the gathered side arrays, and is quantised with its own
+// cuts when it is first trained or evaluated.  The parent is only read.
+B2Handle slice_matrix(Matrix* p, const int64_t* rows, int64_t n) {
+  if (n < 1) fail("slice: no row index given (a slice needs at least one row)");
+  for (int64_t i = 0; i < n; ++i)
+    if (rows[i] < 0 || rows[i] >= p->n)
+      fail("slice: row index %lld (position %lld) is outside [0, %lld)", (long long)rows[i], (long long)i, (long long)p->n);
+  if (!p->has_raw) fail("slice: the matrix has no raw data on the device (re-upload it with B2_MatrixEnsureRaw / B2_MatrixEnsureRawCSR)");
+  std::unique_ptr<Matrix> m = new_matrix(n, p->F, p->missing);
+  Ctx* ctx = p->ctx; cudaStream_t s = ctx->stream;
+  m->ctx = ctx;
+  DevBuf<int64_t> d_rows;
+  upload(d_rows, rows, (size_t)n, s);
+  if (p->csr) {
+    m->csr = true;
+    m->csr_indptr.ensure((size_t)n + 1);
+    DevBuf<int64_t> lengths; lengths.ensure((size_t)n);
+    DevBuf<uint8_t> temp; const size_t tb = b2_csr_slice_temp_bytes(n); temp.ensure(std::max<size_t>(tb, 1));
+    LAUNCH_CHECK(b2_launch_csr_slice_indptr(p->csr_indptr.p, d_rows.p, n, lengths.p, m->csr_indptr.p, temp.p, tb, ctx->num_sms, s));
+    int64_t nnz = 0;
+    CUDA_CHECK(cudaMemcpyAsync(&nnz, m->csr_indptr.p + n, sizeof(nnz), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    m->nnz = nnz;
+    m->csr_indices.ensure((size_t)nnz); m->csr_values.ensure((size_t)nnz);   // the capacities B2_MatrixCreateFromCSR gives
+    LAUNCH_CHECK(b2_launch_csr_slice_entries(p->csr_indptr.p, p->csr_indices.p, p->csr_values.p, d_rows.p, n, m->csr_indptr.p,
+                                             m->csr_indices.p, m->csr_values.p, ctx->num_sms, s));
+  } else {
+    m->raw.ensure((size_t)n * p->F);
+    LAUNCH_CHECK(b2_launch_gather_rows(p->raw.p, p->F, d_rows.p, n, m->raw.p, ctx->num_sms, s));
+  }
+  m->has_raw = true;
+  // a per-row array of `len` values ([p->n][len / p->n]; len 0 = not set)
+  auto gather = [&](const DevBuf<float>& src, int64_t len, DevBuf<float>& dst, int64_t* dst_len) {
+    if (len == 0) return;
+    const int64_t width = len / p->n;
+    dst.ensure((size_t)n * width);
+    LAUNCH_CHECK(b2_launch_gather_rows(src.p, width, d_rows.p, n, dst.p, ctx->num_sms, s));
+    *dst_len = n * width;
+  };
+  gather(p->label, p->n_label, m->label, &m->n_label);
+  m->n_targets = p->n_targets;
+  gather(p->weight, p->n_weight, m->weight, &m->n_weight);
+  gather(p->base_margin, p->n_base_margin, m->base_margin, &m->n_base_margin);
+  gather(p->lower, p->n_lower, m->lower, &m->n_lower);
+  gather(p->upper, p->n_upper, m->upper, &m->n_upper);
+  m->is_cat = p->is_cat; m->cat_feats = p->cat_feats;
+  m->fwq = p->fwq;
+  if (!m->fwq.empty()) upload(m->d_fwq, m->fwq, s);
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  return register_matrix(std::move(m));
+}
+
 static void release_raw(Matrix* m) {
   m->raw.release();
   m->csr_indptr.release(); m->csr_indices.release(); m->csr_values.release();

@@ -73,6 +73,7 @@ ABI = {
     "B2_MatrixQuantizeWithCuts": (C.c_int, [_H, _H, _IP, _FP, _FP, _BP, C.c_int32, C.c_int32]),
     "B2_MatrixEnsureRaw": (C.c_int, [_H, _FP]),
     "B2_MatrixEnsureRawCSR": (C.c_int, [_H, _LP, _IP, _FP]),
+    "B2_MatrixSlice": (C.c_int, [_H, _LP, C.c_int64, C.POINTER(_H)]),
     "B2_MatrixDeviceBytes": (C.c_int, [_H, C.POINTER(C.c_int64)]),
     "B2_MatrixCutsSize": (C.c_int, [_H, _IP]),
     "B2_MatrixGetCuts": (C.c_int, [_H, _IP, _FP, _FP, _BP]),
@@ -562,6 +563,8 @@ class DMatrix:
 
     def _ensure_raw(self):
         if not self._has_raw:
+            if isinstance(self._host, _SliceRows):   # a slice: its host rows, taken out of the parent's once
+                self._host = self._host.rows()
             if isinstance(self._host, CSRArrays):
                 c = self._host
                 _check(lib().B2_MatrixEnsureRawCSR(self.handle, c.indptr.ctypes.data_as(_LP), _ip(c.indices), _fp(c.values)))
@@ -596,6 +599,53 @@ class DMatrix:
         _check(lib().B2_MatrixGetBins(self.handle, _bp(out)))
         return out
 
+    def slice(self, rindex, allow_groups=False):
+        """xgboost's DMatrix.slice: a new DMatrix of rows `rindex` of this one, in that order (duplicates allowed).
+
+        The rows are gathered on the device from this matrix's device data (B2_MatrixSlice), dense values as dense and
+        CSR as CSR, with the label, weights, base_margin and survival bounds of those rows; missing, the feature names
+        and types and feature_weights are copied.  The slice is unquantised: it is sketched with its own cuts when it is
+        trained or evaluated, as xgboost re-sketches a slice, so it gives the cuts, bins, models and predictions of
+        ``DMatrix(X[rindex], label=y[rindex], ...)``.  This matrix is not changed; when its raw values are no longer on
+        the device (quantised without them) they are uploaded again first, as evaluation does.  The slice's host rows
+        are taken out of this matrix's host data only if a later call needs them.
+
+        A matrix with query groups is sliced only with allow_groups=True; the slice then has no groups until
+        set_group is called.  A QuantileDMatrix is not sliced, as in xgboost."""
+        if isinstance(self, QuantileDMatrix):
+            raise XGBoostError("slice: a QuantileDMatrix / DeviceQuantileDMatrix cannot be sliced (xgboost does not "
+                               "slice them either): slice a DMatrix of the same data")
+        if self._group_sizes is not None and not allow_groups:
+            raise XGBoostError("slice: the matrix has query groups; pass allow_groups=True and give the slice its "
+                               "groups with set_group")
+        n = self.num_row()
+        idx = slice_rows(rindex, n)
+        self._ensure_raw()
+        h = _H(0)
+        _check(lib().B2_MatrixSlice(self.handle, idx.ctypes.data_as(_LP), idx.size, C.byref(h)))
+        out = DMatrix.__new__(DMatrix)
+        out.handle = h.value
+
+        def rows(a):   # a per-row host array ([n] or [n][k], base_margin flattened) at the slice's rows
+            if a is None or a.size == 0:
+                return a
+            b = a.reshape(n, -1)[idx]
+            return b if a.ndim == 2 else b.reshape(-1)
+
+        out.__dict__.update(
+            _host=_SliceRows(self._host, idx), missing=self.missing, device=self.device,
+            feature_names=None if self.feature_names is None else list(self.feature_names),
+            feature_types=None if self.feature_types is None else list(self.feature_types),
+            enable_categorical=self.enable_categorical, max_bin=self.max_bin, ref=None, _quantized=False,
+            _has_raw=True, multi_target=self.multi_target, _label=rows(self._label), _weight=rows(self._weight),
+            _base_margin=rows(self._base_margin), _group_sizes=None, ingest="slice")
+        for field in ("_label_lower_bound", "_label_upper_bound"):
+            if field in self.__dict__:
+                setattr(out, field, rows(getattr(self, field)))
+        if "_feature_weights" in self.__dict__:
+            out._feature_weights = self._feature_weights
+        return out
+
     def __del__(self):
         try:
             if getattr(self, "handle", 0):
@@ -611,6 +661,48 @@ class _BlockList:
     def __init__(self, blocks):
         self.blocks = blocks
         self.shape = (sum(b.shape[0] for b in blocks), blocks[0].shape[1])
+
+
+def slice_rows(rindex, n):
+    """The row indices of DMatrix.slice as int64, checked: at least one, every one an integer in [0, n)."""
+    a = np.asarray(rindex).reshape(-1)
+    if a.size == 0:
+        raise XGBoostError("slice: rindex is empty (a slice needs at least one row)")
+    if a.dtype == bool or not np.issubdtype(a.dtype, np.integer):
+        vals = a.tolist()   # name the first value that is not even integral (else the first: its type is not int)
+        bad = [i for i, v in enumerate(vals) if isinstance(v, bool) or not (
+            isinstance(v, numbers.Integral) or (isinstance(v, float) and v.is_integer()))]
+        i = bad[0] if bad else 0
+        raise XGBoostError("slice: rindex[%d] = %r is not an integer" % (i, vals[i]))
+    a = np.ascontiguousarray(a, np.int64)
+    out = np.flatnonzero((a < 0) | (a >= n))
+    if out.size:
+        i = int(out[0])
+        raise XGBoostError("slice: rindex[%d] = %d is outside [0, %d)" % (i, int(a[i]), n))
+    return a
+
+
+class _SliceRows:
+    """The host rows of a slice: its parent's host data and the row indices, turned into rows only when a call needs
+    them (a slice's values live on the device; the host rows serve a re-upload after they were freed there)."""
+
+    def __init__(self, host, idx):
+        if isinstance(host, _SliceRows):   # a slice of a slice indexes the first parent
+            host, idx = host.host, host.idx[idx]
+        self.host, self.idx = host, idx
+        self.shape = (idx.size, host.shape[1])
+
+    def rows(self):
+        h, idx = self.host, self.idx
+        if isinstance(h, CSRArrays):
+            lens = np.diff(h.indptr)[idx]
+            indptr = np.zeros(idx.size + 1, np.int64)
+            np.cumsum(lens, out=indptr[1:])
+            pos = np.repeat(h.indptr[idx] - indptr[:-1], lens) + np.arange(indptr[-1], dtype=np.int64)
+            return CSRArrays(indptr, h.indices[pos], h.values[pos], self.shape)
+        if isinstance(h, _BlockList):
+            h = np.concatenate(h.blocks, axis=0)
+        return _f32c(np.asarray(h)[idx])
 
 
 def _drain_data_iter(it, label, weight, base_margin):
@@ -704,7 +796,7 @@ class EarlyStopping(TrainingCallback):
     model's best_iteration and best_score are set; best_iteration counts the model's rounds, those of xgb_model
     included.  With save_best=True, after_training returns ``model[: best_iteration + 1]`` carrying both attributes
     again.  These rules are recalled from xgboost 2.x's callback.py, not checked against its source (DESIGN.md 2
-    item 23).
+    item 23).  Under cv() the history holds (mean, std) pairs and the mean is watched.
 
     The history starts again in before_training, so one instance can serve several train() calls.  Actors receive the
     callback pickled; every rank sees the same allreduced metric values and stops at the same round.  An actor restart
@@ -733,7 +825,8 @@ class EarlyStopping(TrainingCallback):
         if metric not in log:
             raise ValueError("EarlyStopping: eval set %r has no metric named %r (metrics: %s)"
                              % (data, metric, ", ".join(log)))
-        score = float(log[metric][-1])
+        score = log[metric][-1]
+        score = float(score[0] if isinstance(score, tuple) else score)   # cv() logs (mean, std): the mean is watched
         mx = self.maximize if self.maximize is not None else _maximized(metric)
         if self.best is None or (score - self.min_delta > self.best if mx else self.best - self.min_delta > score):
             self.best, self.stale = score, 0
@@ -1960,6 +2053,234 @@ def train(params, dtrain, num_boost_round=10, evals=(), obj=None, feval=None, ma
         evals_result.clear()
         evals_result.update(evals_log)
     return bst
+
+
+# ----------------------------------------------------------------------------- cv()
+def cv_folds(n_rows, nfold=3, label=None, group_sizes=None, stratified=False, folds=None, seed=0, shuffle=True):
+    """The folds of cv() as xgboost 2.x's mknfold / mkgroupfold make them, recalled and not checked against its source
+    (DESIGN.md 2 item 24): a list of (train rows, test rows, train group sizes, test group sizes); the group sizes are
+    None unless the rows are split by query groups.  Needs no device.
+
+    - Default: np.random.seed(seed); the rows (with `group_sizes`, the groups) are permuted if `shuffle`, else kept in
+      order, and split by np.array_split into nfold test sets.  Fold k trains on the other folds' rows concatenated in
+      fold order.  Groups are turned back into their rows, in the group order of each side.
+    - stratified=True: scikit-learn's StratifiedKFold(nfold, shuffle=True, random_state=seed) on the label.
+    - folds: a list of (train_idx, test_idx) pairs, or an object with split(X, y) (such as a KFold), called with the
+      label as X and y; nfold is then the number of folds."""
+    np.random.seed(seed)
+    if folds is not None:
+        try:
+            pairs = [(f[0], f[1]) for f in folds]
+        except TypeError:
+            if not hasattr(folds, "split"):
+                raise XGBoostError("cv: folds must be a list of (train_idx, test_idx) pairs or an object with "
+                                   "split(X, y), got %s" % type(folds).__name__) from None
+            pairs = [(f[0], f[1]) for f in folds.split(X=label, y=label)]
+        except (IndexError, KeyError):
+            raise XGBoostError("cv: every entry of folds must be a (train_idx, test_idx) pair") from None
+        if not pairs:
+            raise XGBoostError("cv: folds holds no fold")
+        return [(np.asarray(a), np.asarray(b), None, None) for a, b in pairs]
+    if isinstance(nfold, bool) or not isinstance(nfold, numbers.Integral) or nfold < 2:
+        raise XGBoostError("cv: nfold must be an integer >= 2, got %r" % (nfold,))
+    nfold = int(nfold)
+    if stratified:
+        try:
+            from sklearn.model_selection import StratifiedKFold
+        except ImportError:
+            raise XGBoostError("cv(stratified=True) needs scikit-learn (StratifiedKFold), which is not installed") from None
+        skf = StratifiedKFold(n_splits=nfold, shuffle=True, random_state=seed)
+        return [(a, b, None, None) for a, b in skf.split(X=label, y=label)]
+    if group_sizes is not None:
+        sizes = np.asarray(group_sizes, np.int64)
+        bounds = np.r_[0, np.cumsum(sizes)]
+        idx = np.random.permutation(sizes.size) if shuffle else np.arange(sizes.size)
+        out_g = np.array_split(idx, nfold)
+        in_g = [np.concatenate([out_g[i] for i in range(nfold) if i != k]) for k in range(nfold)]
+
+        def to_rows(groups):
+            return np.concatenate([np.arange(bounds[g], bounds[g + 1]) for g in groups] or [np.zeros(0, np.int64)])
+
+        return [(to_rows(in_g[k]), to_rows(out_g[k]), sizes[in_g[k]], sizes[out_g[k]]) for k in range(nfold)]
+    idx = np.random.permutation(n_rows) if shuffle else np.arange(n_rows)
+    out_idx = np.array_split(idx, nfold)
+    return [(np.concatenate([out_idx[i] for i in range(nfold) if i != k]), out_idx[k], None, None) for k in range(nfold)]
+
+
+def aggcv(rlist):
+    """xgboost's _aggcv: the eval_set strings of the folds of one round -> [(key, mean, std)], one per 'data-metric'
+    entry in the strings' order; mean and std (np.std, population) of the printed %.6f values."""
+    cvmap = {}
+    it = rlist[0].split()[0]
+    for line in rlist:
+        arr = line.split()
+        if arr[0] != it:
+            raise XGBoostError("cv: folds evaluated different rounds (%s, %s)" % (it, arr[0]))
+        for i, tok in enumerate(arr[1:]):
+            k, v = tok.rsplit(":", 1)
+            cvmap.setdefault((i, k), []).append(float(v))
+    return [(k, float(np.mean(v)), float(np.std(v))) for (_, k), v in sorted(cvmap.items(), key=lambda x: x[0][0])]
+
+
+class _PackedBooster:
+    """The fold boosters of cv() as one model for the callbacks (xgboost's _PackedBooster): set_param, attributes and
+    best_iteration / best_score reach every fold; the rest is read from fold 0."""
+
+    def __init__(self, boosters):
+        self.boosters = boosters
+
+    def num_boosted_rounds(self):
+        return self.boosters[0].num_boosted_rounds()
+
+    def set_param(self, params, value=None):
+        for b in self.boosters:
+            b.set_param(params, value)
+
+    def set_attr(self, **kwargs):
+        for b in self.boosters:
+            b.set_attr(**kwargs)
+
+    def attr(self, key):
+        return self.boosters[0].attr(key)
+
+    @property
+    def best_iteration(self):
+        return self.boosters[0].best_iteration
+
+    @best_iteration.setter
+    def best_iteration(self, v):
+        for b in self.boosters:
+            b.best_iteration = v
+
+    @property
+    def best_score(self):
+        return self.boosters[0].best_score
+
+    @best_score.setter
+    def best_score(self, v):
+        for b in self.boosters:
+            b.best_score = v
+
+
+class _CVMonitor(TrainingCallback):
+    """xgboost's EvaluationMonitor under cv(): '[i]\\tdata-metric:mean+std...' (%.5f; without '+std' if not
+    show_stdv) every `period` rounds, and the last round at the end if it was not printed."""
+
+    def __init__(self, period, show_stdv):
+        self.period, self.show_stdv, self.latest = int(period), bool(show_stdv), None
+
+    def after_iteration(self, model, epoch, evals_log):
+        msg = "[%d]" % epoch
+        for data, log in evals_log.items():
+            for metric, vals in log.items():
+                mean, std = vals[-1]
+                msg += ("\t%s-%s:%.5f+%.5f" % (data, metric, mean, std) if self.show_stdv
+                        else "\t%s-%s:%.5f" % (data, metric, mean))
+        if epoch % self.period == 0 or self.period == 1:
+            if _coll.rank == 0:
+                print(msg, flush=True)
+            self.latest = None
+        else:
+            self.latest = msg
+        return False
+
+    def after_training(self, model):
+        if self.latest is not None and _coll.rank == 0:
+            print(self.latest, flush=True)
+        return model
+
+
+def cv(params, dtrain, num_boost_round=10, nfold=3, stratified=False, folds=None, metrics=(), obj=None, feval=None,
+       maximize=None, early_stopping_rounds=None, fpreproc=None, as_pandas=True, verbose_eval=None, show_stdv=True,
+       seed=0, callbacks=None, shuffle=True, custom_metric=None):
+    """xgboost.cv: k-fold cross-validation.  Returns, per round, the mean and std over the folds of every metric on the
+    train and test side of each fold: keys 'train-<m>-mean', 'train-<m>-std', 'test-<m>-mean', 'test-<m>-std'; a pandas
+    DataFrame when as_pandas and pandas is importable, else a dict of lists.
+
+    The folds are cv_folds(...); each side is dtrain.slice(rows) (gathered on the device), with set_group for a matrix
+    split by query groups.  fpreproc(dtrain_k, dtest_k, params.copy()) may replace both and the params.  A non-empty
+    `metrics` replaces eval_metric.  Each fold trains one Booster on [(train, 'train'), (test, 'test')]; in every round
+    all folds' rounds are enqueued before any metric is read back, and each fold computes what train() computes on its
+    slices.  obj and custom_metric / feval take the paths of train().
+
+    The callbacks see one model for all folds and a history of (mean, std) pairs.  early_stopping_rounds (with
+    maximize) adds EarlyStopping on the last metric of 'test'; verbose_eval (True or a period) with show_stdv prints
+    the rounds.  When a callback stops training, every list is cut to best_iteration + 1 rounds.  LearningRateScheduler
+    sets the rate of every fold.  EarlyStopping(save_best=True) is refused: there is no single model to cut.  These
+    rules are recalled from xgboost 2.x, not checked against its source (DESIGN.md 2 item 24)."""
+    callbacks = list(callbacks or [])
+    for cb in callbacks:
+        if isinstance(cb, EarlyStopping) and cb.save_best:
+            raise XGBoostError("cv: EarlyStopping(save_best=True) is not supported: cv returns the evaluation history "
+                               "of several fold models, not one model to keep the best rounds of")
+    feval = custom_metric if custom_metric is not None else feval
+    if isinstance(params, (list, tuple)):
+        listed = [v for k, v in params if k == "eval_metric"]
+        params = dict(params)
+        if listed:
+            params["eval_metric"] = listed
+    else:
+        params = _params_dict(params)
+    metrics = [metrics] if isinstance(metrics, str) else list(metrics)
+    if not metrics and "eval_metric" in params:
+        m = params["eval_metric"]
+        metrics = list(m) if isinstance(m, (list, tuple)) else [m]
+    params.pop("eval_metric", None)
+
+    spec = cv_folds(dtrain.num_row(), nfold, label=dtrain.get_label(), group_sizes=dtrain._group_sizes,
+                    stratified=stratified, folds=folds, seed=seed, shuffle=shuffle)
+    packs = []
+    for in_idx, out_idx, in_groups, out_groups in spec:
+        grouped = in_groups is not None
+        d_in, d_out = dtrain.slice(in_idx, allow_groups=grouped), dtrain.slice(out_idx, allow_groups=grouped)
+        if grouped:
+            d_in.set_group(in_groups)
+            d_out.set_group(out_groups)
+        tparams = dict(params)
+        if fpreproc is not None:
+            d_in, d_out, tparams = fpreproc(d_in, d_out, dict(params))
+        if metrics:
+            tparams = dict(tparams, eval_metric=list(metrics))
+        bst = Booster(tparams)
+        bst._attach(d_in)
+        packs.append((bst, d_in, d_out))
+    model = _PackedBooster([p[0] for p in packs])
+    if verbose_eval:
+        callbacks.append(_CVMonitor(1 if verbose_eval is True else verbose_eval, show_stdv))
+    if early_stopping_rounds:
+        callbacks.append(EarlyStopping(early_stopping_rounds, maximize=maximize))
+    for cb in callbacks:
+        cb.before_training(model)
+    results, history = {}, {}
+    for epoch in range(num_boost_round):
+        if any(cb.before_iteration(model, epoch, history) for cb in callbacks):
+            break
+        for bst, d_in, _ in packs:   # every fold's round is enqueued before any metric is read back
+            bst.update(d_in, epoch, fobj=obj)
+        msgs = [bst.eval_set([(d_in, "train"), (d_out, "test")], epoch, feval, output_margin=obj is not None)
+                for bst, d_in, d_out in packs]
+        for key, mean, std in aggcv(msgs):
+            data, metric = key.split("-", 1)
+            history.setdefault(data, {}).setdefault(metric, []).append((mean, std))
+            results.setdefault(key + "-mean", []).append(mean)
+            results.setdefault(key + "-std", []).append(std)
+        stop = False
+        for cb in callbacks:
+            if cb.after_iteration(model, epoch, history):
+                stop = True
+        if stop:
+            if model.best_iteration is not None:
+                results = {k: v[: model.best_iteration + 1] for k, v in results.items()}
+            break
+    for cb in callbacks:
+        cb.after_training(model)
+    if as_pandas:
+        try:
+            import pandas as pd
+        except ImportError:
+            return results
+        return pd.DataFrame.from_dict(results)
+    return results
 
 
 def hist_build_raw(bins, qg, qh, ridx=None, window_rows=8192, chunk_rows=2048, device=None):
