@@ -10,6 +10,7 @@ There is NO CPU fallback: if the CUDA extension is not built or no H100 is visib
 compute call raises ``XGBoostError``.
 """
 import ast
+import base64
 import ctypes as C
 import json
 import numbers
@@ -1044,6 +1045,41 @@ def _params_dict(params):
     return {} if params is None else dict(params)
 
 
+def _model_document(raw):
+    """The document of a model file: JSON when, after optional whitespace, `{` is followed by `"`, `}` or whitespace;
+    UBJSON when `{` is followed by a key length, `$`, `#` or no-op marker."""
+    i = len(raw) - len(raw.lstrip(b" \t\r\n"))
+    if raw[i:i + 1] == b"{":
+        nxt = raw[i + 1:i + 2]
+        if nxt in (b'"', b"}", b" ", b"\t", b"\r", b"\n"):
+            return json.loads(raw.decode())
+        if nxt and nxt in b"iUIlL$#N":
+            from xgboost_ray_b200 import ubjson
+            return ubjson.loads(raw, i)
+    raise XGBoostError("not a JSON or UBJSON model; the deprecated binary format is not supported")
+
+
+def _exact_covers(text):
+    """The "b2.sum_hessian" attribute of a UBJSON model: tree -> its float64 covers."""
+    out = {}
+    try:
+        for ti, b in json.loads(text or "[]"):
+            out[int(ti)] = np.frombuffer(base64.b64decode(b, validate=True), "<f8").astype(np.float64)
+    except (ValueError, TypeError) as e:
+        raise XGBoostError("model attribute b2.sum_hessian is malformed: %s" % e)
+    return out
+
+
+def _covers(sum_hessian, exact):
+    """A tree's covers: the file's sum_hessian, or the exact float64 covers of b2.sum_hessian where those round to the
+    file's values node for node (a tool that rewrote the trees without the attribute leaves its covers in charge)."""
+    h = np.asarray(sum_hessian, np.float64)
+    if exact is not None and exact.shape == h.shape and \
+            np.array_equal(exact.astype(np.float32), h.astype(np.float32)):
+        return exact
+    return h
+
+
 class Booster:
     def __init__(self, params=None, cache=(), model_file=None):
         self.params = _params_dict(params)
@@ -1548,19 +1584,54 @@ class Booster:
         }
 
     def save_raw(self, raw_format="json"):
-        return bytearray(json.dumps(self._model_dict(), allow_nan=False).encode())
+        """The model file as bytes: raw_format "json" (the default) or "ubj", xgboost's UBJSON encoding of the same
+        document (DESIGN.md 2 item 25)."""
+        if raw_format == "json":
+            return bytearray(json.dumps(self._model_dict(), allow_nan=False).encode())
+        if raw_format == "ubj":
+            from xgboost_ray_b200 import ubjson
+            return bytearray(ubjson.dumps(self._ubj_dict()))
+        if raw_format == "deprecated":
+            raise XGBoostError("raw_format='deprecated', xgboost's old binary model format, is not supported "
+                               "(supported: json, ubj)")
+        raise XGBoostError("raw_format=%r is not supported (supported: json, ubj)" % (raw_format,))
+
+    def _ubj_dict(self):
+        """_model_dict() as UBJSON carries it: `sum_hessian` is a float32 array in xgboost's dialect, while this engine
+        keeps each node's hessian sum (the cover TreeSHAP weights paths by) in float64.  A tree whose covers float32
+        cannot hold exactly gets its float32 covers in `sum_hessian` and the exact ones, little-endian float64 in
+        base64, in the "b2.sum_hessian" attribute as [tree, "..."] (DESIGN.md 2 item 25)."""
+        d = self._model_dict()
+        gb = d["learner"]["gradient_booster"]
+        trees = (gb["gbtree"] if gb["name"] == "dart" else gb)["model"]["trees"]   # a new list; its trees are cached
+        exact = []
+        for ti, t in enumerate(trees):
+            h = np.asarray(t["sum_hessian"], np.float64)
+            h32 = h.astype(np.float32)
+            if not np.array_equal(h32.astype(np.float64), h):
+                exact.append([ti, base64.b64encode(h.astype("<f8").tobytes()).decode()])
+                trees[ti] = dict(t, sum_hessian=h32)
+        if exact:
+            d["learner"]["attributes"]["b2.sum_hessian"] = json.dumps(exact, separators=(",", ":"))
+        return d
 
     def save_model(self, fname):
+        """Write the model file: UBJSON when the path ends in .ubj (in any case, as xgboost compares the lowercased
+        extension), JSON otherwise."""
         with open(fname, "wb") as f:
-            f.write(bytes(self.save_raw()))
+            f.write(bytes(self.save_raw("ubj" if os.fsdecode(fname).lower().endswith(".ubj") else "json")))
 
     def load_model(self, fname):
+        """Load a model file (a path, bytes or bytearray) in JSON or UBJSON, told apart by its content."""
         if isinstance(fname, (bytes, bytearray)):
             raw = bytes(fname)
         else:
             with open(fname, "rb") as f:
                 raw = f.read()
-        d = json.loads(raw.decode())
+        self._load_document(_model_document(raw))
+
+    def _load_document(self, d):
+        """Fill the booster from a decoded model document, whose arrays are lists (JSON) or NumPy arrays (UBJSON)."""
         L = d["learner"]
         self._free()
         self.__dict__.pop("_tree_json_cache", None)
@@ -1570,6 +1641,7 @@ class Booster:
         exact_conds = {}    # tree -> [(node, condition)]
         for ti, nid, v in json.loads(attrs.pop("b2.split_conds", "[]")):
             exact_conds.setdefault(int(ti), []).append((int(nid), np.float32(float(v))))
+        exact_hess = _exact_covers(attrs.pop("b2.sum_hessian", None))
         params["objective"] = L["objective"]["name"]
         nc = int(L["learner_model_param"].get("num_class", "0"))
         nc = max(nc, int(L["objective"].get("softmax_multiclass_param", {}).get("num_class", "0")))
@@ -1627,7 +1699,8 @@ class Booster:
             left = np.asarray(t["left_children"], np.int32)
             leaf = left < 0
             sc = np.asarray(t["split_conditions"], np.float32)
-            parent = np.asarray([p if p != 2147483647 else -1 for p in t["parents"]], np.int32)
+            parent = np.asarray(t["parents"], np.int64)
+            parent = np.where(parent == 2147483647, -1, parent).astype(np.int32)
             st = np.asarray(t.get("split_type", [0] * len(left)), np.uint8)
             bits = np.zeros((len(left), 8), np.uint32)
             for nid, seg, size in zip(t.get("categories_nodes", []), t.get("categories_segments", []),
@@ -1663,7 +1736,7 @@ class Booster:
                 value=np.where(leaf, sc, bw).astype(np.float32),
                 base_weight=bw,
                 loss_chg=np.asarray(t["loss_changes"], np.float32),
-                sum_hess=np.asarray(t["sum_hessian"], np.float64)))
+                sum_hess=_covers(t["sum_hessian"], exact_hess.get(ti))))
 
     def __getstate__(self):
         return {"raw": bytes(self.save_raw()), "best_iteration": self.best_iteration, "best_score": self.best_score,
