@@ -133,7 +133,15 @@ int B2_MatrixDeviceBytes(B2Handle m, int64_t* out);
 int B2_MatrixCutsSize(B2Handle m, int32_t* total_cuts);
 int B2_MatrixGetCuts(B2Handle m, int32_t* ptrs /*[F+1]*/, float* vals /*[total]*/, float* mins /*[F]*/,
                      uint8_t* has_missing /*[F]*/);
+/* dense (n_rows, n_cols) bins; a matrix with the CSR bin layout is densified on the device (absent entries: 255) */
 int B2_MatrixGetBins(B2Handle m, uint8_t* out /*[n_rows*n_cols] dense row-major*/);
+/* bin layout, set before B2_MatrixQuantize.  DENSE: two n_rows x n_cols byte copies of the bins (row- and
+ * feature-major).  CSR (a matrix created with B2_MatrixCreateFromCSR only): one bin per stored entry, aligned with the
+ * CSR's indices, which stay on the device with indptr; training reads them instead (DESIGN.md 2 item 26), and the
+ * model is byte-identical to the dense layout's.  AUTO (the default): CSR for a CSR matrix whose two dense copies would
+ * take more than half of the device's memory, otherwise DENSE.  A slice takes the layout of its parent. */
+enum { B2_BIN_LAYOUT_AUTO = 0, B2_BIN_LAYOUT_DENSE = 1, B2_BIN_LAYOUT_CSR = 2 };
+int B2_MatrixSetBinLayout(B2Handle m, int32_t layout);
 int B2_MatrixFree(B2Handle m);
 
 /* ---- booster: replaces xgb.train(...) at xgboost_ray/main.py:745-752 (one UpdateOneIter per
@@ -236,6 +244,11 @@ int B2_BoosterFree(B2Handle b);
 int B2_HistBuildRaw(const uint8_t* bins, int64_t n_rows, int32_t n_cols, const int32_t* qg, const int32_t* qh,
                     const int32_t* ridx, int64_t n_sel, int32_t window_rows, int32_t chunk_rows, int device,
                     int64_t* out, float* kernel_ms /* may be NULL */);
+/* the same histogram from the CSR bin layout: row i stores bins[indptr[i] .. indptr[i+1]) of the columns in indices
+ * (increasing within a row); an absent entry has bin 255.  Rows as for B2_HistBuildRaw; chunk_rows <= 0: 2048. */
+int B2_HistBuildRawCSR(int64_t* indptr, const int32_t* indices, const uint8_t* bins, int64_t n_rows, int32_t n_cols,
+                       const int32_t* qg, const int32_t* qh, const int32_t* ridx, int64_t n_sel, int32_t chunk_rows,
+                       int device, int64_t* out, float* kernel_ms /* may be NULL */);
 
 /* ---- kernel-level entry used by the parity tests: the training path's fixed-point quantisation of n gradient pairs
  * (max |g|, |h| -> frexp exponents -> q = rint(v * 2^(qbits - e))).  out_q [n][2] int32 (qg, qh), out_exp [2]. */

@@ -20,6 +20,7 @@ COMMON = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=
           "-Xcompiler", "-fPIC,-ffp-contract=off", "-ccbin", "/usr/bin/g++"]
 SOURCES = {
     "hist_kernel.cu": [],
+    "hist_csr_kernel.cu": [],                  # level histograms from the CSR bin layout
     "split_kernel.cu": ["--fmad=false"],
     "partition_kernel.cu": ["--fmad=false"],
     "control_kernel.cu": ["--fmad=false"],

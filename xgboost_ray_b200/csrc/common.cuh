@@ -6,6 +6,8 @@
 //                                            bin 255 is the missing sentinel
 //   bins_col  uint8 [n_features][col_stride] feature-major copy, read by the row partition (1 byte/row
 //                                            from a 128-byte row would cost a whole DRAM burst per row)
+//   ebins     uint8 [nnz]                    CSR bin layout instead of both: one bin per stored entry
+//                                            (b2_csr_bin), read with the CSR's indptr / indices
 //   gpair     int2  [n_rows]                 (qg, qh) fixed-point gradient / hessian
 //   hist      int64 [node][group][2][256][32] plane 0 = sum qg, plane 1 = sum qh, slot = feature
 //                                            within group; 128 KiB per (node, group)
@@ -180,6 +182,21 @@ __device__ __forceinline__ int b2_tree_leaf(const B2TreeNodeDev* __restrict__ tn
   }
   *leaf_value = nd.value;
   return nid;
+}
+
+// ---- CSR bin layout (DESIGN.md 2 item 26): one bin per stored entry, aligned with the CSR's indices.  The bin of
+// feature f in row `row`: the stored entry's, found by binary search in the row's increasing columns, or the missing
+// sentinel when the row does not store f -- the bin the dense twin holds for that absent cell.
+__device__ __forceinline__ int b2_csr_bin(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
+                                          const uint8_t* __restrict__ ebins, int64_t row, int f) {
+  int64_t lo = __ldg(indptr + row);
+  const int64_t end = __ldg(indptr + row + 1);
+  int64_t hi = end;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (__ldg(indices + mid) < f) lo = mid + 1; else hi = mid;
+  }
+  return (lo < end && __ldg(indices + lo) == f) ? (int)__ldg(ebins + lo) : B2_MISSING_BIN;
 }
 
 // ---- device-resident control tables of the sync-free level loop (control_kernel.cu)

@@ -24,6 +24,22 @@ namespace b2 {
 constexpr int kDartRows = 128;                       // rows (threads) per CTA
 constexpr size_t kDartMaxSmem = (size_t)200 * 1024;  // staged tile limit (227 KB per CTA on sm_90)
 
+// one step of the bin-space walk from node nd, where b is the row's bin of nd.feature
+__device__ __forceinline__ int dart_step(const B2TreeNodeDev& nd, int b, const uint8_t* __restrict__ has_missing,
+                                         const uint32_t* __restrict__ cat_table) {
+  if (b == B2_MISSING_BIN && __ldg(has_missing + nd.feature)) return nd.default_left ? nd.left : nd.right;
+  if (nd.cat_slot >= 0) return ((__ldg(cat_table + (size_t)nd.cat_slot * 8 + (b >> 5)) >> (b & 31)) & 1u) ? nd.right : nd.left;
+  return b <= nd.pad ? nd.left : nd.right;
+}
+
+// tree t's leaf value v added to the margins of row i: drop when the tree is kept, full always
+__device__ __forceinline__ void dart_add(int64_t i, int t, float v, bool keep, int K, int npt, const float* __restrict__ w_drop,
+                                         const float* __restrict__ w_full, float* __restrict__ drop, float* __restrict__ full) {
+  const int64_t o = i * K + (t / npt) % K;
+  if (keep) drop[o] = __fadd_rn(drop[o], __fmul_rn(__ldg(w_drop + t), v));
+  full[o] = __fadd_rn(full[o], __fmul_rn(__ldg(w_full + t), v));
+}
+
 template <bool kSmem, bool kSingle>
 __global__ void __launch_bounds__(kDartRows)
 dart_margins_kernel(const uint8_t* __restrict__ bins, int64_t n, int row_stride, const int32_t* __restrict__ feat_byte,
@@ -53,11 +69,7 @@ dart_margins_kernel(const uint8_t* __restrict__ bins, int64_t n, int row_stride,
       B2TreeNodeDev nd = tn[0];
       while (nd.feature >= 0) {
         const int b = kSmem ? row[__ldg(feat_byte + nd.feature)] : __ldg(row + __ldg(feat_byte + nd.feature));
-        int next;
-        if (b == B2_MISSING_BIN && __ldg(has_missing + nd.feature)) next = nd.default_left ? nd.left : nd.right;
-        else if (nd.cat_slot >= 0) next = ((__ldg(cat_table + (size_t)nd.cat_slot * 8 + (b >> 5)) >> (b & 31)) & 1u) ? nd.right : nd.left;
-        else next = b <= nd.pad ? nd.left : nd.right;
-        nd = tn[next];
+        nd = tn[dart_step(nd, b, has_missing, cat_table)];
       }
       const float v = nd.value;
       const bool keep = drop && !__ldg(dropped + t);
@@ -65,14 +77,29 @@ dart_margins_kernel(const uint8_t* __restrict__ bins, int64_t n, int row_stride,
         if (keep) d1 = __fadd_rn(d1, __fmul_rn(__ldg(w_drop + t), v));
         f1 = __fadd_rn(f1, __fmul_rn(__ldg(w_full + t), v));
       } else {
-        const int64_t o = i * K + (t / npt) % K;
-        if (keep) drop[o] = __fadd_rn(drop[o], __fmul_rn(__ldg(w_drop + t), v));
-        full[o] = __fadd_rn(full[o], __fmul_rn(__ldg(w_full + t), v));
+        dart_add(i, t, v, keep, K, npt, w_drop, w_full, drop, full);
       }
     }
     if (kSingle) {
       if (drop) drop[i] = d1;
       full[i] = f1;
+    }
+  }
+}
+
+// CSR bin layout: one thread per row, the bin of a node's feature found in the row's stored entries (b2_csr_bin)
+__global__ void __launch_bounds__(kDartRows)
+dart_margins_csr_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, const uint8_t* __restrict__ ebins,
+                        int64_t n, const uint8_t* __restrict__ has_missing, const B2TreeNodeDev* __restrict__ nodes,
+                        const int32_t* __restrict__ tree_offset, const uint32_t* __restrict__ cat_table, int T, int K, int npt,
+                        const float* __restrict__ w_drop, const uint8_t* __restrict__ dropped, const float* __restrict__ w_full,
+                        float* __restrict__ drop, float* __restrict__ full) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    for (int t = 0; t < T; ++t) {
+      const B2TreeNodeDev* tn = nodes + __ldg(tree_offset + t);
+      B2TreeNodeDev nd = tn[0];
+      while (nd.feature >= 0) nd = tn[dart_step(nd, b2_csr_bin(indptr, indices, ebins, i, nd.feature), has_missing, cat_table)];
+      dart_add(i, t, nd.value, drop && !__ldg(dropped + t), K, npt, w_drop, w_full, drop, full);
     }
   }
 }
@@ -109,6 +136,17 @@ int b2_launch_dart_margins(const uint8_t* bins, int64_t n, int row_stride, const
     else B2_DART_LAUNCH(false, false, 0);
   }
 #undef B2_DART_LAUNCH
+  return (int)cudaGetLastError();
+}
+int b2_launch_dart_margins_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, int64_t n,
+                               const uint8_t* has_missing, const B2TreeNodeDev* nodes, const int32_t* tree_offset,
+                               const uint32_t* cat_table, int T, int K, int npt, const float* w_drop, const uint8_t* dropped,
+                               const float* w_full, float* drop, float* full, int num_sms, cudaStream_t s) {
+  if (n <= 0 || T <= 0) return 0;
+  if (npt < 1) npt = 1;
+  const int64_t tiles = (n + b2::kDartRows - 1) / b2::kDartRows, cap = (int64_t)num_sms * 16;
+  b2::dart_margins_csr_kernel<<<(int)(tiles < cap ? tiles : cap), b2::kDartRows, 0, s>>>(
+      indptr, indices, ebins, n, has_missing, nodes, tree_offset, cat_table, T, K, npt, w_drop, dropped, w_full, drop, full);
   return (int)cudaGetLastError();
 }
 }

@@ -175,6 +175,12 @@ struct Matrix : HandleBase {
   DevBuf<uint8_t> bins;  // [n][row_stride]
   DevBuf<uint8_t> bins_col;  // [F][col_stride] feature-major copy for the row partition
   int64_t col_stride = 0;
+  // bin layout (B2_MatrixSetBinLayout): the requested B2_BIN_LAYOUT_*, and after quantisation whether the matrix holds the
+  // CSR layout -- ebins [nnz], one bin per stored entry, instead of bins and bins_col; csr_indptr / csr_indices then
+  // stay on the device after the raw values are released (DESIGN.md 2 item 26)
+  int bin_layout = B2_BIN_LAYOUT_AUTO;
+  bool csr_bins = false;
+  DevBuf<uint8_t> ebins;
   bool quantized = false;
   int n_groups = 0, row_stride = 0, max_bin = 0;
   std::vector<int32_t> group_first, group_size, feat_byte;
@@ -251,6 +257,8 @@ size_t matrix_device_bytes(const Matrix* m);
 B2Handle slice_matrix(Matrix* parent, const int64_t* rows, int64_t n);
 
 void setup_groups(Matrix* m);
+// bytes of the two dense bin copies (bins and bins_col) of an n x F matrix, as bin_matrix allocates them
+size_t dense_bin_bytes(int64_t n, int F);
 // cuts (sketched, or borrowed ones checked against the categorical codes), the bin matrix, raw released unless keep_raw
 void quantize_matrix(Matrix* m, Comm* comm, int max_bin, bool borrowed_cuts, bool keep_raw);
 
@@ -415,6 +423,7 @@ struct Booster : HandleBase {
   DevBuf<int2> q;                // [n]
   DevBuf<int32_t> ridx[2];
   DevBuf<long long> hist[2];
+  DevBuf<long long> csr_hist_tot;  // CSR bin layout: [nodes of a level][2] row totals of a histogram build (launch_hist)
   // Everything a peer maps lives in ONE allocation (one cudaIpc handle per peer instead of four): the build buffer, the
   // candidate table, the misc table and the flag words are views into it
   template <typename T> struct View { T* p = nullptr; };

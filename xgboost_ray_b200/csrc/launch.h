@@ -38,6 +38,12 @@ extern "C" {
 int b2_launch_hist(const uint8_t* bins, int row_stride, const int2* gpair, const int32_t* ridx, const B2HistWork* work,
                    int n_work, int total_chunks, int chunk_rows, int window_rows, int n_groups, long long* hist,
                    const B2LevelCtl* ctl, int log2_shards, int node_cap, int num_sms, cudaStream_t stream);
+// hist_csr_kernel.cu: the same histograms from the CSR bin layout (ebins [nnz]).  totals [node_cap][2] must be zero;
+// n_work / total_chunks / chunk_rows as for b2_launch_hist (from ctl when it is given)
+int b2_launch_hist_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, const int32_t* feat_byte,
+                       const int32_t* group_size, const int2* gpair, const int32_t* ridx, const B2HistWork* work, int n_work,
+                       int total_chunks, int chunk_rows, int n_groups, long long* hist, long long* totals,
+                       const B2LevelCtl* ctl, int log2_shards, int node_cap, int num_sms, cudaStream_t stream);
 int b2_launch_hist_subtract(const long long* parent_level, long long* level, const int32_t* triples, int n_pairs,
                             int64_t node_elems, const B2LevelCtl* ctl, cudaStream_t stream);
 
@@ -90,6 +96,14 @@ int b2_split_chunk_rows();
 int b2_launch_partition(const uint8_t* bins_col, int64_t col_stride, const int32_t* ridx_in, int32_t* ridx_out,
                         const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, int32_t* counters, int any_categorical,
                         B2FinalizeArgs fin, int num_sms, cudaStream_t stream);
+// the same two passes on the CSR bin layout: a row's bin of the split feature is found in its stored entries (b2_csr_bin)
+int b2_launch_partition_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, const int32_t* ridx_in,
+                            int32_t* ridx_out, const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, int32_t* counters,
+                            int any_categorical, B2FinalizeArgs fin, int num_sms, cudaStream_t stream);
+int b2_launch_final_assign_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, const int32_t* ridx_in,
+                               const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, const float2* gh,
+                               const int32_t* qexp, int leaf_bits, long long* sums, uint16_t* pos, int any_categorical,
+                               int num_sms, cudaStream_t stream);
 int b2_launch_leaf_sums(const float2* gh, const int32_t* ridx0, const int32_t* ridx1, const B2SegWork* work,
                         const B2LevelCtl* ctl, int max_chunks, const int32_t* qexp, int leaf_bits, long long* sums,
                         uint16_t* pos, int num_sms, cudaStream_t stream);
@@ -176,6 +190,10 @@ int b2_launch_dart_margins(const uint8_t* bins, int64_t n, int row_stride, const
                            const B2TreeNodeDev* nodes, const int32_t* tree_offset, const uint32_t* cat_table, int T, int K,
                            int npt, const float* w_drop, const uint8_t* dropped, const float* w_full, float* drop, float* full,
                            int num_sms, cudaStream_t s);
+int b2_launch_dart_margins_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, int64_t n,
+                               const uint8_t* has_missing, const B2TreeNodeDev* nodes, const int32_t* tree_offset,
+                               const uint32_t* cat_table, int T, int K, int npt, const float* w_drop, const uint8_t* dropped,
+                               const float* w_full, float* drop, float* full, int num_sms, cudaStream_t s);
 
 // shap_kernel.cu
 size_t b2_shap_contribs_smem(int K, int F, int warps);
@@ -231,6 +249,9 @@ int b2_sketch_column(const uint32_t* keys_in, const int32_t* wq_in, uint32_t* ke
 int b2_launch_bin(const float* X, int64_t n, int F, float missing, const int32_t* cut_ptrs, const float* cut_vals,
                   const int32_t* feat_byte, const uint8_t* is_cat, int row_stride, uint8_t* bins, uint8_t* bins_col,
                   int64_t col_stride, int num_sms, cudaStream_t s);
+// ebins [nnz] = the bin of every stored entry of a CSR matrix, by the rule of b2_launch_bin
+int b2_launch_bin_csr(const int32_t* indices, const float* values, int64_t nnz, float missing, const int32_t* cut_ptrs,
+                      const float* cut_vals, const uint8_t* is_cat, uint8_t* ebins, int num_sms, cudaStream_t s);
 int b2_launch_cat_stats(const float* X, int64_t n, int F, float missing, const int32_t* cat_feats, int n_cat, int32_t* stats,
                         int num_sms, cudaStream_t s);
 
@@ -239,6 +260,9 @@ int b2_launch_csr_validate(const int64_t* indptr, const int32_t* indices, int64_
                            int num_sms, cudaStream_t s);
 int b2_launch_csr_densify(const int64_t* indptr, const int32_t* indices, const float* values, int64_t r0, int64_t rows, int F,
                           float* out, int num_sms, cudaStream_t s);
+// out [n][F] = the dense bins of a CSR-layout matrix (absent entries: the missing sentinel)
+int b2_launch_csr_bins_densify(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, int64_t n, int F,
+                               uint8_t* out, int num_sms, cudaStream_t s);
 int b2_launch_csr_extract_keys(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int f0, int nf,
                                float missing, uint32_t* keys, int64_t n_padded, int num_sms, cudaStream_t s);
 

@@ -247,6 +247,7 @@ B2Handle slice_matrix(Matrix* p, const int64_t* rows, int64_t n) {
   upload(d_rows, rows, (size_t)n, s);
   if (p->csr) {
     m->csr = true;
+    m->bin_layout = p->csr_bins ? B2_BIN_LAYOUT_CSR : p->bin_layout;
     m->csr_indptr.ensure((size_t)n + 1);
     DevBuf<int64_t> lengths; lengths.ensure((size_t)n);
     DevBuf<uint8_t> temp; const size_t tb = b2_csr_slice_temp_bytes(n); temp.ensure(std::max<size_t>(tb, 1));
@@ -284,9 +285,11 @@ B2Handle slice_matrix(Matrix* p, const int64_t* rows, int64_t n) {
   return register_matrix(std::move(m));
 }
 
+// the CSR bin layout keeps indptr and indices: they locate its bins
 static void release_raw(Matrix* m) {
   m->raw.release();
-  m->csr_indptr.release(); m->csr_indices.release(); m->csr_values.release();
+  if (!m->csr_bins) { m->csr_indptr.release(); m->csr_indices.release(); }
+  m->csr_values.release();
   m->has_raw = false;
 }
 
@@ -294,7 +297,7 @@ template <typename T>
 static size_t buf_bytes(const DevBuf<T>& d) { return d.cap * sizeof(T); }
 size_t matrix_device_bytes(const Matrix* m) {
   return buf_bytes(m->raw) + buf_bytes(m->csr_indptr) + buf_bytes(m->csr_indices) + buf_bytes(m->csr_values) +
-         buf_bytes(m->bins) + buf_bytes(m->bins_col) + buf_bytes(m->d_group_first) + buf_bytes(m->d_group_size) +
+         buf_bytes(m->bins) + buf_bytes(m->bins_col) + buf_bytes(m->ebins) + buf_bytes(m->d_group_first) + buf_bytes(m->d_group_size) +
          buf_bytes(m->d_feat_byte) + buf_bytes(m->d_cut_ptrs) + buf_bytes(m->d_nbins) + buf_bytes(m->d_cat_feats) +
          buf_bytes(m->d_cut_vals) + buf_bytes(m->d_has_missing) + buf_bytes(m->d_is_cat) + buf_bytes(m->label) +
          buf_bytes(m->weight) + buf_bytes(m->base_margin) + buf_bytes(m->lower) + buf_bytes(m->upper) +
@@ -500,10 +503,35 @@ static void make_cuts(Matrix* m, Comm* comm, int max_bin) {
   m->max_bin = max_bin;
 }
 
+size_t dense_bin_bytes(int64_t n, int F) {
+  Matrix t; t.F = F;
+  setup_groups(&t);
+  const int64_t rows = std::max<int64_t>(n, 1), col_stride = (rows + 127) & ~(int64_t)127;
+  return (size_t)rows * t.row_stride + (size_t)col_stride * F;
+}
+
+// "auto" takes the CSR layout only where the two dense copies would not fit: above half of the device's memory
+static bool use_csr_bins(const Matrix* m) {
+  if (!m->csr || m->bin_layout == B2_BIN_LAYOUT_DENSE) return false;
+  if (m->bin_layout == B2_BIN_LAYOUT_CSR) return true;
+  cudaDeviceProp prop;
+  CUDA_CHECK(cudaGetDeviceProperties(&prop, m->ctx->device));
+  return dense_bin_bytes(m->n, m->F) > prop.totalGlobalMem / 2;
+}
+
 static void bin_matrix(Matrix* m) {
   Ctx* ctx = m->ctx; cudaStream_t s = ctx->stream;
   setup_groups(m);
   upload_cuts(m);
+  if (use_csr_bins(m)) {
+    m->csr_bins = true;
+    m->ebins.ensure((size_t)std::max<int64_t>(m->nnz, 1));
+    LAUNCH_CHECK(b2_launch_bin_csr(m->csr_indices.p, m->csr_values.p, m->nnz, m->missing, m->d_cut_ptrs.p, m->d_cut_vals.p,
+                                   m->any_cat() ? m->d_is_cat.p : nullptr, m->ebins.p, ctx->num_sms, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    m->quantized = true;
+    return;
+  }
   m->bins.ensure((size_t)std::max<int64_t>(m->n, 1) * m->row_stride);
   CUDA_CHECK(cudaMemsetAsync(m->bins.p, 0, (size_t)std::max<int64_t>(m->n, 1) * m->row_stride, s));
   m->col_stride = (std::max<int64_t>(m->n, 1) + 127) & ~(int64_t)127;

@@ -18,6 +18,28 @@ constexpr int kPartChunk = 2048;  // rows per CTA work item
 
 typedef B2SegWork SegWork;
 
+// Where the split kernels read a row's bin of the split feature: the feature-major copy bins_col of the dense layout, or
+// the stored entries of the CSR layout (b2_csr_bin).  Column(f).ld(row) is the bin; ldcs streams it past L2 where the
+// layout allows.
+struct ColBins {
+  const uint8_t* bins_col; int64_t col_stride;
+  struct Column {
+    const uint8_t* col;
+    __device__ __forceinline__ int ld(int rid) const { return (int)__ldg(col + rid); }
+    __device__ __forceinline__ int ldcs(int rid) const { return (int)__ldcs(col + rid); }
+  };
+  __device__ __forceinline__ Column column(int f) const { return Column{bins_col + (int64_t)f * col_stride}; }
+};
+struct CsrBins {
+  const int64_t* indptr; const int32_t* indices; const uint8_t* ebins;
+  struct Column {
+    const int64_t* indptr; const int32_t* indices; const uint8_t* ebins; int f;
+    __device__ __forceinline__ int ld(int rid) const { return b2_csr_bin(indptr, indices, ebins, rid, f); }
+    __device__ __forceinline__ int ldcs(int rid) const { return ld(rid); }
+  };
+  __device__ __forceinline__ Column column(int f) const { return Column{indptr, indices, ebins, f}; }
+};
+
 // kCat = false: the matrix has no categorical feature; the row loop is then straight-line code whose 8 row-id loads
 // and 8 bin-byte loads the compiler batches (48 registers).  With the category test in the body it software-pipelines
 // only 2-3 deep, so numeric matrices keep their own
@@ -31,9 +53,9 @@ constexpr int kSplitPasses = kSplitChunk / kPartChunk;  // a work item is proces
 // atomic claims the output ranges of the whole item, then the rows are written out.  Claiming per 2048 rows would put
 // the counters of all nodes of a shallow level in one cache line and serialise the atomics of thousands of chunks in
 // one L2 slice, a fixed cost per level however little data it moved.
-template <int kMode, bool kRoot>
+template <int kMode, bool kRoot, typename Bins>
 __global__ void __launch_bounds__(kPartThreads)
-partition_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, const int32_t* __restrict__ ridx_in,
+partition_kernel(Bins src, const int32_t* __restrict__ ridx_in,
                  int32_t* __restrict__ ridx_out, const B2SplitWork* __restrict__ work, const B2LevelCtl* __restrict__ ctl,
                  int32_t* counters /* [2*n_work]: low word lefts, high word rows claimed */, B2FinalizeArgs fin) {
   const int n_work = ctl->n_split, total_chunks = ctl->part_chunks;
@@ -76,9 +98,9 @@ partition_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, const
         const int r = pbase + it * kPartThreads + threadIdx.x;
         rid[it] = kRoot ? (r < nrows ? w.seg_begin + row0 + r : 0) : (r < nrows ? __ldg(rsrc + it * kPartThreads) : 0);
       }
-      const uint8_t* col = bins_col + (int64_t)w.feature * col_stride;
+      const typename Bins::Column col = src.column(w.feature);
 #pragma unroll
-      for (int it = 0; it < kIters; ++it) bin[it] = (int)__ldg(col + rid[it]);   // row 0 for lanes past the end: harmless
+      for (int it = 0; it < kIters; ++it) bin[it] = col.ld(rid[it]);   // row 0 for lanes past the end: harmless
 #pragma unroll
       for (int it = 0; it < kIters; ++it) {
         const int r = pbase + it * kPartThreads + threadIdx.x;
@@ -219,9 +241,9 @@ leaf_sums_kernel(const float2* __restrict__ gh, const int32_t* __restrict__ ridx
 // kSums = false (the default whenever the per-leaf accumulators fit in shared memory): only pos is written, and
 // leaf_accumulate_kernel sums the gradient pairs afterwards in row order.  Gathering gh[rid] here costs a 32-byte
 // sector per 8-byte pair at the last level, where a node's rows are spread over the whole matrix.
-template <bool kCat, bool kRoot, bool kSums>
+template <bool kCat, bool kRoot, bool kSums, typename Bins>
 __global__ void __launch_bounds__(kPartThreads)
-final_assign_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, const int32_t* __restrict__ ridx_in,
+final_assign_kernel(Bins src, const int32_t* __restrict__ ridx_in,
                     const B2SplitWork* __restrict__ work, const B2LevelCtl* __restrict__ ctl, const float2* __restrict__ gh,
                     const int32_t* __restrict__ qexp, int leaf_bits, long long* __restrict__ sums,
                     uint16_t* __restrict__ pos) {
@@ -245,7 +267,7 @@ final_assign_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, co
     // (8 rows when no gradient pair is loaded).  Row ids and bin bytes are streamed with the evict-first hint (__ldcs), so that L2
     // keeps the partly written 32-byte sectors of pos until their other rows have been stored
     constexpr int kBatch = kSums ? 4 : 8;
-    const uint8_t* col = bins_col + (int64_t)w.feature * col_stride;
+    const typename Bins::Column col = src.column(w.feature);
     for (int r0 = threadIdx.x; r0 < nrows; r0 += kBatch * kPartThreads) {
       int rid[kBatch]; int bin[kBatch]; float2 v[kBatch];
 #pragma unroll
@@ -255,7 +277,7 @@ final_assign_kernel(const uint8_t* __restrict__ bins_col, int64_t col_stride, co
       }
 #pragma unroll
       for (int k = 0; k < kBatch; ++k) {
-        bin[k] = (int)__ldcs(col + (rid[k] < 0 ? 0 : rid[k]));
+        bin[k] = col.ldcs(rid[k] < 0 ? 0 : rid[k]);
         if (kSums) v[k] = __ldg(gh + (rid[k] < 0 ? 0 : rid[k]));
       }
 #pragma unroll
@@ -387,21 +409,56 @@ extern "C" {
 int b2_part_chunk_rows() { return b2::kPartChunk; }     // leaf-segment work items (leaf_sums)
 int b2_split_chunk_rows() { return b2::kSplitChunk; }   // split-node work items (partition / final_assign)
 
-// partition + finalize of a level: `fin` is what the last CTA writes (level_finalize.cuh)
-int b2_launch_partition(const uint8_t* bins_col, int64_t col_stride, const int32_t* ridx_in, int32_t* ridx_out,
-                        const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, int32_t* counters, int any_categorical,
-                        B2FinalizeArgs fin, int num_sms, cudaStream_t stream) {
+}  // extern "C"
+
+template <typename Bins>
+static int launch_partition(Bins src, const int32_t* ridx_in, int32_t* ridx_out, const B2SplitWork* work, const B2LevelCtl* ctl,
+                            int max_chunks, int32_t* counters, int any_categorical, B2FinalizeArgs fin, int num_sms,
+                            cudaStream_t stream) {
   if (max_chunks <= 0) max_chunks = 1;   // the last CTA finalises the level, so even an empty level launches one
   int grid = max_chunks < num_sms * 6 ? max_chunks : num_sms * 6;   // 6 CTAs per SM are resident (33 KB of shared memory, 48 registers)
 #define B2_PART_LAUNCH(MODE)                                                                                                  \
   do {                                                                                                                        \
-    if (ridx_in) b2::partition_kernel<MODE, false><<<grid, b2::kPartThreads, 0, stream>>>(bins_col, col_stride, ridx_in, ridx_out, work, ctl, counters, fin); \
-    else b2::partition_kernel<MODE, true><<<grid, b2::kPartThreads, 0, stream>>>(bins_col, col_stride, ridx_in, ridx_out, work, ctl, counters, fin);    \
+    if (ridx_in) b2::partition_kernel<MODE, false><<<grid, b2::kPartThreads, 0, stream>>>(src, ridx_in, ridx_out, work, ctl, counters, fin); \
+    else b2::partition_kernel<MODE, true><<<grid, b2::kPartThreads, 0, stream>>>(src, ridx_in, ridx_out, work, ctl, counters, fin);    \
   } while (0)
   if (any_categorical) B2_PART_LAUNCH(1);
   else B2_PART_LAUNCH(0);
 #undef B2_PART_LAUNCH
   return (int)cudaGetLastError();
+}
+
+template <typename Bins>
+static int launch_final_assign(Bins src, const int32_t* ridx_in, const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks,
+                               const float2* gh, const int32_t* qexp, int leaf_bits, long long* sums, uint16_t* pos,
+                               int any_categorical, int num_sms, cudaStream_t stream) {
+  if (max_chunks <= 0) return 0;
+  int grid = max_chunks < num_sms * 8 ? max_chunks : num_sms * 8;
+  // sums == nullptr: pos only (the leaves are summed by leaf_accumulate_kernel)
+#define B2_FA_LAUNCH(CAT, ROOT)                                                                                               \
+  do {                                                                                                                        \
+    if (sums) b2::final_assign_kernel<CAT, ROOT, true><<<grid, b2::kPartThreads, 0, stream>>>(src, ridx_in, work, ctl, gh, qexp, leaf_bits, sums, pos); \
+    else b2::final_assign_kernel<CAT, ROOT, false><<<grid, b2::kPartThreads, 0, stream>>>(src, ridx_in, work, ctl, gh, qexp, leaf_bits, sums, pos);    \
+  } while (0)
+  if (any_categorical) { if (ridx_in) B2_FA_LAUNCH(true, false); else B2_FA_LAUNCH(true, true); }
+  else { if (ridx_in) B2_FA_LAUNCH(false, false); else B2_FA_LAUNCH(false, true); }
+#undef B2_FA_LAUNCH
+  return (int)cudaGetLastError();
+}
+
+extern "C" {
+// partition + finalize of a level: `fin` is what the last CTA writes (level_finalize.cuh)
+int b2_launch_partition(const uint8_t* bins_col, int64_t col_stride, const int32_t* ridx_in, int32_t* ridx_out,
+                        const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, int32_t* counters, int any_categorical,
+                        B2FinalizeArgs fin, int num_sms, cudaStream_t stream) {
+  return launch_partition(b2::ColBins{bins_col, col_stride}, ridx_in, ridx_out, work, ctl, max_chunks, counters, any_categorical,
+                          fin, num_sms, stream);
+}
+int b2_launch_partition_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, const int32_t* ridx_in,
+                            int32_t* ridx_out, const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, int32_t* counters,
+                            int any_categorical, B2FinalizeArgs fin, int num_sms, cudaStream_t stream) {
+  return launch_partition(b2::CsrBins{indptr, indices, ebins}, ridx_in, ridx_out, work, ctl, max_chunks, counters,
+                          any_categorical, fin, num_sms, stream);
 }
 int b2_launch_leaf_sums(const float2* gh, const int32_t* ridx0, const int32_t* ridx1, const B2SegWork* work,
                         const B2LevelCtl* ctl, int max_chunks, const int32_t* qexp, int leaf_bits, long long* sums,
@@ -414,18 +471,15 @@ int b2_launch_leaf_sums(const float2* gh, const int32_t* ridx0, const int32_t* r
 int b2_launch_final_assign(const uint8_t* bins_col, int64_t col_stride, const int32_t* ridx_in, const B2SplitWork* work,
                            const B2LevelCtl* ctl, int max_chunks, const float2* gh, const int32_t* qexp, int leaf_bits,
                            long long* sums, uint16_t* pos, int any_categorical, int num_sms, cudaStream_t stream) {
-  if (max_chunks <= 0) return 0;
-  int grid = max_chunks < num_sms * 8 ? max_chunks : num_sms * 8;
-  // sums == nullptr: pos only (the leaves are summed by leaf_accumulate_kernel)
-#define B2_FA_LAUNCH(CAT, ROOT)                                                                                               \
-  do {                                                                                                                        \
-    if (sums) b2::final_assign_kernel<CAT, ROOT, true><<<grid, b2::kPartThreads, 0, stream>>>(bins_col, col_stride, ridx_in, work, ctl, gh, qexp, leaf_bits, sums, pos); \
-    else b2::final_assign_kernel<CAT, ROOT, false><<<grid, b2::kPartThreads, 0, stream>>>(bins_col, col_stride, ridx_in, work, ctl, gh, qexp, leaf_bits, sums, pos);    \
-  } while (0)
-  if (any_categorical) { if (ridx_in) B2_FA_LAUNCH(true, false); else B2_FA_LAUNCH(true, true); }
-  else { if (ridx_in) B2_FA_LAUNCH(false, false); else B2_FA_LAUNCH(false, true); }
-#undef B2_FA_LAUNCH
-  return (int)cudaGetLastError();
+  return launch_final_assign(b2::ColBins{bins_col, col_stride}, ridx_in, work, ctl, max_chunks, gh, qexp, leaf_bits, sums, pos,
+                             any_categorical, num_sms, stream);
+}
+int b2_launch_final_assign_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, const int32_t* ridx_in,
+                               const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, const float2* gh,
+                               const int32_t* qexp, int leaf_bits, long long* sums, uint16_t* pos, int any_categorical,
+                               int num_sms, cudaStream_t stream) {
+  return launch_final_assign(b2::CsrBins{indptr, indices, ebins}, ridx_in, work, ctl, max_chunks, gh, qexp, leaf_bits, sums,
+                             pos, any_categorical, num_sms, stream);
 }
 int b2_leaf_acc_max_depth() { return b2::kLeafAccMaxDepth; }
 int b2_launch_leaf_accumulate(const float2* gh, const uint16_t* pos, int64_t n, int max_depth, const int32_t* qexp, int leaf_bits,

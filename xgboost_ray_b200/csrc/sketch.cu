@@ -201,8 +201,27 @@ __global__ void cat_stats_kernel(const float* __restrict__ X, int64_t n, int F, 
   }
 }
 
-// bin = upper_bound(cuts_f, x) clamped; missing -> 255.  One thread per matrix element.
+// bin = upper_bound(cuts_f, x) clamped; missing -> 255.
 // Categorical feature: bin = category code (clamped to the codes the cuts know).
+__device__ __forceinline__ int bin_value(float x, int f, float missing, int missing_is_nan, const int32_t* __restrict__ cut_ptrs,
+                                         const float* __restrict__ cut_vals, const uint8_t* __restrict__ is_cat) {
+  int b;
+  if (is_missing(x, missing, missing_is_nan)) b = B2_MISSING_BIN;
+  else if (is_cat && is_cat[f]) {
+    const int nf = cut_ptrs[f + 1] - cut_ptrs[f];
+    b = x >= 0.0f ? (x > 255.0f ? 255 : (int)x) : 0;
+    if (b >= nf) b = nf - 1;
+  } else {
+    const int p0 = cut_ptrs[f], nf = cut_ptrs[f + 1] - p0;
+    const float* cv = cut_vals + p0;
+    int lo = 0, hi = nf;
+    while (lo < hi) { int mid = (lo + hi) >> 1; if (__ldg(cv + mid) > x) hi = mid; else lo = mid + 1; }
+    b = lo >= nf ? nf - 1 : lo;
+  }
+  return b;
+}
+
+// One thread per matrix element.
 __global__ void bin_kernel(const float* __restrict__ X, int64_t n, int F, float missing, int missing_is_nan,
                            const int32_t* __restrict__ cut_ptrs, const float* __restrict__ cut_vals,
                            const int32_t* __restrict__ feat_byte, const uint8_t* __restrict__ is_cat, int row_stride,
@@ -210,20 +229,7 @@ __global__ void bin_kernel(const float* __restrict__ X, int64_t n, int F, float 
   const int64_t total = n * F;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
     const int64_t row = e / F; const int f = (int)(e - row * F);
-    const float x = X[e];
-    int b;
-    if (is_missing(x, missing, missing_is_nan)) b = B2_MISSING_BIN;
-    else if (is_cat && is_cat[f]) {
-      const int nf = cut_ptrs[f + 1] - cut_ptrs[f];
-      b = x >= 0.0f ? (x > 255.0f ? 255 : (int)x) : 0;
-      if (b >= nf) b = nf - 1;
-    } else {
-      const int p0 = cut_ptrs[f], nf = cut_ptrs[f + 1] - p0;
-      const float* cv = cut_vals + p0;
-      int lo = 0, hi = nf;
-      while (lo < hi) { int mid = (lo + hi) >> 1; if (__ldg(cv + mid) > x) hi = mid; else lo = mid + 1; }
-      b = lo >= nf ? nf - 1 : lo;
-    }
+    const int b = bin_value(X[e], f, missing, missing_is_nan, cut_ptrs, cut_vals, is_cat);
     bins[row * row_stride + feat_byte[f]] = (uint8_t)b;
     bins_col[(int64_t)f * col_stride + row] = (uint8_t)b;
   }
@@ -288,6 +294,15 @@ bin_tiled_kernel(const float* __restrict__ X, int64_t n, int F, float missing, i
     }
     __syncthreads();
   }
+}
+
+// CSR bin layout: the bin of every stored entry (one thread per entry), by the rule of bin_kernel.  A stored NaN or
+// `missing` gets the sentinel, as the same cell of the dense twin does.
+__global__ void bin_csr_kernel(const int32_t* __restrict__ indices, const float* __restrict__ values, int64_t nnz, float missing,
+                               int missing_is_nan, const int32_t* __restrict__ cut_ptrs, const float* __restrict__ cut_vals,
+                               const uint8_t* __restrict__ is_cat, uint8_t* __restrict__ ebins) {
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += (int64_t)gridDim.x * blockDim.x)
+    ebins[e] = (uint8_t)bin_value(values[e], indices[e], missing, missing_is_nan, cut_ptrs, cut_vals, is_cat);
 }
 
 }  // namespace b2
@@ -399,6 +414,13 @@ int b2_launch_bin(const float* X, int64_t n, int F, float missing, const int32_t
   }
   b2::bin_kernel<<<sk_grid(n * F, num_sms), 256, 0, s>>>(X, n, F, missing, missing != missing ? 1 : 0, cut_ptrs, cut_vals,
                                                         feat_byte, is_cat, row_stride, bins, bins_col, col_stride);
+  return (int)cudaGetLastError();
+}
+int b2_launch_bin_csr(const int32_t* indices, const float* values, int64_t nnz, float missing, const int32_t* cut_ptrs,
+                      const float* cut_vals, const uint8_t* is_cat, uint8_t* ebins, int num_sms, cudaStream_t s) {
+  if (nnz <= 0) return 0;
+  b2::bin_csr_kernel<<<sk_grid(nnz, num_sms), 256, 0, s>>>(indices, values, nnz, missing, missing != missing ? 1 : 0, cut_ptrs,
+                                                          cut_vals, is_cat, ebins);
   return (int)cudaGetLastError();
 }
 // stats must be initialised to {-1, 0, INT_MIN} per categorical feature

@@ -81,6 +81,18 @@ csr_extract_keys_kernel(const int64_t* __restrict__ indptr, const int32_t* __res
   }
 }
 
+// out [n][F] = the dense bins of a CSR-layout matrix: the sentinel in every cell, then each row's stored bins (one
+// thread per row)
+__global__ void __launch_bounds__(kSparseThreads)
+csr_bins_densify_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, const uint8_t* __restrict__ ebins,
+                        int64_t n, int F, uint8_t* __restrict__ out) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    uint8_t* row = out + i * F;
+    for (int f = 0; f < F; ++f) row[f] = B2_MISSING_BIN;
+    for (int64_t e = indptr[i]; e < indptr[i + 1]; ++e) row[indices[e]] = ebins[e];
+  }
+}
+
 }  // namespace b2
 
 static inline int sparse_grid(int64_t work, int num_sms) {
@@ -100,6 +112,13 @@ int b2_launch_csr_validate(const int64_t* indptr, const int32_t* indices, int64_
   return (int)cudaGetLastError();
 }
 
+int b2_launch_csr_bins_densify(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, int64_t n, int F,
+                               uint8_t* out, int num_sms, cudaStream_t s) {
+  if (n <= 0) return 0;
+  const int64_t want = (n + b2::kSparseThreads - 1) / b2::kSparseThreads, cap = (int64_t)num_sms * 8;
+  b2::csr_bins_densify_kernel<<<(int)std::min(want, cap), b2::kSparseThreads, 0, s>>>(indptr, indices, ebins, n, F, out);
+  return (int)cudaGetLastError();
+}
 int b2_launch_csr_densify(const int64_t* indptr, const int32_t* indices, const float* values, int64_t r0, int64_t rows, int F,
                           float* out, int num_sms, cudaStream_t s) {
   if (rows <= 0) return 0;

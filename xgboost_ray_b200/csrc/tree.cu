@@ -179,6 +179,7 @@ void ensure_ctl_tables(Booster* b) {
   if (!b->d_part_done.p) { b->d_part_done.ensure(1); CUDA_CHECK(cudaMemsetAsync(b->d_part_done.p, 0, sizeof(uint32_t), b->ctx->stream)); }
   if (!b->d_eval_done.p) { b->d_eval_done.ensure(1); CUDA_CHECK(cudaMemsetAsync(b->d_eval_done.p, 0, sizeof(uint32_t), b->ctx->stream)); }
   b->d_cand_best.ensure(half);
+  if (b->train->csr_bins) b->csr_hist_tot.ensure(2 * half);
   b->d_leaves.ensure(L.max_nodes); b->d_seg_work.ensure(L.max_nodes);
   b->d_leaf_sums.ensure(4 * lcap); b->d_leaf_values.ensure(lcap);   // [leaf][g, h][hi, lo] limbs (common.cuh)
   if (b->ic_words > 0) b->d_ic_compat.ensure(L.max_nodes * (size_t)b->ic_words);
@@ -408,10 +409,16 @@ void launch_hist(Booster* b, TreeStats& st, const int2* q, const int32_t* ridx, 
     root = 1; chunk_rows = pick_chunk_rows(b, n); chunks = (int)((n + chunk_rows - 1) / chunk_rows);
   }
   cudaEvent_t e0 = nullptr, e1 = nullptr;
+  if (m->csr_bins) CUDA_CHECK(cudaMemsetAsync(b->csr_hist_tot.p, 0, 2 * (size_t)nodes * sizeof(long long), b->ctx->stream));
   record_hist_launch(b, st, e0, e1, true);
-  LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, q, ridx, b->d_hist_work.p, root, chunks, chunk_rows,
-                              window_rows_for(b->p.qbits), m->n_groups, tgt, ctl, b->log2_shards, nodes, b->ctx->num_sms,
-                              b->ctx->stream));
+  if (m->csr_bins)
+    LAUNCH_CHECK(b2_launch_hist_csr(m->csr_indptr.p, m->csr_indices.p, m->ebins.p, m->d_feat_byte.p, m->d_group_size.p, q, ridx,
+                                    b->d_hist_work.p, root, chunks, chunk_rows, m->n_groups, tgt, b->csr_hist_tot.p, ctl,
+                                    b->log2_shards, nodes, b->ctx->num_sms, b->ctx->stream));
+  else
+    LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, q, ridx, b->d_hist_work.p, root, chunks, chunk_rows,
+                                window_rows_for(b->p.qbits), m->n_groups, tgt, ctl, b->log2_shards, nodes, b->ctx->num_sms,
+                                b->ctx->stream));
   record_hist_launch(b, st, e0, e1, false);
   st.hist_launches++; st.kernel_launches++;
 }
@@ -467,9 +474,14 @@ void partition_level(Booster* b, TreeStats& st, int d) {
   fin.max_pairs = 1 << d; fin.need_hist = d + 1 < p.max_depth ? 1 : 0;
   fin.n_streams = std::max(1, b->ctx->num_sms * 3 / m->n_groups); fin.window_rows = window_rows_for(p.qbits);
   fin.chunk_rows_override = p.hist_chunk_rows;
-  LAUNCH_CHECK(b2_launch_partition(m->bins_col.p, m->col_stride, level_ridx(b, d), b->ridx[nxt].p, b->d_split_work.p,
-                                   ctl + cur, split_work_items(b, d), b->d_counters.p, m->any_cat() ? 1 : 0, fin,
-                                   b->ctx->num_sms, b->ctx->stream));
+  if (m->csr_bins)
+    LAUNCH_CHECK(b2_launch_partition_csr(m->csr_indptr.p, m->csr_indices.p, m->ebins.p, level_ridx(b, d), b->ridx[nxt].p,
+                                         b->d_split_work.p, ctl + cur, split_work_items(b, d), b->d_counters.p,
+                                         m->any_cat() ? 1 : 0, fin, b->ctx->num_sms, b->ctx->stream));
+  else
+    LAUNCH_CHECK(b2_launch_partition(m->bins_col.p, m->col_stride, level_ridx(b, d), b->ridx[nxt].p, b->d_split_work.p,
+                                     ctl + cur, split_work_items(b, d), b->d_counters.p, m->any_cat() ? 1 : 0, fin,
+                                     b->ctx->num_sms, b->ctx->stream));
   st.kernel_launches++;
 }
 
@@ -482,8 +494,13 @@ void assign_leaves(Booster* b, TreeStats& st, int d, const float2* gh, const int
   const int max_leaf_chunks = (int)((m->n + lchunk - 1) / lchunk) + (1 << b->p.max_depth);
   LAUNCH_CHECK(b2_launch_leaf_sums(gh, b->ridx[0].p, b->ridx[1].p, b->d_seg_work.p, ctl + 2, max_leaf_chunks, qexp, 40, sums,
                                    b->pos.p, sms, s));
-  LAUNCH_CHECK(b2_launch_final_assign(m->bins_col.p, m->col_stride, level_ridx(b, d), b->d_split_work.p, ctl + (d & 1),
-                                      split_work_items(b, d), gh, qexp, 40, sums, b->pos.p, m->any_cat() ? 1 : 0, sms, s));
+  if (m->csr_bins)
+    LAUNCH_CHECK(b2_launch_final_assign_csr(m->csr_indptr.p, m->csr_indices.p, m->ebins.p, level_ridx(b, d), b->d_split_work.p,
+                                            ctl + (d & 1), split_work_items(b, d), gh, qexp, 40, sums, b->pos.p,
+                                            m->any_cat() ? 1 : 0, sms, s));
+  else
+    LAUNCH_CHECK(b2_launch_final_assign(m->bins_col.p, m->col_stride, level_ridx(b, d), b->d_split_work.p, ctl + (d & 1),
+                                        split_work_items(b, d), gh, qexp, 40, sums, b->pos.p, m->any_cat() ? 1 : 0, sms, s));
   st.kernel_launches += 2;
 }
 

@@ -79,6 +79,7 @@ ABI = {
     "B2_MatrixCutsSize": (C.c_int, [_H, _IP]),
     "B2_MatrixGetCuts": (C.c_int, [_H, _IP, _FP, _FP, _BP]),
     "B2_MatrixGetBins": (C.c_int, [_H, _BP]),
+    "B2_MatrixSetBinLayout": (C.c_int, [_H, C.c_int32]),
     "B2_MatrixFree": (C.c_int, [_H]),
     "B2_BoosterCreate": (C.c_int, [C.c_char_p, _H, _H, C.POINTER(_H)]),
     "B2_BoosterSetParam": (C.c_int, [_H, C.c_char_p]),
@@ -109,6 +110,8 @@ ABI = {
     "B2_BoosterFree": (C.c_int, [_H]),
     "B2_HistBuildRaw": (C.c_int, [_BP, C.c_int64, C.c_int32, _IP, _IP, _IP, C.c_int64, C.c_int32, C.c_int32, C.c_int,
                                   C.POINTER(C.c_int64), _FP]),
+    "B2_HistBuildRawCSR": (C.c_int, [_LP, _IP, _BP, C.c_int64, C.c_int32, _IP, _IP, _IP, C.c_int64, C.c_int32, C.c_int,
+                                     C.POINTER(C.c_int64), _FP]),
     "B2_QuantizeRaw": (C.c_int, [_FP, _FP, C.c_int64, C.c_int32, C.c_int, _IP, _IP]),
 }
 
@@ -320,6 +323,16 @@ def _row_steps(indptr, indices):
 
 
 # ----------------------------------------------------------------------------- DMatrix
+# DMatrix(bin_layout=...): how a quantised matrix keeps its bins (B2_MatrixSetBinLayout, DESIGN.md 2 item 26)
+BIN_LAYOUTS = {"auto": 0, "dense": 1, "csr": 2}
+
+
+def bin_layout_code(bin_layout):
+    if not isinstance(bin_layout, str) or bin_layout not in BIN_LAYOUTS:
+        raise XGBoostError("bin_layout must be one of %s, got %r" % (", ".join(map(repr, BIN_LAYOUTS)), bin_layout))
+    return BIN_LAYOUTS[bin_layout]
+
+
 class DMatrix:
     """Device matrix.  Float data is uploaded at construction; quantisation (GPU sketch + binning)
     happens when a Booster first trains on it, because cuts are global over the communicator.
@@ -327,12 +340,18 @@ class DMatrix:
     multi_target=True accepts a label of shape (n, T), T > 1: multi-target regression or multi-label classification,
     one tree per column and round.  Without it a label of several columns is refused, so that a label of the wrong
     shape (one-hot classes, a target passed twice) is not trained as T independent outputs.  RayDMatrix and the sklearn
-    estimators, whose users ask for several label columns explicitly, set it for them."""
+    estimators, whose users ask for several label columns explicitly, set it for them.
+
+    bin_layout chooses how the quantised bins are kept on the device.  "dense": two n x F byte copies.  "csr" (a
+    scipy.sparse input only): one byte per stored entry, next to the CSR's column indices, so that a sparse matrix whose
+    dense bins would not fit the GPU still trains; the model is byte-identical to the dense layout's.  "auto" (the
+    default) takes "csr" only when the two dense copies would exceed half of the device's memory."""
 
     def __init__(self, data, label=None, weight=None, base_margin=None, missing=None, feature_names=None,
                  feature_types=None, nthread=None, enable_categorical=False, max_bin=None, ref=None,
                  device=None, label_lower_bound=None, label_upper_bound=None, qid=None, group=None, multi_target=False,
-                 **kwargs):
+                 bin_layout="auto", **kwargs):
+        layout = bin_layout_code(bin_layout)
         if is_sparse(data):
             data = canonical_csr(data)
         elif hasattr(data, "values") and not isinstance(data, np.ndarray):  # pandas
@@ -385,7 +404,10 @@ class DMatrix:
             if data.ndim != 2:
                 raise XGBoostError("DMatrix data must be 2-dimensional")
             data = _f32c(data)
+        if layout == BIN_LAYOUTS["csr"] and not isinstance(data, CSRArrays):
+            raise XGBoostError('bin_layout="csr" needs a scipy.sparse matrix: this DMatrix holds dense rows')
         self._host = data
+        self.bin_layout = bin_layout
         self.missing = float("nan") if missing is None else float(missing)
         self.device = _default_device() if device is None else int(device)
         self.feature_names = list(feature_names) if feature_names is not None else None
@@ -434,6 +456,8 @@ class DMatrix:
         else:
             _check(lib().B2_MatrixCreateFromDense(_fp(self._host), n, f, self.missing, self.device, C.byref(h)))
             self.handle = h.value
+        if layout != BIN_LAYOUTS["auto"]:
+            _check(lib().B2_MatrixSetBinLayout(self.handle, layout))
         if self.feature_types is not None:
             if len(self.feature_types) != f:
                 raise XGBoostError("feature_types has %d entries for %d features" % (len(self.feature_types), f))
@@ -639,7 +663,7 @@ class DMatrix:
             feature_types=None if self.feature_types is None else list(self.feature_types),
             enable_categorical=self.enable_categorical, max_bin=self.max_bin, ref=None, _quantized=False,
             _has_raw=True, multi_target=self.multi_target, _label=rows(self._label), _weight=rows(self._weight),
-            _base_margin=rows(self._base_margin), _group_sizes=None, ingest="slice")
+            _base_margin=rows(self._base_margin), _group_sizes=None, ingest="slice", bin_layout=self.bin_layout)
         for field in ("_label_lower_bound", "_label_upper_bound"):
             if field in self.__dict__:
                 setattr(out, field, rows(getattr(self, field)))
@@ -2369,6 +2393,27 @@ def hist_build_raw(bins, qg, qh, ridx=None, window_rows=8192, chunk_rows=2048, d
     _check(lib().B2_HistBuildRaw(_bp(bins), n, f, _ip(qg), _ip(qh), _ip(ri), nsel, window_rows, chunk_rows,
                                  _default_device() if device is None else device,
                                  out.ctypes.data_as(C.POINTER(C.c_int64)), C.byref(ms)))
+    return out, ms.value
+
+
+def hist_build_raw_csr(indptr, indices, bins, n_cols, qg, qh, ridx=None, chunk_rows=2048, device=None):
+    """Kernel-level entry (tests): hist_build_raw's histogram from the CSR bin layout, one bin per stored entry
+    (absent entries have bin 255).  Returns (hist [F,256,2] int64, kernel_ms)."""
+    indptr = np.ascontiguousarray(indptr, np.int64)
+    indices = np.ascontiguousarray(indices, np.int32)
+    bins = np.ascontiguousarray(bins, np.uint8)
+    n = indptr.size - 1
+    if indices.size != indptr[-1] or bins.size != indptr[-1]:
+        raise ValueError("indices and bins must hold indptr[-1] entries")
+    qg = np.ascontiguousarray(qg, np.int32)
+    qh = np.ascontiguousarray(qh, np.int32)
+    ri = None if ridx is None else np.ascontiguousarray(ridx, np.int32)
+    nsel = n if ri is None else ri.size
+    out = np.zeros((n_cols, 256, 2), np.int64)
+    ms = C.c_float(0)
+    _check(lib().B2_HistBuildRawCSR(indptr.ctypes.data_as(_LP), _ip(indices), _bp(bins), n, n_cols, _ip(qg), _ip(qh), _ip(ri),
+                                    nsel, chunk_rows, _default_device() if device is None else device,
+                                    out.ctypes.data_as(C.POINTER(C.c_int64)), C.byref(ms)))
     return out, ms.value
 
 

@@ -23,7 +23,7 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 import numpy as np
 
 from xgboost_ray_b200.data_sources import LoadedFrame, RayFileType, Sparse, resolve_data_source  # noqa: F401
-from xgboost_ray_b200.engine import CSRArrays
+from xgboost_ray_b200.engine import CSRArrays, bin_layout_code
 
 
 class RayShardingMode(Enum):
@@ -305,7 +305,8 @@ class RayDMatrix:
                  label_lower_bound=None, label_upper_bound=None, feature_names=None, feature_types=None, qid=None,
                  enable_categorical=None, num_actors: Optional[int] = None, filetype: Optional[RayFileType] = None,
                  ignore: Optional[List[str]] = None, distributed: Optional[bool] = None,
-                 sharding: RayShardingMode = RayShardingMode.INTERLEAVED, lazy: bool = False, **kwargs):
+                 sharding: RayShardingMode = RayShardingMode.INTERLEAVED, lazy: bool = False, bin_layout: str = "auto",
+                 **kwargs):
         if kwargs.get("group", None) is not None:
             raise ValueError("`group` parameter is not supported. If you are using XGBoost-Ray, use `qid` parameter instead.")
         if qid is not None and weight is not None:
@@ -317,6 +318,8 @@ class RayDMatrix:
         self.feature_names, self.feature_types = feature_names, feature_types
         self.qid = qid
         self.enable_categorical = enable_categorical
+        bin_layout_code(bin_layout)
+        self.bin_layout = bin_layout   # the actors' DMatrix(bin_layout=...)
         self.missing = missing
         self.num_actors = num_actors
         self.sharding = sharding
