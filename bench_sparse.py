@@ -9,9 +9,9 @@ S1  bench.py's C3 generator (10M x 100) with 90 % and 99 % of the entries droppe
     seconds, rounds/s without and with the evaluation set, predict rows/s, B2_MatrixDeviceBytes before and after
     quantisation (without keep_raw) and the model's sha256 (the CSR and the twin must give the same model).
 S2  8M x 2,500 at 0.1 % density: the twin (80 GB) does not fit on the card, so only the CSR runs (depth 6).
-Kernel times of csr_densify_kernel (one tile) and csr_extract_keys_kernel (one batch of 8 features) from CUDA events,
-with the bytes the algorithm moves (4 rows nf written, 8 per entry of the window and 8 per row read) over the time
-against the 3.35 TB/s HBM3 bandwidth of the H100 SXM data sheet: both kernels are memory-bound (no arithmetic).
+Kernel time of csr_densify_kernel (one tile) from CUDA events, with the bytes the algorithm moves (4 rows F written,
+8 per entry and 8 per row read) over the time against the 3.35 TB/s HBM3 bandwidth of the H100 SXM data sheet: the
+kernel is memory-bound (no arithmetic).  The sketch's entry pass is measured by bench_sparse_native.py.
 The card's name and power limit are read in the same run.  Writes nothing to the tree."""
 import argparse
 import ctypes as C
@@ -101,8 +101,8 @@ def run_input(E, params, X, y, Xe, ye, rounds):
             "model_sha256": hashlib.sha256(bytes(bst.save_raw())).hexdigest()}
 
 
-def kernel_times(E, X, f0, nf, repeats=20):
-    """CUDA-event times of one densified tile and one key batch of the CSR X (indptr / indices / values on the device)."""
+def kernel_times(E, X, repeats=20):
+    """CUDA-event time of one densified tile of the CSR X (indptr / indices / values on the device)."""
     import torch
     lib = E.lib()
     c = E.canonical_csr(X)
@@ -112,27 +112,18 @@ def kernel_times(E, X, f0, nf, repeats=20):
     ix = torch.from_numpy(c.indices).to(dev)
     vs = torch.from_numpy(c.values).to(dev)
     rows = min(E.raw_tile_rows(F), n)
-    n_pad = n
     tile = torch.empty(rows * F, dtype=torch.float32, device=dev)
-    keys = torch.empty(8 * n_pad, dtype=torch.int32, device=dev)
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     vp = C.c_void_p
-    for name, argt in (("b2_launch_csr_densify", [vp, vp, vp, C.c_int64, C.c_int64, C.c_int, vp, C.c_int, vp]),
-                       ("b2_launch_csr_extract_keys", [vp, vp, vp, C.c_int64, C.c_int, C.c_int, C.c_float, vp, C.c_int64,
-                                                       C.c_int, vp])):
-        getattr(lib, name).argtypes = argt
-        getattr(lib, name).restype = C.c_int
+    lib.b2_launch_csr_densify.argtypes = [vp, vp, vp, C.c_int64, C.c_int64, C.c_int, vp, C.c_int, vp]
+    lib.b2_launch_csr_densify.restype = C.c_int
     stream = torch.cuda.current_stream().cuda_stream
 
     def densify():
         return lib.b2_launch_csr_densify(ip.data_ptr(), ix.data_ptr(), vs.data_ptr(), 0, rows, F, tile.data_ptr(), sms, stream)
 
-    def extract():
-        return lib.b2_launch_csr_extract_keys(ip.data_ptr(), ix.data_ptr(), vs.data_ptr(), n, f0, nf, float("nan"),
-                                              keys.data_ptr(), n_pad, sms, stream)
-
     out = {}
-    for name, fn, written_rows, width in (("csr_densify_kernel", densify, rows, F), ("csr_extract_keys_kernel", extract, n, nf)):
+    for name, fn, written_rows, width in (("csr_densify_kernel", densify, rows, F),):
         assert fn() == 0
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -143,7 +134,7 @@ def kernel_times(E, X, f0, nf, repeats=20):
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / repeats
         ind = c.indices[: c.indptr[written_rows]]
-        entries = int(ind.size) if width == F else int(((ind >= f0) & (ind < f0 + nf)).sum())
+        entries = int(ind.size)
         nbytes = 4 * written_rows * width + 8 * entries + 8 * written_rows
         out[name] = {"rows": int(written_rows), "nf": int(width), "entries": entries, "ms": round(ms, 4),
                      "bytes": nbytes, "GBps": round(nbytes / ms / 1e6, 1),
@@ -177,7 +168,7 @@ def main():
         r["same_model"] = r["csr"]["model_sha256"] == r["twin"]["model_sha256"]
         out["S1"]["drop_%d" % round(drop * 100)] = r
         if drop == 0.99:
-            kt["S1_drop_99"] = kernel_times(E, csr, 0, 8)
+            kt["S1_drop_99"] = kernel_times(E, csr)
         del csr, twin
     del X, y
     if not args.no_s2:
@@ -186,7 +177,7 @@ def main():
         ne = min(args.eval_rows, args.s2_rows)
         out["S2"] = dict(run_input(E, p2, Xs, ys, Xs[:ne], ys[:ne], args.s2_rounds), nnz=int(Xs.nnz),
                          dense_twin_bytes=4 * args.s2_rows * 2500)
-        kt["S2"] = kernel_times(E, Xs, 0, 8)
+        kt["S2"] = kernel_times(E, Xs)
     out["kernels"] = kt
     print(json.dumps(out))
 

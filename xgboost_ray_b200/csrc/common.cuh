@@ -171,8 +171,10 @@ __device__ __forceinline__ int b2_tree_step(const B2TreeNodeDev& nd, float v, fl
   return v < nd.cond ? nd.left : nd.right;
 }
 
-// node id of the leaf row x reaches in the tree whose nodes start at tn
-__device__ __forceinline__ int b2_tree_leaf(const B2TreeNodeDev* __restrict__ tn, const float* __restrict__ x, float missing,
+// node id of the leaf row x reaches in the tree whose nodes start at tn; x[f] is the row's raw value of feature f (a
+// dense row pointer, or a B2CsrRow)
+template <typename Row>
+__device__ __forceinline__ int b2_tree_leaf(const B2TreeNodeDev* __restrict__ tn, const Row& x, float missing,
                                             int missing_is_nan, const uint32_t* __restrict__ cat_table, float* leaf_value) {
   int nid = 0;
   B2TreeNodeDev nd = tn[0];
@@ -198,6 +200,36 @@ __device__ __forceinline__ int b2_csr_bin(const int64_t* __restrict__ indptr, co
   }
   return (lo < end && __ldg(indices + lo) == f) ? (int)__ldg(ebins + lo) : B2_MISSING_BIN;
 }
+
+// ---- raw rows of the tree walks (predict, leaf indices, refresh).  A CSR row's value of feature f: the stored float,
+// found by binary search in the row's increasing columns, or NaN when the row does not store f -- the value the dense
+// twin holds in that absent cell, so a walk over the CSR takes the twin's path.
+__device__ __forceinline__ float b2_csr_value(const int32_t* __restrict__ indices, const float* __restrict__ values, int64_t lo,
+                                              int64_t end, int f) {
+  int64_t hi = end;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (__ldg(indices + mid) < f) lo = mid + 1; else hi = mid;
+  }
+  return (lo < end && __ldg(indices + lo) == f) ? __ldg(values + lo) : __int_as_float(0x7fc00000);
+}
+struct B2CsrRow {
+  const int32_t* indices; const float* values; int64_t begin, end;
+  __device__ __forceinline__ float operator[](int f) const { return b2_csr_value(indices, values, begin, end, f); }
+};
+// Where a walk kernel finds row i: b2_row(rows, i, F) is the row accessor.  Dense rows are the kernels' X pointer, kept
+// __restrict__ through the template argument so that the dense instantiations read X as the untemplated kernels did.
+typedef const float* __restrict__ B2DenseRows;
+struct B2CsrRows { const int64_t* indptr; const int32_t* indices; const float* values; };
+__device__ __forceinline__ const float* b2_row(const float* X, int64_t i, int F) { return X + i * F; }
+__device__ __forceinline__ B2CsrRow b2_row(const B2CsrRows& r, int64_t i, int) {
+  return B2CsrRow{r.indices, r.values, __ldg(r.indptr + i), __ldg(r.indptr + i + 1)};
+}
+// x[f] read through the read-only data path (a CSR row's lookup already is)
+__device__ __forceinline__ float b2_ldg_value(const float* x, int f) { return __ldg(x + f); }
+__device__ __forceinline__ float b2_ldg_value(const B2CsrRow& x, int f) { return x[f]; }
+// a matrix's raw values as the walk launchers take them: the CSR arrays when indptr != nullptr, else X [n][F]
+struct B2RawRows { const float* X; const int64_t* indptr; const int32_t* indices; const float* values; };
 
 // ---- device-resident control tables of the sync-free level loop (control_kernel.cu)
 struct B2LevelCtl {

@@ -167,7 +167,7 @@ struct Matrix : HandleBase {
   DevBuf<float> raw;     // [n][F], optional
   // CSR raw values instead of raw (B2_MatrixCreateFromCSR): row i stores entries [indptr[i], indptr[i+1]) of indices /
   // values, columns strictly increasing; an entry a row does not store is missing.  Kernels get raw rows through
-  // raw_rows / for_raw_tiles, never from these buffers directly.
+  // raw_source, raw_rows or for_raw_tiles, never from these buffers directly.
   bool csr = false;
   int64_t nnz = 0;
   DevBuf<int64_t> csr_indptr; DevBuf<int32_t> csr_indices; DevBuf<float> csr_values;
@@ -237,6 +237,8 @@ constexpr size_t kRawTileBytes = (size_t)256 << 20;   // largest dense tile dens
 int64_t raw_tile_rows(const Matrix* m);
 // dense float rows [r0, r0 + rows) x [0, F): a pointer into raw, or `tile` filled from the CSR (rows <= raw_tile_rows)
 const float* raw_rows(Matrix* m, int64_t r0, int64_t rows, DevBuf<float>& tile);
+// every row's raw values for the tree walks, which read a CSR matrix's stored entries directly (no dense tile)
+B2RawRows raw_source(const Matrix* m);
 // fn(X, r0, rows) over consecutive raw tiles of at most max_rows rows covering every row (once with rows = 0 for an
 // empty matrix).  Uncapped, a dense matrix is one call with X = raw: the kernels run as on a plain dense matrix.
 template <typename Fn>

@@ -161,10 +161,10 @@ int b2_launch_quantize(const float2* gh, int64_t n, const int32_t* qexp, int qbi
 // out[2] += the rows of mlogloss / merror whose label is not a class index
 int b2_launch_metric(int objective, int metric, int K, float metric_param, const float* margin, const float* label,
                      const float* weight, int64_t n, double* partial, double* out, int num_sms, cudaStream_t s);
-int b2_launch_predict(const float* X, int64_t n, int F, float missing, const B2TreeNodeDev* nodes, const int32_t* tree_offset,
+int b2_launch_predict(B2RawRows src, int64_t n, int F, float missing, const B2TreeNodeDev* nodes, const int32_t* tree_offset,
                       const uint32_t* cat_table, int tree_begin, int tree_end, int K, int npt, const float* weights, float* out,
                       int num_sms, cudaStream_t s);
-int b2_launch_predict_vector(const float* X, int64_t n, int F, float missing, const B2TreeNodeDev* nodes,
+int b2_launch_predict_vector(B2RawRows src, int64_t n, int F, float missing, const B2TreeNodeDev* nodes,
                              const int32_t* tree_offset, const float* leaf_vec, int tree_begin, int tree_end, int T, float* out,
                              int num_sms, cudaStream_t s);
 int b2_launch_fill(float* out, int64_t n, float v, int num_sms, cudaStream_t s);
@@ -205,7 +205,7 @@ int b2_launch_shap_interactions(const float* X, int64_t row0, int64_t rows, int 
                                 const B2PathInfo* paths, int p_begin, int p_end, const uint32_t* cat_table, int K,
                                 const double* bias_k, const float* base_margin, float base_value, double* gacc, float* out,
                                 int num_sms, cudaStream_t s);
-int b2_launch_leaf_index(const float* X, int64_t row0, int64_t rows, int F, float missing, const B2TreeNodeDev* nodes,
+int b2_launch_leaf_index(B2RawRows src, int64_t row0, int64_t rows, int F, float missing, const B2TreeNodeDev* nodes,
                          const int32_t* tree_offset, const uint32_t* cat_table, int tree_begin, int tree_end, float* out,
                          int num_sms, cudaStream_t s);
 
@@ -246,6 +246,12 @@ int b2_sketch_column(const uint32_t* keys_in, const int32_t* wq_in, uint32_t* ke
                      float* uval, long long* rmin, int32_t* m_scratch, long long* n_valid_scratch, int max_bin,
                      float* cut_out, int32_t* n_cut_out, float* min_out, int32_t* has_missing_out, int num_sms,
                      cudaStream_t s);
+size_t b2_sketch_batch_temp_bytes(int64_t n);
+int b2_sketch_batch(const uint64_t* keys_in, const int32_t* wq_in, uint64_t* keys_sorted, int32_t* wq_sorted, long long* wpre,
+                    int64_t n_sort, const int64_t* seg, const int64_t* h_seg, int f0, int nf, const uint8_t* is_cat, int world,
+                    int rank, long long n_global, void* temp, size_t temp_bytes, int32_t* flags, int32_t* idx, float* uval,
+                    long long* rmin, int max_bin, float* cuts, int32_t* n_cuts, float* mins, int32_t* has_missing, int num_sms,
+                    cudaStream_t s);
 int b2_launch_bin(const float* X, int64_t n, int F, float missing, const int32_t* cut_ptrs, const float* cut_vals,
                   const int32_t* feat_byte, const uint8_t* is_cat, int row_stride, uint8_t* bins, uint8_t* bins_col,
                   int64_t col_stride, int num_sms, cudaStream_t s);
@@ -263,8 +269,15 @@ int b2_launch_csr_densify(const int64_t* indptr, const int32_t* indices, const f
 // out [n][F] = the dense bins of a CSR-layout matrix (absent entries: the missing sentinel)
 int b2_launch_csr_bins_densify(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, int64_t n, int F,
                                uint8_t* out, int num_sms, cudaStream_t s);
-int b2_launch_csr_extract_keys(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int f0, int nf,
-                               float missing, uint32_t* keys, int64_t n_padded, int num_sms, cudaStream_t s);
+// counts [F] (zeroed) += valid stored entries per numeric feature; keys / wq_out of features [f0, f0 + nf) at cursor [nf]
+int b2_launch_csr_column_counts(const int32_t* indices, const float* values, int64_t nnz, float missing, const uint8_t* is_cat,
+                                unsigned long long* counts, int num_sms, cudaStream_t s);
+int b2_launch_csr_sketch_keys(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int f0, int nf,
+                              float missing, const uint8_t* is_cat, const int32_t* wq, unsigned int* cursor, uint64_t* keys,
+                              int32_t* wq_out, int num_sms, cudaStream_t s);
+// stats as b2_launch_cat_stats, from the stored entries of an n-row matrix (stored: n_cat scratch)
+int b2_launch_csr_cat_stats(const int32_t* indices, const float* values, int64_t nnz, int64_t n, float missing, const int32_t* cat_of,
+                            int n_cat, unsigned long long* stored, int32_t* stats, int num_sms, cudaStream_t s);
 
 // slice_kernel.cu (B2_MatrixSlice: rows[0..n) of a parent matrix, in that order, duplicates allowed; every row index is
 // in range, checked by the caller)
@@ -280,7 +293,7 @@ int b2_launch_csr_slice_entries(const int64_t* indptr, const int32_t* indices, c
                                 cudaStream_t s);
 
 // refresh_kernel.cu
-int b2_launch_refresh(const float* X, int64_t n, int F, float missing, const B2TreeNodeDev* nodes, int n_nodes,
+int b2_launch_refresh(B2RawRows src, int64_t n, int F, float missing, const B2TreeNodeDev* nodes, int n_nodes,
                       const uint32_t* cat_table, int n_leaves, const float2* gh, const int32_t* qexp, int leaf_bits,
                       uint16_t* pos, long long* sums, int num_sms, cudaStream_t stream);
 int b2_launch_refresh_nodes(const B2TreeNodeDev* nodes, int n_nodes, const int32_t* order, const int32_t* level_ptr, int n_levels,

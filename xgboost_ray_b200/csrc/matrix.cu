@@ -193,6 +193,12 @@ const float* raw_rows(Matrix* m, int64_t r0, int64_t rows, DevBuf<float>& tile) 
   return tile.p;
 }
 
+B2RawRows raw_source(const Matrix* m) {
+  if (!m->has_raw) fail("matrix has no raw data on the device");
+  if (m->csr) return B2RawRows{nullptr, m->csr_indptr.p, m->csr_indices.p, m->csr_values.p};
+  return B2RawRows{m->raw.p, nullptr, nullptr, nullptr};
+}
+
 // Uploads the CSR arrays of m (n rows, F columns and nnz set) and checks them on the device in one pass; the first row
 // that breaks a rule is named, with the rule read back from the caller's arrays.  The check guards the C ABI: an
 // out-of-range column would be written outside a densified tile.
@@ -304,16 +310,6 @@ size_t matrix_device_bytes(const Matrix* m) {
          buf_bytes(m->qgroup_ptr) + buf_bytes(m->d_fwq);
 }
 
-// sketch keys [kExtractBatch][n_pad] of features [f0, f0 + nf) (missing values and padding rows: 0xffffffff)
-static void extract_keys(Matrix* m, int f0, int nf, uint32_t* keys, int64_t n_pad) {
-  Ctx* ctx = m->ctx;
-  if (m->csr)
-    LAUNCH_CHECK(b2_launch_csr_extract_keys(m->csr_indptr.p, m->csr_indices.p, m->csr_values.p, m->n, f0, nf, m->missing, keys,
-                                            n_pad, ctx->num_sms, ctx->stream));
-  else
-    LAUNCH_CHECK(b2_launch_extract_keys(m->raw.p, m->n, m->F, f0, nf, m->missing, keys, n_pad, ctx->num_sms, ctx->stream));
-}
-
 void upload_cuts(Matrix* m) {
   cudaStream_t s = m->ctx->stream;
   m->nbins.resize(m->F);
@@ -339,6 +335,19 @@ std::vector<int32_t> category_stats(Matrix* m, Comm* comm) {
   d_cat.ensure((size_t)n_cat * 3); d_catf.ensure((size_t)n_cat);
   CUDA_CHECK(cudaMemcpyAsync(d_cat.p, h_cat.data(), (size_t)n_cat * 3 * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   CUDA_CHECK(cudaMemcpyAsync(d_catf.p, m->cat_feats.data(), (size_t)n_cat * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  if (m->csr) {   // one pass over the stored entries; a feature some row does not store has a missing value
+    if (!m->has_raw) fail("matrix has no raw data on the device");
+    std::vector<int32_t> cat_of(m->F, -1);
+    for (int i = 0; i < n_cat; ++i) cat_of[m->cat_feats[i]] = i;
+    DevBuf<int32_t> d_cat_of; DevBuf<unsigned long long> d_stored;
+    upload(d_cat_of, cat_of, s); d_stored.ensure((size_t)n_cat);
+    LAUNCH_CHECK(b2_launch_csr_cat_stats(m->csr_indices.p, m->csr_values.p, m->nnz, m->n, m->missing, d_cat_of.p, n_cat, d_stored.p,
+                                         d_cat.p, m->ctx->num_sms, s));
+    allreduce(comm, d_cat.p, (size_t)n_cat * 3, kNcclInt32, kNcclMax, s);
+    CUDA_CHECK(cudaMemcpyAsync(h_cat.data(), d_cat.p, (size_t)n_cat * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));
+    return h_cat;
+  }
   for_raw_tiles(m, [&](const float* X, int64_t, int64_t rows) {   // the stats are maxima: they accumulate over the tiles
     LAUNCH_CHECK(b2_launch_cat_stats(X, rows, m->F, m->missing, d_catf.p, n_cat, d_cat.p, m->ctx->num_sms, s));
   });
@@ -380,15 +389,162 @@ static void check_borrowed_categories(Matrix* m, Comm* comm) {
   }
 }
 
-// GPU sketch: exact global summary per feature -> cuts (sketch.cu).  No host round trip per feature.
-// Multi-GPU: the column keys of every rank are allgathered (padded to the largest shard); feature f is
-// sorted and pruned only by its owner rank f % world, and the cut tables are merged with one integer
-// allreduce (non-owners contribute zeros), so every rank ends up with identical global cuts.
+// Sketch of a CSR matrix's numeric features from its stored entries only (DESIGN.md 7 "Sketch over the stored entries").
+// A feature's valid keys are the keys the dense twin's sort puts ahead of its missing sentinels, in the same order, so
+// the summaries and cuts are the twin's.  Features are taken in batches of at most kSketchBatchEntries valid entries
+// (summed over the ranks; a feature with more is a batch of its own).  Per batch each rank keys its entries into their
+// feature's segment; with several ranks the blocks are allgathered, padded to the largest rank's block with sentinels
+// that sort last.  Every rank sorts the batch, the owner rank of a feature (f % world) prunes it into the table.
+constexpr int64_t kSketchBatchEntries = (int64_t)1 << 24;   // tests/test_gpu_sparse_native.py BATCH_ENTRIES
+static void sketch_csr(Matrix* m, Comm* comm, int max_bin, long long n_global, const int32_t* wq, float* d_cuts, int32_t* d_ncuts,
+                       float* d_mins, int32_t* d_hasmiss) {
+  Ctx* ctx = m->ctx; cudaStream_t s = ctx->stream;
+  const int world = comm ? comm->world : 1, rank = comm ? comm->rank : 0, F = m->F;
+  DevBuf<uint8_t> d_iscat; upload(d_iscat, m->is_cat, s);
+  // valid entries per feature of every rank: [world][F]
+  DevBuf<unsigned long long> d_counts;
+  d_counts.ensure((size_t)world * F);
+  unsigned long long* mine = d_counts.p + (size_t)rank * F;
+  CUDA_CHECK(cudaMemsetAsync(mine, 0, (size_t)F * sizeof(unsigned long long), s));
+  LAUNCH_CHECK(b2_launch_csr_column_counts(m->csr_indices.p, m->csr_values.p, m->nnz, m->missing, d_iscat.p, mine, ctx->num_sms, s));
+  if (world > 1) NCCL_CHECK(nccl()->AllGather(mine, d_counts.p, (size_t)F, kNcclUint64, comm->comm, s));
+  std::vector<unsigned long long> cnt((size_t)world * F);
+  CUDA_CHECK(cudaMemcpyAsync(cnt.data(), d_counts.p, cnt.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  std::vector<int64_t> total(F, 0);
+  for (int r = 0; r < world; ++r)
+    for (int f = 0; f < F; ++f) total[f] += (int64_t)cnt[(size_t)r * F + f];
+  // batches [f0, f1): the same on every rank (planned from the global counts)
+  std::vector<std::pair<int, int>> batches;
+  int64_t max_local = 1, max_sort = 1;
+  for (int f0 = 0; f0 < F;) {
+    int f1 = f0; int64_t e = 0;
+    while (f1 < F && (f1 == f0 || e + total[f1] <= kSketchBatchEntries)) e += total[f1++];
+    int64_t emax = 0;
+    for (int r = 0; r < world; ++r) {
+      int64_t er = 0;
+      for (int f = f0; f < f1; ++f) er += (int64_t)cnt[(size_t)r * F + f];
+      emax = std::max(emax, er);
+    }
+    if (e >= ((int64_t)1 << 31)) fail("sketch: %lld valid entries in features [%d, %d) exceed the int32 summary index", (long long)e, f0, f1);
+    max_local = std::max(max_local, emax);
+    max_sort = std::max(max_sort, world > 1 ? emax * world : e);
+    batches.push_back({f0, f1});
+    f0 = f1;
+  }
+  // scratch: peak bytes = max_sort * (8 + 8 + 4 + 4 + 4 + 8 [+ 4 + 4 + 8 weighted]) + CUB + world > 1: the local block
+  DevBuf<uint64_t> keys_local, keys_all, keys_sorted; DevBuf<int32_t> wq_local, wq_all, wq_sorted, flags, idx;
+  DevBuf<float> uval; DevBuf<long long> rmin, wpre; DevBuf<int64_t> d_seg; DevBuf<unsigned int> d_cursor; DevBuf<uint8_t> temp;
+  keys_local.ensure((size_t)max_local);
+  if (world > 1) keys_all.ensure((size_t)max_sort);
+  keys_sorted.ensure((size_t)max_sort); flags.ensure((size_t)max_sort); idx.ensure((size_t)max_sort); uval.ensure((size_t)max_sort);
+  rmin.ensure((size_t)max_sort);
+  if (wq) {
+    wq_local.ensure((size_t)max_local); wq_sorted.ensure((size_t)max_sort); wpre.ensure((size_t)max_sort);
+    if (world > 1) wq_all.ensure((size_t)max_sort);
+  }
+  const size_t temp_bytes = b2_sketch_batch_temp_bytes(max_sort);
+  temp.ensure(temp_bytes ? temp_bytes : 1);
+  d_seg.ensure((size_t)F + 1); d_cursor.ensure((size_t)F);
+  for (const auto& bt : batches) {
+    const int f0 = bt.first, nf = bt.second - f0;
+    std::vector<int64_t> seg(nf + 1, 0);
+    std::vector<unsigned int> cursor(nf, 0);
+    int64_t local = 0, emax = 0;
+    for (int j = 0; j < nf; ++j) {
+      seg[j + 1] = seg[j] + total[f0 + j];
+      cursor[j] = (unsigned int)local;
+      local += (int64_t)cnt[(size_t)rank * F + f0 + j];
+    }
+    for (int r = 0; r < world; ++r) {
+      int64_t er = 0;
+      for (int j = 0; j < nf; ++j) er += (int64_t)cnt[(size_t)r * F + f0 + j];
+      emax = std::max(emax, er);
+    }
+    // the local block is in feature-segment order; with several ranks the sort regroups the gathered blocks, whose
+    // per-feature order the global segments in seg describe
+    upload(d_seg, seg, s); upload(d_cursor, cursor, s);
+    LAUNCH_CHECK(b2_launch_csr_sketch_keys(m->csr_indptr.p, m->csr_indices.p, m->csr_values.p, m->n, f0, nf, m->missing, d_iscat.p,
+                                           wq, d_cursor.p, keys_local.p, wq ? wq_local.p : nullptr, ctx->num_sms, s));
+    const uint64_t* kin = keys_local.p; const int32_t* win = wq ? wq_local.p : nullptr;
+    int64_t n_sort = local;
+    if (world > 1) {
+      if (emax > local) {
+        CUDA_CHECK(cudaMemsetAsync(keys_local.p + local, 0xff, (size_t)(emax - local) * sizeof(uint64_t), s));
+        if (wq) CUDA_CHECK(cudaMemsetAsync(wq_local.p + local, 0, (size_t)(emax - local) * sizeof(int32_t), s));
+      }
+      if (emax > 0) {
+        NCCL_CHECK(nccl()->AllGather(keys_local.p, keys_all.p, (size_t)emax, kNcclUint64, comm->comm, s));
+        if (wq) NCCL_CHECK(nccl()->AllGather(wq_local.p, wq_all.p, (size_t)emax, kNcclInt32, comm->comm, s));
+      }
+      kin = keys_all.p; win = wq ? wq_all.p : nullptr; n_sort = emax * world;
+    }
+    LAUNCH_CHECK(b2_sketch_batch(kin, win, keys_sorted.p, wq_sorted.p, wpre.p, n_sort, d_seg.p, seg.data(), f0, nf, d_iscat.p, world,
+                                 rank, n_global, temp.p, temp_bytes, flags.p, idx.p, uval.p, rmin.p, max_bin, d_cuts, d_ncuts, d_mins,
+                                 d_hasmiss, ctx->num_sms, s));
+    CUDA_CHECK(cudaStreamSynchronize(s));   // seg and cursor are host vectors of this iteration
+  }
+}
+
+// Sketch of a dense matrix's numeric features: the keys of kExtractBatch columns per pass, every column of n_pad keys
+// per rank (padding rows and missing values are the 0xffffffff sentinel).  Multi-GPU: the column keys and the integer
+// weights of every rank are allgathered (padded to the largest shard); feature f is sorted and pruned only by its owner
+// rank f % world.
+static void sketch_dense(Matrix* m, Comm* comm, int max_bin, int64_t n_pad, long long n_global, const int32_t* wq_local,
+                         float* d_cuts, int32_t* d_ncuts, float* d_mins, int32_t* d_hasmiss) {
+  Ctx* ctx = m->ctx; cudaStream_t s = ctx->stream;
+  const int world = comm ? comm->world : 1, rank = comm ? comm->rank : 0;
+  const int64_t n_total = n_pad * world;
+  const int B = b2_extract_batch(); const int F = m->F;
+  DevBuf<uint32_t> keys_local, keys_all, keys_sorted;
+  DevBuf<int32_t> flags, idx, m_scratch, wq_all, wq_sorted; DevBuf<float> uval; DevBuf<long long> rmin, nvalid, wpre;
+  DevBuf<uint8_t> temp;
+  const size_t nt = (size_t)std::max<int64_t>(n_total, 1);
+  keys_local.ensure((size_t)std::max<int64_t>(n_pad, 1) * B);
+  if (world > 1) keys_all.ensure(nt);
+  keys_sorted.ensure(nt); flags.ensure(nt); idx.ensure(nt); uval.ensure(nt); rmin.ensure(nt); m_scratch.ensure(1); nvalid.ensure(2);
+  const int32_t* wq = wq_local;
+  if (wq_local) {
+    if (world > 1) {
+      wq_all.ensure(nt);
+      NCCL_CHECK(nccl()->AllGather(wq_local, wq_all.p, (size_t)n_pad, kNcclInt32, comm->comm, s));
+      wq = wq_all.p;
+    }
+    wq_sorted.ensure(nt); wpre.ensure(nt);
+  }
+  const size_t temp_bytes = b2_sort_temp_bytes(n_total > 0 ? n_total : 1);
+  temp.ensure(temp_bytes ? temp_bytes : 1);
+  for (int f0 = 0; f0 < F; f0 += B) {
+    const int nf = std::min(B, F - f0);
+    bool any_numeric = false;
+    for (int j = 0; j < nf; ++j) any_numeric = any_numeric || !m->is_cat[f0 + j];
+    if (!any_numeric) continue;
+    LAUNCH_CHECK(b2_launch_extract_keys(m->raw.p, m->n, m->F, f0, nf, m->missing, keys_local.p, n_pad, ctx->num_sms, s));
+    for (int j = 0; j < nf; ++j) {
+      const int f = f0 + j;
+      if (m->is_cat[f]) continue;   // categorical: cuts are the codes 0..max (make_cuts)
+      const uint32_t* kin = keys_local.p + (size_t)j * n_pad;
+      if (world > 1) {
+        NCCL_CHECK(nccl()->AllGather(kin, keys_all.p, (size_t)n_pad, kNcclUint32, comm->comm, s));
+        kin = keys_all.p;
+        if (f % world != rank) continue;   // the owner rank sketches this feature
+      }
+      LAUNCH_CHECK(b2_sketch_column(kin, wq, keys_sorted.p, wq_sorted.p, wpre.p, n_total, n_global, temp.p, temp_bytes, flags.p, idx.p, uval.p, rmin.p,
+                                    m_scratch.p, nvalid.p, max_bin, d_cuts + (size_t)f * 256, d_ncuts + f, d_mins + f,
+                                    d_hasmiss + f, ctx->num_sms, s));
+    }
+  }
+  CUDA_CHECK(cudaStreamSynchronize(s));   // the scratch buffers are freed on return
+}
+
+// GPU sketch: exact global summary per feature -> cuts (sketch.cu).  No host round trip per feature.  Each feature is
+// sketched by one owner rank (sketch_dense, sketch_csr), and the cut tables are merged with one integer allreduce
+// (non-owners contribute zeros), so every rank ends up with identical global cuts.
 static void make_cuts(Matrix* m, Comm* comm, int max_bin) {
   Ctx* ctx = m->ctx; cudaStream_t s = ctx->stream;
   if (max_bin < 2 || max_bin > 256) fail("max_bin must be in [2, 256] (uint8 bin matrix), got %d", max_bin);
   if (!m->has_raw) fail("matrix has no raw data to sketch");
-  const int world = comm ? comm->world : 1, rank = comm ? comm->rank : 0;
+  const int world = comm ? comm->world : 1;
   // largest shard and global row count
   DevBuf<long long> d_cnt; d_cnt.ensure(2);
   long long h_cnt[2] = {m->n, m->n};
@@ -399,19 +555,12 @@ static void make_cuts(Matrix* m, Comm* comm, int max_bin) {
     CUDA_CHECK(cudaMemcpyAsync(h_cnt, d_cnt.p, sizeof(h_cnt), cudaMemcpyDeviceToHost, s));
     CUDA_CHECK(cudaStreamSynchronize(s));
   }
-  const int64_t n_pad = h_cnt[0], n_total = n_pad * world; const long long n_global = h_cnt[1];
-  const int B = b2_extract_batch(); const int F = m->F;
-  DevBuf<uint32_t> keys_local, keys_all, keys_sorted;
-  DevBuf<int32_t> flags, idx, m_scratch; DevBuf<float> uval; DevBuf<long long> rmin, nvalid;
+  const int64_t n_pad = h_cnt[0]; const long long n_global = h_cnt[1];
+  const int F = m->F;
   DevBuf<int32_t> d_tab;   // [F*256 cut bits][F n_cuts][F min bits][F has_missing]
-  DevBuf<uint8_t> temp;
-  const size_t nt = (size_t)std::max<int64_t>(n_total, 1);
-  keys_local.ensure((size_t)std::max<int64_t>(n_pad, 1) * B);
-  if (world > 1) keys_all.ensure(nt);
-  keys_sorted.ensure(nt); flags.ensure(nt); idx.ensure(nt); uval.ensure(nt); rmin.ensure(nt); m_scratch.ensure(1); nvalid.ensure(2);
   // sample weights make the sketch a weighted one (xgboost SketchContainer pushes info.weights_): quantise them to
   // integers with a global power-of-two scale so that the weighted ranks are exact and identical on every rank
-  DevBuf<int32_t> wq_local, wq_all, wq_sorted; DevBuf<long long> wpre; DevBuf<uint32_t> d_wmax;
+  DevBuf<int32_t> wq_local; DevBuf<uint32_t> d_wmax;
   const int32_t* wq = nullptr;
   {
     long long h_has[1] = {m->n_weight > 0 ? 1 : 0};
@@ -434,42 +583,16 @@ static void make_cuts(Matrix* m, Comm* comm, int max_bin) {
       wq_local.ensure((size_t)std::max<int64_t>(n_pad, 1));
       LAUNCH_CHECK(b2_launch_weight_quantize(m->weight.p, m->n, n_pad, d_wmax.p, wq_local.p, ctx->num_sms, s));
       wq = wq_local.p;
-      if (world > 1) {
-        wq_all.ensure(nt);
-        NCCL_CHECK(nccl()->AllGather(wq_local.p, wq_all.p, (size_t)n_pad, kNcclInt32, comm->comm, s));
-        wq = wq_all.p;
-      }
-      wq_sorted.ensure(nt); wpre.ensure(nt);
     }
   }
-  const size_t temp_bytes = b2_sort_temp_bytes(n_total > 0 ? n_total : 1);
-  temp.ensure(temp_bytes ? temp_bytes : 1);
   const size_t tab_n = (size_t)F * 256 + 3 * (size_t)F;
   d_tab.ensure(tab_n);
   CUDA_CHECK(cudaMemsetAsync(d_tab.p, 0, tab_n * sizeof(int32_t), s));
   float* d_cuts = (float*)d_tab.p; int32_t* d_ncuts = d_tab.p + (size_t)F * 256;
   float* d_mins = (float*)(d_ncuts + F); int32_t* d_hasmiss = d_ncuts + 2 * (size_t)F;
   if (m->is_cat.empty()) m->is_cat.assign(F, 0);
-  for (int f0 = 0; f0 < F; f0 += B) {
-    const int nf = std::min(B, F - f0);
-    bool any_numeric = false;
-    for (int j = 0; j < nf; ++j) any_numeric = any_numeric || !m->is_cat[f0 + j];
-    if (!any_numeric) continue;
-    extract_keys(m, f0, nf, keys_local.p, n_pad);
-    for (int j = 0; j < nf; ++j) {
-      const int f = f0 + j;
-      if (m->is_cat[f]) continue;   // categorical: cuts are the codes 0..max (below)
-      const uint32_t* kin = keys_local.p + (size_t)j * n_pad;
-      if (world > 1) {
-        NCCL_CHECK(nccl()->AllGather(kin, keys_all.p, (size_t)n_pad, kNcclUint32, comm->comm, s));
-        kin = keys_all.p;
-        if (f % world != rank) continue;   // the owner rank sketches this feature
-      }
-      LAUNCH_CHECK(b2_sketch_column(kin, wq, keys_sorted.p, wq_sorted.p, wpre.p, n_total, n_global, temp.p, temp_bytes, flags.p, idx.p, uval.p, rmin.p,
-                                    m_scratch.p, nvalid.p, max_bin, d_cuts + (size_t)f * 256, d_ncuts + f, d_mins + f,
-                                    d_hasmiss + f, ctx->num_sms, s));
-    }
-  }
+  if (m->csr) sketch_csr(m, comm, max_bin, n_global, wq, d_cuts, d_ncuts, d_mins, d_hasmiss);
+  else sketch_dense(m, comm, max_bin, n_pad, n_global, wq, d_cuts, d_ncuts, d_mins, d_hasmiss);
   // merge the per-owner tables: exact because every entry is written by exactly one rank (others hold 0 bits)
   allreduce(comm, d_tab.p, tab_n, kNcclInt32, kNcclSum, s);
   std::vector<int32_t> h_tab(tab_n);

@@ -659,12 +659,14 @@ __global__ void label_check_kernel(int objective, int K, const float* __restrict
 // concatenated; tree_offset[t] is the first node of tree t; tree t adds to class (t / npt) % K (xgboost lays the
 // num_parallel_tree trees of a class out next to each other, GBTree::BoostNewTrees).  weights (DART, nullable): tree t
 // adds fl(weights[t] * leaf), a separate multiply and add like dart_margins_kernel.
-__global__ void predict_kernel(const float* __restrict__ X, int64_t n, int F, float missing, int missing_is_nan,
+// Rows: B2DenseRows or B2CsrRows (common.cuh), where row i's raw values are read.
+template <typename Rows>
+__global__ void predict_kernel(Rows rows, int64_t n, int F, float missing, int missing_is_nan,
                                const B2TreeNodeDev* __restrict__ nodes, const int32_t* __restrict__ tree_offset,
                                const uint32_t* __restrict__ cat_table, int tree_begin, int tree_end, int K, int npt,
                                const float* __restrict__ weights, float* __restrict__ out) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const float* x = X + i * F;
+    const auto x = b2_row(rows, i, F);
     for (int t = tree_begin; t < tree_end; ++t) {
       float v;
       b2_tree_leaf(nodes + tree_offset[t], x, missing, missing_is_nan, cat_table, &v);
@@ -676,12 +678,13 @@ __global__ void predict_kernel(const float* __restrict__ X, int64_t n, int F, fl
 
 // vector-leaf trees: each tree adds the leaf vector of the leaf the row reaches (leaf_vec [node][T], the model's nodes
 // in tree order) to the row's T margins, tree by tree as the train margin receives them
-__global__ void predict_vector_kernel(const float* __restrict__ X, int64_t n, int F, float missing, int missing_is_nan,
+template <typename Rows>
+__global__ void predict_vector_kernel(Rows rows, int64_t n, int F, float missing, int missing_is_nan,
                                       const B2TreeNodeDev* __restrict__ nodes, const int32_t* __restrict__ tree_offset,
                                       const float* __restrict__ leaf_vec, int tree_begin, int tree_end, int T,
                                       float* __restrict__ out) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const float* x = X + i * F;
+    const auto x = b2_row(rows, i, F);
     float* o = out + i * T;
     for (int t = tree_begin; t < tree_end; ++t) {
       float unused;
@@ -848,19 +851,30 @@ int b2_launch_metric(int objective, int metric, int K, float metric_param, const
   b2::metric_kernel<<<g, 256, 0, s>>>(objective, metric, K, metric_param, margin, label, weight, n, partial, out);
   return b2_launch_metric_sum(partial, g, out, s);
 }
-int b2_launch_predict(const float* X, int64_t n, int F, float missing, const B2TreeNodeDev* nodes,
+int b2_launch_predict(B2RawRows src, int64_t n, int F, float missing, const B2TreeNodeDev* nodes,
                       const int32_t* tree_offset, const uint32_t* cat_table, int tree_begin, int tree_end, int K, int npt,
                       const float* weights, float* out, int num_sms, cudaStream_t s) {
   if (n <= 0 || tree_end <= tree_begin) return 0;
-  b2::predict_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(X, n, F, missing, missing != missing ? 1 : 0, nodes, tree_offset,
-                                                         cat_table, tree_begin, tree_end, K, npt < 1 ? 1 : npt, weights, out);
+  const int g = grid_for(n, num_sms), mnan = missing != missing ? 1 : 0;
+  if (npt < 1) npt = 1;
+  if (src.indptr)
+    b2::predict_kernel<<<g, 256, 0, s>>>(B2CsrRows{src.indptr, src.indices, src.values}, n, F, missing, mnan, nodes, tree_offset,
+                                         cat_table, tree_begin, tree_end, K, npt, weights, out);
+  else
+    b2::predict_kernel<B2DenseRows><<<g, 256, 0, s>>>(src.X, n, F, missing, mnan, nodes, tree_offset, cat_table, tree_begin,
+                                         tree_end, K, npt, weights, out);
   return (int)cudaGetLastError();
 }
-int b2_launch_predict_vector(const float* X, int64_t n, int F, float missing, const B2TreeNodeDev* nodes, const int32_t* tree_offset,
+int b2_launch_predict_vector(B2RawRows src, int64_t n, int F, float missing, const B2TreeNodeDev* nodes, const int32_t* tree_offset,
                              const float* leaf_vec, int tree_begin, int tree_end, int T, float* out, int num_sms, cudaStream_t s) {
   if (n <= 0 || tree_end <= tree_begin) return 0;
-  b2::predict_vector_kernel<<<grid_for(n, num_sms), 256, 0, s>>>(X, n, F, missing, missing != missing ? 1 : 0, nodes, tree_offset,
-                                                                 leaf_vec, tree_begin, tree_end, T, out);
+  const int g = grid_for(n, num_sms), mnan = missing != missing ? 1 : 0;
+  if (src.indptr)
+    b2::predict_vector_kernel<<<g, 256, 0, s>>>(B2CsrRows{src.indptr, src.indices, src.values}, n, F, missing, mnan, nodes,
+                                                tree_offset, leaf_vec, tree_begin, tree_end, T, out);
+  else
+    b2::predict_vector_kernel<B2DenseRows><<<g, 256, 0, s>>>(src.X, n, F, missing, mnan, nodes, tree_offset, leaf_vec, tree_begin,
+                                                tree_end, T, out);
   return (int)cudaGetLastError();
 }
 int b2_launch_fill(float* out, int64_t n, float v, int num_sms, cudaStream_t s) {

@@ -111,16 +111,13 @@ const float* device_weights(Booster* b) {
 void predict_trees(Booster* b, Matrix* m, int tree_begin, int tree_end, float* out) {
   sync_device_trees(b);
   const float* w = b->p.vector_leaf() ? nullptr : device_weights(b);
-  for_raw_tiles(m, [&](const float* X, int64_t r0, int64_t rows) {
-    if (b->p.vector_leaf())
-      LAUNCH_CHECK(b2_launch_predict_vector(X, rows, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_leaf_table.p,
-                                            tree_begin, tree_end, b->p.num_target, out + (size_t)r0 * b->p.num_target,
-                                            b->ctx->num_sms, b->ctx->stream));
-    else
-      LAUNCH_CHECK(b2_launch_predict(X, rows, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, tree_begin,
-                                     tree_end, b->p.num_class, b->p.num_parallel_tree, w, out + (size_t)r0 * b->p.num_class,
-                                     b->ctx->num_sms, b->ctx->stream));
-  });
+  const B2RawRows src = raw_source(m);
+  if (b->p.vector_leaf())
+    LAUNCH_CHECK(b2_launch_predict_vector(src, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_leaf_table.p,
+                                          tree_begin, tree_end, b->p.num_target, out, b->ctx->num_sms, b->ctx->stream));
+  else
+    LAUNCH_CHECK(b2_launch_predict(src, m->n, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, tree_begin,
+                                   tree_end, b->p.num_class, b->p.num_parallel_tree, w, out, b->ctx->num_sms, b->ctx->stream));
 }
 
 // margin of matrix m under the current model (cached per matrix, only new trees are applied)
@@ -358,13 +355,16 @@ void predict_leaf(Booster* b, Matrix* m, int tree_begin, int tree_end, float* ou
   if (out_len != m->n * T) fail("output buffer has %lld values, expected %lld", (long long)out_len, (long long)(m->n * T));
   if (T == 0 || m->n == 0) return;
   sync_device_trees(b);
+  // row blocks stage the output; the rows are read in place
   const int64_t blk = rows_per_block(m, (size_t)T * sizeof(float));
   DevBuf<float> d_out; d_out.ensure((size_t)blk * T);
-  for_raw_tiles(m, [&](const float* X, int64_t r0, int64_t rows) {
-    LAUNCH_CHECK(b2_launch_leaf_index(X, 0, rows, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p,
+  const B2RawRows src = raw_source(m);
+  for (int64_t r0 = 0; r0 < m->n; r0 += blk) {
+    const int64_t rows = std::min(blk, m->n - r0);
+    LAUNCH_CHECK(b2_launch_leaf_index(src, r0, rows, m->F, m->missing, b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p,
                                       tree_begin, tree_end, d_out.p, b->ctx->num_sms, s));
     CUDA_CHECK(cudaMemcpyAsync(out + (size_t)r0 * T, d_out.p, (size_t)rows * T * sizeof(float), cudaMemcpyDeviceToHost, s));
-  }, blk);
+  }
   CUDA_CHECK(cudaStreamSynchronize(s));
 }
 

@@ -33,9 +33,9 @@ __device__ __forceinline__ void refresh_add64(uint32_t* lo, uint32_t* hi, long l
 // by the caller).  kSmemNodes: the nodes are copied into shared memory; kSmemAcc: each CTA sums its rows in shared
 // memory and adds one total per leaf, else every row adds to the global limbs with 64-bit atomics.  A tree is a full
 // binary tree (n_nodes = 2 n_leaves - 1, checked by the host), so nodes that fit in shared memory imply leaves that do.
-template <bool kSmemNodes, bool kSmemAcc>
+template <bool kSmemNodes, bool kSmemAcc, typename Rows>
 __global__ void __launch_bounds__(kRefreshThreads)
-refresh_kernel(const float* __restrict__ X, int64_t n, int F, float missing, int missing_is_nan,
+refresh_kernel(Rows rows, int64_t n, int F, float missing, int missing_is_nan,
                const B2TreeNodeDev* __restrict__ nodes, int n_nodes, const uint32_t* __restrict__ cat_table, int n_leaves,
                const float2* __restrict__ gh, const int32_t* __restrict__ qexp, int leaf_bits,
                uint16_t* __restrict__ pos, long long* __restrict__ sums) {
@@ -52,9 +52,9 @@ refresh_kernel(const float* __restrict__ X, int64_t n, int F, float missing, int
   uint32_t *glo = s_acc, *ghi = s_acc + n_leaves, *hlo = s_acc + 2 * n_leaves, *hhi = s_acc + 3 * n_leaves;
   const double kg = ldexp(1.0, leaf_bits - qexp[0]), kh = ldexp(1.0, leaf_bits - qexp[1]);
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const float* x = X + i * F;
+    const auto x = b2_row(rows, i, F);
     B2TreeNodeDev nd = tn[0];
-    while (nd.feature >= 0) nd = tn[b2_tree_step(nd, __ldg(x + nd.feature), missing, missing_is_nan, cat_table)];
+    while (nd.feature >= 0) nd = tn[b2_tree_step(nd, b2_ldg_value(x, nd.feature), missing, missing_is_nan, cat_table)];
     const int leaf = nd.pad;
     pos[i] = (uint16_t)leaf;
     const float2 v = __ldg(gh + i);
@@ -134,7 +134,7 @@ refresh_nodes_kernel(const B2TreeNodeDev* __restrict__ nodes, int n_nodes, const
 }  // namespace b2
 
 extern "C" {
-int b2_launch_refresh(const float* X, int64_t n, int F, float missing, const B2TreeNodeDev* nodes, int n_nodes,
+int b2_launch_refresh(B2RawRows src, int64_t n, int F, float missing, const B2TreeNodeDev* nodes, int n_nodes,
                       const uint32_t* cat_table, int n_leaves, const float2* gh, const int32_t* qexp, int leaf_bits,
                       uint16_t* pos, long long* sums, int num_sms, cudaStream_t stream) {
   if (n <= 0) return 0;
@@ -147,19 +147,25 @@ int b2_launch_refresh(const float* X, int64_t n, int F, float missing, const B2T
   if (cap < exact_min) cap = exact_min;
   const int grid = (int)(want < cap ? want : cap);
   const int missing_is_nan = isnan(missing) ? 1 : 0;
-#define B2_REFRESH_LAUNCH(N, A)                                                                                         \
+#define B2_REFRESH_LAUNCH(N, A, R, ROWS)                                                                                \
   do {                                                                                                                  \
-    auto k = b2::refresh_kernel<N, A>;                                                                                  \
+    auto k = b2::refresh_kernel<N, A, R>;                                                                               \
     if (smem > 48 * 1024) {                                                                                             \
       const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);           \
       if (e != cudaSuccess) return (int)e;                                                                              \
     }                                                                                                                   \
-    k<<<grid, b2::kRefreshThreads, smem, stream>>>(X, n, F, missing, missing_is_nan, nodes, n_nodes, cat_table, n_leaves, \
-                                                   gh, qexp, leaf_bits, pos, sums);                                     \
+    k<<<grid, b2::kRefreshThreads, smem, stream>>>(ROWS, n, F, missing, missing_is_nan, nodes, n_nodes, cat_table,        \
+                                                   n_leaves, gh, qexp, leaf_bits, pos, sums);                           \
   } while (0)
-  if (smem_nodes) B2_REFRESH_LAUNCH(true, true);
-  else if (smem_acc) B2_REFRESH_LAUNCH(false, true);
-  else B2_REFRESH_LAUNCH(false, false);
+#define B2_REFRESH_ROWS(R, ROWS)                                       \
+  do {                                                                 \
+    if (smem_nodes) B2_REFRESH_LAUNCH(true, true, R, ROWS);            \
+    else if (smem_acc) B2_REFRESH_LAUNCH(false, true, R, ROWS);        \
+    else B2_REFRESH_LAUNCH(false, false, R, ROWS);                     \
+  } while (0)
+  if (src.indptr) B2_REFRESH_ROWS(B2CsrRows, (B2CsrRows{src.indptr, src.indices, src.values}));
+  else B2_REFRESH_ROWS(B2DenseRows, src.X);
+#undef B2_REFRESH_ROWS
 #undef B2_REFRESH_LAUNCH
   return (int)cudaGetLastError();
 }

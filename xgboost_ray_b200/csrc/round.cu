@@ -606,11 +606,8 @@ void refresh_tree(Booster* b, int k, int slot, int src) {
   const B2TreeNodeDev* nodes = b->d_rnodes.p + rt.node_off;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   if (p.profile) { e0 = get_event(b); e1 = get_event(b); CUDA_CHECK(cudaEventRecord(e0, s)); }
-  // the leaf sums are exact fixed-point atomics: they accumulate over the raw tiles in any order
-  for_raw_tiles(m, [&](const float* X, int64_t r0, int64_t rows) {
-    LAUNCH_CHECK(b2_launch_refresh(X, rows, m->F, m->missing, nodes, rt.n_nodes, b->d_rcats.p, rt.n_leaves, gh + r0, b->d_qexp.p,
-                                   40, b->pos.p + r0, b->d_rsums.p, ctx->num_sms, s));
-  });
+  LAUNCH_CHECK(b2_launch_refresh(raw_source(m), n, m->F, m->missing, nodes, rt.n_nodes, b->d_rcats.p, rt.n_leaves, gh, b->d_qexp.p,
+                                 40, b->pos.p, b->d_rsums.p, ctx->num_sms, s));
   if (p.profile) { CUDA_CHECK(cudaEventRecord(e1, s)); R.refresh_events.push_back({e0, e1}); }
   b->t.refresh_launches++;
   allreduce(b->comm, b->d_rsums.p, 4 * (size_t)rt.n_leaves, kNcclInt64, kNcclSum, s);   // limb by limb: exact

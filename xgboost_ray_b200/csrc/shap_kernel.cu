@@ -256,7 +256,8 @@ __global__ void __launch_bounds__(256) shap_interactions_kernel(
 }
 
 // pred_leaf: out [rows][tree_end - tree_begin] = node id of the leaf the row reaches (b2_tree_leaf, as predict_kernel)
-__global__ void leaf_index_kernel(const float* __restrict__ X, int64_t row0, int64_t rows, int F, float missing, int missing_is_nan,
+template <typename Rows>
+__global__ void leaf_index_kernel(Rows src, int64_t row0, int64_t rows, int F, float missing, int missing_is_nan,
                                   const B2TreeNodeDev* __restrict__ nodes, const int32_t* __restrict__ tree_offset,
                                   const uint32_t* __restrict__ cat_table, int tree_begin, int tree_end, float* __restrict__ out) {
   const int T = tree_end - tree_begin;
@@ -264,7 +265,7 @@ __global__ void leaf_index_kernel(const float* __restrict__ X, int64_t row0, int
     const int64_t r = i / T;
     const int t = tree_begin + (int)(i - r * T);
     float v;
-    out[i] = (float)b2_tree_leaf(nodes + tree_offset[t], X + (row0 + r) * F, missing, missing_is_nan, cat_table, &v);
+    out[i] = (float)b2_tree_leaf(nodes + tree_offset[t], b2_row(src, row0 + r, F), missing, missing_is_nan, cat_table, &v);
   }
 }
 
@@ -305,15 +306,20 @@ int b2_launch_shap_interactions(const float* X, int64_t row0, int64_t rows, int 
   return (int)cudaGetLastError();
 }
 
-int b2_launch_leaf_index(const float* X, int64_t row0, int64_t rows, int F, float missing, const B2TreeNodeDev* nodes,
+int b2_launch_leaf_index(B2RawRows src, int64_t row0, int64_t rows, int F, float missing, const B2TreeNodeDev* nodes,
                          const int32_t* tree_offset, const uint32_t* cat_table, int tree_begin, int tree_end, float* out,
                          int num_sms, cudaStream_t s) {
   if (rows <= 0 || tree_end <= tree_begin) return 0;
   int64_t g = (rows * (tree_end - tree_begin) + 255) / 256;
   const int64_t cap = (int64_t)num_sms * 16;
   if (g > cap) g = cap;
-  b2::leaf_index_kernel<<<(int)g, 256, 0, s>>>(X, row0, rows, F, missing, missing != missing ? 1 : 0, nodes, tree_offset, cat_table,
-                                               tree_begin, tree_end, out);
+  const int mnan = missing != missing ? 1 : 0;
+  if (src.indptr)
+    b2::leaf_index_kernel<<<(int)g, 256, 0, s>>>(B2CsrRows{src.indptr, src.indices, src.values}, row0, rows, F, missing, mnan, nodes,
+                                                 tree_offset, cat_table, tree_begin, tree_end, out);
+  else
+    b2::leaf_index_kernel<B2DenseRows><<<(int)g, 256, 0, s>>>(src.X, row0, rows, F, missing, mnan, nodes, tree_offset, cat_table,
+                                                 tree_begin, tree_end, out);
   return (int)cudaGetLastError();
 }
 }

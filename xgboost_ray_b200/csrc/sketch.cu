@@ -44,9 +44,12 @@ __global__ void count_valid_kernel(const uint32_t* __restrict__ sorted, int64_t 
   *n_valid = lo;
 }
 
-__global__ void head_flags_kernel(const uint32_t* __restrict__ keys, int64_t n_total, int32_t* __restrict__ flags) {
+// Key: uint32_t (one feature's keys, the all-ones sentinel = missing) or uint64_t (a batch's (feature << 32) | key,
+// where a new feature starts a new run)
+template <typename Key>
+__global__ void head_flags_kernel(const Key* __restrict__ keys, int64_t n_total, int32_t* __restrict__ flags) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_total; i += (int64_t)gridDim.x * blockDim.x)
-    flags[i] = (keys[i] != 0xffffffffu && (i == 0 || keys[i] != keys[i - 1])) ? 1 : 0;
+    flags[i] = (keys[i] != ~(Key)0 && (i == 0 || keys[i] != keys[i - 1])) ? 1 : 0;
 }
 __global__ void scatter_unique_kernel(const uint32_t* __restrict__ keys, const int32_t* __restrict__ flags,
                                       const int32_t* __restrict__ idx, int64_t n_total, float* __restrict__ uval,
@@ -92,21 +95,36 @@ __global__ void scatter_unique_weighted_kernel(const uint32_t* __restrict__ keys
   if (n_valid == 0 && blockIdx.x == 0 && threadIdx.x == 0) *w_total = 0;
 }
 
-// One block.  WQSummary::SetPrune + HistogramCuts::AddCutPoint on the exact summary (A.2).
-// w_total_ptr != nullptr: rmin holds weighted ranks and *w_total_ptr the total weight (the last rmax).
-__global__ void __launch_bounds__(256)
-prune_cuts_kernel(const float* __restrict__ uval, const long long* __restrict__ rmin, const int32_t* __restrict__ m_ptr,
-                  const long long* __restrict__ n_valid_ptr, const long long* __restrict__ w_total_ptr, long long n_global, int max_bin,
-                  float* __restrict__ cut_out /*[256]*/,
-                  int32_t* __restrict__ n_cut_out, float* __restrict__ min_out, int32_t* __restrict__ has_missing_out) {
+// A batch of features sorted as (feature << 32) | key, feature j's entries at [seg[j], seg[j+1]) (only valid keys): the
+// summary entry of every distinct value, its rank relative to its feature's first entry -- the position, or with integer
+// weights the prefix wpre of the weights -- exactly what scatter_unique(_weighted)_kernel computes for the feature alone.
+__global__ void scatter_unique_segments_kernel(const uint64_t* __restrict__ keys, const int32_t* __restrict__ flags,
+                                               const int32_t* __restrict__ idx, const long long* __restrict__ wpre,
+                                               const int64_t* __restrict__ seg, int64_t n_total, float* __restrict__ uval,
+                                               long long* __restrict__ rmin) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_total; i += (int64_t)gridDim.x * blockDim.x) {
+    if (!flags[i]) continue;
+    const uint64_t k = keys[i];
+    const int64_t s = seg[k >> 32];
+    uval[idx[i]] = key2f((uint32_t)k);
+    rmin[idx[i]] = wpre ? wpre[i] - wpre[s] : i - s;
+  }
+}
+
+// WQSummary::SetPrune + HistogramCuts::AddCutPoint on the exact summary of one feature (A.2), by one whole block:
+// get_m() distinct values uval / rmin, n_valid non-missing values of n_global rows, rank_end the total rank (the last
+// rmax: n_valid, or the total weight).
+template <typename MFn>
+__device__ __forceinline__ void prune_cuts(const float* __restrict__ uval, const long long* __restrict__ rmin, MFn get_m,
+                                           long long n_valid, long long rank_end, long long n_global, int max_bin,
+                                           float* __restrict__ cut_out /*[256]*/, int32_t* __restrict__ n_cut_out,
+                                           float* __restrict__ min_out, int32_t* __restrict__ has_missing_out) {
   __shared__ int sel[260];
   __shared__ int choice[260];
-  const long long n_valid = *n_valid_ptr;
-  const long long rank_end = w_total_ptr ? *w_total_ptr : n_valid;
   const bool any_missing = n_valid < n_global;
   const int max_bin_cap = (any_missing && max_bin > 255) ? 255 : max_bin;   // bin 255 is the missing sentinel
   if (threadIdx.x == 0) *has_missing_out = any_missing ? 1 : 0;
-  const int m = n_valid > 0 ? *m_ptr : 0;
+  const int m = n_valid > 0 ? get_m() : 0;
   if (m == 0) {
     if (threadIdx.x == 0) {
       float mval = 0.0f;
@@ -181,23 +199,45 @@ prune_cuts_kernel(const float* __restrict__ uval, const long long* __restrict__ 
   for (int i = threadIdx.x; i < s_nc; i += blockDim.x) cut_out[i] = scut[i];
 }
 
-// Categorical columns (HistogramCuts::AddCategories, src/common/quantile.cc): the cuts are the codes 0..max, so
-// the only statistics needed are the largest code, whether a value is missing and which values are not valid
-// codes.  stats [n_cat][3] int32 = {max code (init -1), has_missing, largest invalid value (init INT_MIN) as the
-// signed order-preserving key f2key(x) ^ 0x80000000, so the error can name it}; merged with an allreduce(max).
+// One block, the summary of b2_sketch_column.  w_total_ptr != nullptr: rmin holds weighted ranks and *w_total_ptr the
+// total weight.
+__global__ void __launch_bounds__(256)
+prune_cuts_kernel(const float* __restrict__ uval, const long long* __restrict__ rmin, const int32_t* __restrict__ m_ptr,
+                  const long long* __restrict__ n_valid_ptr, const long long* __restrict__ w_total_ptr, long long n_global, int max_bin,
+                  float* __restrict__ cut_out /*[256]*/,
+                  int32_t* __restrict__ n_cut_out, float* __restrict__ min_out, int32_t* __restrict__ has_missing_out) {
+  const long long n_valid = *n_valid_ptr;
+  const long long rank_end = w_total_ptr ? *w_total_ptr : n_valid;
+  prune_cuts(uval, rmin, [&] { return *m_ptr; }, n_valid, rank_end, n_global, max_bin, cut_out, n_cut_out, min_out,
+             has_missing_out);
+}
+
+// One block per feature of a batch (scatter_unique_segments_kernel's layout): feature f0 + j's summary is the slice of
+// the batch's that starts at its first entry.  Only the owner rank (f % world) prunes; categorical features are skipped.
+// Outputs are indexed by the global feature id.
+__global__ void __launch_bounds__(256)
+prune_cuts_segments_kernel(const float* __restrict__ uval, const long long* __restrict__ rmin, const int32_t* __restrict__ flags,
+                           const int32_t* __restrict__ idx, const long long* __restrict__ wpre, const int32_t* __restrict__ wq_sorted,
+                           const int64_t* __restrict__ seg, int f0, const uint8_t* __restrict__ is_cat, int world, int rank,
+                           long long n_global, int max_bin, float* __restrict__ cuts /*[F][256]*/, int32_t* __restrict__ n_cuts,
+                           float* __restrict__ mins, int32_t* __restrict__ has_missing) {
+  const int f = f0 + blockIdx.x;
+  if ((is_cat && is_cat[f]) || f % world != rank) return;
+  const int64_t s = seg[blockIdx.x], e = seg[blockIdx.x + 1];
+  const long long n_valid = e - s;
+  const int64_t u0 = n_valid > 0 ? idx[s] : 0;
+  const long long rank_end = !wpre ? n_valid : (n_valid > 0 ? wpre[e - 1] + wq_sorted[e - 1] - wpre[s] : 0);
+  prune_cuts(uval + u0, rmin + u0, [&] { return idx[e - 1] + flags[e - 1] - (int)u0; }, n_valid, rank_end, n_global, max_bin,
+             cuts + (size_t)f * 256, n_cuts + f, mins + f, has_missing + f);
+}
+
+// Categorical columns: the statistics of cat_stats_update (raw_keys.cuh), one thread per cell.
 __global__ void cat_stats_kernel(const float* __restrict__ X, int64_t n, int F, float missing, int missing_is_nan,
                                  const int32_t* __restrict__ cat_feats, int n_cat, int32_t* __restrict__ stats) {
   const int64_t total = n * n_cat;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
     const int64_t row = e / n_cat; const int ci = (int)(e - row * n_cat);
-    const float x = X[row * F + cat_feats[ci]];
-    if (is_missing(x, missing, missing_is_nan)) { if (stats[ci * 3 + 1] == 0) atomicMax(&stats[ci * 3 + 1], 1); continue; }
-    if (!(x >= 0.0f) || x > 255.0f || x != (float)(int)x) {
-      atomicMax(&stats[ci * 3 + 2], (int32_t)(f2key(x) ^ 0x80000000u));
-      continue;
-    }
-    const int c = (int)x;
-    if (stats[ci * 3] < c) atomicMax(&stats[ci * 3], c);
+    cat_stats_update(X[row * F + cat_feats[ci]], missing, missing_is_nan, stats, ci);
   }
 }
 
@@ -368,7 +408,7 @@ int b2_sketch_column(const uint32_t* keys_in, const int32_t* wq_in, uint32_t* ke
     if (wq_in) e = cub::DeviceRadixSort::SortPairs(temp, temp_bytes, keys_in, keys_sorted, wq_in, wq_sorted, n_total, 0, 32, s);
     else e = cub::DeviceRadixSort::SortKeys(temp, temp_bytes, keys_in, keys_sorted, n_total, 0, 32, s);
     if (e != cudaSuccess) return (int)e;
-    b2::head_flags_kernel<<<sk_grid(n_total, num_sms), 256, 0, s>>>(keys_sorted, n_total, flags);
+    b2::head_flags_kernel<uint32_t><<<sk_grid(n_total, num_sms), 256, 0, s>>>(keys_sorted, n_total, flags);
     e = cub::DeviceScan::ExclusiveSum(temp, temp_bytes, flags, idx, n_total, s);
     if (e != cudaSuccess) return (int)e;
   }
@@ -387,6 +427,54 @@ int b2_sketch_column(const uint32_t* keys_in, const int32_t* wq_in, uint32_t* ke
   }
   b2::prune_cuts_kernel<<<1, 256, 0, s>>>(uval, rmin, m_scratch, n_valid_scratch, (wq_in && n_total > 0) ? n_valid_scratch + 1 : nullptr,
                                          n_global, max_bin, cut_out, n_cut_out, min_out, has_missing_out);
+  return (int)cudaGetLastError();
+}
+
+size_t b2_sketch_batch_temp_bytes(int64_t n) {
+  size_t bytes = 0, b2 = 0;
+  cub::DeviceRadixSort::SortKeys(nullptr, bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr, n);
+  cub::DeviceRadixSort::SortPairs(nullptr, b2, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const int32_t*)nullptr,
+                                  (int32_t*)nullptr, n);
+  bytes = bytes > b2 ? bytes : b2;
+  cub::DeviceScan::ExclusiveSum(nullptr, b2, (const int32_t*)nullptr, (int32_t*)nullptr, n);
+  bytes = bytes > b2 ? bytes : b2;
+  cub::TransformInputIterator<long long, b2::CastI64, const int32_t*> it((const int32_t*)nullptr, b2::CastI64());
+  cub::DeviceScan::ExclusiveSum(nullptr, b2, it, (long long*)nullptr, n);
+  return bytes > b2 ? bytes : b2;
+}
+
+// Cuts of features [f0, f0 + nf) from their stored entries: keys_in [n_sort] = (j << 32) | sketch key of every valid
+// entry of feature f0 + j (any order; all-ones sentinels allowed after them, they sort last), wq_in (nullable) the
+// entries' integer weights.  seg [nf + 1]: feature j's entries are [seg[j], seg[j+1]) of the sorted keys, seg[nf] of
+// them valid.  One sort, one summary pass over the batch and one prune block per feature.  Scratch: keys_sorted,
+// wq_sorted, flags, idx, uval, rmin, wpre [n_sort].
+int b2_sketch_batch(const uint64_t* keys_in, const int32_t* wq_in, uint64_t* keys_sorted, int32_t* wq_sorted, long long* wpre,
+                    int64_t n_sort, const int64_t* seg, const int64_t* h_seg, int f0, int nf, const uint8_t* is_cat, int world,
+                    int rank, long long n_global, void* temp, size_t temp_bytes, int32_t* flags, int32_t* idx, float* uval,
+                    long long* rmin, int max_bin, float* cuts, int32_t* n_cuts, float* mins, int32_t* has_missing, int num_sms,
+                    cudaStream_t s) {
+  if (nf <= 0) return 0;
+  const int64_t n_valid = h_seg[nf];
+  int end_bit = 32;
+  while (end_bit < 64 && ((int64_t)1 << (end_bit - 32)) <= nf) ++end_bit;   // the feature bits of (nf - 1) and the sentinel
+  cudaError_t e;
+  if (n_valid > 0) {
+    if (wq_in) e = cub::DeviceRadixSort::SortPairs(temp, temp_bytes, keys_in, keys_sorted, wq_in, wq_sorted, n_sort, 0, end_bit, s);
+    else e = cub::DeviceRadixSort::SortKeys(temp, temp_bytes, keys_in, keys_sorted, n_sort, 0, end_bit, s);
+    if (e != cudaSuccess) return (int)e;
+    b2::head_flags_kernel<uint64_t><<<sk_grid(n_valid, num_sms), 256, 0, s>>>(keys_sorted, n_valid, flags);
+    e = cub::DeviceScan::ExclusiveSum(temp, temp_bytes, flags, idx, n_valid, s);
+    if (e != cudaSuccess) return (int)e;
+    if (wq_in) {
+      cub::TransformInputIterator<long long, b2::CastI64, const int32_t*> it(wq_sorted, b2::CastI64());
+      e = cub::DeviceScan::ExclusiveSum(temp, temp_bytes, it, wpre, n_valid, s);
+      if (e != cudaSuccess) return (int)e;
+    }
+    b2::scatter_unique_segments_kernel<<<sk_grid(n_valid, num_sms), 256, 0, s>>>(keys_sorted, flags, idx, wq_in ? wpre : nullptr,
+                                                                               seg, n_valid, uval, rmin);
+  }
+  b2::prune_cuts_segments_kernel<<<nf, 256, 0, s>>>(uval, rmin, flags, idx, wq_in ? wpre : nullptr, wq_sorted, seg, f0, is_cat, world,
+                                                   rank, n_global, max_bin, cuts, n_cuts, mins, has_missing);
   return (int)cudaGetLastError();
 }
 

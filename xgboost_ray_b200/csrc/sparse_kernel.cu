@@ -1,5 +1,6 @@
 // sparse_kernel.cu -- the raw values of a CSR matrix (B2_MatrixCreateFromCSR): validation of the three arrays, dense
-// row tiles for the kernels that read raw rows, and the sketch keys of a batch of features read straight from the CSR.
+// row tiles for the kernels that read raw rows, and the sketch's entry keys and categorical statistics read straight
+// from the stored entries.
 //
 // An entry a row does not store is missing.  A stored entry is copied bit for bit, so every kernel that reads a tile
 // sees exactly the floats of the matrix's dense twin (the same matrix with NaN in every absent cell).
@@ -61,24 +62,58 @@ csr_densify_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict
   }
 }
 
-// keys [kExtractBatch][n_padded] of features [f0, f0 + nf), the layout of extract_keys_kernel (sketch.cu); the caller
-// sets every key to the missing sentinel 0xffffffff first.  One thread per row: a binary search finds the row's first
-// column >= f0, then the row's entries in the window are keyed.
+// counts [F] += the valid stored entries (not missing) of every numeric feature: the sizes of the sketch's segments
 __global__ void __launch_bounds__(kSparseThreads)
-csr_extract_keys_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, const float* __restrict__ values,
-                        int64_t n, int f0, int nf, float missing, int missing_is_nan, uint32_t* __restrict__ keys,
-                        int64_t n_padded) {
+csr_column_counts_kernel(const int32_t* __restrict__ indices, const float* __restrict__ values, int64_t nnz, float missing,
+                         int missing_is_nan, const uint8_t* __restrict__ is_cat, unsigned long long* __restrict__ counts) {
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += (int64_t)gridDim.x * blockDim.x) {
+    const int f = __ldg(indices + e);
+    if (!is_missing(__ldg(values + e), missing, missing_is_nan) && !(is_cat && is_cat[f])) atomicAdd(counts + f, 1ull);
+  }
+}
+
+// The sketch keys of features [f0, f0 + nf): every valid entry of a numeric feature f0 + j becomes (j << 32) | its
+// sketch key, at the next free slot of feature j's segment (cursor [nf], started at the segment starts), with its row's
+// integer weight when wq != nullptr.  The order inside a segment does not matter: the segments are sorted next.  One
+// thread per row: a binary search finds the row's first column >= f0, then its entries in the window are keyed.
+__global__ void __launch_bounds__(kSparseThreads)
+csr_sketch_keys_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, const float* __restrict__ values,
+                       int64_t n, int f0, int nf, float missing, int missing_is_nan, const uint8_t* __restrict__ is_cat,
+                       const int32_t* __restrict__ wq, unsigned int* __restrict__ cursor, uint64_t* __restrict__ keys,
+                       int32_t* __restrict__ wq_out) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t end = indptr[i + 1];
     int64_t lo = indptr[i], hi = end;
     while (lo < hi) { const int64_t mid = (lo + hi) >> 1; if (__ldg(indices + mid) < f0) lo = mid + 1; else hi = mid; }
     for (int64_t e = lo; e < end; ++e) {
-      const int j = __ldg(indices + e) - f0;
+      const int f = __ldg(indices + e), j = f - f0;
       if (j >= nf) break;
       const float x = __ldg(values + e);
-      if (!is_missing(x, missing, missing_is_nan)) keys[(int64_t)j * n_padded + i] = sketch_key(x);
+      if (is_missing(x, missing, missing_is_nan) || (is_cat && is_cat[f])) continue;
+      const unsigned int p = atomicAdd(cursor + j, 1u);
+      keys[p] = ((uint64_t)j << 32) | sketch_key(x);
+      if (wq) wq_out[p] = wq[i];
     }
   }
+}
+
+// Categorical statistics (cat_stats_update) from the stored entries, one thread per entry; cat_of [F] = the feature's
+// index among the categorical features, or -1.  stored [n_cat] counts the entries, so that a feature some row does not
+// store is marked missing by csr_cat_absent_kernel.
+__global__ void __launch_bounds__(kSparseThreads)
+csr_cat_stats_kernel(const int32_t* __restrict__ indices, const float* __restrict__ values, int64_t nnz, float missing,
+                     int missing_is_nan, const int32_t* __restrict__ cat_of, unsigned long long* __restrict__ stored,
+                     int32_t* __restrict__ stats) {
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += (int64_t)gridDim.x * blockDim.x) {
+    const int ci = cat_of[__ldg(indices + e)];
+    if (ci < 0) continue;
+    atomicAdd(stored + ci, 1ull);
+    cat_stats_update(__ldg(values + e), missing, missing_is_nan, stats, ci);
+  }
+}
+__global__ void csr_cat_absent_kernel(const unsigned long long* __restrict__ stored, int n_cat, int64_t n, int32_t* __restrict__ stats) {
+  for (int ci = blockIdx.x * blockDim.x + threadIdx.x; ci < n_cat; ci += gridDim.x * blockDim.x)
+    if ((int64_t)stored[ci] < n) stats[ci * 3 + 1] = 1;
 }
 
 // out [n][F] = the dense bins of a CSR-layout matrix: the sentinel in every cell, then each row's stored bins (one
@@ -130,13 +165,31 @@ int b2_launch_csr_densify(const int64_t* indptr, const int32_t* indices, const f
   return (int)cudaGetLastError();
 }
 
-int b2_launch_csr_extract_keys(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int f0, int nf,
-                               float missing, uint32_t* keys, int64_t n_padded, int num_sms, cudaStream_t s) {
-  if (n_padded <= 0) return 0;
-  cudaError_t e = cudaMemsetAsync(keys, 0xff, (size_t)nf * n_padded * sizeof(uint32_t), s);
-  if (e != cudaSuccess || n <= 0) return (int)e;
-  b2::csr_extract_keys_kernel<<<sparse_grid(n, num_sms), b2::kSparseThreads, 0, s>>>(indptr, indices, values, n, f0, nf, missing,
-                                                                                   missing != missing ? 1 : 0, keys, n_padded);
+int b2_launch_csr_column_counts(const int32_t* indices, const float* values, int64_t nnz, float missing, const uint8_t* is_cat,
+                                unsigned long long* counts, int num_sms, cudaStream_t s) {
+  if (nnz <= 0) return 0;
+  b2::csr_column_counts_kernel<<<sparse_grid(nnz, num_sms), b2::kSparseThreads, 0, s>>>(indices, values, nnz, missing,
+                                                                                      missing != missing ? 1 : 0, is_cat, counts);
+  return (int)cudaGetLastError();
+}
+int b2_launch_csr_sketch_keys(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int f0, int nf,
+                              float missing, const uint8_t* is_cat, const int32_t* wq, unsigned int* cursor, uint64_t* keys,
+                              int32_t* wq_out, int num_sms, cudaStream_t s) {
+  if (n <= 0 || nf <= 0) return 0;
+  b2::csr_sketch_keys_kernel<<<sparse_grid(n, num_sms), b2::kSparseThreads, 0, s>>>(indptr, indices, values, n, f0, nf, missing,
+                                                                                  missing != missing ? 1 : 0, is_cat, wq, cursor,
+                                                                                  keys, wq_out);
+  return (int)cudaGetLastError();
+}
+int b2_launch_csr_cat_stats(const int32_t* indices, const float* values, int64_t nnz, int64_t n, float missing, const int32_t* cat_of,
+                            int n_cat, unsigned long long* stored, int32_t* stats, int num_sms, cudaStream_t s) {
+  if (n_cat <= 0) return 0;
+  cudaError_t e = cudaMemsetAsync(stored, 0, (size_t)n_cat * sizeof(unsigned long long), s);
+  if (e != cudaSuccess) return (int)e;
+  if (nnz > 0)
+    b2::csr_cat_stats_kernel<<<sparse_grid(nnz, num_sms), b2::kSparseThreads, 0, s>>>(indices, values, nnz, missing,
+                                                                                    missing != missing ? 1 : 0, cat_of, stored, stats);
+  b2::csr_cat_absent_kernel<<<1, 256, 0, s>>>(stored, n_cat, n, stats);
   return (int)cudaGetLastError();
 }
 

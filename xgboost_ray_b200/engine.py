@@ -442,7 +442,7 @@ class DMatrix:
                                                     C.byref(h)))
             self.handle = h.value
         elif isinstance(self._host, CSRArrays):
-            # the device keeps the CSR: absent entries are missing, kernels read densified tiles of it
+            # the device keeps the CSR: absent entries are missing; the sketch and the tree walks read its stored entries
             c = self._host
             _check(lib().B2_MatrixCreateFromCSR(c.indptr.ctypes.data_as(_LP), _ip(c.indices), _fp(c.values), n, f, c.nnz,
                                                 self.missing, self.device, C.byref(h)))
