@@ -230,6 +230,14 @@ __device__ __forceinline__ float b2_ldg_value(const float* x, int f) { return __
 __device__ __forceinline__ float b2_ldg_value(const B2CsrRow& x, int f) { return x[f]; }
 // a matrix's raw values as the walk launchers take them: the CSR arrays when indptr != nullptr, else X [n][F]
 struct B2RawRows { const float* X; const int64_t* indptr; const int32_t* indices; const float* values; };
+// a quantised matrix's bins as the split-side launchers (histogram, partition, final assign, DART) take them: the CSR
+// layout -- ebins [nnz] located by indptr / indices -- when ebins != nullptr, else the dense bins [n][row_stride] and
+// their feature-major copy bins_col [F][col_stride].  feat_byte [F] (the byte of feature f in a dense row) for both.
+struct B2BinRows {
+  const uint8_t* bins; int row_stride; const int32_t* feat_byte;
+  const uint8_t* bins_col; int64_t col_stride;
+  const int64_t* indptr; const int32_t* indices; const uint8_t* ebins;
+};
 
 // ---- device-resident control tables of the sync-free level loop (control_kernel.cu)
 struct B2LevelCtl {

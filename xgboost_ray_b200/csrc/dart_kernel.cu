@@ -109,16 +109,22 @@ dart_margins_csr_kernel(const int64_t* __restrict__ indptr, const int32_t* __res
 extern "C" {
 // drop / full hold the starting margins (base_score or base_margin) on entry.  dropped[t] != 0: tree t is left out of
 // drop.  drop == nullptr rebuilds the full margin only (w_drop / dropped unused).
-int b2_launch_dart_margins(const uint8_t* bins, int64_t n, int row_stride, const int32_t* feat_byte, const uint8_t* has_missing,
-                           const B2TreeNodeDev* nodes, const int32_t* tree_offset, const uint32_t* cat_table, int T, int K,
-                           int npt, const float* w_drop, const uint8_t* dropped, const float* w_full, float* drop, float* full,
-                           int num_sms, cudaStream_t s) {
+int b2_launch_dart_margins(B2BinRows src, int64_t n, const uint8_t* has_missing, const B2TreeNodeDev* nodes,
+                           const int32_t* tree_offset, const uint32_t* cat_table, int T, int K, int npt, const float* w_drop,
+                           const uint8_t* dropped, const float* w_full, float* drop, float* full, int num_sms, cudaStream_t s) {
   if (n <= 0 || T <= 0) return 0;
-  if (row_stride <= 0 || (row_stride & 31)) return (int)cudaErrorInvalidValue;
   if (npt < 1) npt = 1;
   const int64_t tiles = (n + b2::kDartRows - 1) / b2::kDartRows;
   const int64_t cap = (int64_t)num_sms * 16;
   const int grid = (int)(tiles < cap ? tiles : cap);
+  if (src.ebins) {
+    b2::dart_margins_csr_kernel<<<grid, b2::kDartRows, 0, s>>>(src.indptr, src.indices, src.ebins, n, has_missing, nodes,
+                                                              tree_offset, cat_table, T, K, npt, w_drop, dropped, w_full, drop,
+                                                              full);
+    return (int)cudaGetLastError();
+  }
+  const uint8_t* bins = src.bins; const int row_stride = src.row_stride; const int32_t* feat_byte = src.feat_byte;
+  if (row_stride <= 0 || (row_stride & 31)) return (int)cudaErrorInvalidValue;
   const size_t smem = (size_t)b2::kDartRows * (size_t)(row_stride / 4 + 1) * 4;
   const bool single = K == 1;
 #define B2_DART_LAUNCH(SMEM, SINGLE, BYTES)                                                                                  \
@@ -136,17 +142,6 @@ int b2_launch_dart_margins(const uint8_t* bins, int64_t n, int row_stride, const
     else B2_DART_LAUNCH(false, false, 0);
   }
 #undef B2_DART_LAUNCH
-  return (int)cudaGetLastError();
-}
-int b2_launch_dart_margins_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, int64_t n,
-                               const uint8_t* has_missing, const B2TreeNodeDev* nodes, const int32_t* tree_offset,
-                               const uint32_t* cat_table, int T, int K, int npt, const float* w_drop, const uint8_t* dropped,
-                               const float* w_full, float* drop, float* full, int num_sms, cudaStream_t s) {
-  if (n <= 0 || T <= 0) return 0;
-  if (npt < 1) npt = 1;
-  const int64_t tiles = (n + b2::kDartRows - 1) / b2::kDartRows, cap = (int64_t)num_sms * 16;
-  b2::dart_margins_csr_kernel<<<(int)(tiles < cap ? tiles : cap), b2::kDartRows, 0, s>>>(
-      indptr, indices, ebins, n, has_missing, nodes, tree_offset, cat_table, T, K, npt, w_drop, dropped, w_full, drop, full);
   return (int)cudaGetLastError();
 }
 }

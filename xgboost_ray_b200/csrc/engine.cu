@@ -5,6 +5,7 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <climits>
 #include <string>
 #include <vector>
 
@@ -352,12 +353,6 @@ int B2_MatrixEnsureRawCSR(B2Handle mh, int64_t* indptr, const int32_t* indices, 
   Matrix* m = matrix_of(mh);
   if (m->has_raw) return 0;
   if (!m->csr) fail("the matrix was created from dense rows: re-upload them with B2_MatrixEnsureRaw");
-  if (m->csr_bins) {   // indptr and indices stayed on the device with the bins: only the values come back
-    m->csr_values.ensure((size_t)m->nnz);
-    upload_pipelined(m->ctx, m->csr_values.p, values, (size_t)m->nnz * sizeof(float));
-    m->has_raw = true;
-    return 0;
-  }
   upload_csr(m, indptr, indices, values);
   API_END
 }
@@ -401,20 +396,7 @@ int B2_MatrixSetBinLayout(B2Handle mh, int32_t layout) {
 }
 int B2_MatrixGetBins(B2Handle mh, uint8_t* out) {
   API_BEGIN
-  Matrix* m = matrix_of(mh);
-  if (!m->quantized) fail("matrix is not quantised");
-  if (m->csr_bins) {
-    DevBuf<uint8_t> d; d.ensure((size_t)std::max<int64_t>(m->n * m->F, 1));
-    LAUNCH_CHECK(b2_launch_csr_bins_densify(m->csr_indptr.p, m->csr_indices.p, m->ebins.p, m->n, m->F, d.p, m->ctx->num_sms,
-                                            m->ctx->stream));
-    CUDA_CHECK(cudaMemcpyAsync(out, d.p, (size_t)m->n * m->F, cudaMemcpyDeviceToHost, m->ctx->stream));
-    CUDA_CHECK(cudaStreamSynchronize(m->ctx->stream));
-    return 0;
-  }
-  std::vector<uint8_t> h((size_t)m->n * m->row_stride);
-  if (m->n > 0) CUDA_CHECK(cudaMemcpy(h.data(), m->bins.p, h.size(), cudaMemcpyDeviceToHost));
-  for (int64_t i = 0; i < m->n; ++i)
-    for (int f = 0; f < m->F; ++f) out[i * m->F + f] = h[(size_t)i * m->row_stride + m->feat_byte[f]];
+  bins_to_host(matrix_of(mh), out);
   API_END
 }
 int B2_MatrixFree(B2Handle mh) {
@@ -684,50 +666,9 @@ int B2_HistBuildRaw(const uint8_t* bins, int64_t n_rows, int32_t n_cols, const i
                     const int32_t* ridx, int64_t n_sel, int32_t window_rows, int32_t chunk_rows, int device, int64_t* out,
                     float* kernel_ms) {
   API_BEGIN
-  Ctx* ctx = get_ctx(device); cudaStream_t s = ctx->stream;
-  Matrix m; m.kind = kMatrix; m.ctx = ctx; m.n = n_rows; m.F = n_cols;
-  setup_groups(&m);
-  std::vector<uint8_t> padded((size_t)std::max<int64_t>(n_rows, 1) * m.row_stride, 0);
-  for (int64_t i = 0; i < n_rows; ++i)
-    for (int f = 0; f < n_cols; ++f) padded[(size_t)i * m.row_stride + m.feat_byte[f]] = bins[i * n_cols + f];
-  std::vector<int2> gp((size_t)std::max<int64_t>(n_rows, 1));
-  for (int64_t i = 0; i < n_rows; ++i) gp[i] = make_int2(qg[i], qh[i]);
-  DevBuf<uint8_t> d_bins; DevBuf<int2> d_gp; DevBuf<int32_t> d_ridx; DevBuf<long long> d_hist; DevBuf<B2HistWork> d_work;
-  d_bins.ensure(padded.size()); d_gp.ensure(gp.size());
-  CUDA_CHECK(cudaMemcpyAsync(d_bins.p, padded.data(), padded.size(), cudaMemcpyHostToDevice, s));
-  CUDA_CHECK(cudaMemcpyAsync(d_gp.p, gp.data(), gp.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
-  if (ridx) {
-    d_ridx.ensure((size_t)std::max<int64_t>(n_sel, 1));
-    if (n_sel > 0) CUDA_CHECK(cudaMemcpyAsync(d_ridx.p, ridx, n_sel * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-  }
-  const size_t node_elems = (size_t)m.n_groups * B2_GROUP_ELEMS;
-  d_hist.ensure(node_elems);
-  CUDA_CHECK(cudaMemsetAsync(d_hist.p, 0, node_elems * sizeof(long long), s));
-  if (window_rows <= 0) window_rows = 4096;
-  if (chunk_rows <= 0) chunk_rows = 2048;
-  if (chunk_rows > window_rows) chunk_rows = window_rows;
-  B2HistWork w{0, (int32_t)n_sel, 0, 0};
-  d_work.ensure(1);
-  CUDA_CHECK(cudaMemcpyAsync(d_work.p, &w, sizeof(w), cudaMemcpyHostToDevice, s));
-  const int chunks = (int)((n_sel + chunk_rows - 1) / chunk_rows);
-  cudaEvent_t e0, e1; CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
-  CUDA_CHECK(cudaEventRecord(e0, s));
-  if (n_sel > 0)
-    LAUNCH_CHECK(b2_launch_hist(d_bins.p, m.row_stride, d_gp.p, ridx ? d_ridx.p : nullptr, d_work.p, 1, chunks, chunk_rows,
-                                window_rows, m.n_groups, d_hist.p, nullptr, 0, 1, ctx->num_sms, s));
-  CUDA_CHECK(cudaEventRecord(e1, s));
-  std::vector<long long> h(node_elems);
-  CUDA_CHECK(cudaMemcpyAsync(h.data(), d_hist.p, node_elems * sizeof(long long), cudaMemcpyDeviceToHost, s));
-  CUDA_CHECK(cudaStreamSynchronize(s));
-  if (kernel_ms) { float ms = 0; cudaEventElapsedTime(&ms, e0, e1); *kernel_ms = ms; }
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  for (int f = 0; f < n_cols; ++f) {
-    const int g = m.feat_byte[f] / B2_GROUP_SLOTS, sl = m.feat_byte[f] % B2_GROUP_SLOTS;
-    for (int bb = 0; bb < 256; ++bb) {
-      out[((size_t)f * 256 + bb) * 2] = h[(size_t)g * B2_GROUP_ELEMS + bb * 32 + sl];
-      out[((size_t)f * 256 + bb) * 2 + 1] = h[(size_t)g * B2_GROUP_ELEMS + B2_PLANE_ELEMS + bb * 32 + sl];
-    }
-  }
+  Matrix m; m.kind = kMatrix; m.ctx = get_ctx(device); m.n = n_rows; m.F = n_cols;
+  upload_bins(&m, bins);
+  hist_build_raw(&m, qg, qh, ridx, n_sel, window_rows, chunk_rows, out, kernel_ms);
   API_END
 }
 
@@ -735,44 +676,12 @@ int B2_HistBuildRawCSR(int64_t* indptr, const int32_t* indices, const uint8_t* b
                        const int32_t* qg, const int32_t* qh, const int32_t* ridx, int64_t n_sel, int32_t chunk_rows,
                        int device, int64_t* out, float* kernel_ms) {
   API_BEGIN
-  Ctx* ctx = get_ctx(device); cudaStream_t s = ctx->stream;
-  Matrix m; m.kind = kMatrix; m.ctx = ctx; m.n = n_rows; m.F = n_cols; m.nnz = n_rows > 0 ? indptr[n_rows] : 0;
-  setup_groups(&m);
+  Matrix m; m.kind = kMatrix; m.ctx = get_ctx(device); m.n = n_rows; m.F = n_cols;
+  m.csr = true; m.nnz = n_rows > 0 ? indptr[n_rows] : 0;
   const std::vector<float> values((size_t)std::max<int64_t>(m.nnz, 1), 0.0f);   // upload_csr checks indptr and indices
   upload_csr(&m, indptr, indices, values.data());
-  std::vector<int2> gp((size_t)std::max<int64_t>(n_rows, 1));
-  for (int64_t i = 0; i < n_rows; ++i) gp[i] = make_int2(qg[i], qh[i]);
-  DevBuf<uint8_t> d_bins; DevBuf<int2> d_gp; DevBuf<int32_t> d_ridx; DevBuf<long long> d_hist, d_tot; DevBuf<B2HistWork> d_work;
-  upload(d_bins, bins, (size_t)m.nnz, s);
-  upload(d_gp, gp, s); upload(m.d_feat_byte, m.feat_byte, s); upload(m.d_group_size, m.group_size, s);
-  if (ridx) upload(d_ridx, ridx, (size_t)n_sel, s);
-  const size_t node_elems = (size_t)m.n_groups * B2_GROUP_ELEMS;
-  d_hist.ensure(node_elems); d_tot.ensure(2);
-  CUDA_CHECK(cudaMemsetAsync(d_hist.p, 0, node_elems * sizeof(long long), s));
-  CUDA_CHECK(cudaMemsetAsync(d_tot.p, 0, 2 * sizeof(long long), s));
-  if (chunk_rows <= 0) chunk_rows = 2048;
-  B2HistWork w{0, (int32_t)n_sel, 0, 0};
-  upload(d_work, &w, 1, s);
-  const int chunks = (int)((n_sel + chunk_rows - 1) / chunk_rows);
-  cudaEvent_t e0, e1; CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
-  CUDA_CHECK(cudaEventRecord(e0, s));
-  if (n_sel > 0)
-    LAUNCH_CHECK(b2_launch_hist_csr(m.csr_indptr.p, m.csr_indices.p, d_bins.p, m.d_feat_byte.p, m.d_group_size.p, d_gp.p,
-                                    ridx ? d_ridx.p : nullptr, d_work.p, 1, chunks, chunk_rows, m.n_groups, d_hist.p, d_tot.p,
-                                    nullptr, 0, 1, ctx->num_sms, s));
-  CUDA_CHECK(cudaEventRecord(e1, s));
-  std::vector<long long> h(node_elems);
-  CUDA_CHECK(cudaMemcpyAsync(h.data(), d_hist.p, node_elems * sizeof(long long), cudaMemcpyDeviceToHost, s));
-  CUDA_CHECK(cudaStreamSynchronize(s));
-  if (kernel_ms) { float ms = 0; cudaEventElapsedTime(&ms, e0, e1); *kernel_ms = ms; }
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  for (int f = 0; f < n_cols; ++f) {
-    const int g = m.feat_byte[f] / B2_GROUP_SLOTS, sl = m.feat_byte[f] % B2_GROUP_SLOTS;
-    for (int bb = 0; bb < 256; ++bb) {
-      out[((size_t)f * 256 + bb) * 2] = h[(size_t)g * B2_GROUP_ELEMS + bb * 32 + sl];
-      out[((size_t)f * 256 + bb) * 2 + 1] = h[(size_t)g * B2_GROUP_ELEMS + B2_PLANE_ELEMS + bb * 32 + sl];
-    }
-  }
+  upload_bins(&m, bins);
+  hist_build_raw(&m, qg, qh, ridx, n_sel, INT_MAX, chunk_rows, out, kernel_ms);   // the CSR build has no int32 window
   API_END
 }
 

@@ -1,9 +1,14 @@
-// hist_common.cuh -- device helpers of the histogram kernels (hist_kernel.cu): row loads, the conflict-free shared
-// atomics and the flushes to the global int64 histogram.
+// hist_common.cuh -- device helpers of the histogram kernels (hist_kernel.cu, hist_csr_kernel.cu): row loads, the
+// conflict-free shared atomics and the flushes to the global int64 histogram.
 #pragma once
 #include "common.cuh"
 
 namespace b2 {
+
+// b2_launch_hist on the CSR bin layout (hist_csr_kernel.cu); totals: the [node_cap][2] scratch, zeroed here
+int launch_hist_csr(const B2BinRows& src, const int32_t* group_size, const int2* gpair, const int32_t* ridx,
+                    const B2HistWork* work, int n_work, int total_chunks, int chunk_rows, int n_groups, long long* hist,
+                    long long* totals, const B2LevelCtl* ctl, int log2_shards, int node_cap, int num_sms, cudaStream_t stream);
 
 __device__ __forceinline__ uint4 ldg_nc_v4(const void* p) {
   uint4 r;

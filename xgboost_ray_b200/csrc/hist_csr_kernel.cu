@@ -13,7 +13,6 @@
 // The sums are exact integers, so the order of rows, CTAs and GPUs does not matter: the totals are per GPU, and the
 // exchange adds the GPUs' histograms as it adds the dense ones.
 #include "hist_common.cuh"
-#include "launch.h"
 
 namespace b2 {
 
@@ -92,27 +91,24 @@ hist_csr_missing_kernel(const B2HistWork* __restrict__ work, int n_work, const i
   *cell = (unsigned long long)((long long)*cell + (real ? t - rest : t));
 }
 
-}  // namespace b2
-
-extern "C" {
-
-int b2_launch_hist_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, const int32_t* feat_byte,
-                       const int32_t* group_size, const int2* gpair, const int32_t* ridx, const B2HistWork* work, int n_work,
-                       int total_chunks, int chunk_rows, int n_groups, long long* hist, long long* totals,
-                       const B2LevelCtl* ctl, int log2_shards, int node_cap, int num_sms, cudaStream_t stream) {
+int launch_hist_csr(const B2BinRows& src, const int32_t* group_size, const int2* gpair, const int32_t* ridx,
+                    const B2HistWork* work, int n_work, int total_chunks, int chunk_rows, int n_groups, long long* hist,
+                    long long* totals, const B2LevelCtl* ctl, int log2_shards, int node_cap, int num_sms, cudaStream_t stream) {
   if (!ctl && (total_chunks <= 0 || n_work <= 0)) return 0;
+  const cudaError_t e = cudaMemsetAsync(totals, 0, 2 * (size_t)node_cap * sizeof(long long), stream);
+  if (e != cudaSuccess) return (int)e;
   int grid = num_sms * 8;
   if (!ctl && grid > total_chunks) grid = total_chunks;
-  if (ridx) b2::hist_csr_build_kernel<true><<<grid, b2::kCsrHistThreads, 0, stream>>>(
-      indptr, indices, ebins, feat_byte, gpair, ridx, work, n_work, total_chunks, chunk_rows, n_groups, hist, totals, ctl,
-      log2_shards, node_cap);
-  else b2::hist_csr_build_kernel<false><<<grid, b2::kCsrHistThreads, 0, stream>>>(
-      indptr, indices, ebins, feat_byte, gpair, ridx, work, n_work, total_chunks, chunk_rows, n_groups, hist, totals, ctl,
-      log2_shards, node_cap);
+  if (ridx) hist_csr_build_kernel<true><<<grid, kCsrHistThreads, 0, stream>>>(
+      src.indptr, src.indices, src.ebins, src.feat_byte, gpair, ridx, work, n_work, total_chunks, chunk_rows, n_groups, hist,
+      totals, ctl, log2_shards, node_cap);
+  else hist_csr_build_kernel<false><<<grid, kCsrHistThreads, 0, stream>>>(
+      src.indptr, src.indices, src.ebins, src.feat_byte, gpair, ridx, work, n_work, total_chunks, chunk_rows, n_groups, hist,
+      totals, ctl, log2_shards, node_cap);
   const int nodes = ctl ? node_cap : n_work;
-  b2::hist_csr_missing_kernel<<<dim3(n_groups, nodes), 256, 0, stream>>>(work, n_work, group_size, n_groups, hist, totals, ctl,
-                                                                        log2_shards, node_cap);
+  hist_csr_missing_kernel<<<dim3(n_groups, nodes), 256, 0, stream>>>(work, n_work, group_size, n_groups, hist, totals, ctl,
+                                                                     log2_shards, node_cap);
   return (int)cudaGetLastError();
 }
 
-}
+}  // namespace b2

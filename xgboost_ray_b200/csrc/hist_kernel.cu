@@ -221,12 +221,18 @@ __global__ void hist_subtract_kernel(const long long* __restrict__ parent_level,
 
 extern "C" {
 
+// the CSR build's per-node row totals [node_cap][2]; the dense build needs no scratch
+size_t b2_hist_scratch_elems(B2BinRows src, int node_cap) { return src.ebins ? 2 * (size_t)node_cap : 0; }
+
 // Launch on `stream`: a persistent grid of n_types * n_streams group-pair CTAs (n_groups <= kMaxPairGroups) or
 // n_groups * n_streams one-group CTAs; returns the cudaError.
-int b2_launch_hist(const uint8_t* bins, int row_stride, const int2* gpair, const int32_t* ridx,
-                   const B2HistWork* work, int n_work, int total_chunks, int chunk_rows, int window_rows,
-                   int n_groups, long long* hist, const B2LevelCtl* ctl, int log2_shards, int node_cap,
-                   int num_sms, cudaStream_t stream) {
+int b2_launch_hist(B2BinRows src, const int32_t* group_size, const int2* gpair, const int32_t* ridx, const B2HistWork* work,
+                   int n_work, int total_chunks, int chunk_rows, int window_rows, int n_groups, long long* hist,
+                   long long* scratch, const B2LevelCtl* ctl, int log2_shards, int node_cap, int num_sms, cudaStream_t stream) {
+  if (src.ebins)
+    return b2::launch_hist_csr(src, group_size, gpair, ridx, work, n_work, total_chunks, chunk_rows, n_groups, hist, scratch,
+                               ctl, log2_shards, node_cap, num_sms, stream);
+  const uint8_t* bins = src.bins; const int row_stride = src.row_stride;
   static bool attr_set = false;
   if (!attr_set) {
     cudaFuncSetAttribute(b2::hist_build_kernel_v3<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, B2_GROUP_ELEMS * 8);

@@ -157,7 +157,13 @@ T* from_handle(B2Handle h, int kind, const char* what) {
   return reinterpret_cast<T*>(h);
 }
 
+// The bins of a quantised matrix in their layout, dense or CSR (DESIGN.md 2 item 26).  Defined in matrix.cu, the one
+// place that knows the layout: the launchers get the bins through bin_source.
+struct MatrixBins;
+
 struct Matrix : HandleBase {
+  Matrix();
+  ~Matrix();
   uint64_t margin_version = 0;   // bumped when base_margin changes (cached evaluation margins start from it)
   uint64_t uid = 0;       // unique for the life of the process; 0 = not registered (stack temporaries)
   Ctx* ctx = nullptr;
@@ -172,15 +178,8 @@ struct Matrix : HandleBase {
   int64_t nnz = 0;
   DevBuf<int64_t> csr_indptr; DevBuf<int32_t> csr_indices; DevBuf<float> csr_values;
   bool has_raw = false;  // raw, or the CSR buffers, are on the device
-  DevBuf<uint8_t> bins;  // [n][row_stride]
-  DevBuf<uint8_t> bins_col;  // [F][col_stride] feature-major copy for the row partition
-  int64_t col_stride = 0;
-  // bin layout (B2_MatrixSetBinLayout): the requested B2_BIN_LAYOUT_*, and after quantisation whether the matrix holds the
-  // CSR layout -- ebins [nnz], one bin per stored entry, instead of bins and bins_col; csr_indptr / csr_indices then
-  // stay on the device after the raw values are released (DESIGN.md 2 item 26)
-  int bin_layout = B2_BIN_LAYOUT_AUTO;
-  bool csr_bins = false;
-  DevBuf<uint8_t> ebins;
+  int bin_layout = B2_BIN_LAYOUT_AUTO;   // the requested B2_BIN_LAYOUT_* (B2_MatrixSetBinLayout)
+  std::unique_ptr<MatrixBins> qbins;
   bool quantized = false;
   int n_groups = 0, row_stride = 0, max_bin = 0;
   std::vector<int32_t> group_first, group_size, feat_byte;
@@ -252,8 +251,16 @@ void for_raw_tiles(Matrix* m, Fn fn, int64_t max_rows = INT64_MAX) {
     r0 += step;
   } while (r0 < m->n);
 }
+// uploads the CSR arrays and checks them; a matrix in the CSR bin layout kept indptr and indices, so only its values
 void upload_csr(Matrix* m, const int64_t* indptr, const int32_t* indices, const float* values);
 size_t matrix_device_bytes(const Matrix* m);
+
+// ---- bins (matrix.cu): the one place that knows whether a quantised matrix holds its bins dense or as CSR
+B2BinRows bin_source(const Matrix* m);             // fails on a matrix that is not quantised
+void bins_to_host(const Matrix* m, uint8_t* out);  // out [n][F]: every cell's bin (an absent CSR entry: the missing bin)
+// a matrix quantised from host bins, without cuts (the histogram entries B2_HistBuildRaw*): bins [n][F] for a dense
+// matrix, one bin per stored entry [nnz] for a CSR one whose indptr / indices are uploaded (upload_csr)
+void upload_bins(Matrix* m, const uint8_t* bins);
 
 // B2_MatrixSlice: a new unquantised matrix of parent rows rows[0..n) (host array), gathered on the device
 B2Handle slice_matrix(Matrix* parent, const int64_t* rows, int64_t n);
@@ -425,7 +432,7 @@ struct Booster : HandleBase {
   DevBuf<int2> q;                // [n]
   DevBuf<int32_t> ridx[2];
   DevBuf<long long> hist[2];
-  DevBuf<long long> csr_hist_tot;  // CSR bin layout: [nodes of a level][2] row totals of a histogram build (launch_hist)
+  DevBuf<long long> hist_scratch;  // b2_hist_scratch_elems of a level's histogram build (launch_hist)
   // Everything a peer maps lives in ONE allocation (one cudaIpc handle per peer instead of four): the build buffer, the
   // candidate table, the misc table and the flag words are views into it
   template <typename T> struct View { T* p = nullptr; };
@@ -614,6 +621,10 @@ void run_tree(Booster* b, int k, int slot);
 void materialize_tree(Booster* b, const void* block);
 void materialize_vector_tree(Booster* b, const void* block, const void* vblock);
 void sync_device_trees(Booster* b);
+// B2_HistBuildRaw*: one histogram of m's rows ridx[0..n_sel) (nullptr: rows 0..n_sel) from the pairs (qg, qh) into out
+// [F][256][2]; chunk_rows <= 0 and window_rows <= 0 take 2048 and 4096, chunk_rows is capped at window_rows
+void hist_build_raw(Matrix* m, const int32_t* qg, const int32_t* qh, const int32_t* ridx, int64_t n_sel, int window_rows,
+                    int chunk_rows, int64_t* out, float* kernel_ms);
 
 // ---------------------------------------------------------------- round.cu
 cudaEvent_t get_event(Booster* b);

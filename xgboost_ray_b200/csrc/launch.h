@@ -34,16 +34,13 @@ enum B2AftDist { kAftNormal = 0, kAftLogistic = 1, kAftExtreme = 2 };
 
 extern "C" {
 
-// hist_kernel.cu
-int b2_launch_hist(const uint8_t* bins, int row_stride, const int2* gpair, const int32_t* ridx, const B2HistWork* work,
+// hist_kernel.cu (the CSR bin layout's build in hist_csr_kernel.cu).  n_work / total_chunks / chunk_rows are read from
+// ctl when it is given.  window_rows is read by the dense build only, group_size [n_groups] by the CSR build only.
+// scratch: b2_hist_scratch_elems(src, node_cap) int64 of device memory, zeroed by the launch
+size_t b2_hist_scratch_elems(B2BinRows src, int node_cap);
+int b2_launch_hist(B2BinRows src, const int32_t* group_size, const int2* gpair, const int32_t* ridx, const B2HistWork* work,
                    int n_work, int total_chunks, int chunk_rows, int window_rows, int n_groups, long long* hist,
-                   const B2LevelCtl* ctl, int log2_shards, int node_cap, int num_sms, cudaStream_t stream);
-// hist_csr_kernel.cu: the same histograms from the CSR bin layout (ebins [nnz]).  totals [node_cap][2] must be zero;
-// n_work / total_chunks / chunk_rows as for b2_launch_hist (from ctl when it is given)
-int b2_launch_hist_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, const int32_t* feat_byte,
-                       const int32_t* group_size, const int2* gpair, const int32_t* ridx, const B2HistWork* work, int n_work,
-                       int total_chunks, int chunk_rows, int n_groups, long long* hist, long long* totals,
-                       const B2LevelCtl* ctl, int log2_shards, int node_cap, int num_sms, cudaStream_t stream);
+                   long long* scratch, const B2LevelCtl* ctl, int log2_shards, int node_cap, int num_sms, cudaStream_t stream);
 int b2_launch_hist_subtract(const long long* parent_level, long long* level, const int32_t* triples, int n_pairs,
                             int64_t node_elems, const B2LevelCtl* ctl, cudaStream_t stream);
 
@@ -93,23 +90,17 @@ int b2_launch_tree_init(B2TreeDev tree, B2LevelCtl* ctl0, B2NodeSeg* seg0, B2Eva
 // partition_kernel.cu
 int b2_part_chunk_rows();
 int b2_split_chunk_rows();
-int b2_launch_partition(const uint8_t* bins_col, int64_t col_stride, const int32_t* ridx_in, int32_t* ridx_out,
-                        const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, int32_t* counters, int any_categorical,
-                        B2FinalizeArgs fin, int num_sms, cudaStream_t stream);
-// the same two passes on the CSR bin layout: a row's bin of the split feature is found in its stored entries (b2_csr_bin)
-int b2_launch_partition_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, const int32_t* ridx_in,
-                            int32_t* ridx_out, const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, int32_t* counters,
-                            int any_categorical, B2FinalizeArgs fin, int num_sms, cudaStream_t stream);
-int b2_launch_final_assign_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, const int32_t* ridx_in,
-                               const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, const float2* gh,
-                               const int32_t* qexp, int leaf_bits, long long* sums, uint16_t* pos, int any_categorical,
-                               int num_sms, cudaStream_t stream);
+// partition and final assign read a row's bin of the split feature from bins_col, or in the CSR layout from the row's
+// stored entries (b2_csr_bin)
+int b2_launch_partition(B2BinRows src, const int32_t* ridx_in, int32_t* ridx_out, const B2SplitWork* work,
+                        const B2LevelCtl* ctl, int max_chunks, int32_t* counters, int any_categorical, B2FinalizeArgs fin,
+                        int num_sms, cudaStream_t stream);
 int b2_launch_leaf_sums(const float2* gh, const int32_t* ridx0, const int32_t* ridx1, const B2SegWork* work,
                         const B2LevelCtl* ctl, int max_chunks, const int32_t* qexp, int leaf_bits, long long* sums,
                         uint16_t* pos, int num_sms, cudaStream_t stream);
-int b2_launch_final_assign(const uint8_t* bins_col, int64_t col_stride, const int32_t* ridx_in, const B2SplitWork* work,
-                           const B2LevelCtl* ctl, int max_chunks, const float2* gh, const int32_t* qexp, int leaf_bits,
-                           long long* sums, uint16_t* pos, int any_categorical, int num_sms, cudaStream_t stream);
+int b2_launch_final_assign(B2BinRows src, const int32_t* ridx_in, const B2SplitWork* work, const B2LevelCtl* ctl,
+                           int max_chunks, const float2* gh, const int32_t* qexp, int leaf_bits, long long* sums, uint16_t* pos,
+                           int any_categorical, int num_sms, cudaStream_t stream);
 int b2_leaf_acc_max_depth();
 int b2_launch_leaf_accumulate(const float2* gh, const uint16_t* pos, int64_t n, int max_depth, const int32_t* qexp, int leaf_bits,
                               long long* sums, int num_sms, cudaStream_t stream);
@@ -186,14 +177,9 @@ int b2_launch_quantile_scan(int pass, const int32_t* n_leaves, int max_leaves, i
                             float* tree_value, cudaStream_t s);
 
 // dart_kernel.cu
-int b2_launch_dart_margins(const uint8_t* bins, int64_t n, int row_stride, const int32_t* feat_byte, const uint8_t* has_missing,
-                           const B2TreeNodeDev* nodes, const int32_t* tree_offset, const uint32_t* cat_table, int T, int K,
-                           int npt, const float* w_drop, const uint8_t* dropped, const float* w_full, float* drop, float* full,
-                           int num_sms, cudaStream_t s);
-int b2_launch_dart_margins_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, int64_t n,
-                               const uint8_t* has_missing, const B2TreeNodeDev* nodes, const int32_t* tree_offset,
-                               const uint32_t* cat_table, int T, int K, int npt, const float* w_drop, const uint8_t* dropped,
-                               const float* w_full, float* drop, float* full, int num_sms, cudaStream_t s);
+int b2_launch_dart_margins(B2BinRows src, int64_t n, const uint8_t* has_missing, const B2TreeNodeDev* nodes,
+                           const int32_t* tree_offset, const uint32_t* cat_table, int T, int K, int npt, const float* w_drop,
+                           const uint8_t* dropped, const float* w_full, float* drop, float* full, int num_sms, cudaStream_t s);
 
 // shap_kernel.cu
 size_t b2_shap_contribs_smem(int K, int F, int warps);

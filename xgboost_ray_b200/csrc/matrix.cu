@@ -13,6 +13,18 @@
 
 namespace b2host __attribute__((visibility("hidden"))) {
 
+// A quantised matrix normally keeps two byte copies of its bins: bins [n][row_stride] (row-major, read by the histogram
+// build and the DART walk) and bins_col [F][col_stride] (feature-major, read by the partition and the final assign).
+// The CSR layout keeps ebins [nnz] instead, one bin per stored entry aligned with the CSR's indices; csr_indptr /
+// csr_indices then stay on the device after the raw values are released (DESIGN.md 2 item 26).
+struct MatrixBins {
+  bool csr_bins = false;
+  DevBuf<uint8_t> bins, bins_col, ebins;
+  int64_t col_stride = 0;
+};
+Matrix::Matrix() : qbins(new MatrixBins()) {}
+Matrix::~Matrix() = default;
+
 // ids of the matrices that are alive: a Booster's evaluation cache is keyed by the id, never by the address (a freed
 // matrix and a new one of the same shape can share an address)
 static std::mutex g_matrix_mu;
@@ -201,10 +213,17 @@ B2RawRows raw_source(const Matrix* m) {
 
 // Uploads the CSR arrays of m (n rows, F columns and nnz set) and checks them on the device in one pass; the first row
 // that breaks a rule is named, with the rule read back from the caller's arrays.  The check guards the C ABI: an
-// out-of-range column would be written outside a densified tile.
+// out-of-range column would be written outside a densified tile.  A matrix in the CSR bin layout kept indptr and
+// indices on the device with its bins (release_raw): only the values come back.
 void upload_csr(Matrix* m, const int64_t* indptr, const int32_t* indices, const float* values) {
   Ctx* ctx = m->ctx; cudaStream_t s = ctx->stream;
   const int64_t n = m->n, nnz = m->nnz;
+  if (m->qbins->csr_bins) {
+    m->csr_values.ensure((size_t)nnz);
+    upload_pipelined(ctx, m->csr_values.p, values, (size_t)nnz * sizeof(float));
+    m->has_raw = true;
+    return;
+  }
   m->csr_indptr.ensure((size_t)n + 1); m->csr_indices.ensure((size_t)nnz); m->csr_values.ensure((size_t)nnz);
   upload_pipelined(ctx, m->csr_indptr.p, indptr, ((size_t)n + 1) * sizeof(int64_t));
   upload_pipelined(ctx, m->csr_indices.p, indices, (size_t)nnz * sizeof(int32_t));
@@ -253,7 +272,7 @@ B2Handle slice_matrix(Matrix* p, const int64_t* rows, int64_t n) {
   upload(d_rows, rows, (size_t)n, s);
   if (p->csr) {
     m->csr = true;
-    m->bin_layout = p->csr_bins ? B2_BIN_LAYOUT_CSR : p->bin_layout;
+    m->bin_layout = p->qbins->csr_bins ? B2_BIN_LAYOUT_CSR : p->bin_layout;
     m->csr_indptr.ensure((size_t)n + 1);
     DevBuf<int64_t> lengths; lengths.ensure((size_t)n);
     DevBuf<uint8_t> temp; const size_t tb = b2_csr_slice_temp_bytes(n); temp.ensure(std::max<size_t>(tb, 1));
@@ -294,7 +313,7 @@ B2Handle slice_matrix(Matrix* p, const int64_t* rows, int64_t n) {
 // the CSR bin layout keeps indptr and indices: they locate its bins
 static void release_raw(Matrix* m) {
   m->raw.release();
-  if (!m->csr_bins) { m->csr_indptr.release(); m->csr_indices.release(); }
+  if (!m->qbins->csr_bins) { m->csr_indptr.release(); m->csr_indices.release(); }
   m->csr_values.release();
   m->has_raw = false;
 }
@@ -302,8 +321,9 @@ static void release_raw(Matrix* m) {
 template <typename T>
 static size_t buf_bytes(const DevBuf<T>& d) { return d.cap * sizeof(T); }
 size_t matrix_device_bytes(const Matrix* m) {
+  const MatrixBins& q = *m->qbins;
   return buf_bytes(m->raw) + buf_bytes(m->csr_indptr) + buf_bytes(m->csr_indices) + buf_bytes(m->csr_values) +
-         buf_bytes(m->bins) + buf_bytes(m->bins_col) + buf_bytes(m->ebins) + buf_bytes(m->d_group_first) + buf_bytes(m->d_group_size) +
+         buf_bytes(q.bins) + buf_bytes(q.bins_col) + buf_bytes(q.ebins) + buf_bytes(m->d_group_first) + buf_bytes(m->d_group_size) +
          buf_bytes(m->d_feat_byte) + buf_bytes(m->d_cut_ptrs) + buf_bytes(m->d_nbins) + buf_bytes(m->d_cat_feats) +
          buf_bytes(m->d_cut_vals) + buf_bytes(m->d_has_missing) + buf_bytes(m->d_is_cat) + buf_bytes(m->label) +
          buf_bytes(m->weight) + buf_bytes(m->base_margin) + buf_bytes(m->lower) + buf_bytes(m->upper) +
@@ -643,28 +663,28 @@ static bool use_csr_bins(const Matrix* m) {
 }
 
 static void bin_matrix(Matrix* m) {
-  Ctx* ctx = m->ctx; cudaStream_t s = ctx->stream;
+  Ctx* ctx = m->ctx; cudaStream_t s = ctx->stream; MatrixBins& q = *m->qbins;
   setup_groups(m);
   upload_cuts(m);
   if (use_csr_bins(m)) {
-    m->csr_bins = true;
-    m->ebins.ensure((size_t)std::max<int64_t>(m->nnz, 1));
+    q.csr_bins = true;
+    q.ebins.ensure((size_t)std::max<int64_t>(m->nnz, 1));
     LAUNCH_CHECK(b2_launch_bin_csr(m->csr_indices.p, m->csr_values.p, m->nnz, m->missing, m->d_cut_ptrs.p, m->d_cut_vals.p,
-                                   m->any_cat() ? m->d_is_cat.p : nullptr, m->ebins.p, ctx->num_sms, s));
+                                   m->any_cat() ? m->d_is_cat.p : nullptr, q.ebins.p, ctx->num_sms, s));
     CUDA_CHECK(cudaStreamSynchronize(s));
     m->quantized = true;
     return;
   }
-  m->bins.ensure((size_t)std::max<int64_t>(m->n, 1) * m->row_stride);
-  CUDA_CHECK(cudaMemsetAsync(m->bins.p, 0, (size_t)std::max<int64_t>(m->n, 1) * m->row_stride, s));
-  m->col_stride = (std::max<int64_t>(m->n, 1) + 127) & ~(int64_t)127;
-  m->bins_col.ensure((size_t)m->col_stride * m->F);
+  q.bins.ensure((size_t)std::max<int64_t>(m->n, 1) * m->row_stride);
+  CUDA_CHECK(cudaMemsetAsync(q.bins.p, 0, (size_t)std::max<int64_t>(m->n, 1) * m->row_stride, s));
+  q.col_stride = (std::max<int64_t>(m->n, 1) + 127) & ~(int64_t)127;
+  q.bins_col.ensure((size_t)q.col_stride * m->F);
   // both bin kernels write rows [0, rows) of the bins / bins_col they are given and nothing else, so a tile writes its
   // own rows only
   for_raw_tiles(m, [&](const float* X, int64_t r0, int64_t rows) {
     LAUNCH_CHECK(b2_launch_bin(X, rows, m->F, m->missing, m->d_cut_ptrs.p, m->d_cut_vals.p, m->d_feat_byte.p,
-                               m->any_cat() ? m->d_is_cat.p : nullptr, m->row_stride, m->bins.p + (size_t)r0 * m->row_stride,
-                               m->bins_col.p + r0, m->col_stride, ctx->num_sms, s));
+                               m->any_cat() ? m->d_is_cat.p : nullptr, m->row_stride, q.bins.p + (size_t)r0 * m->row_stride,
+                               q.bins_col.p + r0, q.col_stride, ctx->num_sms, s));
   });
   CUDA_CHECK(cudaStreamSynchronize(s));
   m->quantized = true;
@@ -675,6 +695,46 @@ void quantize_matrix(Matrix* m, Comm* comm, int max_bin, bool borrowed_cuts, boo
   else make_cuts(m, comm, max_bin);
   bin_matrix(m);
   if (!keep_raw) release_raw(m);
+}
+
+B2BinRows bin_source(const Matrix* m) {
+  if (!m->quantized) fail("matrix is not quantised");
+  const MatrixBins& q = *m->qbins;
+  if (q.csr_bins) return B2BinRows{nullptr, 0, m->d_feat_byte.p, nullptr, 0, m->csr_indptr.p, m->csr_indices.p, q.ebins.p};
+  return B2BinRows{q.bins.p, m->row_stride, m->d_feat_byte.p, q.bins_col.p, q.col_stride, nullptr, nullptr, nullptr};
+}
+
+void bins_to_host(const Matrix* m, uint8_t* out) {
+  if (!m->quantized) fail("matrix is not quantised");
+  const MatrixBins& q = *m->qbins;
+  if (q.csr_bins) {
+    DevBuf<uint8_t> d; d.ensure((size_t)std::max<int64_t>(m->n * m->F, 1));
+    LAUNCH_CHECK(b2_launch_csr_bins_densify(m->csr_indptr.p, m->csr_indices.p, q.ebins.p, m->n, m->F, d.p, m->ctx->num_sms,
+                                            m->ctx->stream));
+    CUDA_CHECK(cudaMemcpyAsync(out, d.p, (size_t)m->n * m->F, cudaMemcpyDeviceToHost, m->ctx->stream));
+    CUDA_CHECK(cudaStreamSynchronize(m->ctx->stream));
+    return;
+  }
+  std::vector<uint8_t> h((size_t)m->n * m->row_stride);
+  if (m->n > 0) CUDA_CHECK(cudaMemcpy(h.data(), q.bins.p, h.size(), cudaMemcpyDeviceToHost));
+  for (int64_t i = 0; i < m->n; ++i)
+    for (int f = 0; f < m->F; ++f) out[i * m->F + f] = h[(size_t)i * m->row_stride + m->feat_byte[f]];
+}
+
+void upload_bins(Matrix* m, const uint8_t* bins) {
+  cudaStream_t s = m->ctx->stream; MatrixBins& q = *m->qbins;
+  setup_groups(m);
+  upload(m->d_feat_byte, m->feat_byte, s); upload(m->d_group_size, m->group_size, s);
+  if (m->csr) {
+    q.csr_bins = true;
+    upload(q.ebins, bins, (size_t)m->nnz, s);
+  } else {
+    std::vector<uint8_t> padded((size_t)std::max<int64_t>(m->n, 1) * m->row_stride, 0);
+    for (int64_t i = 0; i < m->n; ++i)
+      for (int f = 0; f < m->F; ++f) padded[(size_t)i * m->row_stride + m->feat_byte[f]] = bins[i * m->F + f];
+    upload(q.bins, padded, s);   // pageable source: staged before return
+  }
+  m->quantized = true;
 }
 
 }  // namespace b2host

@@ -448,16 +448,13 @@ static int launch_final_assign(Bins src, const int32_t* ridx_in, const B2SplitWo
 
 extern "C" {
 // partition + finalize of a level: `fin` is what the last CTA writes (level_finalize.cuh)
-int b2_launch_partition(const uint8_t* bins_col, int64_t col_stride, const int32_t* ridx_in, int32_t* ridx_out,
-                        const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, int32_t* counters, int any_categorical,
-                        B2FinalizeArgs fin, int num_sms, cudaStream_t stream) {
-  return launch_partition(b2::ColBins{bins_col, col_stride}, ridx_in, ridx_out, work, ctl, max_chunks, counters, any_categorical,
-                          fin, num_sms, stream);
-}
-int b2_launch_partition_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, const int32_t* ridx_in,
-                            int32_t* ridx_out, const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, int32_t* counters,
-                            int any_categorical, B2FinalizeArgs fin, int num_sms, cudaStream_t stream) {
-  return launch_partition(b2::CsrBins{indptr, indices, ebins}, ridx_in, ridx_out, work, ctl, max_chunks, counters,
+int b2_launch_partition(B2BinRows src, const int32_t* ridx_in, int32_t* ridx_out, const B2SplitWork* work,
+                        const B2LevelCtl* ctl, int max_chunks, int32_t* counters, int any_categorical, B2FinalizeArgs fin,
+                        int num_sms, cudaStream_t stream) {
+  if (src.ebins)
+    return launch_partition(b2::CsrBins{src.indptr, src.indices, src.ebins}, ridx_in, ridx_out, work, ctl, max_chunks, counters,
+                            any_categorical, fin, num_sms, stream);
+  return launch_partition(b2::ColBins{src.bins_col, src.col_stride}, ridx_in, ridx_out, work, ctl, max_chunks, counters,
                           any_categorical, fin, num_sms, stream);
 }
 int b2_launch_leaf_sums(const float2* gh, const int32_t* ridx0, const int32_t* ridx1, const B2SegWork* work,
@@ -468,17 +465,13 @@ int b2_launch_leaf_sums(const float2* gh, const int32_t* ridx0, const int32_t* r
   b2::leaf_sums_kernel<<<grid, 256, 0, stream>>>(gh, ridx0, ridx1, work, ctl, qexp, leaf_bits, sums, pos);
   return (int)cudaGetLastError();
 }
-int b2_launch_final_assign(const uint8_t* bins_col, int64_t col_stride, const int32_t* ridx_in, const B2SplitWork* work,
-                           const B2LevelCtl* ctl, int max_chunks, const float2* gh, const int32_t* qexp, int leaf_bits,
-                           long long* sums, uint16_t* pos, int any_categorical, int num_sms, cudaStream_t stream) {
-  return launch_final_assign(b2::ColBins{bins_col, col_stride}, ridx_in, work, ctl, max_chunks, gh, qexp, leaf_bits, sums, pos,
-                             any_categorical, num_sms, stream);
-}
-int b2_launch_final_assign_csr(const int64_t* indptr, const int32_t* indices, const uint8_t* ebins, const int32_t* ridx_in,
-                               const B2SplitWork* work, const B2LevelCtl* ctl, int max_chunks, const float2* gh,
-                               const int32_t* qexp, int leaf_bits, long long* sums, uint16_t* pos, int any_categorical,
-                               int num_sms, cudaStream_t stream) {
-  return launch_final_assign(b2::CsrBins{indptr, indices, ebins}, ridx_in, work, ctl, max_chunks, gh, qexp, leaf_bits, sums,
+int b2_launch_final_assign(B2BinRows src, const int32_t* ridx_in, const B2SplitWork* work, const B2LevelCtl* ctl,
+                           int max_chunks, const float2* gh, const int32_t* qexp, int leaf_bits, long long* sums, uint16_t* pos,
+                           int any_categorical, int num_sms, cudaStream_t stream) {
+  if (src.ebins)
+    return launch_final_assign(b2::CsrBins{src.indptr, src.indices, src.ebins}, ridx_in, work, ctl, max_chunks, gh, qexp,
+                               leaf_bits, sums, pos, any_categorical, num_sms, stream);
+  return launch_final_assign(b2::ColBins{src.bins_col, src.col_stride}, ridx_in, work, ctl, max_chunks, gh, qexp, leaf_bits, sums,
                              pos, any_categorical, num_sms, stream);
 }
 int b2_leaf_acc_max_depth() { return b2::kLeafAccMaxDepth; }

@@ -476,17 +476,10 @@ void dart_margins(Booster* b, const std::vector<float>& w_old, const std::vector
   sync_device_trees(b);
   upload(b->d_dart_w_full, w_full, s);
   if (drop) { upload(b->d_dart_w_old, w_old, s); upload(b->d_dart_dropped, dropped, s); }
-  if (m->csr_bins)
-    LAUNCH_CHECK(b2_launch_dart_margins_csr(m->csr_indptr.p, m->csr_indices.p, m->ebins.p, m->n, m->d_has_missing.p,
-                                            b->d_nodes.p, b->d_tree_offset.p, b->d_cat_table.p, T, b->p.num_class,
-                                            b->p.num_parallel_tree, drop ? b->d_dart_w_old.p : nullptr,
-                                            drop ? b->d_dart_dropped.p : nullptr, b->d_dart_w_full.p, drop, full,
-                                            b->ctx->num_sms, s));
-  else
-    LAUNCH_CHECK(b2_launch_dart_margins(m->bins.p, m->n, m->row_stride, m->d_feat_byte.p, m->d_has_missing.p, b->d_nodes.p,
-                                        b->d_tree_offset.p, b->d_cat_table.p, T, b->p.num_class, b->p.num_parallel_tree,
-                                        drop ? b->d_dart_w_old.p : nullptr, drop ? b->d_dart_dropped.p : nullptr,
-                                        b->d_dart_w_full.p, drop, full, b->ctx->num_sms, s));
+  LAUNCH_CHECK(b2_launch_dart_margins(bin_source(m), m->n, m->d_has_missing.p, b->d_nodes.p, b->d_tree_offset.p,
+                                      b->d_cat_table.p, T, b->p.num_class, b->p.num_parallel_tree,
+                                      drop ? b->d_dart_w_old.p : nullptr, drop ? b->d_dart_dropped.p : nullptr,
+                                      b->d_dart_w_full.p, drop, full, b->ctx->num_sms, s));
 }
 
 void ensure_train_margin(Booster* b) {

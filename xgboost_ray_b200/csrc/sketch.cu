@@ -8,7 +8,6 @@
 // values are emitted.  Binning is bin = upper_bound(cuts_f, x) into the padded group-major row
 // layout used by the histogram kernel.
 #include <algorithm>
-#include <stdlib.h>
 
 #include <cub/cub.cuh>
 
@@ -482,9 +481,7 @@ int b2_launch_bin(const float* X, int64_t n, int F, float missing, const int32_t
                   const int32_t* feat_byte, const uint8_t* is_cat, int row_stride, uint8_t* bins, uint8_t* bins_col,
                   int64_t col_stride, int num_sms, cudaStream_t s) {
   if (n <= 0) return 0;
-  static int use_tiled = -1;
-  if (use_tiled < 0) { const char* e = getenv("B2_BIN_TILED"); use_tiled = (e && atoi(e) == 0) ? 0 : 1; }
-  if (use_tiled && F <= b2::kBinMaxF) {
+  if (F <= b2::kBinMaxF) {
     const int smem = b2::kBinTileRows * ((F | 1) * (int)sizeof(float) + row_stride + 4);
     static bool attr_set = false;
     if (!attr_set) {

@@ -179,7 +179,7 @@ void ensure_ctl_tables(Booster* b) {
   if (!b->d_part_done.p) { b->d_part_done.ensure(1); CUDA_CHECK(cudaMemsetAsync(b->d_part_done.p, 0, sizeof(uint32_t), b->ctx->stream)); }
   if (!b->d_eval_done.p) { b->d_eval_done.ensure(1); CUDA_CHECK(cudaMemsetAsync(b->d_eval_done.p, 0, sizeof(uint32_t), b->ctx->stream)); }
   b->d_cand_best.ensure(half);
-  if (b->train->csr_bins) b->csr_hist_tot.ensure(2 * half);
+  b->hist_scratch.ensure(b2_hist_scratch_elems(bin_source(b->train), (int)half));
   b->d_leaves.ensure(L.max_nodes); b->d_seg_work.ensure(L.max_nodes);
   b->d_leaf_sums.ensure(4 * lcap); b->d_leaf_values.ensure(lcap);   // [leaf][g, h][hi, lo] limbs (common.cuh)
   if (b->ic_words > 0) b->d_ic_compat.ensure(L.max_nodes * (size_t)b->ic_words);
@@ -409,18 +409,49 @@ void launch_hist(Booster* b, TreeStats& st, const int2* q, const int32_t* ridx, 
     root = 1; chunk_rows = pick_chunk_rows(b, n); chunks = (int)((n + chunk_rows - 1) / chunk_rows);
   }
   cudaEvent_t e0 = nullptr, e1 = nullptr;
-  if (m->csr_bins) CUDA_CHECK(cudaMemsetAsync(b->csr_hist_tot.p, 0, 2 * (size_t)nodes * sizeof(long long), b->ctx->stream));
   record_hist_launch(b, st, e0, e1, true);
-  if (m->csr_bins)
-    LAUNCH_CHECK(b2_launch_hist_csr(m->csr_indptr.p, m->csr_indices.p, m->ebins.p, m->d_feat_byte.p, m->d_group_size.p, q, ridx,
-                                    b->d_hist_work.p, root, chunks, chunk_rows, m->n_groups, tgt, b->csr_hist_tot.p, ctl,
-                                    b->log2_shards, nodes, b->ctx->num_sms, b->ctx->stream));
-  else
-    LAUNCH_CHECK(b2_launch_hist(m->bins.p, m->row_stride, q, ridx, b->d_hist_work.p, root, chunks, chunk_rows,
-                                window_rows_for(b->p.qbits), m->n_groups, tgt, ctl, b->log2_shards, nodes, b->ctx->num_sms,
-                                b->ctx->stream));
+  LAUNCH_CHECK(b2_launch_hist(bin_source(m), m->d_group_size.p, q, ridx, b->d_hist_work.p, root, chunks, chunk_rows,
+                              window_rows_for(b->p.qbits), m->n_groups, tgt, b->hist_scratch.p, ctl, b->log2_shards, nodes,
+                              b->ctx->num_sms, b->ctx->stream));
   record_hist_launch(b, st, e0, e1, false);
   st.hist_launches++; st.kernel_launches++;
+}
+
+void hist_build_raw(Matrix* m, const int32_t* qg, const int32_t* qh, const int32_t* ridx, int64_t n_sel, int window_rows,
+                    int chunk_rows, int64_t* out, float* kernel_ms) {
+  Ctx* ctx = m->ctx; cudaStream_t s = ctx->stream; const B2BinRows src = bin_source(m);
+  std::vector<int2> gp((size_t)std::max<int64_t>(m->n, 1));
+  for (int64_t i = 0; i < m->n; ++i) gp[i] = make_int2(qg[i], qh[i]);
+  DevBuf<int2> d_gp; DevBuf<int32_t> d_ridx; DevBuf<long long> d_hist, d_scratch; DevBuf<B2HistWork> d_work;
+  upload(d_gp, gp, s);
+  if (ridx) upload(d_ridx, ridx, (size_t)std::max<int64_t>(n_sel, 0), s);
+  const size_t node_elems = (size_t)m->n_groups * B2_GROUP_ELEMS;
+  d_hist.ensure(node_elems); d_scratch.ensure(b2_hist_scratch_elems(src, 1));
+  CUDA_CHECK(cudaMemsetAsync(d_hist.p, 0, node_elems * sizeof(long long), s));
+  if (window_rows <= 0) window_rows = 4096;
+  if (chunk_rows <= 0) chunk_rows = 2048;
+  if (chunk_rows > window_rows) chunk_rows = window_rows;
+  B2HistWork w{0, (int32_t)n_sel, 0, 0};
+  upload(d_work, &w, 1, s);
+  const int chunks = (int)((n_sel + chunk_rows - 1) / chunk_rows);
+  cudaEvent_t e0, e1; CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
+  CUDA_CHECK(cudaEventRecord(e0, s));
+  if (n_sel > 0)
+    LAUNCH_CHECK(b2_launch_hist(src, m->d_group_size.p, d_gp.p, ridx ? d_ridx.p : nullptr, d_work.p, 1, chunks, chunk_rows,
+                                window_rows, m->n_groups, d_hist.p, d_scratch.p, nullptr, 0, 1, ctx->num_sms, s));
+  CUDA_CHECK(cudaEventRecord(e1, s));
+  std::vector<long long> h(node_elems);
+  CUDA_CHECK(cudaMemcpyAsync(h.data(), d_hist.p, node_elems * sizeof(long long), cudaMemcpyDeviceToHost, s));
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  if (kernel_ms) { float ms = 0; cudaEventElapsedTime(&ms, e0, e1); *kernel_ms = ms; }
+  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  for (int f = 0; f < m->F; ++f) {
+    const int g = m->feat_byte[f] / B2_GROUP_SLOTS, sl = m->feat_byte[f] % B2_GROUP_SLOTS;
+    for (int bb = 0; bb < 256; ++bb) {
+      out[((size_t)f * 256 + bb) * 2] = h[(size_t)g * B2_GROUP_ELEMS + bb * 32 + sl];
+      out[((size_t)f * 256 + bb) * 2 + 1] = h[(size_t)g * B2_GROUP_ELEMS + B2_PLANE_ELEMS + bb * 32 + sl];
+    }
+  }
 }
 
 // What decide does at the end of level d's split scan, with cpn candidates per node and rank
@@ -474,14 +505,9 @@ void partition_level(Booster* b, TreeStats& st, int d) {
   fin.max_pairs = 1 << d; fin.need_hist = d + 1 < p.max_depth ? 1 : 0;
   fin.n_streams = std::max(1, b->ctx->num_sms * 3 / m->n_groups); fin.window_rows = window_rows_for(p.qbits);
   fin.chunk_rows_override = p.hist_chunk_rows;
-  if (m->csr_bins)
-    LAUNCH_CHECK(b2_launch_partition_csr(m->csr_indptr.p, m->csr_indices.p, m->ebins.p, level_ridx(b, d), b->ridx[nxt].p,
-                                         b->d_split_work.p, ctl + cur, split_work_items(b, d), b->d_counters.p,
-                                         m->any_cat() ? 1 : 0, fin, b->ctx->num_sms, b->ctx->stream));
-  else
-    LAUNCH_CHECK(b2_launch_partition(m->bins_col.p, m->col_stride, level_ridx(b, d), b->ridx[nxt].p, b->d_split_work.p,
-                                     ctl + cur, split_work_items(b, d), b->d_counters.p, m->any_cat() ? 1 : 0, fin,
-                                     b->ctx->num_sms, b->ctx->stream));
+  LAUNCH_CHECK(b2_launch_partition(bin_source(m), level_ridx(b, d), b->ridx[nxt].p, b->d_split_work.p, ctl + cur,
+                                   split_work_items(b, d), b->d_counters.p, m->any_cat() ? 1 : 0, fin, b->ctx->num_sms,
+                                   b->ctx->stream));
   st.kernel_launches++;
 }
 
@@ -494,13 +520,8 @@ void assign_leaves(Booster* b, TreeStats& st, int d, const float2* gh, const int
   const int max_leaf_chunks = (int)((m->n + lchunk - 1) / lchunk) + (1 << b->p.max_depth);
   LAUNCH_CHECK(b2_launch_leaf_sums(gh, b->ridx[0].p, b->ridx[1].p, b->d_seg_work.p, ctl + 2, max_leaf_chunks, qexp, 40, sums,
                                    b->pos.p, sms, s));
-  if (m->csr_bins)
-    LAUNCH_CHECK(b2_launch_final_assign_csr(m->csr_indptr.p, m->csr_indices.p, m->ebins.p, level_ridx(b, d), b->d_split_work.p,
-                                            ctl + (d & 1), split_work_items(b, d), gh, qexp, 40, sums, b->pos.p,
-                                            m->any_cat() ? 1 : 0, sms, s));
-  else
-    LAUNCH_CHECK(b2_launch_final_assign(m->bins_col.p, m->col_stride, level_ridx(b, d), b->d_split_work.p, ctl + (d & 1),
-                                        split_work_items(b, d), gh, qexp, 40, sums, b->pos.p, m->any_cat() ? 1 : 0, sms, s));
+  LAUNCH_CHECK(b2_launch_final_assign(bin_source(m), level_ridx(b, d), b->d_split_work.p, ctl + (d & 1), split_work_items(b, d),
+                                      gh, qexp, 40, sums, b->pos.p, m->any_cat() ? 1 : 0, sms, s));
   st.kernel_launches += 2;
 }
 
