@@ -22,27 +22,8 @@ MULTI_TARGET_OBJECTIVES = ("reg:squarederror", "reg:squaredlogerror", "reg:logis
 
 def column_gradients(params, margin, label, weight=None):
     """(g, h, non-finite count) [n][T] in binary32: the single-target sequence of every column."""
-    obj = params["objective"]
-    m, y = np.asarray(margin, F32), np.asarray(label, F32)
-    g, h = np.zeros_like(m), np.zeros_like(m)
-    bad = 0
-    for k in range(y.shape[1]):
-        if obj in ("reg:squarederror", "binary:logistic"):
-            # the first two objectives live in the oracle; restated in their binary32 sequence
-            w = np.ones(len(y), F32) if weight is None else np.asarray(weight, F32)
-            yk, mk = y[:, k], m[:, k]
-            if obj == "binary:logistic":
-                w = np.where(yk == F32(1.0), w * F32(params.get("scale_pos_weight", 1.0)), w).astype(F32)
-                s = O.sigmoid_(mk)
-                gk, hk = (s - yk).astype(F32), np.maximum((s * (F32(1.0) - s)).astype(F32), F32(1e-16))
-            else:
-                gk, hk = (mk - yk).astype(F32), np.ones_like(mk)
-            gk, hk, b = (gk * w).astype(F32), (hk * w).astype(F32), 0
-        else:
-            gk, hk, b = O.gradients(params, m[:, k], y[:, k], weight)
-        g[:, k], h[:, k] = gk, hk
-        bad += b
-    return g, h, bad
+    g, h, bad = O.gradients_multi_target(params, margin, label, weight)
+    return g.T.copy(), h.T.copy(), bad
 
 
 def intercept(params, label, weight=None):

@@ -1,7 +1,7 @@
-"""Reference for the objectives beyond squared error / logistic / softmax (reg:logistic, binary:logitraw,
+"""Reference for the scalar objectives (reg:squarederror / reg:linear, binary:logistic, reg:logistic, binary:logitraw,
 reg:squaredlogerror, reg:pseudohubererror, count:poisson, reg:gamma, reg:tweedie): a NumPy restatement of their
-gradients, intercept, transform, metrics and label domains (DESIGN.md 4.4), and a trainer that grows trees with the
-CPU oracle (oracle/hist_oracle.c) from those gradients through its custom-gradient path.
+gradients (one target or several), intercept, transform, metrics and label domains (DESIGN.md 4.4), and a trainer that
+grows trees with the CPU oracle (oracle/hist_oracle.c) from those gradients through its custom-gradient path.
 
 TEST INFRASTRUCTURE ONLY, like the oracle.  The gradients replay the binary32 sequences of objective_kernel.cu
 operation for operation: NumPy's float32 +, -, *, / and sqrt round correctly, b2_expf and b2_log1pf are restated on
@@ -17,7 +17,14 @@ F = np.float32
 OBJECTIVES = ("reg:logistic", "binary:logitraw", "reg:squaredlogerror", "reg:pseudohubererror", "count:poisson",
               "reg:gamma", "reg:tweedie")
 LOG_LINK = ("count:poisson", "reg:gamma", "reg:tweedie")
-REG_LOSS = ("reg:logistic", "binary:logitraw", "reg:squaredlogerror")   # scale_pos_weight applies to these
+# every objective whose gradient is gradient_scalar_kernel's, gradient_param_kernel's or gradient_multi_target_kernel's
+SCALAR_OBJECTIVES = ("reg:squarederror", "reg:linear", "binary:logistic") + OBJECTIVES
+LOGISTIC = ("binary:logistic", "reg:logistic", "binary:logitraw")   # one gradient sequence, different transforms
+SIGMOID_LINK = ("binary:logistic", "reg:logistic")
+REG_LOSS = ("binary:logistic", "reg:logistic", "binary:logitraw", "reg:squaredlogerror")   # scale_pos_weight applies
+# the objectives whose kernel writes a pair that is not finite as (0, 0) and fails the round (checks_finite in the
+# objective table); squared error and the logistic family write whatever the binary32 sequence gives
+CHECKS_FINITE = ("reg:squaredlogerror", "reg:pseudohubererror", "count:poisson", "reg:gamma", "reg:tweedie")
 DEFAULT_METRIC = {"reg:logistic": "rmse", "binary:logitraw": "logloss", "reg:squaredlogerror": "rmsle",
                   "reg:pseudohubererror": "mphe", "count:poisson": "poisson-nloglik", "reg:gamma": "gamma-nloglik",
                   "reg:tweedie": "tweedie-nloglik"}
@@ -27,6 +34,8 @@ LABEL_DOMAIN = {"reg:logistic": ("label must be in [0, 1]", lambda y: (y >= 0) &
                 "count:poisson": ("label must be nonnegative", lambda y: y >= 0),
                 "reg:tweedie": ("label must be nonnegative", lambda y: y >= 0),
                 "reg:gamma": ("label must be positive", lambda y: y > 0)}
+for _o in ("reg:squarederror", "reg:linear", "binary:logistic", "reg:pseudohubererror"):
+    LABEL_DOMAIN[_o] = ("label must be finite", lambda y: np.abs(y) <= np.finfo(F).max)
 
 _libm = ctypes.CDLL(ctypes.util.find_library("m"))
 _libm.logf.restype = ctypes.c_float
@@ -117,7 +126,8 @@ def max_delta_step(params):
 
 
 def gradients(params, margin, label, weight=None):
-    """(g, h, number of non-finite rows) in binary32 for one scalar objective; non-finite pairs are (0, 0)."""
+    """(g, h, number of non-finite rows) in binary32 for one scalar objective.  For the objectives in CHECKS_FINITE a
+    non-finite pair is written as (0, 0) and counted; the others keep it and count nothing, like their kernel."""
     obj = params["objective"]
     p, y = np.asarray(margin, F).reshape(-1), np.asarray(label, F)
     w = np.ones_like(y) if weight is None else np.asarray(weight, F)
@@ -125,7 +135,9 @@ def gradients(params, margin, label, weight=None):
     with np.errstate(all="ignore"):
         if obj in REG_LOSS:
             w = np.where(y == F(1.0), w * F(params.get("scale_pos_weight", 1.0)), w).astype(F)
-        if obj in ("reg:logistic", "binary:logitraw"):
+        if obj in ("reg:squarederror", "reg:linear"):
+            g, h = p - y, np.ones_like(p)
+        elif obj in LOGISTIC:
             s = sigmoid_(p)
             g, h = s - y, np.maximum(s * (F(1.0) - s), F(1e-16))
         elif obj == "reg:squaredlogerror":
@@ -154,14 +166,29 @@ def gradients(params, margin, label, weight=None):
             raise KeyError(obj)
         g, h = (g * w).astype(F), (h * w).astype(F)
         bad = ~((np.abs(g) <= np.finfo(F).max) & (np.abs(h) <= np.finfo(F).max))
+    if obj not in CHECKS_FINITE:
+        return g, h, 0
     g[bad] = 0.0
     h[bad] = 0.0
     return g, h, int(bad.sum())
 
 
+def gradients_multi_target(params, margin, label, weight=None):
+    """(g, h, number of non-finite elements) of a label of T columns: margin and label [n][T], one weight per row, g and
+    h class-major [T][n] like the engine's gh (target k's pairs are row k).  Element (i, k) is gradients()'s sequence."""
+    m, y = np.asarray(margin, F), np.asarray(label, F)
+    n, T = y.shape
+    g, h = np.zeros((T, n), F), np.zeros((T, n), F)
+    bad = 0
+    for k in range(T):
+        g[k], h[k], b = gradients(params, m[:, k], y[:, k], weight)
+        bad += b
+    return g, h, bad
+
+
 def transform(obj, m):
     m = np.asarray(m, F)
-    if obj == "reg:logistic":
+    if obj in SIGMOID_LINK:
         return sigmoid_(m)
     if obj in LOG_LINK:
         return expf_(m)
@@ -188,7 +215,7 @@ def estimate_base_score(params, label, weight=None):
 def base_margin(obj, b):
     """Margin of base_score b: the inverse transform, evaluated with libm's logf like the engine's host code."""
     b = F(b)
-    if obj == "reg:logistic":
+    if obj in SIGMOID_LINK:
         return float(F(-_libm.logf(float(F(1.0) / b - F(1.0)))))
     if obj in LOG_LINK:
         return float(F(_libm.logf(float(b))))

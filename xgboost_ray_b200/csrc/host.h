@@ -328,7 +328,7 @@ struct Params {
 // What an objective is on the host: one row of params.cu kObjectives per accepted name (DESIGN.md 4.4)
 enum ObjLink { kLinkIdentity, kLinkSigmoid, kLinkExp, kLinkSoftmax };
 enum ObjGrad { kGradScalar, kGradSoftprob, kGradAft, kGradRank, kGradQuantile };
-enum ObjLabels { kLabelsAny, kLabelsDomain, kLabelsBounds, kLabelsRank };
+enum ObjLabels { kLabelsDomain, kLabelsBounds, kLabelsRank };
 enum ObjIntercept { kInterceptStump, kInterceptQuantile, kInterceptFixed, kInterceptNone };
 struct Objective {
   const char* name;

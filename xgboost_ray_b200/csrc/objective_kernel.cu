@@ -649,7 +649,8 @@ __global__ void label_check_kernel(int objective, int K, const float* __restrict
     else if (objective == kObjSquaredLog) ok = y > -1.0f;
     else if (objective == kObjPoisson || objective == kObjTweedie) ok = y >= 0.0f;
     else if (objective == kObjGamma) ok = y > 0.0f;
-    else if (objective == kObjQuantile) ok = fabsf(y) <= FLT_MAX;
+    else if (objective == kObjSquaredError || objective == kObjLogistic || objective == kObjPseudoHuber ||
+             objective == kObjQuantile) ok = fabsf(y) <= FLT_MAX;
     any |= !ok;
   }
   if (__any_sync(0xffffffffu, any) && (threadIdx.x & 31) == 0) atomicOr(bad, 1u);

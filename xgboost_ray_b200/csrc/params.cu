@@ -17,17 +17,19 @@ constexpr char kIn01[] = "label must be in [0, 1] for %s", kNonneg[] = "label mu
                kFinite[] = "label must be finite for %s",
                kClassIndex[] = "label must be in [0, num_class) for %s, num_class = %d";
 
-// Every accepted objective name.  reg:quantileerror's gradient pairs are finite for finite labels and weights (both
-// checked before the first round), so its rounds stay pipelined.
+// Every accepted objective name.  Every objective has a label rule: the ones without a narrower domain need a finite
+// label (kFinite), so that a NaN or infinite label fails training instead of reaching the gradient pairs, their
+// quantisation scale or the intercept.  reg:quantileerror's gradient pairs are finite for finite labels and weights
+// (both checked before the first round), so its rounds stay pipelined.
 constexpr Objective kObjectives[] = {
   // name, id, link, grad, param, multi_target, checks_finite, labels, intercept[, label_rule]
-  {"reg:squarederror", kObjSquaredError, kLinkIdentity, kGradScalar, nullptr, true, false, kLabelsAny, kInterceptStump},
-  {"reg:linear", kObjSquaredError, kLinkIdentity, kGradScalar, nullptr, true, false, kLabelsAny, kInterceptStump},
+  {"reg:squarederror", kObjSquaredError, kLinkIdentity, kGradScalar, nullptr, true, false, kLabelsDomain, kInterceptStump, kFinite},
+  {"reg:linear", kObjSquaredError, kLinkIdentity, kGradScalar, nullptr, true, false, kLabelsDomain, kInterceptStump, kFinite},
   {"reg:logistic", kObjRegLogistic, kLinkSigmoid, kGradScalar, nullptr, true, false, kLabelsDomain, kInterceptStump, kIn01},
-  {"binary:logistic", kObjLogistic, kLinkSigmoid, kGradScalar, nullptr, true, false, kLabelsAny, kInterceptStump},
+  {"binary:logistic", kObjLogistic, kLinkSigmoid, kGradScalar, nullptr, true, false, kLabelsDomain, kInterceptStump, kFinite},
   {"binary:logitraw", kObjLogitRaw, kLinkIdentity, kGradScalar, nullptr, true, false, kLabelsDomain, kInterceptStump, kIn01},
   {"reg:squaredlogerror", kObjSquaredLog, kLinkIdentity, kGradScalar, nullptr, true, true, kLabelsDomain, kInterceptStump, kAboveMinus1},
-  {"reg:pseudohubererror", kObjPseudoHuber, kLinkIdentity, kGradScalar, &Params::huber_slope, true, true, kLabelsAny, kInterceptStump},
+  {"reg:pseudohubererror", kObjPseudoHuber, kLinkIdentity, kGradScalar, &Params::huber_slope, true, true, kLabelsDomain, kInterceptStump, kFinite},
   {"count:poisson", kObjPoisson, kLinkExp, kGradScalar, &Params::max_delta_step, false, true, kLabelsDomain, kInterceptStump, kNonneg},
   {"reg:gamma", kObjGamma, kLinkExp, kGradScalar, nullptr, false, true, kLabelsDomain, kInterceptStump, kPositive},
   {"reg:tweedie", kObjTweedie, kLinkExp, kGradScalar, &Params::tweedie_variance_power, false, true, kLabelsDomain, kInterceptStump, kNonneg},

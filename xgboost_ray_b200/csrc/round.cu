@@ -155,7 +155,7 @@ void check_labels(Booster* b) {
   Matrix* m = b->train; const Params& p = b->p; const Objective& o = objective_row(p);
   if (o.labels == kLabelsBounds) { check_bounds(b); return; }
   if (o.labels == kLabelsRank) { check_rank_labels(b); return; }
-  if (o.labels == kLabelsAny || b->labels_checked) return;
+  if (b->labels_checked) return;
   check_train_labels(b);
   const std::vector<uint32_t> h = check_flags(b, 1, [&](uint32_t* bad) {
     return b2_launch_label_check(p.objective, p.num_class, m->label.p, m->n * p.num_target, bad, b->ctx->num_sms,
