@@ -161,8 +161,8 @@ int B2_BoosterUpdateOneIter(B2Handle b, int32_t iter);
 /* custom objective (xgb.train(obj=...), tests/test_xgboost_api.py:77-102): grad/hess [n_rows*num_class] */
 int B2_BoosterBoostOneIter(B2Handle b, const float* grad, const float* hess, int64_t len);
 /* update mode (params process_type=update, updater=refresh, refresh_leaf; xgb.train(xgb_model=...) of xgboost's
- * TreeRefresher): the trees added with B2_BoosterAddTree / B2_BoosterSetTreeCategories before the first round are the
- * trees to update, and the model starts empty.  Call r (0-based) takes round r of them (num_class x num_parallel_tree
+ * TreeRefresher): the trees added with B2_BoosterAddTree before the first round are the trees to update (the root
+ * must reach each of their nodes, and each has at most 65,536 leaves), and the model starts empty.  Call r (0-based) takes round r of them (num_class x num_parallel_tree
  * trees), computes the gradients at the margin of base_score / base_margin plus the rounds already refreshed, re-fits
  * every node's sum_hess, base_weight and loss_chg (and with refresh_leaf the leaf values) on the raw rows of the train
  * matrix, and appends the refreshed trees.  grad / hess == NULL: the objective's gradients, else a custom objective's
@@ -205,24 +205,44 @@ int B2_BoosterGetBaseScore(B2Handle b, float* out, int32_t* is_final);
  * num_target=<T> in params (a loaded model; a train matrix must then have T columns) */
 int B2_BoosterNumTargets(B2Handle b, int32_t* out);
 int B2_BoosterNumTrees(B2Handle b, int32_t* out);
+/* One tree of n_nodes nodes, every array [n_nodes] unless noted.  Node i splits when split_feature[i] >= 0 (rows with
+ * x < split_cond, or missing with default_left, go to left[i], the others to right[i]); otherwise it is a leaf of
+ * leaf value value[i].  Node 0 is the root; parent[i] is -1 for it.  Categorical part (model JSON split_type /
+ * categories*, SURVEY.md 8f row f1): split_type[i] = 1 for a categorical split; cat_bits[i*8 + (c >> 5)] bit (c & 31)
+ * set = category c goes RIGHT.  Vector-leaf tree (multi_strategy=multi_output_tree, T = num_target > 1):
+ * leaf_vector[i*T + k] is node i's value of target k -- a leaf's leaf value, an internal node's eta-scaled weight
+ * (model JSON base_weights) -- and leaf_vector_len = n_nodes * T.  A single-output tree has leaf_vector NULL (or
+ * leaf_vector_len 0). */
+typedef struct B2Tree {
+  int32_t n_nodes;
+  int32_t* left;
+  int32_t* right;
+  int32_t* parent;
+  int32_t* split_feature;
+  int32_t* split_bin;
+  float* split_cond;
+  uint8_t* default_left;
+  float* value;
+  float* base_weight;
+  float* loss_chg;
+  double* sum_hess;
+  uint8_t* split_type;
+  uint32_t* cat_bits;     /* [n_nodes * 8] */
+  float* leaf_vector;     /* [leaf_vector_len] */
+  int64_t leaf_vector_len;
+} B2Tree;
 int B2_BoosterTreeNumNodes(B2Handle b, int32_t tree, int32_t* out);
-int B2_BoosterGetTree(B2Handle b, int32_t tree, int32_t* left, int32_t* right, int32_t* parent,
-                      int32_t* split_feature, int32_t* split_bin, float* split_cond, uint8_t* default_left,
-                      float* value, float* base_weight, float* loss_chg, double* sum_hess);
-int B2_BoosterAddTree(B2Handle b, int32_t n_nodes, const int32_t* left, const int32_t* right,
-                      const int32_t* parent, const int32_t* split_feature, const int32_t* split_bin,
-                      const float* split_cond, const uint8_t* default_left, const float* value,
-                      const float* base_weight, const float* loss_chg, const double* sum_hess);
-/* categorical part of a tree (model JSON fields split_type / categories*, SURVEY.md 8f row f1): split_type[i] = 1
- * for a categorical split; cat_bits[i*8 + (c >> 5)] bit (c & 31) set = category c goes RIGHT.  Set* is called
- * after B2_BoosterAddTree when a model with categorical splits is loaded. */
-int B2_BoosterGetTreeCategories(B2Handle b, int32_t tree, uint8_t* split_type /*[n]*/, uint32_t* cat_bits /*[n*8]*/);
-int B2_BoosterSetTreeCategories(B2Handle b, int32_t tree, const uint8_t* split_type, const uint32_t* cat_bits);
-/* vector-leaf tree (multi_strategy=multi_output_tree, T = num_target > 1): v[i*T + k] is node i's value of target k --
- * a leaf's leaf value, an internal node's eta-scaled weight (model JSON base_weights).  Set is called after
- * B2_BoosterAddTree on a booster created with multi_strategy=multi_output_tree; Get fails on a single-output tree. */
-int B2_BoosterGetTreeLeafVector(B2Handle b, int32_t tree, float* v /*[n*T]*/, int64_t len);
-int B2_BoosterSetTreeLeafVector(B2Handle b, int32_t tree, const float* v, int64_t len);
+/* Fill the caller's arrays with tree `tree`: t->n_nodes must be its node count (B2_BoosterTreeNumNodes), every array
+ * is written, and leaf_vector_len must be the tree's leaf vector length (0 for a single-output tree). */
+int B2_BoosterGetTree(B2Handle b, int32_t tree, B2Tree* t);
+/* Append a whole tree to the model; the arrays are only read.  split_bin, base_weight, loss_chg and sum_hess may be
+ * NULL (-1, 0, 0, 0); split_type and cat_bits may be NULL (no categorical split); a leaf vector is given exactly on a
+ * booster created with multi_strategy=multi_output_tree.  The tree is refused, naming the tree, the node and the
+ * value, when it has no nodes, a split child outside [0, n_nodes), a split node reached twice from the root (a cycle
+ * or a shared subtree), a split feature outside the booster's features, a categorical split_type on a leaf, or a leaf
+ * vector that does not fit the booster's kind of tree.  Nodes the root does not reach (xgboost's deleted nodes) are
+ * allowed. */
+int B2_BoosterAddTree(B2Handle b, const B2Tree* t);
 /* booster=dart: the weight of every tree in model order (model JSON gradient_booster.weight_drop); tree t adds
  * fl(w[t] * leaf) to the margin.  Get on a gbtree booster returns 1 for every tree.  Set (after the trees were added
  * with B2_BoosterAddTree; a tree added to a dart booster starts at weight 1) needs finite weights >= 0 and one per

@@ -68,7 +68,8 @@ def test_python_binding_argument_types_match_header(built):
             "const uint32_t*": C.POINTER(C.c_uint32), "uint32_t*": C.POINTER(C.c_uint32),
             "const uint8_t*": C.POINTER(C.c_uint8), "uint8_t*": C.POINTER(C.c_uint8),
             "int64_t*": C.POINTER(C.c_int64), "int*": C.POINTER(C.c_int),
-            "float": C.c_float, "double": C.c_double, "int": C.c_int, "int32_t": C.c_int32, "int64_t": C.c_int64, "uint64_t": C.c_uint64}
+            "float": C.c_float, "double": C.c_double, "int": C.c_int, "int32_t": C.c_int32, "int64_t": C.c_int64, "uint64_t": C.c_uint64,
+            "const B2Tree*": C.POINTER(engine.B2Tree), "B2Tree*": C.POINTER(engine.B2Tree)}
     text = open(os.path.join(ROOT, "include", "b2hist.h")).read()
     text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
     checked = 0
@@ -92,3 +93,22 @@ def test_python_binding_argument_types_match_header(built):
             assert ok, "%s argument %d: binding %s, header %s" % (name, i + 1, g, w)
         checked += 1
     assert checked == len(declared_symbols())
+
+
+def test_tree_record_matches_header():
+    """engine.B2Tree has the fields of the header's B2Tree, in its order, and each array's element type: ctypes lays the
+    record out from this list alone, so a field out of place would hand the engine one array for another."""
+    from xgboost_ray_b200 import engine
+    C = ctypes
+    scalar = {"int32_t": C.c_int32, "int64_t": C.c_int64}
+    element = {"int32_t": np.int32, "float": np.float32, "double": np.float64, "uint8_t": np.uint8, "uint32_t": np.uint32}
+    text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "b2hist.h")).read(), flags=re.S)
+    body = re.search(r"typedef struct B2Tree \{(.*?)\} B2Tree;", text, flags=re.S).group(1)
+    fields = re.findall(r"(\w+)\s*(\*?)\s*(\w+);", body)
+    assert len(fields) == 16
+    assert [name for name, _ in engine.B2Tree._fields_] == [name for _, _, name in fields]
+    for (name, got), (typ, star, _) in zip(engine.B2Tree._fields_, fields):
+        if star:
+            assert got is C.c_void_p and engine.B2Tree.DTYPES[name] is element[typ], name
+        else:
+            assert got is scalar[typ], name

@@ -1,8 +1,9 @@
-"""The C entries of prediction, called through ctypes: each refusal of B2_BoosterPredict, B2_BoosterPredictContribs and
-B2_BoosterPredictLeaf matched against its whole message, which refusal wins when a call breaks two rules, and that an
-edit of an existing tree (B2_BoosterSetTreeCategories, B2_BoosterSetTreeLeafVector) reaches every cached copy of the
-model: the device node table, the TreeSHAP paths and the evaluation margins."""
+"""The C entries of prediction and of the tree record, called through ctypes: each refusal of B2_BoosterPredict,
+B2_BoosterPredictContribs, B2_BoosterPredictLeaf and B2_BoosterAddTree matched against its whole message, which refusal
+wins when a call breaks two rules, a categorical and a vector-leaf tree added whole through B2_BoosterAddTree in every
+prediction mode, and malformed model files refused before any tree walk."""
 import ctypes as C
+import json
 
 import numpy as np
 import pytest
@@ -10,6 +11,7 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 N, F = 8, 3
+VECTOR = "\nnum_target=2\nmulti_strategy=multi_output_tree"   # booster() params of a two-target vector-leaf model
 
 
 @pytest.fixture(scope="module")
@@ -62,40 +64,35 @@ def booster(eng, handles, extra=""):
     return h.value
 
 
-def add_stump(eng, bst, feature, cond, values):
-    """A root split on `feature` with two leaves of `values`; the leaves cover the same hessian."""
-    topology = [np.asarray(a, np.int32) for a in ([1, -1, -1], [2, -1, -1], [-1, 0, 0], [feature, -1, -1])]
-    cond_a, value_a = np.asarray([cond, 0, 0], np.float32), np.asarray([0, values[0], values[1]], np.float32)
-    default_left, hess = np.asarray([1, 0, 0], np.uint8), np.asarray([2.0, 1.0, 1.0], np.float64)
-    call(eng, "B2_BoosterAddTree", bst, 3, *(eng._ip(a) for a in topology), None, eng._fp(cond_a), eng._bp(default_left),
-         eng._fp(value_a), None, None, hess.ctypes.data_as(eng._DP))
+def stump(feature, cond, values, right_codes=None, leaf_vector=None):
+    """A root split on `feature` with two leaves of `values`, as a tree dict; the leaves cover the same hessian.  With
+    right_codes the split is categorical: those category codes go right."""
+    t = dict(left=[1, -1, -1], right=[2, -1, -1], parent=[-1, 0, 0], split_feature=[feature, -1, -1],
+             split_bin=[-1, -1, -1], split_cond=[cond, 0, 0], default_left=[1, 0, 0], value=[0, values[0], values[1]],
+             base_weight=[0, 0, 0], loss_chg=[0, 0, 0], sum_hess=[2.0, 1.0, 1.0], leaf_vector=leaf_vector)
+    if right_codes is not None:
+        t["split_type"] = np.asarray([1, 0, 0], np.uint8)
+        t["cat_bits"] = np.zeros((3, 8), np.uint32)
+        for c in right_codes:
+            t["cat_bits"][0, c >> 5] |= np.uint32(1 << (c & 31))
+    return t
+
+
+def add_tree(eng, bst, t):
+    rec, _arrays = eng.B2Tree.of(t)
+    call(eng, "B2_BoosterAddTree", bst, C.byref(rec))
 
 
 def categorical_stump(eng, handles, right_codes):
     bst = booster(eng, handles)
-    add_stump(eng, bst, 0, 0.0, (-1.0, 1.0))
-    set_categories(eng, bst, right_codes)
+    add_tree(eng, bst, stump(0, 0.0, (-1.0, 1.0), right_codes=right_codes))
     return bst
-
-
-def set_categories(eng, bst, right_codes):
-    split_type = np.asarray([1, 0, 0], np.uint8)
-    bits = np.zeros((3, 8), np.uint32)
-    for c in right_codes:
-        bits[0, c >> 5] |= np.uint32(1 << (c & 31))
-    call(eng, "B2_BoosterSetTreeCategories", bst, 0, eng._bp(split_type), bits.ctypes.data_as(C.POINTER(C.c_uint32)))
 
 
 def vector_stump(eng, handles, leaf_vec):
-    bst = booster(eng, handles, "\nnum_target=2\nmulti_strategy=multi_output_tree")
-    add_stump(eng, bst, 1, 0.5, (0.0, 0.0))
-    set_leaf_vector(eng, bst, leaf_vec)
+    bst = booster(eng, handles, VECTOR)
+    add_tree(eng, bst, stump(1, 0.5, (0.0, 0.0), leaf_vector=leaf_vec))
     return bst
-
-
-def set_leaf_vector(eng, bst, leaf_vec):
-    v = np.ascontiguousarray(leaf_vec, np.float32).reshape(-1)
-    call(eng, "B2_BoosterSetTreeLeafVector", bst, 0, eng._fp(v), v.size)
 
 
 def predict(eng, bst, m, out_len, tree_begin=0, tree_end=0):
@@ -201,34 +198,151 @@ def test_precedence(eng, handles):
     assert refused(eng, leaf, bst, matrix(eng, handles), 1, 2) == RANGE
 
 
-def test_category_edit_reaches_every_cache(eng, handles):
+def test_categorical_stump_in_every_prediction_mode(eng, handles):
     codes = features()[:, 0].astype(int)
-    old, new = [1, 2], [0, 3]
-    expect_old = np.where(np.isin(codes, old), 1.0, -1.0).astype(np.float32)
-    bst = categorical_stump(eng, handles, old)
-    m = matrix(eng, handles, label=expect_old)
+    expect = np.where(np.isin(codes, [1, 2]), 1.0, -1.0).astype(np.float32)
+    bst = categorical_stump(eng, handles, [1, 2])
+    m = matrix(eng, handles, label=expect)
     shap = np.zeros((N, F + 1), np.float32)
     # leaves of equal cover: the tree's expected value is 0, so feature 0's contribution is the whole prediction
-    shap[:, 0] = expect_old
-    np.testing.assert_array_equal(predict(eng, bst, m, N), expect_old)
+    shap[:, 0] = expect
+    np.testing.assert_array_equal(predict(eng, bst, m, N), expect)
     np.testing.assert_allclose(contribs(eng, bst, m, N * (F + 1)).reshape(N, F + 1), shap, atol=1e-6)
-    np.testing.assert_array_equal(leaf(eng, bst, m, N), np.where(expect_old > 0, 2.0, 1.0))
+    np.testing.assert_array_equal(leaf(eng, bst, m, N), np.where(expect > 0, 2.0, 1.0))
     assert evaluate(eng, bst, m, "rmse") == 0.0
-    set_categories(eng, bst, new)
-    expect_new = -expect_old
-    shap[:, 0] = expect_new
-    np.testing.assert_array_equal(predict(eng, bst, m, N), expect_new)
-    np.testing.assert_allclose(contribs(eng, bst, m, N * (F + 1)).reshape(N, F + 1), shap, atol=1e-6)
-    np.testing.assert_array_equal(leaf(eng, bst, m, N), np.where(expect_new > 0, 2.0, 1.0))
-    assert evaluate(eng, bst, m, "rmse") == pytest.approx(2.0, abs=1e-6)
 
 
-def test_leaf_vector_edit_reaches_prediction(eng, handles):
+def test_vector_stump_prediction(eng, handles):
     right = features()[:, 1] >= 0.5
-    old = np.asarray([[0, 0], [1, 2], [3, 4]], np.float32)
-    new = np.asarray([[0, 0], [-5, 6], [7, -8]], np.float32)
-    bst = vector_stump(eng, handles, old)
+    vec = np.asarray([[0, 0], [1, 2], [3, 4]], np.float32)
+    bst = vector_stump(eng, handles, vec)
     m = matrix(eng, handles)
-    np.testing.assert_array_equal(predict(eng, bst, m, 2 * N).reshape(N, 2), np.where(right[:, None], old[2], old[1]))
-    set_leaf_vector(eng, bst, new)
-    np.testing.assert_array_equal(predict(eng, bst, m, 2 * N).reshape(N, 2), np.where(right[:, None], new[2], new[1]))
+    np.testing.assert_array_equal(predict(eng, bst, m, 2 * N).reshape(N, 2), np.where(right[:, None], vec[2], vec[1]))
+
+
+def blank(n, vector=False):
+    """Zeroed arrays for B2_BoosterGetTree to fill, as Booster.get_tree allocates them."""
+    t = {k: np.zeros(n, np.int32) for k in ("left", "right", "parent", "split_feature", "split_bin")}
+    t.update({k: np.zeros(n, np.float32) for k in ("split_cond", "value", "base_weight", "loss_chg")})
+    t.update(default_left=np.zeros(n, np.uint8), sum_hess=np.zeros(n), split_type=np.zeros(n, np.uint8),
+             cat_bits=np.zeros((n, 8), np.uint32), leaf_vector=np.zeros((n, 2), np.float32) if vector else None)
+    return t
+
+
+def get_tree(eng, bst, t):
+    rec, _arrays = eng.B2Tree.of(t)
+    call(eng, "B2_BoosterGetTree", bst, 0, C.byref(rec))
+    return t
+
+
+def test_get_tree_fills_the_record(eng, handles):
+    """B2_BoosterGetTree returns a tree as it was added, into buffers of its node count and leaf vector length."""
+    vec = np.arange(6, dtype=np.float32).reshape(3, 2)
+    cat, cat_tree = categorical_stump(eng, handles, [1, 200]), stump(0, 0.0, (-1.0, 1.0), right_codes=[1, 200])
+    vector, vector_tree = vector_stump(eng, handles, vec), stump(1, 0.5, (0.0, 0.0), leaf_vector=vec)
+    for bst, want in ((cat, cat_tree), (vector, vector_tree)):
+        got = get_tree(eng, bst, blank(3, vector=want["leaf_vector"] is not None))
+        for k, v in got.items():
+            if v is not None:
+                np.testing.assert_array_equal(v, want[k] if want.get(k) is not None else 0, err_msg=k)
+    assert refused(eng, get_tree, cat, blank(4)) == "tree buffers have 4 nodes, tree 0 has 3"
+    assert refused(eng, get_tree, cat, blank(3, vector=True)) == "leaf vector buffer has 6 values, tree 0 has 0"
+    assert refused(eng, get_tree, vector, blank(3)) == "leaf vector buffer has 0 values, tree 0 has 6"
+
+
+def refused_tree(eng, bst, t):
+    """The message B2_BoosterAddTree refuses tree t with; the model keeps the trees it had."""
+    before = C.c_int32(0)
+    call(eng, "B2_BoosterNumTrees", bst, C.byref(before))
+    with pytest.raises(eng.XGBoostError) as e:
+        add_tree(eng, bst, t)
+    after = C.c_int32(0)
+    call(eng, "B2_BoosterNumTrees", bst, C.byref(after))
+    assert after.value == before.value
+    return str(e.value)
+
+
+def edited(t, **fields):
+    return dict(t, **{k: np.asarray(v) for k, v in fields.items()})
+
+
+def test_add_tree_refuses_no_nodes(eng, handles):
+    bst = booster(eng, handles)
+    empty = {k: np.zeros(0) for k in stump(0, 0.5, (1, 2))}
+    assert refused_tree(eng, bst, dict(empty, leaf_vector=None)) == "tree 0 has no nodes"
+
+
+def test_add_tree_refuses_child_outside_the_tree(eng, handles):
+    bst = booster(eng, handles)
+    t = stump(1, 0.5, (1.0, 2.0))
+    assert refused_tree(eng, bst, edited(t, right=[-5, -1, -1])) == "tree 0 node 0 has child -5 outside [0, 3)"
+    add_tree(eng, bst, t)   # a refused tree is named by the index it would have had in the model
+    assert refused_tree(eng, bst, edited(t, left=[3, -1, -1])) == "tree 1 node 0 has child 3 outside [0, 3)"
+
+
+def test_add_tree_refuses_a_split_reached_twice(eng, handles):
+    bst = booster(eng, handles)
+    t = stump(1, 0.5, (1.0, 2.0))
+    assert refused_tree(eng, bst, edited(t, left=[0, -1, -1])) == "tree 0 node 0 splits and is reached twice from the root"
+    # a shared subtree: both children of the root are split node 1
+    shared = dict(left=[1, 2, -1, -1], right=[1, 3, -1, -1], parent=[-1, 0, 1, 1], split_feature=[1, 2, -1, -1],
+                  split_bin=[-1] * 4, split_cond=[0.5, 0.5, 0, 0], default_left=[0] * 4, value=[0, 0, 1, 2],
+                  base_weight=[0] * 4, loss_chg=[0] * 4, sum_hess=[1.0] * 4)
+    assert refused_tree(eng, bst, shared) == "tree 0 node 1 splits and is reached twice from the root"
+    # a leaf shared by two splits, and a node the root does not reach (xgboost's deleted nodes), are walked safely
+    add_tree(eng, bst, edited(t, right=[1, -1, -1]))
+    np.testing.assert_array_equal(predict(eng, bst, matrix(eng, handles), N), np.ones(N, np.float32))
+
+
+def test_add_tree_refuses_a_feature_outside_the_model(eng, handles):
+    bst = booster(eng, handles)
+    assert refused_tree(eng, bst, stump(F, 0.5, (1.0, 2.0))) == "tree 0 node 0 splits on feature 3; the model has 3 features"
+
+
+def test_add_tree_refuses_a_categorical_leaf(eng, handles):
+    bst = booster(eng, handles)
+    t = stump(0, 0.0, (-1.0, 1.0), right_codes=[1])
+    assert refused_tree(eng, bst, edited(t, split_type=np.asarray([1, 0, 1], np.uint8))) == (
+        "tree 0 node 2 is a leaf with split_type 1 (categorical)")
+
+
+def test_add_tree_refuses_a_leaf_vector_on_a_single_output_booster(eng, handles):
+    bst = booster(eng, handles)
+    assert refused_tree(eng, bst, stump(1, 0.5, (0.0, 0.0), leaf_vector=np.zeros((3, 2)))) == (
+        "tree 0 is a vector-leaf tree (multi_strategy=multi_output_tree); this booster grows single-output trees "
+        "(multi_strategy=one_output_per_tree, 1 target(s)): a model keeps the strategy it was trained with")
+
+
+def test_add_tree_refuses_a_missing_leaf_vector(eng, handles):
+    bst = booster(eng, handles, VECTOR)
+    assert refused_tree(eng, bst, stump(1, 0.5, (1.0, 2.0))) == (
+        "tree 0 is a single-output tree (multi_strategy=one_output_per_tree); this booster grows vector-leaf trees "
+        "(multi_strategy=multi_output_tree): a model keeps the strategy it was trained with")
+
+
+def test_add_tree_refuses_a_leaf_vector_of_the_wrong_length(eng, handles):
+    bst = booster(eng, handles, VECTOR)
+    assert refused_tree(eng, bst, stump(1, 0.5, (0.0, 0.0), leaf_vector=np.zeros(5))) == (
+        "tree 0 has a leaf vector of 5 values; it needs 6 (3 nodes x 2 targets)")
+    assert refused_tree(eng, bst, stump(1, 0.5, (0.0, 0.0), leaf_vector=np.zeros((3, 3)))) == (
+        "tree 0 has a leaf vector of 9 values; it needs 6 (3 nodes x 2 targets)")
+
+
+@pytest.mark.parametrize("children, message", [
+    ({"right_children": [-5, -1, -1]}, "tree 0 node 0 has child -5 outside [0, 3)"),
+    ({"left_children": [0, -1, -1]}, "tree 0 node 0 splits and is reached twice from the root"),
+])
+def test_malformed_model_file_refused(eng, tmp_path, children, message):
+    """A model file whose tree walk would leave the tree or never end is refused when the predictor is built, before
+    any kernel walks it; so is every later prediction."""
+    from tests.model_files import xgb_model_file
+    doc = json.loads(xgb_model_file(1, n_features=F))
+    doc["learner"]["gradient_booster"]["model"]["trees"][0].update(children)
+    path = str(tmp_path / "model.json")
+    with open(path, "w") as f:
+        json.dump(doc, f)
+    bst = eng.Booster(model_file=path)
+    for _ in range(2):
+        with pytest.raises(eng.XGBoostError) as e:
+            bst.predict(eng.DMatrix(features()))
+        assert str(e.value) == message

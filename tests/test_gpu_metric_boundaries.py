@@ -492,41 +492,3 @@ def test_cache_follows_twenty_more_rounds(eng):
     for i in range(20):
         bst.update(dtrain, 3 + i)
     assert_metric_fresh(eng, bst, dv, y[:5000])
-
-
-def test_cache_follows_leaf_vector_edits(eng):
-    X, y = data()
-    Y = np.stack([y, -y], axis=1).astype(F32)
-    bst = eng.train({"max_depth": 3, "multi_strategy": "multi_output_tree"},
-                    eng.DMatrix(X, label=Y, multi_target=True), 3, verbose_eval=False)
-    dv = eng.DMatrix(X[:5000], label=Y[:5000], multi_target=True)
-    before = evaluate(eng, bst, dv, "rmse")
-    t = bst.get_trees()[1]
-    v = (np.asarray(t["leaf_vector"], F32).reshape(-1) * F32(3) + F32(0.5)).astype(F32)
-    eng._check(eng.lib().B2_BoosterSetTreeLeafVector(bst.handle, 1, eng._fp(v), v.size))
-    m = bst.predict(dv, output_margin=True).reshape(5000, 2)
-    got = evaluate(eng, bst, dv, "rmse")
-    want = MT.metric("rmse", "reg:squarederror", m, Y[:5000])
-    assert got != before
-    B.assert_within(got, want, B.elementwise_terms("rmse", "reg:squarederror", m.reshape(-1), Y[:5000].reshape(-1)),
-                    None, "rmse")
-
-
-def test_cache_follows_category_edits(eng):
-    rng = np.random.default_rng(17)
-    n = 20000
-    X = np.stack([rng.integers(0, 12, n), rng.uniform(size=n)], axis=1).astype(F32)
-    y = (np.isin(X[:, 0], [1, 4, 7]) * 2.0 + X[:, 1]).astype(F32)
-    kw = dict(feature_types=["c", "q"], enable_categorical=True)
-    bst = eng.train({"max_depth": 3, "max_cat_to_onehot": 1}, eng.DMatrix(X, label=y, **kw), 3, verbose_eval=False)
-    dv = eng.DMatrix(X[:5000], label=y[:5000], **kw)
-    assert_metric_fresh(eng, bst, dv, y[:5000])
-    t = bst.get_trees()[0]
-    st = np.ascontiguousarray(t["split_type"], np.uint8)
-    assert st.any(), "the tree has no categorical split"
-    bits = ~np.asarray(t["cat_bits"], np.uint32).reshape(st.size, 8)   # every category changes side
-    bits[st == 0] = 0
-    bits = np.ascontiguousarray(bits, np.uint32)
-    eng._check(eng.lib().B2_BoosterSetTreeCategories(bst.handle, 0, eng._bp(st),
-                                                    bits.ctypes.data_as(C.POINTER(C.c_uint32))))
-    assert_metric_fresh(eng, bst, dv, y[:5000])

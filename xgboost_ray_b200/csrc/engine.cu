@@ -525,37 +525,42 @@ int B2_BoosterTreeNumNodes(B2Handle bh, int32_t tree, int32_t* out) {
   *out = tree_at(drained(bh), tree).size();
   API_END
 }
-int B2_BoosterGetTree(B2Handle bh, int32_t tree, int32_t* left, int32_t* right, int32_t* parent, int32_t* split_feature,
-                      int32_t* split_bin, float* split_cond, uint8_t* default_left, float* value, float* base_weight,
-                      float* loss_chg, double* sum_hess) {
+int B2_BoosterGetTree(B2Handle bh, int32_t tree, B2Tree* out) {
   API_BEGIN
   Booster* b = drained(bh);
   const TreeHost& t = tree_at(b, tree); const size_t n = t.size();
-  memcpy(left, t.left.data(), n * 4); memcpy(right, t.right.data(), n * 4); memcpy(parent, t.parent.data(), n * 4);
-  memcpy(split_feature, t.feature.data(), n * 4); memcpy(split_bin, t.split_bin.data(), n * 4);
-  memcpy(split_cond, t.cond.data(), n * 4); memcpy(default_left, t.default_left.data(), n);
-  memcpy(value, t.value.data(), n * 4); memcpy(base_weight, t.base_weight.data(), n * 4);
-  memcpy(loss_chg, t.loss_chg.data(), n * 4); memcpy(sum_hess, t.sum_hess.data(), n * 8);
+  if (out->n_nodes != t.size()) fail("tree buffers have %d nodes, tree %d has %d", out->n_nodes, tree, t.size());
+  const int64_t len = out->leaf_vector ? out->leaf_vector_len : 0;
+  if (len != (int64_t)t.leaf_vec.size()) fail("leaf vector buffer has %lld values, tree %d has %zu", (long long)len, tree, t.leaf_vec.size());
+  memcpy(out->left, t.left.data(), n * 4); memcpy(out->right, t.right.data(), n * 4); memcpy(out->parent, t.parent.data(), n * 4);
+  memcpy(out->split_feature, t.feature.data(), n * 4); memcpy(out->split_bin, t.split_bin.data(), n * 4);
+  memcpy(out->split_cond, t.cond.data(), n * 4); memcpy(out->default_left, t.default_left.data(), n);
+  memcpy(out->value, t.value.data(), n * 4); memcpy(out->base_weight, t.base_weight.data(), n * 4);
+  memcpy(out->loss_chg, t.loss_chg.data(), n * 4); memcpy(out->sum_hess, t.sum_hess.data(), n * 8);
+  memcpy(out->split_type, t.split_type.data(), n); memcpy(out->cat_bits, t.cat_bits.data(), n * 8 * sizeof(uint32_t));
+  if (len > 0) memcpy(out->leaf_vector, t.leaf_vec.data(), len * sizeof(float));
   API_END
 }
-int B2_BoosterAddTree(B2Handle bh, int32_t n_nodes, const int32_t* left, const int32_t* right, const int32_t* parent,
-                      const int32_t* split_feature, const int32_t* split_bin, const float* split_cond,
-                      const uint8_t* default_left, const float* value, const float* base_weight, const float* loss_chg,
-                      const double* sum_hess) {
+int B2_BoosterAddTree(B2Handle bh, const B2Tree* in) {
   API_BEGIN
   Booster* b = drained(bh);
   if (b->update_started) fail("process_type=update: trees are added before the first refresh round, not after");
-  if (n_nodes < 1) fail("a tree needs at least one node");
   TreeHost t;
-  for (int i = 0; i < n_nodes; ++i) {
-    t.add(parent[i]);
-    if (left[i] >= n_nodes || right[i] >= n_nodes) fail("child index out of range in tree");
-    if (split_feature[i] >= b->n_features) fail("split feature %d out of range", split_feature[i]);
-    t.left[i] = left[i]; t.right[i] = right[i]; t.feature[i] = split_feature[i]; t.split_bin[i] = split_bin ? split_bin[i] : -1;
-    t.cond[i] = split_cond[i]; t.default_left[i] = default_left[i]; t.value[i] = value[i];
-    t.base_weight[i] = base_weight ? base_weight[i] : 0.f; t.loss_chg[i] = loss_chg ? loss_chg[i] : 0.f;
-    t.sum_hess[i] = sum_hess ? sum_hess[i] : 0.0;
+  for (int i = 0; i < in->n_nodes; ++i) {
+    t.add(in->parent[i]);
+    t.left[i] = in->left[i]; t.right[i] = in->right[i]; t.feature[i] = in->split_feature[i];
+    t.split_bin[i] = in->split_bin ? in->split_bin[i] : -1;
+    t.cond[i] = in->split_cond[i]; t.default_left[i] = in->default_left[i]; t.value[i] = in->value[i];
+    t.base_weight[i] = in->base_weight ? in->base_weight[i] : 0.f; t.loss_chg[i] = in->loss_chg ? in->loss_chg[i] : 0.f;
+    t.sum_hess[i] = in->sum_hess ? in->sum_hess[i] : 0.0;
+    if (in->split_type && in->split_type[i]) {   // numeric nodes keep all-zero category bits
+      if (!in->cat_bits) fail("tree %zu node %d has a categorical split_type and no cat_bits", b->trees.size(), i);
+      t.split_type[i] = 1; t.any_cat = true;
+      for (int w8 = 0; w8 < 8; ++w8) t.cat_bits[(size_t)i * 8 + w8] = in->cat_bits[(size_t)i * 8 + w8];
+    }
   }
+  if (in->leaf_vector && in->leaf_vector_len > 0) t.leaf_vec.assign(in->leaf_vector, in->leaf_vector + in->leaf_vector_len);
+  check_tree(b, t);
   b->trees.push_back(std::move(t));
   if (b->p.dart) b->tree_w.push_back(1.0f);   // B2_BoosterSetTreeWeights sets the model's weights
   b->margin_ready = false;
@@ -583,48 +588,6 @@ int B2_BoosterSetTreeWeights(B2Handle bh, const float* w, int64_t len) {
   b->tree_w.assign(w, w + len);
   b->weights_version++;
   b->margin_ready = false;
-  API_END
-}
-int B2_BoosterGetTreeCategories(B2Handle bh, int32_t tree, uint8_t* split_type, uint32_t* cat_bits) {
-  API_BEGIN
-  Booster* b = drained(bh);
-  const TreeHost& t = tree_at(b, tree); const size_t n = t.size();
-  memcpy(split_type, t.split_type.data(), n); memcpy(cat_bits, t.cat_bits.data(), n * 8 * sizeof(uint32_t));
-  API_END
-}
-int B2_BoosterSetTreeCategories(B2Handle bh, int32_t tree, const uint8_t* split_type, const uint32_t* cat_bits) {
-  API_BEGIN
-  Booster* b = drained(bh);
-  TreeHost& t = tree_at(b, tree); const size_t n = t.size();
-  for (size_t i = 0; i < n; ++i) {
-    t.split_type[i] = split_type[i] ? 1 : 0;
-    if (t.split_type[i]) t.any_cat = true;
-    for (int w8 = 0; w8 < 8; ++w8) t.cat_bits[i * 8 + w8] = split_type[i] ? cat_bits[i * 8 + w8] : 0u;
-  }
-  trees_edited(b);
-  API_END
-}
-int B2_BoosterGetTreeLeafVector(B2Handle bh, int32_t tree, float* out, int64_t len) {
-  API_BEGIN
-  Booster* b = drained(bh);
-  const TreeHost& t = tree_at(b, tree);
-  if (t.leaf_vec.empty()) fail("tree %d is not a vector-leaf tree", tree);
-  if (len != (int64_t)t.leaf_vec.size()) fail("leaf vector buffer has %lld values, tree %d has %zu", (long long)len, tree, t.leaf_vec.size());
-  memcpy(out, t.leaf_vec.data(), t.leaf_vec.size() * sizeof(float));
-  API_END
-}
-int B2_BoosterSetTreeLeafVector(B2Handle bh, int32_t tree, const float* v, int64_t len) {
-  API_BEGIN
-  Booster* b = drained(bh);
-  TreeHost& t = tree_at(b, tree);
-  if (!b->p.vector_leaf())
-    fail("this booster grows single-output trees (multi_strategy=one_output_per_tree, %d target(s)); a vector-leaf tree "
-         "needs multi_strategy=multi_output_tree and num_target > 1", b->p.num_target);
-  const int64_t want = (int64_t)t.size() * b->p.num_target;
-  if (len != want) fail("leaf vector has %lld values, tree %d needs %lld (%d nodes x %d targets)", (long long)len, tree,
-                        (long long)want, t.size(), b->p.num_target);
-  t.leaf_vec.assign(v, v + len);
-  trees_edited(b);
   API_END
 }
 int B2_BoosterGetTimers(B2Handle bh, int32_t reset, char* out, int64_t out_cap) {

@@ -621,6 +621,9 @@ void run_tree(Booster* b, int k, int slot);
 void materialize_tree(Booster* b, const void* block);
 void materialize_vector_tree(Booster* b, const void* block, const void* vblock);
 void sync_device_trees(Booster* b);
+// B2_BoosterAddTree: fails unless tree t can be appended to b's model (every walk from the root ends at a leaf, the
+// split features exist, the leaf vector fits b's kind of tree); names the tree, the node and the value
+void check_tree(const Booster* b, const TreeHost& t);
 // B2_HistBuildRaw*: one histogram of m's rows ridx[0..n_sel) (nullptr: rows 0..n_sel) from the pairs (qg, qh) into out
 // [F][256][2]; chunk_rows <= 0 and window_rows <= 0 take 2048 and 4096, chunk_rows is capped at window_rows
 void hist_build_raw(Matrix* m, const int32_t* qg, const int32_t* qh, const int32_t* ridx, int64_t n_sel, int window_rows,

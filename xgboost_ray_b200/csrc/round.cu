@@ -377,10 +377,10 @@ void set_booster_params(Booster* b, const char* params) {
 }
 
 // Update mode, before anything reads the train margin: the trees added so far become the trees to update and the model
-// starts empty (xgboost's gbtree moves them to trees_to_update).  Every tree is checked to be a proper binary tree
-// reachable from node 0 with at most 65,536 leaves (compact indices 0..65,535 fit pos), and copied to the device once:
-// B2TreeNodeDev nodes whose pad holds the compact leaf index (leaves numbered in node order), the category sets, and
-// the node ids grouped by depth.
+// starts empty (xgboost's gbtree moves them to trees_to_update).  Beyond check_tree, every node of a tree must be
+// reached from node 0, each once, and a tree has at most 65,536 leaves (compact indices 0..65,535 fit pos).  The trees
+// are copied to the device once: B2TreeNodeDev nodes whose pad holds the compact leaf index (leaves numbered in node
+// order), the category sets, and the node ids grouped by depth.
 void begin_update(Booster* b) {
   if (!b->p.update_mode || b->update_started) return;
   drain_round(b);
@@ -401,14 +401,14 @@ void begin_update(Booster* b) {
     int n_leaves = 0;
     for (int i = 0; i < nn; ++i) if (t.feature[i] < 0) leaf_of[i] = n_leaves++;
     if (n_leaves > 65536) fail("tree %zu has %d leaves; the refresh updater supports at most 65536", ti, n_leaves);
-    // breadth-first from the root: every node reached exactly once, splits with two children, leaves with none
+    // breadth-first from the root (check_tree: the children are nodes, no split is reached twice): every node reached,
+    // a leaf only once
     std::vector<int32_t> bfs{0}; depth[0] = 0;
     for (size_t q = 0; q < bfs.size(); ++q) {
       const int i = bfs[q];
       if (t.feature[i] < 0) continue;
       for (int c : {t.left[i], t.right[i]}) {
-        if (c < 0 || c >= nn || depth[c] >= 0)
-          fail("tree %zu is not a binary tree: node %d has child %d (%d nodes)", ti, i, c, nn);
+        if (depth[c] >= 0) fail("tree %zu is not a binary tree: node %d is reached twice from the root", ti, c);
         depth[c] = depth[i] + 1;
         bfs.push_back(c);
       }

@@ -987,24 +987,46 @@ void materialize_vector_tree(Booster* b, const void* block, const void* vblock) 
   b->trees.push_back(std::move(t));
 }
 
-// every tree of a vector-leaf model has a leaf vector, no tree of a scalar model has one (continuing a model with the
-// other multi_strategy is refused)
-void check_tree_kinds(const Booster* b) {
-  const int T = b->p.num_target;
-  for (size_t i = 0; i < b->trees.size(); ++i) {
-    const TreeHost& t = b->trees[i];
-    if (b->p.vector_leaf() && t.leaf_vec.size() != (size_t)t.size() * T)
-      fail("tree %zu is a single-output tree (multi_strategy=one_output_per_tree); this model uses multi_strategy="
-           "multi_output_tree: a model keeps the strategy it was trained with", i);
-    if (!b->p.vector_leaf() && !t.leaf_vec.empty())
-      fail("tree %zu is a vector-leaf tree (multi_strategy=multi_output_tree); this model uses multi_strategy="
-           "one_output_per_tree: a model keeps the strategy it was trained with", i);
+// B2_BoosterAddTree: a tree from outside the engine is walked by the prediction kernels, the TreeSHAP path builder and
+// the refresh updater, which follow split children until they reach a leaf.  So every split's children are nodes of
+// the tree and no split is reached twice from the root (no cycle, no shared subtree); nodes the root does not reach
+// (xgboost's deleted nodes) are never walked.  A model keeps the multi_strategy it was trained with.
+void check_tree(const Booster* b, const TreeHost& t) {
+  const size_t ti = b->trees.size();
+  const int n = t.size(), T = b->p.num_target;
+  if (n < 1) fail("tree %zu has no nodes", ti);
+  for (int i = 0; i < n; ++i) {
+    if (t.feature[i] < 0) {
+      if (t.split_type[i]) fail("tree %zu node %d is a leaf with split_type %d (categorical)", ti, i, t.split_type[i]);
+      continue;
+    }
+    if (t.feature[i] >= b->n_features)
+      fail("tree %zu node %d splits on feature %d; the model has %d features", ti, i, t.feature[i], b->n_features);
+    for (int c : {t.left[i], t.right[i]})
+      if (c < 0 || c >= n) fail("tree %zu node %d has child %d outside [0, %d)", ti, i, c, n);
   }
+  std::vector<uint8_t> seen(n, 0);
+  std::vector<int> stack{0};
+  while (!stack.empty()) {
+    const int i = stack.back(); stack.pop_back();
+    if (t.feature[i] < 0) continue;
+    if (seen[i]) fail("tree %zu node %d splits and is reached twice from the root", ti, i);
+    seen[i] = 1;
+    stack.push_back(t.left[i]); stack.push_back(t.right[i]);
+  }
+  if (!b->p.vector_leaf() && !t.leaf_vec.empty())
+    fail("tree %zu is a vector-leaf tree (multi_strategy=multi_output_tree); this booster grows single-output trees "
+         "(multi_strategy=one_output_per_tree, %d target(s)): a model keeps the strategy it was trained with", ti, T);
+  if (b->p.vector_leaf() && t.leaf_vec.empty())
+    fail("tree %zu is a single-output tree (multi_strategy=one_output_per_tree); this booster grows vector-leaf trees "
+         "(multi_strategy=multi_output_tree): a model keeps the strategy it was trained with", ti);
+  if (b->p.vector_leaf() && t.leaf_vec.size() != (size_t)n * T)
+    fail("tree %zu has a leaf vector of %zu values; it needs %lld (%d nodes x %d targets)", ti, t.leaf_vec.size(),
+         (long long)n * T, n, T);
 }
 
 void sync_device_trees(Booster* b) {
   if (b->d_trees_synced == (int)b->trees.size()) return;
-  check_tree_kinds(b);
   if (b->p.vector_leaf()) {   // [model nodes][T], in the order of d_nodes
     b->h_leaf_table.clear();
     for (auto& t : b->trees) b->h_leaf_table.insert(b->h_leaf_table.end(), t.leaf_vec.begin(), t.leaf_vec.end());

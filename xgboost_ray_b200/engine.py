@@ -42,6 +42,28 @@ _LP = C.POINTER(C.c_int64)
 _H = C.c_uint64
 _FLT_MAX = np.finfo(np.float32).max
 
+
+class B2Tree(C.Structure):
+    """One tree as B2_BoosterAddTree takes it and B2_BoosterGetTree fills it (include/b2hist.h).  Its arrays are named
+    as the keys of a tree dict; each is a void pointer here (a typed ctypes pointer costs microseconds per array, per
+    tree, to make) and DTYPES gives its element type."""
+    DTYPES = {"left": np.int32, "right": np.int32, "parent": np.int32, "split_feature": np.int32, "split_bin": np.int32,
+              "split_cond": np.float32, "default_left": np.uint8, "value": np.float32, "base_weight": np.float32,
+              "loss_chg": np.float32, "sum_hess": np.float64, "split_type": np.uint8, "cat_bits": np.uint32,
+              "leaf_vector": np.float32}
+    _fields_ = [("n_nodes", C.c_int32)] + [(k, C.c_void_p) for k in DTYPES] + [("leaf_vector_len", C.c_int64)]
+    OPTIONAL = ("split_type", "cat_bits", "leaf_vector")   # NULL when the tree dict has none
+
+    @classmethod
+    def of(cls, t):
+        """The record of tree dict t, and the arrays it points into (which must outlive its use)."""
+        arrays = [None if k in cls.OPTIONAL and t.get(k) is None else np.ascontiguousarray(t[k], dt)
+                  for k, dt in cls.DTYPES.items()]
+        vec = arrays[-1]
+        return cls(arrays[0].size, *[None if a is None else a.ctypes.data for a in arrays],
+                   0 if vec is None else vec.size), arrays
+
+
 # name -> (restype, argtypes); every symbol declared in include/b2hist.h
 ABI = {
     "B2_GetLastError": (C.c_char_p, []),
@@ -97,12 +119,8 @@ ABI = {
     "B2_BoosterNumTargets": (C.c_int, [_H, _IP]),
     "B2_BoosterNumTrees": (C.c_int, [_H, _IP]),
     "B2_BoosterTreeNumNodes": (C.c_int, [_H, C.c_int32, _IP]),
-    "B2_BoosterGetTree": (C.c_int, [_H, C.c_int32, _IP, _IP, _IP, _IP, _IP, _FP, _BP, _FP, _FP, _FP, _DP]),
-    "B2_BoosterAddTree": (C.c_int, [_H, C.c_int32, _IP, _IP, _IP, _IP, _IP, _FP, _BP, _FP, _FP, _FP, _DP]),
-    "B2_BoosterGetTreeCategories": (C.c_int, [_H, C.c_int32, _BP, C.POINTER(C.c_uint32)]),
-    "B2_BoosterSetTreeCategories": (C.c_int, [_H, C.c_int32, _BP, C.POINTER(C.c_uint32)]),
-    "B2_BoosterGetTreeLeafVector": (C.c_int, [_H, C.c_int32, _FP, C.c_int64]),
-    "B2_BoosterSetTreeLeafVector": (C.c_int, [_H, C.c_int32, _FP, C.c_int64]),
+    "B2_BoosterGetTree": (C.c_int, [_H, C.c_int32, C.POINTER(B2Tree)]),
+    "B2_BoosterAddTree": (C.c_int, [_H, C.POINTER(B2Tree)]),
     "B2_BoosterGetTreeWeights": (C.c_int, [_H, _FP, C.c_int64]),
     "B2_BoosterSetTreeWeights": (C.c_int, [_H, _FP, C.c_int64]),
     "B2_BoosterGetTimers": (C.c_int, [_H, C.c_int32, C.c_char_p, C.c_int64]),
@@ -959,8 +977,6 @@ def _objective(name):
     return o
 
 
-_TREE_FIELDS = ("left", "right", "parent", "split_feature", "split_bin", "split_cond", "default_left", "value",
-                "base_weight", "loss_chg", "sum_hess")
 _ENGINE_KEYS = ("objective", "num_class", "max_depth", "eta", "learning_rate", "gamma", "min_split_loss",
                 "min_child_weight", "lambda", "reg_lambda", "alpha", "reg_alpha", "base_score", "hist_qbits",
                 "hist_chunk_rows", "profile", "max_cat_to_onehot", "max_cat_threshold", "scale_pos_weight",
@@ -1190,36 +1206,16 @@ class Booster:
         extra = {"num_feature": self.n_features, "device": _default_device() if device is None else device}
         _check(lib().B2_BoosterCreate(self._param_text(extra), 0, 0, C.byref(h)))
         self.handle = h.value
-        self._push_trees(self._trees, self._weights)
+        try:
+            self._push_trees(self._trees, self._weights)
+        except XGBoostError:   # a refused tree: no predictor of part of the model
+            self._free()
+            raise
 
     def _push_trees(self, trees, weights=None):
         for t in trees:
-            n = len(t["left"])
-            _check(lib().B2_BoosterAddTree(
-                self.handle, n, _ip(np.ascontiguousarray(t["left"], np.int32)),
-                _ip(np.ascontiguousarray(t["right"], np.int32)), _ip(np.ascontiguousarray(t["parent"], np.int32)),
-                _ip(np.ascontiguousarray(t["split_feature"], np.int32)),
-                _ip(np.ascontiguousarray(t["split_bin"], np.int32)), _fp(_f32c(t["split_cond"])),
-                _bp(np.ascontiguousarray(t["default_left"], np.uint8)), _fp(_f32c(t["value"])),
-                _fp(_f32c(t["base_weight"])), _fp(_f32c(t["loss_chg"])),
-                np.ascontiguousarray(t["sum_hess"], np.float64).ctypes.data_as(_DP)))
-            st = t.get("split_type")
-            if st is not None and np.any(st):
-                nt = C.c_int32(0)
-                _check(lib().B2_BoosterNumTrees(self.handle, C.byref(nt)))
-                _check(lib().B2_BoosterSetTreeCategories(
-                    self.handle, nt.value - 1, _bp(np.ascontiguousarray(st, np.uint8)),
-                    np.ascontiguousarray(t["cat_bits"], np.uint32).ctypes.data_as(C.POINTER(C.c_uint32))))
-            if t.get("leaf_vector") is not None or self.is_vector_leaf:
-                # the engine refuses a vector where it grows single-output trees, and a tree without one where it
-                # grows vector-leaf trees: a model keeps its multi_strategy
-                if t.get("leaf_vector") is None:
-                    raise XGBoostError("multi_strategy='multi_output_tree' cannot continue a model of single-output trees "
-                                       "(multi_strategy='one_output_per_tree')")
-                nt = C.c_int32(0)
-                _check(lib().B2_BoosterNumTrees(self.handle, C.byref(nt)))
-                v = _f32c(np.asarray(t["leaf_vector"]).reshape(-1))
-                _check(lib().B2_BoosterSetTreeLeafVector(self.handle, nt.value - 1, _fp(v), v.size))
+            rec, _arrays = B2Tree.of(t)
+            _check(lib().B2_BoosterAddTree(self.handle, C.byref(rec)))
         if self.is_dart and trees and weights is not None:
             w = _f32c(weights)
             if w.size != len(trees):
@@ -1305,16 +1301,10 @@ class Booster:
                  value=np.zeros(n, np.float32), base_weight=np.zeros(n, np.float32),
                  loss_chg=np.zeros(n, np.float32), sum_hess=np.zeros(n, np.float64),
                  split_type=np.zeros(n, np.uint8), cat_bits=np.zeros((n, 8), np.uint32))
-        _check(lib().B2_BoosterGetTreeCategories(self.handle, i, _bp(t["split_type"]),
-                                                 t["cat_bits"].ctypes.data_as(C.POINTER(C.c_uint32))))
-        _check(lib().B2_BoosterGetTree(self.handle, i, _ip(t["left"]), _ip(t["right"]), _ip(t["parent"]),
-                                       _ip(t["split_feature"]), _ip(t["split_bin"]), _fp(t["split_cond"]),
-                                       _bp(t["default_left"]), _fp(t["value"]), _fp(t["base_weight"]),
-                                       _fp(t["loss_chg"]), t["sum_hess"].ctypes.data_as(_DP)))
         if self.is_vector_leaf:
-            v = np.zeros((n, self._num_target()), np.float32)
-            _check(lib().B2_BoosterGetTreeLeafVector(self.handle, i, _fp(v), v.size))
-            t["leaf_vector"] = v
+            t["leaf_vector"] = np.zeros((n, self._num_target()), np.float32)
+        rec, _arrays = B2Tree.of(t)
+        _check(lib().B2_BoosterGetTree(self.handle, i, C.byref(rec)))
         return t
 
     def get_trees(self):
